@@ -49,7 +49,7 @@ def workload(B, dtype="bf16"):
     return {"workload": f"MyCNN5-arch forward, [{B},{C},{W}] {dtype} per GPU, mode=independent",
             "arch": KIND, "batch_per_gpu": B, "channels": C, "window": W, "mode": "independent",
             "values": "N(0,1) seed 1234+rank", "weights": "default init, seed 0",
-            "l2": "inputs (1.84 GB per GPU) are larger than the 126 MB L2; no flush needed"}
+            "l2": "inputs (1.84 GB per GPU) are larger than the 50 MB L2; no flush needed"}
 
 
 def peaks():
@@ -57,13 +57,12 @@ def peaks():
     if os.path.exists(p):
         j = json.load(open(p))
         return float(j["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3, 3.35 TB/s), not measured"
 
 
 # ------------------------------------------------------------------------------------------
 class ClockSampler:
-    """SM clock + throttle reasons sampled DURING the timed region (B200_PROFILING.md's clocks
-    line), through NVML in a background thread: the timed region is only tens of milliseconds,
+    """SM clock + throttle reasons sampled DURING the timed region, through NVML in a background thread: the timed region is only tens of milliseconds,
     too short for an `nvidia-smi -lms` child process to produce a sample."""
 
     def __init__(self, index):
@@ -353,7 +352,7 @@ def oracle_parity(model, x, ages, y, n_check):
     t0 = time.perf_counter()
     # ONE thread: torch's multi-threaded GEMV over the 18745 LSTM inputs splits the reduction by thread, and how many threads
     # the OpenMP runtime actually hands out varies from run to run on a busy box -- seen once as a parity figure of 8.4e-6
-    # instead of 1.6e-6 for bit-identical GPU results (scripts/cross_process_check.sh); single-threaded the oracle is reproducible
+    # instead of 1.6e-6 for bit-identical GPU results; single-threaded the oracle is reproducible
     nt = torch.get_num_threads()
     torch.set_num_threads(1)
     want = O.ref_independent(ref, xs, ags).double()
@@ -467,6 +466,8 @@ def main():
     ap.add_argument("--dtype", default="bf16", choices=["bf16", "f32"],
                     help="window dtype: bf16 is the BASELINE workload; f32 (the reference's native dtype) is an extra line")
     ap.add_argument("--tc-splits", type=int, default=3, help="bf16 pieces per fp32 conv1 weight on the tensor cores (3 = fp32-equivalent)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed (the [batch] logits predict() returned) as DIR/logits.npy, float32")
     args = ap.parse_args()
 
     rank = int(os.environ.get("RANK", "0"))
@@ -537,6 +538,11 @@ def main():
     total_ms = float(t.item())
     value = world * B * args.steps / (total_ms / 1e3)
     assert torch.isfinite(y).all()
+    if args.dump_outputs and rank == 0:
+        # the inputs are seeded (weights seed 0, windows / ages seed 1234), so two builds can be compared output for output
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "logits.npy"), y.float().cpu().numpy())
 
     # ---- sustained: >= 3 s of back-to-back steps (the 12 ms headline region is a burst; an issue-bound
     #      kernel scales with the SM clock, which sags under sustained load) -----------------------------
@@ -605,11 +611,11 @@ def main():
         alg_bytes = B * (C * W * esz + 4) + n_w * 4
         achieved = alg_bytes / (k_ms / 1e3) / 1e9 if k_ms and k_ms > 0 else None
         step_gbs = alg_bytes / (total_ms / args.steps / 1e3) / 1e9
-        roof = {"bound": "hbm", "kernel": {"generic": "front end (conv1+pool+conv2+pool)", "stream": "fp32 streaming front end (CUDA-core conv1 + tcgen05 projection)"}.get(path, "tcgen05 fused front end"),
+        roof = {"bound": "hbm", "kernel": {"generic": "front end (conv1+pool+conv2+pool)", "stream": "fp32 streaming front end (CUDA-core conv1 + wgmma projection)"}.get(path, "wgmma fused front end"),
                 "achieved": achieved, "peak": hbm_peak, "unit": "GB/s",
                 "frac": (achieved / hbm_peak) if achieved else None, "peak_source": peak_src,
                 "kernel_ms": k_ms, "head_ms": head_ms, "algorithmic_bytes_per_launch": alg_bytes,
-                "traffic": TRAFFIC.get(path),
+                "traffic": None,                   # DRAM bytes per launch: no hardware-counter capture on this GPU
                 "whole_step_frac": step_gbs / hbm_peak,
                 "sustained_step_frac": (alg_bytes / (sustained["ms_per_step"] / 1e3) / 1e9 / hbm_peak) if sustained else None,
                 "compute_note": "co-bound by FP32/MUFU: 21.9 MFLOP + 169k tanh per window (DESIGN.md)"}
@@ -627,8 +633,7 @@ def main():
                "gpu_launches": launches_per_step * args.steps}
         if world == 1 and args.dtype == "bf16" and args.tc_splits == 3 and args.extra_steps > 0:
             # NOT the headline: the library option tc_splits=2 (conv1 weights as two bf16 pieces = 16 mantissa bits, 6 instead
-            # of 9 MMAs per block; samples exact, fp32 accumulation).  The kernel sits on the board's power cap and the tensor
-            # cores draw most of it, so a third fewer MMAs is a large step; reported with its own in-run parity figure.
+            # of 9 MMAs per block; samples exact, fp32 accumulation); reported with its own in-run parity figure.
             m2 = tskd_b200.B200MyCNN(arch, path=args.path, tc_splits=2).to(dev)
             m2.load_state_dict(model.state_dict())
             for _ in range(3):
@@ -668,12 +673,6 @@ def main():
     if world > 1:
         dist.destroy_process_group()
 
-
-# dram__bytes_read.sum + dram__bytes_write.sum per launch of the dominant kernel, from the
-# committed ncu captures under profiles/ (None until a capture exists for that path).
-TRAFFIC = {"generic": 1.846642e9 + 0.297926e9,      # profiles/r01_generic_frontend_ncu_full.txt (features written to HBM)
-           "tensorcore": 1.974513e9 + 0.032842e9,   # profiles/r02_final2_fused_ncu_full.txt (halo re-reads + gate partials)
-           "stream": 3.801502e9 + 0.034493e9}       # profiles/r01_final_stream_ncu_full.txt (fp32 windows)
 
 if __name__ == "__main__":
     main()

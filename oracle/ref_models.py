@@ -2,7 +2,7 @@
 
 ``__graft_entry__.build()`` copies ``/root/reference/bin/models.py`` (35 lines, torch only) into the
 git-ignored ``oracle/_ref/models.py`` whenever the reference tree is present (the authoring container);
-``oracle/_ref/`` is not gpurun-ignored, so the file travels to the GPU box with the snapshot the way a
+``oracle/_ref/`` travels with the built tree to the GPU machine the way a
 built ``.so`` does, and is never committed.  ``bench.py --impl reference`` and the ``cpu_baseline`` leg
 time THIS class (``cpu_baseline.kind = "reference"``); when the copy is absent they fall back to the
 restatement in ``oracle/mycnn_torch.py`` (``kind = "port"``).

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """BASELINE.json configs[3]: architectures {MyCNN3/4-arch (k1=5, pool(2,2)), MyCNN5-arch (k1=10,
-pool(3,2))} x W in {7500, 37500, 75000}, B=1024, C=3, bf16 and fp32, one B200.  One JSON line per
+pool(3,2))} x W in {7500, 37500, 75000}, B=1024, C=3, bf16 and fp32, one GPU.  One JSON line per
 case: windows/s, the dominant stage's duration and its fraction of the measured HBM roofline.
 Also the production shape [1,10,120] fp32 latency.   python scripts/sweep.py > profiles/<tag>.jsonl"""
 import json, os, sys, time

@@ -1,4 +1,4 @@
-"""GPU: the tcgen05 / TMA front end (b2cnn_tc.cu) against the PyTorch-CPU oracle and against
+"""GPU: the wgmma / TMA front end (b2cnn_tc.cu) against the PyTorch-CPU oracle and against
 the exact generic kernel.  path="tensorcore" makes the library refuse instead of falling back,
 so a pass here is a pass of the tensor-core kernel itself."""
 from dataclasses import replace
@@ -229,7 +229,7 @@ def test_tc_fused_persistent_grid_many_items_per_cta(kind, C, W, B):
     assert torch.equal(m.predict(x[:300], ages[:300]), got[:300])
 
 
-# ---- fp32 windows: streaming kernel (CUDA-core conv1 + tcgen05 projection), csrc/b2cnn_stream_f32.cuh ----
+# ---- fp32 windows: streaming kernel (CUDA-core conv1 + wgmma projection), csrc/b2cnn_tc_fused.cuh ----
 
 @pytest.mark.parametrize("kind,C,W,B,dist", [
     ("mycnn5", 3, 7504, 200, "normal"), ("mycnn5", 3, 7504, 300, "physio"), ("mycnn5", 1, 2048, 300, "normal"),

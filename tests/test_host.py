@@ -12,9 +12,7 @@ import torch
 import tskd_b200
 from tskd_b200 import capi
 from tskd_b200.arch import BLOB_KEYS, INERT_KEYS, ArchConfig, arch_from_state_dict
-from conftest import ROOT, load_golden
-
-REF_MODELS = "/root/reference/model"
+from conftest import GOLDEN, ROOT, load_golden
 
 
 def test_library_exports_every_declared_symbol():
@@ -24,7 +22,7 @@ def test_library_exports_every_declared_symbol():
     assert declared == set(capi.SYMBOLS), declared ^ set(capi.SYMBOLS)
     for name in declared:
         assert hasattr(lib, name), name
-    assert b"sm_100a" in lib.b2cnn_version()
+    assert b"sm_90a" in lib.b2cnn_version()
 
 
 def test_pure_host_entry_points():
@@ -110,10 +108,10 @@ def test_view_contract_rejected():
         tskd_b200.B200MyCNN.from_reference(sd, window=240)
 
 
-@pytest.mark.skipif(not os.path.isdir(REF_MODELS), reason="reference checkpoints only exist in the authoring container")
 @pytest.mark.parametrize("n", [2, 3, 4, 5])
 def test_load_legacy_pickles(n):
-    ref = tskd_b200.load_reference_checkpoint(f"{REF_MODELS}/MyCNN{n}.pth")
+    """The reference's own model/MyCNN{n}.pth files (whole pickled modules), stored unchanged under tests/golden/."""
+    ref = tskd_b200.load_reference_checkpoint(os.path.join(GOLDEN, f"MyCNN{n}.pth"))
     assert type(ref).__name__ == "PickledMyCNN" and ref.training is False
     m = tskd_b200.B200MyCNN.from_reference(ref)
     g, sd = load_golden("mycnn5_xtestinput.npz" if n == 5 else f"mycnn{n}_ckpt.npz")

@@ -1,6 +1,6 @@
 """B200-native drop-in for the one hot path of travistangvh/time-series-kafka-demo:
 ``output = model(x_arr, a_arr)`` (bin/predictStream.py:157) -> ``MyCNN.forward``
-(bin/models.py:22-36), as hand-written sm_100a CUDA behind the C ABI in ``include/b2cnn.h``.
+(bin/models.py:22-36), as hand-written sm_90a CUDA behind the C ABI in ``include/b2cnn.h``.
 
     from tskd_b200 import B200MyCNN, load_reference_checkpoint
     model = B200MyCNN.from_reference(load_reference_checkpoint("model/MyCNN5.pth")).eval()

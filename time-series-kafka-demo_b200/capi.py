@@ -10,7 +10,7 @@ import os
 from typing import Optional
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-# B2CNN_LIB: experiment hook (scripts/build_ablations.sh builds instrumented copies of the same library)
+# B2CNN_LIB: load another build of the same library (e.g. an instrumented copy)
 _LIB_PATH = os.environ.get("B2CNN_LIB") or os.path.join(_HERE, "lib", "libb2cnn.so")
 
 OK, EINVAL, EARCH, EVIEW, ECUDA, ESTATE = range(6)
@@ -75,7 +75,7 @@ def load_library() -> ctypes.CDLL:
     if not os.path.exists(_LIB_PATH):
         raise LibraryNotBuilt(
             f"{_LIB_PATH} not found: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-            "(nvcc, sm_100a).  There is no CPU fallback for this path.")
+            "(nvcc, sm_90a).  There is no CPU fallback for this path.")
     lib = ctypes.CDLL(_LIB_PATH)
     c_i64, c_int, c_vp = ctypes.c_int64, ctypes.c_int, ctypes.c_void_p
     cfgp = ctypes.POINTER(Config)

@@ -52,7 +52,7 @@ struct b2cnn_handle {
     b2cnn_config cfg;
     Dims d;
     int device = 0;
-    int num_sms = 148;
+    int num_sms = 132;
     bool weights_set = false;
     ConvWeights cw;
     HeadWeights hw;
@@ -257,7 +257,7 @@ extern "C" double b2cnn_parse_decimal(const char *s, int64_t len, int32_t *statu
     return v;
 }
 
-extern "C" const char *b2cnn_version(void) { return "b2cnn 0.3 (sm_100a; tcgen05 fused bf16 path, fp32 streaming path, generic path, device preprocessing + patient ring buffers)"; }
+extern "C" const char *b2cnn_version(void) { return "b2cnn 0.4 (sm_90a; wgmma fused bf16 path, fp32 streaming path, generic path, device preprocessing + patient ring buffers)"; }
 
 extern "C" int b2cnn_create(const b2cnn_config *cfg, b2cnn_handle **out) {
     if (!cfg || !out) return fail(B2CNN_EINVAL, "b2cnn_create: null argument");
@@ -432,7 +432,7 @@ static int forward_device(b2cnn_handle *h, const void *x, int dtype, int64_t B, 
         !(h->opt_path != B2CNN_PATH_TENSORCORE && h->opt_small && mode == B2CNN_MODE_INDEPENDENT && B >= 8 && batch_supported(d)))
         return fail(B2CNN_ESTATE, "b2cnn_forward: this x_pitch takes a path that needs feature rows; size the workspace with b2cnn_workspace_bytes()");
     if (!tc && !stream && h->opt_path == B2CNN_PATH_TENSORCORE)
-        return fail(B2CNN_EARCH, "path=tensorcore requested but this shape/dtype/mode is not supported by the tcgen05 kernel");
+        return fail(B2CNN_EARCH, "path=tensorcore requested but this shape/dtype/mode is not supported by the tensor-core kernel");
     const bool prof = h->opt_profile != 0;
     if (prof) {
         for (int i = 0; i < 3; ++i)
@@ -461,7 +461,7 @@ static int forward_device(b2cnn_handle *h, const void *x, int dtype, int64_t B, 
     int64_t sB = d.L, sP = 1;
     int n;
     if (h->opt_path != B2CNN_PATH_GENERIC && h->opt_stream && tc_stream_supported(h->tc, d, dtype)) {
-        // fp32 windows: TMA-streamed CUDA-core conv1 + tcgen05 projection, features never leave the SM
+        // fp32 windows: TMA-streamed CUDA-core conv1 + wgmma projection, features never leave the SM
         const bool indep = mode == B2CNN_MODE_INDEPENDENT;
         int slices = 0;
         n = tc_stream_gates(h->tc, d, h->cw, h->hw, x, B, feats, partial, gates, tc_ws, h->num_sms, st, &err, !indep, &slices);

@@ -5,9 +5,9 @@
 // One WARP owns a window from the first sample to the logit; nothing but __syncwarp() between the stages
 // (bin/models.py:23-34):
 //   stage 0  the window's C x W samples -> the warp's shared-memory rows (16-byte loads, fp32 or bf16 input)
-//   stage 1  conv1: lane l owns conv positions 4l .. 4l+3 x 4 output channels = 8 packed f32x2 accumulators;
+//   stage 1  conv1: lane l owns conv positions 4l .. 4l+3 x 4 output channels = 8 float2 accumulators;
 //            per input channel 4 LDS.128 of samples, per tap one broadcast LDS.128 of the 4 channel weights and
-//            8 FFMA2.  pool1 BEFORE the activation (max commutes with +bias and monotone tanh / relu; max.NaN
+//            8 FFMA pairs.  pool1 BEFORE the activation (max commutes with +bias and monotone tanh / relu; max.NaN
 //            propagates NaNs like ATen's max_pool1d); the one pooled position that straddles two lanes comes by shuffle
 //   stage 2  conv2 + pool2 + activation: lane l owns feature l (L_out <= 32)
 //   stage 3  LSTM layer 0 from the zero state: lane l owns gate rows l and l + 32 (W_ih_l0^T in shared memory,
@@ -33,17 +33,8 @@ struct BatchParams {
     ConvWeights cw;
 };
 
-__device__ __forceinline__ uint64_t bt_pk2(float2 v) {
-    uint64_t r;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(v.x), "f"(v.y));
-    return r;
-}
 __device__ __forceinline__ float2 bt_fma2(float2 a, float2 b, float2 c) {
-    uint64_t d;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(bt_pk2(a)), "l"(bt_pk2(b)), "l"(bt_pk2(c)));
-    float2 r;
-    asm("mov.b64 {%0, %1}, %2;" : "=f"(r.x), "=f"(r.y) : "l"(d));
-    return r;
+    return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y));
 }
 __device__ __forceinline__ float bt_age_scale(float age, float coef) {
     float s = __fadd_rn(__fmul_rn(age, coef), 1.0f);      // models.py:32: separate multiply and add

@@ -1,6 +1,6 @@
-// b2cnn_internal.cuh -- shared declarations of libb2cnn (sm_100a only).
+// b2cnn_internal.cuh -- shared declarations of libb2cnn (sm_90a only).
 //
-// The hot path being replaced is MyCNN.forward (/root/reference/bin/models.py:22-36):
+// The hot path being replaced is MyCNN.forward (bin/models.py:22-36 of the reference):
 //   conv1+tanh (:23) -> pool (:24) -> [dropout = identity in eval (:25)] -> conv2+tanh (:26)
 //   -> pool (:27) -> view(-1, MAGICNUM) (:29) -> 2-layer LSTM (:30) -> Linear (:31)
 //   -> * relu(age*1e-8+1) (:32-33) -> squeeze (:34)

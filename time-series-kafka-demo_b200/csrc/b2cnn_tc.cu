@@ -1,8 +1,8 @@
-// b2cnn_tc.cu -- tcgen05 / TMEM / TMA front end for bf16 windows (sm_100a).
+// b2cnn_tc.cu -- wgmma / TMA front end for bf16 windows (sm_90a).
 //
 // conv1 (bin/models.py:23) is 82 % of the path's FLOPs at the headline shape [4096,3,75000]:
-// 9.0 M MAC per window, which on the FP32 CUDA cores alone costs ~4x the time the HBM roofline
-// allows.  Here it runs on the 5th-gen tensor cores as a banded-Toeplitz GEMM whose M axis is
+// 9.0 M MAC per window, which on the FP32 CUDA cores alone costs several times what the HBM
+// roofline allows.  Here it runs on the tensor cores as a banded-Toeplitz GEMM whose M axis is
 // the WINDOW index:
 //
 //   D[w, (s,o)] = sum_{c} sum_{k<16}  X_c[w, 8n+k] * T_c[k, (s,o)],   T_c[k,(s,o)] = w1[o][c][k-s]
@@ -14,22 +14,14 @@
 //     (tiles advance by 56 samples; the 8 overlapping samples are re-read from L2, not HBM).
 //   * B = T_c: the fp32 conv1 weights expanded to a 16 x 32 band matrix (8 output shifts s x 4
 //     output channels o) and split into 2 or 3 bf16 pieces (hi/mid/lo) so that, the inputs
-//     being exactly bf16, every product is exact and the fp32 accumulation in TMEM carries the
-//     full fp32 weight precision.  One MMA (M=128,N=32,K=16) per (block, channel, piece).
+//     being exactly bf16, every product is exact and the fp32 accumulation carries the full
+//     fp32 weight precision.  One wgmma m64n32k16 per (row half, block, channel, piece).
 //   * The one tap that does not fit a 16-sample slice (s=7, k=9 -> sample 8n+16) is added by
 //     the epilogue on the CUDA cores from the same shared-memory tile (12 FMA per block).
-//   * Epilogue: thread == window.  Each thread streams through its window's positions in
-//     order, so pool1 -> tanh -> conv2 -> pool2 -> tanh are register-local sliding windows with
-//     no shuffles, seams or shared-memory exchange; tanh is 1 - 2/(1+2^(2x log2 e)) on
-//     MUFU.EX2 + MUFU.RCP with the bias folded into the exponent FMA; pooling runs BEFORE the
-//     activation (monotone) with FMNMX3.NAN so NaNs propagate exactly like ATen's max_pool1d.
 //   * Zero band entries turn an inf/NaN sample into NaN for its whole 8-position block, a
 //     superset of the reference's NaNs: a window whose features contain a NaN is flagged and
 //     recomputed by the exact generic kernel (b2cnn_generic.cu), still on the GPU.
-//
-// Warp roles per CTA (192 threads, 2 CTAs/SM): warp 0 TMA producer, warp 1 TMEM allocator +
-// single-thread MMA issuer, warps 2-5 epilogue (TMEM lane quadrant = warp % 4).
-// Pipelines: 2 smem stages (full/empty mbarriers), 2 TMEM accumulator stages of 4+3 blocks.
+// The kernel itself, its epilogue and the fused layer-0 projection are in b2cnn_tc_fused.cuh.
 #include <cuda.h>
 
 #include <cstdlib>
@@ -41,9 +33,6 @@
 
 namespace b2cnn {
 
-// kind::f16 instruction descriptor: D=f32, A=B=bf16, both K-major, M=128, N=32 (conv1 bands)
-constexpr uint32_t kIdesc = make_idesc_bf16(128, 32);
-
 static thread_local const char *g_tc_err = "";
 const char *tc_error() { return g_tc_err; }
 
@@ -51,211 +40,12 @@ const char *tc_error() { return g_tc_err; }
 #define B2CNN_OWN_FLAGS 1          // NaN-exception flag state owned by the handle and cleaned by the head kernel: no per-call memset (TcState)
 #endif
 constexpr int64_t kOwnFlagCap = 65536;   // windows per call served by the handle's own flag state (512 KB); larger batches use the workspace copy
-constexpr int kTcM = 128;          // windows per CTA == UMMA M
+constexpr int kTcM = 128;          // windows per CTA (two wgmma m64 row halves)
 constexpr int kTcAdv = 56;         // conv1 positions (= samples) a tile advances
 constexpr int kTcBlocks = 7;       // 8-position blocks per 64-sample tile
 constexpr int kTcABytes = 128 * 128;
 constexpr int kTcBBytes = 32 * 16 * 2;   // one band matrix piece: N=32 x K=16 bf16
 constexpr int kTcMaxC = 4;
-constexpr int kTcThreads = 192;
-
-struct TcParams {
-    float *feats;
-    int64_t sB, sP;
-    int *nanflag;
-    const uint8_t *bmats;     // [C][SPLITS][1024] bytes, UMMA K-major no-swizzle core-matrix order
-    int B, W, L;
-    int tiles_per_cta, feats_per_cta;
-    float w9[kCMid][kTcMaxC];   // tap k=9 of conv1: w1[o][c][9]
-    float b1s[kCMid];           // conv1 bias * 2 log2 e
-    float w2[kCMid][5];
-    float b2s;                  // conv2 bias * 2 log2 e
-};
-
-// ------------------------------------------------------------------------------------------
-// The kernel (MyCNN5 architecture: K1=10, pool(3,2), K2=5)
-// ------------------------------------------------------------------------------------------
-template <int C, int SPLITS>
-__global__ void __launch_bounds__(kTcThreads, 2)
-tc_frontend_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ TcParams p) {
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    uint8_t *sA = smem;                                    // [2 stages][C][16 KB]
-    uint8_t *sBm = smem + 2 * C * kTcABytes;               // [C][SPLITS][1 KB]
-    uint64_t *bars = reinterpret_cast<uint64_t *>(sBm + C * SPLITS * kTcBBytes);
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(bars + 8);
-    const uint32_t bar_full = smem_u32(bars + 0), bar_empty = smem_u32(bars + 2);
-    const uint32_t bar_tfull = smem_u32(bars + 4), bar_tempty = smem_u32(bars + 6);
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int b0 = blockIdx.x * kTcM;
-    const int p0 = blockIdx.y * p.feats_per_cta;
-    const int nfeat = min(p.feats_per_cta, p.L - p0);
-    const int nsteps = (nfeat + 4) / 2;                    // features 2j-3, 2j-2 leave at step j
-    const int ntiles = (nsteps + kTcBlocks - 1) / kTcBlocks;
-    const int T0 = p0 * 4;                                 // first conv1 position == first sample
-
-    // band matrices -> smem (generic proxy), barriers, TMEM
-    for (int i = threadIdx.x; i < C * SPLITS * kTcBBytes / 16; i += kTcThreads)
-        reinterpret_cast<uint4 *>(sBm)[i] = reinterpret_cast<const uint4 *>(p.bmats)[i];
-    if (threadIdx.x == 0) {
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(bar_full + 8 * i, 1);
-            mbar_init(bar_empty + 8 * i, 4);
-            mbar_init(bar_tfull + 8 * i, 1);
-            mbar_init(bar_tempty + 8 * i, 4);
-        }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(256) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // band matrices visible to the tensor core
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-
-    if (warp == 0) {
-        // ===================== TMA producer =====================
-        if (lane == 0) {
-            for (int i = 0; i < ntiles; ++i) {
-                const int s = i & 1, ph = (i >> 1) & 1;
-                mbar_wait(bar_empty + 8 * s, ph ^ 1);
-                mbar_expect_tx(bar_full + 8 * s, C * kTcABytes);
-#pragma unroll
-                for (int c = 0; c < C; ++c)
-                    tma_load_3d(smem_u32(sA + (s * C + c) * kTcABytes), &tmap, T0 + kTcAdv * i, c, b0, bar_full + 8 * s);
-            }
-        }
-    } else if (warp == 1) {
-        // ===================== MMA issuer =====================
-        // whole warp runs the loop (warp-uniform descriptor arithmetic); one elected lane issues
-        const uint64_t a_base = desc_sw128_kmajor(smem_u32(sA));
-        const uint64_t b_base = desc_none_kmajor(smem_u32(sBm), 128, 256);
-        const uint32_t a_lo0 = (uint32_t)a_base, a_hi = (uint32_t)(a_base >> 32);
-        const uint32_t b_lo0 = (uint32_t)b_base, b_hi = (uint32_t)(b_base >> 32);
-        for (int i = 0; i < ntiles; ++i) {
-            const int s = i & 1, ph = (i >> 1) & 1;
-            mbar_wait(bar_full + 8 * s, ph);
-            tc_fence_after();
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                mbar_wait(bar_tempty + 8 * h, (i & 1) ^ 1);
-                tc_fence_after();
-                if (elect_one()) {
-                    const int nb0 = h ? 4 : 0, nb1 = h ? kTcBlocks : 4;
-                    for (int n = nb0; n < nb1; ++n) {
-                        const uint32_t d = tmem_base + h * 128 + (n - nb0) * 32;
-                        const uint32_t a_s = a_lo0 + (uint32_t)(s * C) * (kTcABytes >> 4) + n;
-#pragma unroll
-                        for (int c = 0; c < C; ++c)
-#pragma unroll
-                            for (int sp = 0; sp < SPLITS; ++sp)
-                                umma_ss(d, a_s + c * (kTcABytes >> 4), a_hi, b_lo0 + (c * SPLITS + sp) * (kTcBBytes >> 4), b_hi, kIdesc,
-                                        (c | sp) != 0);
-                    }
-                    umma_commit(bar_tfull + 8 * h);
-                }
-                __syncwarp();
-            }
-        }
-    } else {
-        // ===================== epilogue: thread == window =====================
-        const int q = warp & 3;
-        const int row = q * 32 + lane;
-        const int b = b0 + row;
-        const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16);
-        const uint32_t swz = (uint32_t)(row & 7);
-        float pm6[kCMid], pm7[kCMid], ah[4][kCMid], c2c = 0.f, nan_probe = 0.f;
-#pragma unroll
-        for (int o = 0; o < kCMid; ++o) {
-            pm6[o] = 0.f; pm7[o] = 0.f;
-#pragma unroll
-            for (int i = 0; i < 4; ++i) ah[i][o] = 0.f;
-        }
-        const bool row_ok = b < p.B;
-        float *fout = p.feats + (int64_t)b * p.sB + (int64_t)p0 * p.sP;
-
-        for (int i = 0; i < ntiles; ++i) {
-            const int s = i & 1;
-            mbar_wait(bar_full + 8 * s, (i >> 1) & 1);     // TMA bytes visible to this thread too
-            const uint8_t *tile = sA + (size_t)s * C * kTcABytes + row * 128;
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                mbar_wait(bar_tfull + 8 * h, i & 1);
-                tc_fence_after();
-                const int nb0 = h ? 4 : 0, nb1 = h ? kTcBlocks : 4;
-#pragma unroll
-                for (int n = nb0; n < nb1; ++n) {
-                    float D[32];
-                    tmem_ld32(taddr + h * 128 + (n - nb0) * 32, D);
-                    if (n == nb1 - 1) {                    // accumulator stage drained -> MMA may refill it
-                        tc_fence_before();
-                        __syncwarp();
-                        if (lane == 0) mbar_arrive(bar_tempty + 8 * h);
-                    }
-                    const int j = i * kTcBlocks + n;       // global step index
-                    // ---- the tap that does not fit the 16-sample slice: previous block's s=7, k=9
-#pragma unroll
-                    for (int c = 0; c < C; ++c) {
-                        const uint16_t raw = *reinterpret_cast<const uint16_t *>(
-                            tile + c * kTcABytes + ((uint32_t)((n + 1) ^ swz) << 4));
-                        const float xv = __uint_as_float((uint32_t)raw << 16);
-#pragma unroll
-                        for (int o = 0; o < kCMid; ++o) pm7[o] = fmaf(p.w9[o][c], xv, pm7[o]);
-                    }
-                    // ---- pool1 (3,2) on pre-activations, then tanh(+bias): a1 positions 4j-1 .. 4j+2
-                    float an[4][kCMid];
-#pragma unroll
-                    for (int o = 0; o < kCMid; ++o) {
-                        an[0][o] = tanh_fold(max3_nan(pm6[o], pm7[o], D[0 * 4 + o]), p.b1s[o]);
-                        an[1][o] = tanh_fold(max3_nan(D[0 * 4 + o], D[1 * 4 + o], D[2 * 4 + o]), p.b1s[o]);
-                        an[2][o] = tanh_fold(max3_nan(D[2 * 4 + o], D[3 * 4 + o], D[4 * 4 + o]), p.b1s[o]);
-                        an[3][o] = tanh_fold(max3_nan(D[4 * 4 + o], D[5 * 4 + o], D[6 * 4 + o]), p.b1s[o]);
-                        pm6[o] = D[6 * 4 + o];
-                        pm7[o] = D[7 * 4 + o];
-                    }
-                    // ---- conv2 (no bias yet): outputs r = 4j-5 .. 4j-2 from a1[r .. r+4]
-                    float c2[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-                    for (int c = 0; c < kCMid; ++c) {
-                        const float A8[8] = {ah[0][c], ah[1][c], ah[2][c], ah[3][c], an[0][c], an[1][c], an[2][c], an[3][c]};
-#pragma unroll
-                        for (int k = 0; k < 5; ++k)
-#pragma unroll
-                            for (int r = 0; r < 4; ++r) c2[r] = fmaf(p.w2[c][k], A8[r + k], c2[r]);
-                    }
-#pragma unroll
-                    for (int c = 0; c < kCMid; ++c)
-#pragma unroll
-                        for (int r = 0; r < 4; ++r) ah[r][c] = an[r][c];
-                    // ---- pool2 (3,2) + tanh(+bias): features 2j-3 and 2j-2
-                    const float f0 = tanh_fold(max3_nan(c2c, c2[0], c2[1]), p.b2s);
-                    const float f1 = tanh_fold(max3_nan(c2[1], c2[2], c2[3]), p.b2s);
-                    c2c = c2[3];
-                    nan_probe = fmaf(f0, 0.f, nan_probe);
-                    nan_probe = fmaf(f1, 0.f, nan_probe);
-                    const int pr0 = 2 * j - 3;
-                    if (row_ok) {
-                        if (pr0 >= 0 && pr0 < nfeat) fout[(int64_t)pr0 * p.sP] = f0;
-                        if (pr0 + 1 >= 0 && pr0 + 1 < nfeat) fout[(int64_t)(pr0 + 1) * p.sP] = f1;
-                    }
-                }
-            }
-            __syncwarp();
-            if (lane == 0) mbar_arrive(bar_empty + 8 * s);   // smem stage fully consumed
-        }
-        if (row_ok && nan_probe != nan_probe) p.nanflag[b] = 1;
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(256) : "memory");
-    }
-}
 
 // windows flagged by the tensor-core kernel -> compact index list for the exact re-computation
 __global__ void tc_compact_flags_kernel(int *flags, int B, int *list, int *count) {
@@ -265,7 +55,6 @@ __global__ void tc_compact_flags_kernel(int *flags, int B, int *list, int *count
 
 }  // namespace b2cnn
 #include "b2cnn_tc_fused.cuh"
-#include "b2cnn_stream_f32.cuh"
 namespace b2cnn {
 
 // ------------------------------------------------------------------------------------------
@@ -332,13 +121,11 @@ int tc_prepare(TcState &s, const Dims &d, const ConvWeights &cw, const float *d_
         }
     }
 #endif
-    // band matrices: piece sp of T_c[k][(s,o)] = w1[o][c][k-s], stored as UMMA K-major
+    // band matrices: piece sp of T_c[k][(s,o)] = w1[o][c][k-s], stored as GMMA K-major
     // no-swizzle core matrices: byte = (n/8)*256 + (k/8)*128 + (n%8)*16 + (k%8)*2, n = s*4+o.
     //   d_bmats   [C][3][1 KB]  three bf16 pieces (hi/mid/lo: the full 24-bit fp32 mantissa)
     //   d_bmats2  [C][2][1 KB]  the first two pieces only (16 mantissa bits; tc_splits=2, an option:
     //                           6 instead of 9 MMAs per block, weights rounded to 2^-17 relative)
-    // (A mixed-format MMA -- bf16 samples x fp16 weight pieces, 22 bits in two pieces -- was tried:
-    //  kind::f16 with a_format != b_format raises "illegal instruction" on sm_100a.)
     std::vector<uint16_t> host((size_t)d.C * 3 * 512, 0), host2((size_t)d.C * 2 * 512, 0);
     for (int c = 0; c < d.C; ++c)
         for (int sft = 0; sft < 8; ++sft)
@@ -474,7 +261,7 @@ static const void *tc_stage_input(const Dims &d, const void *x, int64_t B, void 
 static int tiles_per_cta_for(const Dims &d) {
     // About 37 position ranges per window whatever its length (depends on L only, so a window's
     // summation order never depends on the batch): L=18745 -> 37 tiles (514 features) per CTA and
-    // 37 ranges x 16 window-tile pairs = 592 CTAs = 4 waves of 148 at B=4096; shorter windows get
+    // 37 ranges x 32 window tiles = 1184 CTAs = 9 waves of 132 at B=4096; shorter windows get
     // proportionally shorter ranges so that small batches still fill the SMs.
     if (const char *e = getenv("B2CNN_TC_TILES")) { const int v = atoi(e); if (v >= 1 && v <= 4096) return v; }
     int nt = ((d.L + 36) / 37 + 4 + 13) / 14;
@@ -484,7 +271,7 @@ static int tiles_per_cta_for(const Dims &d) {
 }
 
 static int tiles_per_cta_s_for(const Dims &d) {
-    // stream_f32_kernel: about 37 position ranges (L only) like the bf16 kernel; a CTA's stream emits
+    // fp32 windows: about 37 position ranges (L only) like the bf16 kernel; a CTA's stream emits
     // 6*tiles - 4 features (even: every range starts 16-byte aligned for TMA)
     if (const char *e = getenv("B2CNN_SF_TILES")) { const int v = atoi(e); if (v >= 1 && v <= 16384) return v; }
     int nt = ((d.L + 36) / 37 + 4 + 5) / 6;
@@ -492,51 +279,74 @@ static int tiles_per_cta_s_for(const Dims &d) {
     return nt;
 }
 
+// epilogue constants of tc_stream_kernel (conv2 consumes r = (1 - tanh)/2: sum w*(1 - 2r) = sum(w) + sum (-2w)*r)
+static void fill_epilogue(TcFusedParams &p, const Dims &d, const ConvWeights &cw) {
+    for (int o = 0; o < kCMid; ++o) {
+        for (int c = 0; c < d.C; ++c) {
+            for (int k = 0; k < d.K1; ++k) p.w1[c][k][o] = cw.w1[(c * d.K1 + k) * kCMid + o];
+            p.w9[c][o] = d.K1 == 10 ? cw.w1[(c * d.K1 + 9) * kCMid + o] : 0.f;
+        }
+        p.b1s[o] = cw.b1[o] * k2Log2e;
+        for (int k = 0; k < 5; ++k) p.w2n[o][k] = -2.f * cw.w2[o * d.K2 + k];
+    }
+    double sw = 0.0;
+    for (int i = 0; i < kCMid * d.K2; ++i) sw += cw.w2[i];
+    p.b2s = (float)((cw.b2 + sw) * (double)k2Log2e);
+}
+
+// one launch of tc_stream_kernel<C, SPLITS, ARCH, F32IN, OUT> over grid (window tiles, position ranges)
+template <int C, int SPLITS, int ARCH, bool F32IN, int OUT>
+static cudaError_t launch_stream(const CUtensorMap &tm, const TcFusedParams &p, dim3 grid, cudaStream_t st) {
+    const size_t smem = hp_smem_bytes(C, SPLITS, F32IN, OUT);
+    cudaError_t e = cudaFuncSetAttribute(tc_stream_kernel<C, SPLITS, ARCH, F32IN, OUT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    tc_stream_kernel<C, SPLITS, ARCH, F32IN, OUT><<<grid, kHpThreads, smem, st>>>(tm, p);
+    return cudaGetLastError();
+}
+
+static int make_tmap(const Dims &d, const void *x, int64_t pitch, int64_t B, bool f32, CUtensorMap *tm, const char **err) {
+    if ((reinterpret_cast<uintptr_t>(x) & 15) != 0) { *err = "x must be 16-byte aligned for TMA"; return -1; }
+    const int esz = f32 ? 4 : 2;
+    cuuint64_t gdim[3] = {(cuuint64_t)d.W, (cuuint64_t)d.C, (cuuint64_t)B};
+    cuuint64_t gstr[2] = {(cuuint64_t)pitch * esz, (cuuint64_t)d.C * pitch * esz};
+    cuuint32_t box[3] = {(cuuint32_t)(128 / esz), 1, kTcM};       // 128-byte rows: one SWIZZLE_128B row per window
+    cuuint32_t estr[3] = {1, 1, 1};
+    CUresult r = get_encode()(tm, f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void *>(x),
+                              gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                              CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) { *err = "cuTensorMapEncodeTiled failed"; return -1; }
+    return 0;
+}
+
 static int launch_tc_kernel(const TcState &s, const Dims &d, const ConvWeights &cw, const void *x, int64_t pitch, int64_t B,
                             float *feats, int64_t sB, int64_t sP, int *nanflag, cudaStream_t st, const char **err) {
-    if ((reinterpret_cast<uintptr_t>(x) & 15) != 0) { *err = "x must be 16-byte aligned for TMA"; return -1; }
     CUtensorMap tm;
-    cuuint64_t gdim[3] = {(cuuint64_t)d.W, (cuuint64_t)d.C, (cuuint64_t)B};
-    cuuint64_t gstr[2] = {(cuuint64_t)pitch * 2, (cuuint64_t)d.C * pitch * 2};
-    cuuint32_t box[3] = {64, 1, kTcM};
-    cuuint32_t estr[3] = {1, 1, 1};
-    CUresult r = get_encode()(&tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void *>(x), gdim, gstr, box, estr,
-                              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { *err = "cuTensorMapEncodeTiled failed"; return -1; }
-    TcParams p;
+    if (make_tmap(d, x, pitch, B, false, &tm, err) != 0) return -1;
+    TcFusedParams p;
     memset(&p, 0, sizeof p);
     p.feats = feats; p.sB = sB; p.sP = sP; p.nanflag = nanflag;
     p.bmats = reinterpret_cast<const uint8_t *>(s.d_bmats);
     p.B = (int)B; p.W = d.W; p.L = d.L;
-    // a CTA's stream can emit 14*tiles - 3 features; an EVEN count keeps every range's first
-    // sample (4 * p0 elements) 16-byte aligned: an unaligned TMA box start faults (measured).
+    // an EVEN feature count per range keeps every range's first sample (4 * p0 elements) 16-byte aligned:
+    // an unaligned TMA box start faults
     p.tiles_per_cta = s.tiles_per_cta;
     p.feats_per_cta = s.feats_per_cta;
-    for (int o = 0; o < kCMid; ++o) {
-        for (int c = 0; c < d.C; ++c) p.w9[o][c] = cw.w1[(c * d.K1 + 9) * kCMid + o];
-        p.b1s[o] = cw.b1[o] * k2Log2e;
-        for (int k = 0; k < 5; ++k) p.w2[o][k] = cw.w2[o * d.K2 + k];
-    }
-    p.b2s = cw.b2 * k2Log2e;
+    fill_epilogue(p, d, cw);
     const int n_pr = (d.L + p.feats_per_cta - 1) / p.feats_per_cta;
     dim3 grid((unsigned)((B + kTcM - 1) / kTcM), n_pr);
-    const size_t smem = (size_t)2 * d.C * kTcABytes + (size_t)d.C * 3 * kTcBBytes + 256 + 1024;
-#define TC_LAUNCH(CC, SS)                                                                              \
-    if (d.C == CC) {                                                                 \
-        cudaError_t e = cudaFuncSetAttribute(tc_frontend_kernel<CC, SS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
-        if (e != cudaSuccess) { *err = cudaGetErrorString(e); return -1; }                             \
-        tc_frontend_kernel<CC, SS><<<grid, kTcThreads, smem, st>>>(tm, p);                             \
-    } else
-    TC_LAUNCH(3, 3) TC_LAUNCH(1, 3) TC_LAUNCH(2, 3) TC_LAUNCH(4, 3)
-    { *err = "no tensor-core instantiation for this channel count"; return -1; }
-#undef TC_LAUNCH
-    cudaError_t e = cudaGetLastError();
+    cudaError_t e;
+    switch (d.C) {
+        case 1: e = launch_stream<1, 3, 0, false, kOutFeatures>(tm, p, grid, st); break;
+        case 2: e = launch_stream<2, 3, 0, false, kOutFeatures>(tm, p, grid, st); break;
+        case 3: e = launch_stream<3, 3, 0, false, kOutFeatures>(tm, p, grid, st); break;
+        case 4: e = launch_stream<4, 3, 0, false, kOutFeatures>(tm, p, grid, st); break;
+        default: *err = "no tensor-core instantiation for this channel count"; return -1;
+    }
     if (e != cudaSuccess) { *err = cudaGetErrorString(e); return -1; }
     return 1;
 }
 
-// TMA/tcgen05 front end + NaN-flag compaction + exact re-computation of flagged windows.
+// TMA/wgmma front end + NaN-flag compaction + exact re-computation of flagged windows.
 // `ws`: 2*B+64 ints of scratch (flags, list, count); pass nullptr to allocate stream-ordered.
 int tc_frontend(TcState &s, const Dims &d, const ConvWeights &cw, const void *x, int64_t B, float *feats,
                 int64_t sB, int64_t sP, void *ws, int num_sms, cudaStream_t st, const char **err) {
@@ -599,19 +409,6 @@ static int flag_bufs(TcState &s, void *ws, int64_t B, cudaStream_t st, bool clea
     return 0;
 }
 
-static int make_tmap(const Dims &d, const void *x, int64_t pitch, int64_t B, CUtensorMap *tm, const char **err) {
-    if ((reinterpret_cast<uintptr_t>(x) & 15) != 0) { *err = "x must be 16-byte aligned for TMA"; return -1; }
-    cuuint64_t gdim[3] = {(cuuint64_t)d.W, (cuuint64_t)d.C, (cuuint64_t)B};
-    cuuint64_t gstr[2] = {(cuuint64_t)pitch * 2, (cuuint64_t)d.C * pitch * 2};
-    cuuint32_t box[3] = {64, 1, kTcM};
-    cuuint32_t estr[3] = {1, 1, 1};
-    CUresult r = get_encode()(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void *>(x), gdim, gstr, box, estr,
-                              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { *err = "cuTensorMapEncodeTiled failed"; return -1; }
-    return 0;
-}
-
 // fused front end + projection -> gates[B][64]; flagged (NaN) windows are recomputed exactly.
 int tc_fused_gates(TcState &s, const Dims &d, const ConvWeights &cw, const HeadWeights &hw, const void *x, int64_t B,
                    float *feats, float *partial, float *gates, void *ws, int num_sms, cudaStream_t st, const char **err,
@@ -624,53 +421,27 @@ int tc_fused_gates(TcState &s, const Dims &d, const ConvWeights &cw, const HeadW
     int64_t pitch = d.XP;
     const void *xin = tc_stage_input(d, x, B, reinterpret_cast<char *>(ws) + flags_bytes(B), &pitch, &staged, st);
     CUtensorMap tm;
-    if (make_tmap(d, xin, pitch, B, &tm, err) != 0) return -1;
+    if (make_tmap(d, xin, pitch, B, false, &tm, err) != 0) return -1;
     TcFusedParams p;
     memset(&p, 0, sizeof p);
     p.partial = partial; p.nanflag = flags; p.list = list; p.count = count;
     p.wpack = reinterpret_cast<const uint8_t *>(s.d_wpack);
     p.B = (int)B; p.W = d.W; p.L = d.L;
     p.tiles_per_cta = s.tiles_per_cta; p.feats_per_cta = s.feats_per_cta; p.chunks_per_cta = s.chunks_per_cta;
-    for (int q2 = 0; q2 < 2; ++q2) {
-        for (int c = 0; c < d.C; ++c)
-            p.w9p[c][q2] = d.K1 == 10 ? make_float2(cw.w1[(c * d.K1 + 9) * kCMid + 2 * q2], cw.w1[(c * d.K1 + 9) * kCMid + 2 * q2 + 1])
-                                      : make_float2(0.f, 0.f);
-        p.b1sp[q2] = make_float2(cw.b1[2 * q2] * k2Log2e, cw.b1[2 * q2 + 1] * k2Log2e);
-        // conv2 consumes r = (1 - tanh)/2 of conv1: sum w*(1 - 2r) = sum(w) + sum (-2w)*r
-        for (int k = 0; k < 5; ++k) p.w2p[q2][k] = make_float2(-2.f * cw.w2[(2 * q2) * d.K2 + k], -2.f * cw.w2[(2 * q2 + 1) * d.K2 + k]);
-    }
-    {
-        double sw = 0.0;
-        for (int i = 0; i < kCMid * d.K2; ++i) sw += cw.w2[i];
-        p.b2s = (float)((cw.b2 + sw) * (double)k2Log2e);
-    }
-    const int arch_id = d.K1 == 10 ? 0 : 1;
+    fill_epilogue(p, d, cw);
     const int sp = s.splits;                          // bf16 pieces per conv1 weight: 3 (fp32-equivalent) or 2
     p.bmats = reinterpret_cast<const uint8_t *>(sp == 2 ? s.d_bmats2 : s.d_bmats);
-    cudaError_t le = cudaSuccess;
-    bool launched = false;
-    {
-        // persistent grid: one CTA per SM (218 KB of shared memory and all 512 TMEM columns each), static round-robin over
-        // the (window-tile pair, position range) items
-        const int64_t n_items = ((B + 2 * kTcM - 1) / (2 * kTcM)) * s.n_ranges;
-        if (n_items > 0x7fffffff) { *err = "batch too large for the fused kernel's item index"; return -1; }
-        p.n_ranges = s.n_ranges; p.n_items = (int)n_items;
-        dim3 grid((unsigned)(n_items < num_sms ? n_items : num_sms));
-        const size_t smem = (size_t)4 * d.C * kTcABytes + (size_t)d.C * sp * kTcBBytes + 2 * kFuWChunkBytes + FuBars::kTotal * 8 + 16;
-#define FU_LAUNCH(CC, SS, AA)                                                                          \
-        if (!launched && d.C == CC && sp == SS && arch_id == AA) {                                     \
-            le = cudaFuncSetAttribute(tc_fused_kernel<CC, SS, AA>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
-            if (le == cudaSuccess) tc_fused_kernel<CC, SS, AA><<<grid, kFuThreads, smem, st>>>(tm, p); \
-            launched = true;                                                                           \
-        }
-        FU_LAUNCH(3, 2, 0) FU_LAUNCH(3, 3, 0) FU_LAUNCH(2, 2, 0) FU_LAUNCH(1, 2, 0) FU_LAUNCH(2, 3, 0) FU_LAUNCH(1, 3, 0)
-        FU_LAUNCH(3, 2, 1) FU_LAUNCH(3, 3, 1) FU_LAUNCH(2, 2, 1) FU_LAUNCH(1, 2, 1) FU_LAUNCH(2, 3, 1) FU_LAUNCH(1, 3, 1)
-#undef FU_LAUNCH
+    dim3 grid((unsigned)((B + kTcM - 1) / kTcM), s.n_ranges);
+    const int key = d.C * 100 + sp * 10 + (d.K1 == 10 ? 0 : 1);
+    cudaError_t le;
+    switch (key) {
+#define FU_CASE(CC, SS, AA) case CC * 100 + SS * 10 + AA: le = launch_stream<CC, SS, AA, false, kOutGates>(tm, p, grid, st); break;
+        FU_CASE(1, 2, 0) FU_CASE(2, 2, 0) FU_CASE(3, 2, 0) FU_CASE(1, 3, 0) FU_CASE(2, 3, 0) FU_CASE(3, 3, 0)
+        FU_CASE(1, 2, 1) FU_CASE(2, 2, 1) FU_CASE(3, 2, 1) FU_CASE(1, 3, 1) FU_CASE(2, 3, 1) FU_CASE(3, 3, 1)
+#undef FU_CASE
+        default: *err = "no fused instantiation for this channel count / split"; return -1;
     }
-    if (!launched) { *err = "no fused instantiation for this channel count / split"; return -1; }
     if (le != cudaSuccess) { *err = cudaGetErrorString(le); return -1; }
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) { *err = cudaGetErrorString(e); return -1; }
     int launches = 1 + staged;
     if (slices_out) *slices_out = s.n_ranges;
     // the exception path: exact gate partials of the flagged windows, written over their rows of `partial`
@@ -684,15 +455,6 @@ int tc_fused_gates(TcState &s, const Dims &d, const ConvWeights &cw, const HeadW
     return launches + n;
 }
 
-#ifdef B2CNN_TIMING
-// experiments only: read and clear the fused kernel's wait counters (cycles summed over warps and CTAs)
-extern "C" int b2cnn_debug_timing(unsigned long long *out16) {
-    if (cudaMemcpyFromSymbol(out16, g_fu_timing, sizeof(unsigned long long) * 16) != cudaSuccess) return -1;
-    unsigned long long z[16] = {0};
-    return cudaMemcpyToSymbol(g_fu_timing, z, sizeof z) == cudaSuccess ? 0 : -1;
-}
-#endif
-
 bool tc_stream_supported(const TcState &s, const Dims &d, int dtype) {
     return s.ready && s.stream_ready && dtype == B2CNN_DTYPE_F32 && (arch_ok(d) || arch1_ok(d)) && d.C <= 3 && (d.XP % 4) == 0;
 }
@@ -704,54 +466,25 @@ int tc_stream_gates(TcState &s, const Dims &d, const ConvWeights &cw, const Head
     (void)feats;
     if (flag_bufs(s, ws, B, st, !reduce_here, err) != 0) return -1;
     int *count = s.cur_count, *flags = s.cur_flags, *list = s.cur_list;
-    if ((reinterpret_cast<uintptr_t>(x) & 15) != 0) { *err = "x must be 16-byte aligned for TMA"; return -1; }
     CUtensorMap tm;
-    {
-        cuuint64_t gdim[3] = {(cuuint64_t)d.W, (cuuint64_t)d.C, (cuuint64_t)B};
-        cuuint64_t gstr[2] = {(cuuint64_t)d.XP * 4, (cuuint64_t)d.C * d.XP * 4};
-        cuuint32_t box[3] = {32, 1, kTcM};
-        cuuint32_t estr[3] = {1, 1, 1};
-        CUresult r = get_encode()(&tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<void *>(x), gdim, gstr, box, estr,
-                                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) { *err = "cuTensorMapEncodeTiled (fp32) failed"; return -1; }
-    }
-    StreamF32Params pp;
-    memset(&pp, 0, sizeof pp);
-    TcFusedParams &p = pp.f;
+    if (make_tmap(d, x, d.XP, B, true, &tm, err) != 0) return -1;
+    TcFusedParams p;
+    memset(&p, 0, sizeof p);
     p.partial = partial; p.nanflag = flags; p.list = list; p.count = count;
     p.wpack = reinterpret_cast<const uint8_t *>(s.d_wpack_s);
     p.B = (int)B; p.W = d.W; p.L = d.L;
     p.tiles_per_cta = s.tiles_per_cta_s; p.feats_per_cta = s.feats_per_cta_s; p.chunks_per_cta = s.chunks_per_cta_s;
-    for (int q2 = 0; q2 < 2; ++q2) {
-        for (int c = 0; c < d.C; ++c)
-            for (int k = 0; k < d.K1; ++k)
-                pp.w1p[c][k][q2] = make_float2(cw.w1[(c * d.K1 + k) * kCMid + 2 * q2], cw.w1[(c * d.K1 + k) * kCMid + 2 * q2 + 1]);
-        p.b1sp[q2] = make_float2(cw.b1[2 * q2] * k2Log2e, cw.b1[2 * q2 + 1] * k2Log2e);
-        for (int k = 0; k < 5; ++k) p.w2p[q2][k] = make_float2(-2.f * cw.w2[(2 * q2) * d.K2 + k], -2.f * cw.w2[(2 * q2 + 1) * d.K2 + k]);
+    fill_epilogue(p, d, cw);
+    dim3 grid((unsigned)((B + kTcM - 1) / kTcM), s.n_ranges_s);
+    const int key = d.C * 10 + (d.K1 == 10 ? 0 : 1);
+    cudaError_t le;
+    switch (key) {
+#define SF_CASE(CC, AA) case CC * 10 + AA: le = launch_stream<CC, 1, AA, true, kOutGates>(tm, p, grid, st); break;
+        SF_CASE(1, 0) SF_CASE(2, 0) SF_CASE(3, 0) SF_CASE(1, 1) SF_CASE(2, 1) SF_CASE(3, 1)
+#undef SF_CASE
+        default: *err = "no fp32 stream instantiation for this channel count"; return -1;
     }
-    {
-        double sw = 0.0;
-        for (int i = 0; i < kCMid * d.K2; ++i) sw += cw.w2[i];
-        p.b2s = (float)((cw.b2 + sw) * (double)k2Log2e);
-    }
-    dim3 grid((unsigned)((B + 2 * kTcM - 1) / (2 * kTcM)), s.n_ranges_s);
-    const size_t smem = (size_t)4 * d.C * kSfABytes + 2 * kFuWChunkBytes + SfBars::kTotal * 8 + 16;
-    const int arch_id = d.K1 == 10 ? 0 : 1;
-    cudaError_t le = cudaSuccess;
-    bool launched = false;
-#define SF_LAUNCH(CC, AA)                                                                              \
-    if (!launched && d.C == CC && arch_id == AA) {                                                     \
-        le = cudaFuncSetAttribute(stream_f32_kernel<CC, AA>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
-        if (le == cudaSuccess) stream_f32_kernel<CC, AA><<<grid, kSfThreads, smem, st>>>(tm, pp);      \
-        launched = true;                                                                               \
-    }
-    SF_LAUNCH(3, 0) SF_LAUNCH(2, 0) SF_LAUNCH(1, 0) SF_LAUNCH(3, 1) SF_LAUNCH(2, 1) SF_LAUNCH(1, 1)
-#undef SF_LAUNCH
-    if (!launched) { *err = "no fp32 stream instantiation for this channel count"; return -1; }
     if (le != cudaSuccess) { *err = cudaGetErrorString(le); return -1; }
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) { *err = cudaGetErrorString(e); return -1; }
     int launches = 1;
     if (slices_out) *slices_out = s.n_ranges_s;
     int n = launch_frontend_generic_gates_listed(d, cw, x, B2CNN_DTYPE_F32, B, hw.wih0T, partial, s.n_ranges_s, list, count, st, num_sms, err);

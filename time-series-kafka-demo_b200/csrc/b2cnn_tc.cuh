@@ -1,4 +1,4 @@
-// b2cnn_tc.cuh -- interface of the tcgen05 (5th-gen tensor core) fast path, b2cnn_tc.cu.
+// b2cnn_tc.cuh -- interface of the wgmma (Hopper tensor core) fast path, b2cnn_tc.cu.
 #pragma once
 #include "b2cnn_internal.cuh"
 
@@ -11,10 +11,10 @@ struct TcState {
     void *d_bmats2 = nullptr;    // the first two pieces only (tc_splits=2)
     void *d_wpack = nullptr;     // W_ih_l0 packed per (position range, 16-position chunk), 3 bf16 pieces
     int tiles_per_cta = 37, feats_per_cta = 514, chunks_per_cta = 33, n_ranges = 1;
-    void *d_wpack_s = nullptr;   // the same packing for the 3-block tiles of stream_f32_kernel (fp32 windows)
+    void *d_wpack_s = nullptr;   // the same packing for the 3-block tiles of the fp32-window kernel
     int tiles_per_cta_s = 86, feats_per_cta_s = 512, chunks_per_cta_s = 33, n_ranges_s = 1;
-    bool stream_ready = false;   // stream_f32_kernel usable (C <= 3)
-    bool has_v1 = false;         // tc_frontend_kernel (features out) exists for this geometry (MyCNN5 only)
+    bool stream_ready = false;   // fp32-window kernel usable (C <= 3)
+    bool has_v1 = false;         // the features-out kernel exists for this geometry (MyCNN5 only)
     bool fused_ready = false;    // fused conv + projection kernel usable (C <= 3)
     int64_t opt_fused = 1;
     // Flag state of the streaming kernels' NaN exception path (count | flags [cap] | list [cap]) owned by the handle:
@@ -50,7 +50,7 @@ int tc_partial_slices(const TcState &s);
 int tc_fused_gates(TcState &s, const Dims &d, const ConvWeights &cw, const HeadWeights &hw, const void *x, int64_t B,
                    float *feats, float *partial, float *gates, void *ws, int num_sms, cudaStream_t st, const char **err,
                    bool reduce_here = true, int *slices_out = nullptr);
-// fp32 windows: streaming kernel with CUDA-core conv1 + tcgen05 projection (b2cnn_stream_f32.cuh)
+// fp32 windows: streaming kernel with CUDA-core conv1 + wgmma projection (b2cnn_tc_fused.cuh)
 bool tc_stream_supported(const TcState &s, const Dims &d, int dtype);
 int tc_stream_gates(TcState &s, const Dims &d, const ConvWeights &cw, const HeadWeights &hw, const void *x, int64_t B,
                     float *feats, float *partial, float *gates, void *ws, int num_sms, cudaStream_t st, const char **err,

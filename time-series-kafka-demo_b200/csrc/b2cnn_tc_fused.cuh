@@ -1,768 +1,367 @@
-// b2cnn_tc_fused.cuh -- the whole front end AND the LSTM layer-0 input projection in one
-// persistent-style kernel (included by b2cnn_tc.cu).
-//
-// On top of the banded-Toeplitz conv1 of tc_frontend_kernel (see b2cnn_tc.cu) this kernel keeps
-// the features on chip: every epilogue thread (== one window) splits the two features it
-// produces per step into three bf16 pieces and stores them into ITS OWN TMEM lane
-// (tcgen05.st), building the A operand [128 windows x 16 positions] of a second GEMM
+// b2cnn_tc_fused.cuh -- the streaming front end on sm_90a (included by b2cnn_tc.cu): conv1 -> pool1 -> tanh ->
+// conv2 -> pool2 -> tanh for 128 windows x one position range per CTA, the features either written out
+// (OUT = kOutFeatures) or multiplied on chip into the LSTM layer-0 input projection (OUT = kOutGates):
 //
 //      gates[w, g] += sum_p  f[w, p] * W_ih_l0[g, p]           (bin/models.py:30, layer 0)
 //
-// issued by the same MMA thread with A in TMEM and B = the packed, bf16-split W_ih chunk that
-// the producer streams with one 1-D bulk TMA per 16 positions.  6 MMAs (M=128, N=64, K=16;
-// piece pairs hh, hm, mh, hl, lh, mm) give fp32-equivalent products; the 64 gate
-// pre-activations accumulate in TMEM across the CTA's whole position range and leave once, as
-// a [range][window][64] partial that reduce_gates_kernel sums in fixed order.  The 307 MB
-// feature round trip through HBM and the CUDA-core projection GEMM disappear.
+// conv1 of bf16 windows is the banded-Toeplitz GEMM described in b2cnn_tc.cu, on wgmma: per 8-position block,
+// two m64n32k16 row halves x C channels x SPLITS weight pieces, A = the TMA tile (SWIZZLE_128B, the block's
+// 16-sample slice selected by a 16n-byte descriptor offset), B = the band-matrix piece, D in registers.  The
+// accumulator fragment (two windows x 16 values per thread) is turned into thread == window through an 18 KB
+// shared-memory transpose; the next block's MMAs run while the epilogue of this one computes.  fp32 windows
+// (F32IN) evaluate conv1 in exact fp32 FMAs straight from the tile instead (32-sample boxes, 3 blocks per tile).
 //
-// CTA = 2 window tiles (2 x 128 windows) x 1 position range, one CTA per SM, 384 threads, one
-// control warp + two epilogue warps on every SM sub-partition (warp % 4):
-//   warp 0      producer: TMA boxes for both window tiles
-//   warp 1 / 2  MMA issuer of window tile 0 / 1 (conv1 bands + projection), one elected lane
-//   warp 3      TMEM allocator (512 columns) + producer of the W_ih chunks
-//   warps 4-7   epilogue of window tile 0 (TMEM lane quadrant = warp % 4)
-//   warps 8-11  epilogue of window tile 1
-// TMEM columns per window tile (256): conv1 ring 4 x 32 | A pieces 2 x 24 | gates 64.
+// Epilogue, thread == window: each thread streams through its window's positions in order, so pool1 -> tanh ->
+// conv2 -> pool2 -> tanh are register-local sliding windows; tanh is 1 - 2/(1+2^(2x log2 e)) on MUFU.EX2 +
+// MUFU.RCP with the bias folded into the exponent FMA; pooling runs BEFORE the activation (monotone) with
+// max.NaN so NaNs propagate exactly like ATen's max_pool1d.  conv2 consumes r = (1 - tanh)/2 (weights
+// pre-multiplied by -2, the bias absorbs sum(w)).
+//
+// Projection: the two features of a step are split into three bf16 pieces and stored into a [128 x 16]
+// K-major A tile per piece; every 16 positions the warpgroup issues 2 row halves x 6 m64n64k16 MMAs (piece
+// pairs hh hm mh hl lh mm: fp32-equivalent products) against the packed W_ih chunk, accumulating the 64 gate
+// pre-activations in registers over the CTA's whole range.  They leave once, as partial[range][window][64].
+//
+// CTA = 192 threads: warps 0-3 the consumer warpgroup, warp 4 the TMA producer of the window tiles, warp 5 the
+// producer of the W_ih chunks (1-D bulk copies).
 #pragma once
-#include <type_traits>
-
 
 namespace b2cnn {
 
-// B2CNN_ABLATE (experiments only, see scripts/build_ablations.sh): 1 = epilogue without math (tensor/TMA-side
-// ceiling), 2 = MUFU replaced by FMUL, 3 = conv1 MMAs not issued (epilogue-side ceiling).  Results are garbage.
-#ifndef B2CNN_ABLATE
-#define B2CNN_ABLATE 0
-#endif
-// experiment switches (scripts/build_variants.sh): who spins and who parks on an mbarrier.  A parked warp
-// (try_wait with a suspend-time hint -> NANOSLEEP.SYNCS) costs no issue slots but wakes up late.
-#ifndef B2CNN_MMA_SPIN
-#define B2CNN_MMA_SPIN 0                          // MMA issuers: 1 = spin on the accumulator-ring / smem-stage barriers
-#endif
-#ifndef B2CNN_EPI_SPIN
-#define B2CNN_EPI_SPIN 1                          // epilogue: 1 = spin on the accumulator-ring barrier (A/B: parked 0.5423 -> spinning 0.5297 ms/step)
-#endif
-#ifndef B2CNN_SEGMENTS
-#define B2CNN_SEGMENTS 0                          // 1 = a scheduling fence (pmevent) after every segment of the epilogue iteration (A/B: slower)
-#endif
-#ifndef B2CNN_LDTM_SEG
-#define B2CNN_LDTM_SEG 8                          // segment after which the next block's accumulators are requested (-1: top of the iteration)
-#endif
-constexpr int kLdtmSeg = B2CNN_LDTM_SEG;
-#ifndef B2CNN_PARTIAL_EVICT_LAST
-#define B2CNN_PARTIAL_EVICT_LAST 0                // experiment: range partials stored with an L2 evict-last hint (A/B: head 18.5 -> 16.3 us, kernel +6 us: no gain)
-#endif
-#ifndef B2CNN_UNROLL8
-#define B2CNN_UNROLL8 1                           // epilogue main loop unrolled over one 8-step projection chunk (compile-time indices)
-#endif
-constexpr int kFuThreads = 384;
+constexpr int kHpThreads = 192;
+constexpr int kHpTStride = 36;                    // floats per window row of the accumulator transpose (conflict-free float4 reads)
+constexpr int kHpTBytes = kTcM * kHpTStride * 4;
+constexpr int kHpPieceBytes = kTcM * 16 * 2;      // one bf16 piece of the projection A operand
 constexpr int kFuWChunkBytes = 3 * 64 * 16 * 2;   // 3 pieces x (64 gates x 16 positions) bf16
-#ifndef B2CNN_COLLECTOR
-#define B2CNN_COLLECTOR 1
-#endif
-constexpr bool kFuCollector = B2CNN_COLLECTOR != 0;   // A-operand collector reuse across the piece-MMAs of a (block, channel)
-constexpr uint32_t kIdescProj = make_idesc_bf16(128, 64);
+constexpr int kSfBlocks = 3;                      // fp32 windows: 8-position blocks per 32-sample tile
+constexpr int kSfAdv = 24;
+constexpr int kOutFeatures = 0, kOutGates = 1;
 
 struct TcFusedParams {
-    float *partial;           // [n_ranges][B][64]
+    float *partial;           // [n_ranges][B][64]                 (kOutGates)
+    float *feats;             // feats[b * sB + p * sP]            (kOutFeatures)
+    int64_t sB, sP;
     int *nanflag;             // [B]
-    int *list, *count;        // flagged windows, compacted by the kernel itself: list[atomicAdd(count, 1)] = b (first flagger only)
+    int *list, *count;        // flagged windows: list[atomicAdd(count, 1)] = b (first flagger only)
     const uint8_t *bmats;     // conv1 band matrices [C][SPLITS][1 KB]
     const uint8_t *wpack;     // [n_ranges][chunks_per_cta][kFuWChunkBytes]
     int B, W, L;
     int tiles_per_cta, feats_per_cta, chunks_per_cta;
-    int n_ranges, n_items;    // work items = (pair of window tiles, position range), range fastest; CTA k runs items k, k + gridDim.x, ...
-    // epilogue constants, paired over (out-)channels (2q, 2q+1) for the packed f32x2 arithmetic
-    float2 w9p[kTcMaxC][2];    // tap k=9 of conv1: (w1[2q][c][9], w1[2q+1][c][9])
-    float2 b1sp[2];            // conv1 bias * 2 log2 e
-    float2 w2p[2][5];          // conv2 weights (w2[2q][k], w2[2q+1][k])
-    float b2s;                 // conv2 bias * 2 log2 e
+    float w1[kTcMaxC][10][kCMid];   // conv1 weights w1[o][c][k] (fp32 windows)
+    float w9[kTcMaxC][kCMid];       // tap k=9 of conv1 (bf16 windows, MyCNN5: it does not fit the 16-sample slice)
+    float b1s[kCMid];               // conv1 bias * 2 log2 e
+    float w2n[kCMid][5];            // -2 * conv2 weights
+    float b2s;                      // (conv2 bias + sum of conv2 weights) * 2 log2 e
 };
 
-// B2CNN_TIMING (experiments only, scripts/fused_timing.py): where the warps of the fused kernel wait.  Every waiting site
-// adds the cycles it spent to a global counter (lane 0 of each warp); b2cnn_debug_timing() reads and clears them.
-//   0 epilogue loop total | 1 TFull spin (conv1 accumulators not ready) | 2 smem-stage wait (tap-9 reads) | 3 PEmpty wait
-//   4 MMA loop total | 5 Full wait (TMA data late) | 6 TEmpty wait (ring full: epilogue behind) | 7 projection waits (W chunk + pieces)
-//   8 producer loop total | 9 Empty wait | 10 epilogue gate drain | 11 launches
-#ifdef B2CNN_TIMING
-__device__ unsigned long long g_fu_timing[16];
-#define FU_T0() const long long t0__ = clock64()
-#define FU_TACC(idx, cond) do { fu_tacc[(idx) & 3] += clock64() - t0__; } while (0)      // per-thread sums, flushed once (FU_TFLUSH)
-#define FU_TDECL() long long fu_tacc[4] = {0, 0, 0, 0}
-#define FU_TFLUSH(base, cond) do { if (cond) for (int i__ = 1; i__ < 4; ++i__) atomicAdd(&g_fu_timing[(base) + i__], (unsigned long long)fu_tacc[i__]); } while (0)
-#else
-#define FU_TDECL() do {} while (0)
-#define FU_TFLUSH(base, cond) do {} while (0)
-#define FU_T0() do {} while (0)
-#define FU_TACC(idx, cond) do {} while (0)
-#endif
-
-// compile-time loop: f(integral_constant<int, I>) for I in [0, N)
-template <int I, int N, typename F>
-__device__ __forceinline__ void static_for(F &&f) {
-    if constexpr (I < N) { f(std::integral_constant<int, I>{}); static_for<I + 1, N>(f); }
+__host__ __device__ constexpr size_t hp_smem_bytes(int C, int SPLITS, bool f32in, int out) {
+    return 1024 + (size_t)2 * C * kTcABytes + (f32in ? 0 : (size_t)C * SPLITS * kTcBBytes + kHpTBytes) +
+           (out == kOutGates ? (size_t)2 * kFuWChunkBytes + 3 * kHpPieceBytes : 0) + 8 * 8;
 }
-// Segment plan of the epilogue step (see the iteration body): which segment runs phase 1 of activation pair p (phases 2
-// and 3 follow one and two segments later), the two conv2 chain steps of each of the first five B segments, and the
-// five pieces of stage B's tail.  MUFU per segment -- plan 0: 2 3 3 3 3 5 5 3 1 0, plan 1: 2 3 3 3 3 3 2 2 3 3 1 0.
-#ifndef B2CNN_SEGPLAN
-#define B2CNN_SEGPLAN 1
-#endif
-struct SegPlan {
-    // MUFU per segment (plan 1): 2 2 4 3 3 3 3 3 3 1 1 0 0
-    static constexpr int kSegs = 13;
-    static constexpr int kDist = 2;                                                  // segments between a MUFU and its consumer's segment
-    __host__ __device__ static constexpr int a1(int p) { return p + 1; }             // phase 1 of activation pair p (phases 2, 3: + kDist, + 2 kDist)
-    __host__ __device__ static constexpr int conv2(int i) { return i; }              // chain step i (q2 = i / 5, tap k = i % 5) of the 10
-    __host__ __device__ static constexpr int tail(int i) { return i < 3 ? 2 * i : i + 2; }   // pool2+exp | rcp | hi piece | mid piece | lo piece: 0 2 4 5 6
-};
-
-// barrier indices (uint64_t slots)
-struct FuBars {
-    // per window tile t (stride kPerTile)
-    static constexpr int kFull = 0, kEmpty = 2, kTFull = 4, kTEmpty = 8, kPFull = 12, kPEmpty = 14, kGFull = 16, kGEmpty = 17, kPerTile = 18;
-    static constexpr int kWFull = 2 * kPerTile, kWEmpty = kWFull + 2, kTotal = kWEmpty + 2;
-};
 
 // ARCH 0: MyCNN5 geometry (K1=10, pool(3,2)) -- bin/models.py.
-// ARCH 1: MyCNN2/3/4 geometry (K1=5, pool(2,2)) -- bin/explore_torch copy.ipynb:189-277: every tap
-//         fits the 16-sample slice (no tap-9 patch), pooling pairs stay inside a block (no carry),
-//         and a step emits features 2j-2, 2j-1 instead of 2j-3, 2j-2.
-template <int C, int SPLITS, int ARCH>
-__global__ void __launch_bounds__(kFuThreads, 1)
-tc_fused_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ TcFusedParams p) {
-    extern __shared__ __align__(1024) uint8_t smem[];
-#ifdef B2CNN_TIMING
-    const long long t_entry = clock64();
-    unsigned long long gt_entry;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(gt_entry));
-#endif
-    // [2 tiles][2 stages][C][16 KB] | bands | W ring [2][6 KB] | barriers | tmem slot
-    uint8_t *sA = smem;
-    uint8_t *sBm = sA + 2 * 2 * C * kTcABytes;
-    uint8_t *sW = sBm + C * SPLITS * kTcBBytes;
-    uint64_t *bars = reinterpret_cast<uint64_t *>(sW + 2 * kFuWChunkBytes);
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(bars + FuBars::kTotal);
-    const uint32_t bar0 = smem_u32(bars);
-    auto BAR = [&](int idx) -> uint32_t { return bar0 + 8u * (uint32_t)idx; };
-
-    const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);   // warp-uniform for the compiler
-    const int lane = threadIdx.x & 31;
+// ARCH 1: MyCNN2/3/4 geometry (K1=5, pool(2,2)) -- bin/explore_torch copy.ipynb:189-277: every tap fits the
+//         16-sample slice (no tap-9 patch), pooling pairs stay inside a block (no carry), and a step emits
+//         features 2j-2, 2j-1 instead of 2j-3, 2j-2.
+template <int C, int SPLITS, int ARCH, bool F32IN, int OUT>
+__global__ void __launch_bounds__(kHpThreads, 1)
+tc_stream_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ TcFusedParams p) {
+    constexpr int K1 = ARCH == 0 ? 10 : 5;
+    constexpr int kBlocks = F32IN ? kSfBlocks : kTcBlocks;
+    constexpr int kAdv = F32IN ? kSfAdv : kTcAdv;
     constexpr int FOFF = ARCH == 0 ? 3 : 2;           // step j emits features 2j-FOFF, 2j-FOFF+1
-    // Persistent CTA: one per SM, items k, k + gridDim.x, ... (static: every role walks the same list, nothing to
-    // exchange).  All pipelines run THROUGH the item boundaries -- the producer prefetches the next item's first tiles and
-    // the MMA warps start its conv1 blocks while the epilogue still drains the gates of the previous one -- so the per-CTA
-    // launch, TMEM allocation, band-matrix copy and pipeline fill are paid once per SM instead of once per item (measured
-    // with B2CNN_TIMING on the one-item-per-CTA kernel: 4.4 us from CTA entry to the first accumulators, and 16 % of the
-    // kernel's duration covered by no CTA at all: block-scheduler gaps between the waves).  Barrier phases carry over: every
-    // role counts tiles / chunks / ring uses globally.
-    struct Item { int r, b_cta, J, ntiles, nchunks, T0; };
-    auto item_geom = [&](int item) -> Item {
-        Item g;
-        g.r = item % p.n_ranges;
-        g.b_cta = (item / p.n_ranges) * 2 * kTcM;
-        const int p0 = g.r * p.feats_per_cta;
-        const int nfeat = min(p.feats_per_cta, p.L - p0);
-        const int nsteps_needed = (nfeat + FOFF - 1) / 2 + 1;
-        g.ntiles = (nsteps_needed + kTcBlocks - 1) / kTcBlocks;
-        g.J = g.ntiles * kTcBlocks;                   // steps actually run
-        g.nchunks = (g.J + 7) / 8;
-        g.T0 = p0 * 4;
-        return g;
-    };
+    extern __shared__ uint8_t smem_raw[];
+    // [2 stages][C][16 KB] | bands | transpose | W ring [2][6 KB] | A pieces [3][4 KB] | barriers
+    uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+    uint8_t *sA = smem;
+    uint8_t *sBm = sA + 2 * C * kTcABytes;
+    float *sT = reinterpret_cast<float *>(sBm + (F32IN ? 0 : C * SPLITS * kTcBBytes));
+    uint8_t *sW = reinterpret_cast<uint8_t *>(sT) + (F32IN ? 0 : kHpTBytes);
+    uint8_t *sPc = sW + (OUT == kOutGates ? 2 * kFuWChunkBytes : 0);
+    uint64_t *bars = reinterpret_cast<uint64_t *>(sPc + (OUT == kOutGates ? 3 * kHpPieceBytes : 0));
+    const uint32_t bar_full = smem_u32(bars + 0), bar_empty = smem_u32(bars + 2);
+    const uint32_t bar_wfull = smem_u32(bars + 4), bar_wempty = smem_u32(bars + 6);
+    auto sA_of = [&](int s, int c) -> uint8_t * { return sA + (size_t)(s * C + c) * kTcABytes; };
 
-    if ((smem_u32(smem) & 1023u) != 0) __trap();      // SWIZZLE_128B tiles need 1 KB alignment
-    for (int i = threadIdx.x; i < C * SPLITS * kTcBBytes / 16; i += kFuThreads)
-        reinterpret_cast<uint4 *>(sBm)[i] = reinterpret_cast<const uint4 *>(p.bmats)[i];
+    const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);
+    const int lane = threadIdx.x & 31;
+    const int b0 = blockIdx.x * kTcM;
+    const int p0 = blockIdx.y * p.feats_per_cta;
+    const int nfeat = min(p.feats_per_cta, p.L - p0);
+    const int nsteps = OUT == kOutGates ? (nfeat + FOFF - 1) / 2 + 1 : (nfeat + 4) / 2;
+    const int ntiles = (nsteps + kBlocks - 1) / kBlocks;
+    const int J = ntiles * kBlocks;                   // steps actually run
+    const int nchunks = (J + 7) / 8;
+    const int T0 = p0 * 4;                            // first conv1 position == first sample
+
+    if (!F32IN)
+        for (int i = threadIdx.x; i < C * SPLITS * kTcBBytes / 16; i += kHpThreads)
+            reinterpret_cast<uint4 *>(sBm)[i] = reinterpret_cast<const uint4 *>(p.bmats)[i];
     if (threadIdx.x == 0) {
-        for (int t = 0; t < 2; ++t) {
-            const int o = t * FuBars::kPerTile;
-            for (int i = 0; i < 2; ++i) { mbar_init(BAR(o + FuBars::kFull + i), 1); mbar_init(BAR(o + FuBars::kEmpty + i), 4); }
-            for (int i = 0; i < 4; ++i) { mbar_init(BAR(o + FuBars::kTFull + i), 1); mbar_init(BAR(o + FuBars::kTEmpty + i), 4); }
-            for (int i = 0; i < 2; ++i) { mbar_init(BAR(o + FuBars::kPFull + i), 4); mbar_init(BAR(o + FuBars::kPEmpty + i), 1); }
-            mbar_init(BAR(o + FuBars::kGFull), 1);
-            mbar_init(BAR(o + FuBars::kGEmpty), 4);
+        for (int i = 0; i < 2; ++i) {
+            mbar_init(bar_full + 8 * i, 1);
+            mbar_init(bar_empty + 8 * i, 4);
+            mbar_init(bar_wfull + 8 * i, 1);
+            mbar_init(bar_wempty + 8 * i, 4);
         }
-        for (int i = 0; i < 2; ++i) { mbar_init(BAR(FuBars::kWFull + i), 1); mbar_init(BAR(FuBars::kWEmpty + i), 1); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 3) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(512) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    tc_fence_before();
+    fence_proxy_async();                              // band matrices visible to the tensor core
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    auto sA_of = [&](int t, int s, int c) -> uint8_t * { return sA + ((size_t)((t * 2 + s) * C + c)) * kTcABytes; };
 
-    if (warp == 0) {
-        // ===================== producer =====================
+    if (warp == 4) {
+        // ===================== TMA producer: window tiles =====================
         if (lane == 0) {
-            FU_TDECL();
-#ifdef B2CNN_TIMING
-            const long long tp0 = clock64();
-#endif
-            int gi = 0;                                     // tiles requested so far (all items): stage = gi & 1
-            for (int item = blockIdx.x; item < p.n_items; item += gridDim.x) {
-                const Item g = item_geom(item);
-                for (int i = 0; i < g.ntiles; ++i, ++gi) {
-                    const int s = gi & 1, ph = (gi >> 1) & 1;
-                    for (int t = 0; t < 2; ++t) {
-                        const int o = t * FuBars::kPerTile;
-                        { FU_T0(); mbar_wait_parked(BAR(o + FuBars::kEmpty + s), ph ^ 1); FU_TACC(9, true); }
-                        mbar_expect_tx(BAR(o + FuBars::kFull + s), C * kTcABytes);
+            for (int i = 0; i < ntiles; ++i) {
+                const int s = i & 1, ph = (i >> 1) & 1;
+                mbar_wait(bar_empty + 8 * s, ph ^ 1);
+                mbar_expect_tx(bar_full + 8 * s, C * kTcABytes);
 #pragma unroll
-                        for (int c = 0; c < C; ++c)
-                            tma_load_3d(smem_u32(sA_of(t, s, c)), &tmap, g.T0 + kTcAdv * i, c, g.b_cta + t * kTcM, BAR(o + FuBars::kFull + s));
-                    }
-                }
+                for (int c = 0; c < C; ++c) tma_load_3d(smem_u32(sA_of(s, c)), &tmap, T0 + kAdv * i, c, b0, bar_full + 8 * s);
             }
-#ifdef B2CNN_TIMING
-            atomicAdd(&g_fu_timing[8], (unsigned long long)(clock64() - tp0));
-#endif
-            FU_TFLUSH(8, true);
         }
-    } else if (warp == 1 || warp == 2) {
-        // ===================== conv1 MMA issuer of window tile t =====================
-        // The whole warp runs the loop (warp-uniform control flow and descriptor arithmetic); one elected lane issues the
-        // tcgen05 instructions.  Nothing but conv1 blocks lives here: what this warp executes between "ring slot free" and
-        // "MMAs queued" is on the critical path of the accumulator ring (A/B with -DB2CNN_MMA_PAD: 32 dependent dummy
-        // instructions per block cost the kernel 16 %), so the projection MMAs -- which used to sit in this loop and block
-        // it while the epilogue's pieces were not ready -- are issued by warp 3, and the descriptors of a block are ready
-        // before its slot is waited for.
-        const int t = warp - 1;
-        const int o = t * FuBars::kPerTile;
-        FU_TDECL();
-        const uint64_t a_base = desc_sw128_kmajor(smem_u32(sA_of(t, 0, 0)));
-        const uint64_t b_base = desc_none_kmajor(smem_u32(sBm), 128, 256);
-        const uint32_t tcol = tmem_base + t * 256;
-        int gi = 0;                                         // tiles done so far (all items): stage = gi & 1
-        uint32_t rpar = 0;                                  // bit s: parity of the number of uses of accumulator-ring slot s
-        uint64_t bdesc[C * SPLITS];                         // loop-invariant band-matrix descriptors
-#pragma unroll
-        for (int i = 0; i < C * SPLITS; ++i) bdesc[i] = b_base + (uint64_t)(i * (kTcBBytes >> 4));
-#ifdef B2CNN_TIMING
-        const long long tm0 = clock64();
-#endif
-        for (int item = blockIdx.x; item < p.n_items; item += gridDim.x) {
-        const Item g = item_geom(item);
-        int j = 0;
-#pragma unroll 1
-        for (int i = 0; i < g.ntiles; ++i, ++gi) {
-            const int s = gi & 1;
-            {
-                FU_T0();
-#if B2CNN_MMA_SPIN
-                mbar_wait(BAR(o + FuBars::kFull + s), (gi >> 1) & 1);
-#else
-                mbar_wait_parked(BAR(o + FuBars::kFull + s), (gi >> 1) & 1);
-#endif
-                FU_TACC(5, lane == 0);
+    } else if (warp == 5) {
+        // ===================== producer of the packed W_ih chunks =====================
+        if (OUT == kOutGates && lane == 0) {
+            const uint8_t *wsrc = p.wpack + (size_t)blockIdx.y * p.chunks_per_cta * kFuWChunkBytes;
+            for (int m = 0; m < nchunks; ++m) {
+                const int u = m & 1;
+                mbar_wait(bar_wempty + 8 * u, ((m >> 1) & 1) ^ 1);
+                mbar_expect_tx(bar_wfull + 8 * u, kFuWChunkBytes);
+                bulk_load_1d(smem_u32(sW + u * kFuWChunkBytes), wsrc + (size_t)m * kFuWChunkBytes, kFuWChunkBytes, bar_wfull + 8 * u);
             }
-            const uint64_t a_stage = a_base + (uint64_t)((uint32_t)(s * C) * (kTcABytes >> 4));
+        }
+    } else {
+        // ===================== consumer warpgroup: thread == window =====================
+        const int row = threadIdx.x;
+        const int b = b0 + row;
+        const bool row_ok = b < p.B;
+        const uint32_t swz = (uint32_t)(row & 7);     // SWIZZLE_128B: 16-byte chunk ^= row % 8
+        float acc[2][16];                             // conv1 accumulators of one block (two m64 row halves)
+        float gacc[2][32];                            // gate pre-activations (two m64 row halves)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+#pragma unroll
+            for (int i = 0; i < 16; ++i) acc[h][i] = 0.f;
+#pragma unroll
+            for (int i = 0; i < 32; ++i) gacc[h][i] = 0.f;
+        }
+        float pm6[kCMid], pm7[kCMid], ah[4][kCMid], c2c = 0.f, nan_probe = 0.f;
+#pragma unroll
+        for (int o = 0; o < kCMid; ++o) {
+            pm6[o] = 0.f; pm7[o] = 0.f;
+#pragma unroll
+            for (int i = 0; i < 4; ++i) ah[i][o] = 0.f;
+        }
+        float *fout = p.feats + (int64_t)b * p.sB + (int64_t)p0 * p.sP;
+
+        auto issue_conv1 = [&](int s, int n) {
+            const uint64_t bdesc0 = gdesc_none_kmajor(smem_u32(sBm), 128, 256);
+            wgmma_fence();
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+#pragma unroll
+                for (int c = 0; c < C; ++c) {
+                    const uint64_t adesc = gdesc_sw128_kmajor(smem_u32(sA_of(s, c)) + h * 64 * 128 + 16 * n);
+#pragma unroll
+                    for (int sp = 0; sp < SPLITS; ++sp)
+                        wgmma_m64n32(acc[h], adesc, bdesc0 + (uint64_t)((c * SPLITS + sp) * (kTcBBytes >> 4)), (c | sp) != 0);
+                }
+            wgmma_commit();
+        };
+        if (!F32IN) {
+            mbar_wait(bar_full, 0);
+            issue_conv1(0, 0);
+        }
+
 #pragma unroll 1
-            for (int n = 0; n < kTcBlocks; ++n, ++j) {
-                const int slot = j & 3;                     // ring slots restart with every item, their phases do not
-                uint64_t a_c[C];
-#pragma unroll
-                for (int c = 0; c < C; ++c) a_c[c] = a_stage + (uint64_t)(c * (kTcABytes >> 4) + n);
-                const uint32_t d = tcol + slot * 32;
-                {
-                    FU_T0();
-#if B2CNN_MMA_SPIN
-                    mbar_wait(BAR(o + FuBars::kTEmpty + slot), ((rpar >> slot) & 1) ^ 1);
-#else
-                    mbar_wait_parked(BAR(o + FuBars::kTEmpty + slot), ((rpar >> slot) & 1) ^ 1);
-#endif
-                    FU_TACC(6, lane == 0);
-                }
-                rpar ^= 1u << slot;
-#ifdef B2CNN_MMA_PAD                                  // experiment: what one extra dispatch slot per block in the MMA-issue warps costs
-                {
-                    uint32_t pad = (uint32_t)j;
-#pragma unroll
-                    for (int z = 0; z < B2CNN_MMA_PAD; ++z) asm volatile("lop3.b32 %0, %0, %0, %0, 0xc0;" : "+r"(pad));
-                    if (pad == 0xdeadbeefu) rpar ^= 16u;
-                }
-#endif
-                tc_fence_after();
-                if (elect_one()) {
-#if B2CNN_ABLATE != 3
-                    // the piece-MMAs of a (block, channel) share their A slice through the collector buffer
-                    // (fill / use / lastuse) instead of re-reading 4 KB of shared memory per piece
+        for (int j = 0; j < J; ++j) {
+            const int i = j / kBlocks, n = j - i * kBlocks, s = i & 1;
+            float D[32];                              // conv1 pre-activations of block j: D[shift * 4 + out channel]
+            if constexpr (!F32IN) {
+                if constexpr (ARCH == 0) {
+                    // tap 9 of the previous block's position 7: sample 8n + 8 of this tile
 #pragma unroll
                     for (int c = 0; c < C; ++c) {
-                        umma_ss_coll64<kFuCollector ? 1 : 0>(d, a_c[c], bdesc[c * SPLITS], kIdesc, c != 0);
-                        if constexpr (SPLITS == 3) umma_ss_coll64<kFuCollector ? 2 : 0>(d, a_c[c], bdesc[c * SPLITS + 1], kIdesc, 1);
-                        umma_ss_coll64<kFuCollector ? 3 : 0>(d, a_c[c], bdesc[c * SPLITS + SPLITS - 1], kIdesc, 1);
+                        const uint16_t raw = *reinterpret_cast<const uint16_t *>(sA_of(s, c) + row * 128 + (((uint32_t)(n + 1) ^ swz) << 4));
+                        const float xv = __uint_as_float((uint32_t)raw << 16);
+#pragma unroll
+                        for (int o = 0; o < kCMid; ++o) pm7[o] = fmaf(p.w9[c][o], xv, pm7[o]);
                     }
-#endif
-                    umma_commit(BAR(o + FuBars::kTFull + slot));
                 }
-                __syncwarp();
-            }
-        }
-        }
-#ifdef B2CNN_TIMING
-        if (lane == 0) atomicAdd(&g_fu_timing[4], (unsigned long long)(clock64() - tm0));
-#endif
-        FU_TFLUSH(4, lane == 0);
-    } else if (warp == 3) {
-        // ===================== W_ih chunk producer + projection MMA issuer (and TMEM allocator) =====================
-        // Per 16-position chunk: request the NEXT chunk of packed W_ih (its stage is free once the projection two chunks back
-        // has completed), then, for each window tile, wait for the epilogue's three bf16 pieces and issue the six
-        // projection MMAs (A in TMEM).  The whole warp runs the loop, one elected lane issues.
-        FU_TDECL();
-        const uint64_t w_base = desc_none_kmajor(smem_u32(sW), 128, 256);
-        const uint32_t w_lo0 = (uint32_t)w_base, w_hi = (uint32_t)(w_base >> 32);
-        int gm = 0, gl = 0, it = 0;                         // chunks projected / chunks requested (all items); items done
-        auto request_chunk = [&](const uint8_t *src) {      // chunk number gl -> stage gl & 1
-            const int u = gl & 1;
-            mbar_wait_parked(BAR(FuBars::kWEmpty + u), ((gl >> 1) & 1) ^ 1);
-            if (lane == 0) {
-                mbar_expect_tx(BAR(FuBars::kWFull + u), kFuWChunkBytes);
-                bulk_load_1d(smem_u32(sW + u * kFuWChunkBytes), src, kFuWChunkBytes, BAR(FuBars::kWFull + u));
-            }
-            __syncwarp();
-            ++gl;
-        };
-        for (int item = blockIdx.x; item < p.n_items; item += gridDim.x, ++it) {
-            const Item g = item_geom(item);
-            const uint8_t *wsrc = p.wpack + (size_t)g.r * p.chunks_per_cta * kFuWChunkBytes;
-            if (gl == gm) request_chunk(wsrc);              // very first chunk of the CTA (later items: requested one chunk ahead)
-            for (int m = 0; m < g.nchunks; ++m, ++gm) {
-                // one chunk ahead: the next chunk of this item, or the first chunk of the next item
-                if (m + 1 < g.nchunks) {
-                    request_chunk(wsrc + (size_t)(m + 1) * kFuWChunkBytes);
-                } else if (item + (int)gridDim.x < p.n_items) {
-                    const Item gn = item_geom(item + (int)gridDim.x);
-                    request_chunk(p.wpack + (size_t)gn.r * p.chunks_per_cta * kFuWChunkBytes);
-                }
-                const int u = gm & 1, ph = (gm >> 1) & 1;
-                { FU_T0(); mbar_wait_parked(BAR(FuBars::kWFull + u), ph); FU_TACC(7, lane == 0); }
+                wgmma_wait<0>();
 #pragma unroll
-                for (int t = 0; t < 2; ++t) {
-                    const int o = t * FuBars::kPerTile;
-                    { FU_T0();
-                    mbar_wait_parked(BAR(o + FuBars::kPFull + u), ph);
-                    if (m == 0) mbar_wait_parked(BAR(o + FuBars::kGEmpty), (it & 1) ^ 1);   // the previous item's gates left TMEM
-                    FU_TACC(7, lane == 0); }
-                    tc_fence_after();
-                    if (elect_one()) {
-                        const uint32_t tcol = tmem_base + t * 256;
-                        const uint32_t d = tcol + 192;
-                        const uint32_t a0 = tcol + 128 + u * 24;
-                        const uint32_t w0 = w_lo0 + u * (kFuWChunkBytes >> 4);
-                        // piece pairs (feature piece, weight piece) with fp + wp <= 2: hh hm mh hl lh mm
-                        umma_ts(d, a0 + 0, w0 + 0 * 128, w_hi, kIdescProj, m != 0);
-                        umma_ts(d, a0 + 0, w0 + 1 * 128, w_hi, kIdescProj, 1);
-                        umma_ts(d, a0 + 8, w0 + 0 * 128, w_hi, kIdescProj, 1);
-                        umma_ts(d, a0 + 0, w0 + 2 * 128, w_hi, kIdescProj, 1);
-                        umma_ts(d, a0 + 16, w0 + 0 * 128, w_hi, kIdescProj, 1);
-                        umma_ts(d, a0 + 8, w0 + 1 * 128, w_hi, kIdescProj, 1);
-                        umma_commit(BAR(o + FuBars::kPEmpty + u));
-                        if (t == 1) umma_commit(BAR(FuBars::kWEmpty + u));          // both tiles' MMAs read this W stage
-                        if (m == g.nchunks - 1) umma_commit(BAR(o + FuBars::kGFull));
+                for (int h = 0; h < 2; ++h)
+#pragma unroll
+                    for (int e = 0; e < 16; e += 2) {
+                        const int r = 64 * h + 16 * warp + (lane >> 2) + 8 * ((e >> 1) & 1);
+                        const int col = 8 * (e >> 2) + 2 * (lane & 3);
+                        *reinterpret_cast<float2 *>(sT + r * kHpTStride + col) = make_float2(acc[h][e], acc[h][e + 1]);
                     }
-                    __syncwarp();
+                wg_bar();
+                if (n == kBlocks - 1 && lane == 0) mbar_arrive(bar_empty + 8 * s);   // stage fully consumed
+                if (j + 1 < J) {                      // the next block's MMAs overlap this block's epilogue
+                    const int i2 = (j + 1) / kBlocks, n2 = j + 1 - i2 * kBlocks;
+                    if (n2 == 0) mbar_wait(bar_full + 8 * (i2 & 1), (i2 >> 1) & 1);
+                    issue_conv1(i2 & 1, n2);
                 }
-            }
-        }
-        FU_TFLUSH(4, lane == 0);
-    } else {
-        // ===================== epilogue: thread == window =====================
-        // Software-pipelined over three steps.  Iteration jj runs
-        //   stage A  of block jj    TMEM -> pool1 -> tanh, kept as r = (1 - tanh)/2           -> a1 registers
-        //   stage Bc of step  jj-1  conv2 over a1(jj-2), a1(jj-1)                             -> 4 conv2 outputs
-        //   stage Bt of step  jj-2  pool2 -> tanh -> three bf16 pieces -> tcgen05.st (A operand of the projection)
-        // The stages touch disjoint registers; every dependent chain of one stage (MUFU -> FADD2 -> FMUL -> MUFU ...,
-        // the 10-deep conv2 FMA chains, the piece splitting) has the other two stages' work to hide behind.  All barrier
-        // traffic sits at the top and bottom of the iteration.
-        const int t = (warp - 4) >> 2;
-        const int o_bar = t * FuBars::kPerTile;
-        const int q = warp & 3;
-        const int row = q * 32 + lane;
-        const uint32_t tlane = tmem_base + ((uint32_t)(q * 32) << 16) + t * 256;
-        const uint32_t swz = (uint32_t)(row & 7);
-        FU_TDECL();
-        int J = 0;                                          // steps of the current item
-        int gmb = 0, it = 0;                                // chunks / items finished so far (A buffer = global chunk & 1)
-        uint32_t tqm = 0, tq[4] = {0, 0, 0, 0};             // parity of the uses of accumulator-ring slot s in the items before (mask, and per slot)
-        // a1 history: abuf[jj & 1] holds the 4 activations x 4 channels produced by stage A of block jj
-        // all per-channel state is held as float2 over channel pairs (0,1) and (2,3)
-        float2 pm6[2], pm7[2], abuf[2][4][2];
-        float c2s[2][4];                                    // conv2 outputs: Bc of iteration jj writes c2s[jj & 1], Bt of jj + 1 reads them
-        float c2c = 0.f;
-        // accumulator registers are double-buffered by step parity (block jj lives in Dbuf[jj & 1]; the
-        // next block's tcgen05.ld is issued into the other half) -- no register-to-register copies
-        uint32_t Dbuf[2][32];
-        int n = 0, ti = 0;                                  // block-in-tile of block jj; tiles consumed so far (all items)
-        float2 w2r[2][5];                                   // conv2 weights stay in registers for the whole stream
-#pragma unroll
-        for (int q2 = 0; q2 < 2; ++q2)
-#pragma unroll
-            for (int k = 0; k < 5; ++k) w2r[q2][k] = p.w2p[q2][k];
-
-        // KK >= 0: (jj - 1) & 7 is a compile-time constant (the main loop is unrolled over the eight steps whose features
-        // fill one 16-position projection chunk): accumulator-ring slots, barrier addresses and parities, the A-operand
-        // column and the chunk-boundary branches all fold, which removes about a third of the loop's instructions (they
-        // were uniform-datapath address / parity arithmetic and branches, not math).  KK == -1: the same iteration with
-        // everything computed at run time (prologue, the tail after the last whole chunk).
-        // m = chunk of step jj - 2 (the one whose features this iteration stores).
-        auto iteration = [&](int jj, int m, auto doA_, auto doBc_, auto doBt_, auto par_, auto kk_) {
-            constexpr bool doA = decltype(doA_)::value, doBc = decltype(doBc_)::value, doBt = decltype(doBt_)::value;
-            constexpr int PAR = decltype(par_)::value;      // == jj & 1 (compile-time register naming)
-            constexpr int KK = decltype(kk_)::value;        // == (jj - 1) & 7, or -1
-            const int s = ti & 1;
-            const int jt = jj - 2, kk = KK >= 0 ? ((KK + 7) & 7) : (jt & 7), u = m & 1;   // stored step, its column, its A buffer
-            const int slot0 = KK >= 0 ? ((KK + 1) & 3) : (jj & 3);                    // ring slot of block jj
-            const int slot1 = KK >= 0 ? ((KK + 2) & 3) : ((jj + 1) & 3);              // ... and of block jj + 1
-            const int par1 = KK >= 0 ? (((KK + 2) & 7) >> 2) : (((jj + 1) >> 2) & 1);
-            // the next block's accumulators -> the other half of Dbuf (dead since the previous iteration copied its carries out).
-            // kLdtmSeg < 0: at the top of the iteration; else after that segment of the math: the later it is asked for,
-            // the more slack the MMA warp has to refill the ring, as long as the load still lands before the next iteration
-            const uint32_t tqs = KK >= 0 ? tq[KK >= 0 ? ((KK + 2) & 3) : 0] : ((tqm >> slot1) & 1u);
-            auto prefetch_next = [&]() {
-                if (KK >= 0 || jj + 1 < J) {
-                    FU_T0();
-#if B2CNN_EPI_SPIN
-                    mbar_wait(BAR(o_bar + FuBars::kTFull + slot1), par1 ^ tqs);
-#else
-                    mbar_wait_parked(BAR(o_bar + FuBars::kTFull + slot1), par1 ^ tqs);
-#endif
-                    FU_TACC(1, lane == 0);
-                    tc_fence_after();
-                    tmem_ld32_issue(tlane + slot1 * 32, Dbuf[PAR ^ 1]);
-                }
-            };
-            // ---------------- top: barriers ----------------
-            if constexpr (doA) {
-                tmem_ld32_wait(Dbuf[PAR]);
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(BAR(o_bar + FuBars::kTEmpty + slot0));
-                if constexpr (kLdtmSeg < 0) prefetch_next();
-                { FU_T0(); if (n == 0) mbar_wait_parked(BAR(o_bar + FuBars::kFull + s), (ti >> 1) & 1); FU_TACC(2, lane == 0); }   // TMA bytes visible for the tap-9 reads
-            }
-            if constexpr (doBt) {
-                if (kk == 0) {                              // first store of chunk m into A buffer u
-                    FU_T0();
-                    mbar_wait_parked(BAR(o_bar + FuBars::kPEmpty + u), ((m >> 1) & 1) ^ 1);
-                    FU_TACC(3, lane == 0);
-                    tc_fence_after();
-                }
-            }
-            // ---------------- middle: straight-line math ----------------
-            float2 an[4][2];
-            const uint32_t acol = tlane + 128 + u * 24 + kk;
-#if B2CNN_ABLATE == 1
-            if constexpr (doA && kLdtmSeg >= 0) prefetch_next();
-            if constexpr (doA) {
-#pragma unroll
-                for (int r = 0; r < 4; ++r) {
-                    an[r][0] = make_float2(__uint_as_float(Dbuf[PAR][r] ^ Dbuf[PAR][8 + r] ^ Dbuf[PAR][16 + r] ^ Dbuf[PAR][24 + r]), 0.f);
-                    an[r][1] = make_float2(__uint_as_float(Dbuf[PAR][4 + r] ^ Dbuf[PAR][12 + r] ^ Dbuf[PAR][20 + r] ^ Dbuf[PAR][28 + r]), 0.f);
-                }
-            }
-            if constexpr (doBt) {
-                const uint32_t h = __float_as_uint(abuf[PAR][0][0].x) ^ __float_as_uint(abuf[PAR ^ 1][1][1].x);
-                tmem_st1(acol, h & 0x3f803f80u);
-                tmem_st1(acol + 8, 0u);
-                tmem_st1(acol + 16, 0u);
-            }
-#else
-            {
-                // The iteration's arithmetic in SegPlan::kSegs segments with a scheduling fence between them.  Left to
-                // itself ptxas sorts the basic block by critical path: the 40 conv2 FFMA2 first, the 28 MUFU (whose results
-                // nothing in the block consumes) in one cluster at the end -- two in-order warps per scheduler then queue
-                // on the 8-cycle MUFU pipe in the same phase while the FMA pipe idles (ncu source view: 40 % of the loop's
-                // samples on that cluster).  Within a segment the MUFUs still sink to the end and their consumers rise to
-                // the top of whatever segment holds them, so consumers sit TWO segments after their producers: one whole
-                // segment of other work covers the MUFU latency.
-                auto Dv = [&](int idx) -> float { return __uint_as_float(Dbuf[PAR][idx]); };
-                float2 ex[8], dd[8], acc[4], te = make_float2(0.f, 0.f), tf = make_float2(0.f, 0.f), tr1 = make_float2(0.f, 0.f);
-                float rp[8], trx = 0.f, try_ = 0.f;
-                uint32_t xraw[C];
-                auto segment = [&](auto s_) {
-                    constexpr int S = decltype(s_)::value;
-                    if constexpr (doA) {
-                        if constexpr (ARCH == 0) {
-                            // tap 9 of the previous block's position 7 (it did not fit that block's 16-sample slice)
-                            if constexpr (S == 0) {
-                                const uint8_t *tile = sA_of(t, s, 0) + row * 128;
-#pragma unroll
-                                for (int c = 0; c < C; ++c)
-                                    xraw[c] = *reinterpret_cast<const uint16_t *>(tile + c * kTcABytes + ((uint32_t)((n + 1) ^ swz) << 4));
-                            }
-                            if constexpr (S == 2) {
-#pragma unroll
-                                for (int c = 0; c < C; ++c) {
-                                    const float xv = __uint_as_float(xraw[c] << 16);
-#pragma unroll
-                                    for (int q2 = 0; q2 < 2; ++q2) pm7[q2] = fma2(p.w9p[c][q2], make_float2(xv, xv), pm7[q2]);
-                                }
-                            }
-                        }
-                        static_for<0, 8>([&](auto p_) {
-                            // pair P: pooled position r, out-channels 2*q2, 2*q2+1 (MyCNN5: position 0 needs the carried
-                            // pre-activations pm6 / pm7 and the tap-9 patch, so it goes last)
-                            constexpr int P = decltype(p_)::value;
-                            constexpr int r = ARCH == 0 ? (((P >> 1) + 1) & 3) : (P >> 1), q2 = P & 1, o0 = 2 * q2, o1 = 2 * q2 + 1;
-                            if constexpr (SegPlan::a1(P) == S) {
-                                float2 m2;
-                                if constexpr (ARCH == 0) {
-                                    if constexpr (r == 0) {
-                                        m2 = make_float2(max3_nan(pm6[q2].x, pm7[q2].x, Dv(o0)), max3_nan(pm6[q2].y, pm7[q2].y, Dv(o1)));
-                                    } else {
-                                        constexpr int c0 = 2 * r - 2;
-                                        m2 = make_float2(max3_nan(Dv(c0 * 4 + o0), Dv((c0 + 1) * 4 + o0), Dv((c0 + 2) * 4 + o0)),
-                                                         max3_nan(Dv(c0 * 4 + o1), Dv((c0 + 1) * 4 + o1), Dv((c0 + 2) * 4 + o1)));
-                                    }
-                                } else {
-                                    // pool(2,2): pooled position 4j+i = max(pre[8j+2i], pre[8j+2i+1])
-                                    m2 = make_float2(max_nan(Dv((2 * r) * 4 + o0), Dv((2 * r + 1) * 4 + o0)),
-                                                     max_nan(Dv((2 * r) * 4 + o1), Dv((2 * r + 1) * 4 + o1)));
-                                }
-                                ex[P] = sig_ph1(m2, p.b1sp[q2]);
-                            }
-                            if constexpr (SegPlan::a1(P) + SegPlan::kDist == S) sig_ph2(ex[P], dd[P], rp[P]);
-                            if constexpr (SegPlan::a1(P) + 2 * SegPlan::kDist == S) an[r][q2] = sig_ph3(dd[P], rp[P]);
-                        });
-                        if constexpr (ARCH == 0 && S == SegPlan::a1(7) + 1) {      // after the last reader of pm6 / pm7
-#pragma unroll
-                            for (int q2 = 0; q2 < 2; ++q2) {
-                                pm6[q2] = make_float2(Dv(6 * 4 + 2 * q2), Dv(6 * 4 + 2 * q2 + 1));
-                                pm7[q2] = make_float2(Dv(7 * 4 + 2 * q2), Dv(7 * 4 + 2 * q2 + 1));
-                            }
-                        }
-                    }
-                    if constexpr (doBc) {
-                        // conv2 on r = (1 - tanh)/2 (weights pre-multiplied by -2, bias absorbs sum(w)): 40 FFMA2, one
-                        // accumulator per output position over both channel pairs (c2 = acc.x + acc.y)
-                        static_for<0, 10>([&](auto i_) {
-                            constexpr int I = decltype(i_)::value, q2 = I / 5, k = I % 5;
-                            if constexpr (SegPlan::conv2(I) == S) {
-                                // a1(step jj-2) = abuf[PAR], a1(step jj-1) = abuf[PAR ^ 1]
-                                const float2 A8[8] = {abuf[PAR][0][q2], abuf[PAR][1][q2], abuf[PAR][2][q2], abuf[PAR][3][q2],
-                                                      abuf[PAR ^ 1][0][q2], abuf[PAR ^ 1][1][q2], abuf[PAR ^ 1][2][q2], abuf[PAR ^ 1][3][q2]};
-#pragma unroll
-                                for (int r = 0; r < 4; ++r) acc[r] = I == 0 ? mul2(w2r[0][0], A8[r]) : fma2(w2r[q2][k], A8[r + k], acc[r]);
-                            }
-                        });
-                        if constexpr (S == SegPlan::conv2(9) + 1) {
-#pragma unroll
-                            for (int r = 0; r < 4; ++r) c2s[PAR][r] = acc[r].x + acc[r].y;
-                        }
-                    }
-                    if constexpr (doBt) {
-                        const float *c2 = c2s[PAR ^ 1];
-                        if constexpr (S == SegPlan::tail(0)) {      // pool2 + the exponent of tanh
-                            float2 m2;
-                            if constexpr (ARCH == 0) {
-                                m2 = make_float2(max3_nan(c2c, c2[0], c2[1]), max3_nan(c2[1], c2[2], c2[3]));
-                                c2c = c2[3];
-                            } else {
-                                m2 = make_float2(max_nan(c2[0], c2[1]), max_nan(c2[2], c2[3]));
-                            }
-                            const float2 a = fma2(m2, make_float2(k2Log2e, k2Log2e), make_float2(p.b2s, p.b2s));
-                            B2CNN_EX2(te.x, a.x);
-                            B2CNN_EX2(te.y, a.y);
-                        }
-                        if constexpr (S == SegPlan::tail(1)) {
-                            const float2 d = add2(te, make_float2(1.0f, 1.0f));
-                            B2CNN_RCP(trx, d.x);
-                            B2CNN_RCP(try_, d.y);
-                        }
-                        // three bf16 pieces of (f0, f1) = features 2*jt-FOFF, 2*jt-FOFF+1 -> column kk of this lane's row of the A operand
-                        if constexpr (S == SegPlan::tail(2)) {
-                            tf = fma2(make_float2(trx, try_), make_float2(-2.0f, -2.0f), make_float2(1.0f, 1.0f));
-                            const uint32_t h = pack_bf16x2(tf.x, tf.y);
-                            tr1 = sub2(tf, make_float2(__uint_as_float(h << 16), __uint_as_float(h & 0xffff0000u)));
-                            tmem_st1(acol, h);
-                        }
-                        if constexpr (S == SegPlan::tail(3)) {
-                            const uint32_t md = pack_bf16x2(tr1.x, tr1.y);
-                            tf = sub2(tr1, make_float2(__uint_as_float(md << 16), __uint_as_float(md & 0xffff0000u)));
-                            tmem_st1(acol + 8, md);
-                        }
-                        if constexpr (S == SegPlan::tail(4)) tmem_st1(acol + 16, pack_bf16x2(tf.x, tf.y));
-                    }
-                };
-                static_for<0, SegPlan::kSegs>([&](auto s_) {
-                    segment(s_);
-                    if constexpr (doA && decltype(s_)::value == kLdtmSeg) prefetch_next();
-#if B2CNN_SEGMENTS
-                    if constexpr (decltype(s_)::value + 1 < SegPlan::kSegs) sched_fence();
-#endif
-                });
-            }
-#endif
-            if constexpr (doA) {                            // a1(block jj) replaces a1(block jj-2)
-#pragma unroll
-                for (int q2 = 0; q2 < 2; ++q2)
-#pragma unroll
-                    for (int r = 0; r < 4; ++r) abuf[PAR][r][q2] = an[r][q2];
-            }
-            // ---------------- bottom: arrivals ----------------
-            if constexpr (doA) {
-                if (n == kTcBlocks - 1) {                  // last read of this smem stage
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(BAR(o_bar + FuBars::kEmpty + s));
-                    n = 0; ++ti;
-                } else {
-                    ++n;
-                }
-            }
-            if constexpr (doBt) {
-                if (kk == 7 || (KK < 0 && jt == J - 1)) {
-                    const uint32_t abase = tlane + 128 + u * 24;
-                    if (KK < 0)
-                        for (int z = kk + 1; z < 8; ++z) { tmem_st1(abase + z, 0u); tmem_st1(abase + z + 8, 0u); tmem_st1(abase + z + 16, 0u); }
-                    tmem_st_wait();
-                    tc_fence_before();
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(BAR(o_bar + FuBars::kPFull + u));
-                }
-            }
-        };
-        using T_ = std::integral_constant<bool, true>;
-        using F_ = std::integral_constant<bool, false>;
-        using P0 = std::integral_constant<int, 0>;
-        using P1 = std::integral_constant<int, 1>;
-        using KR = std::integral_constant<int, -1>;
-        for (int item = blockIdx.x; item < p.n_items; item += gridDim.x) {
-        const Item g = item_geom(item);
-        J = g.J;
-        const int b = g.b_cta + t * kTcM + row;
-        const bool row_ok = b < p.B;
-        // stream state of a new item: everything it emits before its own data arrives is multiplied by zero weights, but
-        // a NaN left over from the previous item's windows must not leak into this one's (0 * NaN = NaN would flag them)
-        c2c = 0.f;
-#pragma unroll
-        for (int q2 = 0; q2 < 2; ++q2) {
-            pm6[q2] = make_float2(0.f, 0.f); pm7[q2] = make_float2(0.f, 0.f);
-#pragma unroll
-            for (int i = 0; i < 4; ++i) { abuf[0][i][q2] = make_float2(0.f, 0.f); abuf[1][i][q2] = make_float2(0.f, 0.f); }
-        }
-#pragma unroll
-        for (int i = 0; i < 4; ++i) { c2s[0][i] = 0.f; c2s[1][i] = 0.f; }
-        n = 0;
-        mbar_wait_parked(BAR(o_bar + FuBars::kTFull + 0), tq[0]);
-        tc_fence_after();
-        tmem_ld32_issue(tlane + 0, Dbuf[0]);
-#ifdef B2CNN_TIMING
-        const long long te0 = clock64();
-        if (lane == 0 && item == (int)blockIdx.x) atomicAdd(&g_fu_timing[12], (unsigned long long)(te0 - t_entry));
-#endif
-        iteration(0, gmb, T_{}, F_{}, F_{}, P0{}, KR{});
-        iteration(1, gmb, T_{}, T_{}, F_{}, P1{}, KR{});   // J is a multiple of kTcBlocks = 7: blocks 0 and 1 always exist
-        int jj = 2;
-#if B2CNN_UNROLL8
-        // whole chunks whose every iteration has a successor block (jj + 1 < J): iterations 8c+2 .. 8c+9 store the features
-        // of steps 8c .. 8c+7 = chunk c, with compile-time indices
-        const int nfull = J >= 11 ? (J - 3) >> 3 : 0;
-#pragma unroll 1
-        for (int c = 0; c < nfull; ++c, jj += 8) {
-            iteration(jj + 0, gmb + c, T_{}, T_{}, T_{}, P0{}, std::integral_constant<int, 1>{});
-            iteration(jj + 1, gmb + c, T_{}, T_{}, T_{}, P1{}, std::integral_constant<int, 2>{});
-            iteration(jj + 2, gmb + c, T_{}, T_{}, T_{}, P0{}, std::integral_constant<int, 3>{});
-            iteration(jj + 3, gmb + c, T_{}, T_{}, T_{}, P1{}, std::integral_constant<int, 4>{});
-            iteration(jj + 4, gmb + c, T_{}, T_{}, T_{}, P0{}, std::integral_constant<int, 5>{});
-            iteration(jj + 5, gmb + c, T_{}, T_{}, T_{}, P1{}, std::integral_constant<int, 6>{});
-            iteration(jj + 6, gmb + c, T_{}, T_{}, T_{}, P0{}, std::integral_constant<int, 7>{});
-            iteration(jj + 7, gmb + c, T_{}, T_{}, T_{}, P1{}, std::integral_constant<int, 0>{});
-        }
-#endif
-#pragma unroll 1
-        for (; jj + 1 < J; jj += 2) {                       // two iterations per trip: register names alternate (jj is even here)
-            iteration(jj, gmb + ((jj - 2) >> 3), T_{}, T_{}, T_{}, P0{}, KR{});
-            iteration(jj + 1, gmb + ((jj - 1) >> 3), T_{}, T_{}, T_{}, P1{}, KR{});
-        }
-        if (jj < J) { iteration(jj, gmb + ((jj - 2) >> 3), T_{}, T_{}, T_{}, P0{}, KR{}); ++jj; }
-        // jj == J: drain the pipeline (conv2 of step J-1, features of steps J-2 and J-1)
-        if (J & 1) {
-            iteration(J, gmb + ((J - 2) >> 3), F_{}, T_{}, T_{}, P1{}, KR{});
-            iteration(J + 1, gmb + ((J - 1) >> 3), F_{}, F_{}, T_{}, P0{}, KR{});
-        } else {
-            iteration(J, gmb + ((J - 2) >> 3), F_{}, T_{}, T_{}, P0{}, KR{});
-            iteration(J + 1, gmb + ((J - 1) >> 3), F_{}, F_{}, T_{}, P1{}, KR{});
-        }
-
-#ifdef B2CNN_TIMING
-        if (lane == 0) atomicAdd(&g_fu_timing[0], (unsigned long long)(clock64() - te0));
-        const long long tg0 = clock64();
-        FU_TFLUSH(0, lane == 0);
-        for (int i__ = 0; i__ < 4; ++i__) fu_tacc[i__] = 0;
-#endif
-        // ---- gate pre-activations of this CTA's position range -> partial[range][window][64]
-        mbar_wait_parked(BAR(o_bar + FuBars::kGFull), it & 1);
-        tc_fence_after();
-        float *dst = p.partial + ((int64_t)g.r * p.B + b) * kGates;
-#if B2CNN_PARTIAL_EVICT_LAST
-        uint64_t pol_last;
-        asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol_last));
-#endif
-        // A NaN feature (a NaN / inf sample met a zero of the band matrix, or a real NaN) makes every gate it is
-        // multiplied into NaN -- zero weights included -- so the 64 sums themselves are the probe: no per-step test.
-        bool bad = false;
-#pragma unroll
-        for (int half = 0; half < 2; ++half) {
-            uint32_t G[32];
-            tmem_ld32_issue(tlane + 192 + half * 32, G);
-            tmem_ld32_wait(G);
-#pragma unroll
-            for (int k = 0; k < 32; ++k) bad |= (G[k] & 0x7fffffffu) > 0x7f800000u;
-            if (row_ok) {
 #pragma unroll
                 for (int k = 0; k < 32; k += 4) {
-#if B2CNN_PARTIAL_EVICT_LAST
-                    // the head reads these 39 MB back right after the kernel: ask the L2 to keep them while 1.8 GB of windows stream through
-                    asm volatile("st.global.L2::cache_hint.v4.b32 [%0], {%1, %2, %3, %4}, %5;" ::"l"(dst + half * 32 + k), "r"(G[k]), "r"(G[k + 1]),
-                                 "r"(G[k + 2]), "r"(G[k + 3]), "l"(pol_last) : "memory");
-#else
-                    *reinterpret_cast<uint4 *>(dst + half * 32 + k) = make_uint4(G[k], G[k + 1], G[k + 2], G[k + 3]);
-#endif
+                    const float4 v = *reinterpret_cast<const float4 *>(sT + row * kHpTStride + k);
+                    D[k] = v.x; D[k + 1] = v.y; D[k + 2] = v.z; D[k + 3] = v.w;
+                }
+                wg_bar();                             // transpose buffer free for the next block
+            } else {
+                // conv1 of block j on the CUDA cores, exact fp32, from the 16 samples at tile offset 8n
+                if (n == 0) mbar_wait(bar_full + 8 * s, (i >> 1) & 1);
+#pragma unroll
+                for (int k = 0; k < 32; ++k) D[k] = 0.f;
+#pragma unroll 1
+                for (int c = 0; c < C; ++c) {
+                    float xs[16];
+#pragma unroll
+                    for (int j4 = 0; j4 < 4; ++j4) {
+                        const float4 v = *reinterpret_cast<const float4 *>(sA_of(s, c) + row * 128 + (((uint32_t)(2 * n + j4) ^ swz) << 4));
+                        xs[4 * j4 + 0] = v.x; xs[4 * j4 + 1] = v.y; xs[4 * j4 + 2] = v.z; xs[4 * j4 + 3] = v.w;
+                    }
+                    if constexpr (ARCH == 0) {
+#pragma unroll
+                        for (int o = 0; o < kCMid; ++o) pm7[o] = fmaf(p.w1[c][9][o], xs[8], pm7[o]);
+                    }
+#pragma unroll
+                    for (int k = 0; k < K1; ++k)
+#pragma unroll
+                        for (int sft = 0; sft < 8; ++sft)
+                            if (sft + k < 16) {
+#pragma unroll
+                                for (int o = 0; o < kCMid; ++o) D[sft * 4 + o] = fmaf(p.w1[c][k][o], xs[sft + k], D[sft * 4 + o]);
+                            }
+                }
+                if (n == kBlocks - 1) {
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(bar_empty + 8 * s);
+                }
+            }
+            // ---- pool1 on pre-activations, then r = (1 - tanh(+bias)) / 2: a1 positions of this block
+            float an[4][kCMid];
+#pragma unroll
+            for (int o = 0; o < kCMid; ++o) {
+                if constexpr (ARCH == 0) {
+                    an[0][o] = sig_fold(max3_nan(pm6[o], pm7[o], D[0 * 4 + o]), p.b1s[o]);
+                    an[1][o] = sig_fold(max3_nan(D[0 * 4 + o], D[1 * 4 + o], D[2 * 4 + o]), p.b1s[o]);
+                    an[2][o] = sig_fold(max3_nan(D[2 * 4 + o], D[3 * 4 + o], D[4 * 4 + o]), p.b1s[o]);
+                    an[3][o] = sig_fold(max3_nan(D[4 * 4 + o], D[5 * 4 + o], D[6 * 4 + o]), p.b1s[o]);
+                    pm6[o] = D[6 * 4 + o];
+                    pm7[o] = D[7 * 4 + o];
+                } else {
+#pragma unroll
+                    for (int r = 0; r < 4; ++r) an[r][o] = sig_fold(max_nan(D[(2 * r) * 4 + o], D[(2 * r + 1) * 4 + o]), p.b1s[o]);
+                }
+            }
+            // ---- conv2 over the previous block's and this block's a1 (no bias yet)
+            float c2[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+            for (int c = 0; c < kCMid; ++c) {
+                const float A8[8] = {ah[0][c], ah[1][c], ah[2][c], ah[3][c], an[0][c], an[1][c], an[2][c], an[3][c]};
+#pragma unroll
+                for (int k = 0; k < 5; ++k)
+#pragma unroll
+                    for (int r = 0; r < 4; ++r) c2[r] = fmaf(p.w2n[c][k], A8[r + k], c2[r]);
+            }
+#pragma unroll
+            for (int c = 0; c < kCMid; ++c)
+#pragma unroll
+                for (int r = 0; r < 4; ++r) ah[r][c] = an[r][c];
+            // ---- pool2 + tanh(+bias): the two features of step j
+            float f0, f1;
+            if constexpr (ARCH == 0) {
+                f0 = tanh_fold(max3_nan(c2c, c2[0], c2[1]), p.b2s);
+                f1 = tanh_fold(max3_nan(c2[1], c2[2], c2[3]), p.b2s);
+                c2c = c2[3];
+            } else {
+                f0 = tanh_fold(max_nan(c2[0], c2[1]), p.b2s);
+                f1 = tanh_fold(max_nan(c2[2], c2[3]), p.b2s);
+            }
+            if constexpr (OUT == kOutFeatures) {
+                nan_probe = fmaf(f0, 0.f, nan_probe);
+                nan_probe = fmaf(f1, 0.f, nan_probe);
+                const int pr0 = 2 * j - FOFF;
+                if (row_ok) {
+                    if (pr0 >= 0 && pr0 < nfeat) fout[(int64_t)pr0 * p.sP] = f0;
+                    if (pr0 + 1 >= 0 && pr0 + 1 < nfeat) fout[(int64_t)(pr0 + 1) * p.sP] = f1;
+                }
+            } else {
+                // three bf16 pieces of (f0, f1) -> word kk of this window's row of the A tiles
+                const int kk = j & 7, m = j >> 3, u = m & 1;
+                const uint32_t h = pack_bf16x2(f0, f1);
+                const float r1x = f0 - __uint_as_float(h << 16), r1y = f1 - __uint_as_float(h & 0xffff0000u);
+                const uint32_t md = pack_bf16x2(r1x, r1y);
+                const uint32_t lo = pack_bf16x2(r1x - __uint_as_float(md << 16), r1y - __uint_as_float(md & 0xffff0000u));
+                uint8_t *arow = sPc + (row >> 3) * 256 + (row & 7) * 16;
+                auto put = [&](int col, uint32_t w0, uint32_t w1, uint32_t w2) {
+                    const int off = (col >> 2) * 128 + (col & 3) * 4;
+                    *reinterpret_cast<uint32_t *>(arow + off) = w0;
+                    *reinterpret_cast<uint32_t *>(arow + kHpPieceBytes + off) = w1;
+                    *reinterpret_cast<uint32_t *>(arow + 2 * kHpPieceBytes + off) = w2;
+                };
+                put(kk, h, md, lo);
+                if (kk == 7 || j == J - 1) {
+                    for (int z = kk + 1; z < 8; ++z) put(z, 0u, 0u, 0u);
+                    fence_proxy_async();
+                    wg_bar();
+                    mbar_wait(bar_wfull + 8 * u, (m >> 1) & 1);
+                    const uint32_t pa = smem_u32(sPc), pw = smem_u32(sW + u * kFuWChunkBytes);
+                    wgmma_fence();
+#pragma unroll
+                    for (int hh = 0; hh < 2; ++hh) {
+                        // piece pairs (feature piece, weight piece) with fp + wp <= 2: hh hm mh hl lh mm
+                        constexpr int kAp[6] = {0, 0, 1, 0, 2, 1}, kWp[6] = {0, 1, 0, 2, 0, 1};
+#pragma unroll
+                        for (int q = 0; q < 6; ++q)
+                            wgmma_m64n64(gacc[hh], gdesc_none_kmajor(pa + kAp[q] * kHpPieceBytes + hh * 2048, 128, 256),
+                                         gdesc_none_kmajor(pw + kWp[q] * 2048, 128, 256));
+                    }
+                    wgmma_commit();
+                    wgmma_wait<0>();
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(bar_wempty + 8 * u);
+                    wg_bar();                         // A tiles free for the next chunk
                 }
             }
         }
-        // up to n_ranges CTAs may flag the same window: the first one appends it to the list of the exact re-computation
-        if (row_ok && bad && atomicExch(&p.nanflag[b], 1) == 0) p.list[atomicAdd(p.count, 1)] = b;
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(BAR(o_bar + FuBars::kGEmpty));          // the MMA warp may start the next item's gate sums
-        // phases of the next item: ring slot s was used ceil((J - s) / 4) times, the chunk counter moves on
-#pragma unroll
-        for (int sl = 0; sl < 4; ++sl) tq[sl] ^= (uint32_t)((J - sl + 3) >> 2) & 1u;
-        tqm = tq[0] | (tq[1] << 1) | (tq[2] << 2) | (tq[3] << 3);
-        gmb += g.nchunks; ++it;
-#ifdef B2CNN_TIMING
-        if (lane == 0) atomicAdd(&g_fu_timing[10], (unsigned long long)(clock64() - tg0));
-#endif
-        }   // items
-#ifdef B2CNN_TIMING
-        if (threadIdx.x == 128 && blockIdx.x == 0) {
-            atomicAdd(&g_fu_timing[11], 1ull);
-            unsigned long long gt_exit;
-            asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(gt_exit));
-            atomicAdd(&g_fu_timing[14], gt_exit - gt_entry);                                  // ns
-            atomicAdd(&g_fu_timing[15], (unsigned long long)(clock64() - t_entry));          // SM cycles over the same span
-        }
-        if (lane == 0) atomicAdd(&g_fu_timing[13], (unsigned long long)(clock64() - t_entry));
-#endif
-    }
 
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 3) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(512) : "memory");
+        if constexpr (OUT == kOutFeatures) {
+            if (row_ok && nan_probe != nan_probe) p.nanflag[b] = 1;
+        } else {
+            // gate pre-activations of this CTA's position range -> partial[range][window][64].  A NaN feature (a NaN / inf
+            // sample met a zero of the band matrix, or a real NaN) makes every gate it is multiplied into NaN -- zero weights
+            // included -- so the sums themselves are the probe.
+#pragma unroll
+            for (int hh = 0; hh < 2; ++hh)
+#pragma unroll
+                for (int e2 = 0; e2 < 2; ++e2) {
+                    const int r = 64 * hh + 16 * warp + (lane >> 2) + 8 * e2;
+                    const int bb = b0 + r;
+                    bool bad = false;
+#pragma unroll
+                    for (int e = 0; e < 32; ++e)
+                        if (((e >> 1) & 1) == e2) bad |= gacc[hh][e] != gacc[hh][e];
+                    if (bb < p.B) {
+                        float *dst = p.partial + ((int64_t)blockIdx.y * p.B + bb) * kGates + 2 * (lane & 3);
+#pragma unroll
+                        for (int e = 2 * e2; e < 32; e += 4)
+                            *reinterpret_cast<float2 *>(dst + 8 * (e >> 2)) = make_float2(gacc[hh][e], gacc[hh][e + 1]);
+                        // up to n_ranges CTAs (and four threads of one) may flag the same window: the first appends it
+                        if (bad && atomicExch(&p.nanflag[bb], 1) == 0) p.list[atomicAdd(p.count, 1)] = bb;
+                    }
+                }
+        }
     }
 }
 
-// W_ih_l0 [64][L] fp32 -> per (range, 16-position chunk) three bf16 pieces in UMMA K-major
+// W_ih_l0 [64][L] fp32 -> per (range, 16-position chunk) three bf16 pieces in GMMA K-major
 // no-swizzle core-matrix order (byte = (g/8)*256 + (k/8)*128 + (g%8)*16 + (k%8)*2 per piece).
-// Chunk m of a range covers relative features 16m-3 .. 16m+12 (the stream emits 2j-3, 2j-2 at
+// Chunk m of a range covers relative features 16m-foff .. 16m-foff+15 (the stream emits 2j-foff, 2j-foff+1 at
 // step j); positions outside the range or beyond L get zero weights, which also masks the
 // stream's warm-up / tail garbage.
 __global__ void tc_pack_wih_kernel(const float *__restrict__ wih, uint8_t *__restrict__ out, int L, int feats_per_cta,
@@ -773,7 +372,7 @@ __global__ void tc_pack_wih_kernel(const float *__restrict__ wih, uint8_t *__res
     const int k = (int)(e & 15), g = (int)((e >> 4) & 63);
     const int64_t cm = e >> 10;
     const int m = (int)(cm % chunks_per_cta), pr = (int)(cm / chunks_per_cta);
-    const int prel = 16 * m - foff + k;              // step j emits features 2j-foff, 2j-foff+1
+    const int prel = 16 * m - foff + k;
     const int pos = pr * feats_per_cta + prel;
     float w = 0.f;
     if (prel >= 0 && prel < feats_per_cta && pos < L) w = wih[(int64_t)g * L + pos];

@@ -1,5 +1,5 @@
-// b2cnn_tc_ptx.cuh -- inline-PTX wrappers for TMA, mbarrier, tcgen05 (MMA / TMEM) on sm_100a,
-// and the UMMA shared-memory / instruction descriptor encodings used by b2cnn_tc*.cu.
+// b2cnn_tc_ptx.cuh -- inline-PTX wrappers for TMA, mbarrier and wgmma (warpgroup MMA) on sm_90a,
+// and the GMMA shared-memory descriptor encodings used by b2cnn_tc*.cu.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -8,9 +8,6 @@
 namespace b2cnn {
 
 constexpr float k2Log2e = 2.8853900817779268f;
-#ifndef B2CNN_MONTGOMERY
-#define B2CNN_MONTGOMERY 1                        // pairs of activations share one MUFU.RCP (see sig_fold2 / sig_ph2)
-#endif
 
 // ------------------------------------------------------------------------------------------
 // PTX wrappers
@@ -28,16 +25,6 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
             : "=r"(done) : "r"(bar), "r"(parity) : "memory");
     } while (!done);
 }
-// same wait with a suspend-time hint: the waiting warp is parked by the hardware (woken by the
-// completing arrive) instead of burning issue slots that the epilogue warps on its scheduler need
-__device__ __forceinline__ void mbar_wait_parked(uint32_t bar, uint32_t parity) {
-    uint32_t done;
-    do {
-        asm volatile(
-            "{\n .reg .pred p;\n mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2, %3;\n selp.u32 %0, 1, 0, p;\n}"
-            : "=r"(done) : "r"(bar), "r"(parity), "r"(20000u) : "memory");
-    } while (!done);
-}
 __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
@@ -49,35 +36,17 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap *tm,
         "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4}], [%5];"
         ::"r"(dst), "l"(tm), "r"(c0), "r"(c1), "r"(c2), "r"(bar) : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void umma_bf16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n .reg .pred p;\n setp.ne.b32 p, %4, 0;\n tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n}"
-        ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
+__device__ __forceinline__ void bulk_load_1d(uint32_t dst, const void *src, uint32_t bytes, uint32_t bar) {
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                 ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
 }
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float *v) {
-    uint32_t r[32];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr) : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
-}
-__device__ __forceinline__ float max3_nan(float a, float b, float c) {
-    float r;
-    asm("max.NaN.f32 %0, %1, %2, %3;" : "=f"(r) : "f"(a), "f"(b), "f"(c));
-    return r;
-}
+// named barrier of the consumer warpgroup (id 1, 128 threads): barrier 0 stays __syncthreads()
+__device__ __forceinline__ void wg_bar() { asm volatile("bar.sync 1, 128;" ::: "memory"); }
+// generic-proxy shared-memory writes -> visible to the async proxy (wgmma operand reads)
+__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+
+// max_nan: b2cnn_internal.cuh
+__device__ __forceinline__ float max3_nan(float a, float b, float c) { return max_nan(max_nan(a, b), c); }
 // tanh(m + bias) with bias pre-multiplied by 2 log2 e:  1 - 2 / (1 + 2^(2 log2e (m + bias)))
 __device__ __forceinline__ float tanh_fold(float m, float bias_scaled) {
     float e, r;
@@ -85,70 +54,13 @@ __device__ __forceinline__ float tanh_fold(float m, float bias_scaled) {
     asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(e + 1.0f));
     return fmaf(-2.0f, r, 1.0f);
 }
-
-// UMMA shared-memory descriptors (cute::UMMA::SmemDescriptor bit layout, version 1 = sm_100)
-__device__ __forceinline__ uint64_t desc_sw128_kmajor(uint32_t saddr) {
-    // rows 128 B apart, 8-row groups 1024 B apart, layout_type 2 = SWIZZLE_128B
-    return (uint64_t)((saddr >> 4) & 0x3FFF) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) |
-           ((uint64_t)1 << 46) | ((uint64_t)2 << 61);
-}
-__device__ __forceinline__ uint64_t desc_none_kmajor(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-    return (uint64_t)((saddr >> 4) & 0x3FFF) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16) |
-           ((uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32) | ((uint64_t)1 << 46);
-}
-
-
-// ---- additions for the fused-projection kernel ------------------------------------------
-__device__ __forceinline__ void bulk_load_1d(uint32_t dst, const void *src, uint32_t bytes, uint32_t bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem]
-__device__ __forceinline__ void umma_bf16_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n .reg .pred p;\n setp.ne.b32 p, %4, 0;\n tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n}"
-        ::"r"(d_tmem), "r"(a_tmem), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void tmem_st1(uint32_t taddr, uint32_t v) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x1.b32 [%0], {%1};" ::"r"(taddr), "r"(v) : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-// asynchronous TMEM load: issue now, consume after tmem_ld32_wait(v)
-__device__ __forceinline__ void tmem_ld32_issue(uint32_t taddr, uint32_t *r) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr) : "memory");
-}
-// the "+r" operands tie every later use of r[] to this wait
-__device__ __forceinline__ void tmem_ld32_wait(uint32_t *r) {
-    asm volatile("tcgen05.wait::ld.sync.aligned;"
-        : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]), "+r"(r[8]),
-          "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]), "+r"(r[15]), "+r"(r[16]),
-          "+r"(r[17]), "+r"(r[18]), "+r"(r[19]), "+r"(r[20]), "+r"(r[21]), "+r"(r[22]), "+r"(r[23]), "+r"(r[24]),
-          "+r"(r[25]), "+r"(r[26]), "+r"(r[27]), "+r"(r[28]), "+r"(r[29]), "+r"(r[30]), "+r"(r[31])
-        :: "memory");
-}
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t *r) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};"
-        ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-          "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]) : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t *r) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr) : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;"
-        : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]), "+r"(r[8]),
-          "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]), "+r"(r[15])
-        :: "memory");
+// r = 1 / (1 + 2^(2 log2e (m + bias))): tanh(m + bias) == 1 - 2 r.  conv2 consumes r directly (its weights are
+// pre-multiplied by -2 and its bias absorbs sum(w)), saving the final FMA.  2^a = inf gives r = 0 without a clamp.
+__device__ __forceinline__ float sig_fold(float m, float bias_scaled) {
+    float e, r;
+    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(fmaf(m, k2Log2e, bias_scaled)));
+    asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(e + 1.0f));
+    return r;
 }
 // two floats -> packed bf16x2 (round to nearest even): low half = lo_elem, high half = hi_elem
 __device__ __forceinline__ uint32_t pack_bf16x2(float lo_elem, float hi_elem) {
@@ -156,193 +68,49 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float lo_elem, float hi_elem) {
     asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi_elem), "f"(lo_elem));
     return r;
 }
-// one lane of a converged warp (the rest of the warp stays warp-uniform, so descriptor
-// arithmetic can live in the uniform datapath instead of being moved there per MMA)
-__device__ __forceinline__ bool elect_one() {
-    uint32_t pred;
-    asm volatile("{\n .reg .pred p;\n elect.sync _|p, 0xffffffff;\n selp.u32 %0, 1, 0, p;\n}" : "=r"(pred));
-    return pred != 0;
-}
-// descriptors passed as (lo, hi) halves: the hi half is a per-operand constant
-__device__ __forceinline__ void umma_ss(uint32_t d_tmem, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo, uint32_t b_hi,
-                                        uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n .reg .pred p;\n .reg .b64 da, db;\n mov.b64 da, {%1, %2};\n mov.b64 db, {%3, %4};\n setp.ne.b32 p, %6, 0;\n"
-        " tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, p;\n}"
-        ::"r"(d_tmem), "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(accumulate) : "memory");
-}
-// The same MMA with an A-collector qualifier.  Consecutive MMAs of ONE issuing thread that multiply the same A
-// slice by different B matrices (the bf16 pieces of a band matrix) keep A in the tensor core's collector buffer
-// -- COLL 1 = ::fill (first), 2 = ::use, 3 = ::lastuse -- instead of re-reading 4 KB of shared memory each time
-// (SASS: UTCHMMA gdesc[..].A_KEEP / .A_REUSE.A_KEEP / .A_REUSE).  No other MMA may be issued in between.
-template <int COLL>
-__device__ __forceinline__ void umma_ss_coll(uint32_t d_tmem, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo, uint32_t b_hi,
-                                             uint32_t idesc, uint32_t accumulate) {
-    if constexpr (COLL == 1)
-        asm volatile(
-            "{\n .reg .pred p;\n .reg .b64 da, db;\n mov.b64 da, {%1, %2};\n mov.b64 db, {%3, %4};\n setp.ne.b32 p, %6, 0;\n"
-            " tcgen05.mma.cta_group::1.kind::f16.collector::a::fill [%0], da, db, %5, p;\n}"
-            ::"r"(d_tmem), "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(accumulate) : "memory");
-    else if constexpr (COLL == 2)
-        asm volatile(
-            "{\n .reg .pred p;\n .reg .b64 da, db;\n mov.b64 da, {%1, %2};\n mov.b64 db, {%3, %4};\n setp.ne.b32 p, %6, 0;\n"
-            " tcgen05.mma.cta_group::1.kind::f16.collector::a::use [%0], da, db, %5, p;\n}"
-            ::"r"(d_tmem), "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(accumulate) : "memory");
-    else if constexpr (COLL == 3)
-        asm volatile(
-            "{\n .reg .pred p;\n .reg .b64 da, db;\n mov.b64 da, {%1, %2};\n mov.b64 db, {%3, %4};\n setp.ne.b32 p, %6, 0;\n"
-            " tcgen05.mma.cta_group::1.kind::f16.collector::a::lastuse [%0], da, db, %5, p;\n}"
-            ::"r"(d_tmem), "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(accumulate) : "memory");
-    else
-        umma_ss(d_tmem, a_lo, a_hi, b_lo, b_hi, idesc, accumulate);
-}
-// The same with ready 64-bit descriptors: loop-invariant B descriptors stay in uniform-register pairs instead of being
-// re-assembled (UMOV of the constant half + add of the offset) in front of every MMA -- the issuing warp's instruction
-// count per block is on the critical path of the accumulator ring (b2cnn_tc_fused.cuh).
-template <int COLL>
-__device__ __forceinline__ void umma_ss_coll64(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    if constexpr (COLL == 1)
-        asm volatile("{\n .reg .pred p;\n setp.ne.b32 p, %4, 0;\n tcgen05.mma.cta_group::1.kind::f16.collector::a::fill [%0], %1, %2, %3, p;\n}"
-                     ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-    else if constexpr (COLL == 2)
-        asm volatile("{\n .reg .pred p;\n setp.ne.b32 p, %4, 0;\n tcgen05.mma.cta_group::1.kind::f16.collector::a::use [%0], %1, %2, %3, p;\n}"
-                     ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-    else if constexpr (COLL == 3)
-        asm volatile("{\n .reg .pred p;\n setp.ne.b32 p, %4, 0;\n tcgen05.mma.cta_group::1.kind::f16.collector::a::lastuse [%0], %1, %2, %3, p;\n}"
-                     ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-    else
-        asm volatile("{\n .reg .pred p;\n setp.ne.b32 p, %4, 0;\n tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n}"
-                     ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void umma_ts(uint32_t d_tmem, uint32_t a_tmem, uint32_t b_lo, uint32_t b_hi, uint32_t idesc,
-                                        uint32_t accumulate) {
-    asm volatile(
-        "{\n .reg .pred p;\n .reg .b64 db;\n mov.b64 db, {%2, %3};\n setp.ne.b32 p, %5, 0;\n"
-        " tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], db, %4, p;\n}"
-        ::"r"(d_tmem), "r"(a_tmem), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(accumulate) : "memory");
-}
-#if defined(B2CNN_ABLATE) && B2CNN_ABLATE == 2
-#define B2CNN_EX2(dst, src) dst = (src) * 0.75f
-#define B2CNN_RCP(dst, src) dst = (src) * 0.75f
-#else
-#define B2CNN_EX2(dst, src) asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(dst) : "f"(src))
-#define B2CNN_RCP(dst, src) asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(dst) : "f"(src))
-#endif
-// ---- packed fp32x2 arithmetic (FFMA2 / FADD2 on sm_100): two FMAs per issue slot ------------
-__device__ __forceinline__ uint64_t pk2(float2 v) {
-    uint64_t r;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(v.x), "f"(v.y));
-    return r;
-}
-__device__ __forceinline__ float2 up2(uint64_t v) {
-    float2 r;
-    asm("mov.b64 {%0, %1}, %2;" : "=f"(r.x), "=f"(r.y) : "l"(v));
-    return r;
-}
-__device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) {
-    uint64_t d;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(pk2(a)), "l"(pk2(b)), "l"(pk2(c)));
-    return up2(d);
-}
-__device__ __forceinline__ float2 add2(float2 a, float2 b) {
-    uint64_t d;
-    asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(pk2(a)), "l"(pk2(b)));
-    return up2(d);
-}
-__device__ __forceinline__ float2 sub2(float2 a, float2 b) {
-    uint64_t d;
-    asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(pk2(a)), "l"(pk2(b)));
-    return up2(d);
-}
-// tanh(m + bias) for two values, bias pre-multiplied by 2 log2 e (see tanh_fold)
-__device__ __forceinline__ float2 tanh_fold2(float2 m, float2 bias_scaled) {
-    const float2 a = fma2(m, make_float2(k2Log2e, k2Log2e), bias_scaled);
-    float e0, e1, r0, r1;
-    B2CNN_EX2(e0, a.x);
-    B2CNN_EX2(e1, a.y);
-    const float2 d = add2(make_float2(e0, e1), make_float2(1.0f, 1.0f));
-    B2CNN_RCP(r0, d.x);
-    B2CNN_RCP(r1, d.y);
-    return fma2(make_float2(r0, r1), make_float2(-2.0f, -2.0f), make_float2(1.0f, 1.0f));
-}
-// r = 1 / (1 + 2^(2 log2e (m + bias))) for two values: tanh(m + bias) == 1 - 2 r.  conv2 consumes r
-// directly (its weights are pre-multiplied by -2 and its bias absorbs sum(w)), saving the final FMA.
-// B2CNN_MONTGOMERY: one MUFU.RCP for the pair -- rp = 1/(d0*d1), r0 = rp*d1, r1 = rp*d0 -- which cuts
-// the MUFU count per pair from 4 to 3 (the MUFU pipe is the busiest unit of the fused kernel).  The
-// exponent is clamped (NaN-propagating) so that d stays finite: 0 * inf can then never appear, and
-// a product that overflows gives rp = 0 -> r = 0, the correctly rounded answer for such arguments.
-__device__ __forceinline__ float min_nan(float a, float b) {
-    float r;
-    asm("min.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
-    return r;
-}
-__device__ __forceinline__ float2 mul2(float2 a, float2 b) {
-    uint64_t d;
-    asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(pk2(a)), "l"(pk2(b)));
-    return up2(d);
-}
-__device__ __forceinline__ float2 sig_fold2(float2 m, float2 bias_scaled) {
-    float2 a = fma2(m, make_float2(k2Log2e, k2Log2e), bias_scaled);
-    float e0, e1;
-#if B2CNN_MONTGOMERY && !defined(B2CNN_EXP_NOCLAMP)           // NOCLAMP: timing experiment only (0 * inf -> NaN for |x| > 44)
-    a.x = min_nan(a.x, 120.0f);
-    a.y = min_nan(a.y, 120.0f);
-#endif
-    B2CNN_EX2(e0, a.x);
-    B2CNN_EX2(e1, a.y);
-    const float2 d = add2(make_float2(e0, e1), make_float2(1.0f, 1.0f));
-#if B2CNN_MONTGOMERY
-    float rp;
-    B2CNN_RCP(rp, d.x * d.y);
-    return mul2(make_float2(rp, rp), make_float2(d.y, d.x));
-#else
-    float r0, r1;
-    B2CNN_RCP(r0, d.x);
-    B2CNN_RCP(r1, d.y);
-    return make_float2(r0, r1);
-#endif
-}
-// The same activation in three phases, for the segmented epilogue (b2cnn_tc_fused.cuh): a segment issues phase 1 of one
-// pair, phase 2 of the pair before and phase 3 of the pair before that, so every MUFU result has a whole segment of
-// other work between its issue and its first use.
-//   phase 1: e = 2^(clamp(2 log2e (m + bias)))          FFMA2, 2 FMNMX, 2 MUFU.EX2
-//   phase 2: d = e + 1, rp = 1 / (d.x * d.y)            FADD2, FMUL, MUFU.RCP
-//   phase 3: r = rp * (d.y, d.x)                        FMUL2
-__device__ __forceinline__ float2 sig_ph1(float2 m, float2 bias_scaled) {
-    float2 a = fma2(m, make_float2(k2Log2e, k2Log2e), bias_scaled);
-    float e0, e1;
-#if B2CNN_MONTGOMERY && !defined(B2CNN_EXP_NOCLAMP)
-    a.x = min_nan(a.x, 120.0f);
-    a.y = min_nan(a.y, 120.0f);
-#endif
-    B2CNN_EX2(e0, a.x);
-    B2CNN_EX2(e1, a.y);
-    return make_float2(e0, e1);
-}
-#if B2CNN_MONTGOMERY
-__device__ __forceinline__ void sig_ph2(float2 e, float2 &d, float &rp) {
-    d = add2(e, make_float2(1.0f, 1.0f));
-    B2CNN_RCP(rp, d.x * d.y);
-}
-__device__ __forceinline__ float2 sig_ph3(float2 d, float rp) { return mul2(make_float2(rp, rp), make_float2(d.y, d.x)); }
-#else
-// one MUFU.RCP per activation: 2^a = inf gives d = inf and r = 0 without any clamp, and the two FMA-pipe products of
-// the batched reciprocal disappear -- per pair 4 MUFU instead of 3, but 6 dispatch cycles fewer (pipes.cu: a packed
-// f32x2 op and an ALU-pipe op each hold the dispatch port 2 cycles and do not overlap; a MUFU overlaps with both)
-__device__ __forceinline__ void sig_ph2(float2 e, float2 &d, float &rp) {
-    const float2 t = add2(e, make_float2(1.0f, 1.0f));
-    B2CNN_RCP(d.x, t.x);
-    B2CNN_RCP(d.y, t.y);
-    rp = 0.f;
-}
-__device__ __forceinline__ float2 sig_ph3(float2 d, float) { return d; }
-#endif
-// scheduling fence: ptxas does not move instructions across a pmevent (SASS PMTRIG, one issue slot, no branch), which
-// is what keeps the segments of the epilogue in source order (b2cnn_tc_fused.cuh)
-__device__ __forceinline__ void sched_fence() { asm volatile("pmevent 1;" ::: "memory"); }
 
-constexpr uint32_t make_idesc_bf16(uint32_t M, uint32_t N) {
-    return (1u << 4) | (1u << 7) | (1u << 10) | ((N >> 3) << 17) | ((M >> 4) << 24);
+// ------------------------------------------------------------------------------------------
+// wgmma (sm_90a): D[64 x N] (+)= A[64 x 16] * B[N x 16]^T, A and B bf16 K-major in shared memory, D fp32 in registers.
+// Fragment of D held by thread t of the warpgroup (warp w = t / 32, lane l): element i of the N/2 registers is
+// row 16 w + l / 4 + 8 ((i / 2) % 2), column 8 (i / 4) + 2 (l % 4) + i % 2.
+// ------------------------------------------------------------------------------------------
+// GMMA shared-memory descriptor: start >> 4 | LBO >> 4 << 16 | SBO >> 4 << 32 | layout << 62 (1 = SWIZZLE_128B, 0 = none)
+__device__ __forceinline__ uint64_t gdesc_sw128_kmajor(uint32_t saddr) {
+    // rows 128 B apart, 8-row groups 1024 B apart (SBO); LBO unused for swizzled K-major
+    return (uint64_t)((saddr >> 4) & 0x3FFF) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 62);
+}
+// no swizzle, K-major core matrices (8 rows x 16 bytes): LBO = K-adjacent core matrices, SBO = M/N-adjacent ones
+__device__ __forceinline__ uint64_t gdesc_none_kmajor(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+    return (uint64_t)((saddr >> 4) & 0x3FFF) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16) |
+           ((uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32);
+}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+
+// the "+f" operands tie the accumulator registers to every wgmma and to the wait that follows
+__device__ __forceinline__ void wgmma_m64n32(float *d, uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+    asm volatile(
+        "{\n .reg .pred p;\n setp.ne.b32 p, %18, 0;\n"
+        " wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
+        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, 0, 0;\n}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(adesc), "l"(bdesc), "r"(accumulate) : "memory");
+}
+// always accumulates: D += A * B
+__device__ __forceinline__ void wgmma_m64n64(float *d, uint64_t adesc, uint64_t bdesc) {
+    asm volatile(
+        "{\n .reg .pred p;\n setp.ne.b32 p, 1, 0;\n"
+        " wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,"
+        "%30,%31}, %32, %33, p, 1, 1, 0, 0;\n}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+          "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+          "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(adesc), "l"(bdesc) : "memory");
 }
 
 }  // namespace b2cnn

@@ -12,7 +12,7 @@ Mirrors the reference's operator interface for the hot path:
   every row an independent window from the zero LSTM state (what looping ``model(x[i:i+1])`` gives).
 
 The sub-modules (``conv1``, ``lstm`` ...) are parameter containers only; the arithmetic runs in
-libb2cnn.so (hand-written sm_100a kernels) through ctypes.  No CUDA device -> RuntimeError.
+libb2cnn.so (hand-written sm_90a kernels) through ctypes.  No CUDA device -> RuntimeError.
 """
 from __future__ import annotations
 
@@ -199,7 +199,7 @@ class B200MyCNN(nn.Module):
             pass
 
     def set_path(self, path: str):
-        """'auto' | 'generic' (exact fp32 CUDA cores) | 'tensorcore' (tcgen05 conv1)."""
+        """'auto' | 'generic' (exact fp32 CUDA cores) | 'tensorcore' (wgmma conv1)."""
         self._path = path
         self.__dict__["_ws_need"] = {}                     # the scratch size depends on the path a call takes
         if self._handle is not None:
