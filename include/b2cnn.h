@@ -236,8 +236,7 @@ const char *b2cnn_version(void);
 /* ---- One training step on the device (SURVEY.md section 8, row f4) ----
  * Replaces the body of the reference's training loop (bin/utils.py:200-208):
  *     optimizer.zero_grad(); output = model(input, age); loss = criterion(output, target); loss.backward(); optimizer.step()
- * with criterion = nn.BCEWithLogitsLoss() (bin/utils.py:663) and torch.optim.Adam (bin/explore_torch.ipynb:3204-3205;
- * no amsgrad, no weight decay), for the model in train() mode: B2CNN_MODE_SEQUENCE is what model(input_batch, age)
+ * with criterion = nn.BCEWithLogitsLoss() and torch.optim.Adam (bin/explore_torch.ipynb:3204-3205; no amsgrad, no weight decay), for the model in train() mode: B2CNN_MODE_SEQUENCE is what model(input_batch, age)
  * computes (the LSTM scans the batch axis, bin/models.py:29-30), B2CNN_MODE_INDEPENDENT treats every window as its own
  * sequence.  All pointers are DEVICE pointers, everything is fp32:
  *   params          the packed blob of b2cnn_weight_count() floats (no affine), updated in place when apply_update != 0
@@ -256,6 +255,27 @@ int b2cnn_train_step(const b2cnn_config *cfg, float *params, float *adam_m, floa
                      const b2cnn_adam *opt, int apply_update, const float *x, int64_t B, const float *age, const float *target,
                      int mode, const float *mask1, const float *mask2, float *loss_out, void *workspace, int64_t workspace_bytes,
                      void *stream);
+/* The same step with the class weight of the reference's training cell (bin/explore_torch.ipynb:3170,3204):
+ * criterion = nn.BCEWithLogitsLoss(pos_weight=pos_weight), pos_weight = num_negatives / num_positives (> 0, finite);
+ * loss_out is mean_b( (1-y) z + (1 + (pos_weight-1) y) (log1p(exp(-|z|)) + max(-z, 0)) ). */
+int b2cnn_train_step_weighted(const b2cnn_config *cfg, float *params, float *adam_m, float *adam_v, float *grads, int64_t step,
+                              const b2cnn_adam *opt, int apply_update, const float *x, int64_t B, const float *age,
+                              const float *target, float pos_weight, int mode, const float *mask1, const float *mask2,
+                              float *loss_out, void *workspace, int64_t workspace_bytes, void *stream);
+
+/* ---- The model in train() mode as a differentiable function, for torch autograd (any loss, any optimizer) ----
+ * Same pointers, modes and masks as b2cnn_train_step; neither call allocates, both are asynchronous on `stream`. */
+/* forward in train() mode; the activations the backward pass needs stay in `workspace`
+ * (b2cnn_train_workspace_bytes(cfg, B) bytes).  z_out[B]: logits (bin/models.py:34). */
+int b2cnn_train_forward(const b2cnn_config *cfg, const float *params, const float *x, int64_t B, const float *age,
+                        int mode, const float *mask1, const float *mask2, float *z_out,
+                        void *workspace, int64_t workspace_bytes, void *stream);
+/* backward from an upstream gradient dz[B] = d loss / d z.  `workspace` must be the one the matching
+ * forward filled, unchanged since.  grads: overwritten (not accumulated), b2cnn_weight_count() floats.
+ * dx [B][C][W] and dage [B] may be NULL (not computed). */
+int b2cnn_train_backward(const b2cnn_config *cfg, const float *params, const float *x, int64_t B, const float *age,
+                         int mode, const float *mask1, const float *mask2, const float *dz, float *grads,
+                         float *dx, float *dage, void *workspace, int64_t workspace_bytes, void *stream);
 
 #ifdef __cplusplus
 }

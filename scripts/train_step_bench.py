@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""ms per training step (row f4) at the reference's training shape [B,10,120]: B200Trainer.step on the GPU, and the same
-loop body (bin/utils.py:200-208: zero_grad, forward in train() mode, BCEWithLogitsLoss, backward, Adam.step) on the
-oracle module with torch on this box's CPU threads.  Prints one JSON line."""
+"""ms per training step (row f4) at the reference's training shape [B,10,120]: B200Trainer.step on the GPU (one fused call),
+the same loop body (bin/utils.py:200-208: zero_grad, forward in train() mode, BCEWithLogitsLoss, backward, Adam.step) on
+B200TrainableMyCNN with torch autograd and torch.optim.Adam on the GPU, and on the oracle module with torch on this box's
+CPU threads.  Prints one JSON line."""
 import json, os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -28,6 +29,18 @@ for B in (32, 256, 2048):
         tr.step(xd, ad, yd)
     ev1.record(); torch.cuda.synchronize()
     gpu_ms = ev0.elapsed_time(ev1) / n
+    am = tskd_b200.B200TrainableMyCNN(arch).to("cuda:0").train()
+    aopt = torch.optim.Adam(am.parameters(), lr=1e-3); crit = nn.BCEWithLogitsLoss()
+    def gpu_body():
+        aopt.zero_grad(); loss = crit(am(xd, ad), yd); loss.backward(); aopt.step()
+    for _ in range(5):
+        gpu_body()
+    torch.cuda.synchronize()
+    ev0.record()
+    for _ in range(n):
+        gpu_body()
+    ev1.record(); torch.cuda.synchronize()
+    autograd_ms = ev0.elapsed_time(ev1) / n
     ref = O.make_ref(O.ARCH_MYCNN5, seed=0); ref.train()
     opt = torch.optim.Adam(ref.parameters(), lr=1e-3); crit = nn.BCEWithLogitsLoss()
     def body():
@@ -39,5 +52,5 @@ for B in (32, 256, 2048):
     for _ in range(k):
         body()
     cpu_ms = (time.perf_counter() - t0) / k * 1e3
-    out[f"B{B}"] = {"gpu_ms_per_step": round(gpu_ms, 4), "cpu_torch_ms_per_step": round(cpu_ms, 3), "cpu_threads": torch.get_num_threads()}
+    out[f"B{B}"] = {"gpu_ms_per_step": round(gpu_ms, 4), "gpu_autograd_adam_ms_per_step": round(autograd_ms, 4), "cpu_torch_ms_per_step": round(cpu_ms, 3), "cpu_threads": torch.get_num_threads()}
 print(json.dumps({"metric": "training step [B,10,120], sequence semantics, dropout 0.1, Adam", "results": out}))

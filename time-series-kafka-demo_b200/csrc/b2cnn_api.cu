@@ -119,22 +119,52 @@ extern "C" int64_t b2cnn_train_workspace_bytes(const b2cnn_config *cfg, int64_t 
     if (n < 0) fail(B2CNN_EINVAL, "b2cnn_train_workspace_bytes: bad configuration / batch");
     return n;
 }
+static int train_step_api(const char *name, const b2cnn_config *cfg, float *params, float *adam_m, float *adam_v, float *grads,
+                          int64_t step, const b2cnn_adam *opt, int apply_update, const float *x, int64_t B, const float *age,
+                          const float *target, int weighted, float pos_weight, int mode, const float *mask1, const float *mask2,
+                          float *loss_out, void *workspace, int64_t workspace_bytes, void *stream) {
+    if (!cfg || !opt) return fail(B2CNN_EINVAL, std::string(name) + ": null configuration");
+    if (mode != B2CNN_MODE_INDEPENDENT && mode != B2CNN_MODE_SEQUENCE) return fail(B2CNN_EINVAL, std::string(name) + ": bad mode");
+    int prev = -1;
+    if (cfg->device >= 0) {
+        if (cudaGetDevice(&prev) != cudaSuccess || cudaSetDevice(cfg->device) != cudaSuccess) return fail(B2CNN_ECUDA, std::string(name) + ": cudaSetDevice");
+    }
+    const char *err = "";
+    const int rc = train_step(cfg, params, adam_m, adam_v, grads, step, opt->lr, opt->beta1, opt->beta2, opt->eps, apply_update, x, B, age,
+                              target, weighted, pos_weight, mode == B2CNN_MODE_SEQUENCE ? 1 : 0, mask1, mask2, loss_out, workspace,
+                              workspace_bytes, reinterpret_cast<cudaStream_t>(stream), &err);
+    if (prev >= 0) cudaSetDevice(prev);
+    return rc == B2CNN_OK ? rc : fail(rc, std::string(name) + ": " + err);
+}
 extern "C" int b2cnn_train_step(const b2cnn_config *cfg, float *params, float *adam_m, float *adam_v, float *grads, int64_t step,
                                 const b2cnn_adam *opt, int apply_update, const float *x, int64_t B, const float *age,
                                 const float *target, int mode, const float *mask1, const float *mask2, float *loss_out,
                                 void *workspace, int64_t workspace_bytes, void *stream) {
-    if (!cfg || !opt) return fail(B2CNN_EINVAL, "b2cnn_train_step: null configuration");
-    if (mode != B2CNN_MODE_INDEPENDENT && mode != B2CNN_MODE_SEQUENCE) return fail(B2CNN_EINVAL, "b2cnn_train_step: bad mode");
-    int prev = -1;
-    if (cfg->device >= 0) {
-        if (cudaGetDevice(&prev) != cudaSuccess || cudaSetDevice(cfg->device) != cudaSuccess) return fail(B2CNN_ECUDA, "b2cnn_train_step: cudaSetDevice");
-    }
+    return train_step_api("b2cnn_train_step", cfg, params, adam_m, adam_v, grads, step, opt, apply_update, x, B, age, target, 0, 1.f, mode,
+                          mask1, mask2, loss_out, workspace, workspace_bytes, stream);
+}
+extern "C" int b2cnn_train_step_weighted(const b2cnn_config *cfg, float *params, float *adam_m, float *adam_v, float *grads, int64_t step,
+                                         const b2cnn_adam *opt, int apply_update, const float *x, int64_t B, const float *age,
+                                         const float *target, float pos_weight, int mode, const float *mask1, const float *mask2,
+                                         float *loss_out, void *workspace, int64_t workspace_bytes, void *stream) {
+    return train_step_api("b2cnn_train_step_weighted", cfg, params, adam_m, adam_v, grads, step, opt, apply_update, x, B, age, target, 1,
+                          pos_weight, mode, mask1, mask2, loss_out, workspace, workspace_bytes, stream);
+}
+extern "C" int b2cnn_train_forward(const b2cnn_config *cfg, const float *params, const float *x, int64_t B, const float *age, int mode,
+                                   const float *mask1, const float *mask2, float *z_out, void *workspace, int64_t workspace_bytes,
+                                   void *stream) {
     const char *err = "";
-    const int rc = train_step(cfg, params, adam_m, adam_v, grads, step, opt->lr, opt->beta1, opt->beta2, opt->eps, apply_update, x, B, age,
-                              target, mode == B2CNN_MODE_SEQUENCE ? 1 : 0, mask1, mask2, loss_out, workspace, workspace_bytes,
-                              reinterpret_cast<cudaStream_t>(stream), &err);
-    if (prev >= 0) cudaSetDevice(prev);
-    return rc == B2CNN_OK ? rc : fail(rc, std::string("b2cnn_train_step: ") + err);
+    const int rc = train_forward(cfg, params, x, B, age, mode, mask1, mask2, z_out, workspace, workspace_bytes,
+                                 reinterpret_cast<cudaStream_t>(stream), &err);
+    return rc == B2CNN_OK ? rc : fail(rc, std::string("b2cnn_train_forward: ") + err);
+}
+extern "C" int b2cnn_train_backward(const b2cnn_config *cfg, const float *params, const float *x, int64_t B, const float *age, int mode,
+                                    const float *mask1, const float *mask2, const float *dz, float *grads, float *dx, float *dage,
+                                    void *workspace, int64_t workspace_bytes, void *stream) {
+    const char *err = "";
+    const int rc = train_backward(cfg, params, x, B, age, mode, mask1, mask2, dz, grads, dx, dage, workspace, workspace_bytes,
+                                  reinterpret_cast<cudaStream_t>(stream), &err);
+    return rc == B2CNN_OK ? rc : fail(rc, std::string("b2cnn_train_backward: ") + err);
 }
 
 // ---- preprocessing + window assembly (b2cnn_prep.cu) ----

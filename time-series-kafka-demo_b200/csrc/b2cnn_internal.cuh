@@ -157,10 +157,17 @@ double wire_parse_decimal_host(const char *s, int64_t len, int *status);
 
 // b2cnn_train.cu: one training step (row f4)
 int64_t train_workspace_bytes(const b2cnn_config *cfg, int64_t B);
+// weighted != 0: BCEWithLogitsLoss(pos_weight=pos_weight), else plain BCEWithLogitsLoss
 int train_step(const b2cnn_config *cfg, float *params, float *adam_m, float *adam_v, float *grads, int64_t step, float lr, float beta1,
-               float beta2, float eps, int apply_update, const float *x, int64_t B, const float *age, const float *target, int sequence,
-               const float *mask1, const float *mask2, float *loss_out, void *workspace, int64_t ws_bytes, cudaStream_t st,
-               const char **err);
+               float beta2, float eps, int apply_update, const float *x, int64_t B, const float *age, const float *target,
+               int weighted, float pos_weight, int sequence, const float *mask1, const float *mask2, float *loss_out, void *workspace,
+               int64_t ws_bytes, cudaStream_t st, const char **err);
+// the autograd seam: mode is B2CNN_MODE_*; both check every argument before any CUDA call and set cfg->device themselves
+int train_forward(const b2cnn_config *cfg, const float *params, const float *x, int64_t B, const float *age, int mode, const float *mask1,
+                  const float *mask2, float *z_out, void *workspace, int64_t ws_bytes, cudaStream_t st, const char **err);
+int train_backward(const b2cnn_config *cfg, const float *params, const float *x, int64_t B, const float *age, int mode,
+                   const float *mask1, const float *mask2, const float *dz, float *grads, float *dx, float *dage, void *workspace,
+                   int64_t ws_bytes, cudaStream_t st, const char **err);
 
 void launch_transpose_wih(const float *wih0, float *wih0T, int L, cudaStream_t st);
 

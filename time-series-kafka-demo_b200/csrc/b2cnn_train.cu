@@ -1,7 +1,8 @@
 // b2cnn_train.cu -- one training step of MyCNN on the device (SURVEY.md section 8, row f4):
 //   optimizer.zero_grad(); output = model(input, age); loss = criterion(output, target); loss.backward(); optimizer.step()
-// (bin/utils.py:200-208 with criterion = nn.BCEWithLogitsLoss(), bin/utils.py:663, and torch.optim.Adam,
-// bin/explore_torch.ipynb:3204-3205) for the layer stack of bin/models.py:22-36 in train() mode:
+// (bin/utils.py:200-208 with criterion = nn.BCEWithLogitsLoss(pos_weight=...), bin/explore_torch.ipynb:3204, optionally
+// without the class weight, and torch.optim.Adam, bin/explore_torch.ipynb:3205) for the layer stack of bin/models.py:22-36 in
+// train() mode:
 //
 //   c1 = conv1(x)            y1 = tanh(c1)   p1 = maxpool(y1)   d1 = dropout(p1)          models.py:23-25
 //   c2 = conv2(d1)           y2 = tanh(c2)   p2 = maxpool(y2)   f  = dropout(p2)          models.py:26-28
@@ -16,9 +17,13 @@
 //   train_lstm_bwd   BPTT over the batch axis: gradients of the head and of every recurrent matrix, d(gates of layer 0)
 //   train_wih0_grad  dW_ih_l0 = d(gates0)^T x f            train_dfeat   d f = d(gates0) x W_ih_l0
 //   train_conv_bwd   per window: dropout / pool (argmax routing, first maximum like ATen) / tanh / conv2 / conv1 backward
+//   train_dx         d x (the input gradient), gather form: one thread per input sample
 //   train_adam       torch.optim.Adam (no amsgrad, weight_decay 0) on the packed parameter blob
+// The head of the two LSTM kernels is a template parameter (Head): the fused step's BCE, BCE with pos_weight, or logits
+// only, with d loss / d z supplied by the caller (b2cnn_train_forward / b2cnn_train_backward, driven by torch autograd).
 // These are launch-latency kernels for the training shape [B,10,120] (44 k MAC per window); they take any geometry the
 // forward path takes (all intermediates live in the caller's workspace), but are not tuned for the stretched windows.
+#include <cfloat>
 #include <cstring>
 
 #include "b2cnn_internal.cuh"
@@ -57,7 +62,7 @@ static BlobOff blob_offsets(const TrainDims &d) {
 
 // workspace layout (floats)
 struct TrainWs {
-    int64_t c1, p1, c2, f, acts, cs, hs, z, da0, dfeat, dc2, dd1, dc1, total;
+    int64_t c1, p1, c2, f, acts, cs, hs, lin, z, da0, dfeat, dc2, dd1, dc1, total;
 };
 static TrainWs train_ws(const TrainDims &d, int64_t B) {
     TrainWs w;
@@ -70,6 +75,7 @@ static TrainWs train_ws(const TrainDims &d, int64_t B) {
     w.acts = take(B * 2 * kGates);      // [t][layer][i f g o] post-activation
     w.cs = take(B * 2 * kHidden);       // [t][layer] cell state
     w.hs = take(B * 2 * kHidden);       // [t][layer] hidden state
+    w.lin = take(B);                    // out(h1) before the age scale (d age needs it)
     w.z = take(B);
     w.da0 = take(B * kGates);           // d loss / d (layer-0 gate pre-activations)
     w.dfeat = take(B * d.L);
@@ -81,6 +87,10 @@ static TrainWs train_ws(const TrainDims &d, int64_t B) {
 }
 
 __device__ __forceinline__ float sigmoidf_(float v) { return 1.0f / (1.0f + expf(-v)); }
+
+// What follows the logits z.  kHeadLogits: no loss in the forward kernel, d loss / d z read from the caller's array in the
+// backward kernel.  kHeadBce: BCEWithLogitsLoss (mean).  kHeadBcePw: BCEWithLogitsLoss(pos_weight=pw) (mean).
+enum Head : int { kHeadLogits = 0, kHeadBce = 1, kHeadBcePw = 2 };
 
 // ------------------------------------------------------------------------------------------------------------------
 // forward, convolutional part: one CTA per window
@@ -130,12 +140,14 @@ train_conv_fwd(const float *__restrict__ x, const float *__restrict__ prm, BlobO
 // ------------------------------------------------------------------------------------------------------------------
 // LSTM forward over the batch axis with everything the backward pass needs kept; logits and loss.
 // One CTA of 64 threads: thread r owns gate row r of every matrix.  sequence == 0: every step starts from the zero state
-// (independent windows).
+// (independent windows).  HEAD == kHeadLogits: target and loss_out are not used.
 // ------------------------------------------------------------------------------------------------------------------
+template <int HEAD>
 __global__ void __launch_bounds__(64)
 train_lstm_fwd(const float *__restrict__ f, const float *__restrict__ prm, BlobOff o, TrainDims d, int64_t B, int sequence,
-               const float *__restrict__ age, const float *__restrict__ target, float *__restrict__ acts, float *__restrict__ cs,
-               float *__restrict__ hs, float *__restrict__ z, float *__restrict__ loss_out) {
+               const float *__restrict__ age, const float *__restrict__ target, float pos_weight, float *__restrict__ acts,
+               float *__restrict__ cs, float *__restrict__ hs, float *__restrict__ lin, float *__restrict__ z,
+               float *__restrict__ loss_out) {
     __shared__ float g[kGates], h0[kHidden], c0[kHidden], h1[kHidden], c1s[kHidden];
     const int r = threadIdx.x;
     if (r < kHidden) { h0[r] = c0[r] = h1[r] = c1s[r] = 0.f; }
@@ -197,26 +209,36 @@ train_lstm_fwd(const float *__restrict__ f, const float *__restrict__ prm, BlobO
             float y = 0.f;
             for (int k = 0; k < kHidden; ++k) y = fmaf(prm[o.wo + k], h1[k], y);
             y += prm[o.bo];
+            lin[t] = y;
             float s = __fadd_rn(__fmul_rn(age[t], d.age_coef), 1.0f);
             s = (s > 0.f || s != s) ? s : 0.f;
             y *= s;
             z[t] = y;
-            const float yt = target[t];
-            loss += fmaxf(y, 0.f) - y * yt + log1pf(expf(-fabsf(y)));   // BCEWithLogitsLoss, the stable form ATen uses
+            if constexpr (HEAD == kHeadBce) {
+                const float yt = target[t];
+                loss += fmaxf(y, 0.f) - y * yt + log1pf(expf(-fabsf(y)));   // BCEWithLogitsLoss, the stable form ATen uses
+            } else if constexpr (HEAD == kHeadBcePw) {
+                const float yt = target[t], lw = 1.f + (pos_weight - 1.f) * yt;
+                loss += (1.f - yt) * y + lw * (log1pf(expf(-fabsf(y))) + fmaxf(-y, 0.f));   // ATen's pos_weight form
+            }
         }
         __syncthreads();
     }
-    if (r == 0) *loss_out = loss / (float)B;
+    if (HEAD != kHeadLogits && r == 0) *loss_out = loss / (float)B;
 }
 
 // ------------------------------------------------------------------------------------------------------------------
 // BPTT over the batch axis.  64 threads: thread r owns gate row r.  Gradients of the recurrent matrices, biases and of
 // the head are accumulated in registers / shared memory and written once; d(gates of layer 0) goes to da0[t][64].
+// HEAD == kHeadLogits: d loss / d z is dz_in[t] and, when dage != NULL, d loss / d age goes to dage[t] (torch's relu
+// backward: zero where relu(age * coef + 1) is not positive); otherwise dz comes from z and target, dage is not written.
 // ------------------------------------------------------------------------------------------------------------------
+template <int HEAD>
 __global__ void __launch_bounds__(64)
 train_lstm_bwd(const float *__restrict__ prm, BlobOff o, TrainDims d, int64_t B, int sequence, const float *__restrict__ age,
-               const float *__restrict__ target, const float *__restrict__ acts, const float *__restrict__ cs,
-               const float *__restrict__ hs, const float *__restrict__ z, float *__restrict__ da0, float *__restrict__ grad) {
+               const float *__restrict__ target, float pos_weight, const float *__restrict__ dz_in, const float *__restrict__ acts,
+               const float *__restrict__ cs, const float *__restrict__ hs, const float *__restrict__ lin, const float *__restrict__ z,
+               float *__restrict__ da0, float *__restrict__ grad, float *__restrict__ dage) {
     __shared__ float da[kGates], dh0c[kHidden], dc0c[kHidden], dh1c[kHidden], dc1c[kHidden], dh0ext[kHidden], dh1ext[kHidden];
     const int r = threadIdx.x, u = r & 15, q = r >> 4;
     float gWhh0[kHidden], gWih1[kHidden], gWhh1[kHidden];
@@ -234,7 +256,16 @@ train_lstm_bwd(const float *__restrict__ prm, BlobOff o, TrainDims d, int64_t B,
         // ---- head: z = (wo . h1 + bo) * s
         float s = __fadd_rn(__fmul_rn(age[t], d.age_coef), 1.0f);
         s = (s > 0.f || s != s) ? s : 0.f;
-        const float dz = (sigmoidf_(z[t]) - target[t]) / (float)B;
+        float dz;
+        if constexpr (HEAD == kHeadBce) {
+            dz = (sigmoidf_(z[t]) - target[t]) / (float)B;
+        } else if constexpr (HEAD == kHeadBcePw) {
+            const float yt = target[t], lw = 1.f + (pos_weight - 1.f) * yt;
+            dz = ((1.f - yt) - lw * sigmoidf_(-z[t])) / (float)B;
+        } else {
+            dz = dz_in[t];
+            if (dage && r == 0) dage[t] = s > 0.f ? dz * lin[t] * d.age_coef : 0.f;
+        }
         const float dlin = dz * s;
         if (r < kHidden) {
             gwo += dlin * hs[(t * 2 + 1) * kHidden + r];
@@ -436,6 +467,24 @@ train_conv_bwd(const float *__restrict__ x, const float *__restrict__ prm, BlobO
     }
 }
 
+// d x[b][c][t] = sum_oc sum_k w1[oc][c][k] * dc1[b][oc][t-k] over the valid t-k in [0, L1): conv1's input gradient in
+// gather form, one thread per input sample (no atomics)
+__global__ void train_dx(const float *__restrict__ dc1, const float *__restrict__ prm, BlobOff o, TrainDims d, int64_t B,
+                         float *__restrict__ dx) {
+    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= B * d.C * d.W) return;
+    const int t = (int)(e % d.W), c = (int)((e / d.W) % d.C);
+    const int64_t b = e / ((int64_t)d.C * d.W);
+    const int k_lo = max(0, t - (d.L1 - 1)), k_hi = min(d.K1 - 1, t);
+    float a = 0.f;
+    for (int oc = 0; oc < kCMid; ++oc) {
+        const float *wr = prm + o.w1 + ((int64_t)oc * d.C + c) * d.K1;
+        const float *dr = dc1 + (b * kCMid + oc) * d.L1 + t;
+        for (int k = k_lo; k <= k_hi; ++k) a = fmaf(wr[k], dr[-k], a);
+    }
+    dx[e] = a;
+}
+
 // torch.optim.Adam, single-tensor form: exp_avg.lerp_(grad, 1-b1); exp_avg_sq = b2*v + (1-b2) g^2;
 // denom = sqrt(v) / sqrt(1 - b2^t) + eps; param -= (lr / (1 - b1^t)) * m / denom
 __global__ void train_adam(float *__restrict__ prm, float *__restrict__ m, float *__restrict__ v, const float *__restrict__ grad, int64_t n,
@@ -472,33 +521,116 @@ int64_t train_workspace_bytes(const b2cnn_config *cfg, int64_t B) {
     return train_ws(d, B).total * (int64_t)sizeof(float);
 }
 
+// Sets cfg->device current for the launches of one call (when it is >= 0) and restores the caller's device afterwards.
+struct DeviceScope {
+    int prev = -1;
+    bool ok = true;
+    explicit DeviceScope(int device) {
+        if (device >= 0) ok = cudaGetDevice(&prev) == cudaSuccess && cudaSetDevice(device) == cudaSuccess;
+    }
+    ~DeviceScope() {
+        if (prev >= 0) cudaSetDevice(prev);
+    }
+};
+
+// everything after d(head): d W_ih_l0, d f, the convolutional backward into `grads` (zeroed by the caller: conv weight
+// gradients are added atomically) and, when dx != NULL, the input gradient
+static void launch_backward_tail(const TrainDims &d, const BlobOff &o, const TrainWs &w, float *ws, const float *params,
+                                 const float *x, int64_t B, const float *mask1, const float *mask2, float *grads, float *dx,
+                                 cudaStream_t st) {
+    const int64_t n1 = (int64_t)kGates * d.L, n2 = B * d.L;
+    train_wih0_grad<<<(unsigned)((n1 + 255) / 256), 256, 0, st>>>(ws + w.da0, ws + w.f, B, d.L, grads + o.wih0);
+    train_dfeat<<<(unsigned)((n2 + 255) / 256), 256, 0, st>>>(ws + w.da0, params + o.wih0, B, d.L, ws + w.dfeat);
+    train_conv_bwd<<<(unsigned)B, 256, 0, st>>>(x, params, o, d, mask1, mask2, ws + w.c1, ws + w.p1, ws + w.c2, ws + w.dfeat, ws + w.dc2,
+                                               ws + w.dd1, ws + w.dc1, grads);
+    if (dx) {
+        const int64_t n = B * d.C * d.W;
+        train_dx<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(ws + w.dc1, params, o, d, B, dx);
+    }
+}
+
 int train_step(const b2cnn_config *cfg, float *params, float *adam_m, float *adam_v, float *grads, int64_t step, float lr, float beta1,
-               float beta2, float eps, int apply_update, const float *x, int64_t B, const float *age, const float *target, int sequence,
-               const float *mask1, const float *mask2, float *loss_out, void *workspace, int64_t ws_bytes, cudaStream_t st,
-               const char **err) {
+               float beta2, float eps, int apply_update, const float *x, int64_t B, const float *age, const float *target,
+               int weighted, float pos_weight, int sequence, const float *mask1, const float *mask2, float *loss_out, void *workspace,
+               int64_t ws_bytes, cudaStream_t st, const char **err) {
     TrainDims d;
     if (!cfg || !train_dims(*cfg, d, err)) return B2CNN_EINVAL;
     if (!params || !grads || !x || !age || !target || !loss_out || !workspace || B < 1 || step < 1) { *err = "training: null argument / bad step"; return B2CNN_EINVAL; }
     if (apply_update && (!adam_m || !adam_v)) { *err = "training: Adam state missing"; return B2CNN_EINVAL; }
+    if (weighted && !(pos_weight > 0.f && pos_weight <= FLT_MAX)) { *err = "training: pos_weight must be positive and finite"; return B2CNN_EINVAL; }
     const TrainWs w = train_ws(d, B);
     if (ws_bytes < w.total * (int64_t)sizeof(float)) { *err = "training: workspace smaller than b2cnn_train_workspace_bytes()"; return B2CNN_ESTATE; }
     const BlobOff o = blob_offsets(d);
     float *ws = reinterpret_cast<float *>(workspace);
     if (cudaMemsetAsync(grads, 0, sizeof(float) * o.total, st) != cudaSuccess) { *err = "memset grads"; return B2CNN_ECUDA; }
     train_conv_fwd<<<(unsigned)B, 256, 0, st>>>(x, params, o, d, mask1, mask2, ws + w.c1, ws + w.p1, ws + w.c2, ws + w.f);
-    train_lstm_fwd<<<1, 64, 0, st>>>(ws + w.f, params, o, d, B, sequence, age, target, ws + w.acts, ws + w.cs, ws + w.hs, ws + w.z, loss_out);
-    train_lstm_bwd<<<1, 64, 0, st>>>(params, o, d, B, sequence, age, target, ws + w.acts, ws + w.cs, ws + w.hs, ws + w.z, ws + w.da0, grads);
-    {
-        const int64_t n1 = (int64_t)kGates * d.L, n2 = B * d.L;
-        train_wih0_grad<<<(unsigned)((n1 + 255) / 256), 256, 0, st>>>(ws + w.da0, ws + w.f, B, d.L, grads + o.wih0);
-        train_dfeat<<<(unsigned)((n2 + 255) / 256), 256, 0, st>>>(ws + w.da0, params + o.wih0, B, d.L, ws + w.dfeat);
+    if (weighted) {
+        train_lstm_fwd<kHeadBcePw><<<1, 64, 0, st>>>(ws + w.f, params, o, d, B, sequence, age, target, pos_weight, ws + w.acts, ws + w.cs,
+                                                     ws + w.hs, ws + w.lin, ws + w.z, loss_out);
+        train_lstm_bwd<kHeadBcePw><<<1, 64, 0, st>>>(params, o, d, B, sequence, age, target, pos_weight, nullptr, ws + w.acts, ws + w.cs,
+                                                     ws + w.hs, ws + w.lin, ws + w.z, ws + w.da0, grads, nullptr);
+    } else {
+        train_lstm_fwd<kHeadBce><<<1, 64, 0, st>>>(ws + w.f, params, o, d, B, sequence, age, target, 1.f, ws + w.acts, ws + w.cs,
+                                                   ws + w.hs, ws + w.lin, ws + w.z, loss_out);
+        train_lstm_bwd<kHeadBce><<<1, 64, 0, st>>>(params, o, d, B, sequence, age, target, 1.f, nullptr, ws + w.acts, ws + w.cs,
+                                                   ws + w.hs, ws + w.lin, ws + w.z, ws + w.da0, grads, nullptr);
     }
-    train_conv_bwd<<<(unsigned)B, 256, 0, st>>>(x, params, o, d, mask1, mask2, ws + w.c1, ws + w.p1, ws + w.c2, ws + w.dfeat, ws + w.dc2,
-                                               ws + w.dd1, ws + w.dc1, grads);
+    launch_backward_tail(d, o, w, ws, params, x, B, mask1, mask2, grads, nullptr, st);
     if (apply_update) {
         const float bc1 = 1.f - powf(beta1, (float)step), bc2 = 1.f - powf(beta2, (float)step);
         train_adam<<<(unsigned)((o.total + 255) / 256), 256, 0, st>>>(params, adam_m, adam_v, grads, o.total, lr, beta1, beta2, eps, bc1, sqrtf(bc2));
     }
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) { *err = cudaGetErrorString(e); return B2CNN_ECUDA; }
+    return B2CNN_OK;
+}
+
+// the checks b2cnn_train_forward and b2cnn_train_backward share; no CUDA call
+static int autograd_args(const b2cnn_config *cfg, int64_t B, int mode, int64_t ws_bytes, bool ptrs_ok, TrainDims &d, TrainWs &w,
+                         const char **err) {
+    if (!cfg || !train_dims(*cfg, d, err)) return B2CNN_EINVAL;
+    if (mode != B2CNN_MODE_INDEPENDENT && mode != B2CNN_MODE_SEQUENCE) { *err = "training: bad mode"; return B2CNN_EINVAL; }
+    if (!ptrs_ok || B < 1) { *err = "training: null argument / bad batch"; return B2CNN_EINVAL; }
+    w = train_ws(d, B);
+    if (ws_bytes < w.total * (int64_t)sizeof(float)) { *err = "training: workspace smaller than b2cnn_train_workspace_bytes()"; return B2CNN_ESTATE; }
+    return B2CNN_OK;
+}
+
+int train_forward(const b2cnn_config *cfg, const float *params, const float *x, int64_t B, const float *age, int mode, const float *mask1,
+                  const float *mask2, float *z_out, void *workspace, int64_t ws_bytes, cudaStream_t st, const char **err) {
+    TrainDims d;
+    TrainWs w;
+    const int rc = autograd_args(cfg, B, mode, ws_bytes, params && x && age && z_out && workspace, d, w, err);
+    if (rc != B2CNN_OK) return rc;
+    DeviceScope dev(cfg->device);
+    if (!dev.ok) { *err = "cudaSetDevice"; return B2CNN_ECUDA; }
+    const BlobOff o = blob_offsets(d);
+    const int sequence = mode == B2CNN_MODE_SEQUENCE ? 1 : 0;
+    float *ws = reinterpret_cast<float *>(workspace);
+    train_conv_fwd<<<(unsigned)B, 256, 0, st>>>(x, params, o, d, mask1, mask2, ws + w.c1, ws + w.p1, ws + w.c2, ws + w.f);
+    train_lstm_fwd<kHeadLogits><<<1, 64, 0, st>>>(ws + w.f, params, o, d, B, sequence, age, nullptr, 1.f, ws + w.acts, ws + w.cs,
+                                                  ws + w.hs, ws + w.lin, z_out, nullptr);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) { *err = cudaGetErrorString(e); return B2CNN_ECUDA; }
+    return B2CNN_OK;
+}
+
+int train_backward(const b2cnn_config *cfg, const float *params, const float *x, int64_t B, const float *age, int mode,
+                   const float *mask1, const float *mask2, const float *dz, float *grads, float *dx, float *dage, void *workspace,
+                   int64_t ws_bytes, cudaStream_t st, const char **err) {
+    TrainDims d;
+    TrainWs w;
+    const int rc = autograd_args(cfg, B, mode, ws_bytes, params && x && age && dz && grads && workspace, d, w, err);
+    if (rc != B2CNN_OK) return rc;
+    DeviceScope dev(cfg->device);
+    if (!dev.ok) { *err = "cudaSetDevice"; return B2CNN_ECUDA; }
+    const BlobOff o = blob_offsets(d);
+    const int sequence = mode == B2CNN_MODE_SEQUENCE ? 1 : 0;
+    float *ws = reinterpret_cast<float *>(workspace);
+    if (cudaMemsetAsync(grads, 0, sizeof(float) * o.total, st) != cudaSuccess) { *err = "memset grads"; return B2CNN_ECUDA; }
+    train_lstm_bwd<kHeadLogits><<<1, 64, 0, st>>>(params, o, d, B, sequence, age, nullptr, 1.f, dz, ws + w.acts, ws + w.cs, ws + w.hs,
+                                                  ws + w.lin, nullptr, ws + w.da0, grads, dage);
+    launch_backward_tail(d, o, w, ws, params, x, B, mask1, mask2, grads, dx, st);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) { *err = cudaGetErrorString(e); return B2CNN_ECUDA; }
     return B2CNN_OK;

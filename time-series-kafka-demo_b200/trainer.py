@@ -5,12 +5,13 @@ The reference trains with ``utils.train`` (bin/utils.py:183-227): per batch
     optimizer.zero_grad(); output = model(input, age); loss = criterion(output, target)
     loss.backward(); optimizer.step()
 
-with ``criterion = nn.BCEWithLogitsLoss()`` (bin/utils.py:663) and ``torch.optim.Adam``
-(bin/explore_torch.ipynb:3204-3205).  :class:`B200Trainer` is that loop body as ONE C-ABI call
-(``b2cnn_train_step``, csrc/b2cnn_train.cu: hand-written forward-with-saved-activations, BPTT over the
-batch axis, pooling/conv backward, Adam) on a :class:`B200MyCNN`'s parameters::
+with ``criterion = nn.BCEWithLogitsLoss(pos_weight=pos_weight)``, ``pos_weight = num_negatives / num_positives``,
+and ``torch.optim.Adam`` (bin/explore_torch.ipynb:3170,3204-3205).  :class:`B200Trainer` is that loop body as ONE
+C-ABI call (``b2cnn_train_step``, or ``b2cnn_train_step_weighted`` when ``pos_weight`` is given; csrc/b2cnn_train.cu:
+hand-written forward-with-saved-activations, BPTT over the batch axis, pooling/conv backward, Adam) on a
+:class:`B200MyCNN`'s parameters::
 
-    trainer = B200Trainer(model, lr=1e-3)
+    trainer = B200Trainer(model, lr=1e-5, pos_weight=13.5)
     for x, age, y in loader:                       # x [B,10,120], age [B], y [B] in {0,1}
         loss = trainer.step(x, age, y)             # == the five reference lines above
     model.predict(...)                             # scores with the updated weights
@@ -19,10 +20,13 @@ batch axis, pooling/conv backward, Adam) on a :class:`B200MyCNN`'s parameters::
 the batch axis (bin/models.py:29-30).  Dropout (bin/models.py:15, p = 0.1) uses masks drawn by torch on the
 device; torch's own Philox stream cannot be reproduced by another implementation, so parity tests pass the
 same explicit masks to both sides.
+
+Any other loss or optimizer: :class:`~tskd_b200.autograd.B200TrainableMyCNN` runs the same kernels under torch autograd.
 """
 from __future__ import annotations
 
 import ctypes
+import math
 from typing import Dict, Optional, Tuple
 
 import torch
@@ -34,17 +38,23 @@ from .model import B200MyCNN
 
 class B200Trainer:
     def __init__(self, model: B200MyCNN, lr: float = 1e-3, betas: Tuple[float, float] = (0.9, 0.999), eps: float = 1e-8,
-                 mode: str = "sequence", dropout: float = 0.1, seed: int = 0):
+                 mode: str = "sequence", dropout: float = 0.1, seed: int = 0, pos_weight: Optional[float] = None):
+        """``pos_weight``: the class weight of ``nn.BCEWithLogitsLoss(pos_weight=...)`` (a positive number; None = the
+        unweighted loss)."""
         if model.arch.affine or model.arch.act_id != 0:
             raise NotImplementedError("training covers the reference's tanh stack (bin/models.py:23,26) without the affine variant")
         if mode not in ("sequence", "independent"):
             raise ValueError("mode must be 'sequence' or 'independent'")
         if not 0.0 <= float(dropout) < 1.0:
             raise ValueError("dropout must be in [0, 1)")
+        if pos_weight is not None:
+            pos_weight = float(pos_weight)
+            if not (math.isfinite(pos_weight) and pos_weight > 0.0):
+                raise ValueError("pos_weight must be a positive finite number")
         dev = model._device()
         if dev.type != "cuda":
             raise RuntimeError("B200Trainer needs the model on a CUDA device (there is no CPU fallback)")
-        self.model, self.mode, self.dropout = model, mode, float(dropout)
+        self.model, self.mode, self.dropout, self.pos_weight = model, mode, float(dropout), pos_weight
         self._lib = capi.load_library()
         self._cfg = capi.make_config(model.arch, dev.index if dev.index is not None else torch.cuda.current_device())
         self._opt = capi.Adam(lr, betas[0], betas[1], eps)
@@ -85,7 +95,8 @@ class B200Trainer:
 
     def step(self, x: torch.Tensor, age: torch.Tensor, target: torch.Tensor,
              masks: Optional[Tuple[Optional[torch.Tensor], Optional[torch.Tensor]]] = None, update: bool = True) -> torch.Tensor:
-        """zero_grad + forward + BCEWithLogitsLoss + backward + Adam step; returns the batch loss (a 0-d device tensor)."""
+        """zero_grad + forward + BCEWithLogitsLoss(pos_weight) + backward + Adam step; returns the batch loss (a 0-d device
+        tensor)."""
         dev = self._params.device
         a = self.model.arch
         if x.dim() != 3 or x.shape[1] != a.in_channels or x.shape[2] != a.window:
@@ -112,11 +123,14 @@ class B200Trainer:
             self._ws = torch.empty(need, dtype=torch.uint8, device=dev)
         ptr = lambda t: ctypes.c_void_p(t.data_ptr()) if t is not None else None
         st = torch.cuda.current_stream(dev).cuda_stream
-        rc = self._lib.b2cnn_train_step(ctypes.byref(self._cfg), ptr(self._params), ptr(self._m), ptr(self._v), ptr(self._grads),
-                                        self.steps + 1, ctypes.byref(self._opt), 1 if update else 0, ptr(x), B, ptr(age), ptr(target),
-                                        capi.MODE_SEQUENCE if self.mode == "sequence" else capi.MODE_INDEPENDENT, ptr(m1), ptr(m2),
-                                        ptr(self._loss), ptr(self._ws), need, ctypes.c_void_p(st))
-        capi.check(rc, "b2cnn_train_step")
+        head = (ctypes.byref(self._cfg), ptr(self._params), ptr(self._m), ptr(self._v), ptr(self._grads), self.steps + 1,
+                ctypes.byref(self._opt), 1 if update else 0, ptr(x), B, ptr(age), ptr(target))
+        tail = (capi.MODE_SEQUENCE if self.mode == "sequence" else capi.MODE_INDEPENDENT, ptr(m1), ptr(m2), ptr(self._loss),
+                ptr(self._ws), need, ctypes.c_void_p(st))
+        if self.pos_weight is None:
+            capi.check(self._lib.b2cnn_train_step(*head, *tail), "b2cnn_train_step")
+        else:
+            capi.check(self._lib.b2cnn_train_step_weighted(*head, self.pos_weight, *tail), "b2cnn_train_step_weighted")
         if update:
             self.steps += 1
             with torch.no_grad():                        # the inference kernels read the module's parameters
