@@ -1,6 +1,6 @@
 """GPU: the model in train() mode under torch autograd (b2cnn_train_forward / b2cnn_train_backward) and the fused step with
 pos_weight, against the oracle module (oracle/mycnn_torch.py) in train() mode with the same explicit dropout masks, the
-way test_gpu_train.py checks the fused step.  The reference's training cell (bin/explore_torch.ipynb:3140-3240) is
+way test_gpu_train.py checks the fused step: per element against that graph in float64 (oracle/train_ref.py).  The reference's training cell (bin/explore_torch.ipynb:3140-3240) is
 nn.BCEWithLogitsLoss(pos_weight=13.5) with optim.Adam(lr=1e-5), optim.Adagrad commented out beside it."""
 from dataclasses import replace
 
@@ -13,7 +13,9 @@ import tskd_b200
 from tskd_b200.arch import BLOB_KEYS, INERT_KEYS
 from tskd_b200.trainer import B200Trainer
 from oracle import mycnn_torch as O
-from test_gpu_train import MaskDropout, _batch, _relerr
+from oracle.train_ref import MaskDropout, assert_close_elem, train_reference
+from conftest import rel_err
+from test_gpu_train import _batch
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -41,30 +43,29 @@ def _logits(m, x, age, mode, m1, m2):
     return tskd_b200.mycnn_train_forward(x, age, [named[k] for k in BLOB_KEYS], m.arch, mode, _dev(m1), _dev(m2))
 
 
-def _ref_logits(ref, x, age, mode, m1, m2):
-    if mode == "sequence":
-        ref.dropout.set(m1, m2)
-        return ref(x, age)
-    outs = []                                      # every window its own sequence
-    for i in range(x.shape[0]):
-        ref.dropout.set(None if m1 is None else m1[i:i + 1], None if m2 is None else m2[i:i + 1])
-        outs.append(ref(x[i:i + 1], age[i:i + 1]))
-    return torch.cat(outs)
-
-
 def _assert_loss_close(got, want, rel, step=None):
     got, want = float(got.detach()), float(want.detach())
     assert abs(got - want) <= rel * max(1.0, abs(want)), (step, got, want)
 
 
-def _check_grads(m, ref, tol=2e-4):
-    got, want = dict(m.named_parameters()), dict(ref.named_parameters())
+def _refs(ref, x, age, mode, m1, m2, **heads):
+    """the float64 truth and the float32 yardstick (oracle/train_ref.py)"""
+    return (train_reference(ref, x, age, mode, m1, m2, **heads),
+            train_reference(ref, x, age, mode, m1, m2, dtype=torch.float32, **heads))
+
+
+def _check_grads(got, truth, ref32):
+    """got: the 14 BLOB_KEYS gradients; truth / ref32: one head of train_reference"""
     for k in BLOB_KEYS:
-        e = _relerr(got[k].grad.cpu().numpy(), want[k].grad.numpy())
-        assert e <= tol, (k, e)
+        assert_close_elem(k, got[k], truth["grads"][k], ref32["grads"][k])
+
+
+def _check_module_grads(m, truth, ref32):
+    named = dict(m.named_parameters())
+    _check_grads({k: named[k].grad for k in BLOB_KEYS}, truth, ref32)
     for k in INERT_KEYS:
-        if k in got:
-            assert got[k].grad is None, k
+        if k in named:
+            assert named[k].grad is None, k
 
 
 @pytest.mark.parametrize("kind,C,W,B,mode,p", [
@@ -80,39 +81,31 @@ def test_logits_and_gradients_match_autograd(kind, C, W, B, mode, p):
     xd, ad = x.to(DEV).requires_grad_(), age.to(DEV).requires_grad_()
     z = _logits(m, xd, ad, mode, m1, m2)
     (z * r.to(DEV)).sum().backward()
-    xr, ar = x.clone().requires_grad_(), age.clone().requires_grad_()
-    zr = _ref_logits(ref, xr, ar, mode, m1, m2)
-    (zr * r).sum().backward()
-    e = _relerr(z.detach().cpu().numpy(), zr.detach().numpy())
-    assert e <= 1e-5, ("logits", e)
-    _check_grads(m, ref)
-    for name, got, want in (("x", xd.grad, xr.grad), ("age", ad.grad, ar.grad)):
-        e = _relerr(got.cpu().numpy(), want.numpy())
-        assert e <= 2e-4, (name, e)
+    truth, ref32 = _refs(ref, x, age, mode, m1, m2, dz=r)
+    assert_close_elem("z", z, truth["z"], ref32["z"])
+    _check_module_grads(m, truth["dz"], ref32["dz"])
+    assert_close_elem("dx", xd.grad, truth["dz"]["dx"], ref32["dz"]["dx"])
+    assert_close_elem("dage", ad.grad, truth["dz"]["dage"], ref32["dz"]["dage"])
 
 
 def test_pos_weight_loss_through_autograd_and_the_fused_step():
     oarch, ref, m = _pair("mycnn5", 10, 120)
     x, age, _, m1, m2 = _batch(oarch, 32, seed=21, p=0.1)
     y = (torch.rand(32, generator=torch.Generator().manual_seed(4)) < 0.2).float()     # imbalanced, hence the class weight
-    ref.dropout.set(m1, m2)
-    want = nn.BCEWithLogitsLoss(pos_weight=torch.tensor(POS_WEIGHT))(ref(x, age), y)
-    want.backward()
+    truth, ref32 = _refs(ref, x, age, "sequence", m1, m2, target=y, pos_weight=POS_WEIGHT)
+    truth, ref32 = truth["bce_pw"], ref32["bce_pw"]
     loss = nn.BCEWithLogitsLoss(pos_weight=torch.tensor(POS_WEIGHT, device=DEV))(
         _logits(m, x.to(DEV), age.to(DEV), "sequence", m1, m2), y.to(DEV))
     loss.backward()
-    _assert_loss_close(loss, want, 1e-5)
-    _check_grads(m, ref)
+    assert_close_elem("loss", loss.reshape(1), truth["loss"].reshape(1), ref32["loss"].reshape(1))
+    _check_module_grads(m, truth, ref32)
 
     plain = tskd_b200.B200MyCNN(m.arch).to(DEV)
     plain.load_state_dict(m.state_dict())
     tr = B200Trainer(plain, dropout=0.1, pos_weight=POS_WEIGHT)
     fused = tr.step(x, age, y, masks=(m1, m2), update=False)
-    _assert_loss_close(fused, want, 1e-5)
-    got, named = tr.grads(), dict(ref.named_parameters())
-    for k in BLOB_KEYS:
-        e = _relerr(got[k].cpu().numpy(), named[k].grad.numpy())
-        assert e <= 2e-4, (k, e)
+    assert_close_elem("fused loss", fused.reshape(1), truth["loss"].reshape(1), ref32["loss"].reshape(1))
+    _check_grads(tr.grads(), truth, ref32)
 
 
 def _check_params_after_steps(sd, ref, lr):
@@ -136,7 +129,7 @@ def _check_eval_scores(m, ref, oarch):
     with torch.no_grad():
         want = ref(xs, ages).numpy()
     got = m(xs.to(DEV), ages.to(DEV)).cpu().numpy()
-    assert _relerr(got, want) <= 1e-4
+    assert rel_err(got, want) <= 1e-4
 
 
 @pytest.mark.parametrize("optim,lr", [(torch.optim.Adam, 1e-5), (torch.optim.Adagrad, 5e-3)])
@@ -195,11 +188,9 @@ def test_module_forward_in_train_mode():
     m.dropout.p = 0.0
     z = m(x.to(DEV), age[:1].to(DEV))                                  # one age for the batch, broadcast like the reference
     nn.BCEWithLogitsLoss()(z, y.to(DEV)).backward()
-    ref.dropout.set(None, None)
-    want_z = ref(x, age[:1])
-    nn.BCEWithLogitsLoss()(want_z, y).backward()
-    assert _relerr(z.detach().cpu().numpy(), want_z.detach().numpy()) <= 1e-5
-    _check_grads(m, ref)
+    truth, ref32 = _refs(ref, x, age[:1], "sequence", None, None, target=y)
+    assert_close_elem("z", z, truth["z"], ref32["z"])
+    _check_module_grads(m, truth["bce"], ref32["bce"])
 
     m.dropout.p = 0.1
     xb = x.to(DEV, torch.bfloat16).requires_grad_()

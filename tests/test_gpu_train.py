@@ -4,7 +4,8 @@ The oracle (oracle/mycnn_torch.py, the layer stack of bin/models.py:5-36) runs t
 (bin/utils.py:200-208) on the CPU: zero_grad, model(input, age) in train() mode, nn.BCEWithLogitsLoss (bin/utils.py:663),
 backward, torch.optim.Adam.step (bin/explore_torch.ipynb:3204-3205).  Dropout masks are explicit on both sides (torch's
 Philox stream cannot be shared): the oracle's nn.Dropout is swapped for a module that multiplies by the same masks, in
-call order, so its own forward() is what gets differentiated."""
+call order, so its own forward() is what gets differentiated.  The loss and the gradients of one step are compared element by
+element with that graph in float64 (oracle/train_ref.py: train_reference, assert_close_elem)."""
 from dataclasses import replace
 
 import numpy as np
@@ -15,23 +16,11 @@ from torch import nn
 import tskd_b200
 from tskd_b200.trainer import B200Trainer
 from oracle import mycnn_torch as O
+from oracle.train_ref import MaskDropout, assert_close_elem, train_reference
+from conftest import rel_err
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
-
-
-class MaskDropout(nn.Module):
-    def __init__(self):
-        super().__init__()
-        self.masks, self.i = [], 0
-
-    def set(self, m1, m2):
-        self.masks, self.i = [m1, None if m2 is None else m2.unsqueeze(1)], 0
-
-    def forward(self, x):
-        m = self.masks[self.i]
-        self.i += 1
-        return x if m is None else x * m
 
 
 def _pair(kind, C, W, seed=0):
@@ -58,11 +47,6 @@ def _batch(oarch, B, seed, p):
     return x, age, y, m1, m2
 
 
-def _relerr(a, b):
-    a, b = np.asarray(a, np.float64), np.asarray(b, np.float64)
-    return float(np.abs(a - b).max() / max(np.abs(b).max(), 1e-12))
-
-
 @pytest.mark.parametrize("kind,C,W,B,mode,p", [
     ("mycnn5", 10, 120, 32, "sequence", 0.1),        # the reference's training shape and semantics
     ("mycnn5", 10, 120, 7, "sequence", 0.0),
@@ -75,24 +59,12 @@ def test_gradients_and_loss_match_autograd(kind, C, W, B, mode, p):
     x, age, y, m1, m2 = _batch(oarch, B, seed=5, p=p)
     tr = B200Trainer(m, mode=mode, dropout=p)
     loss = tr.step(x, age, y, masks=(m1, m2), update=False)
-    ref.dropout.set(m1, m2)
-    if mode == "sequence":
-        z = ref(x, age)
-    else:                                            # every window its own sequence
-        outs = []
-        for i in range(B):
-            ref.dropout.set(None if m1 is None else m1[i:i + 1], None if m2 is None else m2[i:i + 1])
-            outs.append(ref(x[i:i + 1], age[i:i + 1]))
-        z = torch.cat(outs)
-    want = nn.BCEWithLogitsLoss()(z, y)
-    ref.zero_grad()
-    want.backward()
-    assert abs(float(loss) - float(want.detach())) <= 1e-5 * max(1.0, abs(float(want))), (float(loss), float(want.detach()))
+    truth = train_reference(ref, x, age, mode, m1, m2, target=y)["bce"]
+    ref32 = train_reference(ref, x, age, mode, m1, m2, target=y, dtype=torch.float32)["bce"]
+    assert_close_elem("loss", loss.cpu().reshape(1), truth["loss"].reshape(1), ref32["loss"].reshape(1))
     got = tr.grads()
-    named = dict(ref.named_parameters())
     for k in tskd_b200.arch.BLOB_KEYS:
-        e = _relerr(got[k].cpu().numpy(), named[k].grad.numpy())
-        assert e <= 2e-4, (k, e)
+        assert_close_elem(k, got[k], truth["grads"][k], ref32["grads"][k])
 
 
 def test_three_adam_steps_follow_torch_optim():
@@ -124,7 +96,7 @@ def test_three_adam_steps_follow_torch_optim():
     with torch.no_grad():
         want = ref(xs, ages).numpy()
     got = m(xs.to(DEV), ages.to(DEV)).cpu().numpy()
-    assert _relerr(got, want) <= 1e-4
+    assert rel_err(got, want) <= 1e-4
 
 
 def test_training_decreases_the_loss_with_its_own_masks():

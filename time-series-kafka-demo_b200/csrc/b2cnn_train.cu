@@ -87,6 +87,13 @@ static TrainWs train_ws(const TrainDims &d, int64_t B) {
 }
 
 __device__ __forceinline__ float sigmoidf_(float v) { return 1.0f / (1.0f + expf(-v)); }
+// d tanh(v) / dv = 1 - tanh(v)^2 = 4t / (1 + t)^2 with t = exp(-2|v|), from the pre-activation: 1 - y*y of a float y
+// near +-1 cancels to a few ulps of 1 (relative error ~1 at |v| ~ 8), this form has no cancellation.  NaN stays NaN,
+// +-inf gives 0 like 1 - tanh(+-inf)^2.
+__device__ __forceinline__ float dtanhf_(float v) {
+    const float t = expf(-2.f * fabsf(v)), u = 1.f + t;
+    return 4.f * t / (u * u);
+}
 
 // What follows the logits z.  kHeadLogits: no loss in the forward kernel, d loss / d z read from the caller's array in the
 // backward kernel.  kHeadBce: BCEWithLogitsLoss (mean).  kHeadBcePw: BCEWithLogitsLoss(pos_weight=pw) (mean).
@@ -115,8 +122,8 @@ train_conv_fwd(const float *__restrict__ x, const float *__restrict__ prm, BlobO
     for (int e = tid; e < kCMid * d.P1; e += blockDim.x) {
         const int oc = e / d.P1, i = e % d.P1;
         float m = c1b[oc * d.L1 + d.PS * i];
-        for (int j = 1; j < d.PK; ++j) m = fmaxf(m, c1b[oc * d.L1 + d.PS * i + j]);
-        p1b[e] = tanhf(m);                                   // max commutes with the monotone tanh
+        for (int j = 1; j < d.PK; ++j) m = max_nan(m, c1b[oc * d.L1 + d.PS * i + j]);
+        p1b[e] = tanhf(m);                  // pooling before tanh: tanh is monotone, and a NaN in the window wins either way
     }
     __syncthreads();
     for (int t = tid; t < d.L2; t += blockDim.x) {
@@ -132,7 +139,7 @@ train_conv_fwd(const float *__restrict__ x, const float *__restrict__ prm, BlobO
     __syncthreads();
     for (int i = tid; i < d.L; i += blockDim.x) {
         float m = c2b[d.PS * i];
-        for (int j = 1; j < d.PK; ++j) m = fmaxf(m, c2b[d.PS * i + j]);
+        for (int j = 1; j < d.PK; ++j) m = max_nan(m, c2b[d.PS * i + j]);
         fb[i] = tanhf(m) * (mask2 ? mask2[(int64_t)b * d.L + i] : 1.0f);
     }
 }
@@ -293,7 +300,7 @@ train_lstm_bwd(const float *__restrict__ prm, BlobOff o, TrainDims d, int64_t B,
 #pragma unroll
             for (int k = 0; k < kHidden; ++k) {
                 gWih1[k] += v * hs[(t * 2 + 0) * kHidden + k];                      // layer-1 input = h0_t
-                if (!first) gWhh1[k] += v * hs[((t - 1) * 2 + 1) * kHidden + k];
+                gWhh1[k] += v * (first ? 0.f : hs[((t - 1) * 2 + 1) * kHidden + k]);  // v * 0: a NaN v still counts
             }
         }
         __syncthreads();
@@ -325,10 +332,8 @@ train_lstm_bwd(const float *__restrict__ prm, BlobOff o, TrainDims d, int64_t B,
             da0[t * kGates + r] = v;
             if (q == 0) dc0c[u] = dc * a[kHidden + u];
             gb0 += v;
-            if (!first) {
 #pragma unroll
-                for (int k = 0; k < kHidden; ++k) gWhh0[k] += v * hs[((t - 1) * 2 + 0) * kHidden + k];
-            }
+            for (int k = 0; k < kHidden; ++k) gWhh0[k] += v * (first ? 0.f : hs[((t - 1) * 2 + 0) * kHidden + k]);
         }
         __syncthreads();
         if (r < kHidden) {
@@ -370,7 +375,9 @@ __global__ void train_dfeat(const float *__restrict__ da0, const float *__restri
     dfeat[e] = a;
 }
 
-// first maximum of a pooling window, like ATen's max_pool1d ((v > m) || isnan(v) replaces)
+// first maximum of a pooling window, like ATen's max_pool1d ((v > m) || isnan(v) replaces).  This is the first maximum
+// of the pre-activation; the reference pools after tanh and takes the first maximum there.  The two differ only where
+// tanhf maps distinct pre-activations to one float: this choice is the one exact arithmetic makes.
 __device__ __forceinline__ int pool_argmax(const float *v, int start, int pk) {
     int best = start;
     float m = v[start];
@@ -402,8 +409,7 @@ train_conv_bwd(const float *__restrict__ x, const float *__restrict__ prm, BlobO
         if (t - d.PK + 1 <= 0) i_lo = 0;
         for (int i = i_lo; i <= t / d.PS && i < d.L; ++i)
             if (pool_argmax(c2b, d.PS * i, d.PK) == t) a += dfb[i] * (mask2 ? mask2[(int64_t)b * d.L + i] : 1.0f);
-        const float y = tanhf(c2b[t]);
-        dc2b[t] = a * (1.f - y * y);
+        dc2b[t] = a * dtanhf_(c2b[t]);
     }
     __syncthreads();
     // ---- conv2: weight / bias gradients (block reduction, one atomic per value and CTA), d d1
@@ -446,8 +452,7 @@ train_conv_bwd(const float *__restrict__ x, const float *__restrict__ prm, BlobO
         if (t - d.PK + 1 <= 0) i_lo = 0;
         for (int i = i_lo; i <= t / d.PS && i < d.P1; ++i)
             if (pool_argmax(row, d.PS * i, d.PK) == t) a += dd1b[oc * d.P1 + i];
-        const float y = tanhf(row[t]);
-        dc1b[e] = a * (1.f - y * y);
+        dc1b[e] = a * dtanhf_(row[t]);
     }
     __syncthreads();
     // ---- conv1: one thread per weight, a dot product over the positions
