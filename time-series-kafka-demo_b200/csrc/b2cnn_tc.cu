@@ -7,11 +7,12 @@
 //
 //   D[w, (s,o)] = sum_{c} sum_{k<16}  X_c[w, 8n+k] * T_c[k, (s,o)],   T_c[k,(s,o)] = w1[o][c][k-s]
 //
-//   * A = X_c: 128 windows x 64 consecutive samples of channel c, brought by ONE 3-D TMA box
-//     {64 samples, 1 channel, 128 windows} into the canonical K-major SWIZZLE_128B layout; the
+//   * A = X_c: 128 windows x 32 consecutive samples of channel c, brought by ONE 3-D TMA box
+//     {32 samples, 1 channel, 128 windows} into the canonical K-major SWIZZLE_64B layout; the
 //     8-position block n of the tile uses the K=16 slice starting at 16-byte chunk n (descriptor
-//     start address + 16n bytes), so one landed tile feeds 7 blocks = 56 conv1 positions
-//     (tiles advance by 56 samples; the 8 overlapping samples are re-read from L2, not HBM).
+//     start address + 16n bytes), so one landed tile feeds 3 blocks = 24 conv1 positions
+//     (tiles advance by 24 samples; the 8 overlapping samples are re-read from L2, not HBM).
+//     The small tile keeps the kernel at about 100 KB of shared memory: two CTAs share an SM.
 //   * B = T_c: the fp32 conv1 weights expanded to a 16 x 32 band matrix (8 output shifts s x 4
 //     output channels o) and split into 2 or 3 bf16 pieces (hi/mid/lo) so that, the inputs
 //     being exactly bf16, every product is exact and the fp32 accumulation carries the full
@@ -41,9 +42,10 @@ const char *tc_error() { return g_tc_err; }
 #endif
 constexpr int64_t kOwnFlagCap = 65536;   // windows per call served by the handle's own flag state (512 KB); larger batches use the workspace copy
 constexpr int kTcM = 128;          // windows per CTA (two wgmma m64 row halves)
-constexpr int kTcAdv = 56;         // conv1 positions (= samples) a tile advances
-constexpr int kTcBlocks = 7;       // 8-position blocks per 64-sample tile
-constexpr int kTcABytes = 128 * 128;
+constexpr int kTcAdv = 24;         // conv1 positions (= samples) a tile advances
+constexpr int kTcBlocks = 3;       // 8-position blocks per 32-sample tile
+constexpr int kTcARow = 64;        // bytes per window row of a bf16 tile (32 samples, SWIZZLE_64B)
+constexpr int kTcF32ARow = 128;    // ... of an fp32 tile (32 samples, SWIZZLE_128B)
 constexpr int kTcBBytes = 32 * 16 * 2;   // one band matrix piece: N=32 x K=16 bf16
 constexpr int kTcMaxC = 4;
 
@@ -100,7 +102,6 @@ static bool arch_ok(const Dims &d) {
 }
 
 static int tiles_per_cta_for(const Dims &d);
-static int tiles_per_cta_s_for(const Dims &d);
 
 int tc_prepare(TcState &s, const Dims &d, const ConvWeights &cw, const float *d_wih0, const HeadWeights &, int splits, int,
                cudaStream_t st) {
@@ -150,11 +151,11 @@ int tc_prepare(TcState &s, const Dims &d, const ConvWeights &cw, const float *d_
         cudaStreamSynchronize(st) != cudaSuccess) { g_tc_err = "upload band matrices"; return -1; }
     s.ready = true;
     s.has_v1 = arch_ok(d);
-    // ---- fused kernel: W_ih_l0 packed per (range, chunk)
+    // ---- fused kernels (bf16 and fp32 windows: the same 3-block tiles and ranges): W_ih_l0 packed per (range, chunk)
     s.fused_ready = false;
     s.tiles_per_cta = tiles_per_cta_for(d);
-    s.feats_per_cta = 14 * s.tiles_per_cta - 4;      // even: every range starts 16-byte aligned (TMA)
-    s.chunks_per_cta = (7 * s.tiles_per_cta + 7) / 8;
+    s.feats_per_cta = 2 * kTcBlocks * s.tiles_per_cta - 4;   // even: every range starts 16-byte aligned (TMA)
+    s.chunks_per_cta = (kTcBlocks * s.tiles_per_cta + 7) / 8;
     s.n_ranges = (d.L + s.feats_per_cta - 1) / s.feats_per_cta;
     if (d.C <= 3) {
         const size_t bytes = (size_t)s.n_ranges * s.chunks_per_cta * kFuWChunkBytes;
@@ -165,20 +166,6 @@ int tc_prepare(TcState &s, const Dims &d, const ConvWeights &cw, const float *d_
                                                                           s.feats_per_cta, s.chunks_per_cta, s.n_ranges, d.K1 == 10 ? 3 : 2);
         if (cudaGetLastError() != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess) { g_tc_err = "pack W_ih"; return -1; }
         s.fused_ready = true;
-        // stream_f32_kernel: 3-block tiles, its own (L-only) position ranges
-        s.stream_ready = false;
-        s.tiles_per_cta_s = tiles_per_cta_s_for(d);
-        s.feats_per_cta_s = 2 * kSfBlocks * s.tiles_per_cta_s - 4;
-        s.chunks_per_cta_s = (kSfBlocks * s.tiles_per_cta_s + 7) / 8;
-        s.n_ranges_s = (d.L + s.feats_per_cta_s - 1) / s.feats_per_cta_s;
-        const size_t bytes_s = (size_t)s.n_ranges_s * s.chunks_per_cta_s * kFuWChunkBytes;
-        cudaFree(s.d_wpack_s); s.d_wpack_s = nullptr;
-        if (cudaMalloc(&s.d_wpack_s, bytes_s) != cudaSuccess) { g_tc_err = "cudaMalloc(packed W_ih, fp32 stream)"; return -1; }
-        const int64_t total_s = (int64_t)s.n_ranges_s * s.chunks_per_cta_s * 1024;
-        tc_pack_wih_kernel<<<(unsigned)((total_s + 255) / 256), 256, 0, st>>>(d_wih0, reinterpret_cast<uint8_t *>(s.d_wpack_s), d.L,
-                                                                            s.feats_per_cta_s, s.chunks_per_cta_s, s.n_ranges_s, d.K1 == 10 ? 3 : 2);
-        if (cudaGetLastError() != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess) { g_tc_err = "pack W_ih (fp32 stream)"; return -1; }
-        s.stream_ready = true;
     }
     return 0;
 }
@@ -189,9 +176,6 @@ void tc_release(TcState &s) {
     cudaFree(s.d_bmats);
     cudaFree(s.d_bmats2);
     cudaFree(s.d_wpack);
-    cudaFree(s.d_wpack_s);
-    s.d_wpack_s = nullptr;
-    s.stream_ready = false;
     s.d_bmats = nullptr;
     s.d_bmats2 = nullptr;
     s.d_wpack = nullptr;
@@ -259,22 +243,13 @@ static const void *tc_stage_input(const Dims &d, const void *x, int64_t B, void 
 }
 
 static int tiles_per_cta_for(const Dims &d) {
-    // About 37 position ranges per window whatever its length (depends on L only, so a window's
-    // summation order never depends on the batch): L=18745 -> 37 tiles (514 features) per CTA and
-    // 37 ranges x 32 window tiles = 1184 CTAs = 9 waves of 132 at B=4096; shorter windows get
-    // proportionally shorter ranges so that small batches still fill the SMs.
-    if (const char *e = getenv("B2CNN_TC_TILES")) { const int v = atoi(e); if (v >= 1 && v <= 4096) return v; }
-    int nt = ((d.L + 36) / 37 + 4 + 13) / 14;
-    if (nt < 2) nt = 2;
-    if (nt > 37) nt = 37;
-    return nt;
-}
-
-static int tiles_per_cta_s_for(const Dims &d) {
-    // fp32 windows: about 37 position ranges (L only) like the bf16 kernel; a CTA's stream emits
-    // 6*tiles - 4 features (even: every range starts 16-byte aligned for TMA)
-    if (const char *e = getenv("B2CNN_SF_TILES")) { const int v = atoi(e); if (v >= 1 && v <= 16384) return v; }
-    int nt = ((d.L + 36) / 37 + 4 + 5) / 6;
+    // About 33 position ranges per window whatever its length (depends on L only, so a window's
+    // summation order never depends on the batch).  A CTA's stream emits 6*tiles - 4 features.
+    // L=18745 -> 96 tiles (572 features) per CTA and 33 ranges x 32 window tiles = 1056 CTAs at B=4096:
+    // 4 waves of the 264 bf16 CTAs resident on 132 SMs (two per SM), 8 waves of the fp32 kernel (one per
+    // SM).  Shorter windows get proportionally shorter ranges so that small batches still fill the SMs.
+    if (const char *e = getenv("B2CNN_TC_TILES")) { const int v = atoi(e); if (v >= 1 && v <= 16384) return v; }
+    int nt = ((d.L + 32) / 33 + 4 + 2 * kTcBlocks - 1) / (2 * kTcBlocks);
     if (nt < 4) nt = 4;
     return nt;
 }
@@ -309,10 +284,11 @@ static int make_tmap(const Dims &d, const void *x, int64_t pitch, int64_t B, boo
     const int esz = f32 ? 4 : 2;
     cuuint64_t gdim[3] = {(cuuint64_t)d.W, (cuuint64_t)d.C, (cuuint64_t)B};
     cuuint64_t gstr[2] = {(cuuint64_t)pitch * esz, (cuuint64_t)d.C * pitch * esz};
-    cuuint32_t box[3] = {(cuuint32_t)(128 / esz), 1, kTcM};       // 128-byte rows: one SWIZZLE_128B row per window
+    // 32 samples per window: one 64-byte SWIZZLE_64B row (bf16) or one 128-byte SWIZZLE_128B row (fp32)
+    cuuint32_t box[3] = {32, 1, kTcM};
     cuuint32_t estr[3] = {1, 1, 1};
     CUresult r = get_encode()(tm, f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void *>(x),
-                              gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                              gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, f32 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
                               CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) { *err = "cuTensorMapEncodeTiled failed"; return -1; }
     return 0;
@@ -382,10 +358,7 @@ int tc_features(TcState &s, const Dims &d, const ConvWeights &cw, const void *x,
 bool tc_fused_supported(const TcState &s, const Dims &d, int dtype) {
     return s.ready && s.fused_ready && s.opt_fused && dtype == B2CNN_DTYPE_BF16 && (arch_ok(d) || arch1_ok(d)) && d.C <= 3;
 }
-int tc_partial_slices(const TcState &s) {
-    if (!s.fused_ready) return 0;
-    return s.stream_ready && s.n_ranges_s > s.n_ranges ? s.n_ranges_s : s.n_ranges;
-}
+int tc_partial_slices(const TcState &s) { return s.fused_ready ? s.n_ranges : 0; }
 
 // Where this call keeps count | flags | list: the handle's own, already-zero copy (see TcState) or the head of the
 // workspace, zeroed here.  count and flags are adjacent in both, the list needs no zeroing.
@@ -456,7 +429,7 @@ int tc_fused_gates(TcState &s, const Dims &d, const ConvWeights &cw, const HeadW
 }
 
 bool tc_stream_supported(const TcState &s, const Dims &d, int dtype) {
-    return s.ready && s.stream_ready && dtype == B2CNN_DTYPE_F32 && (arch_ok(d) || arch1_ok(d)) && d.C <= 3 && (d.XP % 4) == 0;
+    return s.ready && s.fused_ready && dtype == B2CNN_DTYPE_F32 && (arch_ok(d) || arch1_ok(d)) && d.C <= 3 && (d.XP % 4) == 0;
 }
 
 // fp32 windows: streaming front end + projection -> gates[B][64]; flagged (NaN) windows are recomputed exactly.
@@ -471,11 +444,11 @@ int tc_stream_gates(TcState &s, const Dims &d, const ConvWeights &cw, const Head
     TcFusedParams p;
     memset(&p, 0, sizeof p);
     p.partial = partial; p.nanflag = flags; p.list = list; p.count = count;
-    p.wpack = reinterpret_cast<const uint8_t *>(s.d_wpack_s);
+    p.wpack = reinterpret_cast<const uint8_t *>(s.d_wpack);
     p.B = (int)B; p.W = d.W; p.L = d.L;
-    p.tiles_per_cta = s.tiles_per_cta_s; p.feats_per_cta = s.feats_per_cta_s; p.chunks_per_cta = s.chunks_per_cta_s;
+    p.tiles_per_cta = s.tiles_per_cta; p.feats_per_cta = s.feats_per_cta; p.chunks_per_cta = s.chunks_per_cta;
     fill_epilogue(p, d, cw);
-    dim3 grid((unsigned)((B + kTcM - 1) / kTcM), s.n_ranges_s);
+    dim3 grid((unsigned)((B + kTcM - 1) / kTcM), s.n_ranges);
     const int key = d.C * 10 + (d.K1 == 10 ? 0 : 1);
     cudaError_t le;
     switch (key) {
@@ -486,11 +459,11 @@ int tc_stream_gates(TcState &s, const Dims &d, const ConvWeights &cw, const Head
     }
     if (le != cudaSuccess) { *err = cudaGetErrorString(le); return -1; }
     int launches = 1;
-    if (slices_out) *slices_out = s.n_ranges_s;
-    int n = launch_frontend_generic_gates_listed(d, cw, x, B2CNN_DTYPE_F32, B, hw.wih0T, partial, s.n_ranges_s, list, count, st, num_sms, err);
+    if (slices_out) *slices_out = s.n_ranges;
+    int n = launch_frontend_generic_gates_listed(d, cw, x, B2CNN_DTYPE_F32, B, hw.wih0T, partial, s.n_ranges, list, count, st, num_sms, err);
     if (n < 0) return -1;
     launches += n;
-    n = reduce_here ? launch_reduce_gates(partial, s.n_ranges_s, B, hw, gates, st, err) : 0;
+    n = reduce_here ? launch_reduce_gates(partial, s.n_ranges, B, hw, gates, st, err) : 0;
     if (n < 0) return -1;
     return launches + n;
 }

@@ -10,12 +10,9 @@ struct TcState {
     void *d_bmats = nullptr;     // Toeplitz-expanded conv1 weights, three bf16 pieces (see b2cnn_tc.cu)
     void *d_bmats2 = nullptr;    // the first two pieces only (tc_splits=2)
     void *d_wpack = nullptr;     // W_ih_l0 packed per (position range, 16-position chunk), 3 bf16 pieces
-    int tiles_per_cta = 37, feats_per_cta = 514, chunks_per_cta = 33, n_ranges = 1;
-    void *d_wpack_s = nullptr;   // the same packing for the 3-block tiles of the fp32-window kernel
-    int tiles_per_cta_s = 86, feats_per_cta_s = 512, chunks_per_cta_s = 33, n_ranges_s = 1;
-    bool stream_ready = false;   // fp32-window kernel usable (C <= 3)
+    int tiles_per_cta = 96, feats_per_cta = 572, chunks_per_cta = 36, n_ranges = 1;
     bool has_v1 = false;         // the features-out kernel exists for this geometry (MyCNN5 only)
-    bool fused_ready = false;    // fused conv + projection kernel usable (C <= 3)
+    bool fused_ready = false;    // fused conv + projection kernels (bf16 and fp32 windows) usable (C <= 3)
     int64_t opt_fused = 1;
     // Flag state of the streaming kernels' NaN exception path (count | flags [cap] | list [cap]) owned by the handle:
     // it is all-zero between calls -- the head kernel that consumes a call's list clears exactly what the call set --

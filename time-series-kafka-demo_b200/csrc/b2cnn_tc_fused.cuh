@@ -5,11 +5,13 @@
 //      gates[w, g] += sum_p  f[w, p] * W_ih_l0[g, p]           (bin/models.py:30, layer 0)
 //
 // conv1 of bf16 windows is the banded-Toeplitz GEMM described in b2cnn_tc.cu, on wgmma: per 8-position block,
-// two m64n32k16 row halves x C channels x SPLITS weight pieces, A = the TMA tile (SWIZZLE_128B, the block's
-// 16-sample slice selected by a 16n-byte descriptor offset), B = the band-matrix piece, D in registers.  The
-// accumulator fragment (two windows x 16 values per thread) is turned into thread == window through an 18 KB
-// shared-memory transpose; the next block's MMAs run while the epilogue of this one computes.  fp32 windows
-// (F32IN) evaluate conv1 in exact fp32 FMAs straight from the tile instead (32-sample boxes, 3 blocks per tile).
+// two m64n32k16 row halves x C channels x SPLITS weight pieces, A = the TMA tile (32-sample boxes, SWIZZLE_64B,
+// the block's 16-sample slice selected by a 16n-byte descriptor offset, 3 blocks per tile), B = the band-matrix
+// piece, D in registers.  The accumulator fragment (two windows x 16 values per thread) is turned into thread ==
+// window through an 18 KB shared-memory transpose; the next block's MMAs run while the epilogue of this one
+// computes.  About 100 KB of shared memory and at most 168 registers per thread let two CTAs share an SM, so each
+// SM sub-partition has two consumer warps to interleave.  fp32 windows (F32IN) evaluate conv1 in exact fp32 FMAs
+// straight from the tile instead (the same 32-sample boxes as 128-byte SWIZZLE_128B rows; one CTA per SM).
 //
 // Epilogue, thread == window: each thread streams through its window's positions in order, so pool1 -> tanh ->
 // conv2 -> pool2 -> tanh are register-local sliding windows; tanh is 1 - 2/(1+2^(2x log2 e)) on MUFU.EX2 +
@@ -33,8 +35,6 @@ constexpr int kHpTStride = 36;                    // floats per window row of th
 constexpr int kHpTBytes = kTcM * kHpTStride * 4;
 constexpr int kHpPieceBytes = kTcM * 16 * 2;      // one bf16 piece of the projection A operand
 constexpr int kFuWChunkBytes = 3 * 64 * 16 * 2;   // 3 pieces x (64 gates x 16 positions) bf16
-constexpr int kSfBlocks = 3;                      // fp32 windows: 8-position blocks per 32-sample tile
-constexpr int kSfAdv = 24;
 constexpr int kOutFeatures = 0, kOutGates = 1;
 
 struct TcFusedParams {
@@ -55,7 +55,7 @@ struct TcFusedParams {
 };
 
 __host__ __device__ constexpr size_t hp_smem_bytes(int C, int SPLITS, bool f32in, int out) {
-    return 1024 + (size_t)2 * C * kTcABytes + (f32in ? 0 : (size_t)C * SPLITS * kTcBBytes + kHpTBytes) +
+    return 1024 + (size_t)2 * C * kTcM * (f32in ? kTcF32ARow : kTcARow) + (f32in ? 0 : (size_t)C * SPLITS * kTcBBytes + kHpTBytes) +
            (out == kOutGates ? (size_t)2 * kFuWChunkBytes + 3 * kHpPieceBytes : 0) + 8 * 8;
 }
 
@@ -64,24 +64,25 @@ __host__ __device__ constexpr size_t hp_smem_bytes(int C, int SPLITS, bool f32in
 //         16-sample slice (no tap-9 patch), pooling pairs stay inside a block (no carry), and a step emits
 //         features 2j-2, 2j-1 instead of 2j-3, 2j-2.
 template <int C, int SPLITS, int ARCH, bool F32IN, int OUT>
-__global__ void __launch_bounds__(kHpThreads, 1)
+__global__ void __launch_bounds__(kHpThreads, F32IN ? 1 : 2)
 tc_stream_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ TcFusedParams p) {
     constexpr int K1 = ARCH == 0 ? 10 : 5;
-    constexpr int kBlocks = F32IN ? kSfBlocks : kTcBlocks;
-    constexpr int kAdv = F32IN ? kSfAdv : kTcAdv;
+    constexpr int kBlocks = kTcBlocks;
+    constexpr int kARow = F32IN ? kTcF32ARow : kTcARow;
+    constexpr int kABytes = kTcM * kARow;             // one channel of one stage
     constexpr int FOFF = ARCH == 0 ? 3 : 2;           // step j emits features 2j-FOFF, 2j-FOFF+1
     extern __shared__ uint8_t smem_raw[];
-    // [2 stages][C][16 KB] | bands | transpose | W ring [2][6 KB] | A pieces [3][4 KB] | barriers
+    // [2 stages][C][8 KB bf16 | 16 KB fp32] | bands | transpose | W ring [2][6 KB] | A pieces [3][4 KB] | barriers
     uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     uint8_t *sA = smem;
-    uint8_t *sBm = sA + 2 * C * kTcABytes;
+    uint8_t *sBm = sA + 2 * C * kABytes;
     float *sT = reinterpret_cast<float *>(sBm + (F32IN ? 0 : C * SPLITS * kTcBBytes));
     uint8_t *sW = reinterpret_cast<uint8_t *>(sT) + (F32IN ? 0 : kHpTBytes);
     uint8_t *sPc = sW + (OUT == kOutGates ? 2 * kFuWChunkBytes : 0);
     uint64_t *bars = reinterpret_cast<uint64_t *>(sPc + (OUT == kOutGates ? 3 * kHpPieceBytes : 0));
     const uint32_t bar_full = smem_u32(bars + 0), bar_empty = smem_u32(bars + 2);
     const uint32_t bar_wfull = smem_u32(bars + 4), bar_wempty = smem_u32(bars + 6);
-    auto sA_of = [&](int s, int c) -> uint8_t * { return sA + (size_t)(s * C + c) * kTcABytes; };
+    auto sA_of = [&](int s, int c) -> uint8_t * { return sA + (size_t)(s * C + c) * kABytes; };
 
     const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);
     const int lane = threadIdx.x & 31;
@@ -115,9 +116,9 @@ tc_stream_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant
             for (int i = 0; i < ntiles; ++i) {
                 const int s = i & 1, ph = (i >> 1) & 1;
                 mbar_wait(bar_empty + 8 * s, ph ^ 1);
-                mbar_expect_tx(bar_full + 8 * s, C * kTcABytes);
+                mbar_expect_tx(bar_full + 8 * s, C * kABytes);
 #pragma unroll
-                for (int c = 0; c < C; ++c) tma_load_3d(smem_u32(sA_of(s, c)), &tmap, T0 + kAdv * i, c, b0, bar_full + 8 * s);
+                for (int c = 0; c < C; ++c) tma_load_3d(smem_u32(sA_of(s, c)), &tmap, T0 + kTcAdv * i, c, b0, bar_full + 8 * s);
             }
         }
     } else if (warp == 5) {
@@ -136,7 +137,8 @@ tc_stream_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant
         const int row = threadIdx.x;
         const int b = b0 + row;
         const bool row_ok = b < p.B;
-        const uint32_t swz = (uint32_t)(row & 7);     // SWIZZLE_128B: 16-byte chunk ^= row % 8
+        // 16-byte chunk k of a row sits at chunk k ^ swz: SWIZZLE_64B (bf16) k ^ (row / 2) % 4, SWIZZLE_128B (fp32) k ^ row % 8
+        const uint32_t swz = F32IN ? (uint32_t)(row & 7) : (uint32_t)((row >> 1) & 3);
         float acc[2][16];                             // conv1 accumulators of one block (two m64 row halves)
         float gacc[2][32];                            // gate pre-activations (two m64 row halves)
 #pragma unroll
@@ -155,14 +157,17 @@ tc_stream_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant
         }
         float *fout = p.feats + (int64_t)b * p.sB + (int64_t)p0 * p.sP;
 
+        // descriptors built once: a block's MMAs only add (start address offset) >> 4 to them
+        const uint64_t adesc0 = gdesc_sw64_kmajor(smem_u32(sA));
+        const uint64_t bdesc0 = gdesc_none_kmajor(smem_u32(sBm), 128, 256);
         auto issue_conv1 = [&](int s, int n) {
-            const uint64_t bdesc0 = gdesc_none_kmajor(smem_u32(sBm), 128, 256);
+            const uint64_t adesc_sn = adesc0 + (uint64_t)((s * C * kABytes + 16 * n) >> 4);
             wgmma_fence();
 #pragma unroll
             for (int h = 0; h < 2; ++h)
 #pragma unroll
                 for (int c = 0; c < C; ++c) {
-                    const uint64_t adesc = gdesc_sw128_kmajor(smem_u32(sA_of(s, c)) + h * 64 * 128 + 16 * n);
+                    const uint64_t adesc = adesc_sn + (uint64_t)((c * kABytes + h * 64 * kARow) >> 4);
 #pragma unroll
                     for (int sp = 0; sp < SPLITS; ++sp)
                         wgmma_m64n32(acc[h], adesc, bdesc0 + (uint64_t)((c * SPLITS + sp) * (kTcBBytes >> 4)), (c | sp) != 0);
@@ -183,7 +188,7 @@ tc_stream_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant
                     // tap 9 of the previous block's position 7: sample 8n + 8 of this tile
 #pragma unroll
                     for (int c = 0; c < C; ++c) {
-                        const uint16_t raw = *reinterpret_cast<const uint16_t *>(sA_of(s, c) + row * 128 + (((uint32_t)(n + 1) ^ swz) << 4));
+                        const uint16_t raw = *reinterpret_cast<const uint16_t *>(sA_of(s, c) + row * kARow + (((uint32_t)(n + 1) ^ swz) << 4));
                         const float xv = __uint_as_float((uint32_t)raw << 16);
 #pragma unroll
                         for (int o = 0; o < kCMid; ++o) pm7[o] = fmaf(p.w9[c][o], xv, pm7[o]);
@@ -221,7 +226,7 @@ tc_stream_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant
                     float xs[16];
 #pragma unroll
                     for (int j4 = 0; j4 < 4; ++j4) {
-                        const float4 v = *reinterpret_cast<const float4 *>(sA_of(s, c) + row * 128 + (((uint32_t)(2 * n + j4) ^ swz) << 4));
+                        const float4 v = *reinterpret_cast<const float4 *>(sA_of(s, c) + row * kARow + (((uint32_t)(2 * n + j4) ^ swz) << 4));
                         xs[4 * j4 + 0] = v.x; xs[4 * j4 + 1] = v.y; xs[4 * j4 + 2] = v.z; xs[4 * j4 + 3] = v.w;
                     }
                     if constexpr (ARCH == 0) {

@@ -74,10 +74,10 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float lo_elem, float hi_elem) {
 // Fragment of D held by thread t of the warpgroup (warp w = t / 32, lane l): element i of the N/2 registers is
 // row 16 w + l / 4 + 8 ((i / 2) % 2), column 8 (i / 4) + 2 (l % 4) + i % 2.
 // ------------------------------------------------------------------------------------------
-// GMMA shared-memory descriptor: start >> 4 | LBO >> 4 << 16 | SBO >> 4 << 32 | layout << 62 (1 = SWIZZLE_128B, 0 = none)
-__device__ __forceinline__ uint64_t gdesc_sw128_kmajor(uint32_t saddr) {
-    // rows 128 B apart, 8-row groups 1024 B apart (SBO); LBO unused for swizzled K-major
-    return (uint64_t)((saddr >> 4) & 0x3FFF) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 62);
+// GMMA shared-memory descriptor: start >> 4 | LBO >> 4 << 16 | SBO >> 4 << 32 | layout << 62 (2 = SWIZZLE_64B, 0 = none)
+__device__ __forceinline__ uint64_t gdesc_sw64_kmajor(uint32_t saddr) {
+    // rows 64 B apart, 8-row groups 512 B apart (SBO); LBO unused for swizzled K-major
+    return (uint64_t)((saddr >> 4) & 0x3FFF) | ((uint64_t)1 << 16) | ((uint64_t)(512 >> 4) << 32) | ((uint64_t)2 << 62);
 }
 // no swizzle, K-major core matrices (8 rows x 16 bytes): LBO = K-adjacent core matrices, SBO = M/N-adjacent ones
 __device__ __forceinline__ uint64_t gdesc_none_kmajor(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
