@@ -196,6 +196,46 @@ int b2cnn_ring_set_signals(b2cnn_ring *ring, int32_t patient, const int32_t *sel
 int b2cnn_ring_push(b2cnn_ring *ring, const void *new_samples, int sample_kind, int64_t n_new, void *x_out, int dtype,
                     int32_t *emitted, int64_t *window_index, double *t0_seconds, void *stream);
 
+/* ---- Long waveform windows scored incrementally: a per-patient feature ring (csrc/b2cnn_slide.cu) ----
+ * The reference scores a patient with a W-sample window that slides by S samples (bin/predictStream.py:248-252: 600 s
+ * every 60 s); consecutive windows share W - S samples.  The front end is translation-equivariant with a feature
+ * stride of 4 samples, so for S % 4 == 0 feature i of a window is feature i + S/4 of the previous one: a scorer keeps
+ * every patient's L = lstm_input features on the device and computes only the S/4 features each push completes, then
+ * runs the input projection over the whole feature row and the head.
+ *   b2cnn_slide_create   `h` with weights set; n_patients P >= 1; stride S with 1 <= S <= window and S % 4 == 0
+ *                        (else B2CNN_EINVAL); dtype of the pushed samples, f32 or bf16.  The geometries and channel
+ *                        counts of the streaming tensor-core kernels with both window dtypes and the packed W_ih
+ *                        projection (MyCNN5 or MyCNN2/3/4 conv/pool, 1 to 3 channels, tanh, no affine); anything
+ *                        else is B2CNN_EARCH.  C = 4 is left out on purpose: the fp32-window kernel and the packed
+ *                        W_ih chunks exist for C <= 3 only.  Allocates all device state
+ *                        (the fp32 ring, 4 P L bytes, and staging rows for one segment); the handle must outlive
+ *                        the scorer.
+ *   b2cnn_slide_push     new_samples: DEVICE pointer [P][C][S] in the scorer's dtype, channel rows `pitch` elements
+ *                        apart (pitch >= S; window p starts at new_samples + p * C * pitch).  After push n (from 1 on)
+ *                        every patient's window is the last W samples of its stream, [n S - W, n S).  Once n S >= W
+ *                        the push writes out[P] (logits, or sigmoid(logit) if apply_sigmoid), sets *emitted = 1 and
+ *                        *window_index = n - ceil(W / S); before that *emitted = 0 (the features are still stored).
+ *                        out[p] == b2cnn_forward(window of p, mode INDEPENDENT) within fp32 rounding; age: n_age == 1
+ *                        or P.  Rows 16-byte aligned with W % 4 == 0 stream straight from new_samples; otherwise the
+ *                        segment is first copied into the scorer's aligned staging rows -- also when W % 4 != 0 and
+ *                        the rows are aligned: the feature lattice then starts phi = (-W) mod 4 samples into the
+ *                        segment, and the tensor-core kernel's TMA boxes must start on 16-byte boundaries.  B2CNN_ESTATE after
+ *                        b2cnn_set_weights on the handle since the scorer's last reset (its features are stale).
+ *                        Allocates nothing; asynchronous on `stream`.
+ *   b2cnn_slide_reset    forget every stream (pushes count from 1 again) and accept the handle's current weights.
+ *   b2cnn_slide_features feats[P][L] floats on the device: the features of the current windows in window order
+ *                        (parity tests); B2CNN_ESTATE before the first window is complete or when the weights
+ *                        changed since the last reset.
+ * The scorer's patients are independent windows; a push uses no atomics in its value path, so its results do not
+ * depend on P, on the ring's rotation or on the run. */
+typedef struct b2cnn_slide b2cnn_slide;
+int b2cnn_slide_create(b2cnn_handle *h, int32_t n_patients, int32_t stride, int dtype, b2cnn_slide **out);
+void b2cnn_slide_destroy(b2cnn_slide *slide);
+int b2cnn_slide_reset(b2cnn_slide *slide, void *stream);
+int b2cnn_slide_push(b2cnn_slide *slide, const void *new_samples, int64_t pitch, const float *age, int64_t n_age,
+                     int apply_sigmoid, float *out, int32_t *emitted, int64_t *window_index, void *stream);
+int b2cnn_slide_features(b2cnn_slide *slide, float *feats, void *stream);
+
 /* ---- The reference's wire formats, decoded on the device (SURVEY.md section 8, row f3) ----
  * A trigger's Kafka messages as one DEVICE byte buffer + offsets [n_msgs + 1] (message t = bytes[offsets[t] .. offsets[t+1])).
  * b2cnn_decode_sample_messages: value = json.dumps([i, val]) (bin/sendStream.py:62): idx_out[t] = i, val_out[t] = val

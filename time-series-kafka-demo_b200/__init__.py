@@ -8,6 +8,7 @@
     prob  = model.predict(windows, ages)     # batched, one independent window per row
     loss  = B200Trainer(model).step(x, age, target)   # one training step (bin/utils.py:200-208) on the device
     model = B200TrainableMyCNN.from_reference(sd).cuda().train()   # torch autograd + any loss / optimizer
+    scorer = SlidingScorer(model, n_patients, stride)   # sliding windows: one push of new samples per trigger
 
 There is no CPU fallback: constructing a model without the CUDA library or a GPU raises.
 """
@@ -17,7 +18,9 @@ from .checkpoint import load_reference_checkpoint  # noqa: F401
 from .model import B200MyCNN  # noqa: F401
 from .trainer import B200Trainer  # noqa: F401
 from .autograd import B200TrainableMyCNN, mycnn_train_forward  # noqa: F401
+from .slide import SlidingScorer  # noqa: F401
+from .stream import PatientRing  # noqa: F401
 from . import synth  # noqa: F401
 
-__all__ = ["ArchConfig", "ARCH_PRESETS", "arch_from_state_dict", "B200MyCNN", "B200Trainer", "B200TrainableMyCNN", "mycnn_train_forward",
+__all__ = ["ArchConfig", "ARCH_PRESETS", "arch_from_state_dict", "B200MyCNN", "B200Trainer", "B200TrainableMyCNN", "mycnn_train_forward", "SlidingScorer", "PatientRing",
            "load_reference_checkpoint", "load_library", "lib_path", "LibraryNotBuilt", "synth"]

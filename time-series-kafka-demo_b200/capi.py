@@ -28,6 +28,7 @@ SYMBOLS = ("b2cnn_l_out", "b2cnn_weight_count", "b2cnn_create", "b2cnn_destroy",
            "b2cnn_train_step_weighted", "b2cnn_train_forward", "b2cnn_train_backward",
            "b2cnn_prep_window_count", "b2cnn_prep_workspace_bytes", "b2cnn_prep_windows",
            "b2cnn_ring_create", "b2cnn_ring_destroy", "b2cnn_ring_reset", "b2cnn_ring_set_signals", "b2cnn_ring_push",
+           "b2cnn_slide_create", "b2cnn_slide_destroy", "b2cnn_slide_reset", "b2cnn_slide_push", "b2cnn_slide_features",
            "b2cnn_decode_sample_messages", "b2cnn_decode_array_messages", "b2cnn_parse_decimal", "b2cnn_frame_check")
 
 
@@ -114,6 +115,12 @@ def load_library() -> ctypes.CDLL:
     lib.b2cnn_ring_push.argtypes = [c_vp, c_vp, c_int, c_i64, c_vp, c_int, ctypes.POINTER(c_i32), ctypes.POINTER(c_i64),
                                     ctypes.POINTER(ctypes.c_double), c_vp]
     lib.b2cnn_ring_push.restype = c_int
+    lib.b2cnn_slide_create.argtypes = [c_vp, c_i32, c_i32, c_int, ctypes.POINTER(c_vp)]; lib.b2cnn_slide_create.restype = c_int
+    lib.b2cnn_slide_destroy.argtypes = [c_vp]; lib.b2cnn_slide_destroy.restype = None
+    lib.b2cnn_slide_reset.argtypes = [c_vp, c_vp]; lib.b2cnn_slide_reset.restype = c_int
+    lib.b2cnn_slide_push.argtypes = [c_vp, c_vp, c_i64, c_vp, c_i64, c_int, c_vp, ctypes.POINTER(c_i32), ctypes.POINTER(c_i64), c_vp]
+    lib.b2cnn_slide_push.restype = c_int
+    lib.b2cnn_slide_features.argtypes = [c_vp, c_vp, c_vp]; lib.b2cnn_slide_features.restype = c_int
     lib.b2cnn_decode_sample_messages.argtypes = [c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_i64, c_i32, c_vp, c_vp]
     lib.b2cnn_decode_sample_messages.restype = c_int
     lib.b2cnn_decode_array_messages.argtypes = [c_vp, c_vp, c_i64, c_i32, c_vp, c_vp, c_vp, c_vp]

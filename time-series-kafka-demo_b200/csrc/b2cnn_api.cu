@@ -9,6 +9,7 @@
 #include <vector>
 
 #include "b2cnn_internal.cuh"
+#include "b2cnn_slide.cuh"
 #include "b2cnn_tc.cuh"
 
 using namespace b2cnn;
@@ -54,6 +55,7 @@ struct b2cnn_handle {
     int device = 0;
     int num_sms = 132;
     bool weights_set = false;
+    uint64_t weight_gen = 0;    // bumped by every b2cnn_set_weights: a sliding-window scorer's features go stale
     ConvWeights cw;
     HeadWeights hw;
     float *d_blob = nullptr;    // packed blob as given
@@ -351,6 +353,7 @@ extern "C" int b2cnn_set_weights(b2cnn_handle *h, const float *blob, int64_t n, 
     cudaStream_t st = (cudaStream_t)stream;
     DEVICE_GUARD(h->device);
     const Dims &d = h->d;
+    ++h->weight_gen;
     CU_TRY(cudaMemcpyAsync(h->d_blob, blob, sizeof(float) * n, on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, st));
     // conv weights + affine -> host copy for the kernel-parameter constant bank
     const int64_t n_conv = (int64_t)kCMid * d.C * d.K1 + kCMid + kCMid * d.K2 + 1;
@@ -597,6 +600,76 @@ extern "C" int b2cnn_features(b2cnn_handle *h, const void *x, int dtype, int64_t
     if (n < 0) return fail(B2CNN_ECUDA, std::string("front end: ") + err);
     h->last_launches = n;
     return B2CNN_OK;
+}
+
+// ---- sliding-window scorer over a per-patient feature ring (b2cnn_slide.cu) ----
+struct b2cnn_slide { Slide *s; b2cnn_handle *h; uint64_t gen; };
+
+extern "C" int b2cnn_slide_create(b2cnn_handle *h, int32_t n_patients, int32_t stride, int dtype, b2cnn_slide **out) {
+    if (!h || !out) return fail(B2CNN_EINVAL, "b2cnn_slide_create: null argument");
+    *out = nullptr;
+    if (!h->weights_set) return fail(B2CNN_ESTATE, "b2cnn_slide_create: weights not set (call b2cnn_set_weights)");
+    DEVICE_GUARD(h->device);
+    const char *err = "";
+    Slide *s = nullptr;
+    const int rc = slide_create(h->d, h->tc, n_patients, stride, dtype, h->device, &s, &err);
+    if (rc != B2CNN_OK) return fail(rc, std::string("b2cnn_slide_create: ") + err);
+    b2cnn_slide *o = new (std::nothrow) b2cnn_slide{s, h, h->weight_gen};
+    if (!o) { slide_destroy(s); return fail(B2CNN_ESTATE, "out of host memory"); }
+    if (slide_reset(s, nullptr, &err) != B2CNN_OK || cudaStreamSynchronize(nullptr) != cudaSuccess) {
+        b2cnn_slide_destroy(o);
+        return fail(B2CNN_ECUDA, "b2cnn_slide_create: initial reset");
+    }
+    *out = o;
+    return B2CNN_OK;
+}
+extern "C" void b2cnn_slide_destroy(b2cnn_slide *o) {
+    if (!o) return;
+    DeviceGuard guard(slide_device(o->s));
+    slide_destroy(o->s);
+    delete o;
+}
+extern "C" int b2cnn_slide_reset(b2cnn_slide *o, void *stream) {
+    if (!o) return fail(B2CNN_EINVAL, "b2cnn_slide_reset: null argument");
+    DEVICE_GUARD(slide_device(o->s));
+    const char *err = "";
+    const int rc = slide_reset(o->s, reinterpret_cast<cudaStream_t>(stream), &err);
+    if (rc != B2CNN_OK) return fail(rc, std::string("b2cnn_slide_reset: ") + err);
+    o->gen = o->h->weight_gen;
+    return B2CNN_OK;
+}
+extern "C" int b2cnn_slide_push(b2cnn_slide *o, const void *new_samples, int64_t pitch, const float *age, int64_t n_age,
+                                int apply_sigmoid, float *out, int32_t *emitted, int64_t *window_index, void *stream) {
+    if (!o || !new_samples || !age || !out || !emitted || !window_index) return fail(B2CNN_EINVAL, "b2cnn_slide_push: null argument");
+    b2cnn_handle *h = o->h;
+    if (o->gen != h->weight_gen)
+        return fail(B2CNN_ESTATE, "b2cnn_slide_push: the handle's weights changed since the scorer's last reset (stored features are stale)");
+    DEVICE_GUARD(h->device);
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    cudaEvent_t *ev = nullptr;
+    if (h->opt_profile) {
+        for (int i = 0; i < 3; ++i)
+            if (!h->ev_stage[i]) CU_TRY(cudaEventCreate(&h->ev_stage[i]));
+        ev = h->ev_stage;
+    }
+    const char *err = "";
+    int em = 0;
+    int64_t widx = -1;
+    const int rc = slide_push(o->s, h->cw, h->hw, h->tc, new_samples, pitch, age, n_age, apply_sigmoid, out, &em, &widx, ev, st, &err);
+    if (rc != B2CNN_OK) return fail(rc, std::string("b2cnn_slide_push: ") + err);
+    h->ev_valid = ev != nullptr;
+    *emitted = em;
+    if (em) *window_index = widx;
+    return B2CNN_OK;
+}
+extern "C" int b2cnn_slide_features(b2cnn_slide *o, float *feats, void *stream) {
+    if (!o || !feats) return fail(B2CNN_EINVAL, "b2cnn_slide_features: null argument");
+    if (o->gen != o->h->weight_gen)
+        return fail(B2CNN_ESTATE, "b2cnn_slide_features: the handle's weights changed since the scorer's last reset (stored features are stale)");
+    DEVICE_GUARD(slide_device(o->s));
+    const char *err = "";
+    const int rc = slide_features(o->s, feats, reinterpret_cast<cudaStream_t>(stream), &err);
+    return rc == B2CNN_OK ? rc : fail(rc, std::string("b2cnn_slide_features: ") + err);
 }
 
 // ---- host-pointer entry: chunked H2D overlapped with compute -----------------------------

@@ -1,0 +1,471 @@
+// b2cnn_slide.cu -- sliding-window scorer: P patient streams scored every S samples with the last W samples as the
+// window (the reference's 600 s window sliding by 60 s, bin/predictStream.py:248-252), computing only the features the
+// new samples complete.
+//
+// The front end (conv1 -> pool -> tanh -> conv2 -> pool -> tanh) is translation-equivariant: window feature i of a
+// window starting at sample s reads samples s + 4i .. s + 4i + R - 1 (R = 24 for MyCNN5, 16 for MyCNN2/3/4 geometry).
+// With S % 4 == 0 every window's features lie on one stream lattice: stream feature g starts at sample 4g + phi,
+// phi = (-W) mod 4, and window n (samples [nS - W, nS)) is stream features G_n .. G_n + L - 1, G_n = (nS - W - phi) / 4.
+// Exactly the last L features computed so far, so the ring has L slots, stream feature g in slot g mod L, laid out
+// position-major [slot][P] (rows padded to 4 patients; thread == patient stores coalesce).
+//
+// Per push (segment = samples [(n-1)S, nS) of every patient):
+//   * main features, those whose samples all lie in the segment: tc_stream_kernel's ring store mode (b2cnn_tc.cu)
+//     reading the segment straight from the caller's buffer (first feature at segment sample phi; a segment with
+//     phi != 0 or rows not 16-byte aligned is first copied, shifted by phi, into the scorer's staging rows);
+//   * windows the tensor-core kernel flagged (a NaN / inf sample turns a whole block NaN there) get these features
+//     recomputed by slide_exact_kernel, the generic kernel's fp32 arithmetic term for term;
+//   * seam features, whose receptive field starts in the previous push: slide_exact_kernel again, reading the
+//     last 24 samples of each patient's stream (kept per patient, fp32) in front of the segment;
+//   * once n S >= W: slide_ring_proj_kernel, [P x L] . [L x 64] over the ring on wgmma with window feature j in slot
+//     (G_n + j) mod L, split-K over the streaming kernels' position ranges (they depend on L only) ->
+//     partial[range][P][64]; then the head kernel of the independent forward sums the ranges in fixed order and runs
+//     the LSTM cells, Linear, age scale and sigmoid.
+#include <cstring>
+#include <new>
+
+#include "b2cnn_slide.cuh"
+#include "b2cnn_tc_ptx.cuh"
+
+namespace b2cnn {
+
+constexpr int kSlideTail = 24;       // stream samples kept per patient and channel: the largest receptive field
+
+struct Slide {
+    int device;
+    Dims d;
+    int P, S, dtype, R, phi;
+    int ranges;                      // projection split-K: the streaming kernels' position ranges (TcState, from L only)
+    int64_t n = 0;                   // pushes since the last reset
+    int64_t g_done = -1;             // last stream feature computed (-1: none)
+    int tail_cur = 0;                // which of the two tail buffers holds the current tail
+    float *ring = nullptr;           // [L][ring_pitch]
+    int64_t ring_pitch = 0;          // P rounded up to 4: 16-byte rows for the projection's TMA boxes
+    float *tail = nullptr;           // [2][P][C][kSlideTail]
+    float *partial = nullptr;        // [ranges][P][64]
+    int *flags = nullptr;            // flags [P] | list [P] | count
+    void *stage = nullptr;           // [P][C][Sp] in the window dtype
+    int64_t Sp = 0;
+};
+
+static int64_t fdiv4(int64_t a) { return a >= 0 ? a / 4 : -((-a + 3) / 4); }
+
+template <typename T>
+__device__ __forceinline__ float ld_sample(const T *p);
+template <>
+__device__ __forceinline__ float ld_sample<float>(const float *p) { return __ldg(p); }
+template <>
+__device__ __forceinline__ float ld_sample<__nv_bfloat16>(const __nv_bfloat16 *p) { return __bfloat162float(__ldg(p)); }
+
+struct SlideExactParams {
+    const void *x;                   // the segment, [P][C][pitch]
+    int64_t pitch;
+    const float *tail;               // [P][C][kSlideTail]: the stream samples just before the segment
+    float *ring;
+    int64_t ring_pitch;
+    int cap, P;
+    int64_t g0;                      // first stream feature of the launch
+    int ng;                          // features
+    int64_t seg0;                    // stream index of the segment's first sample
+    int phi;
+    const int *list, *count;         // listed form: only these patients (count read on the device)
+    ConvWeights cw;
+};
+
+// One feature, exact fp32, in the generic kernel's order (b2cnn_generic.cu): conv1 sums channel-major then tap,
+// pooling before bias + tanh with max.NaN, conv2 over the 4 channels then taps.
+template <int C, int K1, int PK, typename Tin>
+__device__ float exact_feature(const SlideExactParams &p, int b, int64_t g) {
+    constexpr int K2 = 5, PS = 2, NA = PK + K2 - 1, NT = PS * (NA - 1) + PK, NX = NT + K1 - 1;
+    const int64_t s0 = 4 * g + p.phi - p.seg0;           // first sample relative to the segment; < 0: in the tail
+    const Tin *xb = reinterpret_cast<const Tin *>(p.x) + (int64_t)b * C * p.pitch;
+    const float *tb = p.tail + (int64_t)b * C * kSlideTail;
+    float xs[C][NX];
+#pragma unroll
+    for (int c = 0; c < C; ++c)
+#pragma unroll
+        for (int i = 0; i < NX; ++i) {
+            const int64_t r = s0 + i;
+            xs[c][i] = r >= 0 ? ld_sample<Tin>(xb + c * p.pitch + r) : tb[c * kSlideTail + kSlideTail + r];
+        }
+    float a1[kCMid][NA];
+#pragma unroll
+    for (int j = 0; j < NA; ++j)
+#pragma unroll
+        for (int o = 0; o < kCMid; ++o) {
+            float m = 0.f;
+#pragma unroll
+            for (int u = 0; u < PK; ++u) {
+                const int t = PS * j + u;
+                float s = 0.f;
+#pragma unroll
+                for (int c = 0; c < C; ++c)
+#pragma unroll
+                    for (int k = 0; k < K1; ++k) s = fmaf(p.cw.w1[(c * K1 + k) * kCMid + o], xs[c][t + k], s);
+                m = u == 0 ? s : max_nan(m, s);
+            }
+            a1[o][j] = tanhf(m + p.cw.b1[o]);
+        }
+    float best = 0.f;
+#pragma unroll
+    for (int u = 0; u < PK; ++u) {
+        float s = 0.f;
+#pragma unroll
+        for (int c = 0; c < kCMid; ++c)
+#pragma unroll
+            for (int k = 0; k < K2; ++k) s = fmaf(p.cw.w2[c * K2 + k], a1[c][u + k], s);
+        best = u == 0 ? s : max_nan(best, s);
+    }
+    return tanhf(best + p.cw.b2);
+}
+
+// all patients: thread x = patient, blockIdx.y = feature; listed: thread x = feature, blockIdx.y strides the list
+template <int C, int K1, int PK, typename Tin>
+__global__ void __launch_bounds__(128) slide_exact_kernel(const __grid_constant__ SlideExactParams p) {
+    auto store = [&](int b, int gi) {
+        const int64_t g = p.g0 + gi;
+        p.ring[(g % p.cap) * p.ring_pitch + b] = exact_feature<C, K1, PK, Tin>(p, b, g);
+    };
+    if (!p.list) {
+        const int b = blockIdx.x * blockDim.x + threadIdx.x;
+        if (b < p.P) store(b, blockIdx.y);
+        return;
+    }
+    const int gi = blockIdx.x * blockDim.x + threadIdx.x;
+    const int nwin = *p.count;
+    if (gi >= p.ng) return;
+    for (int wi = blockIdx.y; wi < nwin; wi += gridDim.y) store(p.list[wi], gi);
+}
+
+// new tail = the last kSlideTail samples of (old tail | segment)
+template <typename Tin>
+__global__ void slide_tail_kernel(const Tin *__restrict__ x, int64_t pitch, int S, const float *__restrict__ tin,
+                                  float *__restrict__ tout, int64_t rows) {
+    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= rows * kSlideTail) return;
+    const int64_t r = e / kSlideTail;
+    const int u = S + (int)(e % kSlideTail);
+    tout[e] = u < kSlideTail ? tin[r * kSlideTail + u] : ld_sample<Tin>(x + r * pitch + (u - kSlideTail));
+}
+
+// segment rows shifted by phi into 16-byte aligned rows of Sp samples (tail zero-filled)
+template <typename T>
+__global__ void slide_stage_kernel(const T *__restrict__ src, int64_t sp, int phi, int n, T *__restrict__ dst, int64_t dp,
+                                   int64_t rows) {
+    const int64_t total = rows * dp;
+    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t r = e / dp, i = e - r * dp;
+        dst[e] = i < n ? src[r * sp + i + phi] : T(0);
+    }
+}
+
+// ---- projection over the ring on the tensor cores -----------------------------------------------------------------
+// The split-K ranges and 16-position chunks are those of the streaming kernels (TcState: feats_per_cta, chunks_per_cta,
+// n_ranges, all from L only), so the packed W_ih chunks of tc_prepare serve unchanged: chunk m of range r holds the
+// weights of window positions r F + 16 m - foff + k (k < 16), zero outside the range.  CTA = (128 patients, range):
+//   warp 4: TMA producer -- per chunk one {128 patients x 16 slots} fp32 box of the ring at the chunk's first slot and,
+//           when the 16 slots wrap past L, a second box at slot 0; plus the 6 KB W_ih chunk (bulk copy); two stages;
+//   warps 0-3: thread == patient: the chunk's 16 features (0 outside the range) split into three bf16 pieces written
+//           as the K-major A tile, then 2 row halves x 6 m64n64k16 piece pairs (hh hm mh hl lh mm, fp32-equivalent
+//           products, as the fused kernel) accumulating partial[range][patient][64] in registers.
+constexpr int kRpThreads = 160;
+constexpr int kRpM = 128;                            // patients per CTA
+constexpr int kRpBox = 16 * kRpM * 4;                // one TMA box: 16 slots x 128 patients fp32
+constexpr int kRpWChunk = 3 * 64 * 16 * 2;           // a packed W_ih chunk (tc_pack_wih_kernel, kFuWChunkBytes)
+constexpr int kRpPiece = kRpM * 16 * 2;              // one bf16 piece of the A tile
+constexpr size_t kRpSmem = 1024 + 2 * 2 * kRpBox + 2 * kRpWChunk + 3 * kRpPiece + 64;
+
+struct RingProjParams {
+    const uint8_t *wpack;            // [n_ranges][chunks_per_cta][kRpWChunk]
+    float *partial;                  // [n_ranges][P][64]
+    int P, L, head, feats_per_cta, chunks_per_cta, foff;
+};
+
+__global__ void __launch_bounds__(kRpThreads, 1)
+slide_ring_proj_kernel(const __grid_constant__ CUtensorMap tm, const __grid_constant__ RingProjParams p) {
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+    float *sF = reinterpret_cast<float *>(smem);                  // [2 stages][2 boxes][16][128]
+    uint8_t *sW = smem + 2 * 2 * kRpBox;                           // [2 stages][6 KB]
+    uint8_t *sPc = sW + 2 * kRpWChunk;                             // [3 pieces][4 KB]
+    uint64_t *bars = reinterpret_cast<uint64_t *>(sPc + 3 * kRpPiece);
+    const uint32_t bar_full = smem_u32(bars + 0), bar_empty = smem_u32(bars + 2);
+    const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);
+    const int lane = threadIdx.x & 31;
+    const int b0 = blockIdx.x * kRpM;
+    const int lo = blockIdx.y * p.feats_per_cta, hi = min(p.L, lo + p.feats_per_cta);
+    const int nch = p.chunks_per_cta;
+    if (threadIdx.x == 0) {
+        for (int i = 0; i < 2; ++i) { mbar_init(bar_full + 8 * i, 1); mbar_init(bar_empty + 8 * i, 4); }
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+    // ring slot of the chunk's first window position (which may lie before 0 or past L: those features are masked)
+    auto first_slot = [&](int m) {
+        int s = (p.head + lo + 16 * m - p.foff) % p.L;
+        return s < 0 ? s + p.L : s;
+    };
+    if (warp == 4) {
+        if (lane == 0) {
+            for (int m = 0; m < nch; ++m) {
+                const int u = m & 1;
+                mbar_wait(bar_empty + 8 * u, ((m >> 1) & 1) ^ 1);
+                const int s0 = first_slot(m);
+                const bool wraps = s0 + 16 > p.L;
+                mbar_expect_tx(bar_full + 8 * u, (wraps ? 2 : 1) * kRpBox + kRpWChunk);
+                const uint32_t dst = smem_u32(sF + (size_t)u * 2 * 16 * kRpM);
+                tma_load_2d(dst, &tm, b0, s0, bar_full + 8 * u);
+                if (wraps) tma_load_2d(dst + kRpBox, &tm, b0, 0, bar_full + 8 * u);
+                bulk_load_1d(smem_u32(sW + u * kRpWChunk), p.wpack + ((size_t)blockIdx.y * nch + m) * kRpWChunk, kRpWChunk,
+                             bar_full + 8 * u);
+            }
+        }
+        return;
+    }
+    const int row = threadIdx.x;
+    float gacc[2][32];
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int i = 0; i < 32; ++i) gacc[h][i] = 0.f;
+    uint8_t *arow = sPc + (row >> 3) * 256 + (row & 7) * 16;
+#pragma unroll 1
+    for (int m = 0; m < nch; ++m) {
+        const int u = m & 1;
+        mbar_wait(bar_full + 8 * u, (m >> 1) & 1);
+        const int s0 = first_slot(m), q0 = lo + 16 * m - p.foff;
+        const float *fa = sF + (size_t)u * 2 * 16 * kRpM, *fb = fa + 16 * kRpM;
+        auto feat = [&](int k) {
+            const int q = q0 + k;
+            if (q < lo || q >= hi) return 0.f;
+            return s0 + k < p.L ? fa[k * kRpM + row] : fb[(s0 + k - p.L) * kRpM + row];
+        };
+#pragma unroll
+        for (int kk = 0; kk < 8; ++kk) {
+            const float f0 = feat(2 * kk), f1 = feat(2 * kk + 1);
+            const uint32_t h = pack_bf16x2(f0, f1);
+            const float r1x = f0 - __uint_as_float(h << 16), r1y = f1 - __uint_as_float(h & 0xffff0000u);
+            const uint32_t md = pack_bf16x2(r1x, r1y);
+            const uint32_t lw = pack_bf16x2(r1x - __uint_as_float(md << 16), r1y - __uint_as_float(md & 0xffff0000u));
+            const int off = (kk >> 2) * 128 + (kk & 3) * 4;
+            *reinterpret_cast<uint32_t *>(arow + off) = h;
+            *reinterpret_cast<uint32_t *>(arow + kRpPiece + off) = md;
+            *reinterpret_cast<uint32_t *>(arow + 2 * kRpPiece + off) = lw;
+        }
+        fence_proxy_async();
+        wg_bar();
+        const uint32_t pa = smem_u32(sPc), pw = smem_u32(sW + u * kRpWChunk);
+        wgmma_fence();
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+            constexpr int kAp[6] = {0, 0, 1, 0, 2, 1}, kWp[6] = {0, 1, 0, 2, 0, 1};
+#pragma unroll
+            for (int q = 0; q < 6; ++q)
+                wgmma_m64n64(gacc[hh], gdesc_none_kmajor(pa + kAp[q] * kRpPiece + hh * 2048, 128, 256),
+                             gdesc_none_kmajor(pw + kWp[q] * 2048, 128, 256));
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        __syncwarp();
+        if (lane == 0) mbar_arrive(bar_empty + 8 * u);
+        wg_bar();                                                  // A tile free for the next chunk
+    }
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh)
+#pragma unroll
+        for (int e2 = 0; e2 < 2; ++e2) {
+            const int bb = b0 + 64 * hh + 16 * warp + (lane >> 2) + 8 * e2;
+            if (bb < p.P) {
+                float *dst = p.partial + ((int64_t)blockIdx.y * p.P + bb) * kGates + 2 * (lane & 3);
+#pragma unroll
+                for (int e = 2 * e2; e < 32; e += 4)
+                    *reinterpret_cast<float2 *>(dst + 8 * (e >> 2)) = make_float2(gacc[hh][e], gacc[hh][e + 1]);
+            }
+        }
+}
+
+// feats[b][j] = ring[(head + j) mod cap][b]
+__global__ void slide_gather_kernel(const float *__restrict__ ring, int64_t pitch, int cap, int P, int head, int L,
+                                    float *__restrict__ feats) {
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= P) return;
+    for (int j = blockIdx.y; j < L; j += gridDim.y) feats[(int64_t)b * L + j] = ring[(int64_t)((head + j) % cap) * pitch + b];
+}
+
+// ------------------------------------------------------------------------------------------
+template <int C, int K1, int PK>
+static void launch_exact_t(const SlideExactParams &p, int dtype, dim3 grid, cudaStream_t st) {
+    if (dtype == B2CNN_DTYPE_F32) slide_exact_kernel<C, K1, PK, float><<<grid, 128, 0, st>>>(p);
+    else slide_exact_kernel<C, K1, PK, __nv_bfloat16><<<grid, 128, 0, st>>>(p);
+}
+
+// features [g0, g0 + ng) exactly: of every patient (list == nullptr) or of the listed ones
+static int launch_exact(const Slide &s, const ConvWeights &cw, const void *x, int64_t pitch, const float *tail, int64_t g0,
+                        int64_t ng, const int *list, const int *count, cudaStream_t st, const char **err) {
+    if (ng <= 0) return 0;
+    SlideExactParams p;
+    memset(&p, 0, sizeof p);
+    p.x = x; p.pitch = pitch; p.tail = tail; p.ring = s.ring; p.ring_pitch = s.ring_pitch; p.cap = s.d.L; p.P = s.P;
+    p.g0 = g0; p.ng = (int)ng; p.seg0 = s.n * s.S; p.phi = s.phi; p.list = list; p.count = count; p.cw = cw;
+    const dim3 grid = list ? dim3((unsigned)((ng + 127) / 128), 16) : dim3((unsigned)((s.P + 127) / 128), (unsigned)ng);
+    const int key = s.d.C * 10 + (s.d.K1 == 10 ? 0 : 1);
+    switch (key) {
+        case 10: launch_exact_t<1, 10, 3>(p, s.dtype, grid, st); break;
+        case 20: launch_exact_t<2, 10, 3>(p, s.dtype, grid, st); break;
+        case 30: launch_exact_t<3, 10, 3>(p, s.dtype, grid, st); break;
+        case 11: launch_exact_t<1, 5, 2>(p, s.dtype, grid, st); break;
+        case 21: launch_exact_t<2, 5, 2>(p, s.dtype, grid, st); break;
+        case 31: launch_exact_t<3, 5, 2>(p, s.dtype, grid, st); break;
+        default: *err = "no exact feature kernel for this geometry"; return -1;
+    }
+    if (cudaGetLastError() != cudaSuccess) { *err = "exact feature kernel launch"; return -1; }
+    return 1;
+}
+
+int slide_create(const Dims &d, const TcState &tc, int n_patients, int stride, int dtype, int device, Slide **out,
+                 const char **err) {
+    *out = nullptr;
+    if (dtype != B2CNN_DTYPE_F32 && dtype != B2CNN_DTYPE_BF16) { *err = "dtype must be f32 (0) or bf16 (1)"; return B2CNN_EINVAL; }
+    if (n_patients < 1 || n_patients > (1 << 24)) { *err = "n_patients out of range"; return B2CNN_EINVAL; }
+    if (stride < 1 || stride > d.W) { *err = "stride must be in [1, window]"; return B2CNN_EINVAL; }
+    if (stride % 4 != 0) { *err = "stride must be a multiple of the feature stride (4 samples)"; return B2CNN_EINVAL; }
+    if (!tc_ring_supported(tc, d)) {
+        *err = "the sliding-window scorer covers the streaming tensor-core geometries only (MyCNN5 or MyCNN2/3/4 conv/pool, "
+               "1 to 3 channels, tanh, no affine)";
+        return B2CNN_EARCH;
+    }
+    Slide *s = new (std::nothrow) Slide();
+    if (!s) { *err = "out of host memory"; return B2CNN_ESTATE; }
+    s->device = device; s->d = d; s->P = n_patients; s->S = stride; s->dtype = dtype;
+    s->R = d.K1 == 10 ? 24 : 16;
+    s->phi = (4 - d.W % 4) % 4;
+    s->ranges = tc.n_ranges;
+    s->ring_pitch = (n_patients + 3) & ~3;
+    s->Sp = (stride + 7) & ~7;
+    const int64_t P = n_patients, esz = dtype == B2CNN_DTYPE_BF16 ? 2 : 4;
+    bool ok = cudaMalloc(&s->ring, sizeof(float) * (size_t)d.L * s->ring_pitch) == cudaSuccess &&
+              cudaMalloc(&s->tail, sizeof(float) * (size_t)2 * P * d.C * kSlideTail) == cudaSuccess &&
+              cudaMalloc(&s->partial, sizeof(float) * (size_t)s->ranges * P * kGates) == cudaSuccess &&
+              cudaMalloc(&s->flags, sizeof(int) * (size_t)(2 * P + 1)) == cudaSuccess &&
+              cudaMalloc(&s->stage, (size_t)(P * d.C * s->Sp * esz)) == cudaSuccess;
+    if (!ok) { (void)cudaGetLastError(); slide_destroy(s); *err = "cudaMalloc(scorer state)"; return B2CNN_ECUDA; }
+    *out = s;
+    return B2CNN_OK;
+}
+
+void slide_destroy(Slide *s) {
+    if (!s) return;
+    cudaFree(s->ring); cudaFree(s->tail); cudaFree(s->partial); cudaFree(s->flags); cudaFree(s->stage);
+    delete s;
+}
+
+int slide_device(const Slide *s) { return s->device; }
+
+int slide_reset(Slide *s, cudaStream_t st, const char **err) {
+    s->n = 0; s->g_done = -1; s->tail_cur = 0;
+    if (cudaMemsetAsync(s->tail, 0, sizeof(float) * (size_t)2 * s->P * s->d.C * kSlideTail, st) != cudaSuccess) {
+        *err = "memset tail"; return B2CNN_ECUDA;
+    }
+    return B2CNN_OK;
+}
+
+static int64_t window_head(const Slide &s, int64_t n) { return fdiv4(n * s.S - s.d.W - s.phi); }
+
+int slide_push(Slide *s, const ConvWeights &cw, const HeadWeights &hw, const TcState &tc, const void *x, int64_t pitch,
+               const float *age, int64_t n_age, int apply_sigmoid, float *out, int *emitted, int64_t *window_index,
+               cudaEvent_t *ev, cudaStream_t st, const char **err) {
+    const Dims &d = s->d;
+    const int64_t P = s->P, S = s->S, esz = s->dtype == B2CNN_DTYPE_BF16 ? 2 : 4;
+    if (pitch < S) { *err = "pitch must be >= stride"; return B2CNN_EINVAL; }
+    if (n_age != 1 && n_age != P) { *err = "age must have 1 or n_patients elements"; return B2CNN_EINVAL; }
+    const int64_t n1 = s->n + 1;
+    const int64_t g_hi = fdiv4(n1 * S - s->R - s->phi);      // last feature whose samples have all arrived
+    const int64_t g_m0 = s->n * S / 4;                        // first feature that starts inside the segment
+    int64_t g_lo = s->g_done + 1;
+    const int64_t G = window_head(*s, n1);
+    if (g_lo < G) g_lo = G;                                   // earlier features never enter a window
+    if (g_lo < 0) g_lo = 0;
+    const float *tail_in = s->tail + (size_t)s->tail_cur * P * d.C * kSlideTail;
+    float *tail_out = s->tail + (size_t)(s->tail_cur ^ 1) * P * d.C * kSlideTail;
+    if (ev && cudaEventRecord(ev[0], st) != cudaSuccess) { *err = "cudaEventRecord"; return B2CNN_ECUDA; }
+
+    // ---- main features [g_m0, g_hi]: tensor cores from the segment, exact re-computation of flagged patients
+    const int64_t Q = g_hi - g_m0 + 1;
+    if (Q >= 32) {
+        const int unit = 16 / (int)esz;
+        const void *xin = x;
+        int64_t xp = pitch;
+        if (s->phi != 0 || pitch % unit != 0 || (reinterpret_cast<uintptr_t>(x) & 15) != 0) {
+            const int64_t rows = P * d.C;
+            const unsigned blocks = (unsigned)((rows * s->Sp + 255) / 256 < 65536 ? (rows * s->Sp + 255) / 256 : 65536);
+            if (esz == 2)
+                slide_stage_kernel<uint16_t><<<blocks, 256, 0, st>>>(reinterpret_cast<const uint16_t *>(x), pitch, s->phi, (int)(S - s->phi),
+                                                                     reinterpret_cast<uint16_t *>(s->stage), s->Sp, rows);
+            else
+                slide_stage_kernel<float><<<blocks, 256, 0, st>>>(reinterpret_cast<const float *>(x), pitch, s->phi, (int)(S - s->phi),
+                                                                  reinterpret_cast<float *>(s->stage), s->Sp, rows);
+            if (cudaGetLastError() != cudaSuccess) { *err = "staging launch"; return B2CNN_ECUDA; }
+            xin = s->stage; xp = s->Sp;
+        }
+        Dims dseg = d;
+        dseg.W = (int)(S - s->phi); dseg.L = (int)Q; dseg.XP = (int)xp;
+        if (cudaMemsetAsync(s->flags, 0, sizeof(int) * (size_t)(2 * P + 1), st) != cudaSuccess) { *err = "memset flags"; return B2CNN_ECUDA; }
+        if (tc_ring_features(tc, dseg, cw, xin, xp, s->dtype, P, s->ring, s->ring_pitch, d.L, (int)(g_m0 % d.L), s->flags, st, err) < 0)
+            return B2CNN_ECUDA;
+        if (launch_exact(*s, cw, x, pitch, tail_in, g_m0, Q, s->flags + P, s->flags + 2 * P, st, err) < 0) return B2CNN_ECUDA;
+    } else if (launch_exact(*s, cw, x, pitch, tail_in, g_m0, Q, nullptr, nullptr, st, err) < 0) {
+        return B2CNN_ECUDA;
+    }
+    // ---- seam features [g_lo, g_m0 - 1]: receptive field starts in the previous push
+    const int64_t seam_hi = g_hi < g_m0 - 1 ? g_hi : g_m0 - 1;
+    if (launch_exact(*s, cw, x, pitch, tail_in, g_lo, seam_hi - g_lo + 1, nullptr, nullptr, st, err) < 0) return B2CNN_ECUDA;
+    {
+        const int64_t rows = P * d.C, total = rows * kSlideTail;
+        if (esz == 2)
+            slide_tail_kernel<__nv_bfloat16><<<(unsigned)((total + 255) / 256), 256, 0, st>>>(
+                reinterpret_cast<const __nv_bfloat16 *>(x), pitch, (int)S, tail_in, tail_out, rows);
+        else
+            slide_tail_kernel<float><<<(unsigned)((total + 255) / 256), 256, 0, st>>>(reinterpret_cast<const float *>(x), pitch, (int)S,
+                                                                                    tail_in, tail_out, rows);
+        if (cudaGetLastError() != cudaSuccess) { *err = "tail launch"; return B2CNN_ECUDA; }
+    }
+    if (ev && cudaEventRecord(ev[1], st) != cudaSuccess) { *err = "cudaEventRecord"; return B2CNN_ECUDA; }
+    s->n = n1;
+    if (g_hi >= g_lo) s->g_done = g_hi;
+    s->tail_cur ^= 1;
+
+    // ---- projection over the ring + head, once the first window is complete
+    *emitted = 0;
+    if (n1 * S < d.W) {
+        if (ev && cudaEventRecord(ev[2], st) != cudaSuccess) { *err = "cudaEventRecord"; return B2CNN_ECUDA; }
+        return B2CNN_OK;
+    }
+    const int head = (int)(G % d.L);
+    if (tc.n_ranges != s->ranges) { *err = "the handle's position ranges changed since create"; return B2CNN_ESTATE; }
+    CUtensorMap tm;
+    if (tc_ring_tmap(s->ring, P, s->ring_pitch, d.L, &tm, err) != 0) return B2CNN_ECUDA;
+    RingProjParams rp;
+    rp.wpack = reinterpret_cast<const uint8_t *>(tc.d_wpack); rp.partial = s->partial;
+    rp.P = (int)P; rp.L = d.L; rp.head = head;
+    rp.feats_per_cta = tc.feats_per_cta; rp.chunks_per_cta = tc.chunks_per_cta; rp.foff = d.K1 == 10 ? 3 : 2;
+    if (cudaFuncSetAttribute(slide_ring_proj_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kRpSmem) != cudaSuccess) {
+        *err = "projection smem attribute"; return B2CNN_ECUDA;
+    }
+    slide_ring_proj_kernel<<<dim3((unsigned)((P + kRpM - 1) / kRpM), (unsigned)s->ranges), kRpThreads, kRpSmem, st>>>(tm, rp);
+    if (cudaGetLastError() != cudaSuccess) { *err = "projection launch"; return B2CNN_ECUDA; }
+    if (launch_reduce_lstm_head(d, hw, s->partial, s->ranges, P, age, n_age, apply_sigmoid, out, st, err) < 0) return B2CNN_ECUDA;
+    if (ev && cudaEventRecord(ev[2], st) != cudaSuccess) { *err = "cudaEventRecord"; return B2CNN_ECUDA; }
+    *emitted = 1;
+    *window_index = n1 - (d.W + S - 1) / S;
+    return B2CNN_OK;
+}
+
+int slide_features(const Slide *s, float *feats, cudaStream_t st, const char **err) {
+    if (s->n * s->S < s->d.W) { *err = "no window yet: the first window is still filling"; return B2CNN_ESTATE; }
+    const int head = (int)(window_head(*s, s->n) % s->d.L);
+    slide_gather_kernel<<<dim3((unsigned)((s->P + 127) / 128), 64), 128, 0, st>>>(s->ring, s->ring_pitch, s->d.L, s->P, head, s->d.L, feats);
+    if (cudaGetLastError() != cudaSuccess) { *err = "gather launch"; return B2CNN_ECUDA; }
+    return B2CNN_OK;
+}
+
+}  // namespace b2cnn

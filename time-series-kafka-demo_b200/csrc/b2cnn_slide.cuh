@@ -1,0 +1,20 @@
+// b2cnn_slide.cuh -- interface of the sliding-window scorer, b2cnn_slide.cu (b2cnn_slide_* in include/b2cnn.h).
+#pragma once
+#include "b2cnn_tc.cuh"
+
+namespace b2cnn {
+
+struct Slide;
+// `d`: the model's geometry; the scorer keeps a copy.  Checks stride and geometry, allocates all device state.
+int slide_create(const Dims &d, const TcState &tc, int n_patients, int stride, int dtype, int device, Slide **out,
+                 const char **err);
+void slide_destroy(Slide *s);
+int slide_device(const Slide *s);
+int slide_reset(Slide *s, cudaStream_t st, const char **err);
+// ev: nullptr, or three events recorded at the start, after the front end and after the head (profiling)
+int slide_push(Slide *s, const ConvWeights &cw, const HeadWeights &hw, const TcState &tc, const void *x, int64_t pitch,
+               const float *age, int64_t n_age, int apply_sigmoid, float *out, int *emitted, int64_t *window_index,
+               cudaEvent_t *ev, cudaStream_t st, const char **err);
+int slide_features(const Slide *s, float *feats, cudaStream_t st, const char **err);
+
+}  // namespace b2cnn

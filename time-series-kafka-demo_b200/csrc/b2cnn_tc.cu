@@ -428,6 +428,57 @@ int tc_fused_gates(TcState &s, const Dims &d, const ConvWeights &cw, const HeadW
     return launches + n;
 }
 
+bool tc_ring_supported(const TcState &s, const Dims &d) { return s.ready && s.fused_ready && (arch_ok(d) || arch1_ok(d)) && d.C <= 3; }
+
+// 2-D map of a scorer's feature ring [L][pitch] fp32 (pitch % 4 == 0): boxes of 16 positions x 128 patients
+int tc_ring_tmap(const float *ring, int64_t P, int64_t pitch, int L, CUtensorMap *tm, const char **err) {
+    if (!get_encode()) { *err = "cuTensorMapEncodeTiled unavailable"; return -1; }
+    cuuint64_t gdim[2] = {(cuuint64_t)P, (cuuint64_t)L};
+    cuuint64_t gstr[1] = {(cuuint64_t)pitch * 4};
+    cuuint32_t box[2] = {kTcM, 16};
+    cuuint32_t estr[2] = {1, 1};
+    CUresult r = get_encode()(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float *>(ring), gdim, gstr, box, estr,
+                              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) { *err = "cuTensorMapEncodeTiled(ring) failed"; return -1; }
+    return 0;
+}
+
+// The new features of a sliding-window scorer (b2cnn_slide.cu) straight into its position-major ring.  `dseg`
+// describes the segment from its first feature's first sample (W = samples, L = features, C); x: 16-byte aligned,
+// `pitch` a multiple of 16 bytes.  flags [P] (zeroed by the caller) | list [P] | count: windows whose features
+// may hold a tensor-core NaN, compacted for the exact re-computation.  Returns the launch count.
+int tc_ring_features(const TcState &s, const Dims &dseg, const ConvWeights &cw, const void *x, int64_t pitch, int dtype,
+                     int64_t P, float *ring, int64_t ring_pitch, int cap, int slot0, int *flags, cudaStream_t st, const char **err) {
+    const bool f32 = dtype == B2CNN_DTYPE_F32;
+    CUtensorMap tm;
+    if (make_tmap(dseg, x, pitch, P, f32, &tm, err) != 0) return -1;
+    TcFusedParams p;
+    memset(&p, 0, sizeof p);
+    p.feats = ring; p.sB = 1; p.sP = ring_pitch; p.nanflag = flags;
+    p.ring_slot0 = slot0; p.ring_cap = cap;
+    p.bmats = reinterpret_cast<const uint8_t *>(s.d_bmats);
+    p.B = (int)P; p.W = dseg.W; p.L = dseg.L;
+    p.tiles_per_cta = tiles_per_cta_for(dseg);
+    p.feats_per_cta = 2 * kTcBlocks * p.tiles_per_cta - 4;
+    fill_epilogue(p, dseg, cw);
+    dim3 grid((unsigned)((P + kTcM - 1) / kTcM), (dseg.L + p.feats_per_cta - 1) / p.feats_per_cta);
+    const int key = dseg.C * 100 + (f32 ? 10 : 0) + (dseg.K1 == 10 ? 0 : 1);
+    cudaError_t e;
+    switch (key) {
+#define RING_CASE(CC, FF, AA) case CC * 100 + FF * 10 + AA: e = launch_stream<CC, FF ? 1 : 3, AA, FF == 1, kOutRing>(tm, p, grid, st); break;
+        RING_CASE(1, 0, 0) RING_CASE(2, 0, 0) RING_CASE(3, 0, 0) RING_CASE(1, 0, 1) RING_CASE(2, 0, 1) RING_CASE(3, 0, 1)
+        RING_CASE(1, 1, 0) RING_CASE(2, 1, 0) RING_CASE(3, 1, 0) RING_CASE(1, 1, 1) RING_CASE(2, 1, 1) RING_CASE(3, 1, 1)
+#undef RING_CASE
+        default: *err = "no feature-ring instantiation for this channel count"; return -1;
+    }
+    if (e != cudaSuccess) { *err = cudaGetErrorString(e); return -1; }
+    int *list = flags + P, *count = list + P;
+    tc_compact_flags_kernel<<<(unsigned)((P + 255) / 256), 256, 0, st>>>(flags, (int)P, list, count);
+    if (cudaGetLastError() != cudaSuccess) { *err = "flag compaction launch"; return -1; }
+    return 2;
+}
+
 bool tc_stream_supported(const TcState &s, const Dims &d, int dtype) {
     return s.ready && s.fused_ready && dtype == B2CNN_DTYPE_F32 && (arch_ok(d) || arch1_ok(d)) && d.C <= 3 && (d.XP % 4) == 0;
 }

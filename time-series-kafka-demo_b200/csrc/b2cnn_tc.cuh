@@ -1,5 +1,7 @@
 // b2cnn_tc.cuh -- interface of the wgmma (Hopper tensor core) fast path, b2cnn_tc.cu.
 #pragma once
+#include <cuda.h>
+
 #include "b2cnn_internal.cuh"
 
 namespace b2cnn {
@@ -54,5 +56,10 @@ int tc_stream_gates(TcState &s, const Dims &d, const ConvWeights &cw, const Head
                     bool reduce_here = true, int *slices_out = nullptr);
 int tc_features(TcState &s, const Dims &d, const ConvWeights &cw, const void *x, int64_t B, float *feats,
                 int num_sms, cudaStream_t st, const char **err);
+// sliding-window scorer (b2cnn_slide.cu): a segment's features into the position-major feature ring
+bool tc_ring_supported(const TcState &s, const Dims &d);
+int tc_ring_features(const TcState &s, const Dims &dseg, const ConvWeights &cw, const void *x, int64_t pitch, int dtype,
+                     int64_t P, float *ring, int64_t ring_pitch, int cap, int slot0, int *flags, cudaStream_t st, const char **err);
+int tc_ring_tmap(const float *ring, int64_t P, int64_t pitch, int L, CUtensorMap *tm, const char **err);
 
 }  // namespace b2cnn

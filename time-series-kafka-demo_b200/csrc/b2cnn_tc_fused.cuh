@@ -35,7 +35,10 @@ constexpr int kHpTStride = 36;                    // floats per window row of th
 constexpr int kHpTBytes = kTcM * kHpTStride * 4;
 constexpr int kHpPieceBytes = kTcM * 16 * 2;      // one bf16 piece of the projection A operand
 constexpr int kFuWChunkBytes = 3 * 64 * 16 * 2;   // 3 pieces x (64 gates x 16 positions) bf16
-constexpr int kOutFeatures = 0, kOutGates = 1;
+// kOutRing: the features of a sliding-window scorer's new segment (b2cnn_slide.cu) into its position-major
+// feature ring, feats[((ring_slot0 + p) mod ring_cap) * sP + b]: thread == window, so a warp stores 32
+// consecutive floats per position.
+constexpr int kOutFeatures = 0, kOutGates = 1, kOutRing = 2;
 
 struct TcFusedParams {
     float *partial;           // [n_ranges][B][64]                 (kOutGates)
@@ -52,6 +55,7 @@ struct TcFusedParams {
     float b1s[kCMid];               // conv1 bias * 2 log2 e
     float w2n[kCMid][5];            // -2 * conv2 weights
     float b2s;                      // (conv2 bias + sum of conv2 weights) * 2 log2 e
+    int ring_slot0, ring_cap;       // kOutRing: ring slot of feature 0, slots in the ring
 };
 
 __host__ __device__ constexpr size_t hp_smem_bytes(int C, int SPLITS, bool f32in, int out) {
@@ -295,6 +299,18 @@ tc_stream_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant
                     if (pr0 >= 0 && pr0 < nfeat) fout[(int64_t)pr0 * p.sP] = f0;
                     if (pr0 + 1 >= 0 && pr0 + 1 < nfeat) fout[(int64_t)(pr0 + 1) * p.sP] = f1;
                 }
+            } else if constexpr (OUT == kOutRing) {
+                nan_probe = fmaf(f0, 0.f, nan_probe);
+                nan_probe = fmaf(f1, 0.f, nan_probe);
+                const int pr0 = 2 * j - FOFF;
+                if (row_ok) {
+                    // p0 + pr < L <= ring_cap and ring_slot0 < ring_cap: one subtraction wraps the slot
+                    int slot = p.ring_slot0 + p0 + pr0;
+                    if (slot >= p.ring_cap) slot -= p.ring_cap;
+                    if (pr0 >= 0 && pr0 < nfeat) p.feats[(int64_t)slot * p.sP + b] = f0;
+                    if (++slot == p.ring_cap) slot = 0;
+                    if (pr0 + 1 >= 0 && pr0 + 1 < nfeat) p.feats[(int64_t)slot * p.sP + b] = f1;
+                }
             } else {
                 // three bf16 pieces of (f0, f1) -> word kk of this window's row of the A tiles
                 const int kk = j & 7, m = j >> 3, u = m & 1;
@@ -335,7 +351,7 @@ tc_stream_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant
             }
         }
 
-        if constexpr (OUT == kOutFeatures) {
+        if constexpr (OUT != kOutGates) {
             if (row_ok && nan_probe != nan_probe) p.nanflag[b] = 1;
         } else {
             // gate pre-activations of this CTA's position range -> partial[range][window][64].  A NaN feature (a NaN / inf

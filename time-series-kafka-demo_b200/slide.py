@@ -1,0 +1,130 @@
+"""``SlidingScorer`` -- long waveform windows scored incrementally (libb2cnn's b2cnn_slide_*, csrc/b2cnn_slide.cu).
+
+The reference scores every patient with a window of the last W samples that slides by S samples
+(bin/predictStream.py:248-252: 600 s every 60 s).  Instead of keeping a ``[P, C, W]`` buffer, shifting it and calling
+``predict()`` on whole windows, a scorer keeps every patient's window features on the device; each ``push`` brings the
+S new samples of all patients, computes only the features they complete and scores the P windows::
+
+    scorer = SlidingScorer(model, n_patients=P, stride=7500)         # 60 s at 125 Hz
+    for samples in triggers:                                         # [P, C, 7500] on the device
+        logits = scorer.push(samples, age=ages)                      # None until the first W samples arrived
+"""
+from __future__ import annotations
+
+import ctypes
+
+import torch
+
+from . import capi
+
+
+class SlidingScorer:
+    """P independent patient streams scored with the model's window ``W = model.arch.window`` every ``stride``
+    samples.  After push n (from 1) a patient's window is the last W samples of its stream; ``push`` returns the
+    ``Tensor[P]`` of ``predict(window, age, mode="independent")`` from the first push with ``n * stride >= W`` on,
+    ``None`` before.  ``dtype`` is the dtype of the pushed samples (``torch.bfloat16`` or ``torch.float32``)."""
+
+    def __init__(self, model, n_patients: int, stride: int, dtype=torch.bfloat16):
+        if dtype not in (torch.bfloat16, torch.float32):
+            raise ValueError("dtype must be torch.bfloat16 or torch.float32")
+        n_patients, stride = int(n_patients), int(stride)
+        if n_patients < 1:
+            raise ValueError(f"n_patients must be >= 1, got {n_patients}")
+        W = model.arch.window
+        if stride < 1 or stride > W or stride % 4:
+            raise ValueError(f"stride must be a multiple of 4 in [4, {W}] (the window), got {stride}")
+        self.model, self.n_patients, self.stride, self.dtype = model, n_patients, stride, dtype
+        self.channels, self.window = model.arch.in_channels, W
+        self._lib, h = model._ensure_handle()
+        self._hv = h.value
+        self.device = model._handle_device
+        s = ctypes.c_void_p()
+        with torch.cuda.device(self.device):
+            capi.check(self._lib.b2cnn_slide_create(h, n_patients, stride, self._dt(), ctypes.byref(s)), "b2cnn_slide_create")
+        self._s = s
+        self.window_index = -1
+
+    def _dt(self) -> int:
+        return capi.DTYPE_BF16 if self.dtype == torch.bfloat16 else capi.DTYPE_F32
+
+    def close(self):
+        s, self._s = getattr(self, "_s", None), None
+        if s is not None:
+            self._lib.b2cnn_slide_destroy(s)
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def _handle(self):
+        # weight changes made through the model reach the library here; the library then refuses pushes until reset()
+        _, h = self.model._ensure_handle()
+        if h.value != self._hv:
+            raise RuntimeError("the model's library handle was replaced (device change); create a new SlidingScorer")
+        if self._s is None:
+            raise RuntimeError("SlidingScorer is closed")
+
+    def reset(self):
+        """Forget all streams (the next push is push 1 again) and take the model's current weights."""
+        self._handle()
+        with torch.cuda.device(self.device):
+            capi.check(self._lib.b2cnn_slide_reset(self._s, torch.cuda.current_stream().cuda_stream), "b2cnn_slide_reset")
+        self.window_index = -1
+
+    def check_samples(self, samples: torch.Tensor) -> int:
+        """Validates a push's ``[P, C, stride]`` tensor; returns its row pitch in elements."""
+        if not torch.is_tensor(samples) or samples.dim() != 3:
+            raise RuntimeError(f"expected samples [{self.n_patients}, {self.channels}, {self.stride}], got "
+                               f"{tuple(samples.shape) if torch.is_tensor(samples) else type(samples).__name__}")
+        if tuple(samples.shape) != (self.n_patients, self.channels, self.stride):
+            raise RuntimeError(f"expected samples [{self.n_patients}, {self.channels}, {self.stride}], got {tuple(samples.shape)}")
+        if samples.dtype != self.dtype:
+            raise RuntimeError(f"expected {self.dtype} samples (the scorer's dtype), got {samples.dtype}")
+        if samples.is_contiguous():
+            return self.stride
+        # a row-padded view ([P, C, Sp][:, :, :S]) is read in place whatever its alignment: the library copies unaligned
+        # rows into its staging rows itself, so a contiguous copy here would copy the segment twice
+        if samples.device.type == "cuda" and samples.stride(2) == 1 and samples.stride(1) >= self.stride \
+                and (self.n_patients == 1 or samples.stride(0) == self.channels * samples.stride(1)):
+            return samples.stride(1)
+        return 0
+
+    @torch.no_grad()
+    def push(self, samples: torch.Tensor, age=65.0, return_prob: bool = False):
+        """``samples`` [P, C, stride] of the scorer's dtype (a row-padded view is read in place, like ``predict``);
+        ``age`` scalar or [P].  Returns the logits (or probabilities) of the P current windows, or ``None`` while the
+        first window fills."""
+        pitch = self.check_samples(samples)
+        self._handle()
+        if samples.device != self.device:
+            samples = samples.to(self.device)
+            pitch = self.stride if samples.is_contiguous() else pitch
+        if not pitch:
+            samples, pitch = samples.contiguous(), self.stride
+        if not torch.is_tensor(age):
+            age = torch.tensor(float(age), dtype=torch.float32)
+        age = age.detach().reshape(-1).to(device=self.device, dtype=torch.float32).contiguous()
+        if age.numel() not in (1, self.n_patients):
+            raise RuntimeError(f"age must be a scalar or have {self.n_patients} elements")
+        em, widx = ctypes.c_int32(0), ctypes.c_int64(-1)
+        out = torch.empty(self.n_patients, dtype=torch.float32, device=self.device)
+        with torch.cuda.device(self.device):
+            st = torch.cuda.current_stream().cuda_stream
+            capi.check(self._lib.b2cnn_slide_push(self._s, samples.data_ptr(), pitch, age.data_ptr(), age.numel(), int(return_prob),
+                                                  out.data_ptr(), ctypes.byref(em), ctypes.byref(widx), st), "b2cnn_slide_push")
+        if not em.value:
+            return None
+        self.window_index = int(widx.value)
+        return out
+
+    @torch.no_grad()
+    def features(self) -> torch.Tensor:
+        """[P, L] fp32: the stored features of the current windows in window order (== ``model.features(window)``)."""
+        self._handle()
+        feats = torch.empty(self.n_patients, self.model.arch.l_out, dtype=torch.float32, device=self.device)
+        with torch.cuda.device(self.device):
+            capi.check(self._lib.b2cnn_slide_features(self._s, feats.data_ptr(), torch.cuda.current_stream().cuda_stream),
+                       "b2cnn_slide_features")
+        return feats
