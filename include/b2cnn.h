@@ -88,9 +88,13 @@ int b2cnn_set_weights(b2cnn_handle *h, const float *blob, int64_t n_floats, int 
                       void *stream);
 
 /* Bytes of caller-provided device scratch b2cnn_forward needs for a batch of B windows.
- * b2cnn_workspace_bytes is dtype-blind (enough for any path, the generic path's [B][L_out] feature rows included);
- * b2cnn_workspace_bytes_for is exact for windows of `dtype`: where the streaming tensor-core kernels apply, the
- * features never leave the SM and the scratch is the range partials only (39 MB instead of 346 MB at [4096,3,75000]). */
+ * b2cnn_workspace_bytes is dtype-blind: enough for any path and any row pitch, the generic path's [B][L_out] feature
+ * rows and, where the tensor-core kernels exist for the handle, the B*C*round_up(W,8) bf16 staging rows included
+ * (also when W % 8 == 0: a bf16 b2cnn_forward_pitched call whose x_pitch is not a multiple of 8 needs them);
+ * b2cnn_workspace_bytes_for is exact for contiguous windows of `dtype`: where the streaming tensor-core kernels apply,
+ * the features never leave the SM and the scratch is the range partials only (39 MB instead of 346 MB at
+ * [4096,3,75000]).  A pitched call with rows that are not a multiple of 16 bytes may need more than the _for size;
+ * it is refused with B2CNN_ESTATE instead. */
 int64_t b2cnn_workspace_bytes(b2cnn_handle *h, int64_t B, int mode);
 int64_t b2cnn_workspace_bytes_for(b2cnn_handle *h, int64_t B, int mode, int dtype);
 
@@ -123,7 +127,6 @@ int b2cnn_features(b2cnn_handle *h, const void *x, int dtype, int64_t B, float *
 
 /* Options: "path" = B2CNN_PATH_*; "tc_splits" = 2|3: bf16 pieces per fp32 conv1 weight on the
  * tensor cores (3, default: exact fp32 weights; 2: weights rounded to 16 mantissa bits);
- * "stream_f32" = 0|1 (default 1): fp32 windows take the streaming kernel instead of the generic one;
  * "tc_fused" = 0|1 (default 1): bf16 windows take the fused conv+projection kernel; "small_kernel" = 0|1;
  * "profile" = 0|1: record CUDA events around the stages of each b2cnn_forward on its stream. */
 int b2cnn_set_option(b2cnn_handle *h, const char *key, int64_t value);

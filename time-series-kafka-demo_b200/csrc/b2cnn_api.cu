@@ -62,7 +62,7 @@ struct b2cnn_handle {
     float *d_wih0T = nullptr;   // [L][64]
     int64_t n_weights = 0;
     int64_t opt_path = B2CNN_PATH_AUTO;
-    int64_t opt_stream = 1;      // fp32 windows: streaming kernel instead of the generic one
+    int64_t opt_tc_fused = 1;    // bf16 windows: conv + projection fused in the streaming kernel (C <= 3)
     int64_t opt_tc_splits = 3;   // bf16 pieces per conv1 weight in the fused kernels
     int64_t last_launches = 0;
     int last_path = 0;
@@ -394,52 +394,74 @@ extern "C" int b2cnn_set_weights(b2cnn_handle *h, const float *blob, int64_t n, 
     h->hw.wih0T = h->d_wih0T;
     launch_transpose_wih(wih0, h->d_wih0T, d.L, st);
     CU_TRY(cudaGetLastError());
-    int rc = tc_prepare(h->tc, d, cw, wih0, h->hw, (int)h->opt_tc_splits, h->num_sms, st);
+    int rc = tc_prepare(h->tc, d, cw, wih0, (int)h->opt_tc_splits, st);
     if (rc != 0) return fail(B2CNN_ECUDA, std::string("tc_prepare: ") + tc_error());
     h->weights_set = true;
     return B2CNN_OK;
 }
 
-// Which kernels a (dtype, B, mode) call takes decides its scratch: the streaming tensor-core kernels need the range
-// partials [slices][B][64] (+ [B][64] gates for a sequence scan) and a few ints per window; only the generic and the
-// unfused tensor-core paths round-trip feature rows [B][L] through HBM.
-struct WsLayout { int64_t feats, partial, gates, tc, total; int ks_ws; };
+// ---- which kernels a forward call runs: DESIGN.md §2 is the table this code implements ----
+// The front end turns the windows into layer-0 gate partials (Stream, Fused) or feature rows (TcUnfused, Generic).
+// A short-window kernel, where one applies, runs the whole call instead; the workspace stays that of the front end,
+// so a size taken once serves every batch size and option.
+enum class Front { Stream, Fused, TcUnfused, Generic };
+enum class Short { None, Batch, Small };
+struct Route { Front front; Short short_kernel; };
 
-static bool use_tc(b2cnn_handle *h, int dtype, int64_t B, int mode);
+static Front front_end(const b2cnn_handle *h, const Dims &d, int dtype) {
+    if (h->opt_path == B2CNN_PATH_GENERIC) return Front::Generic;
+    if (dtype == B2CNN_DTYPE_F32) return h->tc.fused && d.XP % 4 == 0 ? Front::Stream : Front::Generic;   // TMA: 16-byte rows
+    if (h->tc.fused && h->opt_tc_fused) return Front::Fused;
+    return h->tc.features ? Front::TcUnfused : Front::Generic;
+}
 
-static WsLayout ws_layout(b2cnn_handle *h, int64_t B, int mode, int dtype) {
+static Route route(const b2cnn_handle *h, const Dims &d, int dtype, int64_t B, int mode) {
+    Route r{front_end(h, d, dtype), Short::None};
+    if (h->opt_path == B2CNN_PATH_TENSORCORE || !h->opt_small) return r;
+    const bool indep = mode == B2CNN_MODE_INDEPENDENT;
+    // many short windows ([P,10,120], all patients of a trigger): one launch, one warp per window
+    if (indep && B >= 8 && batch_supported(d)) r.short_kernel = Short::Batch;
+    // few short windows (the production call is [1,10,120]): one launch does everything
+    else if ((indep || B == 1) && B <= 256 && (int64_t)d.C * d.W <= 8192 && small_supported(d)) r.short_kernel = Short::Small;
+    return r;
+}
+
+// Scratch of one call, in this order: feature rows [B][L] | range partials [slices][B][64] | gates [B][64] | the
+// tensor-core region: NaN flags, then the pitch-aligned bf16 copy of x.
+struct WsLayout { int64_t feats, partial, gates, tc, total; };
+
+static WsLayout ws_layout(const b2cnn_handle *h, int64_t B, bool feats, bool stage) {
     const Dims &d = h->d;
+    const int ks = choose_ksplit(d.L), ranges = h->tc.fused ? h->tc.n_ranges : 0;
     WsLayout w;
-    const int ks = choose_ksplit(B, d.L, h->num_sms);
-    w.ks_ws = tc_partial_slices(h->tc) > ks ? tc_partial_slices(h->tc) : ks;
-    bool streaming = false;
-    if (dtype >= 0 && h->opt_path != B2CNN_PATH_GENERIC) {
-        if (dtype == B2CNN_DTYPE_F32) streaming = h->opt_stream && tc_stream_supported(h->tc, d, dtype);
-        else streaming = use_tc(h, dtype, B, mode) && tc_fused_supported(h->tc, d, dtype);
-    }
-    w.feats = streaming ? 0 : align_up(B * d.L * 4, 256);
-    w.partial = align_up((int64_t)w.ks_ws * B * kGates * 4, 256);
+    w.feats = feats ? align_up(B * d.L * 4, 256) : 0;
+    w.partial = align_up((int64_t)(ranges > ks ? ranges : ks) * B * kGates * 4, 256);
     w.gates = align_up(B * kGates * 4, 256);
-    w.tc = tc_workspace_bytes(h->tc, d, B);
+    w.tc = h->tc.features || h->tc.fused ? tc_flags_bytes(B) + (stage ? tc_stage_bytes(d, B) : 0) : 0;
     w.total = w.feats + w.partial + w.gates + w.tc;
     return w;
 }
 
-// dtype-blind size: enough for whatever path a call may take (the generic path's feature rows included)
+// Only the unfused tensor-core and the generic front ends round-trip feature rows through HBM.  The bf16 tensor-core
+// front ends copy x into the staging rows when its pitch is not a multiple of 8 samples; the staging region is also
+// reserved whenever W is not, which is what b2cnn_workspace_bytes_for has always returned for such windows.
+static WsLayout call_layout(const b2cnn_handle *h, const Dims &d, int64_t B, Front f) {
+    const bool tc_bf16 = f == Front::Fused || f == Front::TcUnfused;
+    return ws_layout(h, B, f == Front::TcUnfused || f == Front::Generic, d.W % 8 != 0 || (tc_bf16 && d.XP % 8 != 0));
+}
+
+// dtype-blind size: enough for whatever route a call of any dtype and row pitch may take
 extern "C" int64_t b2cnn_workspace_bytes(b2cnn_handle *h, int64_t B, int mode) {
+    (void)mode;
     if (!h || B < 1) return -1;
-    return ws_layout(h, B, mode, -1).total;
+    return ws_layout(h, B, true, true).total;
 }
 
-// exact size for windows of `dtype`: 307 MB smaller at [4096,3,75000] bf16, where the features never leave the SM
+// exact size for contiguous windows of `dtype`: 307 MB smaller at [4096,3,75000] bf16, where the features never leave the SM
 extern "C" int64_t b2cnn_workspace_bytes_for(b2cnn_handle *h, int64_t B, int mode, int dtype) {
+    (void)mode;
     if (!h || B < 1 || (dtype != B2CNN_DTYPE_F32 && dtype != B2CNN_DTYPE_BF16)) return -1;
-    return ws_layout(h, B, mode, dtype).total;
-}
-
-static bool use_tc(b2cnn_handle *h, int dtype, int64_t B, int mode) {
-    if (h->opt_path == B2CNN_PATH_GENERIC) return false;
-    return tc_supported(h->tc, h->d, dtype, B, mode);
+    return call_layout(h, h->d, B, front_end(h, h->d, dtype)).total;
 }
 
 static int forward_device(b2cnn_handle *h, const void *x, int dtype, int64_t B, int64_t xpitch, const float *age, int64_t n_age,
@@ -447,115 +469,87 @@ static int forward_device(b2cnn_handle *h, const void *x, int dtype, int64_t B, 
     Dims d = h->d;
     if (xpitch < d.W || xpitch > 0x7fffffff) return fail(B2CNN_EINVAL, "b2cnn_forward: x_pitch must be >= window");
     d.XP = (int)xpitch;
-    const int ks = choose_ksplit(B, d.L, h->num_sms);
-    const WsLayout wl = ws_layout(h, B, mode, dtype);
-    if (ws_bytes < wl.total) return fail(B2CNN_ESTATE, "b2cnn_forward: workspace smaller than b2cnn_workspace_bytes_for()");
+    const Route r = route(h, d, dtype, B, mode);
+    const WsLayout wl = call_layout(h, d, B, r.front);
+    if (!ws || ws_bytes < wl.total)
+        return fail(B2CNN_ESTATE, "b2cnn_forward: workspace missing or smaller than b2cnn_workspace_bytes_for(); rows whose pitch is not "
+                                  "a multiple of 16 bytes may need more: pad the rows, or size the workspace with b2cnn_workspace_bytes()");
+    if (h->opt_path == B2CNN_PATH_TENSORCORE && r.front == Front::Generic)
+        return fail(B2CNN_EARCH, "path=tensorcore requested but this shape/dtype/mode is not supported by the tensor-core kernel");
     char *base = (char *)ws;
-    float *feats = wl.feats ? (float *)base : nullptr; base += wl.feats;
+    float *feats = (float *)base; base += wl.feats;
     float *partial = (float *)base; base += wl.partial;
     float *gates = (float *)base; base += wl.gates;
     void *tc_ws = base;
-    const char *err = "";
-    int launches = 0;
-    const bool tc = use_tc(h, dtype, B, mode);
-    const bool stream = h->opt_path != B2CNN_PATH_GENERIC && h->opt_stream && tc_stream_supported(h->tc, d, dtype);
-    if (!wl.feats && !stream && !(tc && tc_fused_supported(h->tc, d, dtype)) &&
-        !(h->opt_path != B2CNN_PATH_TENSORCORE && h->opt_small && (mode == B2CNN_MODE_INDEPENDENT || B == 1) && B <= 256 &&
-          (int64_t)d.C * d.W <= 8192 && small_supported(d)) &&
-        !(h->opt_path != B2CNN_PATH_TENSORCORE && h->opt_small && mode == B2CNN_MODE_INDEPENDENT && B >= 8 && batch_supported(d)))
-        return fail(B2CNN_ESTATE, "b2cnn_forward: this x_pitch takes a path that needs feature rows; size the workspace with b2cnn_workspace_bytes()");
-    if (!tc && !stream && h->opt_path == B2CNN_PATH_TENSORCORE)
-        return fail(B2CNN_EARCH, "path=tensorcore requested but this shape/dtype/mode is not supported by the tensor-core kernel");
     const bool prof = h->opt_profile != 0;
     if (prof) {
         for (int i = 0; i < 3; ++i)
             if (!h->ev_stage[i]) CU_TRY(cudaEventCreate(&h->ev_stage[i]));
         CU_TRY(cudaEventRecord(h->ev_stage[0], st));
     }
-    // short windows, many of them (all patients of a trigger, [P,10,120]): one launch, one warp per window
-    if (h->opt_path != B2CNN_PATH_TENSORCORE && h->opt_small && mode == B2CNN_MODE_INDEPENDENT && B >= 8 && batch_supported(d)) {
-        int n1 = launch_short_batch(d, h->cw, h->hw, x, dtype, B, age, n_age, apply_sigmoid, out, h->num_sms, st, &err);
-        if (n1 < 0) return fail(B2CNN_ECUDA, std::string("short-window batch kernel: ") + err);
-        if (prof) { CU_TRY(cudaEventRecord(h->ev_stage[1], st)); CU_TRY(cudaEventRecord(h->ev_stage[2], st)); h->ev_valid = true; }
-        h->last_launches = n1; h->last_path = B2CNN_PATH_GENERIC;
-        return B2CNN_OK;
-    }
-    // short windows, few of them (the production call is [1,10,120]): one launch does everything
-    if (h->opt_path != B2CNN_PATH_TENSORCORE && h->opt_small && (mode == B2CNN_MODE_INDEPENDENT || B == 1) && B <= 256 &&
-        (int64_t)d.C * d.W <= 8192 && small_supported(d)) {
-        int n1 = launch_small_forward(d, h->cw, h->hw, x, dtype, B, age, n_age, apply_sigmoid, out, st, &err);
-        if (n1 < 0) return fail(B2CNN_ECUDA, std::string("small-window kernel: ") + err);
-        if (prof) { CU_TRY(cudaEventRecord(h->ev_stage[1], st)); CU_TRY(cudaEventRecord(h->ev_stage[2], st)); h->ev_valid = true; }
-        h->last_launches = n1; h->last_path = B2CNN_PATH_GENERIC;
-        return B2CNN_OK;
-    }
-    // feature layout: the generic kernel writes rows [B][L]; the tensor-core kernel's threads
-    // are windows, so it writes the transpose [L][B] (coalesced across lanes).
+    // stage 0: the front end, or the short-window kernel that does the whole call
+    const bool indep = mode == B2CNN_MODE_INDEPENDENT;
+    const bool to_gates = r.front == Front::Stream || r.front == Front::Fused;   // the streaming kernels: features never leave the SM
+    // feature layout: the generic kernel writes rows [B][L]; the tensor-core kernel's threads are windows, so it
+    // writes the transpose [L][B] (coalesced across lanes)
     int64_t sB = d.L, sP = 1;
+    const char *err = "", *what;
     int n;
-    if (h->opt_path != B2CNN_PATH_GENERIC && h->opt_stream && tc_stream_supported(h->tc, d, dtype)) {
-        // fp32 windows: TMA-streamed CUDA-core conv1 + wgmma projection, features never leave the SM
-        const bool indep = mode == B2CNN_MODE_INDEPENDENT;
-        int slices = 0;
-        n = tc_stream_gates(h->tc, d, h->cw, h->hw, x, B, feats, partial, gates, tc_ws, h->num_sms, st, &err, !indep, &slices);
-        if (n < 0) return fail(B2CNN_ECUDA, std::string("fp32 stream kernel: ") + err);
-        launches += n;
-        if (prof) CU_TRY(cudaEventRecord(h->ev_stage[1], st));
-        // the head kernel is the last reader of the call's exception list: it also puts the handle's flag state back to zero
-        const bool cleans = indep && h->tc.cur_own;
-        n = indep ? launch_reduce_lstm_head(d, h->hw, partial, slices, B, age, n_age, apply_sigmoid, out, st, &err,
-                                            cleans ? h->tc.cur_count : nullptr, h->tc.cur_flags, h->tc.cur_list)
-                  : launch_lstm_head(d, h->hw, gates, B, age, n_age, mode, apply_sigmoid, out, st, &err);
-        if (n < 0) return fail(B2CNN_ECUDA, std::string("head: ") + err);
-        if (cleans) h->tc.flags_clean = true;
-        launches += n;
-        if (prof) { CU_TRY(cudaEventRecord(h->ev_stage[2], st)); h->ev_valid = true; }
-        h->last_launches = launches; h->last_path = B2CNN_PATH_STREAM;
-        return B2CNN_OK;
-    }
-    if (tc && tc_fused_supported(h->tc, d, dtype)) {
-        // conv + pool + projection fused on the tensor cores: the features never leave the SM
-        const bool indep = mode == B2CNN_MODE_INDEPENDENT;
-        int slices = 0;
-        n = tc_fused_gates(h->tc, d, h->cw, h->hw, x, B, feats, partial, gates, tc_ws, h->num_sms, st, &err, !indep, &slices);
-        if (n < 0) return fail(B2CNN_ECUDA, std::string("tensor-core fused kernel: ") + err);
-        launches += n;
-        if (prof) CU_TRY(cudaEventRecord(h->ev_stage[1], st));
-        // the head kernel is the last reader of the call's exception list: it also puts the handle's flag state back to zero
-        const bool cleans = indep && h->tc.cur_own;
-        n = indep ? launch_reduce_lstm_head(d, h->hw, partial, slices, B, age, n_age, apply_sigmoid, out, st, &err,
-                                            cleans ? h->tc.cur_count : nullptr, h->tc.cur_flags, h->tc.cur_list)
-                  : launch_lstm_head(d, h->hw, gates, B, age, n_age, mode, apply_sigmoid, out, st, &err);
-        if (n < 0) return fail(B2CNN_ECUDA, std::string("head: ") + err);
-        if (cleans) h->tc.flags_clean = true;
-        launches += n;
-        if (prof) { CU_TRY(cudaEventRecord(h->ev_stage[2], st)); h->ev_valid = true; }
-        h->last_launches = launches; h->last_path = B2CNN_PATH_TENSORCORE;
-        return B2CNN_OK;
-    }
-    if (tc) {
+    if (r.short_kernel == Short::Batch) {
+        what = "short-window batch kernel";
+        n = launch_short_batch(d, h->cw, h->hw, x, dtype, B, age, n_age, apply_sigmoid, out, h->num_sms, st, &err);
+    } else if (r.short_kernel == Short::Small) {
+        what = "small-window kernel";
+        n = launch_small_forward(d, h->cw, h->hw, x, dtype, B, age, n_age, apply_sigmoid, out, st, &err);
+    } else if (to_gates) {
+        what = r.front == Front::Stream ? "fp32 stream kernel" : "tensor-core fused kernel";
+        n = tc_gates(h->tc, d, h->cw, h->hw, x, dtype, B, partial, gates, tc_ws, h->num_sms, st, &err, !indep);
+    } else if (r.front == Front::TcUnfused) {
+        what = "tensor-core front end";
         sB = 1; sP = B;
         n = tc_frontend(h->tc, d, h->cw, x, B, feats, sB, sP, tc_ws, h->num_sms, st, &err);
-        if (n < 0) return fail(B2CNN_ECUDA, std::string("tensor-core front end: ") + err);
     } else {
+        what = "front end";
         n = launch_frontend_generic(d, h->cw, x, dtype, B, feats, sB, sP, st, h->num_sms, &err);
-        if (n < 0) return fail(B2CNN_ECUDA, std::string("front end: ") + err);
     }
-    launches += n;
+    if (n < 0) return fail(B2CNN_ECUDA, std::string(what) + ": " + err);
+    int launches = n;
     if (prof) CU_TRY(cudaEventRecord(h->ev_stage[1], st));
-    n = launch_head(d, h->hw, feats, sB, sP, B, age, n_age, mode, apply_sigmoid, out, gates, partial, ks, st, &err);
-    if (n < 0) return fail(B2CNN_ECUDA, std::string("head: ") + err);
-    launches += n;
+    // stage 1: projection + LSTM head
+    if (r.short_kernel == Short::None) {
+        // the head kernel is the last reader of the call's exception list: it also puts the handle's flag state back to zero
+        const bool cleans = to_gates && indep && h->tc.cur_own;
+        if (!to_gates)
+            n = launch_head(d, h->hw, feats, sB, sP, B, age, n_age, mode, apply_sigmoid, out, gates, partial, choose_ksplit(d.L), st, &err);
+        else if (indep)
+            n = launch_reduce_lstm_head(d, h->hw, partial, h->tc.n_ranges, B, age, n_age, apply_sigmoid, out, st, &err,
+                                        cleans ? h->tc.cur_count : nullptr, h->tc.cur_flags, h->tc.cur_list);
+        else
+            n = launch_lstm_head(d, h->hw, gates, B, age, n_age, mode, apply_sigmoid, out, st, &err);
+        if (n < 0) return fail(B2CNN_ECUDA, std::string("head: ") + err);
+        if (cleans) h->tc.flags_clean = true;
+        launches += n;
+    }
     if (prof) { CU_TRY(cudaEventRecord(h->ev_stage[2], st)); h->ev_valid = true; }
-    h->last_launches = launches; h->last_path = tc ? B2CNN_PATH_TENSORCORE : B2CNN_PATH_GENERIC;
+    h->last_launches = launches;
+    h->last_path = r.short_kernel != Short::None || r.front == Front::Generic ? B2CNN_PATH_GENERIC
+                   : r.front == Front::Stream                               ? B2CNN_PATH_STREAM
+                                                                            : B2CNN_PATH_TENSORCORE;
+    return B2CNN_OK;
+}
+
+// the arguments every call on B windows of `dtype` shares (the forward calls also take age and mode)
+static int check_windows(const char *fn, b2cnn_handle *h, const void *x, int dtype, int64_t B, const float *out) {
+    if (!h || !x || !out) return fail(B2CNN_EINVAL, std::string(fn) + ": null argument");
+    if (!h->weights_set) return fail(B2CNN_ESTATE, std::string(fn) + ": weights not set (call b2cnn_set_weights)");
+    if (B < 1 || B > (int64_t)0x7fffffff / 64) return fail(B2CNN_EINVAL, std::string(fn) + ": batch size out of range");
+    if (dtype != B2CNN_DTYPE_F32 && dtype != B2CNN_DTYPE_BF16) return fail(B2CNN_EINVAL, std::string(fn) + ": dtype must be f32 (0) or bf16 (1)");
     return B2CNN_OK;
 }
 
 static int check_call(b2cnn_handle *h, const void *x, int dtype, int64_t B, const float *age, int64_t n_age, int mode, float *out) {
-    if (!h || !x || !age || !out) return fail(B2CNN_EINVAL, "b2cnn_forward: null argument");
-    if (!h->weights_set) return fail(B2CNN_ESTATE, "b2cnn_forward: weights not set (call b2cnn_set_weights)");
-    if (B < 1 || B > (int64_t)0x7fffffff / 64) return fail(B2CNN_EINVAL, "b2cnn_forward: batch size out of range");
-    if (dtype != B2CNN_DTYPE_F32 && dtype != B2CNN_DTYPE_BF16) return fail(B2CNN_EINVAL, "b2cnn_forward: dtype must be f32 (0) or bf16 (1)");
+    if (!age) return fail(B2CNN_EINVAL, "b2cnn_forward: null argument");
+    if (int rc = check_windows("b2cnn_forward", h, x, dtype, B, out)) return rc;
     if (mode != B2CNN_MODE_INDEPENDENT && mode != B2CNN_MODE_SEQUENCE) return fail(B2CNN_EINVAL, "b2cnn_forward: bad mode");
     if (n_age != 1 && n_age != B) return fail(B2CNN_EINVAL, "b2cnn_forward: age must have 1 or B elements");
     return B2CNN_OK;
@@ -563,12 +557,8 @@ static int check_call(b2cnn_handle *h, const void *x, int dtype, int64_t B, cons
 
 extern "C" int b2cnn_forward(b2cnn_handle *h, const void *x, int dtype, int64_t B, const float *age, int64_t n_age,
                              int mode, int apply_sigmoid, float *out, void *workspace, int64_t workspace_bytes, void *stream) {
-    int rc = check_call(h, x, dtype, B, age, n_age, mode, out);
-    if (rc) return rc;
-    if (!workspace || workspace_bytes < ws_layout(h, B, mode, dtype).total)
-        return fail(B2CNN_ESTATE, "b2cnn_forward: workspace missing or smaller than b2cnn_workspace_bytes_for()");
-    DEVICE_GUARD(h->device);
-    return forward_device(h, x, dtype, B, h->d.W, age, n_age, mode, apply_sigmoid, out, workspace, workspace_bytes, (cudaStream_t)stream);
+    return b2cnn_forward_pitched(h, x, dtype, B, h ? h->d.W : 0, age, n_age, mode, apply_sigmoid, out, workspace, workspace_bytes,
+                                 stream);
 }
 
 extern "C" int b2cnn_forward_pitched(b2cnn_handle *h, const void *x, int dtype, int64_t B, int64_t x_pitch, const float *age,
@@ -576,20 +566,17 @@ extern "C" int b2cnn_forward_pitched(b2cnn_handle *h, const void *x, int dtype, 
                                      int64_t workspace_bytes, void *stream) {
     int rc = check_call(h, x, dtype, B, age, n_age, mode, out);
     if (rc) return rc;
-    if (!workspace || workspace_bytes < ws_layout(h, B, mode, dtype).total)
-        return fail(B2CNN_ESTATE, "b2cnn_forward_pitched: workspace missing or smaller than b2cnn_workspace_bytes_for()");
     DEVICE_GUARD(h->device);
     return forward_device(h, x, dtype, B, x_pitch, age, n_age, mode, apply_sigmoid, out, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
 extern "C" int b2cnn_features(b2cnn_handle *h, const void *x, int dtype, int64_t B, float *feats, void *stream) {
-    if (!h || !x || !feats) return fail(B2CNN_EINVAL, "b2cnn_features: null argument");
-    if (!h->weights_set) return fail(B2CNN_ESTATE, "b2cnn_features: weights not set");
-    if (B < 1) return fail(B2CNN_EINVAL, "b2cnn_features: B < 1");
+    int rc = check_windows("b2cnn_features", h, x, dtype, B, feats);
+    if (rc) return rc;
     DEVICE_GUARD(h->device);
     const char *err = "";
     int n;
-    if (use_tc(h, dtype, B, B2CNN_MODE_INDEPENDENT) && tc_can_emit_features(h->tc)) {
+    if (h->opt_path != B2CNN_PATH_GENERIC && dtype == B2CNN_DTYPE_BF16 && h->tc.features) {
         n = tc_features(h->tc, h->d, h->cw, x, B, feats, h->num_sms, (cudaStream_t)stream, &err);
         h->last_path = B2CNN_PATH_TENSORCORE;
     } else {
@@ -715,7 +702,7 @@ extern "C" int b2cnn_forward_host(b2cnn_handle *h, const void *x_host, int dtype
         if (chunk < 1) chunk = 1;
         if (chunk > B) chunk = B;
     }
-    const int64_t ws_bytes = ws_layout(h, chunk, mode, dtype).total;
+    const int64_t ws_bytes = b2cnn_workspace_bytes_for(h, chunk, mode, dtype);
     rc = ensure_host_staging(h, (size_t)chunk * win_bytes, B, (size_t)ws_bytes);
     if (rc) return rc;
     CU_TRY(cudaMemcpyAsync(h->st_age, age_host, sizeof(float) * n_age, cudaMemcpyHostToDevice, h->s_copy));
@@ -750,8 +737,7 @@ extern "C" int b2cnn_set_option(b2cnn_handle *h, const char *key, int64_t value)
         return B2CNN_OK;
     }
     if (!strcmp(key, "small_kernel")) { h->opt_small = value ? 1 : 0; return B2CNN_OK; }
-    if (!strcmp(key, "tc_fused")) { h->tc.opt_fused = value ? 1 : 0; return B2CNN_OK; }
-    if (!strcmp(key, "stream_f32")) { h->opt_stream = value ? 1 : 0; return B2CNN_OK; }
+    if (!strcmp(key, "tc_fused")) { h->opt_tc_fused = value ? 1 : 0; return B2CNN_OK; }
     if (!strcmp(key, "profile")) { h->opt_profile = value ? 1 : 0; h->ev_valid = false; return B2CNN_OK; }
     if (!strcmp(key, "tc_splits")) {
         if (value != 2 && value != 3) return fail(B2CNN_EINVAL, "tc_splits must be 2 or 3");
@@ -768,7 +754,7 @@ extern "C" int64_t b2cnn_get_option(b2cnn_handle *h, const char *key) {
     if (!strcmp(key, "tc_splits")) return h->opt_tc_splits;
     if (!strcmp(key, "num_sms")) return h->num_sms;
     if (!strcmp(key, "profile")) return h->opt_profile;
-    if (!strcmp(key, "tc_available")) return tc_supported(h->tc, h->d, B2CNN_DTYPE_BF16, 128, B2CNN_MODE_INDEPENDENT) ? 1 : 0;
+    if (!strcmp(key, "tc_available")) return h->tc.features || (h->tc.fused && h->opt_tc_fused) ? 1 : 0;   // for bf16 windows
     return -1;
 }
 

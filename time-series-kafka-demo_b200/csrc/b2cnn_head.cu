@@ -261,10 +261,9 @@ head_sequence_kernel(const float *__restrict__ gates0, HeadWeights hw, const flo
 }
 
 // ---------------------------------------------------------------------------------------
-int choose_ksplit(int64_t B, int L, int num_sms) {
+int choose_ksplit(int L) {
     // Depends on L only: the summation order of a window's projection must not change with the
     // batch it arrives in (prefix / chunking consistency is tested bit-for-bit).
-    (void)B; (void)num_sms;
     int ks = (L + 2047) / 2048;
     return ks < 1 ? 1 : ks;
 }

@@ -117,7 +117,7 @@ int launch_reduce_lstm_head(const Dims &d, const HeadWeights &hw, const float *p
                             const float *age, int64_t n_age, int apply_sigmoid, float *out, cudaStream_t st, const char **err,
                             int *clean_count = nullptr, int *clean_flags = nullptr, const int *clean_list = nullptr);
 
-int choose_ksplit(int64_t B, int L, int num_sms);
+int choose_ksplit(int L);
 
 // b2cnn_small.cu: whole forward pass of short windows in one launch (independent windows only)
 bool small_supported(const Dims &d);

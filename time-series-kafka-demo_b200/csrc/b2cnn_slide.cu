@@ -329,7 +329,7 @@ int slide_create(const Dims &d, const TcState &tc, int n_patients, int stride, i
     if (n_patients < 1 || n_patients > (1 << 24)) { *err = "n_patients out of range"; return B2CNN_EINVAL; }
     if (stride < 1 || stride > d.W) { *err = "stride must be in [1, window]"; return B2CNN_EINVAL; }
     if (stride % 4 != 0) { *err = "stride must be a multiple of the feature stride (4 samples)"; return B2CNN_EINVAL; }
-    if (!tc_ring_supported(tc, d)) {
+    if (!tc.fused) {
         *err = "the sliding-window scorer covers the streaming tensor-core geometries only (MyCNN5 or MyCNN2/3/4 conv/pool, "
                "1 to 3 channels, tanh, no affine)";
         return B2CNN_EARCH;

@@ -37,9 +37,6 @@ namespace b2cnn {
 static thread_local const char *g_tc_err = "";
 const char *tc_error() { return g_tc_err; }
 
-#ifndef B2CNN_OWN_FLAGS
-#define B2CNN_OWN_FLAGS 1          // NaN-exception flag state owned by the handle and cleaned by the head kernel: no per-call memset (TcState)
-#endif
 constexpr int64_t kOwnFlagCap = 65536;   // windows per call served by the handle's own flag state (512 KB); larger batches use the workspace copy
 constexpr int kTcM = 128;          // windows per CTA (two wgmma m64 row halves)
 constexpr int kTcAdv = 24;         // conv1 positions (= samples) a tile advances
@@ -103,14 +100,11 @@ static bool arch_ok(const Dims &d) {
 
 static int tiles_per_cta_for(const Dims &d);
 
-int tc_prepare(TcState &s, const Dims &d, const ConvWeights &cw, const float *d_wih0, const HeadWeights &, int splits, int,
-               cudaStream_t st) {
-    s.ready = false;
+int tc_prepare(TcState &s, const Dims &d, const ConvWeights &cw, const float *d_wih0, int splits, cudaStream_t st) {
+    s.features = s.fused = false;
     s.splits = splits;
-    s.fused_ready = false;
     if (!arch_ok(d) && !arch1_ok(d)) return 0;   // not an error: this shape takes the generic path
     if (!get_encode()) return 0;
-#if B2CNN_OWN_FLAGS
     if (!s.d_flagstate) {
         const int64_t cap = kOwnFlagCap;
         if (cudaMalloc(reinterpret_cast<void **>(&s.d_flagstate), sizeof(int) * (2 * cap + 16)) == cudaSuccess &&
@@ -121,7 +115,6 @@ int tc_prepare(TcState &s, const Dims &d, const ConvWeights &cw, const float *d_
             (void)cudaGetLastError();
         }
     }
-#endif
     // band matrices: piece sp of T_c[k][(s,o)] = w1[o][c][k-s], stored as GMMA K-major
     // no-swizzle core matrices: byte = (n/8)*256 + (k/8)*128 + (n%8)*16 + (k%8)*2, n = s*4+o.
     //   d_bmats   [C][3][1 KB]  three bf16 pieces (hi/mid/lo: the full 24-bit fp32 mantissa)
@@ -149,10 +142,8 @@ int tc_prepare(TcState &s, const Dims &d, const ConvWeights &cw, const float *d_
     if (cudaMemcpyAsync(s.d_bmats, host.data(), host.size() * 2, cudaMemcpyHostToDevice, st) != cudaSuccess ||
         cudaMemcpyAsync(s.d_bmats2, host2.data(), host2.size() * 2, cudaMemcpyHostToDevice, st) != cudaSuccess ||
         cudaStreamSynchronize(st) != cudaSuccess) { g_tc_err = "upload band matrices"; return -1; }
-    s.ready = true;
-    s.has_v1 = arch_ok(d);
+    s.features = arch_ok(d);
     // ---- fused kernels (bf16 and fp32 windows: the same 3-block tiles and ranges): W_ih_l0 packed per (range, chunk)
-    s.fused_ready = false;
     s.tiles_per_cta = tiles_per_cta_for(d);
     s.feats_per_cta = 2 * kTcBlocks * s.tiles_per_cta - 4;   // even: every range starts 16-byte aligned (TMA)
     s.chunks_per_cta = (kTcBlocks * s.tiles_per_cta + 7) / 8;
@@ -165,7 +156,7 @@ int tc_prepare(TcState &s, const Dims &d, const ConvWeights &cw, const float *d_
         tc_pack_wih_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(d_wih0, reinterpret_cast<uint8_t *>(s.d_wpack), d.L,
                                                                           s.feats_per_cta, s.chunks_per_cta, s.n_ranges, d.K1 == 10 ? 3 : 2);
         if (cudaGetLastError() != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess) { g_tc_err = "pack W_ih"; return -1; }
-        s.fused_ready = true;
+        s.fused = true;
     }
     return 0;
 }
@@ -179,27 +170,15 @@ void tc_release(TcState &s) {
     s.d_bmats = nullptr;
     s.d_bmats2 = nullptr;
     s.d_wpack = nullptr;
-    s.ready = s.fused_ready = false;
+    s.features = s.fused = false;
 }
 
-bool tc_supported(const TcState &s, const Dims &d, int dtype, int64_t B, int mode) {
-    (void)mode; (void)B;
-    return s.ready && dtype == B2CNN_DTYPE_BF16 && (arch_ok(d) || (arch1_ok(d) && s.fused_ready && s.opt_fused));
-}
-bool tc_can_emit_features(const TcState &s) { return s.ready && s.has_v1; }
-
-// A TMA tensor map needs a row pitch that is a multiple of 16 bytes.  Windows whose length is not a
-// multiple of 8 samples (7500, 37500 ...) are copied once into a pitch-aligned scratch (costs one
+// A TMA tensor map needs a row pitch that is a multiple of 16 bytes.  bf16 windows whose pitch is not a
+// multiple of 8 samples (contiguous 7500, 37500 ...) are copied once into a pitch-aligned scratch (costs one
 // extra read + write of the input; W % 8 == 0, e.g. the headline 75000, streams straight from x).
 static int64_t padded_w(const Dims &d) { return (d.W + 7) & ~7; }
-static int64_t flags_bytes(int64_t B) { return ((2 * B + 64) * 4 + 255) / 256 * 256; }
-static int64_t xpad_bytes(const Dims &d, int64_t B) { return (d.W % 8) ? (B * d.C * padded_w(d) * 2 + 255) / 256 * 256 : 0; }
-
-// tc workspace: nan flags [B] + list [B] + count, then the optional pitch-aligned copy of x
-int64_t tc_workspace_bytes(const TcState &s, const Dims &d, int64_t B) {
-    if (!s.ready) return 0;
-    return flags_bytes(B) + xpad_bytes(d, B);
-}
+int64_t tc_flags_bytes(int64_t B) { return ((2 * B + 64) * 4 + 255) / 256 * 256; }
+int64_t tc_stage_bytes(const Dims &d, int64_t B) { return (B * d.C * padded_w(d) * 2 + 255) / 256 * 256; }
 
 // rows of W samples, `sp` elements apart -> rows Wp (multiple of 8) apart, tail zero-filled.
 // VEC 8: W % 4 == 0 and sp % 4 == 0: every row starts 8-byte aligned; one thread moves 16 output bytes with two
@@ -328,7 +307,8 @@ int tc_frontend(TcState &s, const Dims &d, const ConvWeights &cw, const void *x,
                 int64_t sB, int64_t sP, void *ws, int num_sms, cudaStream_t st, const char **err) {
     int *flags = reinterpret_cast<int *>(ws);
     const bool own = flags == nullptr;
-    if (own && cudaMallocAsync(&flags, (size_t)tc_workspace_bytes(s, d, B), st) != cudaSuccess) { *err = "cudaMallocAsync"; return -1; }
+    const int64_t own_bytes = tc_flags_bytes(B) + (d.XP % 8 ? tc_stage_bytes(d, B) : 0);
+    if (own && cudaMallocAsync(&flags, (size_t)own_bytes, st) != cudaSuccess) { *err = "cudaMallocAsync"; return -1; }
     int *list = flags + B, *count = list + B;
     int launches = -1;
     if (cudaMemsetAsync(flags, 0, sizeof(int) * (2 * B + 1), st) != cudaSuccess) {
@@ -336,7 +316,7 @@ int tc_frontend(TcState &s, const Dims &d, const ConvWeights &cw, const void *x,
     } else {
         int staged = 0;
         int64_t pitch = d.XP;
-        const void *xin = tc_stage_input(d, x, B, reinterpret_cast<char *>(flags) + flags_bytes(B), &pitch, &staged, st);
+        const void *xin = tc_stage_input(d, x, B, reinterpret_cast<char *>(flags) + tc_flags_bytes(B), &pitch, &staged, st);
         int n = launch_tc_kernel(s, d, cw, xin, pitch, B, feats, sB, sP, flags, st, err);
         if (n >= 0) {
             tc_compact_flags_kernel<<<(unsigned)((B + 255) / 256), 256, 0, st>>>(flags, (int)B, list, count);
@@ -354,22 +334,14 @@ int tc_features(TcState &s, const Dims &d, const ConvWeights &cw, const void *x,
     return tc_frontend(s, d, cw, x, B, feats, d.L, 1, nullptr, num_sms, st, err);
 }
 
-
-bool tc_fused_supported(const TcState &s, const Dims &d, int dtype) {
-    return s.ready && s.fused_ready && s.opt_fused && dtype == B2CNN_DTYPE_BF16 && (arch_ok(d) || arch1_ok(d)) && d.C <= 3;
-}
-int tc_partial_slices(const TcState &s) { return s.fused_ready ? s.n_ranges : 0; }
-
 // Where this call keeps count | flags | list: the handle's own, already-zero copy (see TcState) or the head of the
 // workspace, zeroed here.  count and flags are adjacent in both, the list needs no zeroing.
 static int flag_bufs(TcState &s, void *ws, int64_t B, cudaStream_t st, bool cleaning_head_follows, const char **err) {
     bool own = false;
-#if B2CNN_OWN_FLAGS
     if (s.d_flagstate && B <= s.flag_cap && cleaning_head_follows) {
         if (!s.owner_set) { s.owner_set = true; s.owner_stream = st; }
         own = s.owner_stream == st;
     }
-#endif
     if (own) {
         s.cur_count = s.d_flagstate; s.cur_flags = s.cur_count + 16; s.cur_list = s.cur_flags + s.flag_cap;
         if (!s.flags_clean && cudaMemsetAsync(s.cur_count, 0, sizeof(int) * (s.flag_cap + 16), st) != cudaSuccess) { *err = "memset flags"; return -1; }
@@ -382,19 +354,18 @@ static int flag_bufs(TcState &s, void *ws, int64_t B, cudaStream_t st, bool clea
     return 0;
 }
 
-// fused front end + projection -> gates[B][64]; flagged (NaN) windows are recomputed exactly.
-int tc_fused_gates(TcState &s, const Dims &d, const ConvWeights &cw, const HeadWeights &hw, const void *x, int64_t B,
-                   float *feats, float *partial, float *gates, void *ws, int num_sms, cudaStream_t st, const char **err,
-                   bool reduce_here, int *slices_out) {
-    (void)feats;
+// streaming front end + projection -> range partials (and gates[B][64]); flagged (NaN) windows are recomputed exactly.
+int tc_gates(TcState &s, const Dims &d, const ConvWeights &cw, const HeadWeights &hw, const void *x, int dtype, int64_t B,
+             float *partial, float *gates, void *ws, int num_sms, cudaStream_t st, const char **err, bool reduce_here) {
+    const bool f32 = dtype == B2CNN_DTYPE_F32;
     // scratch ints: count | flags | list  (the handle's own zero-between-calls copy, or the head of the workspace)
     if (flag_bufs(s, ws, B, st, !reduce_here, err) != 0) return -1;
     int *count = s.cur_count, *flags = s.cur_flags, *list = s.cur_list;
     int staged = 0;
-    int64_t pitch = d.XP;
-    const void *xin = tc_stage_input(d, x, B, reinterpret_cast<char *>(ws) + flags_bytes(B), &pitch, &staged, st);
+    int64_t pitch = d.XP;         // fp32 windows arrive with 16-byte rows (the caller routes any other pitch elsewhere)
+    const void *xin = f32 ? x : tc_stage_input(d, x, B, reinterpret_cast<char *>(ws) + tc_flags_bytes(B), &pitch, &staged, st);
     CUtensorMap tm;
-    if (make_tmap(d, xin, pitch, B, false, &tm, err) != 0) return -1;
+    if (make_tmap(d, xin, pitch, B, f32, &tm, err) != 0) return -1;
     TcFusedParams p;
     memset(&p, 0, sizeof p);
     p.partial = partial; p.nanflag = flags; p.list = list; p.count = count;
@@ -402,24 +373,25 @@ int tc_fused_gates(TcState &s, const Dims &d, const ConvWeights &cw, const HeadW
     p.B = (int)B; p.W = d.W; p.L = d.L;
     p.tiles_per_cta = s.tiles_per_cta; p.feats_per_cta = s.feats_per_cta; p.chunks_per_cta = s.chunks_per_cta;
     fill_epilogue(p, d, cw);
-    const int sp = s.splits;                          // bf16 pieces per conv1 weight: 3 (fp32-equivalent) or 2
-    p.bmats = reinterpret_cast<const uint8_t *>(sp == 2 ? s.d_bmats2 : s.d_bmats);
+    // bf16 pieces per conv1 weight: 3 (fp32-equivalent) or 2; fp32 windows multiply the fp32 weights (key 1)
+    const int sp = f32 ? 1 : s.splits;
+    if (!f32) p.bmats = reinterpret_cast<const uint8_t *>(sp == 2 ? s.d_bmats2 : s.d_bmats);
     dim3 grid((unsigned)((B + kTcM - 1) / kTcM), s.n_ranges);
     const int key = d.C * 100 + sp * 10 + (d.K1 == 10 ? 0 : 1);
     cudaError_t le;
     switch (key) {
-#define FU_CASE(CC, SS, AA) case CC * 100 + SS * 10 + AA: le = launch_stream<CC, SS, AA, false, kOutGates>(tm, p, grid, st); break;
-        FU_CASE(1, 2, 0) FU_CASE(2, 2, 0) FU_CASE(3, 2, 0) FU_CASE(1, 3, 0) FU_CASE(2, 3, 0) FU_CASE(3, 3, 0)
-        FU_CASE(1, 2, 1) FU_CASE(2, 2, 1) FU_CASE(3, 2, 1) FU_CASE(1, 3, 1) FU_CASE(2, 3, 1) FU_CASE(3, 3, 1)
-#undef FU_CASE
-        default: *err = "no fused instantiation for this channel count / split"; return -1;
+#define GATES_CASE(CC, SS, AA) case CC * 100 + SS * 10 + AA: le = launch_stream<CC, SS, AA, SS == 1, kOutGates>(tm, p, grid, st); break;
+        GATES_CASE(1, 2, 0) GATES_CASE(2, 2, 0) GATES_CASE(3, 2, 0) GATES_CASE(1, 3, 0) GATES_CASE(2, 3, 0) GATES_CASE(3, 3, 0)
+        GATES_CASE(1, 2, 1) GATES_CASE(2, 2, 1) GATES_CASE(3, 2, 1) GATES_CASE(1, 3, 1) GATES_CASE(2, 3, 1) GATES_CASE(3, 3, 1)
+        GATES_CASE(1, 1, 0) GATES_CASE(2, 1, 0) GATES_CASE(3, 1, 0) GATES_CASE(1, 1, 1) GATES_CASE(2, 1, 1) GATES_CASE(3, 1, 1)
+#undef GATES_CASE
+        default: *err = "no streaming instantiation for this channel count / split"; return -1;
     }
     if (le != cudaSuccess) { *err = cudaGetErrorString(le); return -1; }
     int launches = 1 + staged;
-    if (slices_out) *slices_out = s.n_ranges;
     // the exception path: exact gate partials of the flagged windows, written over their rows of `partial`
     // (one launch; the list was compacted by the kernel itself, an empty list costs one almost-empty launch)
-    int n = launch_frontend_generic_gates_listed(d, cw, x, B2CNN_DTYPE_BF16, B, hw.wih0T, partial, s.n_ranges, list, count, st, num_sms, err);
+    int n = launch_frontend_generic_gates_listed(d, cw, x, dtype, B, hw.wih0T, partial, s.n_ranges, list, count, st, num_sms, err);
     if (n < 0) return -1;
     launches += n;
     // reduce_here == false: the caller's head kernel sums the range partials itself (independent windows)
@@ -427,8 +399,6 @@ int tc_fused_gates(TcState &s, const Dims &d, const ConvWeights &cw, const HeadW
     if (n < 0) return -1;
     return launches + n;
 }
-
-bool tc_ring_supported(const TcState &s, const Dims &d) { return s.ready && s.fused_ready && (arch_ok(d) || arch1_ok(d)) && d.C <= 3; }
 
 // 2-D map of a scorer's feature ring [L][pitch] fp32 (pitch % 4 == 0): boxes of 16 positions x 128 patients
 int tc_ring_tmap(const float *ring, int64_t P, int64_t pitch, int L, CUtensorMap *tm, const char **err) {
@@ -477,46 +447,6 @@ int tc_ring_features(const TcState &s, const Dims &dseg, const ConvWeights &cw, 
     tc_compact_flags_kernel<<<(unsigned)((P + 255) / 256), 256, 0, st>>>(flags, (int)P, list, count);
     if (cudaGetLastError() != cudaSuccess) { *err = "flag compaction launch"; return -1; }
     return 2;
-}
-
-bool tc_stream_supported(const TcState &s, const Dims &d, int dtype) {
-    return s.ready && s.fused_ready && dtype == B2CNN_DTYPE_F32 && (arch_ok(d) || arch1_ok(d)) && d.C <= 3 && (d.XP % 4) == 0;
-}
-
-// fp32 windows: streaming front end + projection -> gates[B][64]; flagged (NaN) windows are recomputed exactly.
-int tc_stream_gates(TcState &s, const Dims &d, const ConvWeights &cw, const HeadWeights &hw, const void *x, int64_t B,
-                    float *feats, float *partial, float *gates, void *ws, int num_sms, cudaStream_t st, const char **err,
-                    bool reduce_here, int *slices_out) {
-    (void)feats;
-    if (flag_bufs(s, ws, B, st, !reduce_here, err) != 0) return -1;
-    int *count = s.cur_count, *flags = s.cur_flags, *list = s.cur_list;
-    CUtensorMap tm;
-    if (make_tmap(d, x, d.XP, B, true, &tm, err) != 0) return -1;
-    TcFusedParams p;
-    memset(&p, 0, sizeof p);
-    p.partial = partial; p.nanflag = flags; p.list = list; p.count = count;
-    p.wpack = reinterpret_cast<const uint8_t *>(s.d_wpack);
-    p.B = (int)B; p.W = d.W; p.L = d.L;
-    p.tiles_per_cta = s.tiles_per_cta; p.feats_per_cta = s.feats_per_cta; p.chunks_per_cta = s.chunks_per_cta;
-    fill_epilogue(p, d, cw);
-    dim3 grid((unsigned)((B + kTcM - 1) / kTcM), s.n_ranges);
-    const int key = d.C * 10 + (d.K1 == 10 ? 0 : 1);
-    cudaError_t le;
-    switch (key) {
-#define SF_CASE(CC, AA) case CC * 10 + AA: le = launch_stream<CC, 1, AA, true, kOutGates>(tm, p, grid, st); break;
-        SF_CASE(1, 0) SF_CASE(2, 0) SF_CASE(3, 0) SF_CASE(1, 1) SF_CASE(2, 1) SF_CASE(3, 1)
-#undef SF_CASE
-        default: *err = "no fp32 stream instantiation for this channel count"; return -1;
-    }
-    if (le != cudaSuccess) { *err = cudaGetErrorString(le); return -1; }
-    int launches = 1;
-    if (slices_out) *slices_out = s.n_ranges;
-    int n = launch_frontend_generic_gates_listed(d, cw, x, B2CNN_DTYPE_F32, B, hw.wih0T, partial, s.n_ranges, list, count, st, num_sms, err);
-    if (n < 0) return -1;
-    launches += n;
-    n = reduce_here ? launch_reduce_gates(partial, s.n_ranges, B, hw, gates, st, err) : 0;
-    if (n < 0) return -1;
-    return launches + n;
 }
 
 }  // namespace b2cnn
