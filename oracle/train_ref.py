@@ -151,3 +151,28 @@ def assert_close_elem(name, got, truth, ref32, alpha=ALPHA, beta=BETA):
         raise AssertionError(f"{name}: {int(bad.sum())} of {got.size} elements off; worst at {i}: got {got[i]!r}, "
                              f"truth {truth[i]!r}, ref32 {ref32[i]!r} (bound {bound[i]:.3e}, max|truth| {scale:.3e}, "
                              f"beta would have to be {need:.2e})")
+
+
+def smallest_beta(got, truth, ref32, alpha=ALPHA):
+    """(the smallest beta :func:`assert_close_elem` would accept, the number of finite elements it judges); the beta is
+    <= 0 where every element lies inside alpha |ref32 - truth|, and 0.0 when no element is finite"""
+    got, truth, ref32 = (np.asarray(torch.as_tensor(t).detach().cpu().double()) for t in (got, truth, ref32))
+    fin = np.isfinite(truth) & np.isfinite(got)
+    if not fin.any():
+        return 0.0, 0
+    slack = np.nan_to_num(np.abs(ref32[fin] - truth[fin]), nan=0.0, posinf=0.0)
+    return float(((np.abs(got[fin] - truth[fin]) - alpha * slack) / np.abs(truth[fin]).max()).max()), int(fin.sum())
+
+
+def check_elems(pairs, label=""):
+    """:func:`assert_close_elem` on every ``(name, got, truth, ref32, beta)``, all failures reported together.  Prints,
+    per comparison, the smallest beta it would pass with and how many of its elements are finite (pytest -s shows it)."""
+    errors = []
+    for name, got, truth, ref32, beta in pairs:
+        b, n = smallest_beta(got, truth, ref32)
+        print(f"{label} {name}: smallest beta {b:.2e} (granted {beta:.2e}; {n} of {torch.as_tensor(truth).numel()} finite)")
+        try:
+            assert_close_elem(name, got, truth, ref32, beta=beta)
+        except AssertionError as e:
+            errors.append(str(e))
+    assert not errors, "\n".join(errors)

@@ -20,7 +20,7 @@ import torch
 import tskd_b200
 from oracle import mycnn_torch as O
 from oracle.infer_ref import TC_FEATURES_BETA, infer_reference
-from oracle.train_ref import ALPHA, BETA, assert_close_elem
+from oracle.train_ref import BETA, assert_close_elem, check_elems
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -152,27 +152,10 @@ def _to_dev(c, m, x):
     return xp
 
 
-def _smallest_beta(got, truth, ref32):
-    """the smallest beta assert_close_elem would accept (finite elements; <= 0: inside 8 |ref32 - truth| everywhere)"""
-    got, truth, ref32 = (np.asarray(torch.as_tensor(t).detach().cpu().double()) for t in (got, truth, ref32))
-    fin = np.isfinite(truth) & np.isfinite(got)
-    if not fin.any():
-        return 0.0
-    slack = np.nan_to_num(np.abs(ref32[fin] - truth[fin]), nan=0.0, posinf=0.0)
-    return float(((np.abs(got[fin] - truth[fin]) - ALPHA * slack) / np.abs(truth[fin]).max()).max())
-
-
 def _check(pairs):
-    """(name, got, truth, ref32, beta) per element; all failures reported together.  Prints the smallest beta each
-    comparison would pass with (pytest -s shows it)."""
-    errors = []
-    for name, got, truth, ref32, beta in pairs:
-        print(f"{os.environ.get('PYTEST_CURRENT_TEST', '').split(' ')[0]} {name}: smallest beta {_smallest_beta(got, truth, ref32):.2e} (granted {beta:.2e})")
-        try:
-            assert_close_elem(name, got, truth, ref32, beta=beta)
-        except AssertionError as e:
-            errors.append(str(e))
-    assert not errors, "\n".join(errors)
+    """(name, got, truth, ref32, beta) per element; all failures reported together; prints each comparison's smallest
+    passing beta and how many elements it judged (oracle/train_ref.py::check_elems)"""
+    check_elems(pairs, os.environ.get("PYTEST_CURRENT_TEST", "").split(" ")[0])
 
 
 # ------------------------------------------------------------------ per-path grants (beta per path and output)

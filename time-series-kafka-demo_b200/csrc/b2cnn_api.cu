@@ -512,7 +512,7 @@ static int forward_device(b2cnn_handle *h, const void *x, int dtype, int64_t B, 
         what = "front end";
         n = launch_frontend_generic(d, h->cw, x, dtype, B, feats, sB, sP, st, h->num_sms, &err);
     }
-    if (n < 0) return fail(B2CNN_ECUDA, std::string(what) + ": " + err);
+    if (n < 0) return fail(n == kLaunchArch ? B2CNN_EARCH : B2CNN_ECUDA, std::string(what) + ": " + err);
     int launches = n;
     if (prof) CU_TRY(cudaEventRecord(h->ev_stage[1], st));
     // stage 1: projection + LSTM head
@@ -584,7 +584,7 @@ extern "C" int b2cnn_features(b2cnn_handle *h, const void *x, int dtype, int64_t
         n = launch_frontend_generic(h->d, h->cw, x, dtype, B, feats, h->d.L, 1, (cudaStream_t)stream, h->num_sms, &err);
         h->last_path = B2CNN_PATH_GENERIC;
     }
-    if (n < 0) return fail(B2CNN_ECUDA, std::string("front end: ") + err);
+    if (n < 0) return fail(n == kLaunchArch ? B2CNN_EARCH : B2CNN_ECUDA, std::string("front end: ") + err);
     h->last_launches = n;
     return B2CNN_OK;
 }

@@ -319,7 +319,10 @@ static int launch_frontend_impl(const Dims &d, const ConvWeights &cw, const void
     p.xs_stride = padi(ni + d.PS * 4 + d.PK + d.K1 + 8) + 1;
     p.a1_stride = padi(nj + d.PS * 2 + d.PK + d.K2 + 8) + 1;
     const size_t smem = (size_t)(d.C * p.xs_stride + kCMid * p.a1_stride) * sizeof(float);
-    if (smem > 220 * 1024) { *err = "front end: tile does not fit shared memory (in_channels too large)"; return -1; }
+    if (smem > 220 * 1024) {
+        *err = "the generic front end's tile does not fit shared memory (in_channels * pool_s^2 too large for this window length)";
+        return kLaunchArch;
+    }
     int gx = p.n_tiles;
     if (gate_part) {                            // every slice of the partial buffer gets a CTA (empty ones write zeros)
         p.tiles_per_slice = (p.n_tiles + gate_slices - 1) / gate_slices;

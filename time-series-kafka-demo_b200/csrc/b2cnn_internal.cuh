@@ -89,7 +89,10 @@ __device__ __forceinline__ float sigmoid_acc(float v) { return 1.0f / (1.0f + ex
 __host__ __device__ __forceinline__ int padi(int g) { return g + (g >> 5); }
 
 // ---- launchers (b2cnn_generic.cu / b2cnn_head.cu) ----------------------------------------
-// Each returns the number of kernels it launched, or <0 with the message in `err`.
+// Each returns the number of kernels it launched, or <0 with the message in `err`: kLaunchArch when the
+// configuration exceeds what the kernel can hold (nothing was launched; the API reports B2CNN_EARCH), any other
+// negative value for a CUDA error.
+constexpr int kLaunchArch = -2;
 int launch_frontend_generic(const Dims &d, const ConvWeights &cw, const void *x, int dtype,
                             int64_t B, float *feats, int64_t sB, int64_t sP, cudaStream_t st,
                             int num_sms, const char **err);
