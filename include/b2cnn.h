@@ -230,7 +230,32 @@ int b2cnn_ring_push(b2cnn_ring *ring, const void *new_samples, int sample_kind, 
  *                        (parity tests); B2CNN_ESTATE before the first window is complete or when the weights
  *                        changed since the last reset.
  * The scorer's patients are independent windows; a push uses no atomics in its value path, so its results do not
- * depend on P, on the ring's rotation or on the run. */
+ * depend on P, on the ring's rotation or on the run.
+ *
+ * Per-patient lifecycle (a bed reassigned, a monitor reconnected).  Every patient p has seen[p]: its stream samples
+ * since its admission, or -1 once discharged.  b2cnn_slide_reset admits every patient with seen = 0; a push adds S to
+ * every admitted patient's count.  `patients` are HOST arrays of n distinct indices in [0, P).
+ *   b2cnn_slide_admit    restarts the listed patients' streams.  history: DEVICE pointer [n][C][history_len] in the
+ *                        scorer's dtype (`dtype` must name it), channel rows `pitch` elements apart (pitch >=
+ *                        history_len; any alignment), or NULL with history_len == 0; 0 <= history_len <= window.  Its
+ *                        last sample immediately precedes the next push's first one.  Then seen[p] = history_len, and
+ *                        p's window after a later push is the last W samples of (history | pushes since admission),
+ *                        defined once seen[p] >= W: with history_len == W at the very next push, and b2cnn_slide_features
+ *                        returns that window right away.  Computes the history's features that lie in the current
+ *                        window or a later one (the push kernels, into a scratch ring in
+ *                        `workspace`, then scattered into the patients' ring columns) and their last 24 samples.
+ *                        workspace: DEVICE, >= b2cnn_slide_admit_workspace_bytes(slide, n, history_len) bytes (else
+ *                        B2CNN_ESTATE); allocates nothing; asynchronous on `stream` except for two small host-to-device
+ *                        copies (the indices and the counts) from pageable memory.  B2CNN_ESTATE after
+ *                        b2cnn_set_weights without a reset, as for a push.
+ *   b2cnn_slide_discharge  seen[p] = -1 for the listed patients; their samples in later pushes are ignored.
+ *   b2cnn_slide_samples_seen  seen[P] into a DEVICE int64 array (asynchronous on `stream`).
+ * Once admit or discharge has been called (until the next reset), a push writes out[p] for patients with
+ * seen[p] >= W and NaN for every other patient, sets *emitted = 1 when at least one patient has a complete window
+ * (*window_index keeps its meaning, n - ceil(W / S), and may be negative), and b2cnn_slide_features writes NaN rows
+ * for patients without a complete window and fails with B2CNN_ESTATE when no patient has one.  A scorer that never
+ * calls either runs exactly the launches above.  Bad indices (out of range, listed twice), history_len outside
+ * [0, window], a NULL history with history_len > 0, pitch < history_len or another dtype: B2CNN_EINVAL. */
 typedef struct b2cnn_slide b2cnn_slide;
 int b2cnn_slide_create(b2cnn_handle *h, int32_t n_patients, int32_t stride, int dtype, b2cnn_slide **out);
 void b2cnn_slide_destroy(b2cnn_slide *slide);
@@ -238,6 +263,11 @@ int b2cnn_slide_reset(b2cnn_slide *slide, void *stream);
 int b2cnn_slide_push(b2cnn_slide *slide, const void *new_samples, int64_t pitch, const float *age, int64_t n_age,
                      int apply_sigmoid, float *out, int32_t *emitted, int64_t *window_index, void *stream);
 int b2cnn_slide_features(b2cnn_slide *slide, float *feats, void *stream);
+int64_t b2cnn_slide_admit_workspace_bytes(b2cnn_slide *slide, int32_t n, int64_t history_len);
+int b2cnn_slide_admit(b2cnn_slide *slide, const int32_t *patients, int32_t n, const void *history, int64_t history_len,
+                      int64_t pitch, int dtype, void *workspace, int64_t workspace_bytes, void *stream);
+int b2cnn_slide_discharge(b2cnn_slide *slide, const int32_t *patients, int32_t n, void *stream);
+int b2cnn_slide_samples_seen(b2cnn_slide *slide, int64_t *seen, void *stream);
 
 /* ---- The reference's wire formats, decoded on the device (SURVEY.md section 8, row f3) ----
  * A trigger's Kafka messages as one DEVICE byte buffer + offsets [n_msgs + 1] (message t = bytes[offsets[t] .. offsets[t+1])).

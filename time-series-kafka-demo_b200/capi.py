@@ -29,6 +29,7 @@ SYMBOLS = ("b2cnn_l_out", "b2cnn_weight_count", "b2cnn_create", "b2cnn_destroy",
            "b2cnn_prep_window_count", "b2cnn_prep_workspace_bytes", "b2cnn_prep_windows",
            "b2cnn_ring_create", "b2cnn_ring_destroy", "b2cnn_ring_reset", "b2cnn_ring_set_signals", "b2cnn_ring_push",
            "b2cnn_slide_create", "b2cnn_slide_destroy", "b2cnn_slide_reset", "b2cnn_slide_push", "b2cnn_slide_features",
+           "b2cnn_slide_admit_workspace_bytes", "b2cnn_slide_admit", "b2cnn_slide_discharge", "b2cnn_slide_samples_seen",
            "b2cnn_decode_sample_messages", "b2cnn_decode_array_messages", "b2cnn_parse_decimal", "b2cnn_frame_check")
 
 
@@ -121,6 +122,11 @@ def load_library() -> ctypes.CDLL:
     lib.b2cnn_slide_push.argtypes = [c_vp, c_vp, c_i64, c_vp, c_i64, c_int, c_vp, ctypes.POINTER(c_i32), ctypes.POINTER(c_i64), c_vp]
     lib.b2cnn_slide_push.restype = c_int
     lib.b2cnn_slide_features.argtypes = [c_vp, c_vp, c_vp]; lib.b2cnn_slide_features.restype = c_int
+    lib.b2cnn_slide_admit_workspace_bytes.argtypes = [c_vp, c_i32, c_i64]; lib.b2cnn_slide_admit_workspace_bytes.restype = c_i64
+    lib.b2cnn_slide_admit.argtypes = [c_vp, c_vp, c_i32, c_vp, c_i64, c_i64, c_int, c_vp, c_i64, c_vp]
+    lib.b2cnn_slide_admit.restype = c_int
+    lib.b2cnn_slide_discharge.argtypes = [c_vp, c_vp, c_i32, c_vp]; lib.b2cnn_slide_discharge.restype = c_int
+    lib.b2cnn_slide_samples_seen.argtypes = [c_vp, c_vp, c_vp]; lib.b2cnn_slide_samples_seen.restype = c_int
     lib.b2cnn_decode_sample_messages.argtypes = [c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_i64, c_i32, c_vp, c_vp]
     lib.b2cnn_decode_sample_messages.restype = c_int
     lib.b2cnn_decode_array_messages.argtypes = [c_vp, c_vp, c_i64, c_i32, c_vp, c_vp, c_vp, c_vp]

@@ -659,6 +659,37 @@ extern "C" int b2cnn_slide_features(b2cnn_slide *o, float *feats, void *stream) 
     return rc == B2CNN_OK ? rc : fail(rc, std::string("b2cnn_slide_features: ") + err);
 }
 
+extern "C" int64_t b2cnn_slide_admit_workspace_bytes(b2cnn_slide *o, int32_t n, int64_t history_len) {
+    return o ? slide_admit_workspace_bytes(o->s, n, history_len) : -1;
+}
+extern "C" int b2cnn_slide_admit(b2cnn_slide *o, const int32_t *patients, int32_t n, const void *history, int64_t history_len,
+                                 int64_t pitch, int dtype, void *workspace, int64_t workspace_bytes, void *stream) {
+    if (!o) return fail(B2CNN_EINVAL, "b2cnn_slide_admit: null argument");
+    if (dtype != slide_dtype(o->s)) return fail(B2CNN_EINVAL, "b2cnn_slide_admit: the history's dtype is not the scorer's");
+    if (o->gen != o->h->weight_gen)
+        return fail(B2CNN_ESTATE, "b2cnn_slide_admit: the handle's weights changed since the scorer's last reset (stored features are stale)");
+    b2cnn_handle *h = o->h;
+    DEVICE_GUARD(h->device);
+    const char *err = "";
+    const int rc = slide_admit(o->s, h->cw, h->tc, patients, n, history, history_len, pitch, workspace, workspace_bytes,
+                               reinterpret_cast<cudaStream_t>(stream), &err);
+    return rc == B2CNN_OK ? rc : fail(rc, std::string("b2cnn_slide_admit: ") + err);
+}
+extern "C" int b2cnn_slide_discharge(b2cnn_slide *o, const int32_t *patients, int32_t n, void *stream) {
+    if (!o) return fail(B2CNN_EINVAL, "b2cnn_slide_discharge: null argument");
+    DEVICE_GUARD(slide_device(o->s));
+    const char *err = "";
+    const int rc = slide_discharge(o->s, patients, n, reinterpret_cast<cudaStream_t>(stream), &err);
+    return rc == B2CNN_OK ? rc : fail(rc, std::string("b2cnn_slide_discharge: ") + err);
+}
+extern "C" int b2cnn_slide_samples_seen(b2cnn_slide *o, int64_t *seen, void *stream) {
+    if (!o || !seen) return fail(B2CNN_EINVAL, "b2cnn_slide_samples_seen: null argument");
+    DEVICE_GUARD(slide_device(o->s));
+    const char *err = "";
+    const int rc = slide_samples_seen(o->s, seen, reinterpret_cast<cudaStream_t>(stream), &err);
+    return rc == B2CNN_OK ? rc : fail(rc, std::string("b2cnn_slide_samples_seen: ") + err);
+}
+
 // ---- host-pointer entry: chunked H2D overlapped with compute -----------------------------
 static int ensure_host_staging(b2cnn_handle *h, size_t x_chunk_bytes, int64_t B, size_t ws_bytes) {
     if (!h->s_copy) {

@@ -21,8 +21,17 @@
 //     (G_n + j) mod L, split-K over the streaming kernels' position ranges (they depend on L only) ->
 //     partial[range][P][64]; then the head kernel of the independent forward sums the ranges in fixed order and runs
 //     the LSTM cells, Linear, age scale and sigmoid.
+//
+// Per-patient lifecycle (b2cnn_slide_admit / _discharge): seen[p] counts patient p's samples since its admission (-1:
+// discharged); its window after a push is the last W samples of (history | pushes since admission), defined once
+// seen[p] >= W.  An admission with history is a push of the listed patients aimed at a k-patient scratch ring (the same
+// tensor-core / exact kernels), scattered into their ring columns, plus their tail.  Pushes then run unchanged for all
+// P patients; slide_live_kernel advances seen and writes NaN for patients without a complete window.  None of this
+// runs for a scorer that never admitted or discharged a patient since its last reset.
+#include <algorithm>
 #include <cstring>
 #include <new>
+#include <vector>
 
 #include "b2cnn_slide.cuh"
 #include "b2cnn_tc_ptx.cuh"
@@ -46,9 +55,17 @@ struct Slide {
     int *flags = nullptr;            // flags [P] | list [P] | count
     void *stage = nullptr;           // [P][C][Sp] in the window dtype
     int64_t Sp = 0;
+    bool lifecycle = false;          // set by the first admit / discharge since the last reset
+    int64_t *seen = nullptr;         // [P] on the device: samples since admission, -1: discharged (while lifecycle)
+    std::vector<int64_t> seen_h;     // its host mirror, equal to it in stream order
 };
 
 static int64_t fdiv4(int64_t a) { return a >= 0 ? a / 4 : -((-a + 3) / 4); }
+// a mod m in [0, m): stream features before sample 0 (negative g) exist once a patient is admitted with history
+__host__ __device__ __forceinline__ int64_t mod_nn(int64_t a, int64_t m) {
+    const int64_t r = a % m;
+    return r < 0 ? r + m : r;
+}
 
 template <typename T>
 __device__ __forceinline__ float ld_sample(const T *p);
@@ -124,7 +141,7 @@ template <int C, int K1, int PK, typename Tin>
 __global__ void __launch_bounds__(128) slide_exact_kernel(const __grid_constant__ SlideExactParams p) {
     auto store = [&](int b, int gi) {
         const int64_t g = p.g0 + gi;
-        p.ring[(g % p.cap) * p.ring_pitch + b] = exact_feature<C, K1, PK, Tin>(p, b, g);
+        p.ring[mod_nn(g, p.cap) * p.ring_pitch + b] = exact_feature<C, K1, PK, Tin>(p, b, g);
     };
     if (!p.list) {
         const int b = blockIdx.x * blockDim.x + threadIdx.x;
@@ -292,6 +309,43 @@ __global__ void slide_gather_kernel(const float *__restrict__ ring, int64_t pitc
     for (int j = blockIdx.y; j < L; j += gridDim.y) feats[(int64_t)b * L + j] = ring[(int64_t)((head + j) % cap) * pitch + b];
 }
 
+// ---- lifecycle kernels ------------------------------------------------------------------------------------------
+// ring[(g mod L)][idx[j]] = scratch[(g mod cap)][j], g in [g0, g0 + ng): an admission's features into the ring
+__global__ void slide_scatter_kernel(const float *__restrict__ scratch, int64_t spitch, int cap, const int *__restrict__ idx, int k,
+                                     int64_t g0, int ng, float *__restrict__ ring, int64_t rpitch, int L) {
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= k) return;
+    const int q = idx[j];
+    for (int i = blockIdx.y; i < ng; i += gridDim.y) {
+        const int64_t g = g0 + i;
+        ring[mod_nn(g, L) * rpitch + q] = scratch[mod_nn(g, cap) * spitch + j];
+    }
+}
+
+// tail rows of the admitted patients = the last kSlideTail samples of their history [k][C][pitch] (zeros in front of
+// a shorter one: they only reach features that start before the history, which no valid window holds)
+template <typename Tin>
+__global__ void slide_admit_tail_kernel(const Tin *__restrict__ h, int64_t pitch, int64_t H, const int *__restrict__ idx, int k,
+                                        int C, float *__restrict__ tail) {
+    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= (int64_t)k * C * kSlideTail) return;
+    const int64_t r = e / kSlideTail;                     // history row j * C + c
+    const int u = (int)(e % kSlideTail);
+    const int64_t t = H - kSlideTail + u;
+    tail[((int64_t)idx[r / C] * C + r % C) * kSlideTail + u] = t >= 0 ? ld_sample<Tin>(h + r * pitch + t) : 0.f;
+}
+
+// seen[b] += adv for admitted patients (seen >= 0); then row b of x [P][len] = NaN unless seen[b] >= W.
+// adv != 0 only with gridDim.y == 1 (one thread per patient reads and writes seen).
+__global__ void slide_live_kernel(int64_t *__restrict__ seen, int P, int64_t adv, int64_t W, float *__restrict__ x, int64_t len) {
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= P) return;
+    int64_t v = seen[b];
+    if (adv != 0 && v >= 0) seen[b] = v += adv;
+    if (!x || v >= W) return;
+    for (int64_t j = blockIdx.y; j < len; j += gridDim.y) x[b * len + j] = __int_as_float(0x7fc00000);
+}
+
 // ------------------------------------------------------------------------------------------
 template <int C, int K1, int PK>
 static void launch_exact_t(const SlideExactParams &p, int dtype, dim3 grid, cudaStream_t st) {
@@ -299,15 +353,11 @@ static void launch_exact_t(const SlideExactParams &p, int dtype, dim3 grid, cuda
     else slide_exact_kernel<C, K1, PK, __nv_bfloat16><<<grid, 128, 0, st>>>(p);
 }
 
-// features [g0, g0 + ng) exactly: of every patient (list == nullptr) or of the listed ones
-static int launch_exact(const Slide &s, const ConvWeights &cw, const void *x, int64_t pitch, const float *tail, int64_t g0,
-                        int64_t ng, const int *list, const int *count, cudaStream_t st, const char **err) {
+// features [p.g0, p.g0 + ng) exactly into p.ring: of every one of its p.P rows (p.list == nullptr) or of the listed ones
+static int launch_exact_p(SlideExactParams p, const Slide &s, int64_t ng, cudaStream_t st, const char **err) {
     if (ng <= 0) return 0;
-    SlideExactParams p;
-    memset(&p, 0, sizeof p);
-    p.x = x; p.pitch = pitch; p.tail = tail; p.ring = s.ring; p.ring_pitch = s.ring_pitch; p.cap = s.d.L; p.P = s.P;
-    p.g0 = g0; p.ng = (int)ng; p.seg0 = s.n * s.S; p.phi = s.phi; p.list = list; p.count = count; p.cw = cw;
-    const dim3 grid = list ? dim3((unsigned)((ng + 127) / 128), 16) : dim3((unsigned)((s.P + 127) / 128), (unsigned)ng);
+    p.ng = (int)ng;
+    const dim3 grid = p.list ? dim3((unsigned)((ng + 127) / 128), 16) : dim3((unsigned)((p.P + 127) / 128), (unsigned)ng);
     const int key = s.d.C * 10 + (s.d.K1 == 10 ? 0 : 1);
     switch (key) {
         case 10: launch_exact_t<1, 10, 3>(p, s.dtype, grid, st); break;
@@ -320,6 +370,17 @@ static int launch_exact(const Slide &s, const ConvWeights &cw, const void *x, in
     }
     if (cudaGetLastError() != cudaSuccess) { *err = "exact feature kernel launch"; return -1; }
     return 1;
+}
+
+// features [g0, g0 + ng) of the pushed segment exactly into the scorer's ring: of every patient (list == nullptr) or
+// of the listed ones
+static int launch_exact(const Slide &s, const ConvWeights &cw, const void *x, int64_t pitch, const float *tail, int64_t g0,
+                        int64_t ng, const int *list, const int *count, cudaStream_t st, const char **err) {
+    SlideExactParams p;
+    memset(&p, 0, sizeof p);
+    p.x = x; p.pitch = pitch; p.tail = tail; p.ring = s.ring; p.ring_pitch = s.ring_pitch; p.cap = s.d.L; p.P = s.P;
+    p.g0 = g0; p.seg0 = s.n * s.S; p.phi = s.phi; p.list = list; p.count = count; p.cw = cw;
+    return launch_exact_p(p, s, ng, st, err);
 }
 
 int slide_create(const Dims &d, const TcState &tc, int n_patients, int stride, int dtype, int device, Slide **out,
@@ -347,7 +408,8 @@ int slide_create(const Dims &d, const TcState &tc, int n_patients, int stride, i
               cudaMalloc(&s->tail, sizeof(float) * (size_t)2 * P * d.C * kSlideTail) == cudaSuccess &&
               cudaMalloc(&s->partial, sizeof(float) * (size_t)s->ranges * P * kGates) == cudaSuccess &&
               cudaMalloc(&s->flags, sizeof(int) * (size_t)(2 * P + 1)) == cudaSuccess &&
-              cudaMalloc(&s->stage, (size_t)(P * d.C * s->Sp * esz)) == cudaSuccess;
+              cudaMalloc(&s->stage, (size_t)(P * d.C * s->Sp * esz)) == cudaSuccess &&
+              cudaMalloc(&s->seen, sizeof(int64_t) * (size_t)P) == cudaSuccess;
     if (!ok) { (void)cudaGetLastError(); slide_destroy(s); *err = "cudaMalloc(scorer state)"; return B2CNN_ECUDA; }
     *out = s;
     return B2CNN_OK;
@@ -355,14 +417,15 @@ int slide_create(const Dims &d, const TcState &tc, int n_patients, int stride, i
 
 void slide_destroy(Slide *s) {
     if (!s) return;
-    cudaFree(s->ring); cudaFree(s->tail); cudaFree(s->partial); cudaFree(s->flags); cudaFree(s->stage);
+    cudaFree(s->ring); cudaFree(s->tail); cudaFree(s->partial); cudaFree(s->flags); cudaFree(s->stage); cudaFree(s->seen);
     delete s;
 }
 
 int slide_device(const Slide *s) { return s->device; }
+int slide_dtype(const Slide *s) { return s->dtype; }
 
 int slide_reset(Slide *s, cudaStream_t st, const char **err) {
-    s->n = 0; s->g_done = -1; s->tail_cur = 0;
+    s->n = 0; s->g_done = -1; s->tail_cur = 0; s->lifecycle = false;
     if (cudaMemsetAsync(s->tail, 0, sizeof(float) * (size_t)2 * s->P * s->d.C * kSlideTail, st) != cudaSuccess) {
         *err = "memset tail"; return B2CNN_ECUDA;
     }
@@ -371,6 +434,23 @@ int slide_reset(Slide *s, cudaStream_t st, const char **err) {
 
 static int64_t window_head(const Slide &s, int64_t n) { return fdiv4(n * s.S - s.d.W - s.phi); }
 
+// slide_live_kernel over the P patients: seen += adv, then NaN rows of x [P][len] without a complete window
+static int launch_live(const Slide &s, int64_t adv, float *x, int64_t len, cudaStream_t st, const char **err) {
+    const unsigned gy = adv != 0 || len <= 1 ? 1u : (unsigned)std::min<int64_t>(len, 64);
+    slide_live_kernel<<<dim3((unsigned)((s.P + 127) / 128), gy), 128, 0, st>>>(s.seen, s.P, adv, s.d.W, x, len);
+    if (cudaGetLastError() != cudaSuccess) { *err = "lifecycle mask launch"; return -1; }
+    return 1;
+}
+
+// a push's lifecycle step: the device counts advance by S (and out[P] gets its NaNs), then the host mirror -- only once
+// the launch went out, so that the two never disagree
+static int advance_seen(Slide *s, float *out, cudaStream_t st, const char **err) {
+    if (launch_live(*s, s->S, out, 1, st, err) < 0) return -1;
+    for (int64_t &v : s->seen_h)
+        if (v >= 0) v += s->S;
+    return 1;
+}
+
 int slide_push(Slide *s, const ConvWeights &cw, const HeadWeights &hw, const TcState &tc, const void *x, int64_t pitch,
                const float *age, int64_t n_age, int apply_sigmoid, float *out, int *emitted, int64_t *window_index,
                cudaEvent_t *ev, cudaStream_t st, const char **err) {
@@ -378,13 +458,13 @@ int slide_push(Slide *s, const ConvWeights &cw, const HeadWeights &hw, const TcS
     const int64_t P = s->P, S = s->S, esz = s->dtype == B2CNN_DTYPE_BF16 ? 2 : 4;
     if (pitch < S) { *err = "pitch must be >= stride"; return B2CNN_EINVAL; }
     if (n_age != 1 && n_age != P) { *err = "age must have 1 or n_patients elements"; return B2CNN_EINVAL; }
+    if (tc.n_ranges != s->ranges) { *err = "the handle's position ranges changed since create"; return B2CNN_ESTATE; }
     const int64_t n1 = s->n + 1;
     const int64_t g_hi = fdiv4(n1 * S - s->R - s->phi);      // last feature whose samples have all arrived
     const int64_t g_m0 = s->n * S / 4;                        // first feature that starts inside the segment
     int64_t g_lo = s->g_done + 1;
     const int64_t G = window_head(*s, n1);
     if (g_lo < G) g_lo = G;                                   // earlier features never enter a window
-    if (g_lo < 0) g_lo = 0;
     const float *tail_in = s->tail + (size_t)s->tail_cur * P * d.C * kSlideTail;
     float *tail_out = s->tail + (size_t)(s->tail_cur ^ 1) * P * d.C * kSlideTail;
     if (ev && cudaEventRecord(ev[0], st) != cudaSuccess) { *err = "cudaEventRecord"; return B2CNN_ECUDA; }
@@ -434,14 +514,17 @@ int slide_push(Slide *s, const ConvWeights &cw, const HeadWeights &hw, const TcS
     if (g_hi >= g_lo) s->g_done = g_hi;
     s->tail_cur ^= 1;
 
-    // ---- projection over the ring + head, once the first window is complete
+    // ---- projection over the ring + head, once a window is complete (every patient's, or with the lifecycle on, one)
+    bool live = n1 * S >= d.W;
+    if (s->lifecycle)
+        live = std::any_of(s->seen_h.begin(), s->seen_h.end(), [&](int64_t v) { return v >= 0 && v + S >= d.W; });
     *emitted = 0;
-    if (n1 * S < d.W) {
+    if (!live) {
+        if (s->lifecycle && advance_seen(s, nullptr, st, err) < 0) return B2CNN_ECUDA;
         if (ev && cudaEventRecord(ev[2], st) != cudaSuccess) { *err = "cudaEventRecord"; return B2CNN_ECUDA; }
         return B2CNN_OK;
     }
-    const int head = (int)(G % d.L);
-    if (tc.n_ranges != s->ranges) { *err = "the handle's position ranges changed since create"; return B2CNN_ESTATE; }
+    const int head = (int)mod_nn(G, d.L);
     CUtensorMap tm;
     if (tc_ring_tmap(s->ring, P, s->ring_pitch, d.L, &tm, err) != 0) return B2CNN_ECUDA;
     RingProjParams rp;
@@ -454,6 +537,7 @@ int slide_push(Slide *s, const ConvWeights &cw, const HeadWeights &hw, const TcS
     slide_ring_proj_kernel<<<dim3((unsigned)((P + kRpM - 1) / kRpM), (unsigned)s->ranges), kRpThreads, kRpSmem, st>>>(tm, rp);
     if (cudaGetLastError() != cudaSuccess) { *err = "projection launch"; return B2CNN_ECUDA; }
     if (launch_reduce_lstm_head(d, hw, s->partial, s->ranges, P, age, n_age, apply_sigmoid, out, st, err) < 0) return B2CNN_ECUDA;
+    if (s->lifecycle && advance_seen(s, out, st, err) < 0) return B2CNN_ECUDA;
     if (ev && cudaEventRecord(ev[2], st) != cudaSuccess) { *err = "cudaEventRecord"; return B2CNN_ECUDA; }
     *emitted = 1;
     *window_index = n1 - (d.W + S - 1) / S;
@@ -461,10 +545,175 @@ int slide_push(Slide *s, const ConvWeights &cw, const HeadWeights &hw, const TcS
 }
 
 int slide_features(const Slide *s, float *feats, cudaStream_t st, const char **err) {
-    if (s->n * s->S < s->d.W) { *err = "no window yet: the first window is still filling"; return B2CNN_ESTATE; }
-    const int head = (int)(window_head(*s, s->n) % s->d.L);
+    bool live = s->n * s->S >= s->d.W;
+    if (s->lifecycle) live = std::any_of(s->seen_h.begin(), s->seen_h.end(), [&](int64_t v) { return v >= s->d.W; });
+    if (!live) { *err = "no window yet: no patient's window is complete"; return B2CNN_ESTATE; }
+    const int head = (int)mod_nn(window_head(*s, s->n), s->d.L);
     slide_gather_kernel<<<dim3((unsigned)((s->P + 127) / 128), 64), 128, 0, st>>>(s->ring, s->ring_pitch, s->d.L, s->P, head, s->d.L, feats);
     if (cudaGetLastError() != cudaSuccess) { *err = "gather launch"; return B2CNN_ECUDA; }
+    if (s->lifecycle && launch_live(*s, 0, feats, s->d.L, st, err) < 0) return B2CNN_ECUDA;
+    return B2CNN_OK;
+}
+
+// ---- per-patient lifecycle ----------------------------------------------------------------------------------------
+static int check_patients(const Slide &s, const int *patients, int64_t k, const char **err) {
+    if (k < 0 || k > s.P) { *err = "patient count must be in [0, n_patients]"; return B2CNN_EINVAL; }
+    if (k > 0 && !patients) { *err = "null patient indices"; return B2CNN_EINVAL; }
+    std::vector<char> hit((size_t)s.P, 0);
+    for (int64_t j = 0; j < k; ++j) {
+        const int q = patients[j];
+        if (q < 0 || q >= s.P) { *err = "patient index out of range"; return B2CNN_EINVAL; }
+        if (hit[q]) { *err = "patient index listed twice"; return B2CNN_EINVAL; }
+        hit[q] = 1;
+    }
+    return B2CNN_OK;
+}
+
+// the counts after a lifecycle call: before the first one every patient has seen the whole stream
+static std::vector<int64_t> next_seen(const Slide &s, const int *patients, int64_t k, int64_t value) {
+    std::vector<int64_t> v = s.lifecycle ? s.seen_h : std::vector<int64_t>((size_t)s.P, s.n * s.S);
+    for (int64_t j = 0; j < k; ++j) v[patients[j]] = value;
+    return v;
+}
+
+// uploads `next` (pageable: the driver has copied it when the call returns) and makes it the host mirror; called after
+// every other launch of the lifecycle call succeeded, so a failed call leaves the lifecycle state as it was
+static int commit_seen(Slide *s, std::vector<int64_t> &next, cudaStream_t st, const char **err) {
+    if (cudaMemcpyAsync(s->seen, next.data(), sizeof(int64_t) * (size_t)s->P, cudaMemcpyHostToDevice, st) != cudaSuccess) {
+        *err = "copy of the sample counts"; return B2CNN_ECUDA;
+    }
+    s->seen_h.swap(next);
+    s->lifecycle = true;
+    return B2CNN_OK;
+}
+
+// workspace of an admission of k patients with H history samples: scratch ring [cap][round_up(k, 4)] fp32 (cap: the
+// features that fit in H samples, at most L) | flags [k] + list [k] + count | indices [k] | staging rows
+// [k][C][round_up(H, 8)] in the window dtype (always counted: an unaligned or phase-shifted history is copied there)
+struct AdmitLayout {
+    int64_t kp, cap, hp;
+    size_t scratch, flags, idx, stage, total;
+};
+static size_t al256(size_t b) { return (b + 255) & ~(size_t)255; }
+static AdmitLayout admit_layout(const Slide &s, int64_t k, int64_t H) {
+    AdmitLayout a;
+    const int64_t esz = s.dtype == B2CNN_DTYPE_BF16 ? 2 : 4;
+    a.kp = (k + 3) & ~3;
+    a.cap = H >= s.R ? std::min<int64_t>((H - s.R) / 4 + 1, s.d.L) : 0;
+    a.hp = (H + 7) & ~7;
+    a.scratch = al256(sizeof(float) * (size_t)(a.cap * a.kp));
+    a.flags = al256(sizeof(int) * (size_t)(2 * k + 1));
+    a.idx = al256(sizeof(int) * (size_t)k);
+    a.stage = al256((size_t)(k * s.d.C * a.hp * esz));
+    a.total = a.scratch + a.flags + a.idx + a.stage;
+    return a;
+}
+
+int64_t slide_admit_workspace_bytes(const Slide *s, int64_t k, int64_t H) {
+    if (k < 0 || k > s->P || H < 0 || H > s->d.W) return -1;
+    return (int64_t)admit_layout(*s, k, H).total;
+}
+
+int slide_admit(Slide *s, const ConvWeights &cw, const TcState &tc, const int *patients, int64_t k, const void *hist, int64_t H,
+                int64_t pitch, void *ws, int64_t ws_bytes, cudaStream_t st, const char **err) {
+    const Dims &d = s->d;
+    int rc = check_patients(*s, patients, k, err);
+    if (rc != B2CNN_OK) return rc;
+    if (H < 0 || H > d.W) { *err = "history length must be in [0, window]"; return B2CNN_EINVAL; }
+    if (H > 0 && !hist) { *err = "null history with a positive length"; return B2CNN_EINVAL; }
+    if (H > 0 && pitch < H) { *err = "history pitch must be >= its length"; return B2CNN_EINVAL; }
+    if (k == 0) return B2CNN_OK;
+    const AdmitLayout a = admit_layout(*s, k, H);
+    if (!ws || ws_bytes < (int64_t)a.total) {
+        *err = "workspace missing or smaller than b2cnn_slide_admit_workspace_bytes()"; return B2CNN_ESTATE;
+    }
+    char *base = static_cast<char *>(ws);
+    float *scratch = reinterpret_cast<float *>(base);
+    int *flags = reinterpret_cast<int *>(base + a.scratch);
+    int *idx = reinterpret_cast<int *>(base + a.scratch + a.flags);
+    void *stage = base + a.scratch + a.flags + a.idx;
+
+    if (cudaMemcpyAsync(idx, patients, sizeof(int) * (size_t)k, cudaMemcpyHostToDevice, st) != cudaSuccess) {
+        *err = "copy of the patient indices"; return B2CNN_ECUDA;
+    }
+    const int64_t esz = s->dtype == B2CNN_DTYPE_BF16 ? 2 : 4;
+    // the history is stream samples [nS - H, nS): the features wholly inside it that lie in the current window n
+    // (features() may read it before the next push) or can still enter a later one
+    const int64_t nS = s->n * s->S;
+    const int64_t g_lo = std::max(-fdiv4(-(nS - H - s->phi)), window_head(*s, s->n));
+    const int64_t g_hi = fdiv4(nS - s->R - s->phi);
+    const int64_t Q = g_hi - g_lo + 1;
+    if (H > 0 && Q > 0) {
+        const int cap = (int)Q;                                        // Q <= a.cap
+        const int64_t off = 4 * g_lo + s->phi - (nS - H);               // (H - W) mod 4 + 4 (g_lo - first feature inside)
+        SlideExactParams p;
+        memset(&p, 0, sizeof p);
+        p.x = hist; p.pitch = pitch; p.tail = s->tail; p.ring = scratch; p.ring_pitch = a.kp; p.cap = cap; p.P = (int)k;
+        p.g0 = g_lo; p.seg0 = nS - H; p.phi = s->phi; p.cw = cw;
+        if (Q >= 32) {
+            const int unit = 16 / (int)esz;
+            const void *xin = hist;
+            int64_t xp = pitch;
+            if (off != 0 || pitch % unit != 0 || (reinterpret_cast<uintptr_t>(hist) & 15) != 0) {
+                const int64_t rows = k * d.C;
+                const unsigned blocks = (unsigned)std::min<int64_t>((rows * a.hp + 255) / 256, 65536);
+                if (esz == 2)
+                    slide_stage_kernel<uint16_t><<<blocks, 256, 0, st>>>(reinterpret_cast<const uint16_t *>(hist), pitch, (int)off,
+                                                                         (int)(H - off), reinterpret_cast<uint16_t *>(stage), a.hp, rows);
+                else
+                    slide_stage_kernel<float><<<blocks, 256, 0, st>>>(reinterpret_cast<const float *>(hist), pitch, (int)off,
+                                                                      (int)(H - off), reinterpret_cast<float *>(stage), a.hp, rows);
+                if (cudaGetLastError() != cudaSuccess) { *err = "staging launch"; return B2CNN_ECUDA; }
+                xin = stage; xp = a.hp;
+            }
+            Dims dh = d;
+            dh.W = (int)(H - off); dh.L = cap; dh.XP = (int)xp;
+            if (cudaMemsetAsync(flags, 0, sizeof(int) * (size_t)(2 * k + 1), st) != cudaSuccess) { *err = "memset flags"; return B2CNN_ECUDA; }
+            if (tc_ring_features(tc, dh, cw, xin, xp, s->dtype, k, scratch, a.kp, cap, (int)mod_nn(g_lo, cap), flags, st, err) < 0)
+                return B2CNN_ECUDA;
+            p.list = flags + k; p.count = flags + 2 * k;                // flagged histories: exact, over all Q features
+        }
+        if (launch_exact_p(p, *s, Q, st, err) < 0) return B2CNN_ECUDA;
+        const unsigned gy = (unsigned)std::min<int64_t>(Q, 1024);
+        slide_scatter_kernel<<<dim3((unsigned)((k + 127) / 128), gy), 128, 0, st>>>(scratch, a.kp, cap, idx, (int)k, g_lo, (int)Q,
+                                                                                   s->ring, s->ring_pitch, d.L);
+        if (cudaGetLastError() != cudaSuccess) { *err = "scatter launch"; return B2CNN_ECUDA; }
+    }
+    // the next push's seam features read the history's last samples from the current tail
+    float *tail = s->tail + (size_t)s->tail_cur * s->P * d.C * kSlideTail;
+    const int64_t total = k * d.C * kSlideTail;
+    if (esz == 2)
+        slide_admit_tail_kernel<__nv_bfloat16><<<(unsigned)((total + 255) / 256), 256, 0, st>>>(
+            reinterpret_cast<const __nv_bfloat16 *>(hist), pitch, H, idx, (int)k, d.C, tail);
+    else
+        slide_admit_tail_kernel<float><<<(unsigned)((total + 255) / 256), 256, 0, st>>>(reinterpret_cast<const float *>(hist), pitch, H,
+                                                                                        idx, (int)k, d.C, tail);
+    if (cudaGetLastError() != cudaSuccess) { *err = "tail launch"; return B2CNN_ECUDA; }
+    std::vector<int64_t> next = next_seen(*s, patients, k, H);
+    if ((rc = commit_seen(s, next, st, err)) != B2CNN_OK) return rc;
+    // features from the history's last complete one on are seam features of the next push, for every patient (before
+    // sample 0 of the stream they have negative indices: the other patients' copies of them are never read)
+    if (H > 0 && g_hi < s->g_done) s->g_done = g_hi;
+    return B2CNN_OK;
+}
+
+int slide_discharge(Slide *s, const int *patients, int64_t k, cudaStream_t st, const char **err) {
+    const int rc = check_patients(*s, patients, k, err);
+    if (rc != B2CNN_OK || k == 0) return rc;
+    std::vector<int64_t> next = next_seen(*s, patients, k, -1);
+    return commit_seen(s, next, st, err);
+}
+
+int slide_samples_seen(Slide *s, int64_t *out, cudaStream_t st, const char **err) {
+    const size_t bytes = sizeof(int64_t) * (size_t)s->P;
+    cudaError_t e;
+    if (s->lifecycle) {
+        e = cudaMemcpyAsync(out, s->seen, bytes, cudaMemcpyDeviceToDevice, st);
+    } else {
+        s->seen_h.assign((size_t)s->P, s->n * s->S);
+        e = cudaMemcpyAsync(out, s->seen_h.data(), bytes, cudaMemcpyHostToDevice, st);
+    }
+    if (e != cudaSuccess) { *err = "copy of the sample counts"; return B2CNN_ECUDA; }
     return B2CNN_OK;
 }
 

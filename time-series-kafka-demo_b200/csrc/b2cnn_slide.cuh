@@ -16,5 +16,12 @@ int slide_push(Slide *s, const ConvWeights &cw, const HeadWeights &hw, const TcS
                const float *age, int64_t n_age, int apply_sigmoid, float *out, int *emitted, int64_t *window_index,
                cudaEvent_t *ev, cudaStream_t st, const char **err);
 int slide_features(const Slide *s, float *feats, cudaStream_t st, const char **err);
+// per-patient lifecycle: `patients` host indices; `hist` [k][C][pitch] device samples in the scorer's dtype
+int64_t slide_admit_workspace_bytes(const Slide *s, int64_t k, int64_t H);
+int slide_admit(Slide *s, const ConvWeights &cw, const TcState &tc, const int *patients, int64_t k, const void *hist, int64_t H,
+                int64_t pitch, void *ws, int64_t ws_bytes, cudaStream_t st, const char **err);
+int slide_discharge(Slide *s, const int *patients, int64_t k, cudaStream_t st, const char **err);
+int slide_samples_seen(Slide *s, int64_t *out, cudaStream_t st, const char **err);
+int slide_dtype(const Slide *s);
 
 }  // namespace b2cnn
