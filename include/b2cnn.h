@@ -255,9 +255,24 @@ int b2cnn_ring_push(b2cnn_ring *ring, const void *new_samples, int sample_kind, 
  * (*window_index keeps its meaning, n - ceil(W / S), and may be negative), and b2cnn_slide_features writes NaN rows
  * for patients without a complete window and fails with B2CNN_ESTATE when no patient has one.  A scorer that never
  * calls either runs exactly the launches above.  Bad indices (out of range, listed twice), history_len outside
- * [0, window], a NULL history with history_len > 0, pitch < history_len or another dtype: B2CNN_EINVAL. */
+ * [0, window], a NULL history with history_len > 0, pitch < history_len or another dtype: B2CNN_EINVAL.
+ *
+ * Two implementations (DESIGN.md §6).  b2cnn_slide_create is the tensor-core path described above.
+ *   b2cnn_slide_create_path  the same with a path: B2CNN_PATH_TENSORCORE is exactly b2cnn_slide_create;
+ *                        B2CNN_PATH_GENERIC is exact fp32 on CUDA cores for every model b2cnn_create accepts (any channel
+ *                        count, activation, affine and conv/pool geometry): the feature stride is F = pool_s^2 samples,
+ *                        so stride % F == 0 (else B2CNN_EINVAL), and each patient keeps its last R - 1 samples, R =
+ *                        pool_s (pool_k + k2 - 2) + pool_k + k1 - 1 the receptive field of one feature.  Its logits are
+ *                        b2cnn_forward's with path = generic and small_kernel = 0 on the same windows.  B2CNN_EARCH, before
+ *                        allocating anything, where b2cnn_forward on the whole windows would refuse the generic front end
+ *                        (its tile does not fit shared memory).  B2CNN_PATH_AUTO: the tensor-core path where
+ *                        b2cnn_slide_create succeeds, the generic path where it returns B2CNN_EARCH.  Any other path:
+ *                        B2CNN_EINVAL.  Every b2cnn_slide_* call works on either path with the semantics above.
+ *   b2cnn_slide_path     B2CNN_PATH_TENSORCORE or B2CNN_PATH_GENERIC: the path a scorer runs (-1 for NULL). */
 typedef struct b2cnn_slide b2cnn_slide;
 int b2cnn_slide_create(b2cnn_handle *h, int32_t n_patients, int32_t stride, int dtype, b2cnn_slide **out);
+int b2cnn_slide_create_path(b2cnn_handle *h, int32_t n_patients, int32_t stride, int dtype, int path, b2cnn_slide **out);
+int b2cnn_slide_path(const b2cnn_slide *slide);
 void b2cnn_slide_destroy(b2cnn_slide *slide);
 int b2cnn_slide_reset(b2cnn_slide *slide, void *stream);
 int b2cnn_slide_push(b2cnn_slide *slide, const void *new_samples, int64_t pitch, const float *age, int64_t n_age,

@@ -592,24 +592,37 @@ extern "C" int b2cnn_features(b2cnn_handle *h, const void *x, int dtype, int64_t
 // ---- sliding-window scorer over a per-patient feature ring (b2cnn_slide.cu) ----
 struct b2cnn_slide { Slide *s; b2cnn_handle *h; uint64_t gen; };
 
-extern "C" int b2cnn_slide_create(b2cnn_handle *h, int32_t n_patients, int32_t stride, int dtype, b2cnn_slide **out) {
-    if (!h || !out) return fail(B2CNN_EINVAL, "b2cnn_slide_create: null argument");
+static int slide_create_on(const char *fn, b2cnn_handle *h, int32_t n_patients, int32_t stride, int dtype, int path, b2cnn_slide **out) {
+    if (!h || !out) return fail(B2CNN_EINVAL, std::string(fn) + ": null argument");
     *out = nullptr;
-    if (!h->weights_set) return fail(B2CNN_ESTATE, "b2cnn_slide_create: weights not set (call b2cnn_set_weights)");
+    if (path != B2CNN_PATH_TENSORCORE && path != B2CNN_PATH_GENERIC && path != B2CNN_PATH_AUTO)
+        return fail(B2CNN_EINVAL, std::string(fn) + ": path must be B2CNN_PATH_AUTO, B2CNN_PATH_GENERIC or B2CNN_PATH_TENSORCORE");
+    if (!h->weights_set) return fail(B2CNN_ESTATE, std::string(fn) + ": weights not set (call b2cnn_set_weights)");
     DEVICE_GUARD(h->device);
     const char *err = "";
     Slide *s = nullptr;
-    const int rc = slide_create(h->d, h->tc, n_patients, stride, dtype, h->device, &s, &err);
-    if (rc != B2CNN_OK) return fail(rc, std::string("b2cnn_slide_create: ") + err);
+    // auto: the tensor-core path where it holds the model (slide_create refuses everything else with B2CNN_EARCH; its
+    // geometries have F = 4, so a stride it refuses the generic path refuses too), else the generic path
+    const bool tc = path == B2CNN_PATH_TENSORCORE || (path == B2CNN_PATH_AUTO && h->tc.fused);
+    const int rc = tc ? slide_create(h->d, h->tc, n_patients, stride, dtype, h->device, &s, &err)
+                      : slide_create_generic(h->d, n_patients, stride, dtype, h->device, h->num_sms, &s, &err);
+    if (rc != B2CNN_OK) return fail(rc, std::string(fn) + ": " + err);
     b2cnn_slide *o = new (std::nothrow) b2cnn_slide{s, h, h->weight_gen};
     if (!o) { slide_destroy(s); return fail(B2CNN_ESTATE, "out of host memory"); }
     if (slide_reset(s, nullptr, &err) != B2CNN_OK || cudaStreamSynchronize(nullptr) != cudaSuccess) {
         b2cnn_slide_destroy(o);
-        return fail(B2CNN_ECUDA, "b2cnn_slide_create: initial reset");
+        return fail(B2CNN_ECUDA, std::string(fn) + ": initial reset");
     }
     *out = o;
     return B2CNN_OK;
 }
+extern "C" int b2cnn_slide_create(b2cnn_handle *h, int32_t n_patients, int32_t stride, int dtype, b2cnn_slide **out) {
+    return slide_create_on("b2cnn_slide_create", h, n_patients, stride, dtype, B2CNN_PATH_TENSORCORE, out);
+}
+extern "C" int b2cnn_slide_create_path(b2cnn_handle *h, int32_t n_patients, int32_t stride, int dtype, int path, b2cnn_slide **out) {
+    return slide_create_on("b2cnn_slide_create_path", h, n_patients, stride, dtype, path, out);
+}
+extern "C" int b2cnn_slide_path(const b2cnn_slide *o) { return o ? slide_path(o->s) : -1; }
 extern "C" void b2cnn_slide_destroy(b2cnn_slide *o) {
     if (!o) return;
     DeviceGuard guard(slide_device(o->s));

@@ -302,6 +302,25 @@ int launch_frontend_generic_gates_listed(const Dims &d, const ConvWeights &cw, c
     return launch_frontend_impl(d, cw, x, dtype, B, nullptr, 0, 0, win_list, win_count, wih0T, gate_part, gate_slices, st, num_sms, err);
 }
 
+// 508 final positions -> <= 256 thread-runs of 4 pooled outputs in stage 2 (see header).
+constexpr int kFrontTile = 508;
+constexpr size_t kFrontSmemMax = 220 * 1024;
+
+// the tile of d.L final positions and its padded shared-memory rows: the tile's bytes
+static size_t front_tile(const Dims &d, int *tile_p, int *xs_stride, int *a1_stride) {
+    *tile_p = d.L < kFrontTile ? d.L : kFrontTile;
+    const int nq = (*tile_p - 1) * d.PS + d.PK, nj = nq + d.K2 - 1;
+    const int nt = (nj - 1) * d.PS + d.PK, ni = nt + d.K1 - 1;
+    *xs_stride = padi(ni + d.PS * 4 + d.PK + d.K1 + 8) + 1;
+    *a1_stride = padi(nj + d.PS * 2 + d.PK + d.K2 + 8) + 1;
+    return (size_t)(d.C * *xs_stride + kCMid * *a1_stride) * sizeof(float);
+}
+
+bool frontend_generic_fits(const Dims &d) {
+    int tp, xs, a1;
+    return front_tile(d, &tp, &xs, &a1) <= kFrontSmemMax;
+}
+
 static int launch_frontend_impl(const Dims &d, const ConvWeights &cw, const void *x, int dtype, int64_t B, float *feats,
                                 int64_t sB, int64_t sP, const int *win_list, const int *win_count, const float *wih0T,
                                 float *gate_part, int gate_slices, cudaStream_t st, int num_sms, const char **err) {
@@ -309,17 +328,10 @@ static int launch_frontend_impl(const Dims &d, const ConvWeights &cw, const void
     p.x = x; p.feats = feats; p.sB = sB; p.sP = sP; p.B = (int)B; p.d = d; p.cw = cw;
     p.win_list = win_list; p.win_count = win_count;
     p.gate_part = gate_part; p.wih0T = wih0T; p.gate_slices = gate_slices; p.tiles_per_slice = 1;
-    // 508 final positions -> <= 256 thread-runs of 4 pooled outputs in stage 2 (see header).
-    const int kTile = 508;
-    p.tile_p = d.L < kTile ? d.L : kTile;
+    const size_t smem = front_tile(d, &p.tile_p, &p.xs_stride, &p.a1_stride);
     p.n_tiles = (d.L + p.tile_p - 1) / p.tile_p;
     const int run = (p.tile_p >= 96) ? 4 : 1;   // tiny windows: spread conv1 over more threads
-    const int nq = (p.tile_p - 1) * d.PS + d.PK, nj = nq + d.K2 - 1;
-    const int nt = (nj - 1) * d.PS + d.PK, ni = nt + d.K1 - 1;
-    p.xs_stride = padi(ni + d.PS * 4 + d.PK + d.K1 + 8) + 1;
-    p.a1_stride = padi(nj + d.PS * 2 + d.PK + d.K2 + 8) + 1;
-    const size_t smem = (size_t)(d.C * p.xs_stride + kCMid * p.a1_stride) * sizeof(float);
-    if (smem > 220 * 1024) {
+    if (smem > kFrontSmemMax) {
         *err = "the generic front end's tile does not fit shared memory (in_channels * pool_s^2 too large for this window length)";
         return kLaunchArch;
     }

@@ -44,9 +44,12 @@ void launch_transpose_wih(const float *wih0, float *wih0T, int L, cudaStream_t s
 // ---------------------------------------------------------------------------------------
 constexpr int kPM = 64, kPK = 32, kFsStride = 68;
 
-__global__ void __launch_bounds__(256)
-proj_kernel(const float *__restrict__ F, int64_t sB, int64_t sP, const float *__restrict__ WT,
-            float *__restrict__ part, int B, int L, int k_per_split) {
+// kRing: F is a sliding scorer's position-major feature ring (sB = 1, sP = its row pitch) whose L slots hold window
+// position k in slot (head + k) mod L; otherwise position k of window b is F[b sB + k sP].  The tiles, the zero padding
+// and the summation order are the same either way.
+template <bool kRing>
+__device__ __forceinline__ void proj_body(const float *__restrict__ F, int64_t sB, int64_t sP, int head,
+                                          const float *__restrict__ WT, float *__restrict__ part, int B, int L, int k_per_split) {
     __shared__ __align__(16) float Fs[kPK][kFsStride];
     __shared__ __align__(16) float Ws[kPK][kGates];
     const int tid = threadIdx.x;
@@ -68,7 +71,12 @@ proj_kernel(const float *__restrict__ F, int64_t sB, int64_t sP, const float *__
             int m, kk;
             if (sP == 1) { m = e >> 5; kk = e & 31; } else { m = e & 63; kk = e >> 6; }
             const int b = b0 + m, k = k0 + kk;
-            Fs[kk][m] = (b < B && k < kend) ? __ldg(F + (int64_t)b * sB + (int64_t)k * sP) : 0.f;
+            int slot = k;
+            if (kRing) {
+                slot = head + k;
+                if (slot >= L) slot -= L;
+            }
+            Fs[kk][m] = (b < B && k < kend) ? __ldg(F + (int64_t)b * sB + (int64_t)slot * sP) : 0.f;
         }
 #pragma unroll
         for (int it = 0; it < (kPK * kGates) / 256; ++it) {
@@ -99,6 +107,19 @@ proj_kernel(const float *__restrict__ F, int64_t sB, int64_t sP, const float *__
             *reinterpret_cast<float4 *>(part + ((int64_t)ks * B + b) * kGates + 4 * tn) = v;
         }
     }
+}
+
+__global__ void __launch_bounds__(256)
+proj_kernel(const float *__restrict__ F, int64_t sB, int64_t sP, const float *__restrict__ WT,
+            float *__restrict__ part, int B, int L, int k_per_split) {
+    proj_body<false>(F, sB, sP, 0, WT, part, B, L, k_per_split);
+}
+
+// the sliding scorer's projection over its feature ring (b2cnn_slide.cu, generic path): head in [0, L)
+__global__ void __launch_bounds__(256)
+ring_proj_kernel(const float *__restrict__ ring, int64_t pitch, int head, const float *__restrict__ WT,
+                 float *__restrict__ part, int B, int L, int k_per_split) {
+    proj_body<true>(ring, 1, pitch, head, WT, part, B, L, k_per_split);
 }
 
 // gates[b][g] = (sum_ks partial[ks][b][g] + b_ih[g]) + b_hh[g]
@@ -268,14 +289,27 @@ int choose_ksplit(int L) {
     return ks < 1 ? 1 : ks;
 }
 
+// positions per split-K slice (whole K-chunks) and the number of slices the projection writes
+static int proj_split(int L, int ksplit, int *ks_eff) {
+    int kps = (L + ksplit - 1) / ksplit;
+    kps = ((kps + kPK - 1) / kPK) * kPK;           // whole K-chunks per split
+    *ks_eff = (L + kps - 1) / kps;
+    return kps;
+}
+
+int proj_slices(int L) {
+    int ks_eff;
+    proj_split(L, choose_ksplit(L), &ks_eff);
+    return ks_eff;
+}
+
 int launch_head(const Dims &d, const HeadWeights &hw, const float *feats, int64_t sB, int64_t sP,
                 int64_t B, const float *age, int64_t n_age, int mode, int apply_sigmoid,
                 float *out, float *gates_ws, float *partial_ws, int ksplit, cudaStream_t st,
                 const char **err) {
     int launches = 0;
-    int kps = (d.L + ksplit - 1) / ksplit;
-    kps = ((kps + kPK - 1) / kPK) * kPK;           // whole K-chunks per split
-    const int ks_eff = (d.L + kps - 1) / kps;
+    int ks_eff;
+    const int kps = proj_split(d.L, ksplit, &ks_eff);
     dim3 grid((unsigned)((B + kPM - 1) / kPM), ks_eff);
     proj_kernel<<<grid, 256, 0, st>>>(feats, sB, sP, hw.wih0T, partial_ws, (int)B, d.L, kps);
     ++launches;
@@ -285,6 +319,22 @@ int launch_head(const Dims &d, const HeadWeights &hw, const float *feats, int64_
     n = launch_lstm_head(d, hw, gates_ws, B, age, n_age, mode, apply_sigmoid, out, st, err);
     if (n < 0) return -1;
     return launches + n;
+}
+
+// launch_head of independent windows over a feature ring: window b's position k in ring[((head + k) mod L) pitch + b]
+int launch_ring_head(const Dims &d, const HeadWeights &hw, const float *ring, int64_t pitch, int head, int64_t B,
+                     const float *age, int64_t n_age, int apply_sigmoid, float *out, float *gates_ws, float *partial_ws,
+                     cudaStream_t st, const char **err) {
+    int ks_eff;
+    const int kps = proj_split(d.L, choose_ksplit(d.L), &ks_eff);
+    ring_proj_kernel<<<dim3((unsigned)((B + kPM - 1) / kPM), ks_eff), 256, 0, st>>>(ring, pitch, head, hw.wih0T, partial_ws, (int)B,
+                                                                                    d.L, kps);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) { *err = cudaGetErrorString(e); return -1; }
+    int n = launch_reduce_gates(partial_ws, ks_eff, B, hw, gates_ws, st, err);
+    if (n < 0) return -1;
+    n = launch_lstm_head(d, hw, gates_ws, B, age, n_age, B2CNN_MODE_INDEPENDENT, apply_sigmoid, out, st, err);
+    return n < 0 ? -1 : 3;
 }
 
 // gates[b][g] = (sum over `slices` partial[s][b][g] + b_ih[g]) + b_hh[g], fixed summation order

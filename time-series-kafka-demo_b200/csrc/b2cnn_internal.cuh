@@ -101,6 +101,9 @@ int launch_frontend_generic_listed(const Dims &d, const ConvWeights &cw, const v
                                    int64_t B, float *feats, int64_t sB, int64_t sP, const int *win_list,
                                    const int *win_count, cudaStream_t st, int num_sms, const char **err);
 
+// whether the generic front end's tile of min(d.L, 508) final positions fits shared memory (else kLaunchArch)
+bool frontend_generic_fits(const Dims &d);
+
 // exact gate partials of the listed windows straight into the range-partial buffer the head sums (no feature rows)
 int launch_frontend_generic_gates_listed(const Dims &d, const ConvWeights &cw, const void *x, int dtype, int64_t B,
                                          const float *wih0T, float *gate_part, int gate_slices, const int *win_list,
@@ -121,6 +124,13 @@ int launch_reduce_lstm_head(const Dims &d, const HeadWeights &hw, const float *p
                             int *clean_count = nullptr, int *clean_flags = nullptr, const int *clean_list = nullptr);
 
 int choose_ksplit(int L);
+int proj_slices(int L);       // split-K slices launch_head's projection writes for L positions: [slices][B][64] partials
+
+// launch_head of independent windows whose features sit in a sliding scorer's position-major ring (b2cnn_slide.cu):
+// position k of window b in ring[((head + k) mod L) * pitch + b]; the same tiles and summation order as launch_head
+int launch_ring_head(const Dims &d, const HeadWeights &hw, const float *ring, int64_t pitch, int head, int64_t B,
+                     const float *age, int64_t n_age, int apply_sigmoid, float *out, float *gates_ws, float *partial_ws,
+                     cudaStream_t st, const char **err);
 
 // b2cnn_small.cu: whole forward pass of short windows in one launch (independent windows only)
 bool small_supported(const Dims &d);

@@ -28,6 +28,9 @@
 // tensor-core / exact kernels), scattered into their ring columns, plus their tail.  Pushes then run unchanged for all
 // P patients; slide_live_kernel advances seen and writes NaN for patients without a complete window.  None of this
 // runs for a scorer that never admitted or discharged a patient since its last reset.
+//
+// All of the above is the tensor-core path.  The generic path (slide_create_generic, "generic path" below) runs the
+// same ring and lifecycle for every geometry on exact CUDA-core kernels, with F = pool_s^2 in place of 4.
 #include <algorithm>
 #include <cstring>
 #include <new>
@@ -44,16 +47,21 @@ struct Slide {
     int device;
     Dims d;
     int P, S, dtype, R, phi;
+    int path = B2CNN_PATH_TENSORCORE;  // or B2CNN_PATH_GENERIC: exact CUDA-core kernels for any geometry (below)
+    int F = 4;                       // feature stride pool_s^2 in samples
+    int T = kSlideTail;              // tail samples kept per patient and channel: kSlideTail, R - 1 on the generic path
+    int num_sms = 0;                 // generic path: sizes the generic front end's grid
     int ranges;                      // projection split-K: the streaming kernels' position ranges (TcState, from L only)
     int64_t n = 0;                   // pushes since the last reset
     int64_t g_done = -1;             // last stream feature computed (-1: none)
     int tail_cur = 0;                // which of the two tail buffers holds the current tail
     float *ring = nullptr;           // [L][ring_pitch]
     int64_t ring_pitch = 0;          // P rounded up to 4: 16-byte rows for the projection's TMA boxes
-    float *tail = nullptr;           // [2][P][C][kSlideTail]
+    float *tail = nullptr;           // [2][P][C][T]
     float *partial = nullptr;        // [ranges][P][64]
+    float *gates = nullptr;          // generic path: [P][64] layer-0 gate pre-activations
     int *flags = nullptr;            // flags [P] | list [P] | count
-    void *stage = nullptr;           // [P][C][Sp] in the window dtype
+    void *stage = nullptr;           // [P][C][Sp] in the window dtype; generic path: fp32 seam rows [P][C][Sp]
     int64_t Sp = 0;
     bool lifecycle = false;          // set by the first admit / discharge since the last reset
     int64_t *seen = nullptr;         // [P] on the device: samples since admission, -1: discharged (while lifecycle)
@@ -61,6 +69,7 @@ struct Slide {
 };
 
 static int64_t fdiv4(int64_t a) { return a >= 0 ? a / 4 : -((-a + 3) / 4); }
+static int64_t fdiv(int64_t a, int64_t m) { return a >= 0 ? a / m : -((-a + m - 1) / m); }
 // a mod m in [0, m): stream features before sample 0 (negative g) exist once a patient is admitted with history
 __host__ __device__ __forceinline__ int64_t mod_nn(int64_t a, int64_t m) {
     const int64_t r = a % m;
@@ -346,6 +355,41 @@ __global__ void slide_live_kernel(int64_t *__restrict__ seen, int P, int64_t adv
     for (int64_t j = blockIdx.y; j < len; j += gridDim.y) x[b * len + j] = __int_as_float(0x7fc00000);
 }
 
+// ---- generic path kernels: tails of any length T ------------------------------------------------------------------
+// new tail = the last T samples of (old tail | segment)
+template <typename Tin>
+__global__ void slide_gtail_kernel(const Tin *__restrict__ x, int64_t pitch, int S, int T, const float *__restrict__ tin,
+                                   float *__restrict__ tout, int64_t rows) {
+    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= rows * T) return;
+    const int64_t r = e / T;
+    const int64_t u = S + e % T;
+    tout[e] = u < T ? tin[r * T + u] : ld_sample<Tin>(x + r * pitch + (u - T));
+}
+
+// seam rows [rows][T + n] fp32: the tail's T samples, then the segment's first n
+template <typename Tin>
+__global__ void slide_seam_rows_kernel(const Tin *__restrict__ x, int64_t pitch, const float *__restrict__ tail, int T, int n,
+                                       float *__restrict__ dst, int64_t rows) {
+    const int64_t w = T + n, total = rows * w;
+    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t r = e / w, i = e - r * w;
+        dst[e] = i < T ? tail[r * T + i] : ld_sample<Tin>(x + r * pitch + (i - T));
+    }
+}
+
+// tail rows of the admitted patients = the last T samples of their history (zeros in front of a shorter one)
+template <typename Tin>
+__global__ void slide_admit_gtail_kernel(const Tin *__restrict__ h, int64_t pitch, int64_t H, const int *__restrict__ idx, int k,
+                                         int C, int T, float *__restrict__ tail) {
+    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= (int64_t)k * C * T) return;
+    const int64_t r = e / T;                               // history row j * C + c
+    const int64_t u = e % T;
+    const int64_t t = H - T + u;
+    tail[((int64_t)idx[r / C] * C + r % C) * T + u] = t >= 0 ? ld_sample<Tin>(h + r * pitch + t) : 0.f;
+}
+
 // ------------------------------------------------------------------------------------------
 template <int C, int K1, int PK>
 static void launch_exact_t(const SlideExactParams &p, int dtype, dim3 grid, cudaStream_t st) {
@@ -383,6 +427,127 @@ static int launch_exact(const Slide &s, const ConvWeights &cw, const void *x, in
     return launch_exact_p(p, s, ng, st, err);
 }
 
+// ---- generic path: every geometry, exact fp32 on CUDA cores --------------------------------------------------------
+// Lattice of a conv/pool geometry: feature stride F = pool_s^2, receptive field R = pool_s (pool_k + k2 - 2) + pool_k +
+// k1 - 1 (L = (W - R) / F + 1), phase phi = (-W) mod F; stream feature g reads samples F g + phi .. F g + phi + R - 1.
+// Every feature comes from the generic front end predict() runs on whole windows (launch_frontend_generic: the
+// templated frontend_kernel or frontend_any_kernel, the same arithmetic term for term), pointed at the first feature's
+// sample with the window's row pitch and writing straight into ring slots:
+//   * main features (samples all in the segment): the pushed segment, read in place (any pitch, any alignment);
+//   * seam features: fp32 seam rows = the patient's last T = R - 1 samples | the segment's first min(S, T);
+//   * an admission's features: the history rows, read in place, into a scratch ring (then slide_scatter_kernel).
+// The projection is launch_head's proj_kernel tiles and order reading the ring with its rotation (ring_proj_kernel),
+// then launch_head's reduction and LSTM head.
+
+static int64_t window_head(const Slide &s, int64_t n);
+
+// features [g0, g0 + ng) of B windows into dst, feature g of window b at dst[(g mod cap) dpitch + b]; feature g0's first
+// sample at sample x0 of each channel row (rows `pitch` samples apart, windows C pitch apart).  One front-end launch per
+// run of consecutive slots: two when the range wraps.  ng <= cap.
+static int ring_front(const Slide &s, const ConvWeights &cw, const void *x, int dtype, int64_t pitch, int64_t B, int64_t x0,
+                      int64_t g0, int64_t ng, float *dst, int64_t dpitch, int64_t cap, cudaStream_t st, const char **err) {
+    const int64_t esz = dtype == B2CNN_DTYPE_BF16 ? 2 : 4;
+    while (ng > 0) {
+        const int64_t slot = mod_nn(g0, cap), n = std::min(ng, cap - slot);
+        Dims d = s.d;
+        d.L = (int)n; d.W = (int)((n - 1) * s.F + s.R); d.XP = (int)pitch;
+        const int rc = launch_frontend_generic(d, cw, static_cast<const char *>(x) + x0 * esz, dtype, B, dst + slot * dpitch, 1, dpitch,
+                                               st, s.num_sms, err);
+        if (rc < 0) return rc;
+        g0 += n; ng -= n; x0 += n * s.F;
+    }
+    return 1;
+}
+
+int slide_create_generic(const Dims &d, int n_patients, int stride, int dtype, int device, int num_sms, Slide **out,
+                         const char **err) {
+    *out = nullptr;
+    if (dtype != B2CNN_DTYPE_F32 && dtype != B2CNN_DTYPE_BF16) { *err = "dtype must be f32 (0) or bf16 (1)"; return B2CNN_EINVAL; }
+    if (n_patients < 1 || n_patients > (1 << 24)) { *err = "n_patients out of range"; return B2CNN_EINVAL; }
+    if (stride < 1 || stride > d.W) { *err = "stride must be in [1, window]"; return B2CNN_EINVAL; }
+    const int F = d.PS * d.PS, R = d.PS * (d.PK + d.K2 - 2) + d.PK + d.K1 - 1;
+    if (stride % F != 0) { *err = "stride must be a multiple of the feature stride (pool_s^2 samples)"; return B2CNN_EINVAL; }
+    if (d.W < R || d.L != (d.W - R) / F + 1) { *err = "the feature lattice does not match the window's feature count"; return B2CNN_EARCH; }
+    if (!frontend_generic_fits(d)) {
+        *err = "the generic front end's tile does not fit shared memory (in_channels * pool_s^2 too large for this window length)";
+        return B2CNN_EARCH;
+    }
+    Slide *s = new (std::nothrow) Slide();
+    if (!s) { *err = "out of host memory"; return B2CNN_ESTATE; }
+    s->device = device; s->d = d; s->P = n_patients; s->S = stride; s->dtype = dtype;
+    s->path = B2CNN_PATH_GENERIC; s->F = F; s->R = R; s->T = std::max(R - 1, 1); s->num_sms = num_sms;
+    s->phi = (F - d.W % F) % F;
+    s->ranges = proj_slices(d.L);
+    s->ring_pitch = (n_patients + 3) & ~3;
+    s->Sp = s->T + std::min(stride, s->T);
+    const int64_t P = n_patients;
+    bool ok = cudaMalloc(&s->ring, sizeof(float) * (size_t)d.L * s->ring_pitch) == cudaSuccess &&
+              cudaMalloc(&s->tail, sizeof(float) * (size_t)2 * P * d.C * s->T) == cudaSuccess &&
+              cudaMalloc(&s->partial, sizeof(float) * (size_t)s->ranges * P * kGates) == cudaSuccess &&
+              cudaMalloc(&s->gates, sizeof(float) * (size_t)P * kGates) == cudaSuccess &&
+              cudaMalloc(&s->stage, sizeof(float) * (size_t)(P * d.C * s->Sp)) == cudaSuccess &&
+              cudaMalloc(&s->seen, sizeof(int64_t) * (size_t)P) == cudaSuccess;
+    if (!ok) { (void)cudaGetLastError(); slide_destroy(s); *err = "cudaMalloc(scorer state)"; return B2CNN_ECUDA; }
+    *out = s;
+    return B2CNN_OK;
+}
+
+static int score_windows(Slide *s, const HeadWeights &hw, const TcState *tc, const float *age, int64_t n_age, int apply_sigmoid,
+                         float *out, int *emitted, int64_t *window_index, cudaEvent_t *ev, cudaStream_t st, const char **err);
+
+static int slide_push_generic(Slide *s, const ConvWeights &cw, const HeadWeights &hw, const void *x, int64_t pitch, const float *age,
+                              int64_t n_age, int apply_sigmoid, float *out, int *emitted, int64_t *window_index, cudaEvent_t *ev,
+                              cudaStream_t st, const char **err) {
+    const Dims &d = s->d;
+    const int64_t P = s->P, S = s->S, T = s->T;
+    if (pitch < S || pitch > 0x7fffffff) { *err = "pitch must be in [stride, 2^31)"; return B2CNN_EINVAL; }
+    if (n_age != 1 && n_age != P) { *err = "age must have 1 or n_patients elements"; return B2CNN_EINVAL; }
+    const int64_t n1 = s->n + 1, seg0 = s->n * S;
+    const int64_t g_hi = fdiv(n1 * S - s->R - s->phi, s->F);   // last feature whose samples have all arrived
+    const int64_t g_m0 = seg0 / s->F;                           // first feature that starts inside the segment
+    const int64_t g_lo = std::max(s->g_done + 1, window_head(*s, n1));   // earlier features never enter a window
+    const float *tail_in = s->tail + (size_t)s->tail_cur * P * d.C * T;
+    float *tail_out = s->tail + (size_t)(s->tail_cur ^ 1) * P * d.C * T;
+    if (ev && cudaEventRecord(ev[0], st) != cudaSuccess) { *err = "cudaEventRecord"; return B2CNN_ECUDA; }
+    // ---- main features [g_m0, g_hi], straight from the segment (feature g_m0 starts at its sample phi)
+    if (g_hi >= g_m0 &&
+        ring_front(*s, cw, x, s->dtype, pitch, P, s->phi, g_m0, g_hi - g_m0 + 1, s->ring, s->ring_pitch, d.L, st, err) < 0)
+        return B2CNN_ECUDA;
+    // ---- seam features [g_lo, min(g_hi, g_m0 - 1)]: they start in the last T samples before the segment and end in its
+    // first min(S, T) (F g_lo + phi >= seg0 - T: g_lo - 1 is at most the last feature complete before this push)
+    const int64_t seam_hi = std::min(g_hi, g_m0 - 1);
+    if (seam_hi >= g_lo) {
+        const int64_t rows = P * d.C, total = rows * s->Sp;
+        const unsigned blocks = (unsigned)std::min<int64_t>((total + 255) / 256, 65536);
+        const int nseg = (int)(s->Sp - T);
+        if (s->dtype == B2CNN_DTYPE_BF16)
+            slide_seam_rows_kernel<__nv_bfloat16><<<blocks, 256, 0, st>>>(reinterpret_cast<const __nv_bfloat16 *>(x), pitch, tail_in,
+                                                                          (int)T, nseg, reinterpret_cast<float *>(s->stage), rows);
+        else
+            slide_seam_rows_kernel<float><<<blocks, 256, 0, st>>>(reinterpret_cast<const float *>(x), pitch, tail_in, (int)T, nseg,
+                                                                  reinterpret_cast<float *>(s->stage), rows);
+        if (cudaGetLastError() != cudaSuccess) { *err = "seam rows launch"; return B2CNN_ECUDA; }
+        if (ring_front(*s, cw, s->stage, B2CNN_DTYPE_F32, s->Sp, P, s->F * g_lo + s->phi - seg0 + T, g_lo, seam_hi - g_lo + 1, s->ring,
+                       s->ring_pitch, d.L, st, err) < 0)
+            return B2CNN_ECUDA;
+    }
+    {
+        const int64_t rows = P * d.C, total = rows * T;
+        if (s->dtype == B2CNN_DTYPE_BF16)
+            slide_gtail_kernel<__nv_bfloat16><<<(unsigned)((total + 255) / 256), 256, 0, st>>>(
+                reinterpret_cast<const __nv_bfloat16 *>(x), pitch, (int)S, (int)T, tail_in, tail_out, rows);
+        else
+            slide_gtail_kernel<float><<<(unsigned)((total + 255) / 256), 256, 0, st>>>(reinterpret_cast<const float *>(x), pitch, (int)S,
+                                                                                     (int)T, tail_in, tail_out, rows);
+        if (cudaGetLastError() != cudaSuccess) { *err = "tail launch"; return B2CNN_ECUDA; }
+    }
+    if (ev && cudaEventRecord(ev[1], st) != cudaSuccess) { *err = "cudaEventRecord"; return B2CNN_ECUDA; }
+    s->n = n1;
+    if (g_hi >= g_lo) s->g_done = g_hi;
+    s->tail_cur ^= 1;
+    return score_windows(s, hw, nullptr, age, n_age, apply_sigmoid, out, emitted, window_index, ev, st, err);
+}
+
 int slide_create(const Dims &d, const TcState &tc, int n_patients, int stride, int dtype, int device, Slide **out,
                  const char **err) {
     *out = nullptr;
@@ -417,22 +582,24 @@ int slide_create(const Dims &d, const TcState &tc, int n_patients, int stride, i
 
 void slide_destroy(Slide *s) {
     if (!s) return;
-    cudaFree(s->ring); cudaFree(s->tail); cudaFree(s->partial); cudaFree(s->flags); cudaFree(s->stage); cudaFree(s->seen);
+    cudaFree(s->ring); cudaFree(s->tail); cudaFree(s->partial); cudaFree(s->gates); cudaFree(s->flags); cudaFree(s->stage);
+    cudaFree(s->seen);
     delete s;
 }
 
 int slide_device(const Slide *s) { return s->device; }
 int slide_dtype(const Slide *s) { return s->dtype; }
+int slide_path(const Slide *s) { return s->path; }
 
 int slide_reset(Slide *s, cudaStream_t st, const char **err) {
     s->n = 0; s->g_done = -1; s->tail_cur = 0; s->lifecycle = false;
-    if (cudaMemsetAsync(s->tail, 0, sizeof(float) * (size_t)2 * s->P * s->d.C * kSlideTail, st) != cudaSuccess) {
+    if (cudaMemsetAsync(s->tail, 0, sizeof(float) * (size_t)2 * s->P * s->d.C * s->T, st) != cudaSuccess) {
         *err = "memset tail"; return B2CNN_ECUDA;
     }
     return B2CNN_OK;
 }
 
-static int64_t window_head(const Slide &s, int64_t n) { return fdiv4(n * s.S - s.d.W - s.phi); }
+static int64_t window_head(const Slide &s, int64_t n) { return fdiv(n * s.S - s.d.W - s.phi, s.F); }
 
 // slide_live_kernel over the P patients: seen += adv, then NaN rows of x [P][len] without a complete window
 static int launch_live(const Slide &s, int64_t adv, float *x, int64_t len, cudaStream_t st, const char **err) {
@@ -454,6 +621,8 @@ static int advance_seen(Slide *s, float *out, cudaStream_t st, const char **err)
 int slide_push(Slide *s, const ConvWeights &cw, const HeadWeights &hw, const TcState &tc, const void *x, int64_t pitch,
                const float *age, int64_t n_age, int apply_sigmoid, float *out, int *emitted, int64_t *window_index,
                cudaEvent_t *ev, cudaStream_t st, const char **err) {
+    if (s->path == B2CNN_PATH_GENERIC)
+        return slide_push_generic(s, cw, hw, x, pitch, age, n_age, apply_sigmoid, out, emitted, window_index, ev, st, err);
     const Dims &d = s->d;
     const int64_t P = s->P, S = s->S, esz = s->dtype == B2CNN_DTYPE_BF16 ? 2 : 4;
     if (pitch < S) { *err = "pitch must be >= stride"; return B2CNN_EINVAL; }
@@ -513,8 +682,15 @@ int slide_push(Slide *s, const ConvWeights &cw, const HeadWeights &hw, const TcS
     s->n = n1;
     if (g_hi >= g_lo) s->g_done = g_hi;
     s->tail_cur ^= 1;
+    return score_windows(s, hw, &tc, age, n_age, apply_sigmoid, out, emitted, window_index, ev, st, err);
+}
 
-    // ---- projection over the ring + head, once a window is complete (every patient's, or with the lifecycle on, one)
+// the end of push n = s->n: projection over the ring + head, once a window is complete (every patient's, or with the
+// lifecycle on, one); on tensor cores with `tc`, else (generic path) on CUDA cores
+static int score_windows(Slide *s, const HeadWeights &hw, const TcState *tc, const float *age, int64_t n_age, int apply_sigmoid,
+                         float *out, int *emitted, int64_t *window_index, cudaEvent_t *ev, cudaStream_t st, const char **err) {
+    const Dims &d = s->d;
+    const int64_t P = s->P, S = s->S, n1 = s->n;
     bool live = n1 * S >= d.W;
     if (s->lifecycle)
         live = std::any_of(s->seen_h.begin(), s->seen_h.end(), [&](int64_t v) { return v >= 0 && v + S >= d.W; });
@@ -524,19 +700,24 @@ int slide_push(Slide *s, const ConvWeights &cw, const HeadWeights &hw, const TcS
         if (ev && cudaEventRecord(ev[2], st) != cudaSuccess) { *err = "cudaEventRecord"; return B2CNN_ECUDA; }
         return B2CNN_OK;
     }
-    const int head = (int)mod_nn(G, d.L);
-    CUtensorMap tm;
-    if (tc_ring_tmap(s->ring, P, s->ring_pitch, d.L, &tm, err) != 0) return B2CNN_ECUDA;
-    RingProjParams rp;
-    rp.wpack = reinterpret_cast<const uint8_t *>(tc.d_wpack); rp.partial = s->partial;
-    rp.P = (int)P; rp.L = d.L; rp.head = head;
-    rp.feats_per_cta = tc.feats_per_cta; rp.chunks_per_cta = tc.chunks_per_cta; rp.foff = d.K1 == 10 ? 3 : 2;
-    if (cudaFuncSetAttribute(slide_ring_proj_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kRpSmem) != cudaSuccess) {
-        *err = "projection smem attribute"; return B2CNN_ECUDA;
+    const int head = (int)mod_nn(window_head(*s, n1), d.L);
+    if (!tc) {
+        if (launch_ring_head(d, hw, s->ring, s->ring_pitch, head, P, age, n_age, apply_sigmoid, out, s->gates, s->partial, st, err) < 0)
+            return B2CNN_ECUDA;
+    } else {
+        CUtensorMap tm;
+        if (tc_ring_tmap(s->ring, P, s->ring_pitch, d.L, &tm, err) != 0) return B2CNN_ECUDA;
+        RingProjParams rp;
+        rp.wpack = reinterpret_cast<const uint8_t *>(tc->d_wpack); rp.partial = s->partial;
+        rp.P = (int)P; rp.L = d.L; rp.head = head;
+        rp.feats_per_cta = tc->feats_per_cta; rp.chunks_per_cta = tc->chunks_per_cta; rp.foff = d.K1 == 10 ? 3 : 2;
+        if (cudaFuncSetAttribute(slide_ring_proj_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kRpSmem) != cudaSuccess) {
+            *err = "projection smem attribute"; return B2CNN_ECUDA;
+        }
+        slide_ring_proj_kernel<<<dim3((unsigned)((P + kRpM - 1) / kRpM), (unsigned)s->ranges), kRpThreads, kRpSmem, st>>>(tm, rp);
+        if (cudaGetLastError() != cudaSuccess) { *err = "projection launch"; return B2CNN_ECUDA; }
+        if (launch_reduce_lstm_head(d, hw, s->partial, s->ranges, P, age, n_age, apply_sigmoid, out, st, err) < 0) return B2CNN_ECUDA;
     }
-    slide_ring_proj_kernel<<<dim3((unsigned)((P + kRpM - 1) / kRpM), (unsigned)s->ranges), kRpThreads, kRpSmem, st>>>(tm, rp);
-    if (cudaGetLastError() != cudaSuccess) { *err = "projection launch"; return B2CNN_ECUDA; }
-    if (launch_reduce_lstm_head(d, hw, s->partial, s->ranges, P, age, n_age, apply_sigmoid, out, st, err) < 0) return B2CNN_ECUDA;
     if (s->lifecycle && advance_seen(s, out, st, err) < 0) return B2CNN_ECUDA;
     if (ev && cudaEventRecord(ev[2], st) != cudaSuccess) { *err = "cudaEventRecord"; return B2CNN_ECUDA; }
     *emitted = 1;
@@ -599,12 +780,13 @@ static AdmitLayout admit_layout(const Slide &s, int64_t k, int64_t H) {
     AdmitLayout a;
     const int64_t esz = s.dtype == B2CNN_DTYPE_BF16 ? 2 : 4;
     a.kp = (k + 3) & ~3;
-    a.cap = H >= s.R ? std::min<int64_t>((H - s.R) / 4 + 1, s.d.L) : 0;
+    a.cap = H >= s.R ? std::min<int64_t>((H - s.R) / s.F + 1, s.d.L) : 0;
     a.hp = (H + 7) & ~7;
     a.scratch = al256(sizeof(float) * (size_t)(a.cap * a.kp));
     a.flags = al256(sizeof(int) * (size_t)(2 * k + 1));
     a.idx = al256(sizeof(int) * (size_t)k);
-    a.stage = al256((size_t)(k * s.d.C * a.hp * esz));
+    // the generic path reads the history in place, whatever its alignment
+    a.stage = s.path == B2CNN_PATH_GENERIC ? 0 : al256((size_t)(k * s.d.C * a.hp * esz));
     a.total = a.scratch + a.flags + a.idx + a.stage;
     return a;
 }
@@ -622,6 +804,7 @@ int slide_admit(Slide *s, const ConvWeights &cw, const TcState &tc, const int *p
     if (H < 0 || H > d.W) { *err = "history length must be in [0, window]"; return B2CNN_EINVAL; }
     if (H > 0 && !hist) { *err = "null history with a positive length"; return B2CNN_EINVAL; }
     if (H > 0 && pitch < H) { *err = "history pitch must be >= its length"; return B2CNN_EINVAL; }
+    if (H > 0 && pitch > 0x7fffffff) { *err = "history pitch must be < 2^31"; return B2CNN_EINVAL; }
     if (k == 0) return B2CNN_OK;
     const AdmitLayout a = admit_layout(*s, k, H);
     if (!ws || ws_bytes < (int64_t)a.total) {
@@ -640,10 +823,14 @@ int slide_admit(Slide *s, const ConvWeights &cw, const TcState &tc, const int *p
     // the history is stream samples [nS - H, nS): the features wholly inside it that lie in the current window n
     // (features() may read it before the next push) or can still enter a later one
     const int64_t nS = s->n * s->S;
-    const int64_t g_lo = std::max(-fdiv4(-(nS - H - s->phi)), window_head(*s, s->n));
-    const int64_t g_hi = fdiv4(nS - s->R - s->phi);
+    const int64_t g_lo = std::max(-fdiv(-(nS - H - s->phi), s->F), window_head(*s, s->n));
+    const int64_t g_hi = fdiv(nS - s->R - s->phi, s->F);
     const int64_t Q = g_hi - g_lo + 1;
-    if (H > 0 && Q > 0) {
+    if (H > 0 && Q > 0 && s->path == B2CNN_PATH_GENERIC) {
+        // the generic front end straight from the history rows into the scratch ring, slot g mod Q
+        const int rc2 = ring_front(*s, cw, hist, s->dtype, pitch, k, s->F * g_lo + s->phi - (nS - H), g_lo, Q, scratch, a.kp, Q, st, err);
+        if (rc2 < 0) return rc2 == kLaunchArch ? B2CNN_EARCH : B2CNN_ECUDA;
+    } else if (H > 0 && Q > 0) {
         const int cap = (int)Q;                                        // Q <= a.cap
         const int64_t off = 4 * g_lo + s->phi - (nS - H);               // (H - W) mod 4 + 4 (g_lo - first feature inside)
         SlideExactParams p;
@@ -674,15 +861,24 @@ int slide_admit(Slide *s, const ConvWeights &cw, const TcState &tc, const int *p
             p.list = flags + k; p.count = flags + 2 * k;                // flagged histories: exact, over all Q features
         }
         if (launch_exact_p(p, *s, Q, st, err) < 0) return B2CNN_ECUDA;
+    }
+    if (H > 0 && Q > 0) {
         const unsigned gy = (unsigned)std::min<int64_t>(Q, 1024);
-        slide_scatter_kernel<<<dim3((unsigned)((k + 127) / 128), gy), 128, 0, st>>>(scratch, a.kp, cap, idx, (int)k, g_lo, (int)Q,
+        slide_scatter_kernel<<<dim3((unsigned)((k + 127) / 128), gy), 128, 0, st>>>(scratch, a.kp, (int)Q, idx, (int)k, g_lo, (int)Q,
                                                                                    s->ring, s->ring_pitch, d.L);
         if (cudaGetLastError() != cudaSuccess) { *err = "scatter launch"; return B2CNN_ECUDA; }
     }
     // the next push's seam features read the history's last samples from the current tail
-    float *tail = s->tail + (size_t)s->tail_cur * s->P * d.C * kSlideTail;
-    const int64_t total = k * d.C * kSlideTail;
-    if (esz == 2)
+    float *tail = s->tail + (size_t)s->tail_cur * s->P * d.C * s->T;
+    const int64_t total = k * d.C * s->T;
+    if (s->path == B2CNN_PATH_GENERIC) {
+        if (esz == 2)
+            slide_admit_gtail_kernel<__nv_bfloat16><<<(unsigned)((total + 255) / 256), 256, 0, st>>>(
+                reinterpret_cast<const __nv_bfloat16 *>(hist), pitch, H, idx, (int)k, d.C, s->T, tail);
+        else
+            slide_admit_gtail_kernel<float><<<(unsigned)((total + 255) / 256), 256, 0, st>>>(reinterpret_cast<const float *>(hist), pitch,
+                                                                                             H, idx, (int)k, d.C, s->T, tail);
+    } else if (esz == 2)
         slide_admit_tail_kernel<__nv_bfloat16><<<(unsigned)((total + 255) / 256), 256, 0, st>>>(
             reinterpret_cast<const __nv_bfloat16 *>(hist), pitch, H, idx, (int)k, d.C, tail);
     else

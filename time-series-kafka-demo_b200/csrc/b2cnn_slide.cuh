@@ -8,6 +8,11 @@ struct Slide;
 // `d`: the model's geometry; the scorer keeps a copy.  Checks stride and geometry, allocates all device state.
 int slide_create(const Dims &d, const TcState &tc, int n_patients, int stride, int dtype, int device, Slide **out,
                  const char **err);
+// the generic path: exact CUDA-core kernels for any geometry b2cnn_create accepts (B2CNN_EARCH, before allocating
+// anything, where the generic front end's tile does not fit shared memory); stride % pool_s^2 == 0
+int slide_create_generic(const Dims &d, int n_patients, int stride, int dtype, int device, int num_sms, Slide **out,
+                         const char **err);
+int slide_path(const Slide *s);   // B2CNN_PATH_TENSORCORE or B2CNN_PATH_GENERIC
 void slide_destroy(Slide *s);
 int slide_device(const Slide *s);
 int slide_reset(Slide *s, cudaStream_t st, const char **err);

@@ -30,17 +30,28 @@ class SlidingScorer:
 
     Each patient has its own count of samples, ``samples_seen``: ``reset()`` starts all at 0, a push adds ``stride``,
     ``admit`` restarts listed patients (at the length of the history given), ``discharge`` sets -1.  Once ``admit`` or
-    ``discharge`` was called, a patient's score is NaN until its count reaches W."""
+    ``discharge`` was called, a patient's score is NaN until its count reaches W.
 
-    def __init__(self, model, n_patients: int, stride: int, dtype=torch.bfloat16):
+    ``path``: ``"tensorcore"`` (the default) runs the tensor-core kernels, which hold tanh models without affine of the
+    MyCNN5 or MyCNN2/3/4 conv/pool geometry with 1 to 3 channels; ``"generic"`` runs exact fp32 CUDA-core kernels for
+    any model the library accepts (its logits are ``predict()``'s with ``path="generic"`` and ``small_kernel=0``), with
+    ``stride`` a multiple of the feature stride ``pool_s ** 2``; ``"auto"`` takes the tensor-core path where it holds
+    the model and the generic one otherwise.  ``scorer.path`` tells which one runs."""
+
+    PATHS = {"tensorcore": capi.PATH_TENSORCORE, "generic": capi.PATH_GENERIC, "auto": capi.PATH_AUTO}
+
+    def __init__(self, model, n_patients: int, stride: int, dtype=torch.bfloat16, path: str = "tensorcore"):
         if dtype not in (torch.bfloat16, torch.float32):
             raise ValueError("dtype must be torch.bfloat16 or torch.float32")
+        if path not in self.PATHS:
+            raise ValueError(f"path must be one of {sorted(self.PATHS)}, got {path!r}")
         n_patients, stride = int(n_patients), int(stride)
         if n_patients < 1:
             raise ValueError(f"n_patients must be >= 1, got {n_patients}")
         W = model.arch.window
-        if stride < 1 or stride > W or stride % 4:
-            raise ValueError(f"stride must be a multiple of 4 in [4, {W}] (the window), got {stride}")
+        F = 4 if path == "tensorcore" else model.arch.pool_s ** 2           # the feature stride in samples
+        if stride < 1 or stride > W or stride % F:
+            raise ValueError(f"stride must be a multiple of {F} in [{F}, {W}] (the window), got {stride}")
         self.model, self.n_patients, self.stride, self.dtype = model, n_patients, stride, dtype
         self.channels, self.window = model.arch.in_channels, W
         self._lib, h = model._ensure_handle()
@@ -48,8 +59,13 @@ class SlidingScorer:
         self.device = model._handle_device
         s = ctypes.c_void_p()
         with torch.cuda.device(self.device):
-            capi.check(self._lib.b2cnn_slide_create(h, n_patients, stride, self._dt(), ctypes.byref(s)), "b2cnn_slide_create")
+            if path == "tensorcore":
+                capi.check(self._lib.b2cnn_slide_create(h, n_patients, stride, self._dt(), ctypes.byref(s)), "b2cnn_slide_create")
+            else:
+                capi.check(self._lib.b2cnn_slide_create_path(h, n_patients, stride, self._dt(), self.PATHS[path], ctypes.byref(s)),
+                           "b2cnn_slide_create_path")
         self._s = s
+        self.path = "generic" if self._lib.b2cnn_slide_path(s) == capi.PATH_GENERIC else "tensorcore"
         self.window_index = -1
 
     def _dt(self) -> int:
