@@ -284,6 +284,50 @@ int b2cnn_slide_admit(b2cnn_slide *slide, const int32_t *patients, int32_t n, co
 int b2cnn_slide_discharge(b2cnn_slide *slide, const int32_t *patients, int32_t n, void *stream);
 int b2cnn_slide_samples_seen(b2cnn_slide *slide, int64_t *seen, void *stream);
 
+/* Export and import of patients (a restart, beds moved to another scorer or GPU, new LSTM / head weights).  A
+ * patient's state is its current window's L features in window order, raw and unmasked (for a complete window
+ * bit-identical to its b2cnn_slide_features row), its T-sample tail (the stream's last T samples per channel, fp32;
+ * T = 24 on the tensor-core path, R - 1 on the generic path) and its sample count seen (as b2cnn_slide_samples_seen).
+ * It does not depend on the ring's rotation, the push count, P, the patient's slot or the stride, so it can be imported
+ * into any scorer of the same path, dtype, C, W, L, F and T whose handle has the same front-end weights.
+ * The header's frontend_digest is 64-bit FNV-1a over the bit patterns of the conv1 / conv2 weights and biases, the
+ * affine scales and shifts when B2CNN_FLAG_AFFINE is set, and the front-end geometry (C, k1, k2, pool_k, pool_s, act,
+ * affine flag) -- not the LSTM, Linear or head weights, which the features do not depend on.
+ *   b2cnn_slide_describe_state  the header of this scorer's state (the digest of the handle's current weights).
+ *   b2cnn_slide_state_workspace_bytes  DEVICE workspace both calls need for n patients (-1 for n outside [0, P]).
+ *   b2cnn_slide_export   features [n][L] and tails [n][C][T] into DEVICE fp32 arrays, seen [n] into a HOST int64 array,
+ *                        *header filled.  Reads the scorer and changes nothing in it.
+ *   b2cnn_slide_import   writes the listed patients' windows and tails, then seen[p] = seen_host[j], as an admission with
+ *                        a full history does (the per-patient masking is on afterwards): a patient with seen >= W is
+ *                        in b2cnn_slide_features at once and scored at the next push, one with seen == -1 stays
+ *                        discharged.  Patient p's window after a later push is the last W samples of (the exported
+ *                        stream | pushes since the import).
+ * `patients`: HOST arrays of n distinct indices in [0, P); row j belongs to patients[j].  Both calls allocate nothing
+ * and are asynchronous on `stream` apart from the pageable host-to-device copy of the indices (and, for an import, of
+ * the counts).  Every check runs before the first launch.  B2CNN_EINVAL: bad indices, NULL arrays with n > 0, a bad
+ * magic or version, a path, dtype, C, W, L, F or T that is not the scorer's, a seen value below -1.  B2CNN_ESTATE: a
+ * digest that is not the handle's (the features come from other conv weights), a scorer whose handle's weights changed
+ * since its last reset, or a workspace smaller than b2cnn_slide_state_workspace_bytes. */
+#define B2CNN_SLIDE_STATE_MAGIC 0x53533242u /* "B2SS" */
+#define B2CNN_SLIDE_STATE_VERSION 1
+typedef struct b2cnn_slide_state_header {
+    uint32_t magic;              /* B2CNN_SLIDE_STATE_MAGIC */
+    uint16_t version;            /* B2CNN_SLIDE_STATE_VERSION */
+    uint16_t path;               /* B2CNN_PATH_TENSORCORE or B2CNN_PATH_GENERIC */
+    int32_t dtype, in_channels, window;
+    int32_t lstm_input;          /* L: features per patient */
+    int32_t feature_stride;      /* F: 4 on the tensor-core path, pool_s^2 on the generic path */
+    int32_t tail_len;            /* T: tail samples per patient and channel */
+    uint64_t frontend_digest;
+} b2cnn_slide_state_header;
+int b2cnn_slide_describe_state(b2cnn_slide *slide, b2cnn_slide_state_header *out);
+int64_t b2cnn_slide_state_workspace_bytes(b2cnn_slide *slide, int32_t n);
+int b2cnn_slide_export(b2cnn_slide *slide, const int32_t *patients, int32_t n, float *features, float *tails, int64_t *seen_host,
+                       b2cnn_slide_state_header *header, void *workspace, int64_t workspace_bytes, void *stream);
+int b2cnn_slide_import(b2cnn_slide *slide, const int32_t *patients, int32_t n, const b2cnn_slide_state_header *header,
+                       const float *features, const float *tails, const int64_t *seen_host, void *workspace,
+                       int64_t workspace_bytes, void *stream);
+
 /* ---- The reference's wire formats, decoded on the device (SURVEY.md section 8, row f3) ----
  * A trigger's Kafka messages as one DEVICE byte buffer + offsets [n_msgs + 1] (message t = bytes[offsets[t] .. offsets[t+1])).
  * b2cnn_decode_sample_messages: value = json.dumps([i, val]) (bin/sendStream.py:62): idx_out[t] = i, val_out[t] = val

@@ -31,6 +31,7 @@ SYMBOLS = ("b2cnn_l_out", "b2cnn_weight_count", "b2cnn_create", "b2cnn_destroy",
            "b2cnn_slide_create", "b2cnn_slide_destroy", "b2cnn_slide_reset", "b2cnn_slide_push", "b2cnn_slide_features",
            "b2cnn_slide_admit_workspace_bytes", "b2cnn_slide_admit", "b2cnn_slide_discharge", "b2cnn_slide_samples_seen",
            "b2cnn_slide_create_path", "b2cnn_slide_path",
+           "b2cnn_slide_describe_state", "b2cnn_slide_state_workspace_bytes", "b2cnn_slide_export", "b2cnn_slide_import",
            "b2cnn_decode_sample_messages", "b2cnn_decode_array_messages", "b2cnn_parse_decimal", "b2cnn_frame_check")
 
 
@@ -52,6 +53,16 @@ class FrameHeader(ctypes.Structure):
 
 
 FRAME_MAGIC = 0x46573242
+
+
+class SlideStateHeader(ctypes.Structure):
+    """b2cnn_slide_state_header: what a SlidingScorer's exported patients fit (include/b2cnn.h)."""
+    _fields_ = [("magic", ctypes.c_uint32), ("version", ctypes.c_uint16), ("path", ctypes.c_uint16), ("dtype", ctypes.c_int32),
+                ("in_channels", ctypes.c_int32), ("window", ctypes.c_int32), ("lstm_input", ctypes.c_int32),
+                ("feature_stride", ctypes.c_int32), ("tail_len", ctypes.c_int32), ("frontend_digest", ctypes.c_uint64)]
+
+
+SLIDE_STATE_MAGIC, SLIDE_STATE_VERSION = 0x53533242, 1
 
 
 class Adam(ctypes.Structure):
@@ -131,6 +142,13 @@ def load_library() -> ctypes.CDLL:
     lib.b2cnn_slide_create_path.argtypes = [c_vp, c_i32, c_i32, c_int, c_int, ctypes.POINTER(c_vp)]
     lib.b2cnn_slide_create_path.restype = c_int
     lib.b2cnn_slide_path.argtypes = [c_vp]; lib.b2cnn_slide_path.restype = c_int
+    hdrp = ctypes.POINTER(SlideStateHeader)
+    lib.b2cnn_slide_describe_state.argtypes = [c_vp, hdrp]; lib.b2cnn_slide_describe_state.restype = c_int
+    lib.b2cnn_slide_state_workspace_bytes.argtypes = [c_vp, c_i32]; lib.b2cnn_slide_state_workspace_bytes.restype = c_i64
+    lib.b2cnn_slide_export.argtypes = [c_vp, c_vp, c_i32, c_vp, c_vp, c_vp, hdrp, c_vp, c_i64, c_vp]
+    lib.b2cnn_slide_export.restype = c_int
+    lib.b2cnn_slide_import.argtypes = [c_vp, c_vp, c_i32, hdrp, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp]
+    lib.b2cnn_slide_import.restype = c_int
     lib.b2cnn_decode_sample_messages.argtypes = [c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_i64, c_i32, c_vp, c_vp]
     lib.b2cnn_decode_sample_messages.restype = c_int
     lib.b2cnn_decode_array_messages.argtypes = [c_vp, c_vp, c_i64, c_i32, c_vp, c_vp, c_vp, c_vp]

@@ -702,6 +702,37 @@ extern "C" int b2cnn_slide_samples_seen(b2cnn_slide *o, int64_t *seen, void *str
     const int rc = slide_samples_seen(o->s, seen, reinterpret_cast<cudaStream_t>(stream), &err);
     return rc == B2CNN_OK ? rc : fail(rc, std::string("b2cnn_slide_samples_seen: ") + err);
 }
+extern "C" int b2cnn_slide_describe_state(b2cnn_slide *o, b2cnn_slide_state_header *out) {
+    if (!o || !out) return fail(B2CNN_EINVAL, "b2cnn_slide_describe_state: null argument");
+    slide_describe_state(o->s, o->h->cw, out);
+    return B2CNN_OK;
+}
+extern "C" int64_t b2cnn_slide_state_workspace_bytes(b2cnn_slide *o, int32_t n) {
+    return o ? slide_state_workspace_bytes(o->s, n) : -1;
+}
+extern "C" int b2cnn_slide_export(b2cnn_slide *o, const int32_t *patients, int32_t n, float *features, float *tails, int64_t *seen_host,
+                                  b2cnn_slide_state_header *header, void *workspace, int64_t workspace_bytes, void *stream) {
+    if (!o || !header) return fail(B2CNN_EINVAL, "b2cnn_slide_export: null argument");
+    if (o->gen != o->h->weight_gen)
+        return fail(B2CNN_ESTATE, "b2cnn_slide_export: the handle's weights changed since the scorer's last reset (stored features are stale)");
+    DEVICE_GUARD(slide_device(o->s));
+    const char *err = "";
+    const int rc = slide_export(o->s, o->h->cw, patients, n, features, tails, seen_host, header, workspace, workspace_bytes,
+                                reinterpret_cast<cudaStream_t>(stream), &err);
+    return rc == B2CNN_OK ? rc : fail(rc, std::string("b2cnn_slide_export: ") + err);
+}
+extern "C" int b2cnn_slide_import(b2cnn_slide *o, const int32_t *patients, int32_t n, const b2cnn_slide_state_header *header,
+                                  const float *features, const float *tails, const int64_t *seen_host, void *workspace,
+                                  int64_t workspace_bytes, void *stream) {
+    if (!o || !header) return fail(B2CNN_EINVAL, "b2cnn_slide_import: null argument");
+    if (o->gen != o->h->weight_gen)
+        return fail(B2CNN_ESTATE, "b2cnn_slide_import: the handle's weights changed since the scorer's last reset (stored features are stale)");
+    DEVICE_GUARD(slide_device(o->s));
+    const char *err = "";
+    const int rc = slide_import(o->s, o->h->cw, patients, n, *header, features, tails, seen_host, workspace, workspace_bytes,
+                                reinterpret_cast<cudaStream_t>(stream), &err);
+    return rc == B2CNN_OK ? rc : fail(rc, std::string("b2cnn_slide_import: ") + err);
+}
 
 // ---- host-pointer entry: chunked H2D overlapped with compute -----------------------------
 static int ensure_host_staging(b2cnn_handle *h, size_t x_chunk_bytes, int64_t B, size_t ws_bytes) {

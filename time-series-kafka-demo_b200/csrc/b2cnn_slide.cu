@@ -913,4 +913,170 @@ int slide_samples_seen(Slide *s, int64_t *out, cudaStream_t st, const char **err
     return B2CNN_OK;
 }
 
+// ---- export / import of patients ----------------------------------------------------------------------------------
+// A patient's state is its current window in window order (features [L], position j from ring slot (G_n + j) mod L),
+// its tail [C][T] and its count.  Window position j is stream feature G_n + j, which starts at sample F (G_n + j) + phi
+// = nS - W + F j: F j samples into the window, for any scorer with the same W and F.  So the state does not depend on
+// the ring's rotation, P, the slot, the push count or the stride, and an import is an admission with a full history
+// whose features come from the state instead of the front end.
+
+// rows[j][i] <-> ring[(head + i) mod L][idx[j]] (i < L, j < k) through a 32 x 32 shared-memory tile, so that both the
+// position-major ring side (consecutive patient columns of one slot) and the patient-major row side (consecutive
+// positions of one patient) move in whole 128-byte lines.  kExport: src = ring, dst = rows; else src = rows, dst = ring.
+constexpr int kStTile = 32, kStRows = 8;
+template <bool kExport>
+__global__ void __launch_bounds__(kStTile * kStRows)
+slide_state_kernel(const float *__restrict__ src, float *__restrict__ dst, int64_t ring_pitch, int L, int head,
+                   const int *__restrict__ idx, int k) {
+    __shared__ float tile[kStTile][kStTile + 1];                   // [position][patient]
+    const int tx = threadIdx.x, ty = threadIdx.y, j0 = blockIdx.x * kStTile;
+    const bool col_ok = j0 + tx < k;                               // ring side: lane = patient
+    const int64_t col = col_ok ? idx[j0 + tx] : 0;
+    for (int i0 = blockIdx.y * kStTile; i0 < L; i0 += gridDim.y * kStTile) {
+#pragma unroll
+        for (int r = ty; r < kStTile; r += kStRows) {
+            const int i = i0 + r, j = j0 + r;
+            if constexpr (kExport) {
+                if (col_ok && i < L) tile[r][tx] = src[(int64_t)(head + i - (head + i >= L ? L : 0)) * ring_pitch + col];
+            } else {
+                if (j < k && i0 + tx < L) tile[tx][r] = src[(int64_t)j * L + i0 + tx];
+            }
+        }
+        __syncthreads();
+#pragma unroll
+        for (int r = ty; r < kStTile; r += kStRows) {
+            const int i = i0 + r, j = j0 + r;
+            if constexpr (kExport) {
+                if (j < k && i0 + tx < L) dst[(int64_t)j * L + i0 + tx] = tile[tx][r];
+            } else {
+                if (col_ok && i < L) dst[(int64_t)(head + i - (head + i >= L ? L : 0)) * ring_pitch + col] = tile[r][tx];
+            }
+        }
+        __syncthreads();
+    }
+}
+
+// tails[j][c][t] <-> tail[idx[j]][c][t]: one contiguous row of ct = C T floats per patient.  kExport: src = the
+// scorer's tail, dst = tails; else the reverse.
+template <bool kExport>
+__global__ void slide_state_tail_kernel(const float *__restrict__ src, float *__restrict__ dst, const int *__restrict__ idx, int64_t k,
+                                        int64_t ct) {
+    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= k * ct) return;
+    const int64_t j = e / ct, own = (int64_t)idx[j] * ct + (e - j * ct);
+    if constexpr (kExport) dst[e] = src[own];
+    else dst[own] = src[e];
+}
+
+static uint64_t fnv1a(uint64_t h, const void *p, size_t n) {
+    const unsigned char *b = static_cast<const unsigned char *>(p);
+    for (size_t i = 0; i < n; ++i) { h ^= b[i]; h *= 0x100000001b3ull; }
+    return h;
+}
+
+// FNV-1a over what the features depend on: the front-end geometry and the used conv weights (affine when on)
+static uint64_t frontend_digest(const Dims &d, const ConvWeights &cw) {
+    const int32_t geo[7] = {d.C, d.K1, d.K2, d.PK, d.PS, d.act, d.has_affine};
+    uint64_t h = fnv1a(0xcbf29ce484222325ull, geo, sizeof geo);
+    h = fnv1a(h, cw.w1, sizeof(float) * (size_t)d.C * d.K1 * kCMid);
+    h = fnv1a(h, cw.b1, sizeof cw.b1);
+    h = fnv1a(h, cw.w2, sizeof(float) * (size_t)kCMid * d.K2);
+    h = fnv1a(h, &cw.b2, sizeof cw.b2);
+    if (d.has_affine) {
+        h = fnv1a(h, cw.s1, sizeof cw.s1);
+        h = fnv1a(h, cw.t1, sizeof cw.t1);
+        h = fnv1a(h, &cw.s2, sizeof cw.s2);
+        h = fnv1a(h, &cw.t2, sizeof cw.t2);
+    }
+    return h;
+}
+
+void slide_describe_state(const Slide *s, const ConvWeights &cw, b2cnn_slide_state_header *o) {
+    memset(o, 0, sizeof *o);
+    o->magic = B2CNN_SLIDE_STATE_MAGIC; o->version = B2CNN_SLIDE_STATE_VERSION; o->path = (uint16_t)s->path;
+    o->dtype = s->dtype; o->in_channels = s->d.C; o->window = s->d.W; o->lstm_input = s->d.L;
+    o->feature_stride = s->F; o->tail_len = s->T;
+    o->frontend_digest = frontend_digest(s->d, cw);
+}
+
+// the workspace holds the k device indices
+int64_t slide_state_workspace_bytes(const Slide *s, int64_t k) {
+    if (k < 0 || k > s->P) return -1;
+    return (int64_t)al256(sizeof(int) * (size_t)k);
+}
+
+// the indices into the workspace, then the feature tile kernel and the tail kernel in one direction
+template <bool kExport>
+static int launch_state(const Slide &s, const int *patients, int64_t k, const float *src_rows, float *dst_rows, const float *src_tails,
+                        float *dst_tails, void *ws, cudaStream_t st, const char **err) {
+    int *idx = static_cast<int *>(ws);
+    if (cudaMemcpyAsync(idx, patients, sizeof(int) * (size_t)k, cudaMemcpyHostToDevice, st) != cudaSuccess) {
+        *err = "copy of the patient indices"; return B2CNN_ECUDA;
+    }
+    const int L = s.d.L, head = (int)mod_nn(window_head(s, s.n), L);
+    const dim3 grid((unsigned)((k + kStTile - 1) / kStTile), (unsigned)std::min<int64_t>((L + kStTile - 1) / kStTile, 65535));
+    if constexpr (kExport) slide_state_kernel<true><<<grid, dim3(kStTile, kStRows), 0, st>>>(s.ring, dst_rows, s.ring_pitch, L, head, idx, (int)k);
+    else slide_state_kernel<false><<<grid, dim3(kStTile, kStRows), 0, st>>>(src_rows, s.ring, s.ring_pitch, L, head, idx, (int)k);
+    if (cudaGetLastError() != cudaSuccess) { *err = "state feature launch"; return B2CNN_ECUDA; }
+    float *tail = s.tail + (size_t)s.tail_cur * s.P * s.d.C * s.T;
+    const int64_t ct = (int64_t)s.d.C * s.T, blocks = (k * ct + 255) / 256;
+    if constexpr (kExport) slide_state_tail_kernel<true><<<(unsigned)blocks, 256, 0, st>>>(tail, dst_tails, idx, k, ct);
+    else slide_state_tail_kernel<false><<<(unsigned)blocks, 256, 0, st>>>(src_tails, tail, idx, k, ct);
+    if (cudaGetLastError() != cudaSuccess) { *err = "state tail launch"; return B2CNN_ECUDA; }
+    return B2CNN_OK;
+}
+
+static int check_state_args(const Slide &s, const int *patients, int64_t k, const void *feats, const void *tails, const void *seen,
+                            void *ws, int64_t ws_bytes, const char **err) {
+    const int rc = check_patients(s, patients, k, err);
+    if (rc != B2CNN_OK) return rc;
+    if (k > 0 && (!feats || !tails || !seen)) { *err = "null feature, tail or count array with patients listed"; return B2CNN_EINVAL; }
+    if (k > 0 && (!ws || ws_bytes < slide_state_workspace_bytes(&s, k))) {
+        *err = "workspace missing or smaller than b2cnn_slide_state_workspace_bytes()"; return B2CNN_ESTATE;
+    }
+    return B2CNN_OK;
+}
+
+int slide_export(const Slide *s, const ConvWeights &cw, const int *patients, int64_t k, float *feats, float *tails, int64_t *seen_host,
+                 b2cnn_slide_state_header *hdr, void *ws, int64_t ws_bytes, cudaStream_t st, const char **err) {
+    int rc = check_state_args(*s, patients, k, feats, tails, seen_host, ws, ws_bytes, err);
+    if (rc != B2CNN_OK) return rc;
+    if (k > 0 && (rc = launch_state<true>(*s, patients, k, nullptr, feats, nullptr, tails, ws, st, err)) != B2CNN_OK) return rc;
+    // the host mirror: the counts need no device read (before any lifecycle call every patient has seen n S samples)
+    for (int64_t j = 0; j < k; ++j) seen_host[j] = s->lifecycle ? s->seen_h[patients[j]] : s->n * s->S;
+    slide_describe_state(s, cw, hdr);
+    return B2CNN_OK;
+}
+
+int slide_import(Slide *s, const ConvWeights &cw, const int *patients, int64_t k, const b2cnn_slide_state_header &hdr, const float *feats,
+                 const float *tails, const int64_t *seen_host, void *ws, int64_t ws_bytes, cudaStream_t st, const char **err) {
+    if (hdr.magic != B2CNN_SLIDE_STATE_MAGIC || hdr.version != B2CNN_SLIDE_STATE_VERSION) {
+        *err = "not a scorer state header of this version (magic, version)"; return B2CNN_EINVAL;
+    }
+    b2cnn_slide_state_header mine;
+    slide_describe_state(s, cw, &mine);
+    if (hdr.path != mine.path || hdr.dtype != mine.dtype || hdr.in_channels != mine.in_channels || hdr.window != mine.window ||
+        hdr.lstm_input != mine.lstm_input || hdr.feature_stride != mine.feature_stride || hdr.tail_len != mine.tail_len) {
+        *err = "the state's path, dtype, in_channels, window, lstm_input, feature stride or tail length is not the scorer's";
+        return B2CNN_EINVAL;
+    }
+    if (hdr.frontend_digest != mine.frontend_digest) {
+        *err = "the state's features come from other front-end weights than the handle's (conv / affine digest differs)";
+        return B2CNN_ESTATE;
+    }
+    int rc = check_state_args(*s, patients, k, feats, tails, seen_host, ws, ws_bytes, err);
+    if (rc != B2CNN_OK) return rc;
+    for (int64_t j = 0; j < k; ++j)
+        if (seen_host[j] < -1) { *err = "a sample count below -1"; return B2CNN_EINVAL; }
+    if (k == 0) return B2CNN_OK;
+    if ((rc = launch_state<false>(*s, patients, k, feats, nullptr, tails, nullptr, ws, st, err)) != B2CNN_OK) return rc;
+    std::vector<int64_t> next = next_seen(*s, patients, 0, 0);
+    for (int64_t j = 0; j < k; ++j) next[patients[j]] = seen_host[j];
+    if ((rc = commit_seen(s, next, st, err)) != B2CNN_OK) return rc;
+    // as after an admission with a full history: the next push computes the seam features from the window's last one on
+    const int64_t g_hi = fdiv(s->n * s->S - s->R - s->phi, s->F);
+    if (g_hi < s->g_done) s->g_done = g_hi;
+    return B2CNN_OK;
+}
+
 }  // namespace b2cnn

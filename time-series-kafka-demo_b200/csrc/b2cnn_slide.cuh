@@ -28,5 +28,12 @@ int slide_admit(Slide *s, const ConvWeights &cw, const TcState &tc, const int *p
 int slide_discharge(Slide *s, const int *patients, int64_t k, cudaStream_t st, const char **err);
 int slide_samples_seen(Slide *s, int64_t *out, cudaStream_t st, const char **err);
 int slide_dtype(const Slide *s);
+// export / import of patients (b2cnn_slide_export / _import): `cw` the handle's current conv weights (the digest)
+void slide_describe_state(const Slide *s, const ConvWeights &cw, b2cnn_slide_state_header *out);
+int64_t slide_state_workspace_bytes(const Slide *s, int64_t k);
+int slide_export(const Slide *s, const ConvWeights &cw, const int *patients, int64_t k, float *feats, float *tails, int64_t *seen_host,
+                 b2cnn_slide_state_header *hdr, void *ws, int64_t ws_bytes, cudaStream_t st, const char **err);
+int slide_import(Slide *s, const ConvWeights &cw, const int *patients, int64_t k, const b2cnn_slide_state_header &hdr, const float *feats,
+                 const float *tails, const int64_t *seen_host, void *ws, int64_t ws_bytes, cudaStream_t st, const char **err);
 
 }  // namespace b2cnn

@@ -11,6 +11,13 @@ S new samples of all patients, computes only the features they complete and scor
 
 Patients come and go one at a time: ``admit(patients, history)`` restarts their streams (optionally from the samples a
 monitor already holds), ``discharge(patients)`` stops scoring them; the others are not disturbed.
+
+``export(patients)`` takes the listed patients' state out of a scorer (their window features, last samples and counts,
+as plain tensors ``torch.save`` can write) and ``restore(patients, state)`` puts it into this or another scorer of
+the same model front end, path and dtype, which then continues those streams bit for bit::
+
+    torch.save(scorer.export(range(P)), "ward.pt")                   # before a restart
+    scorer.restore(range(P), torch.load("ward.pt"))                  # in the new process: no window is lost
 """
 from __future__ import annotations
 
@@ -39,6 +46,7 @@ class SlidingScorer:
     the model and the generic one otherwise.  ``scorer.path`` tells which one runs."""
 
     PATHS = {"tensorcore": capi.PATH_TENSORCORE, "generic": capi.PATH_GENERIC, "auto": capi.PATH_AUTO}
+    STATE_HEADER = tuple(n for n, _ in capi.SlideStateHeader._fields_)
 
     def __init__(self, model, n_patients: int, stride: int, dtype=torch.bfloat16, path: str = "tensorcore"):
         if dtype not in (torch.bfloat16, torch.float32):
@@ -67,6 +75,10 @@ class SlidingScorer:
         self._s = s
         self.path = "generic" if self._lib.b2cnn_slide_path(s) == capi.PATH_GENERIC else "tensorcore"
         self.window_index = -1
+        hdr = capi.SlideStateHeader()
+        capi.check(self._lib.b2cnn_slide_describe_state(s, ctypes.byref(hdr)), "b2cnn_slide_describe_state")
+        # what an imported state must match here (its digest is checked by the library against the current weights)
+        self._state_fields = {n: int(getattr(hdr, n)) for n in self.STATE_HEADER if n != "frontend_digest"}
 
     def _dt(self) -> int:
         return capi.DTYPE_BF16 if self.dtype == torch.bfloat16 else capi.DTYPE_F32
@@ -239,3 +251,82 @@ class SlidingScorer:
             capi.check(self._lib.b2cnn_slide_samples_seen(self._s, out.data_ptr(), torch.cuda.current_stream().cuda_stream),
                        "b2cnn_slide_samples_seen")
         return out
+
+    @torch.no_grad()
+    def export(self, patients) -> dict:
+        """The state of ``patients`` (distinct indices in [0, P)), row j for ``patients[j]``, as plain tensors and ints
+        ``torch.save`` can write: ``features`` [k, L] fp32 (each current window in window order, raw: a patient without
+        a complete window has no NaN mask here), ``tail`` [k, C, T] fp32 (the stream's last T samples per channel),
+        both on the scorer's device, ``seen`` [k] CPU int64 (``samples_seen``), and the header fields (path, dtype,
+        C, W, L, feature stride F, T and a digest of the conv weights).  Changes nothing in the scorer.
+        ``window_index`` is not part of it: it counts this scorer's own pushes."""
+        idx = self.check_patients(patients)
+        k = len(idx)
+        self._handle()
+        f = self._state_fields
+        feats = torch.empty(k, f["lstm_input"], dtype=torch.float32, device=self.device)
+        tail = torch.empty(k, self.channels, f["tail_len"], dtype=torch.float32, device=self.device)
+        seen = torch.empty(k, dtype=torch.int64)
+        hdr = capi.SlideStateHeader()
+        arr = (ctypes.c_int32 * max(k, 1))(*idx)
+        with torch.cuda.device(self.device):
+            nbytes = int(self._lib.b2cnn_slide_state_workspace_bytes(self._s, k))
+            ws = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=self.device)
+            capi.check(self._lib.b2cnn_slide_export(self._s, arr, k, feats.data_ptr(), tail.data_ptr(), seen.data_ptr(), ctypes.byref(hdr),
+                                                    ws.data_ptr(), nbytes, torch.cuda.current_stream().cuda_stream), "b2cnn_slide_export")
+        state = {"features": feats, "tail": tail, "seen": seen}
+        state.update({n: int(getattr(hdr, n)) for n in self.STATE_HEADER})
+        return state
+
+    def check_state(self, state, k: int):
+        """Validates a state of k patients (``export``'s dict) against this scorer; returns (features, tail, seen)."""
+        if not isinstance(state, dict):
+            raise ValueError(f"expected the dict of SlidingScorer.export(), got {type(state).__name__}")
+        missing = [n for n in ("features", "tail", "seen") + self.STATE_HEADER if n not in state]
+        if missing:
+            raise ValueError(f"the state lacks {missing}")
+        for n in self.STATE_HEADER:
+            try:
+                operator.index(state[n])
+            except TypeError:
+                raise ValueError(f"state[{n!r}] must be an integer, got {type(state[n]).__name__}") from None
+        if not 0 <= int(state["frontend_digest"]) < 1 << 64:
+            raise ValueError("state['frontend_digest'] must be a 64-bit unsigned integer")
+        bad = {n: (int(state[n]), v) for n, v in self._state_fields.items() if int(state[n]) != v}
+        if bad:
+            raise ValueError("the state does not fit this scorer (field: (state, scorer)): "
+                             + ", ".join(f"{n}: {a}" for n, a in bad.items()))
+        L, T = self._state_fields["lstm_input"], self._state_fields["tail_len"]
+        want = {"features": ((k, L), torch.float32), "tail": ((k, self.channels, T), torch.float32), "seen": ((k,), torch.int64)}
+        for n, (shape, dtype) in want.items():
+            t = state[n]
+            if not torch.is_tensor(t) or tuple(t.shape) != shape or t.dtype != dtype:
+                got = (tuple(t.shape), t.dtype) if torch.is_tensor(t) else type(t).__name__
+                raise ValueError(f"state[{n!r}]: expected {dtype} {list(shape)}, got {got}")
+        seen = state["seen"].cpu()
+        if k and int(seen.min()) < -1:
+            raise ValueError("state['seen'] holds a count below -1")
+        return state["features"], state["tail"], seen
+
+    @torch.no_grad()
+    def restore(self, patients, state: dict):
+        """Put ``export``'s ``state`` into the streams of ``patients`` (row j into ``patients[j]``; any slots, any P and
+        stride, on any device: the tensors are moved to this scorer's).  As ``admit`` with the full exported window:
+        a patient with ``samples_seen >= W`` is in ``features()`` at once and scored from the next push on, exactly as
+        the exporting scorer would have scored it on the same samples; one exported discharged stays discharged.  The
+        state must come from a scorer of the same path, dtype, C, W and conv weights (the LSTM and head weights may
+        differ: change them, ``reset()``, then restore).  Errors leave the scorer unchanged."""
+        idx = self.check_patients(patients)
+        k = len(idx)
+        feats, tail, seen = self.check_state(state, k)
+        self._handle()
+        feats = feats.to(self.device).contiguous()
+        tail = tail.to(self.device).contiguous()
+        seen = seen.contiguous()
+        hdr = capi.SlideStateHeader(**{n: int(state[n]) for n in self.STATE_HEADER})
+        arr = (ctypes.c_int32 * max(k, 1))(*idx)
+        with torch.cuda.device(self.device):
+            nbytes = int(self._lib.b2cnn_slide_state_workspace_bytes(self._s, k))
+            ws = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=self.device)
+            capi.check(self._lib.b2cnn_slide_import(self._s, arr, k, ctypes.byref(hdr), feats.data_ptr(), tail.data_ptr(), seen.data_ptr(),
+                                                    ws.data_ptr(), nbytes, torch.cuda.current_stream().cuda_stream), "b2cnn_slide_import")
