@@ -328,6 +328,36 @@ int b2cnn_slide_import(b2cnn_slide *slide, const int32_t *patients, int32_t n, c
                        const float *features, const float *tails, const int64_t *seen_host, void *workspace,
                        int64_t workspace_bytes, void *stream);
 
+/* Extra heads over one scorer's features (shadow scoring a retrained head, ensembles of heads over one front end).
+ * The stored ring holds everything a head needs, so K extra heads cost one projection over the ring each (on the
+ * tensor-core path two per CTA, sharing the ring reads and the bf16 split of the features) plus their LSTM heads.
+ *   b2cnn_slide_set_heads  replaces the scorer's heads with SNAPSHOTS of heads[0 .. n) (0 <= n <= B2CNN_SLIDE_MAX_HEADS;
+ *                        a head may be the scorer's own handle): each one's LSTM / Linear weights, W_ih^T, age_coef and,
+ *                        on the tensor-core path, its packed W_ih chunks are copied, so a later b2cnn_set_weights on a
+ *                        head's handle has no effect until the next b2cnn_slide_set_heads.  Every head needs the scorer's
+ *                        architecture (b2cnn_config apart from age_coef and device), weights set, the scorer's device and
+ *                        the same front-end digest (b2cnn_slide_state_header) as the scorer's weights.  Every check runs
+ *                        before anything changes: a failed call leaves the previous heads.  Allocates here (a push still
+ *                        allocates nothing), per head: 4 * 3345 bytes of LSTM / Linear weights + 4 * L * 64 of W_ih^T,
+ *                        each rounded up to 256, plus on the tensor-core path the packed chunks (n_ranges *
+ *                        chunks_per_cta * 6144 bytes, as the handle's) and the range partials 4 * n_ranges * P * 64.
+ *                        Synchronises `stream`.
+ *   b2cnn_slide_n_heads  the number of heads attached (-1 for NULL).
+ *   b2cnn_slide_push_heads  b2cnn_slide_push, with out [1 + n_heads][P] on the DEVICE: row 0 exactly what
+ *                        b2cnn_slide_push writes, row i head i - 1's logits (or probabilities) of the same windows with
+ *                        its own LSTM, Linear and age_coef and the same ages, NaN for the patients whose row 0 is NaN.
+ *                        A head attached at push n scores from push n on, as a scorer of its model running since the
+ *                        start would.
+ * B2CNN_EINVAL: a NULL argument, n outside [0, B2CNN_SLIDE_MAX_HEADS], a head without weights or on another device.
+ * B2CNN_EARCH: a head of another architecture.  B2CNN_ESTATE: a head whose front-end digest is not the scorer's (at
+ * set_heads, or at push_heads after a reset that took other conv weights; the message names the head), or a scorer whose
+ * handle's weights changed since its last reset. */
+#define B2CNN_SLIDE_MAX_HEADS 8
+int b2cnn_slide_set_heads(b2cnn_slide *slide, b2cnn_handle *const *heads, int32_t n, void *stream);
+int b2cnn_slide_n_heads(const b2cnn_slide *slide);
+int b2cnn_slide_push_heads(b2cnn_slide *slide, const void *new_samples, int64_t pitch, const float *age, int64_t n_age,
+                           int apply_sigmoid, float *out, int32_t *emitted, int64_t *window_index, void *stream);
+
 /* ---- The reference's wire formats, decoded on the device (SURVEY.md section 8, row f3) ----
  * A trigger's Kafka messages as one DEVICE byte buffer + offsets [n_msgs + 1] (message t = bytes[offsets[t] .. offsets[t+1])).
  * b2cnn_decode_sample_messages: value = json.dumps([i, val]) (bin/sendStream.py:62): idx_out[t] = i, val_out[t] = val

@@ -590,7 +590,14 @@ extern "C" int b2cnn_features(b2cnn_handle *h, const void *x, int dtype, int64_t
 }
 
 // ---- sliding-window scorer over a per-patient feature ring (b2cnn_slide.cu) ----
-struct b2cnn_slide { Slide *s; b2cnn_handle *h; uint64_t gen; };
+// digest: the front-end digest of the handle's weights at the last reset (what every extra head must have)
+struct b2cnn_slide { Slide *s; b2cnn_handle *h; uint64_t gen; uint64_t digest; };
+
+static uint64_t weights_digest(const Slide *s, const ConvWeights &cw) {
+    b2cnn_slide_state_header hdr;
+    slide_describe_state(s, cw, &hdr);
+    return hdr.frontend_digest;
+}
 
 static int slide_create_on(const char *fn, b2cnn_handle *h, int32_t n_patients, int32_t stride, int dtype, int path, b2cnn_slide **out) {
     if (!h || !out) return fail(B2CNN_EINVAL, std::string(fn) + ": null argument");
@@ -607,7 +614,7 @@ static int slide_create_on(const char *fn, b2cnn_handle *h, int32_t n_patients, 
     const int rc = tc ? slide_create(h->d, h->tc, n_patients, stride, dtype, h->device, &s, &err)
                       : slide_create_generic(h->d, n_patients, stride, dtype, h->device, h->num_sms, &s, &err);
     if (rc != B2CNN_OK) return fail(rc, std::string(fn) + ": " + err);
-    b2cnn_slide *o = new (std::nothrow) b2cnn_slide{s, h, h->weight_gen};
+    b2cnn_slide *o = new (std::nothrow) b2cnn_slide{s, h, h->weight_gen, weights_digest(s, h->cw)};
     if (!o) { slide_destroy(s); return fail(B2CNN_ESTATE, "out of host memory"); }
     if (slide_reset(s, nullptr, &err) != B2CNN_OK || cudaStreamSynchronize(nullptr) != cudaSuccess) {
         b2cnn_slide_destroy(o);
@@ -636,14 +643,19 @@ extern "C" int b2cnn_slide_reset(b2cnn_slide *o, void *stream) {
     const int rc = slide_reset(o->s, reinterpret_cast<cudaStream_t>(stream), &err);
     if (rc != B2CNN_OK) return fail(rc, std::string("b2cnn_slide_reset: ") + err);
     o->gen = o->h->weight_gen;
+    o->digest = weights_digest(o->s, o->h->cw);
     return B2CNN_OK;
 }
-extern "C" int b2cnn_slide_push(b2cnn_slide *o, const void *new_samples, int64_t pitch, const float *age, int64_t n_age,
-                                int apply_sigmoid, float *out, int32_t *emitted, int64_t *window_index, void *stream) {
-    if (!o || !new_samples || !age || !out || !emitted || !window_index) return fail(B2CNN_EINVAL, "b2cnn_slide_push: null argument");
+static int slide_push_api(const char *fn, b2cnn_slide *o, const void *new_samples, int64_t pitch, const float *age, int64_t n_age,
+                          int apply_sigmoid, float *out, bool heads, int32_t *emitted, int64_t *window_index, void *stream) {
+    if (!o || !new_samples || !age || !out || !emitted || !window_index) return fail(B2CNN_EINVAL, std::string(fn) + ": null argument");
     b2cnn_handle *h = o->h;
     if (o->gen != h->weight_gen)
-        return fail(B2CNN_ESTATE, "b2cnn_slide_push: the handle's weights changed since the scorer's last reset (stored features are stale)");
+        return fail(B2CNN_ESTATE, std::string(fn) + ": the handle's weights changed since the scorer's last reset (stored features are stale)");
+    const int stale = heads ? slide_stale_head(o->s, o->digest) : -1;
+    if (stale >= 0)
+        return fail(B2CNN_ESTATE, std::string(fn) + ": head " + std::to_string(stale) +
+                                      " has other front-end weights than the scorer (its conv weights changed at the last reset)");
     DEVICE_GUARD(h->device);
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     cudaEvent_t *ev = nullptr;
@@ -655,12 +667,57 @@ extern "C" int b2cnn_slide_push(b2cnn_slide *o, const void *new_samples, int64_t
     const char *err = "";
     int em = 0;
     int64_t widx = -1;
-    const int rc = slide_push(o->s, h->cw, h->hw, h->tc, new_samples, pitch, age, n_age, apply_sigmoid, out, &em, &widx, ev, st, &err);
-    if (rc != B2CNN_OK) return fail(rc, std::string("b2cnn_slide_push: ") + err);
+    const int rc = slide_push(o->s, h->cw, h->hw, h->tc, new_samples, pitch, age, n_age, apply_sigmoid, out, heads, &em, &widx, ev, st,
+                              &err);
+    if (rc != B2CNN_OK) return fail(rc, std::string(fn) + ": " + err);
     h->ev_valid = ev != nullptr;
     *emitted = em;
     if (em) *window_index = widx;
     return B2CNN_OK;
+}
+extern "C" int b2cnn_slide_push(b2cnn_slide *o, const void *new_samples, int64_t pitch, const float *age, int64_t n_age,
+                                int apply_sigmoid, float *out, int32_t *emitted, int64_t *window_index, void *stream) {
+    return slide_push_api("b2cnn_slide_push", o, new_samples, pitch, age, n_age, apply_sigmoid, out, false, emitted, window_index, stream);
+}
+extern "C" int b2cnn_slide_push_heads(b2cnn_slide *o, const void *new_samples, int64_t pitch, const float *age, int64_t n_age,
+                                      int apply_sigmoid, float *out, int32_t *emitted, int64_t *window_index, void *stream) {
+    return slide_push_api("b2cnn_slide_push_heads", o, new_samples, pitch, age, n_age, apply_sigmoid, out, true, emitted, window_index,
+                          stream);
+}
+extern "C" int b2cnn_slide_n_heads(const b2cnn_slide *o) { return o ? slide_n_heads(o->s) : -1; }
+extern "C" int b2cnn_slide_set_heads(b2cnn_slide *o, b2cnn_handle *const *heads, int32_t n, void *stream) {
+    const char *fn = "b2cnn_slide_set_heads: ";
+    if (!o || (n > 0 && !heads)) return fail(B2CNN_EINVAL, std::string(fn) + "null argument");
+    if (n < 0 || n > B2CNN_SLIDE_MAX_HEADS)
+        return fail(B2CNN_EINVAL, std::string(fn) + "n must be in [0, " + std::to_string(B2CNN_SLIDE_MAX_HEADS) + "]");
+    const b2cnn_handle *h = o->h;
+    const b2cnn_config &c = h->cfg;
+    std::vector<SlideHeadSource> src((size_t)n);
+    for (int i = 0; i < n; ++i) {
+        const b2cnn_handle *x = heads[i];
+        const std::string which = "head " + std::to_string(i) + ": ";
+        if (!x) return fail(B2CNN_EINVAL, fn + which + "null handle");
+        if (!x->weights_set) return fail(B2CNN_EINVAL, fn + which + "weights not set (call b2cnn_set_weights)");
+        if (x->device != h->device) return fail(B2CNN_EINVAL, fn + which + "on another device than the scorer");
+        const b2cnn_config &e = x->cfg;
+        if (e.in_channels != c.in_channels || e.k1 != c.k1 || e.c_mid != c.c_mid || e.k2 != c.k2 || e.pool_k != c.pool_k ||
+            e.pool_s != c.pool_s || e.hidden != c.hidden || e.layers != c.layers || e.window != c.window ||
+            e.lstm_input != c.lstm_input || e.act != c.act || e.flags != c.flags)
+            return fail(B2CNN_EARCH, fn + which + "another architecture than the scorer's model (only age_coef may differ)");
+        if (slide_path(o->s) == B2CNN_PATH_TENSORCORE && (!x->tc.fused || x->tc.n_ranges != h->tc.n_ranges ||
+                                                          x->tc.chunks_per_cta != h->tc.chunks_per_cta))
+            return fail(B2CNN_EARCH, fn + which + "no packed W_ih chunks of the scorer's layout");
+        src[i] = SlideHeadSource{x->hw, &x->tc, x->d.age_coef, weights_digest(o->s, x->cw)};
+    }
+    if (o->gen != h->weight_gen)
+        return fail(B2CNN_ESTATE, std::string(fn) + "the scorer's handle's weights changed since its last reset (call reset first)");
+    for (int i = 0; i < n; ++i)
+        if (src[i].digest != o->digest)
+            return fail(B2CNN_ESTATE, fn + ("head " + std::to_string(i)) + ": other front-end (conv / affine) weights than the scorer's");
+    DEVICE_GUARD(h->device);
+    const char *err = "";
+    const int rc = slide_set_heads(o->s, src.data(), n, reinterpret_cast<cudaStream_t>(stream), &err);
+    return rc == B2CNN_OK ? rc : fail(rc, fn + std::string(err));
 }
 extern "C" int b2cnn_slide_features(b2cnn_slide *o, float *feats, void *stream) {
     if (!o || !feats) return fail(B2CNN_EINVAL, "b2cnn_slide_features: null argument");

@@ -34,6 +34,7 @@
 #include <algorithm>
 #include <cstring>
 #include <new>
+#include <type_traits>
 #include <vector>
 
 #include "b2cnn_slide.cuh"
@@ -42,6 +43,17 @@
 namespace b2cnn {
 
 constexpr int kSlideTail = 24;       // stream samples kept per patient and channel: the largest receptive field
+
+// An extra head scored from the scorer's ring (b2cnn_slide_set_heads): a snapshot of a model's LSTM / Linear weights,
+// W_ih^T, age coefficient and (tensor-core path) packed W_ih chunks, with its range partials, in one allocation.
+struct SlideHead {
+    HeadWeights hw;                  // into mem
+    float age_coef = 0.f;
+    uint64_t digest = 0;             // the model's front-end digest when it was attached
+    const uint8_t *wpack = nullptr;  // tensor-core path: [n_ranges][chunks_per_cta][6 KB], into mem
+    float *partial = nullptr;        // tensor-core path: [n_ranges][P][64], into mem
+    void *mem = nullptr;
+};
 
 struct Slide {
     int device;
@@ -66,6 +78,7 @@ struct Slide {
     bool lifecycle = false;          // set by the first admit / discharge since the last reset
     int64_t *seen = nullptr;         // [P] on the device: samples since admission, -1: discharged (while lifecycle)
     std::vector<int64_t> seen_h;     // its host mirror, equal to it in stream order
+    std::vector<SlideHead> heads;    // extra heads, rows 1.. of a push with heads
 };
 
 static int64_t fdiv4(int64_t a) { return a >= 0 ? a / 4 : -((-a + 3) / 4); }
@@ -199,7 +212,10 @@ constexpr int kRpM = 128;                            // patients per CTA
 constexpr int kRpBox = 16 * kRpM * 4;                // one TMA box: 16 slots x 128 patients fp32
 constexpr int kRpWChunk = 3 * 64 * 16 * 2;           // a packed W_ih chunk (tc_pack_wih_kernel, kFuWChunkBytes)
 constexpr int kRpPiece = kRpM * 16 * 2;              // one bf16 piece of the A tile
-constexpr size_t kRpSmem = 1024 + 2 * 2 * kRpBox + 2 * kRpWChunk + 3 * kRpPiece + 64;
+// HP: heads per CTA, each with its own W_ih chunk slot per stage (HP = 1: the scorer's own model alone)
+template <int HP>
+constexpr size_t kRpSmemHP = 1024 + 2 * 2 * kRpBox + 2 * HP * kRpWChunk + 3 * kRpPiece + 64;
+constexpr size_t kRpSmem = kRpSmemHP<1>;
 
 struct RingProjParams {
     const uint8_t *wpack;            // [n_ranges][chunks_per_cta][kRpWChunk]
@@ -207,18 +223,46 @@ struct RingProjParams {
     int P, L, head, feats_per_cta, chunks_per_cta, foff;
 };
 
+// A push with heads: rows 0 (the scorer's model) .. K (its heads) of the output, HP rows per CTA.  CTA x = tile * pairs
+// + pair, so that the pairs of one (patient tile, range) are neighbours in launch order and may find its ring box in L2.
+constexpr int kRpMaxRows = 1 + B2CNN_SLIDE_MAX_HEADS;
+struct RingProjHeads {
+    RingProjParams p;                         // its wpack / partial are not read
+    const uint8_t *wpack[kRpMaxRows + 1];     // row r's packed W_ih chunks
+    float *partial[kRpMaxRows + 1];           // row r's [n_ranges][P][64]; nullptr: a padding row, computed, not stored
+    int pairs;                                // CTAs per (patient tile, range)
+};
+template <int HP>
+using RingProjArgs = std::conditional_t<HP == 1, RingProjParams, RingProjHeads>;
+__device__ __forceinline__ const RingProjParams &rp_base(const RingProjParams &a) { return a; }
+__device__ __forceinline__ const RingProjParams &rp_base(const RingProjHeads &a) { return a.p; }
+
+// Per head the instructions are those of HP = 1: the same A pieces, the same 12 MMAs per chunk in the same order, the
+// same chunk order.  So each head's partials are bit-identical to those of a scorer of its model.
+template <int HP>
 __global__ void __launch_bounds__(kRpThreads, 1)
-slide_ring_proj_kernel(const __grid_constant__ CUtensorMap tm, const __grid_constant__ RingProjParams p) {
+slide_ring_proj_kernel(const __grid_constant__ CUtensorMap tm, const __grid_constant__ RingProjArgs<HP> args) {
+    const RingProjParams &p = rp_base(args);
     extern __shared__ uint8_t smem_raw[];
     uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     float *sF = reinterpret_cast<float *>(smem);                  // [2 stages][2 boxes][16][128]
-    uint8_t *sW = smem + 2 * 2 * kRpBox;                           // [2 stages][6 KB]
-    uint8_t *sPc = sW + 2 * kRpWChunk;                             // [3 pieces][4 KB]
+    uint8_t *sW = smem + 2 * 2 * kRpBox;                           // [2 stages][HP][6 KB]
+    uint8_t *sPc = sW + 2 * HP * kRpWChunk;                        // [3 pieces][4 KB]
     uint64_t *bars = reinterpret_cast<uint64_t *>(sPc + 3 * kRpPiece);
     const uint32_t bar_full = smem_u32(bars + 0), bar_empty = smem_u32(bars + 2);
     const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);
     const int lane = threadIdx.x & 31;
-    const int b0 = blockIdx.x * kRpM;
+    int tile = blockIdx.x, row0 = 0;
+    if constexpr (HP > 1) { tile = blockIdx.x / args.pairs; row0 = HP * (blockIdx.x - tile * args.pairs); }
+    auto wpack_of = [&](int j) {
+        if constexpr (HP == 1) return p.wpack;
+        else return args.wpack[row0 + j];
+    };
+    auto partial_of = [&](int j) {
+        if constexpr (HP == 1) return p.partial;
+        else return args.partial[row0 + j];
+    };
+    const int b0 = tile * kRpM;
     const int lo = blockIdx.y * p.feats_per_cta, hi = min(p.L, lo + p.feats_per_cta);
     const int nch = p.chunks_per_cta;
     if (threadIdx.x == 0) {
@@ -238,22 +282,26 @@ slide_ring_proj_kernel(const __grid_constant__ CUtensorMap tm, const __grid_cons
                 mbar_wait(bar_empty + 8 * u, ((m >> 1) & 1) ^ 1);
                 const int s0 = first_slot(m);
                 const bool wraps = s0 + 16 > p.L;
-                mbar_expect_tx(bar_full + 8 * u, (wraps ? 2 : 1) * kRpBox + kRpWChunk);
+                mbar_expect_tx(bar_full + 8 * u, (wraps ? 2 : 1) * kRpBox + HP * kRpWChunk);
                 const uint32_t dst = smem_u32(sF + (size_t)u * 2 * 16 * kRpM);
                 tma_load_2d(dst, &tm, b0, s0, bar_full + 8 * u);
                 if (wraps) tma_load_2d(dst + kRpBox, &tm, b0, 0, bar_full + 8 * u);
-                bulk_load_1d(smem_u32(sW + u * kRpWChunk), p.wpack + ((size_t)blockIdx.y * nch + m) * kRpWChunk, kRpWChunk,
-                             bar_full + 8 * u);
+#pragma unroll
+                for (int j = 0; j < HP; ++j)
+                    bulk_load_1d(smem_u32(sW + (u * HP + j) * kRpWChunk), wpack_of(j) + ((size_t)blockIdx.y * nch + m) * kRpWChunk,
+                                 kRpWChunk, bar_full + 8 * u);
             }
         }
         return;
     }
     const int row = threadIdx.x;
-    float gacc[2][32];
+    float gacc[HP][2][32];
 #pragma unroll
-    for (int h = 0; h < 2; ++h)
+    for (int j = 0; j < HP; ++j)
 #pragma unroll
-        for (int i = 0; i < 32; ++i) gacc[h][i] = 0.f;
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int i = 0; i < 32; ++i) gacc[j][h][i] = 0.f;
     uint8_t *arow = sPc + (row >> 3) * 256 + (row & 7) * 16;
 #pragma unroll 1
     for (int m = 0; m < nch; ++m) {
@@ -280,15 +328,19 @@ slide_ring_proj_kernel(const __grid_constant__ CUtensorMap tm, const __grid_cons
         }
         fence_proxy_async();
         wg_bar();
-        const uint32_t pa = smem_u32(sPc), pw = smem_u32(sW + u * kRpWChunk);
+        const uint32_t pa = smem_u32(sPc);
         wgmma_fence();
 #pragma unroll
-        for (int hh = 0; hh < 2; ++hh) {
-            constexpr int kAp[6] = {0, 0, 1, 0, 2, 1}, kWp[6] = {0, 1, 0, 2, 0, 1};
+        for (int j = 0; j < HP; ++j) {
+            const uint32_t pw = smem_u32(sW + (u * HP + j) * kRpWChunk);
 #pragma unroll
-            for (int q = 0; q < 6; ++q)
-                wgmma_m64n64(gacc[hh], gdesc_none_kmajor(pa + kAp[q] * kRpPiece + hh * 2048, 128, 256),
-                             gdesc_none_kmajor(pw + kWp[q] * 2048, 128, 256));
+            for (int hh = 0; hh < 2; ++hh) {
+                constexpr int kAp[6] = {0, 0, 1, 0, 2, 1}, kWp[6] = {0, 1, 0, 2, 0, 1};
+#pragma unroll
+                for (int q = 0; q < 6; ++q)
+                    wgmma_m64n64(gacc[j][hh], gdesc_none_kmajor(pa + kAp[q] * kRpPiece + hh * 2048, 128, 256),
+                                 gdesc_none_kmajor(pw + kWp[q] * 2048, 128, 256));
+            }
         }
         wgmma_commit();
         wgmma_wait<0>();
@@ -297,17 +349,22 @@ slide_ring_proj_kernel(const __grid_constant__ CUtensorMap tm, const __grid_cons
         wg_bar();                                                  // A tile free for the next chunk
     }
 #pragma unroll
-    for (int hh = 0; hh < 2; ++hh)
+    for (int j = 0; j < HP; ++j) {
+        float *const part = partial_of(j);
+        if (HP > 1 && !part) continue;
 #pragma unroll
-        for (int e2 = 0; e2 < 2; ++e2) {
-            const int bb = b0 + 64 * hh + 16 * warp + (lane >> 2) + 8 * e2;
-            if (bb < p.P) {
-                float *dst = p.partial + ((int64_t)blockIdx.y * p.P + bb) * kGates + 2 * (lane & 3);
+        for (int hh = 0; hh < 2; ++hh)
 #pragma unroll
-                for (int e = 2 * e2; e < 32; e += 4)
-                    *reinterpret_cast<float2 *>(dst + 8 * (e >> 2)) = make_float2(gacc[hh][e], gacc[hh][e + 1]);
+            for (int e2 = 0; e2 < 2; ++e2) {
+                const int bb = b0 + 64 * hh + 16 * warp + (lane >> 2) + 8 * e2;
+                if (bb < p.P) {
+                    float *dst = part + ((int64_t)blockIdx.y * p.P + bb) * kGates + 2 * (lane & 3);
+#pragma unroll
+                    for (int e = 2 * e2; e < 32; e += 4)
+                        *reinterpret_cast<float2 *>(dst + 8 * (e >> 2)) = make_float2(gacc[j][hh][e], gacc[j][hh][e + 1]);
+                }
             }
-        }
+    }
 }
 
 // feats[b][j] = ring[(head + j) mod cap][b]
@@ -493,11 +550,11 @@ int slide_create_generic(const Dims &d, int n_patients, int stride, int dtype, i
 }
 
 static int score_windows(Slide *s, const HeadWeights &hw, const TcState *tc, const float *age, int64_t n_age, int apply_sigmoid,
-                         float *out, int *emitted, int64_t *window_index, cudaEvent_t *ev, cudaStream_t st, const char **err);
+                         float *out, bool heads, int *emitted, int64_t *window_index, cudaEvent_t *ev, cudaStream_t st, const char **err);
 
 static int slide_push_generic(Slide *s, const ConvWeights &cw, const HeadWeights &hw, const void *x, int64_t pitch, const float *age,
-                              int64_t n_age, int apply_sigmoid, float *out, int *emitted, int64_t *window_index, cudaEvent_t *ev,
-                              cudaStream_t st, const char **err) {
+                              int64_t n_age, int apply_sigmoid, float *out, bool heads, int *emitted, int64_t *window_index,
+                              cudaEvent_t *ev, cudaStream_t st, const char **err) {
     const Dims &d = s->d;
     const int64_t P = s->P, S = s->S, T = s->T;
     if (pitch < S || pitch > 0x7fffffff) { *err = "pitch must be in [stride, 2^31)"; return B2CNN_EINVAL; }
@@ -545,7 +602,7 @@ static int slide_push_generic(Slide *s, const ConvWeights &cw, const HeadWeights
     s->n = n1;
     if (g_hi >= g_lo) s->g_done = g_hi;
     s->tail_cur ^= 1;
-    return score_windows(s, hw, nullptr, age, n_age, apply_sigmoid, out, emitted, window_index, ev, st, err);
+    return score_windows(s, hw, nullptr, age, n_age, apply_sigmoid, out, heads, emitted, window_index, ev, st, err);
 }
 
 int slide_create(const Dims &d, const TcState &tc, int n_patients, int stride, int dtype, int device, Slide **out,
@@ -584,6 +641,7 @@ void slide_destroy(Slide *s) {
     if (!s) return;
     cudaFree(s->ring); cudaFree(s->tail); cudaFree(s->partial); cudaFree(s->gates); cudaFree(s->flags); cudaFree(s->stage);
     cudaFree(s->seen);
+    for (SlideHead &hd : s->heads) cudaFree(hd.mem);
     delete s;
 }
 
@@ -619,10 +677,10 @@ static int advance_seen(Slide *s, float *out, cudaStream_t st, const char **err)
 }
 
 int slide_push(Slide *s, const ConvWeights &cw, const HeadWeights &hw, const TcState &tc, const void *x, int64_t pitch,
-               const float *age, int64_t n_age, int apply_sigmoid, float *out, int *emitted, int64_t *window_index,
+               const float *age, int64_t n_age, int apply_sigmoid, float *out, bool heads, int *emitted, int64_t *window_index,
                cudaEvent_t *ev, cudaStream_t st, const char **err) {
     if (s->path == B2CNN_PATH_GENERIC)
-        return slide_push_generic(s, cw, hw, x, pitch, age, n_age, apply_sigmoid, out, emitted, window_index, ev, st, err);
+        return slide_push_generic(s, cw, hw, x, pitch, age, n_age, apply_sigmoid, out, heads, emitted, window_index, ev, st, err);
     const Dims &d = s->d;
     const int64_t P = s->P, S = s->S, esz = s->dtype == B2CNN_DTYPE_BF16 ? 2 : 4;
     if (pitch < S) { *err = "pitch must be >= stride"; return B2CNN_EINVAL; }
@@ -682,15 +740,25 @@ int slide_push(Slide *s, const ConvWeights &cw, const HeadWeights &hw, const TcS
     s->n = n1;
     if (g_hi >= g_lo) s->g_done = g_hi;
     s->tail_cur ^= 1;
-    return score_windows(s, hw, &tc, age, n_age, apply_sigmoid, out, emitted, window_index, ev, st, err);
+    return score_windows(s, hw, &tc, age, n_age, apply_sigmoid, out, heads, emitted, window_index, ev, st, err);
+}
+
+// the model's Dims with a head's age coefficient: the reduction / LSTM head launchers take it from there
+static Dims head_dims(const Dims &d, const SlideHead &hd) {
+    Dims dh = d;
+    dh.age_coef = hd.age_coef;
+    return dh;
 }
 
 // the end of push n = s->n: projection over the ring + head, once a window is complete (every patient's, or with the
-// lifecycle on, one); on tensor cores with `tc`, else (generic path) on CUDA cores
+// lifecycle on, one); on tensor cores with `tc`, else (generic path) on CUDA cores.  With `heads`, out is [1 + K][P]:
+// row 0 the scorer's model as without, row i head i - 1 from the same ring.
 static int score_windows(Slide *s, const HeadWeights &hw, const TcState *tc, const float *age, int64_t n_age, int apply_sigmoid,
-                         float *out, int *emitted, int64_t *window_index, cudaEvent_t *ev, cudaStream_t st, const char **err) {
+                         float *out, bool heads, int *emitted, int64_t *window_index, cudaEvent_t *ev, cudaStream_t st,
+                         const char **err) {
     const Dims &d = s->d;
     const int64_t P = s->P, S = s->S, n1 = s->n;
+    const int K = heads ? (int)s->heads.size() : 0;
     bool live = n1 * S >= d.W;
     if (s->lifecycle)
         live = std::any_of(s->seen_h.begin(), s->seen_h.end(), [&](int64_t v) { return v >= 0 && v + S >= d.W; });
@@ -704,6 +772,13 @@ static int score_windows(Slide *s, const HeadWeights &hw, const TcState *tc, con
     if (!tc) {
         if (launch_ring_head(d, hw, s->ring, s->ring_pitch, head, P, age, n_age, apply_sigmoid, out, s->gates, s->partial, st, err) < 0)
             return B2CNN_ECUDA;
+        // each head: the same kernels over the same ring with its own W_ih^T, LSTM, Linear and age coefficient
+        for (int i = 0; i < K; ++i) {
+            const SlideHead &hd = s->heads[i];
+            if (launch_ring_head(head_dims(d, hd), hd.hw, s->ring, s->ring_pitch, head, P, age, n_age, apply_sigmoid, out + (i + 1) * P,
+                                 s->gates, s->partial, st, err) < 0)
+                return B2CNN_ECUDA;
+        }
     } else {
         CUtensorMap tm;
         if (tc_ring_tmap(s->ring, P, s->ring_pitch, d.L, &tm, err) != 0) return B2CNN_ECUDA;
@@ -711,14 +786,41 @@ static int score_windows(Slide *s, const HeadWeights &hw, const TcState *tc, con
         rp.wpack = reinterpret_cast<const uint8_t *>(tc->d_wpack); rp.partial = s->partial;
         rp.P = (int)P; rp.L = d.L; rp.head = head;
         rp.feats_per_cta = tc->feats_per_cta; rp.chunks_per_cta = tc->chunks_per_cta; rp.foff = d.K1 == 10 ? 3 : 2;
-        if (cudaFuncSetAttribute(slide_ring_proj_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kRpSmem) != cudaSuccess) {
-            *err = "projection smem attribute"; return B2CNN_ECUDA;
+        const unsigned tiles = (unsigned)((P + kRpM - 1) / kRpM);
+        if (K == 0) {
+            if (cudaFuncSetAttribute(slide_ring_proj_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kRpSmem) != cudaSuccess) {
+                *err = "projection smem attribute"; return B2CNN_ECUDA;
+            }
+            slide_ring_proj_kernel<1><<<dim3(tiles, (unsigned)s->ranges), kRpThreads, kRpSmem, st>>>(tm, rp);
+        } else {
+            // rows 0 .. K in pairs; an odd count pads the last pair with a copy of its row that is not stored
+            RingProjHeads a;
+            memset(&a, 0, sizeof a);
+            a.p = rp;
+            a.wpack[0] = rp.wpack; a.partial[0] = s->partial;
+            for (int i = 0; i < K; ++i) { a.wpack[i + 1] = s->heads[i].wpack; a.partial[i + 1] = s->heads[i].partial; }
+            const int rows = K + 1;
+            a.pairs = (rows + 1) / 2;
+            if (rows % 2) a.wpack[rows] = a.wpack[rows - 1];             // partial[rows] stays nullptr
+            if (cudaFuncSetAttribute(slide_ring_proj_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kRpSmemHP<2>) !=
+                cudaSuccess) {
+                *err = "projection smem attribute"; return B2CNN_ECUDA;
+            }
+            slide_ring_proj_kernel<2><<<dim3(tiles * (unsigned)a.pairs, (unsigned)s->ranges), kRpThreads, kRpSmemHP<2>, st>>>(tm, a);
         }
-        slide_ring_proj_kernel<<<dim3((unsigned)((P + kRpM - 1) / kRpM), (unsigned)s->ranges), kRpThreads, kRpSmem, st>>>(tm, rp);
         if (cudaGetLastError() != cudaSuccess) { *err = "projection launch"; return B2CNN_ECUDA; }
         if (launch_reduce_lstm_head(d, hw, s->partial, s->ranges, P, age, n_age, apply_sigmoid, out, st, err) < 0) return B2CNN_ECUDA;
+        for (int i = 0; i < K; ++i) {
+            const SlideHead &hd = s->heads[i];
+            if (launch_reduce_lstm_head(head_dims(d, hd), hd.hw, hd.partial, s->ranges, P, age, n_age, apply_sigmoid, out + (i + 1) * P,
+                                        st, err) < 0)
+                return B2CNN_ECUDA;
+        }
     }
+    // row 0 is masked as without heads, and seen advances once; rows 1..K take the mask from the advanced counts
     if (s->lifecycle && advance_seen(s, out, st, err) < 0) return B2CNN_ECUDA;
+    for (int i = 0; s->lifecycle && i < K; ++i)
+        if (launch_live(*s, 0, out + (i + 1) * P, 1, st, err) < 0) return B2CNN_ECUDA;
     if (ev && cudaEventRecord(ev[2], st) != cudaSuccess) { *err = "cudaEventRecord"; return B2CNN_ECUDA; }
     *emitted = 1;
     *window_index = n1 - (d.W + S - 1) / S;
@@ -989,6 +1091,78 @@ static uint64_t frontend_digest(const Dims &d, const ConvWeights &cw) {
         h = fnv1a(h, &cw.t2, sizeof cw.t2);
     }
     return h;
+}
+
+// ---- extra heads --------------------------------------------------------------------------------------------------
+// One allocation per head: the blob's LSTM / Linear part (whh0 .. bo, contiguous in b2cnn_set_weights' blob) | W_ih^T
+// [L][64] | tensor-core path: the packed W_ih chunks | the range partials [n_ranges][P][64].  The generic path's heads
+// run one after another on the scorer's own partials and gates.
+struct HeadLayout {
+    size_t lstm, wih0T, wpack, partial, total;
+    int64_t n_lstm;
+};
+static HeadLayout head_layout(const Slide &s, const HeadWeights &hw, const TcState *tc) {
+    HeadLayout a;
+    a.n_lstm = hw.bo + 1 - hw.whh0;
+    a.lstm = al256(sizeof(float) * (size_t)a.n_lstm);
+    a.wih0T = al256(sizeof(float) * (size_t)s.d.L * kGates);
+    const bool tcp = s.path == B2CNN_PATH_TENSORCORE;
+    a.wpack = tcp ? al256((size_t)tc->n_ranges * tc->chunks_per_cta * kRpWChunk) : 0;
+    a.partial = tcp ? al256(sizeof(float) * (size_t)s.ranges * s.P * kGates) : 0;
+    a.total = a.lstm + a.wih0T + a.wpack + a.partial;
+    return a;
+}
+
+static const float *rebase(const float *p, const float *from, float *to) { return to + (p - from); }
+
+int slide_set_heads(Slide *s, const SlideHeadSource *src, int n, cudaStream_t st, const char **err) {
+    std::vector<SlideHead> next((size_t)n);
+    auto drop = [&](const char *what) {
+        (void)cudaGetLastError();
+        for (SlideHead &hd : next) cudaFree(hd.mem);
+        *err = what;
+        return B2CNN_ECUDA;
+    };
+    for (int i = 0; i < n; ++i) {
+        const HeadWeights &w = src[i].hw;
+        const HeadLayout a = head_layout(*s, w, src[i].tc);
+        SlideHead &hd = next[i];
+        if (cudaMalloc(&hd.mem, a.total) != cudaSuccess) return drop("cudaMalloc(head weights)");
+        char *base = static_cast<char *>(hd.mem);
+        float *lstm = reinterpret_cast<float *>(base), *wih0T = reinterpret_cast<float *>(base + a.lstm);
+        if (cudaMemcpyAsync(lstm, w.whh0, sizeof(float) * (size_t)a.n_lstm, cudaMemcpyDeviceToDevice, st) != cudaSuccess ||
+            cudaMemcpyAsync(wih0T, w.wih0T, sizeof(float) * (size_t)s->d.L * kGates, cudaMemcpyDeviceToDevice, st) != cudaSuccess)
+            return drop("copy of the head weights");
+        hd.hw.wih0T = wih0T;
+        hd.hw.whh0 = rebase(w.whh0, w.whh0, lstm); hd.hw.bih0 = rebase(w.bih0, w.whh0, lstm); hd.hw.bhh0 = rebase(w.bhh0, w.whh0, lstm);
+        hd.hw.wih1 = rebase(w.wih1, w.whh0, lstm); hd.hw.whh1 = rebase(w.whh1, w.whh0, lstm);
+        hd.hw.bih1 = rebase(w.bih1, w.whh0, lstm); hd.hw.bhh1 = rebase(w.bhh1, w.whh0, lstm);
+        hd.hw.wo = rebase(w.wo, w.whh0, lstm); hd.hw.bo = rebase(w.bo, w.whh0, lstm);
+        hd.age_coef = src[i].age_coef;
+        hd.digest = src[i].digest;
+        if (s->path == B2CNN_PATH_TENSORCORE) {
+            uint8_t *wp = reinterpret_cast<uint8_t *>(base + a.lstm + a.wih0T);
+            if (cudaMemcpyAsync(wp, src[i].tc->d_wpack, (size_t)src[i].tc->n_ranges * src[i].tc->chunks_per_cta * kRpWChunk,
+                                cudaMemcpyDeviceToDevice, st) != cudaSuccess)
+                return drop("copy of the packed W_ih chunks");
+            hd.wpack = wp;
+            hd.partial = reinterpret_cast<float *>(base + a.lstm + a.wih0T + a.wpack);
+        }
+    }
+    // the snapshot is complete when the call returns: later weight changes of the models cannot reach it
+    if (cudaStreamSynchronize(st) != cudaSuccess) return drop("copy of the head weights");
+    for (SlideHead &hd : s->heads) cudaFree(hd.mem);
+    s->heads.swap(next);
+    return B2CNN_OK;
+}
+
+int slide_n_heads(const Slide *s) { return (int)s->heads.size(); }
+
+// the first head whose front-end digest is not `digest`, or -1
+int slide_stale_head(const Slide *s, uint64_t digest) {
+    for (size_t i = 0; i < s->heads.size(); ++i)
+        if (s->heads[i].digest != digest) return (int)i;
+    return -1;
 }
 
 void slide_describe_state(const Slide *s, const ConvWeights &cw, b2cnn_slide_state_header *o) {

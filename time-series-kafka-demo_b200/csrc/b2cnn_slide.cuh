@@ -16,10 +16,23 @@ int slide_path(const Slide *s);   // B2CNN_PATH_TENSORCORE or B2CNN_PATH_GENERIC
 void slide_destroy(Slide *s);
 int slide_device(const Slide *s);
 int slide_reset(Slide *s, cudaStream_t st, const char **err);
-// ev: nullptr, or three events recorded at the start, after the front end and after the head (profiling)
+// ev: nullptr, or three events recorded at the start, after the front end and after the head (profiling).
+// heads: out is [1 + slide_n_heads][P], row 0 the model's logits as without, row i those of head i - 1.
 int slide_push(Slide *s, const ConvWeights &cw, const HeadWeights &hw, const TcState &tc, const void *x, int64_t pitch,
-               const float *age, int64_t n_age, int apply_sigmoid, float *out, int *emitted, int64_t *window_index,
+               const float *age, int64_t n_age, int apply_sigmoid, float *out, bool heads, int *emitted, int64_t *window_index,
                cudaEvent_t *ev, cudaStream_t st, const char **err);
+// extra heads (b2cnn_slide_set_heads): what a head is copied from -- a handle of the same architecture and front end
+struct SlideHeadSource {
+    HeadWeights hw;                  // the handle's pointers into its blob and its W_ih^T
+    const TcState *tc;               // its packed W_ih chunks (tensor-core path)
+    float age_coef;
+    uint64_t digest;                 // its front-end digest
+};
+// replaces the heads with copies of src[0 .. n) (allocated and copied here, the stream synchronised); on failure the
+// previous heads stay
+int slide_set_heads(Slide *s, const SlideHeadSource *src, int n, cudaStream_t st, const char **err);
+int slide_n_heads(const Slide *s);
+int slide_stale_head(const Slide *s, uint64_t digest);
 int slide_features(const Slide *s, float *feats, cudaStream_t st, const char **err);
 // per-patient lifecycle: `patients` host indices; `hist` [k][C][pitch] device samples in the scorer's dtype
 int64_t slide_admit_workspace_bytes(const Slide *s, int64_t k, int64_t H);

@@ -18,6 +18,13 @@ the same model front end, path and dtype, which then continues those streams bit
 
     torch.save(scorer.export(range(P)), "ward.pt")                   # before a restart
     scorer.restore(range(P), torch.load("ward.pt"))                  # in the new process: no window is lost
+
+``set_heads(models)`` attaches up to 8 extra heads -- models with the scorer's architecture and conv weights whose
+LSTM, Linear or age coefficient differ (a retrained candidate, an ensemble) -- scored at every push from the same
+stored features, with no cold start and no second front end::
+
+    scorer.set_heads([candidate])
+    out = scorer.push(samples, age=ages, heads=True)                 # [2, P]: production row 0, candidate row 1
 """
 from __future__ import annotations
 
@@ -43,7 +50,13 @@ class SlidingScorer:
     MyCNN5 or MyCNN2/3/4 conv/pool geometry with 1 to 3 channels; ``"generic"`` runs exact fp32 CUDA-core kernels for
     any model the library accepts (its logits are ``predict()``'s with ``path="generic"`` and ``small_kernel=0``), with
     ``stride`` a multiple of the feature stride ``pool_s ** 2``; ``"auto"`` takes the tensor-core path where it holds
-    the model and the generic one otherwise.  ``scorer.path`` tells which one runs."""
+    the model and the generic one otherwise.  ``scorer.path`` tells which one runs.
+
+    Extra heads: ``set_heads(models)`` attaches models of the same architecture and front-end (conv / affine) weights,
+    ``push(..., heads=True)`` returns ``Tensor[1 + K, P]``, row 0 what ``push`` returns and row i ``heads[i - 1]``'s
+    logits of the same windows.  ``heads`` is the tuple attached."""
+
+    ARCH_FIELDS = ("in_channels", "window", "k1", "k2", "pool_k", "pool_s", "act", "affine", "l_out", "c_mid", "hidden", "layers")
 
     PATHS = {"tensorcore": capi.PATH_TENSORCORE, "generic": capi.PATH_GENERIC, "auto": capi.PATH_AUTO}
     STATE_HEADER = tuple(n for n, _ in capi.SlideStateHeader._fields_)
@@ -73,6 +86,7 @@ class SlidingScorer:
                 capi.check(self._lib.b2cnn_slide_create_path(h, n_patients, stride, self._dt(), self.PATHS[path], ctypes.byref(s)),
                            "b2cnn_slide_create_path")
         self._s = s
+        self._heads = ()
         self.path = "generic" if self._lib.b2cnn_slide_path(s) == capi.PATH_GENERIC else "tensorcore"
         self.window_index = -1
         hdr = capi.SlideStateHeader()
@@ -161,12 +175,55 @@ class SlidingScorer:
             raise ValueError(f"expected a {self.dtype} history (the scorer's dtype), got {history.dtype}")
         return self._pitch(history)
 
+    @property
+    def heads(self) -> tuple:
+        """The models attached by ``set_heads`` (read-only)."""
+        return self._heads
+
+    def check_heads(self, models) -> tuple:
+        """Validates ``set_heads``' argument without touching the library; returns the models as a tuple."""
+        from .model import B200MyCNN
+        if isinstance(models, (B200MyCNN, torch.Tensor, str, bytes)) or not hasattr(models, "__iter__"):
+            raise TypeError("set_heads takes a list of B200MyCNN models")
+        models = tuple(models)
+        if len(models) > capi.SLIDE_MAX_HEADS:
+            raise ValueError(f"at most {capi.SLIDE_MAX_HEADS} heads, got {len(models)}")
+        mine = self.model.arch
+        for i, m in enumerate(models):
+            if not isinstance(m, B200MyCNN):
+                raise TypeError(f"heads[{i}] is a {type(m).__name__}, not a B200MyCNN")
+            bad = [f for f in self.ARCH_FIELDS if getattr(m.arch, f) != getattr(mine, f)]
+            if bad:
+                raise ValueError(f"heads[{i}] differs from the scorer's model in {', '.join(bad)}")
+            if m._device() != self.device:
+                raise ValueError(f"heads[{i}] is on {m._device()}, the scorer on {self.device}")
+        return models
+
+    def set_heads(self, models):
+        """Replace the extra heads with ``models`` (a list of ``B200MyCNN``, possibly empty, at most 8): each with the
+        scorer model's architecture (``age_coef`` may differ), its conv / affine weights and its device.  Takes a
+        SNAPSHOT of each head's LSTM / Linear weights and ``age_coef``: a later change to a head model's weights has no
+        effect until ``set_heads`` is called again.  A head attached at push n is scored from push n on, as a scorer of
+        that model running since the start would score it.  Atomic: a failed call leaves the previous heads."""
+        models = self.check_heads(models)
+        self._handle()
+        hs = [m._ensure_handle()[1].value for m in models]
+        arr = (ctypes.c_void_p * max(len(hs), 1))(*hs)
+        with torch.cuda.device(self.device):
+            capi.check(self._lib.b2cnn_slide_set_heads(self._s, arr, len(hs), torch.cuda.current_stream().cuda_stream),
+                       "b2cnn_slide_set_heads")
+        self._heads = models
+
     @torch.no_grad()
-    def push(self, samples: torch.Tensor, age=65.0, return_prob: bool = False):
+    def push(self, samples: torch.Tensor, age=65.0, return_prob: bool = False, heads: bool = False):
         """``samples`` [P, C, stride] of the scorer's dtype (a row-padded view is read in place, like ``predict``);
         ``age`` scalar or [P].  Returns the logits (or probabilities) of the P current windows, or ``None`` while the
         first window fills.  After ``admit`` / ``discharge``: NaN for every patient whose window is not complete
-        (``samples_seen < W``; a discharged patient's samples are ignored), ``None`` when no patient's window is."""
+        (``samples_seen < W``; a discharged patient's samples are ignored), ``None`` when no patient's window is.
+        ``heads=True``: ``Tensor[1 + K, P]`` (or ``None`` as above), row 0 exactly what ``heads=False`` returns, row i
+        the scores of ``heads[i - 1]`` on the same windows and ages, NaN where row 0 is."""
+        if not isinstance(heads, bool):
+            raise TypeError(f"heads must be True or False, got {type(heads).__name__}")
         pitch = self.check_samples(samples)
         self._handle()
         if samples.device != self.device:
@@ -180,11 +237,13 @@ class SlidingScorer:
         if age.numel() not in (1, self.n_patients):
             raise RuntimeError(f"age must be a scalar or have {self.n_patients} elements")
         em, widx = ctypes.c_int32(0), ctypes.c_int64(-1)
-        out = torch.empty(self.n_patients, dtype=torch.float32, device=self.device)
+        shape = (1 + len(self._heads), self.n_patients) if heads else (self.n_patients,)
+        out = torch.empty(shape, dtype=torch.float32, device=self.device)
+        fn = "b2cnn_slide_push_heads" if heads else "b2cnn_slide_push"
         with torch.cuda.device(self.device):
             st = torch.cuda.current_stream().cuda_stream
-            capi.check(self._lib.b2cnn_slide_push(self._s, samples.data_ptr(), pitch, age.data_ptr(), age.numel(), int(return_prob),
-                                                  out.data_ptr(), ctypes.byref(em), ctypes.byref(widx), st), "b2cnn_slide_push")
+            capi.check(getattr(self._lib, fn)(self._s, samples.data_ptr(), pitch, age.data_ptr(), age.numel(), int(return_prob),
+                                              out.data_ptr(), ctypes.byref(em), ctypes.byref(widx), st), fn)
         if not em.value:
             return None
         self.window_index = int(widx.value)
