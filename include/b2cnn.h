@@ -177,13 +177,16 @@ int b2cnn_prep_windows(const int16_t *raw, int64_t n_samples, int32_t n_sig, con
  * completed is written for ONE b2cnn_forward call.  Pushing a record trigger by trigger reproduces
  * b2cnn_prep_windows on the whole record bit-for-bit (tests/test_stream.py).
  *   n_sig        signals per sample frame (columns of the pushed arrays)
- *   fs           sampling rate shared by the ring's patients (1/60 Hz for MIMIC numerics)
+ *   fs           sampling rate shared by the ring's patients (1/60 Hz for MIMIC numerics), at least 1 / stride_s
  *   new_samples  DEVICE pointer [n_patients][n_new][n_sig]: B2CNN_SAMPLES_ADC16 = int16 ADC units as in a WFDB
  *                format-16 file (-32768 = missing; gain / baseline from b2cnn_ring_set_signals), or
  *                B2CNN_SAMPLES_F64 = physical values as fp64 (NaN = missing) -- what bin/sendStream.py:59-64 publishes
  *   emitted      host int: 1 when x_out was written (from the 10th trigger on), 0 while the first window fills
- * One push may carry at most stride_s seconds of samples.  The ring owns its device buffers; b2cnn_ring_push allocates
- * nothing and is asynchronous on `stream`. */
+ * One push may carry at most stride_s seconds of samples (stride_s / grid_s grid points) and emits at most one window:
+ * a push after which the window following the one it emits would also be complete is refused with B2CNN_EINVAL and
+ * leaves the ring unchanged.  Pushes cut at cumulative stride boundaries (push n carries the samples with time
+ * < n * stride_s) never are.  The ring owns its device buffers; b2cnn_ring_push allocates nothing and is asynchronous
+ * on `stream`. */
 enum { B2CNN_SAMPLES_ADC16 = 0, B2CNN_SAMPLES_F64 = 1,
        B2CNN_SAMPLES_GRID = 2 /* fp64 5-second grid points [n_patients][n_new][n_sig] as bin/processStream.py:126-131 publishes
                                  them on `call-stream` (already smoothed and filled, 12 per trigger): appended as they are */ };
@@ -367,8 +370,9 @@ int b2cnn_slide_push_heads(b2cnn_slide *slide, const void *new_samples, int64_t 
  * b2cnn_decode_array_messages: value = "[v0,v1,...]" (bin/processStream.py:128, read back at bin/predictStream.py:241):
  *   vals_out[t][0 .. max_vals) (NaN-padded), counts_out[t] = number of values (-1: malformed).
  * Numbers are converted with correct rounding (== json.loads / float() / Double.parseDouble) for up to 19 significant
- * digits and |decimal exponent| <= 27; NaN / Infinity / null are accepted; anything else counts in *n_bad (device int)
- * and yields NaN.  b2cnn_parse_decimal is the same parser compiled for the host (tests; status 0 ok, 1 malformed,
+ * digits and |decimal exponent| <= 27; NaN / Infinity / null (quoted or not) are accepted; JSON whitespace may separate
+ * the tokens, nothing may follow the closing bracket, and the signal index must fit an int32; anything else counts in
+ * *n_bad (device int) and yields NaN (idx_out -1).  b2cnn_parse_decimal is the same parser compiled for the host (tests; status 0 ok, 1 malformed,
  * 2 out of range). */
 int b2cnn_decode_sample_messages(const void *bytes, const int64_t *offsets, int64_t n_msgs, int32_t *idx_out, double *val_out,
                                  const int64_t *row_of_msg, double *frame, int64_t frame_rows, int32_t n_sig, int32_t *n_bad,

@@ -39,12 +39,14 @@ def sample_period_ns(fs: float) -> int:
     return int(round(1e9 / fs))
 
 
-def smooth_to_grid(samples: np.ndarray, fs: float, fill: bool = True) -> np.ndarray:
+def smooth_to_grid(samples: np.ndarray, fs: float, fill: bool = True, n_grid: int | None = None) -> np.ndarray:
     """One signal: value at grid label tau (multiples of 5 s) = mean of the valid samples with time in
-    [tau - 175, tau + 5); NaN samples are skipped (Spark avg ignores nulls); then ffill, bfill, 0-fill."""
+    [tau - 175, tau + 5); NaN samples are skipped (Spark avg ignores nulls); then ffill, bfill, 0-fill.
+    ``n_grid`` overrides the number of grid points (default: labels up to the last sample's time)."""
     period_ns = sample_period_ns(fs)
     t = np.arange(samples.shape[0], dtype=np.int64) * period_ns       # integer nanoseconds: edges compare exactly
-    n_grid = int(t[-1] // (GRID_S * NS)) + 1
+    if n_grid is None:
+        n_grid = int(t[-1] // (GRID_S * NS)) + 1
     tau = np.arange(n_grid, dtype=np.int64) * (GRID_S * NS)
     lo = np.searchsorted(t, tau - (SMOOTH_S - GRID_S) * NS, side="left")   # first sample with t >= tau - 175
     hi = np.searchsorted(t, tau + GRID_S * NS, side="left")                # first sample with t >= tau + 5
@@ -98,3 +100,48 @@ def assemble_windows(record, sel) -> Tuple[np.ndarray, np.ndarray]:
     if not len(sel):
         return np.zeros((0, N_CHANNELS, WINDOW_POINTS)), np.zeros((0,))
     return windows_from_grids(grids_of_record(record, sel))
+
+
+def ring_schedule(fs: float, sizes, grid_points: bool = False):
+    """The bookkeeping of a per-patient ring (b2cnn_ring_push) restated: one push of sizes[i] samples (grid points with
+    ``grid_points``) finalises grid points 0 .. k_end-1 (k_end = floor(t_next / 5 s), t_next = time of the first sample
+    not yet received) and emits the next window once its last point is final.  A push after which the window after that
+    one would be complete too is refused and changes nothing.  Returns [(k_end, emitted window or -1, refused)]."""
+    period_ns, grid_ns, step = sample_period_ns(fs), GRID_S * NS, STRIDE_S // GRID_S
+    n, k_done, w_next, out = 0, 0, 0, []
+    for s in sizes:
+        k_end = k_done + s if grid_points else (n + s) * period_ns // grid_ns
+        if step * (w_next + 1) + WINDOW_POINTS <= k_end:
+            out.append((k_end, -1, True))
+            continue
+        emit = step * w_next + WINDOW_POINTS <= k_end
+        out.append((k_end, w_next if emit else -1, False))
+        w_next += emit
+        n, k_done = n + (0 if grid_points else s), k_end
+    return out
+
+
+def causal_windows(unfilled: np.ndarray, k_ends) -> np.ndarray:
+    """The windows a stream can emit: window w is cut when grid points 0 .. k_ends[w]-1 are final (its emitting push
+    has finalised them; k_ends[w] >= 12 w + 120).  ``unfilled`` [n_sel][>= max(k_ends)] are the smoothed grid points
+    before any fill (``smooth_to_grid(..., fill=False)``).  Forward fill is causal already; the leading gap is
+    back-filled from the first valid point among the final ones, else 0 -- where the whole-record form back-fills from
+    the future.  Returns x [len(k_ends), 10, 120] float64."""
+    step = STRIDE_S // GRID_S
+    n_sel = unfilled.shape[0]
+    x = np.zeros((len(k_ends), N_CHANNELS, WINDOW_POINTS), dtype=np.float64)
+    for ch in range(n_sel):
+        g = unfilled[ch]
+        idx = np.where(~np.isnan(g), np.arange(g.shape[0]), -1)       # forward fill
+        np.maximum.accumulate(idx, out=idx)
+        ff = np.where(idx >= 0, g[np.maximum(idx, 0)], np.nan)
+        valid = np.nonzero(~np.isnan(g))[0]
+        for w, k_end in enumerate(k_ends):
+            k_end = int(k_end)
+            if k_end < step * w + WINDOW_POINTS or k_end > g.shape[0]:
+                raise ValueError(f"window {w} is not complete at k_end {k_end} / beyond the grid")
+            v = ff[step * w:step * w + WINDOW_POINTS].copy()
+            first = valid[0] if valid.size and valid[0] < k_end else -1
+            v[np.isnan(v)] = g[first] if first >= 0 else 0.0
+            x[w, ch] = v
+    return x

@@ -62,28 +62,38 @@ def test_host_parser_equals_json_loads_on_the_reference_messages_of_p000194():
         assert st == 0 and (math.isnan(got) if math.isnan(want) else _same_bits(got, want)), value
 
 
-def test_host_parser_is_correctly_rounded():
-    """Shortest-repr strings (Python repr, Java Double.toString), 17-digit cases, exact halfway cases, both exponent
-    spellings -- against float(); out-of-range exponents and malformed text are flagged, never mis-parsed."""
+# exact halfway cases, 17 - 19 digits, both exponent spellings, the edges of the supported exponent range
+EDGE_NUMBERS = ["0.30000000000000004", "9007199254740993", "9007199254740992", "4503599627370497.5", "4503599627370496.5",
+                "1e22", "1e23", "8.5e-10", "123456789012345678", "1234567890123456789", "0.1", "1.0E-5", "1e-05", "-0.0",
+                "2.5e+16", "0.000001", "1e27", "1E-27", "00012.50"]
+OUT_OF_RANGE = ["1e28", "1e-300", "5e-324", "1.7976931348623157e308", "12345678901234567891"]
+MALFORMED = ["abc", "1e", "--1", "", "1 ", "1,2", "0x10"]
+# json.dumps writes bare NaN / Infinity, Spark's to_json quotes them (sign inside the quotes); null is a missing value
+NON_FINITE = [("NaN", math.nan), ('"NaN"', math.nan), ("null", math.nan), ("Infinity", math.inf), ("-Infinity", -math.inf),
+              ('"Infinity"', math.inf), ('"-Infinity"', -math.inf)]
+
+
+def _corpus():
+    """Shortest-repr strings (Python repr, Java Double.toString) of 36 000 values from 1e-6 to 1e15, both spellings."""
     rng = random.Random(7)
     vals = [rng.uniform(0, 300) for _ in range(20000)] + [round(rng.uniform(0, 250), 1) for _ in range(5000)]
     vals += [rng.uniform(-1e-6, 1e-6) for _ in range(3000)] + [rng.uniform(-1e15, 1e15) for _ in range(3000)]
     vals += [rng.randint(0, 10 ** 17) / rng.choice([3, 7, 10, 1000]) for _ in range(5000)]
-    for v in vals:
-        for s in (repr(v), R.java_double_to_string(v)):
-            got, st = _parse(s.encode())
-            assert st == 0 and _same_bits(got, float(s)), s
-    for s in ["0.30000000000000004", "9007199254740993", "9007199254740992", "4503599627370497.5", "4503599627370496.5",
-              "1e22", "1e23", "8.5e-10", "123456789012345678", "1234567890123456789", "0.1", "1.0E-5", "1e-05", "-0.0",
-              "2.5e+16", "0.000001", "1e27", "1E-27", "00012.50"]:
+    return [s for v in vals for s in (repr(v), R.java_double_to_string(v))]
+
+
+def test_host_parser_is_correctly_rounded():
+    """Shortest-repr strings (Python repr, Java Double.toString), 17-digit cases, exact halfway cases, both exponent
+    spellings -- against float(); out-of-range exponents and malformed text are flagged, never mis-parsed."""
+    for s in _corpus() + EDGE_NUMBERS:
         got, st = _parse(s.encode())
         assert st == 0 and _same_bits(got, float(s)), s
-    for s, want in [("NaN", math.nan), ('"NaN"', math.nan), ("null", math.nan), ("Infinity", math.inf), ("-Infinity", -math.inf)]:
+    for s, want in NON_FINITE:
         got, st = _parse(s.encode())
         assert st == 0 and (math.isnan(got) if math.isnan(want) else got == want)
-    for s in ["abc", "1e", "--1", "", "1 ", "1,2", "0x10"]:
+    for s in MALFORMED:
         assert _parse(s.encode())[1] == 1, s
-    for s in ["1e28", "1e-300", "5e-324", "1.7976931348623157e308", "12345678901234567891"]:
+    for s in OUT_OF_RANGE:
         got, st = _parse(s.encode())
         assert st == 2 and math.isnan(got), s            # outside the supported range: flagged
 
@@ -212,3 +222,114 @@ def test_binary_frames_feed_the_ring_without_decoding():
         if r is not None:
             out.append(r[0].clone())
     assert len(out) == 191 and torch.equal(torch.stack([o[1] for o in out]), whole[:191])
+
+
+def _decode_pairs_raw(msgs, rows=None, frame=None, frame_rows=0, n_sig=0):
+    """b2cnn_decode_sample_messages with idx_out / val_out (and optionally a caller-owned frame): (idx, val, n_bad)."""
+    lib = capi.load_library()
+    b, offs, n = S._message_buffer(msgs, "cuda:0")
+    idx = torch.full((n,), -7, dtype=torch.int32, device="cuda:0")
+    val = torch.empty((n,), dtype=torch.float64, device="cuda:0")
+    bad = torch.zeros(1, dtype=torch.int32, device="cuda:0")
+    rows_t = None if rows is None else torch.as_tensor(np.asarray(rows, dtype=np.int64)).to("cuda:0")
+    capi.check(lib.b2cnn_decode_sample_messages(b.data_ptr(), offs.data_ptr(), n, idx.data_ptr(), val.data_ptr(),
+                                                None if rows_t is None else rows_t.data_ptr(), frame, frame_rows, n_sig,
+                                                bad.data_ptr(), torch.cuda.current_stream().cuda_stream), "decode")
+    torch.cuda.synchronize()
+    return idx.cpu().numpy(), val.cpu().numpy(), int(bad.item())
+
+
+def _float(s: str) -> float:
+    """float() of a message value; Spark's quoted non-finite doubles unquoted, null = missing."""
+    return math.nan if s == "null" else float(s.strip('"'))
+
+
+def _same_values(got: np.ndarray, want: np.ndarray) -> bool:
+    nan = np.isnan(want)
+    return bool(np.array_equal(np.isnan(got), nan) and np.array_equal(got[~nan].view(np.int64), want[~nan].view(np.int64)))
+
+
+@pytest.mark.gpu
+def test_gpu_decoders_equal_float_on_the_whole_parser_corpus():
+    """The nvcc build of the parser (128-bit division, __clzll, device ldexp) on every string the host build is checked
+    with: each of 72 000 shortest-repr strings plus the edge, non-finite, out-of-range and malformed cases, once through
+    each device kernel in one call.  Values match float() bit for bit; a message is flagged exactly when the host build
+    flags the string, and the flagged count is n_bad."""
+    strings = _corpus() + EDGE_NUMBERS + [s for s, _ in NON_FINITE] + OUT_OF_RANGE + ["abc", "1e", "--1", "0x10", "+-1", ".", "e5"]
+    host = [_parse(s.encode()) for s in strings]
+    ok = np.array([st == 0 for _, st in host])
+    assert ok.sum() == len(strings) - len(OUT_OF_RANGE) - 7
+    want = np.array([_float(s) if o else math.nan for s, o in zip(strings, ok)])
+    assert _same_values(np.array([v for v, _ in host])[ok], want[ok])
+    # [i, val] messages, the index cycling through 0 .. 9
+    idx, val, bad = _decode_pairs_raw([f"[{t % 10}, {s}]".encode() for t, s in enumerate(strings)])
+    assert bad == (~ok).sum()
+    assert np.array_equal(idx, np.where(ok, np.arange(len(strings)) % 10, -1))
+    assert _same_values(val, want)
+    # one-element arrays
+    vals, counts, bad = S.decode_array_messages([f"[{s}]".encode() for s in strings], 1, "cuda:0")
+    assert bad == (~ok).sum()
+    assert np.array_equal(counts.cpu().numpy(), np.where(ok, 1, -1))
+    assert _same_values(vals.cpu().numpy()[:, 0], want)
+    # and call-stream messages of twelve Double.toString values each (bin/processStream.py:128)
+    js = [R.java_double_to_string(float(v)) for v in want[ok][:12 * 3000]]
+    msgs = ["[" + ",".join(js[12 * m:12 * m + 12]) + "]" for m in range(len(js) // 12)]
+    vals, counts, bad = S.decode_array_messages([m.encode() for m in msgs], 12, "cuda:0")
+    assert bad == 0 and (counts.cpu().numpy() == 12).all()
+    assert _same_values(vals.cpu().numpy().ravel(), np.array([_float(s) for s in js]))
+
+
+@pytest.mark.gpu
+def test_gpu_pair_decoder_flags_indices_that_do_not_fit():
+    """The signal index is read in full: one that an int32 cannot hold is malformed (counted, idx -1, NaN), never
+    truncated to its leading digits."""
+    msgs = [b"[1234567, 5.0]", b"[2147483647, 1.0]", b"[2147483648, 1.0]", b"[99999999999999999999, 2.0]", b"[100000, 3.0]",
+            b"[0000000000003, 4.0]"]
+    idx, val, bad = _decode_pairs_raw(msgs)
+    assert list(idx) == [1234567, 2147483647, -1, -1, 100000, 3] and bad == 2
+    assert list(val[[0, 1, 4, 5]]) == [5.0, 1.0, 3.0, 4.0] and np.isnan(val[[2, 3]]).all()
+
+
+@pytest.mark.gpu
+def test_gpu_decoders_on_empty_messages_whitespace_and_truncation():
+    """What json.loads accepts -- whitespace between tokens, quoted non-finite values -- decodes; an empty message, a
+    missing value or bracket, or anything after the closing bracket is malformed; arrays longer than max_vals keep
+    their first max_vals values, report the full count and are counted in n_bad."""
+    nan, inf = math.nan, math.inf
+    pairs = [(b"", None), (b"[]", None), (b"[0]", None), (b"[0,]", None), (b"[, 1.0]", None), (b"[0, 1.0", None),
+             (b" [ 1 , 2.5 ] ", (1, 2.5)), (b"\t[2,\t-3.25\t]\n", (2, -3.25)), (b"[3,\r\n1e2]", (3, 100.0)),
+             (b'[4, "NaN"]', (4, nan)), (b'[5, "Infinity"]', (5, inf)), (b'[6, "-Infinity"]', (6, -inf)), (b"[7, null]", (7, nan)),
+             (b"[8, -Infinity]", (8, -inf)), (b"[0, 1.0] x", None), (b"[0, 1.0]]", None), (b"[-1, 1.0]", None), (b"[1.5, 2.0]", None)]
+    idx, val, bad = _decode_pairs_raw([m for m, _ in pairs])
+    assert bad == sum(w is None for _, w in pairs)
+    for t, (m, w) in enumerate(pairs):
+        wi, wv = w if w is not None else (-1, nan)
+        assert idx[t] == wi and _same_values(val[t:t + 1], np.array([wv])), m
+    arrays = [(b"", -1, []), (b"[]", 0, []), (b" [ ] ", 0, []), (b"[\t1.0 ,\n2.0\r]", 2, [1.0, 2.0]),
+              (b'["NaN","Infinity","-Infinity"]', 3, [nan, inf, -inf]), (b"[1.0,2.0,3.0,4.0,5.0]", 5, [1.0, 2.0, 3.0]),
+              (b"[1.0,,2.0]", -1, []), (b"[1.0] 7", -1, []), (b"[1.0", -1, []), (b"1.0", -1, []), (b"[1.0,2.0,3.0]", 3, [1.0, 2.0, 3.0]),
+              (b"[1e28]", -1, []), (b"[0.5, null]", 2, [0.5, nan])]
+    vals, counts, bad = S.decode_array_messages([m for m, _, _ in arrays], 3, "cuda:0")
+    vals, counts = vals.cpu().numpy(), counts.cpu().numpy()
+    assert bad == sum(c < 0 or c > 3 for _, c, _ in arrays)
+    for t, (m, c, v) in enumerate(arrays):
+        assert counts[t] == c, m
+        assert _same_values(vals[t], np.array(v + [nan] * (3 - len(v)))), m
+    vals, counts, bad = S.decode_array_messages([], 3, "cuda:0")
+    assert vals.shape == (0, 3) and bad == 0
+
+
+@pytest.mark.gpu
+def test_gpu_frame_scatter_stays_inside_the_frame():
+    """The frame is rows 1 .. 3 of a larger buffer: messages with rows or signal indices outside it write nothing, the
+    frame is NaN where no message landed, and the rows around it keep their contents."""
+    buf = torch.full((6, 4), 7.0, dtype=torch.float64, device="cuda:0")
+    msgs = [(b"[0, 1.0]", 0), (b"[3, 2.0]", 2), (b"[4, 3.0]", 0), (b"[0, 4.0]", 3), (b"[0, 5.0]", -1), (b"[1, 6.0]", 1),
+            (b"[99999999999, 7.0]", 1), (b"[2, oops]", 1), (b"[2147483647, 8.0]", 0), (b"[1, 9.0]", 1 << 40), (b"[2, -0.0]", 0)]
+    idx, val, bad = _decode_pairs_raw([m for m, _ in msgs], rows=[r for _, r in msgs], frame=buf[1].data_ptr(), frame_rows=3, n_sig=4)
+    assert bad == 2 and list(idx) == [0, 3, 4, 0, 0, 1, -1, -1, 2147483647, 1, 2]
+    want = np.full((3, 4), np.nan)
+    want[0, 0], want[2, 3], want[1, 1], want[0, 2] = 1.0, 2.0, 6.0, -0.0
+    got = buf.cpu().numpy()
+    assert _same_values(got[1:4].ravel(), want.ravel())
+    assert (got[0] == 7.0).all() and (got[4:] == 7.0).all()

@@ -334,10 +334,12 @@ int ring_create(const b2cnn_prep_config *cfg, int n_patients, int n_sig, double 
     if (!prep_dims(1, n_sig, 0, fs, cfg, &d, err)) return B2CNN_EINVAL;
     if (n_patients < 1 || n_patients > (1 << 20)) { *err = "n_patients out of range"; return B2CNN_EINVAL; }
     if (cfg->window_points + kRingMaxNewPts > kRingGrid) { *err = "window_points too large for the grid ring"; return B2CNN_EINVAL; }
+    const int64_t stride_ns = (int64_t)cfg->stride_s * 1000000000ll;
+    // a single sample must not complete two windows, or no push schedule could keep to one window per push
+    if (d.period_ns > stride_ns) { *err = "sampling period longer than the stride"; return B2CNN_EINVAL; }
     Ring *r = new Ring();
     r->cfg = *cfg; r->n_patients = n_patients; r->n_sig = n_sig; r->device = device;
     r->period_ns = d.period_ns; r->grid_ns = d.grid_ns; r->smooth_ns = d.smooth_ns;
-    const int64_t stride_ns = (int64_t)cfg->stride_s * 1000000000ll;
     const int64_t max_new = stride_ns / d.period_ns + 2;
     r->R = (d.smooth_ns + 2 * d.grid_ns) / d.period_ns + max_new + 4;
     const int64_t P = n_patients;
@@ -408,13 +410,18 @@ int ring_push(Ring *r, const void *new_samples, int sample_kind, int64_t n_new, 
     const int64_t t_next = N1 * r->period_ns;                        // time of the first sample NOT yet received
     const int64_t k_end = is_grid ? r->k_done + n_new : t_next / r->grid_ns;   // grid points 0 .. k_end-1 are final
     const int64_t n_pts = k_end - r->k_done;
-    const int step_pts = r->cfg.stride_s / r->cfg.grid_s;
-    if (n_pts > kRingMaxNewPts || (is_grid && n_new > step_pts) ||
+    const int step = r->cfg.stride_s / r->cfg.grid_s;
+    if (n_pts > kRingMaxNewPts || (is_grid && n_new > step) ||
         (!is_grid && n_new * r->period_ns > (int64_t)r->cfg.stride_s * 1000000000ll + r->period_ns)) {
         *err = "one push may carry at most stride_s seconds of samples / grid points"; return B2CNN_EINVAL;
     }
-    const int step = r->cfg.stride_s / r->cfg.grid_s;
+    // One push emits at most one window.  A push that would also complete the window after the one it emits would leave
+    // a backlog, and a backlog that outgrows the grid ring is read back from overwritten slots: refuse it, state unchanged.
     const int64_t w_last_k = r->w_next * step + r->cfg.window_points - 1;
+    if (w_last_k + step <= k_end - 1) {
+        *err = "push would complete two windows: one push may finalise at most one window (cut pushes at stride boundaries)";
+        return B2CNN_EINVAL;
+    }
     const bool emit = w_last_k <= k_end - 1;
     RingPush a;
     a.samples = r->d_samples; a.grid = r->d_grid; a.last = r->d_last; a.first = r->d_first;

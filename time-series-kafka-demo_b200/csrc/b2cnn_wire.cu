@@ -73,12 +73,17 @@ __host__ __device__ double scale_decimal(unsigned long long m, int e10, bool neg
     return neg ? -v : v;
 }
 
+// the whitespace json.loads skips between tokens
+__host__ __device__ inline bool json_ws(uint8_t c) { return c == ' ' || c == '\t' || c == '\n' || c == '\r'; }
+
 // parses a JSON number / NaN / Infinity / null starting at s[i]; advances i.  status: 0 ok, 1 malformed, 2 out of range
 __host__ __device__ double parse_number(const uint8_t *s, int64_t &i, int64_t end, int *status) {
-    while (i < end && (s[i] == ' ' || s[i] == '\t')) ++i;
+    while (i < end && json_ws(s[i])) ++i;
     bool neg = false;
+    const bool quoted = i < end && s[i] == '"';              // Spark quotes non-finite doubles: "NaN", "Infinity", "-Infinity"
+    if (quoted) ++i;
     if (i < end && (s[i] == '-' || s[i] == '+')) { neg = s[i] == '-'; ++i; }
-    if (i < end && s[i] == '"') ++i;                          // Spark quotes non-finite doubles: "NaN", "Infinity"
+    if (!quoted && i < end && s[i] == '"') ++i;
     if (i + 3 <= end && s[i] == 'N' && s[i + 1] == 'a' && s[i + 2] == 'N') { i += 3; if (i < end && s[i] == '"') ++i; return nan(""); }
     if (i + 4 <= end && s[i] == 'n' && s[i + 1] == 'u' && s[i + 2] == 'l' && s[i + 3] == 'l') { i += 4; return nan(""); }
     if (i + 8 <= end && s[i] == 'I' && s[i + 1] == 'n' && s[i + 2] == 'f' && s[i + 3] == 'i' && s[i + 4] == 'n' && s[i + 5] == 'i' &&
@@ -128,20 +133,28 @@ __global__ void decode_pairs_kernel(const uint8_t *__restrict__ bytes, const int
     const int64_t end = offsets[t + 1];
     int status = 0, idx = -1;
     double v = nan("");
-    while (i < end && (bytes[i] == ' ' || bytes[i] == '\t')) ++i;
+    while (i < end && json_ws(bytes[i])) ++i;
     if (i < end && bytes[i] == '[') {
         ++i;
-        while (i < end && bytes[i] == ' ') ++i;
-        int k = 0; bool any = false;
-        for (; i < end && bytes[i] >= '0' && bytes[i] <= '9'; ++i) { any = true; if (k < 100000) k = k * 10 + (bytes[i] - '0'); }
-        while (i < end && bytes[i] == ' ') ++i;
-        if (any && i < end && bytes[i] == ',') {
+        while (i < end && json_ws(bytes[i])) ++i;
+        long long k = 0; bool any = false, big = false;      // an index idx_out cannot hold is malformed, not truncated
+        for (; i < end && bytes[i] >= '0' && bytes[i] <= '9'; ++i) {
+            any = true;
+            k = k * 10 + (bytes[i] - '0');
+            if (k > 0x7fffffffll) { big = true; k = 0x7fffffffll; }
+        }
+        while (i < end && json_ws(bytes[i])) ++i;
+        if (big) status = 1;
+        else if (any && i < end && bytes[i] == ',') {
             ++i;
-            idx = k;
+            idx = (int)k;
             v = parse_number(bytes, i, end, &status);
-            while (i < end && bytes[i] == ' ') ++i;
+            while (i < end && json_ws(bytes[i])) ++i;
             if (!(i < end && bytes[i] == ']')) status = status ? status : 1;
+            else ++i;
         } else status = 1;
+        while (i < end && json_ws(bytes[i])) ++i;
+        if (i < end) status = status ? status : 1;            // nothing but whitespace after the closing bracket
     } else status = 1;
     if (status) { idx = -1; v = nan(""); atomicAdd(n_bad, 1); }
     if (idx_out) idx_out[t] = idx;
@@ -162,10 +175,10 @@ __global__ void decode_arrays_kernel(const uint8_t *__restrict__ bytes, const in
     const int64_t end = offsets[t + 1];
     int status = 0, n = 0;
     double *out = vals_out + t * max_vals;
-    while (i < end && (bytes[i] == ' ' || bytes[i] == '\t')) ++i;
+    while (i < end && json_ws(bytes[i])) ++i;
     if (i < end && bytes[i] == '[') {
         ++i;
-        while (i < end && bytes[i] == ' ') ++i;
+        while (i < end && json_ws(bytes[i])) ++i;
         if (i < end && bytes[i] == ']') { ++i; }
         else {
             while (true) {
@@ -173,12 +186,14 @@ __global__ void decode_arrays_kernel(const uint8_t *__restrict__ bytes, const in
                 if (status) break;
                 if (n < max_vals) out[n] = v;
                 ++n;
-                while (i < end && bytes[i] == ' ') ++i;
+                while (i < end && json_ws(bytes[i])) ++i;
                 if (i < end && bytes[i] == ',') { ++i; continue; }
                 if (i < end && bytes[i] == ']') { ++i; break; }
                 status = 1; break;
             }
         }
+        while (i < end && json_ws(bytes[i])) ++i;
+        if (!status && i < end) status = 1;                    // nothing but whitespace after the closing bracket
     } else status = 1;
     if (status || n > max_vals) { atomicAdd(n_bad, 1); n = status ? -1 : n; }
     for (int k = n < 0 ? 0 : (n < max_vals ? n : max_vals); k < max_vals; ++k) out[k] = nan("");
@@ -208,7 +223,10 @@ int wire_decode_pairs(const uint8_t *bytes, const int64_t *offsets, int64_t n_ms
 
 int wire_decode_arrays(const uint8_t *bytes, const int64_t *offsets, int64_t n_msgs, int max_vals, double *vals_out, int *counts_out,
                        int *n_bad, cudaStream_t st, const char **err) {
-    if (!bytes || !offsets || n_msgs < 0 || max_vals < 1 || !vals_out || !counts_out || !n_bad) { *err = "null pointer / bad shape"; return B2CNN_EINVAL; }
+    // a trigger without messages has nothing to write: its (empty) output tensors may have null data pointers
+    if (!bytes || !offsets || n_msgs < 0 || max_vals < 1 || (n_msgs > 0 && (!vals_out || !counts_out)) || !n_bad) {
+        *err = "null pointer / bad shape"; return B2CNN_EINVAL;
+    }
     cudaError_t e = cudaMemsetAsync(n_bad, 0, sizeof(int), st);
     if (e == cudaSuccess && n_msgs > 0)
         decode_arrays_kernel<<<(unsigned)((n_msgs + 127) / 128), 128, 0, st>>>(bytes, offsets, n_msgs, max_vals, vals_out, counts_out, n_bad);

@@ -209,7 +209,10 @@ class PatientRing:
         """``new_samples`` [P, n_new, n_sig]: int16 ADC units (WFDB format 16, -32768 = missing) or float64 physical
         values (NaN = missing), host or device; with ``grid_points`` the rows are 5-second grid points that
         bin/processStream.py already smoothed and filled (the ``call-stream`` payload).  Returns ``(x [P,10,120] on the device, window_index, t0_seconds)`` or
-        ``None`` while the first window is still filling.  The returned tensor is reused by the next push."""
+        ``None`` while the first window is still filling.  The returned tensor is reused by the next push.
+        One push carries at most one stride (60 s) of samples or 12 grid points and emits at most one window: a push
+        after which the next window would be complete too raises RuntimeError and leaves the ring as it was.  Cutting
+        the stream at cumulative stride boundaries (push n = the samples with time < n * 60 s) never does."""
         import ctypes
 
         import torch
@@ -237,12 +240,26 @@ class PatientRing:
         return (self.x, int(widx.value), float(t0.value)) if em.value else None
 
 
+def trigger_cuts(n_samples: int, fs: float) -> List[int]:
+    """Where the triggers of a record sampled at ``fs`` begin and end: trigger n (n = 1, 2, ...) holds the samples with
+    time < n * STRIDE_S on the ring's integer-nanosecond time base (sample i at i * round(1e9 / fs) ns).  Returns
+    ``[0, c_1, c_2, ..., n_samples]``; trigger n = samples ``c_{n-1} .. c_n - 1``."""
+    period_ns, stride_ns = int(round(1e9 / fs)), STRIDE_S * 1_000_000_000
+    cuts, k = [0], 1
+    while cuts[-1] < n_samples:
+        cuts.append(min(n_samples, -(-k * stride_ns // period_ns)))     # number of samples with i * period < k * stride
+        k += 1
+    return cuts
+
+
 def replay_stream(model, records: Sequence[NumericsRecord], subject_ids: Sequence[int], ages=65.0,
                   samples_per_trigger: int = 0) -> List[Tuple[int, float, float]]:
     """The live path's shape (bin/predictStream.py:263: one foreachBatch per 60 s trigger) with the B = 1 per-row loop
     turned into the batched dispatch: all records (same sampling rate and length, one per patient) are fed trigger by
-    trigger into a PatientRing and every trigger costs ONE ``predict()`` over ``[P, 10, 120]``.  Returns the
-    ``predictions`` rows (db/init.sql:24-28) of all patients, trigger-major."""
+    trigger into a PatientRing and every trigger costs ONE ``predict()`` over ``[P, 10, 120]``.  Trigger n carries the
+    samples with time < n * 60 s, so every trigger from the 10th on emits exactly the window that just completed, at
+    any sampling rate; ``samples_per_trigger`` > 0 cuts fixed-size triggers instead (each must keep to one window per
+    push, see ``PatientRing.push``).  Returns the ``predictions`` rows (db/init.sql:24-28) of all patients, trigger-major."""
     P = len(records)
     if P == 0:
         return []
@@ -264,7 +281,7 @@ def _replay_ring(model, ring, records, subject_ids, ages, samples_per_trigger, d
     P, fs, n = len(records), records[0].fs, records[0].raw.shape[0]
     for p, r in enumerate(records):
         ring.set_record_signals(p, r)
-    per = samples_per_trigger or max(1, int(round(STRIDE_S * fs)))
+    cuts = list(range(0, n, samples_per_trigger)) + [n] if samples_per_trigger else trigger_cuts(n, fs)
     raw = torch.from_numpy(np.stack([np.ascontiguousarray(r.raw, dtype=np.int16) for r in records])).to(dev)
     age_t = torch.as_tensor(ages, dtype=torch.float32).reshape(-1)
     if age_t.numel() not in (1, P):
@@ -272,8 +289,8 @@ def _replay_ring(model, ring, records, subject_ids, ages, samples_per_trigger, d
     rows: List[Tuple[int, float, float]] = []
     # the ring rewrites ONE [P, 10, 120] tensor per trigger: shapes, pointers and the output buffer are resolved once
     score = model.call_plan(ring.x, age_t.to(dev), return_prob=True) if hasattr(model, "call_plan") else None
-    for i0 in range(0, n, per):
-        out = ring.push(raw[:, i0:i0 + per])
+    for i0, i1 in zip(cuts[:-1], cuts[1:]):
+        out = ring.push(raw[:, i0:i1])
         if out is None:
             continue
         x, _, t0 = out
