@@ -77,7 +77,9 @@ tc_stream_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant
     constexpr int FOFF = ARCH == 0 ? 3 : 2;           // step j emits features 2j-FOFF, 2j-FOFF+1
     extern __shared__ uint8_t smem_raw[];
     // [2 stages][C][8 KB bf16 | 16 KB fp32] | bands | transpose | W ring [2][6 KB] | A pieces [3][4 KB] | barriers
-    uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+    // aligned by an offset from smem_raw, not by rounding the generic address as an integer: the compiler then still
+    // knows every pointer below is shared memory and emits 32-bit LDS / STS instead of 64-bit generic LD / ST
+    uint8_t *smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     uint8_t *sA = smem;
     uint8_t *sBm = sA + 2 * C * kABytes;
     float *sT = reinterpret_cast<float *>(sBm + (F32IN ? 0 : C * SPLITS * kTcBBytes));
