@@ -254,7 +254,7 @@ static cudaError_t launch_stream(const CUtensorMap &tm, const TcFusedParams &p, 
     const size_t smem = hp_smem_bytes(C, SPLITS, F32IN, OUT);
     cudaError_t e = cudaFuncSetAttribute(tc_stream_kernel<C, SPLITS, ARCH, F32IN, OUT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
-    tc_stream_kernel<C, SPLITS, ARCH, F32IN, OUT><<<grid, kHpThreads, smem, st>>>(tm, p);
+    tc_stream_kernel<C, SPLITS, ARCH, F32IN, OUT><<<grid, hp_threads(F32IN), smem, st>>>(tm, p);
     return cudaGetLastError();
 }
 

@@ -5,13 +5,14 @@
 //      gates[w, g] += sum_p  f[w, p] * W_ih_l0[g, p]           (bin/models.py:30, layer 0)
 //
 // conv1 of bf16 windows is the banded-Toeplitz GEMM described in b2cnn_tc.cu, on wgmma: per 8-position block,
-// two m64n32k16 row halves x C channels x SPLITS weight pieces, A = the TMA tile (32-sample boxes, SWIZZLE_64B,
-// the block's 16-sample slice selected by a 16n-byte descriptor offset, 3 blocks per tile), B = the band-matrix
-// piece, D in registers.  The accumulator fragment (two windows x 16 values per thread) is turned into thread ==
-// window through an 18 KB shared-memory transpose; the next block's MMAs run while the epilogue of this one
-// computes.  About 100 KB of shared memory and at most 168 registers per thread let two CTAs share an SM, so each
-// SM sub-partition has two consumer warps to interleave.  fp32 windows (F32IN) evaluate conv1 in exact fp32 FMAs
-// straight from the tile instead (the same 32-sample boxes as 128-byte SWIZZLE_128B rows; one CTA per SM).
+// two m64n32k16 row halves x C channels x SPLITS weight pieces, A in registers (one ldmatrix.x4 per row half and
+// channel of the block's 16-sample slice of the TMA tile: 32-sample boxes, SWIZZLE_64B, 3 blocks per tile, shared by
+// the SPLITS pieces), B = the band-matrix piece, D in registers.  The accumulator fragment (two windows x 16 values
+// per thread) is turned into thread == window through an 18 KB shared-memory transpose; the next block's MMAs run
+// while the epilogue of this one computes.  About 100 KB of shared memory and 128 registers per thread at launch let
+// two CTAs share an SM, so each SM sub-partition has two consumer warps to interleave; setmaxnreg then gives the
+// consumer warpgroup 216 of them and the producer warpgroup 40.  fp32 windows (F32IN) evaluate conv1 in exact fp32
+// FMAs straight from the tile instead (the same 32-sample boxes as 128-byte SWIZZLE_128B rows; one CTA per SM).
 //
 // Epilogue, thread == window: each thread streams through its window's positions in order, so pool1 -> tanh ->
 // conv2 -> pool2 -> tanh are register-local sliding windows; tanh is 1 - 2/(1+2^(2x log2 e)) on MUFU.EX2 +
@@ -24,13 +25,16 @@
 // pairs hh hm mh hl lh mm: fp32-equivalent products) against the packed W_ih chunk, accumulating the 64 gate
 // pre-activations in registers over the CTA's whole range.  They leave once, as partial[range][window][64].
 //
-// CTA = 192 threads: warps 0-3 the consumer warpgroup, warp 4 the TMA producer of the window tiles, warp 5 the
-// producer of the W_ih chunks (1-D bulk copies).
+// CTA = 256 threads for bf16 windows, 192 for fp32: warps 0-3 the consumer warpgroup, warp 4 the TMA producer of the
+// window tiles, warp 5 the producer of the W_ih chunks (1-D bulk copies), warps 6-7 (bf16) idle.
 #pragma once
 
 namespace b2cnn {
 
-constexpr int kHpThreads = 192;
+// bf16 windows: two full warpgroups, so that setmaxnreg can move registers from the producer warpgroup (warps 4-7,
+// 6 and 7 idle) to the consumer one; fp32 windows: 192 threads
+__host__ __device__ constexpr int hp_threads(bool f32in) { return f32in ? 192 : 256; }
+constexpr int kHpProducerRegs = 40, kHpConsumerRegs = 216;   // 128 x 40 + 128 x 216 = 256 x 128: two CTAs per SM
 constexpr int kHpTStride = 36;                    // floats per window row of the accumulator transpose (conflict-free float4 reads)
 constexpr int kHpTBytes = kTcM * kHpTStride * 4;
 constexpr int kHpPieceBytes = kTcM * 16 * 2;      // one bf16 piece of the projection A operand
@@ -68,7 +72,7 @@ __host__ __device__ constexpr size_t hp_smem_bytes(int C, int SPLITS, bool f32in
 //         16-sample slice (no tap-9 patch), pooling pairs stay inside a block (no carry), and a step emits
 //         features 2j-2, 2j-1 instead of 2j-3, 2j-2.
 template <int C, int SPLITS, int ARCH, bool F32IN, int OUT>
-__global__ void __launch_bounds__(kHpThreads, F32IN ? 1 : 2)
+__global__ void __launch_bounds__(hp_threads(F32IN), F32IN ? 1 : 2)
 tc_stream_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ TcFusedParams p) {
     constexpr int K1 = ARCH == 0 ? 10 : 5;
     constexpr int kBlocks = kTcBlocks;
@@ -102,7 +106,7 @@ tc_stream_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant
     const int T0 = p0 * 4;                            // first conv1 position == first sample
 
     if (!F32IN)
-        for (int i = threadIdx.x; i < C * SPLITS * kTcBBytes / 16; i += kHpThreads)
+        for (int i = threadIdx.x; i < C * SPLITS * kTcBBytes / 16; i += hp_threads(F32IN))
             reinterpret_cast<uint4 *>(sBm)[i] = reinterpret_cast<const uint4 *>(p.bmats)[i];
     if (threadIdx.x == 0) {
         for (int i = 0; i < 2; ++i) {
@@ -116,30 +120,37 @@ tc_stream_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant
     fence_proxy_async();                              // band matrices visible to the tensor core
     __syncthreads();
 
-    if (warp == 4) {
-        // ===================== TMA producer: window tiles =====================
-        if (lane == 0) {
-            for (int i = 0; i < ntiles; ++i) {
-                const int s = i & 1, ph = (i >> 1) & 1;
-                mbar_wait(bar_empty + 8 * s, ph ^ 1);
-                mbar_expect_tx(bar_full + 8 * s, C * kABytes);
+    // bf16 windows: the consumer's conv1 A fragments stay live across the epilogue, so it needs more than the 128
+    // registers per thread of two 256-thread CTAs; the producers need far fewer.  Each setmaxnreg opens its own branch,
+    // so that ptxas allocates each role's code under its own limit.
+    if (warp >= 4) {
+        if constexpr (!F32IN) setmaxnreg_dec<kHpProducerRegs>();
+        if (warp == 4) {
+            // ===================== TMA producer: window tiles =====================
+            if (lane == 0) {
+                for (int i = 0; i < ntiles; ++i) {
+                    const int s = i & 1, ph = (i >> 1) & 1;
+                    mbar_wait(bar_empty + 8 * s, ph ^ 1);
+                    mbar_expect_tx(bar_full + 8 * s, C * kABytes);
 #pragma unroll
-                for (int c = 0; c < C; ++c) tma_load_3d(smem_u32(sA_of(s, c)), &tmap, T0 + kTcAdv * i, c, b0, bar_full + 8 * s);
+                    for (int c = 0; c < C; ++c) tma_load_3d(smem_u32(sA_of(s, c)), &tmap, T0 + kTcAdv * i, c, b0, bar_full + 8 * s);
+                }
             }
-        }
-    } else if (warp == 5) {
-        // ===================== producer of the packed W_ih chunks =====================
-        if (OUT == kOutGates && lane == 0) {
-            const uint8_t *wsrc = p.wpack + (size_t)blockIdx.y * p.chunks_per_cta * kFuWChunkBytes;
-            for (int m = 0; m < nchunks; ++m) {
-                const int u = m & 1;
-                mbar_wait(bar_wempty + 8 * u, ((m >> 1) & 1) ^ 1);
-                mbar_expect_tx(bar_wfull + 8 * u, kFuWChunkBytes);
-                bulk_load_1d(smem_u32(sW + u * kFuWChunkBytes), wsrc + (size_t)m * kFuWChunkBytes, kFuWChunkBytes, bar_wfull + 8 * u);
+        } else if (warp == 5) {
+            // ===================== producer of the packed W_ih chunks =====================
+            if (OUT == kOutGates && lane == 0) {
+                const uint8_t *wsrc = p.wpack + (size_t)blockIdx.y * p.chunks_per_cta * kFuWChunkBytes;
+                for (int m = 0; m < nchunks; ++m) {
+                    const int u = m & 1;
+                    mbar_wait(bar_wempty + 8 * u, ((m >> 1) & 1) ^ 1);
+                    mbar_expect_tx(bar_wfull + 8 * u, kFuWChunkBytes);
+                    bulk_load_1d(smem_u32(sW + u * kFuWChunkBytes), wsrc + (size_t)m * kFuWChunkBytes, kFuWChunkBytes, bar_wfull + 8 * u);
+                }
             }
         }
     } else {
         // ===================== consumer warpgroup: thread == window =====================
+        if constexpr (!F32IN) setmaxnreg_inc<kHpConsumerRegs>();
         const int row = threadIdx.x;
         const int b = b0 + row;
         const bool row_ok = b < p.B;
@@ -163,21 +174,30 @@ tc_stream_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant
         }
         float *fout = p.feats + (int64_t)b * p.sB + (int64_t)p0 * p.sP;
 
-        // descriptors built once: a block's MMAs only add (start address offset) >> 4 to them
-        const uint64_t adesc0 = gdesc_sw64_kmajor(smem_u32(sA));
+        // conv1's A operand from registers: per (row half h, channel c) one ldmatrix.x4 loads this warp's 16 rows of the
+        // block's 16-sample slice (chunks n, n+1 of the tile) and all SPLITS weight pieces multiply that one fragment,
+        // so the tile is read once instead of once per piece.  Lane l gives the address of row (l & 7) + 8 ((l >> 3) & 1)
+        // of chunk n + (l >> 4): matrices (rows 0-7, 8-15) x (chunk n, n+1) = a0..a3 of the m16k16 fragment.  Its
+        // SWIZZLE_64B term (row / 2) % 4 depends on l only.  The fragments stay live until the wait that retires the MMAs.
+        uint32_t afr[2][C][4];
+        const uint32_t a_lane = smem_u32(sA) + (uint32_t)(16 * warp + (lane & 7) + 8 * ((lane >> 3) & 1)) * kARow;
+        const uint32_t a_swz = (lane >> 1) & 3, a_k = lane >> 4;
+        // B descriptor built once: a block's MMAs only add (start address offset) >> 4 to it
         const uint64_t bdesc0 = gdesc_none_kmajor(smem_u32(sBm), 128, 256);
         auto issue_conv1 = [&](int s, int n) {
-            const uint64_t adesc_sn = adesc0 + (uint64_t)((s * C * kABytes + 16 * n) >> 4);
+            const uint32_t a_sn = a_lane + (uint32_t)(s * C * kABytes) + ((((uint32_t)n + a_k) ^ a_swz) << 4);
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+#pragma unroll
+                for (int c = 0; c < C; ++c) ldmatrix_x4(afr[h][c], a_sn + (uint32_t)(c * kABytes + h * 64 * kARow));
             wgmma_fence();
 #pragma unroll
             for (int h = 0; h < 2; ++h)
 #pragma unroll
-                for (int c = 0; c < C; ++c) {
-                    const uint64_t adesc = adesc_sn + (uint64_t)((c * kABytes + h * 64 * kARow) >> 4);
+                for (int c = 0; c < C; ++c)
 #pragma unroll
                     for (int sp = 0; sp < SPLITS; ++sp)
-                        wgmma_m64n32(acc[h], adesc, bdesc0 + (uint64_t)((c * SPLITS + sp) * (kTcBBytes >> 4)), (c | sp) != 0);
-                }
+                        wgmma_m64n32_rs(acc[h], afr[h][c], bdesc0 + (uint64_t)((c * SPLITS + sp) * (kTcBBytes >> 4)), (c | sp) != 0);
             wgmma_commit();
         };
         if (!F32IN) {
@@ -201,6 +221,10 @@ tc_stream_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant
                     }
                 }
                 wgmma_wait<0>();
+#pragma unroll
+                for (int h = 0; h < 2; ++h)
+#pragma unroll
+                    for (int c = 0; c < C; ++c) wgmma_keep(afr[h][c]);
 #pragma unroll
                 for (int h = 0; h < 2; ++h)
 #pragma unroll

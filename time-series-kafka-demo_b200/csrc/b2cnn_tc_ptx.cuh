@@ -45,6 +45,11 @@ __device__ __forceinline__ void bulk_load_1d(uint32_t dst, const void *src, uint
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                  ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
 }
+// register reallocation between warpgroups (every warp of a warpgroup executes the same one)
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 // named barrier of the consumer warpgroup (id 1, 128 threads): barrier 0 stays __syncthreads()
 __device__ __forceinline__ void wg_bar() { asm volatile("bar.sync 1, 128;" ::: "memory"); }
 // generic-proxy shared-memory writes -> visible to the async proxy (wgmma operand reads)
@@ -75,16 +80,13 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float lo_elem, float hi_elem) {
 }
 
 // ------------------------------------------------------------------------------------------
-// wgmma (sm_90a): D[64 x N] (+)= A[64 x 16] * B[N x 16]^T, A and B bf16 K-major in shared memory, D fp32 in registers.
+// wgmma (sm_90a): D[64 x N] (+)= A[64 x 16] * B[N x 16]^T, A and B bf16 K-major in shared memory
+// (m64n32: A in registers), D fp32 in registers.
 // Fragment of D held by thread t of the warpgroup (warp w = t / 32, lane l): element i of the N/2 registers is
 // row 16 w + l / 4 + 8 ((i / 2) % 2), column 8 (i / 4) + 2 (l % 4) + i % 2.
 // ------------------------------------------------------------------------------------------
-// GMMA shared-memory descriptor: start >> 4 | LBO >> 4 << 16 | SBO >> 4 << 32 | layout << 62 (2 = SWIZZLE_64B, 0 = none)
-__device__ __forceinline__ uint64_t gdesc_sw64_kmajor(uint32_t saddr) {
-    // rows 64 B apart, 8-row groups 512 B apart (SBO); LBO unused for swizzled K-major
-    return (uint64_t)((saddr >> 4) & 0x3FFF) | ((uint64_t)1 << 16) | ((uint64_t)(512 >> 4) << 32) | ((uint64_t)2 << 62);
-}
-// no swizzle, K-major core matrices (8 rows x 16 bytes): LBO = K-adjacent core matrices, SBO = M/N-adjacent ones
+// GMMA shared-memory descriptor: start >> 4 | LBO >> 4 << 16 | SBO >> 4 << 32 | layout << 62 (0 = no swizzle).
+// No swizzle, K-major core matrices (8 rows x 16 bytes): LBO = K-adjacent core matrices, SBO = M/N-adjacent ones
 __device__ __forceinline__ uint64_t gdesc_none_kmajor(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
     return (uint64_t)((saddr >> 4) & 0x3FFF) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16) |
            ((uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32);
@@ -94,15 +96,27 @@ __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_grou
 template <int N>
 __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
-// the "+f" operands tie the accumulator registers to every wgmma and to the wait that follows
-__device__ __forceinline__ void wgmma_m64n32(float *d, uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+// the "+f" operands tie the accumulator registers to every wgmma and to the wait that follows.  A in registers:
+// a[0..3] is thread t's m16k16 bf16 fragment of rows 16 w .. 16 w + 15 (the mma.m16n8k16 A layout, as ldmatrix_x4
+// below loads it).  A wgmma reads a[] asynchronously: the registers must not change until the wait that retires it
+// (wgmma_keep ties them to that wait).
+__device__ __forceinline__ void wgmma_m64n32_rs(float *d, const uint32_t *a, uint64_t bdesc, uint32_t accumulate) {
     asm volatile(
-        "{\n .reg .pred p;\n setp.ne.b32 p, %18, 0;\n"
+        "{\n .reg .pred p;\n setp.ne.b32 p, %21, 0;\n"
         " wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
-        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, 0, 0;\n}"
+        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, {%16,%17,%18,%19}, %20, p, 1, 1, 0;\n}"
         : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
           "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-        : "l"(adesc), "l"(bdesc), "r"(accumulate) : "memory");
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate) : "memory");
+}
+// keeps the A fragment registers of in-flight wgmmas alive (and unmodified) up to this point: place after the wait
+__device__ __forceinline__ void wgmma_keep(uint32_t *a) {
+    asm volatile("" : "+r"(a[0]), "+r"(a[1]), "+r"(a[2]), "+r"(a[3]) :: "memory");
+}
+// four 8x8 b16 matrices from shared memory; lanes 8i .. 8i+7 give the row addresses of matrix i, which lands in r[i]
+__device__ __forceinline__ void ldmatrix_x4(uint32_t *r, uint32_t saddr) {
+    asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
+                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(saddr) : "memory");
 }
 // always accumulates: D += A * B
 __device__ __forceinline__ void wgmma_m64n64(float *d, uint64_t adesc, uint64_t bdesc) {
