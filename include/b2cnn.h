@@ -354,9 +354,33 @@ int b2cnn_slide_import(b2cnn_slide *slide, const int32_t *patients, int32_t n, c
  * B2CNN_EINVAL: a NULL argument, n outside [0, B2CNN_SLIDE_MAX_HEADS], a head without weights or on another device.
  * B2CNN_EARCH: a head of another architecture.  B2CNN_ESTATE: a head whose front-end digest is not the scorer's (at
  * set_heads, or at push_heads after a reset that took other conv weights; the message names the head), or a scorer whose
- * handle's weights changed since its last reset. */
+ * handle's weights changed since its last reset.
+ *
+ * Heads with shorter windows (risk over the last 60 s, 300 s and 600 s from one scorer).  The front end is
+ * translation-equivariant with feature stride F (4 on the tensor-core path, pool_s^2 on the generic path), so a window
+ * W_k <= W that ends where the scorer's ends, with (W - W_k) % F == 0, is the same stream features on the same lattice:
+ * its L_k = lstm_input features are the last L_k of the scorer's window, positions d .. L - 1 with d = (W - W_k) / F.
+ *   b2cnn_slide_set_heads_ex  b2cnn_slide_set_heads with flags; flags == 0 is exactly b2cnn_slide_set_heads.  With
+ *                        B2CNN_SLIDE_HEADS_SHORTER_WINDOWS a head may also differ from the scorer's b2cnn_config in window
+ *                        and lstm_input: window <= W, (W - window) % F == 0, lstm_input == L_out(window) and, on the
+ *                        tensor-core path, the packed W_ih chunks of the streaming kernels for its own L_k (any
+ *                        handle b2cnn_create accepted on the tensor-core geometries has them); anything else is
+ *                        B2CNN_EARCH.  Any other flag bit: B2CNN_EINVAL.  The digest check is unchanged (the window
+ *                        is not part of the digest), and every check runs before anything changes.  Memory per head
+ *                        as above with its own L_k and range count: 4 * L_k * 64 of W_ih^T and on the tensor-core path
+ *                        n_ranges_k * chunks_per_cta_k * 6144 of packed chunks and 4 * n_ranges_k * P * 64 of partials.
+ *   b2cnn_slide_push_heads  then writes row i NaN for every patient whose window W_i for that row is incomplete
+ *                        (seen < W_i, or n S < W_i before any lifecycle call; row 0 keeps W), sets *emitted = 1 once any
+ *                        row has a complete window for at least one patient (a push before the scorer's own first
+ *                        window may emit, row 0 all NaN; *window_index keeps n - ceil(W / S) and may be negative), and
+ *                        runs no projection for a row whose window is incomplete for every patient.  Row i equals what a
+ *                        scorer of head i - 1's model at window W_i and the same stride computes from the same pushes.
+ *                        b2cnn_slide_push, features, admit, discharge, export, import and reset do not change, and a
+ *                        scorer whose heads all have window W runs the launches it runs with b2cnn_slide_set_heads. */
 #define B2CNN_SLIDE_MAX_HEADS 8
+#define B2CNN_SLIDE_HEADS_SHORTER_WINDOWS 1
 int b2cnn_slide_set_heads(b2cnn_slide *slide, b2cnn_handle *const *heads, int32_t n, void *stream);
+int b2cnn_slide_set_heads_ex(b2cnn_slide *slide, b2cnn_handle *const *heads, int32_t n, int32_t flags, void *stream);
 int b2cnn_slide_n_heads(const b2cnn_slide *slide);
 int b2cnn_slide_push_heads(b2cnn_slide *slide, const void *new_samples, int64_t pitch, const float *age, int64_t n_age,
                            int apply_sigmoid, float *out, int32_t *emitted, int64_t *window_index, void *stream);

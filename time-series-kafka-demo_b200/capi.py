@@ -32,7 +32,7 @@ SYMBOLS = ("b2cnn_l_out", "b2cnn_weight_count", "b2cnn_create", "b2cnn_destroy",
            "b2cnn_slide_admit_workspace_bytes", "b2cnn_slide_admit", "b2cnn_slide_discharge", "b2cnn_slide_samples_seen",
            "b2cnn_slide_create_path", "b2cnn_slide_path",
            "b2cnn_slide_describe_state", "b2cnn_slide_state_workspace_bytes", "b2cnn_slide_export", "b2cnn_slide_import",
-           "b2cnn_slide_set_heads", "b2cnn_slide_n_heads", "b2cnn_slide_push_heads",
+           "b2cnn_slide_set_heads", "b2cnn_slide_set_heads_ex", "b2cnn_slide_n_heads", "b2cnn_slide_push_heads",
            "b2cnn_decode_sample_messages", "b2cnn_decode_array_messages", "b2cnn_parse_decimal", "b2cnn_frame_check")
 
 
@@ -65,6 +65,7 @@ class SlideStateHeader(ctypes.Structure):
 
 SLIDE_STATE_MAGIC, SLIDE_STATE_VERSION = 0x53533242, 1
 SLIDE_MAX_HEADS = 8                  # B2CNN_SLIDE_MAX_HEADS
+SLIDE_HEADS_SHORTER_WINDOWS = 1      # B2CNN_SLIDE_HEADS_SHORTER_WINDOWS
 
 
 class Adam(ctypes.Structure):
@@ -152,6 +153,7 @@ def load_library() -> ctypes.CDLL:
     lib.b2cnn_slide_import.argtypes = [c_vp, c_vp, c_i32, hdrp, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp]
     lib.b2cnn_slide_import.restype = c_int
     lib.b2cnn_slide_set_heads.argtypes = [c_vp, c_vp, c_i32, c_vp]; lib.b2cnn_slide_set_heads.restype = c_int
+    lib.b2cnn_slide_set_heads_ex.argtypes = [c_vp, c_vp, c_i32, c_i32, c_vp]; lib.b2cnn_slide_set_heads_ex.restype = c_int
     lib.b2cnn_slide_n_heads.argtypes = [c_vp]; lib.b2cnn_slide_n_heads.restype = c_int
     lib.b2cnn_slide_push_heads.argtypes = lib.b2cnn_slide_push.argtypes; lib.b2cnn_slide_push_heads.restype = c_int
     lib.b2cnn_decode_sample_messages.argtypes = [c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_i64, c_i32, c_vp, c_vp]

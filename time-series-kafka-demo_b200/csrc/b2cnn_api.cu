@@ -685,13 +685,18 @@ extern "C" int b2cnn_slide_push_heads(b2cnn_slide *o, const void *new_samples, i
                           stream);
 }
 extern "C" int b2cnn_slide_n_heads(const b2cnn_slide *o) { return o ? slide_n_heads(o->s) : -1; }
-extern "C" int b2cnn_slide_set_heads(b2cnn_slide *o, b2cnn_handle *const *heads, int32_t n, void *stream) {
-    const char *fn = "b2cnn_slide_set_heads: ";
+static int slide_set_heads_api(const char *fn, b2cnn_slide *o, b2cnn_handle *const *heads, int32_t n, int32_t flags, void *stream) {
     if (!o || (n > 0 && !heads)) return fail(B2CNN_EINVAL, std::string(fn) + "null argument");
+    if (flags & ~B2CNN_SLIDE_HEADS_SHORTER_WINDOWS) return fail(B2CNN_EINVAL, std::string(fn) + "unknown flag bits");
     if (n < 0 || n > B2CNN_SLIDE_MAX_HEADS)
         return fail(B2CNN_EINVAL, std::string(fn) + "n must be in [0, " + std::to_string(B2CNN_SLIDE_MAX_HEADS) + "]");
     const b2cnn_handle *h = o->h;
     const b2cnn_config &c = h->cfg;
+    const bool shorter = flags & B2CNN_SLIDE_HEADS_SHORTER_WINDOWS;
+    b2cnn_slide_state_header mine;
+    slide_describe_state(o->s, h->cw, &mine);
+    const int F = mine.feature_stride;
+    const int R = c.pool_s * (c.pool_k + c.k2 - 2) + c.pool_k + c.k1 - 1;     // the receptive field of one feature
     std::vector<SlideHeadSource> src((size_t)n);
     for (int i = 0; i < n; ++i) {
         const b2cnn_handle *x = heads[i];
@@ -701,13 +706,21 @@ extern "C" int b2cnn_slide_set_heads(b2cnn_slide *o, b2cnn_handle *const *heads,
         if (x->device != h->device) return fail(B2CNN_EINVAL, fn + which + "on another device than the scorer");
         const b2cnn_config &e = x->cfg;
         if (e.in_channels != c.in_channels || e.k1 != c.k1 || e.c_mid != c.c_mid || e.k2 != c.k2 || e.pool_k != c.pool_k ||
-            e.pool_s != c.pool_s || e.hidden != c.hidden || e.layers != c.layers || e.window != c.window ||
-            e.lstm_input != c.lstm_input || e.act != c.act || e.flags != c.flags)
-            return fail(B2CNN_EARCH, fn + which + "another architecture than the scorer's model (only age_coef may differ)");
-        if (slide_path(o->s) == B2CNN_PATH_TENSORCORE && (!x->tc.fused || x->tc.n_ranges != h->tc.n_ranges ||
-                                                          x->tc.chunks_per_cta != h->tc.chunks_per_cta))
-            return fail(B2CNN_EARCH, fn + which + "no packed W_ih chunks of the scorer's layout");
-        src[i] = SlideHeadSource{x->hw, &x->tc, x->d.age_coef, weights_digest(o->s, x->cw)};
+            e.pool_s != c.pool_s || e.hidden != c.hidden || e.layers != c.layers || e.act != c.act || e.flags != c.flags ||
+            (!shorter && (e.window != c.window || e.lstm_input != c.lstm_input)))
+            return fail(B2CNN_EARCH, fn + which + (shorter ? "another architecture than the scorer's model (only window, lstm_input and age_coef may differ)"
+                                                           : "another architecture than the scorer's model (only age_coef may differ)"));
+        if (e.window > c.window) return fail(B2CNN_EARCH, fn + which + "a longer window than the scorer's");
+        if ((c.window - e.window) % F != 0)
+            return fail(B2CNN_EARCH, fn + which + "the scorer's window minus the head's is not a multiple of the feature stride " +
+                                         std::to_string(F) + " (another feature lattice)");
+        if (e.window < R || e.lstm_input != (e.window - R) / F + 1)
+            return fail(B2CNN_EARCH, fn + which + "lstm_input is not the feature count of the head's window");
+        if (slide_path(o->s) == B2CNN_PATH_TENSORCORE &&
+            (!x->tc.fused || (e.window == c.window && (x->tc.n_ranges != h->tc.n_ranges || x->tc.chunks_per_cta != h->tc.chunks_per_cta))))
+            return fail(B2CNN_EARCH, fn + which + (e.window == c.window ? "no packed W_ih chunks of the scorer's layout"
+                                                                        : "no packed W_ih chunks of the streaming kernels for its window"));
+        src[i] = SlideHeadSource{x->hw, &x->tc, x->d.age_coef, weights_digest(o->s, x->cw), e.window, e.lstm_input};
     }
     if (o->gen != h->weight_gen)
         return fail(B2CNN_ESTATE, std::string(fn) + "the scorer's handle's weights changed since its last reset (call reset first)");
@@ -718,6 +731,12 @@ extern "C" int b2cnn_slide_set_heads(b2cnn_slide *o, b2cnn_handle *const *heads,
     const char *err = "";
     const int rc = slide_set_heads(o->s, src.data(), n, reinterpret_cast<cudaStream_t>(stream), &err);
     return rc == B2CNN_OK ? rc : fail(rc, fn + std::string(err));
+}
+extern "C" int b2cnn_slide_set_heads(b2cnn_slide *o, b2cnn_handle *const *heads, int32_t n, void *stream) {
+    return slide_set_heads_api("b2cnn_slide_set_heads: ", o, heads, n, 0, stream);
+}
+extern "C" int b2cnn_slide_set_heads_ex(b2cnn_slide *o, b2cnn_handle *const *heads, int32_t n, int32_t flags, void *stream) {
+    return slide_set_heads_api("b2cnn_slide_set_heads_ex: ", o, heads, n, flags, stream);
 }
 extern "C" int b2cnn_slide_features(b2cnn_slide *o, float *feats, void *stream) {
     if (!o || !feats) return fail(B2CNN_EINVAL, "b2cnn_slide_features: null argument");

@@ -44,11 +44,11 @@ void launch_transpose_wih(const float *wih0, float *wih0T, int L, cudaStream_t s
 // ---------------------------------------------------------------------------------------
 constexpr int kPM = 64, kPK = 32, kFsStride = 68;
 
-// kRing: F is a sliding scorer's position-major feature ring (sB = 1, sP = its row pitch) whose L slots hold window
-// position k in slot (head + k) mod L; otherwise position k of window b is F[b sB + k sP].  The tiles, the zero padding
+// kRing: F is a sliding scorer's position-major feature ring (sB = 1, sP = its row pitch) whose cap >= L slots hold
+// window position k in slot (head + k) mod cap; otherwise position k of window b is F[b sB + k sP].  The tiles, the zero padding
 // and the summation order are the same either way.
 template <bool kRing>
-__device__ __forceinline__ void proj_body(const float *__restrict__ F, int64_t sB, int64_t sP, int head,
+__device__ __forceinline__ void proj_body(const float *__restrict__ F, int64_t sB, int64_t sP, int head, int cap,
                                           const float *__restrict__ WT, float *__restrict__ part, int B, int L, int k_per_split) {
     __shared__ __align__(16) float Fs[kPK][kFsStride];
     __shared__ __align__(16) float Ws[kPK][kGates];
@@ -74,7 +74,7 @@ __device__ __forceinline__ void proj_body(const float *__restrict__ F, int64_t s
             int slot = k;
             if (kRing) {
                 slot = head + k;
-                if (slot >= L) slot -= L;
+                if (slot >= cap) slot -= cap;
             }
             Fs[kk][m] = (b < B && k < kend) ? __ldg(F + (int64_t)b * sB + (int64_t)slot * sP) : 0.f;
         }
@@ -112,14 +112,15 @@ __device__ __forceinline__ void proj_body(const float *__restrict__ F, int64_t s
 __global__ void __launch_bounds__(256)
 proj_kernel(const float *__restrict__ F, int64_t sB, int64_t sP, const float *__restrict__ WT,
             float *__restrict__ part, int B, int L, int k_per_split) {
-    proj_body<false>(F, sB, sP, 0, WT, part, B, L, k_per_split);
+    proj_body<false>(F, sB, sP, 0, L, WT, part, B, L, k_per_split);
 }
 
-// the sliding scorer's projection over its feature ring (b2cnn_slide.cu, generic path): head in [0, L)
+// the sliding scorer's projection over its feature ring of cap slots (b2cnn_slide.cu, generic path): head in [0, cap),
+// L <= cap window positions
 __global__ void __launch_bounds__(256)
-ring_proj_kernel(const float *__restrict__ ring, int64_t pitch, int head, const float *__restrict__ WT,
+ring_proj_kernel(const float *__restrict__ ring, int64_t pitch, int head, int cap, const float *__restrict__ WT,
                  float *__restrict__ part, int B, int L, int k_per_split) {
-    proj_body<true>(ring, 1, pitch, head, WT, part, B, L, k_per_split);
+    proj_body<true>(ring, 1, pitch, head, cap, WT, part, B, L, k_per_split);
 }
 
 // gates[b][g] = (sum_ks partial[ks][b][g] + b_ih[g]) + b_hh[g]
@@ -321,13 +322,13 @@ int launch_head(const Dims &d, const HeadWeights &hw, const float *feats, int64_
     return launches + n;
 }
 
-// launch_head of independent windows over a feature ring: window b's position k in ring[((head + k) mod L) pitch + b]
-int launch_ring_head(const Dims &d, const HeadWeights &hw, const float *ring, int64_t pitch, int head, int64_t B,
+// launch_head of independent windows over a feature ring: window b's position k in ring[((head + k) mod cap) pitch + b]
+int launch_ring_head(const Dims &d, const HeadWeights &hw, const float *ring, int64_t pitch, int cap, int head, int64_t B,
                      const float *age, int64_t n_age, int apply_sigmoid, float *out, float *gates_ws, float *partial_ws,
                      cudaStream_t st, const char **err) {
     int ks_eff;
     const int kps = proj_split(d.L, choose_ksplit(d.L), &ks_eff);
-    ring_proj_kernel<<<dim3((unsigned)((B + kPM - 1) / kPM), ks_eff), 256, 0, st>>>(ring, pitch, head, hw.wih0T, partial_ws, (int)B,
+    ring_proj_kernel<<<dim3((unsigned)((B + kPM - 1) / kPM), ks_eff), 256, 0, st>>>(ring, pitch, head, cap, hw.wih0T, partial_ws, (int)B,
                                                                                     d.L, kps);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) { *err = cudaGetErrorString(e); return -1; }

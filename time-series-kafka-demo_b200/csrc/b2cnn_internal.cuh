@@ -127,8 +127,9 @@ int choose_ksplit(int L);
 int proj_slices(int L);       // split-K slices launch_head's projection writes for L positions: [slices][B][64] partials
 
 // launch_head of independent windows whose features sit in a sliding scorer's position-major ring (b2cnn_slide.cu):
-// position k of window b in ring[((head + k) mod L) * pitch + b]; the same tiles and summation order as launch_head
-int launch_ring_head(const Dims &d, const HeadWeights &hw, const float *ring, int64_t pitch, int head, int64_t B,
+// position k < d.L of window b in ring[((head + k) mod cap) * pitch + b] (cap >= d.L: the window may be a suffix of the
+// ring's); the same tiles and summation order as launch_head
+int launch_ring_head(const Dims &d, const HeadWeights &hw, const float *ring, int64_t pitch, int cap, int head, int64_t B,
                      const float *age, int64_t n_age, int apply_sigmoid, float *out, float *gates_ws, float *partial_ws,
                      cudaStream_t st, const char **err);
 

@@ -20,7 +20,8 @@
 //   * once n S >= W: slide_ring_proj_kernel, [P x L] . [L x 64] over the ring on wgmma with window feature j in slot
 //     (G_n + j) mod L, split-K over the streaming kernels' position ranges (they depend on L only) ->
 //     partial[range][P][64]; then the head kernel of the independent forward sums the ranges in fixed order and runs
-//     the LSTM cells, Linear, age scale and sigmoid.
+//     the LSTM cells, Linear, age scale and sigmoid.  Extra heads (b2cnn_slide_set_heads_ex) may have a shorter window
+//     W_k ending at nS: window positions d .. L - 1 of the scorer's, d = (W - W_k) / F, with their own ranges.
 //
 // Per-patient lifecycle (b2cnn_slide_admit / _discharge): seen[p] counts patient p's samples since its admission (-1:
 // discharged); its window after a push is the last W samples of (history | pushes since admission), defined once
@@ -45,11 +46,15 @@ namespace b2cnn {
 constexpr int kSlideTail = 24;       // stream samples kept per patient and channel: the largest receptive field
 
 // An extra head scored from the scorer's ring (b2cnn_slide_set_heads): a snapshot of a model's LSTM / Linear weights,
-// W_ih^T, age coefficient and (tensor-core path) packed W_ih chunks, with its range partials, in one allocation.
+// W_ih^T, age coefficient and (tensor-core path) packed W_ih chunks, with its range partials, in one allocation.  Its
+// window W_k <= W ends where the scorer's does (b2cnn_slide_set_heads_ex): its L_k features are the last L_k of the
+// scorer's window, window positions d .. L - 1 with d = (W - W_k) / F = L - L_k.
 struct SlideHead {
     HeadWeights hw;                  // into mem
     float age_coef = 0.f;
     uint64_t digest = 0;             // the model's front-end digest when it was attached
+    int W = 0, L = 0;                // its window and feature count
+    int ranges = 0, feats_per_cta = 0, chunks_per_cta = 0;   // tensor-core path: its handle's TcState (from L_k only)
     const uint8_t *wpack = nullptr;  // tensor-core path: [n_ranges][chunks_per_cta][6 KB], into mem
     float *partial = nullptr;        // tensor-core path: [n_ranges][P][64], into mem
     void *mem = nullptr;
@@ -201,9 +206,11 @@ __global__ void slide_stage_kernel(const T *__restrict__ src, int64_t sp, int ph
 // ---- projection over the ring on the tensor cores -----------------------------------------------------------------
 // The split-K ranges and 16-position chunks are those of the streaming kernels (TcState: feats_per_cta, chunks_per_cta,
 // n_ranges, all from L only), so the packed W_ih chunks of tc_prepare serve unchanged: chunk m of range r holds the
-// weights of window positions r F + 16 m - foff + k (k < 16), zero outside the range.  CTA = (128 patients, range):
+// weights of window positions r F + 16 m - foff + k (k < 16), zero outside the range.  A row's window (L positions,
+// its first in slot `head`) may be a suffix of the ring's (cap >= L slots): a head with a shorter window.
+// CTA = (128 patients, range):
 //   warp 4: TMA producer -- per chunk one {128 patients x 16 slots} fp32 box of the ring at the chunk's first slot and,
-//           when the 16 slots wrap past L, a second box at slot 0; plus the 6 KB W_ih chunk (bulk copy); two stages;
+//           when the 16 slots wrap past cap, a second box at slot 0; plus the 6 KB W_ih chunk (bulk copy); two stages;
 //   warps 0-3: thread == patient: the chunk's 16 features (0 outside the range) split into three bf16 pieces written
 //           as the K-major A tile, then 2 row halves x 6 m64n64k16 piece pairs (hh hm mh hl lh mm, fp32-equivalent
 //           products, as the fused kernel) accumulating partial[range][patient][64] in registers.
@@ -220,7 +227,7 @@ constexpr size_t kRpSmem = kRpSmemHP<1>;
 struct RingProjParams {
     const uint8_t *wpack;            // [n_ranges][chunks_per_cta][kRpWChunk]
     float *partial;                  // [n_ranges][P][64]
-    int P, L, head, feats_per_cta, chunks_per_cta, foff;
+    int P, L, cap, head, feats_per_cta, chunks_per_cta, foff;   // L: the row's window positions; cap: the ring's slots
 };
 
 // A push with heads: rows 0 (the scorer's model) .. K (its heads) of the output, HP rows per CTA.  CTA x = tile * pairs
@@ -272,8 +279,8 @@ slide_ring_proj_kernel(const __grid_constant__ CUtensorMap tm, const __grid_cons
     __syncthreads();
     // ring slot of the chunk's first window position (which may lie before 0 or past L: those features are masked)
     auto first_slot = [&](int m) {
-        int s = (p.head + lo + 16 * m - p.foff) % p.L;
-        return s < 0 ? s + p.L : s;
+        int s = (p.head + lo + 16 * m - p.foff) % p.cap;
+        return s < 0 ? s + p.cap : s;
     };
     if (warp == 4) {
         if (lane == 0) {
@@ -281,7 +288,7 @@ slide_ring_proj_kernel(const __grid_constant__ CUtensorMap tm, const __grid_cons
                 const int u = m & 1;
                 mbar_wait(bar_empty + 8 * u, ((m >> 1) & 1) ^ 1);
                 const int s0 = first_slot(m);
-                const bool wraps = s0 + 16 > p.L;
+                const bool wraps = s0 + 16 > p.cap;
                 mbar_expect_tx(bar_full + 8 * u, (wraps ? 2 : 1) * kRpBox + HP * kRpWChunk);
                 const uint32_t dst = smem_u32(sF + (size_t)u * 2 * 16 * kRpM);
                 tma_load_2d(dst, &tm, b0, s0, bar_full + 8 * u);
@@ -312,7 +319,7 @@ slide_ring_proj_kernel(const __grid_constant__ CUtensorMap tm, const __grid_cons
         auto feat = [&](int k) {
             const int q = q0 + k;
             if (q < lo || q >= hi) return 0.f;
-            return s0 + k < p.L ? fa[k * kRpM + row] : fb[(s0 + k - p.L) * kRpM + row];
+            return s0 + k < p.cap ? fa[k * kRpM + row] : fb[(s0 + k - p.cap) * kRpM + row];
         };
 #pragma unroll
         for (int kk = 0; kk < 8; ++kk) {
@@ -410,6 +417,13 @@ __global__ void slide_live_kernel(int64_t *__restrict__ seen, int P, int64_t adv
     if (adv != 0 && v >= 0) seen[b] = v += adv;
     if (!x || v >= W) return;
     for (int64_t j = blockIdx.y; j < len; j += gridDim.y) x[b * len + j] = __int_as_float(0x7fc00000);
+}
+
+// out[r][P] = NaN for every row r with bit r of `rows` set (blockIdx.y = r): the rows of a push with heads whose window
+// no patient has complete yet (a scorer without lifecycle calls; with them slide_live_kernel masks those rows whole)
+__global__ void slide_nan_rows_kernel(float *__restrict__ out, int P, unsigned rows) {
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b < P && ((rows >> blockIdx.y) & 1u)) out[(int64_t)blockIdx.y * P + b] = __int_as_float(0x7fc00000);
 }
 
 // ---- generic path kernels: tails of any length T ------------------------------------------------------------------
@@ -659,10 +673,10 @@ int slide_reset(Slide *s, cudaStream_t st, const char **err) {
 
 static int64_t window_head(const Slide &s, int64_t n) { return fdiv(n * s.S - s.d.W - s.phi, s.F); }
 
-// slide_live_kernel over the P patients: seen += adv, then NaN rows of x [P][len] without a complete window
-static int launch_live(const Slide &s, int64_t adv, float *x, int64_t len, cudaStream_t st, const char **err) {
+// slide_live_kernel over the P patients: seen += adv, then NaN rows of x [P][len] without a complete window of W samples
+static int launch_live(const Slide &s, int64_t adv, int64_t W, float *x, int64_t len, cudaStream_t st, const char **err) {
     const unsigned gy = adv != 0 || len <= 1 ? 1u : (unsigned)std::min<int64_t>(len, 64);
-    slide_live_kernel<<<dim3((unsigned)((s.P + 127) / 128), gy), 128, 0, st>>>(s.seen, s.P, adv, s.d.W, x, len);
+    slide_live_kernel<<<dim3((unsigned)((s.P + 127) / 128), gy), 128, 0, st>>>(s.seen, s.P, adv, W, x, len);
     if (cudaGetLastError() != cudaSuccess) { *err = "lifecycle mask launch"; return -1; }
     return 1;
 }
@@ -670,7 +684,7 @@ static int launch_live(const Slide &s, int64_t adv, float *x, int64_t len, cudaS
 // a push's lifecycle step: the device counts advance by S (and out[P] gets its NaNs), then the host mirror -- only once
 // the launch went out, so that the two never disagree
 static int advance_seen(Slide *s, float *out, cudaStream_t st, const char **err) {
-    if (launch_live(*s, s->S, out, 1, st, err) < 0) return -1;
+    if (launch_live(*s, s->S, s->d.W, out, 1, st, err) < 0) return -1;
     for (int64_t &v : s->seen_h)
         if (v >= 0) v += s->S;
     return 1;
@@ -743,84 +757,121 @@ int slide_push(Slide *s, const ConvWeights &cw, const HeadWeights &hw, const TcS
     return score_windows(s, hw, &tc, age, n_age, apply_sigmoid, out, heads, emitted, window_index, ev, st, err);
 }
 
-// the model's Dims with a head's age coefficient: the reduction / LSTM head launchers take it from there
-static Dims head_dims(const Dims &d, const SlideHead &hd) {
-    Dims dh = d;
-    dh.age_coef = hd.age_coef;
-    return dh;
-}
+// one row of a push: the scorer's model (row 0) or head r - 1, with what its projection and head need
+struct ScoreRow {
+    const HeadWeights *hw;
+    Dims d;                          // the model's Dims with the row's window, feature count and age coefficient
+    int ranges, feats_per_cta, chunks_per_cta;   // split-K slices of its partials (tensor-core path: its TcState)
+    const uint8_t *wpack;            // tensor-core path: its packed W_ih chunks
+    float *partial;
+    int head;                        // ring slot of its window position 0
+};
 
-// the end of push n = s->n: projection over the ring + head, once a window is complete (every patient's, or with the
-// lifecycle on, one); on tensor cores with `tc`, else (generic path) on CUDA cores.  With `heads`, out is [1 + K][P]:
-// row 0 the scorer's model as without, row i head i - 1 from the same ring.
+// the end of push n = s->n: projection over the ring + head for every row whose window is complete (every patient's,
+// or with the lifecycle on, one); on tensor cores with `tc`, else (generic path) on CUDA cores.  With `heads`, out is
+// [1 + K][P]: row 0 the scorer's model as without, row i head i - 1 from the same ring.  A head with window W_k < W
+// reads the last L_k positions of the scorer's window: its position 0 is the scorer's position d = (W - W_k) / F.
 static int score_windows(Slide *s, const HeadWeights &hw, const TcState *tc, const float *age, int64_t n_age, int apply_sigmoid,
                          float *out, bool heads, int *emitted, int64_t *window_index, cudaEvent_t *ev, cudaStream_t st,
                          const char **err) {
     const Dims &d = s->d;
     const int64_t P = s->P, S = s->S, n1 = s->n;
-    const int K = heads ? (int)s->heads.size() : 0;
-    bool live = n1 * S >= d.W;
-    if (s->lifecycle)
-        live = std::any_of(s->seen_h.begin(), s->seen_h.end(), [&](int64_t v) { return v >= 0 && v + S >= d.W; });
+    const int rows = 1 + (heads ? (int)s->heads.size() : 0);
+    auto complete = [&](int64_t Wr) {
+        if (!s->lifecycle) return n1 * S >= Wr;
+        return std::any_of(s->seen_h.begin(), s->seen_h.end(), [&](int64_t v) { return v >= 0 && v + S >= Wr; });
+    };
+    const int64_t G = window_head(*s, n1);
+    ScoreRow row[kRpMaxRows];
+    unsigned live = 0;                                             // bit r: row r is scored
+    for (int r = 0; r < rows; ++r) {
+        ScoreRow &w = row[r];
+        w.d = d;
+        if (r == 0) {
+            w.hw = &hw; w.ranges = s->ranges; w.partial = s->partial;
+            w.feats_per_cta = tc ? tc->feats_per_cta : 0; w.chunks_per_cta = tc ? tc->chunks_per_cta : 0;
+            w.wpack = tc ? reinterpret_cast<const uint8_t *>(tc->d_wpack) : nullptr;
+        } else {
+            const SlideHead &hd = s->heads[r - 1];
+            w.hw = &hd.hw; w.d.W = hd.W; w.d.L = hd.L; w.d.age_coef = hd.age_coef;
+            w.ranges = hd.ranges; w.feats_per_cta = hd.feats_per_cta; w.chunks_per_cta = hd.chunks_per_cta;
+            w.wpack = hd.wpack; w.partial = tc ? hd.partial : s->partial;   // generic path: one after another on the scorer's
+        }
+        w.head = (int)mod_nn(G + (d.W - w.d.W) / s->F, d.L);
+        if (complete(w.d.W)) live |= 1u << r;
+    }
     *emitted = 0;
     if (!live) {
         if (s->lifecycle && advance_seen(s, nullptr, st, err) < 0) return B2CNN_ECUDA;
         if (ev && cudaEventRecord(ev[2], st) != cudaSuccess) { *err = "cudaEventRecord"; return B2CNN_ECUDA; }
         return B2CNN_OK;
     }
-    const int head = (int)mod_nn(window_head(*s, n1), d.L);
     if (!tc) {
-        if (launch_ring_head(d, hw, s->ring, s->ring_pitch, head, P, age, n_age, apply_sigmoid, out, s->gates, s->partial, st, err) < 0)
-            return B2CNN_ECUDA;
-        // each head: the same kernels over the same ring with its own W_ih^T, LSTM, Linear and age coefficient
-        for (int i = 0; i < K; ++i) {
-            const SlideHead &hd = s->heads[i];
-            if (launch_ring_head(head_dims(d, hd), hd.hw, s->ring, s->ring_pitch, head, P, age, n_age, apply_sigmoid, out + (i + 1) * P,
+        // each row: the same kernels over the same ring with its own W_ih^T, LSTM, Linear and age coefficient
+        for (int r = 0; r < rows; ++r) {
+            if (!((live >> r) & 1u)) continue;
+            if (launch_ring_head(row[r].d, *row[r].hw, s->ring, s->ring_pitch, d.L, row[r].head, P, age, n_age, apply_sigmoid, out + r * P,
                                  s->gates, s->partial, st, err) < 0)
                 return B2CNN_ECUDA;
         }
     } else {
         CUtensorMap tm;
         if (tc_ring_tmap(s->ring, P, s->ring_pitch, d.L, &tm, err) != 0) return B2CNN_ECUDA;
-        RingProjParams rp;
-        rp.wpack = reinterpret_cast<const uint8_t *>(tc->d_wpack); rp.partial = s->partial;
-        rp.P = (int)P; rp.L = d.L; rp.head = head;
-        rp.feats_per_cta = tc->feats_per_cta; rp.chunks_per_cta = tc->chunks_per_cta; rp.foff = d.K1 == 10 ? 3 : 2;
         const unsigned tiles = (unsigned)((P + kRpM - 1) / kRpM);
-        if (K == 0) {
-            if (cudaFuncSetAttribute(slide_ring_proj_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kRpSmem) != cudaSuccess) {
-                *err = "projection smem attribute"; return B2CNN_ECUDA;
+        // rows of one window share its ranges, chunks and A pieces: they run in pairs (HP = 2; an odd count pads the last
+        // pair with a copy of its row that is not stored); a row whose window no other scored row has runs alone (HP = 1)
+        for (unsigned todo = live; todo;) {
+            const int r0 = __builtin_ctz(todo);
+            const ScoreRow &w0 = row[r0];
+            int grp[kRpMaxRows], g = 0;
+            for (int r = r0; r < rows; ++r)
+                if (((todo >> r) & 1u) && row[r].d.W == w0.d.W && row[r].ranges == w0.ranges &&
+                    row[r].feats_per_cta == w0.feats_per_cta && row[r].chunks_per_cta == w0.chunks_per_cta) {
+                    grp[g++] = r;
+                    todo &= ~(1u << r);
+                }
+            RingProjParams rp;
+            rp.wpack = w0.wpack; rp.partial = w0.partial;
+            rp.P = (int)P; rp.L = w0.d.L; rp.cap = d.L; rp.head = w0.head;
+            rp.feats_per_cta = w0.feats_per_cta; rp.chunks_per_cta = w0.chunks_per_cta; rp.foff = d.K1 == 10 ? 3 : 2;
+            if (g == 1) {
+                if (cudaFuncSetAttribute(slide_ring_proj_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kRpSmem) != cudaSuccess) {
+                    *err = "projection smem attribute"; return B2CNN_ECUDA;
+                }
+                slide_ring_proj_kernel<1><<<dim3(tiles, (unsigned)w0.ranges), kRpThreads, kRpSmem, st>>>(tm, rp);
+            } else {
+                RingProjHeads a;
+                memset(&a, 0, sizeof a);
+                a.p = rp;
+                for (int j = 0; j < g; ++j) { a.wpack[j] = row[grp[j]].wpack; a.partial[j] = row[grp[j]].partial; }
+                a.pairs = (g + 1) / 2;
+                if (g % 2) a.wpack[g] = a.wpack[g - 1];                 // partial[g] stays nullptr
+                if (cudaFuncSetAttribute(slide_ring_proj_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kRpSmemHP<2>) !=
+                    cudaSuccess) {
+                    *err = "projection smem attribute"; return B2CNN_ECUDA;
+                }
+                slide_ring_proj_kernel<2><<<dim3(tiles * (unsigned)a.pairs, (unsigned)w0.ranges), kRpThreads, kRpSmemHP<2>, st>>>(tm, a);
             }
-            slide_ring_proj_kernel<1><<<dim3(tiles, (unsigned)s->ranges), kRpThreads, kRpSmem, st>>>(tm, rp);
-        } else {
-            // rows 0 .. K in pairs; an odd count pads the last pair with a copy of its row that is not stored
-            RingProjHeads a;
-            memset(&a, 0, sizeof a);
-            a.p = rp;
-            a.wpack[0] = rp.wpack; a.partial[0] = s->partial;
-            for (int i = 0; i < K; ++i) { a.wpack[i + 1] = s->heads[i].wpack; a.partial[i + 1] = s->heads[i].partial; }
-            const int rows = K + 1;
-            a.pairs = (rows + 1) / 2;
-            if (rows % 2) a.wpack[rows] = a.wpack[rows - 1];             // partial[rows] stays nullptr
-            if (cudaFuncSetAttribute(slide_ring_proj_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kRpSmemHP<2>) !=
-                cudaSuccess) {
-                *err = "projection smem attribute"; return B2CNN_ECUDA;
-            }
-            slide_ring_proj_kernel<2><<<dim3(tiles * (unsigned)a.pairs, (unsigned)s->ranges), kRpThreads, kRpSmemHP<2>, st>>>(tm, a);
+            if (cudaGetLastError() != cudaSuccess) { *err = "projection launch"; return B2CNN_ECUDA; }
         }
-        if (cudaGetLastError() != cudaSuccess) { *err = "projection launch"; return B2CNN_ECUDA; }
-        if (launch_reduce_lstm_head(d, hw, s->partial, s->ranges, P, age, n_age, apply_sigmoid, out, st, err) < 0) return B2CNN_ECUDA;
-        for (int i = 0; i < K; ++i) {
-            const SlideHead &hd = s->heads[i];
-            if (launch_reduce_lstm_head(head_dims(d, hd), hd.hw, hd.partial, s->ranges, P, age, n_age, apply_sigmoid, out + (i + 1) * P,
-                                        st, err) < 0)
+        for (int r = 0; r < rows; ++r) {
+            if (!((live >> r) & 1u)) continue;
+            if (launch_reduce_lstm_head(row[r].d, *row[r].hw, row[r].partial, row[r].ranges, P, age, n_age, apply_sigmoid, out + r * P, st,
+                                        err) < 0)
                 return B2CNN_ECUDA;
         }
     }
-    // row 0 is masked as without heads, and seen advances once; rows 1..K take the mask from the advanced counts
+    // rows no patient has a complete window for yet: NaN (with the lifecycle on, the masks below write them whole)
+    const unsigned all = (1u << rows) - 1u;
+    if (!s->lifecycle && live != all) {
+        slide_nan_rows_kernel<<<dim3((unsigned)((P + 127) / 128), (unsigned)rows), 128, 0, st>>>(out, (int)P, all & ~live);
+        if (cudaGetLastError() != cudaSuccess) { *err = "NaN rows launch"; return B2CNN_ECUDA; }
+    }
+    // row 0 is masked as without heads, and seen advances once; rows 1..K take the mask of their own windows from the
+    // advanced counts
     if (s->lifecycle && advance_seen(s, out, st, err) < 0) return B2CNN_ECUDA;
-    for (int i = 0; s->lifecycle && i < K; ++i)
-        if (launch_live(*s, 0, out + (i + 1) * P, 1, st, err) < 0) return B2CNN_ECUDA;
+    for (int r = 1; s->lifecycle && r < rows; ++r)
+        if (launch_live(*s, 0, row[r].d.W, out + r * P, 1, st, err) < 0) return B2CNN_ECUDA;
     if (ev && cudaEventRecord(ev[2], st) != cudaSuccess) { *err = "cudaEventRecord"; return B2CNN_ECUDA; }
     *emitted = 1;
     *window_index = n1 - (d.W + S - 1) / S;
@@ -834,7 +885,7 @@ int slide_features(const Slide *s, float *feats, cudaStream_t st, const char **e
     const int head = (int)mod_nn(window_head(*s, s->n), s->d.L);
     slide_gather_kernel<<<dim3((unsigned)((s->P + 127) / 128), 64), 128, 0, st>>>(s->ring, s->ring_pitch, s->d.L, s->P, head, s->d.L, feats);
     if (cudaGetLastError() != cudaSuccess) { *err = "gather launch"; return B2CNN_ECUDA; }
-    if (s->lifecycle && launch_live(*s, 0, feats, s->d.L, st, err) < 0) return B2CNN_ECUDA;
+    if (s->lifecycle && launch_live(*s, 0, s->d.W, feats, s->d.L, st, err) < 0) return B2CNN_ECUDA;
     return B2CNN_OK;
 }
 
@@ -1095,20 +1146,21 @@ static uint64_t frontend_digest(const Dims &d, const ConvWeights &cw) {
 
 // ---- extra heads --------------------------------------------------------------------------------------------------
 // One allocation per head: the blob's LSTM / Linear part (whh0 .. bo, contiguous in b2cnn_set_weights' blob) | W_ih^T
-// [L][64] | tensor-core path: the packed W_ih chunks | the range partials [n_ranges][P][64].  The generic path's heads
-// run one after another on the scorer's own partials and gates.
+// [L_k][64] | tensor-core path: the packed W_ih chunks | the range partials [n_ranges][P][64], both of the head's own
+// TcState (L_k).  The generic path's heads run one after another on the scorer's own partials and gates
+// (proj_slices(L_k) <= proj_slices(L) for L_k <= L: it is ceil(L / 2048) for every L below 2^24).
 struct HeadLayout {
     size_t lstm, wih0T, wpack, partial, total;
     int64_t n_lstm;
 };
-static HeadLayout head_layout(const Slide &s, const HeadWeights &hw, const TcState *tc) {
+static HeadLayout head_layout(const Slide &s, const SlideHeadSource &src) {
     HeadLayout a;
-    a.n_lstm = hw.bo + 1 - hw.whh0;
+    a.n_lstm = src.hw.bo + 1 - src.hw.whh0;
     a.lstm = al256(sizeof(float) * (size_t)a.n_lstm);
-    a.wih0T = al256(sizeof(float) * (size_t)s.d.L * kGates);
+    a.wih0T = al256(sizeof(float) * (size_t)src.L * kGates);
     const bool tcp = s.path == B2CNN_PATH_TENSORCORE;
-    a.wpack = tcp ? al256((size_t)tc->n_ranges * tc->chunks_per_cta * kRpWChunk) : 0;
-    a.partial = tcp ? al256(sizeof(float) * (size_t)s.ranges * s.P * kGates) : 0;
+    a.wpack = tcp ? al256((size_t)src.tc->n_ranges * src.tc->chunks_per_cta * kRpWChunk) : 0;
+    a.partial = tcp ? al256(sizeof(float) * (size_t)src.tc->n_ranges * s.P * kGates) : 0;
     a.total = a.lstm + a.wih0T + a.wpack + a.partial;
     return a;
 }
@@ -1125,13 +1177,13 @@ int slide_set_heads(Slide *s, const SlideHeadSource *src, int n, cudaStream_t st
     };
     for (int i = 0; i < n; ++i) {
         const HeadWeights &w = src[i].hw;
-        const HeadLayout a = head_layout(*s, w, src[i].tc);
+        const HeadLayout a = head_layout(*s, src[i]);
         SlideHead &hd = next[i];
         if (cudaMalloc(&hd.mem, a.total) != cudaSuccess) return drop("cudaMalloc(head weights)");
         char *base = static_cast<char *>(hd.mem);
         float *lstm = reinterpret_cast<float *>(base), *wih0T = reinterpret_cast<float *>(base + a.lstm);
         if (cudaMemcpyAsync(lstm, w.whh0, sizeof(float) * (size_t)a.n_lstm, cudaMemcpyDeviceToDevice, st) != cudaSuccess ||
-            cudaMemcpyAsync(wih0T, w.wih0T, sizeof(float) * (size_t)s->d.L * kGates, cudaMemcpyDeviceToDevice, st) != cudaSuccess)
+            cudaMemcpyAsync(wih0T, w.wih0T, sizeof(float) * (size_t)src[i].L * kGates, cudaMemcpyDeviceToDevice, st) != cudaSuccess)
             return drop("copy of the head weights");
         hd.hw.wih0T = wih0T;
         hd.hw.whh0 = rebase(w.whh0, w.whh0, lstm); hd.hw.bih0 = rebase(w.bih0, w.whh0, lstm); hd.hw.bhh0 = rebase(w.bhh0, w.whh0, lstm);
@@ -1140,7 +1192,11 @@ int slide_set_heads(Slide *s, const SlideHeadSource *src, int n, cudaStream_t st
         hd.hw.wo = rebase(w.wo, w.whh0, lstm); hd.hw.bo = rebase(w.bo, w.whh0, lstm);
         hd.age_coef = src[i].age_coef;
         hd.digest = src[i].digest;
+        hd.W = src[i].W; hd.L = src[i].L;
+        hd.ranges = proj_slices(hd.L);
         if (s->path == B2CNN_PATH_TENSORCORE) {
+            hd.ranges = src[i].tc->n_ranges;
+            hd.feats_per_cta = src[i].tc->feats_per_cta; hd.chunks_per_cta = src[i].tc->chunks_per_cta;
             uint8_t *wp = reinterpret_cast<uint8_t *>(base + a.lstm + a.wih0T);
             if (cudaMemcpyAsync(wp, src[i].tc->d_wpack, (size_t)src[i].tc->n_ranges * src[i].tc->chunks_per_cta * kRpWChunk,
                                 cudaMemcpyDeviceToDevice, st) != cudaSuccess)

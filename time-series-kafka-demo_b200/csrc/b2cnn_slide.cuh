@@ -21,12 +21,14 @@ int slide_reset(Slide *s, cudaStream_t st, const char **err);
 int slide_push(Slide *s, const ConvWeights &cw, const HeadWeights &hw, const TcState &tc, const void *x, int64_t pitch,
                const float *age, int64_t n_age, int apply_sigmoid, float *out, bool heads, int *emitted, int64_t *window_index,
                cudaEvent_t *ev, cudaStream_t st, const char **err);
-// extra heads (b2cnn_slide_set_heads): what a head is copied from -- a handle of the same architecture and front end
+// extra heads (b2cnn_slide_set_heads): what a head is copied from -- a handle of the same architecture and front end,
+// its window W <= the scorer's with (scorer W - W) % F == 0 and L = L_out(W) (checked by the caller)
 struct SlideHeadSource {
-    HeadWeights hw;                  // the handle's pointers into its blob and its W_ih^T
+    HeadWeights hw;                  // the handle's pointers into its blob and its W_ih^T [L][64]
     const TcState *tc;               // its packed W_ih chunks (tensor-core path)
     float age_coef;
     uint64_t digest;                 // its front-end digest
+    int W, L;                        // its window and feature count
 };
 // replaces the heads with copies of src[0 .. n) (allocated and copied here, the stream synchronised); on failure the
 // previous heads stay

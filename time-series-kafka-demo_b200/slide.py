@@ -25,6 +25,13 @@ stored features, with no cold start and no second front end::
 
     scorer.set_heads([candidate])
     out = scorer.push(samples, age=ages, heads=True)                 # [2, P]: production row 0, candidate row 1
+
+With ``shorter_windows=True`` a head may have a shorter window than the scorer's (risk over the last 60 s, 300 s and
+600 s of one stream), scored from the tail of the same stored window instead of by a scorer of its own::
+
+    scorer = SlidingScorer(m600, n_patients=P, stride=7500)          # W = 75000: 600 s at 125 Hz
+    scorer.set_heads([m60, m300], shorter_windows=True)              # W_k = 7500 and 37500, the same conv weights
+    out = scorer.push(samples, age=ages, heads=True)                 # [3, P] once the 60 s window is complete
 """
 from __future__ import annotations
 
@@ -54,7 +61,9 @@ class SlidingScorer:
 
     Extra heads: ``set_heads(models)`` attaches models of the same architecture and front-end (conv / affine) weights,
     ``push(..., heads=True)`` returns ``Tensor[1 + K, P]``, row 0 what ``push`` returns and row i ``heads[i - 1]``'s
-    logits of the same windows.  ``heads`` is the tuple attached."""
+    logits of the same windows.  ``heads`` is the tuple attached.  ``set_heads(models, shorter_windows=True)`` also
+    takes heads whose window ``W_k <= W`` ends where the scorer's does (``W - W_k`` a multiple of the feature stride);
+    ``head_windows`` lists each row's window."""
 
     ARCH_FIELDS = ("in_channels", "window", "k1", "k2", "pool_k", "pool_s", "act", "affine", "l_out", "c_mid", "hidden", "layers")
 
@@ -180,38 +189,73 @@ class SlidingScorer:
         """The models attached by ``set_heads`` (read-only)."""
         return self._heads
 
-    def check_heads(self, models) -> tuple:
+    @property
+    def head_windows(self) -> tuple:
+        """The window of each row of ``push(heads=True)`` in samples, row 0 (the scorer's own, W) first (read-only)."""
+        return (self.window,) + tuple(m.arch.window for m in self._heads)
+
+    def check_heads(self, models, shorter_windows: bool = False) -> tuple:
         """Validates ``set_heads``' argument without touching the library; returns the models as a tuple."""
         from .model import B200MyCNN
         if isinstance(models, (B200MyCNN, torch.Tensor, str, bytes)) or not hasattr(models, "__iter__"):
             raise TypeError("set_heads takes a list of B200MyCNN models")
+        if not isinstance(shorter_windows, bool):
+            raise TypeError(f"shorter_windows must be True or False, got {type(shorter_windows).__name__}")
         models = tuple(models)
         if len(models) > capi.SLIDE_MAX_HEADS:
             raise ValueError(f"at most {capi.SLIDE_MAX_HEADS} heads, got {len(models)}")
         mine = self.model.arch
+        fields = [f for f in self.ARCH_FIELDS if not (shorter_windows and f in ("window", "l_out"))]
         for i, m in enumerate(models):
             if not isinstance(m, B200MyCNN):
                 raise TypeError(f"heads[{i}] is a {type(m).__name__}, not a B200MyCNN")
-            bad = [f for f in self.ARCH_FIELDS if getattr(m.arch, f) != getattr(mine, f)]
+            bad = [f for f in fields if getattr(m.arch, f) != getattr(mine, f)]
             if bad:
                 raise ValueError(f"heads[{i}] differs from the scorer's model in {', '.join(bad)}")
+            if shorter_windows:
+                self._check_head_window(i, m.arch)
             if m._device() != self.device:
                 raise ValueError(f"heads[{i}] is on {m._device()}, the scorer on {self.device}")
         return models
 
-    def set_heads(self, models):
+    def _check_head_window(self, i: int, arch):
+        """a head window W_k ends where the scorer's does: W_k <= W, W - W_k a multiple of the feature stride F, and
+        the head's LSTM input size the feature count of W_k"""
+        a = self.model.arch
+        F = a.pool_s ** 2                                         # 4 on the tensor-core path's geometries too
+        R = a.pool_s * (a.pool_k + a.k2 - 2) + a.pool_k + a.k1 - 1   # samples one feature reads
+        Wk = arch.window
+        if Wk > self.window:
+            raise ValueError(f"heads[{i}]'s window {Wk} is longer than the scorer's, {self.window}")
+        if (self.window - Wk) % F:
+            raise ValueError(f"heads[{i}]'s window {Wk} is not the scorer's window {self.window} minus a multiple of the "
+                             f"feature stride {F}")
+        if Wk < R or arch.l_out != (Wk - R) // F + 1:
+            raise ValueError(f"heads[{i}]'s l_out {arch.l_out} is not the feature count of its window {Wk}")
+
+    def set_heads(self, models, shorter_windows: bool = False):
         """Replace the extra heads with ``models`` (a list of ``B200MyCNN``, possibly empty, at most 8): each with the
         scorer model's architecture (``age_coef`` may differ), its conv / affine weights and its device.  Takes a
         SNAPSHOT of each head's LSTM / Linear weights and ``age_coef``: a later change to a head model's weights has no
         effect until ``set_heads`` is called again.  A head attached at push n is scored from push n on, as a scorer of
-        that model running since the start would score it.  Atomic: a failed call leaves the previous heads."""
-        models = self.check_heads(models)
+        that model running since the start would score it.  Atomic: a failed call leaves the previous heads.
+
+        ``shorter_windows=True``: a head's ``window`` (and with it its LSTM input size) may also be shorter than the
+        scorer's W, as long as ``W - window`` is a multiple of the feature stride (4 on the tensor-core path,
+        ``pool_s ** 2`` on the generic path).  Its window ends where the scorer's does, so its features are the last
+        ones of the stored window, and its row equals what a scorer of that model at its own window and the same
+        stride computes from the same pushes, NaN for a patient whose ``samples_seen`` is below its window."""
+        models = self.check_heads(models, shorter_windows)
         self._handle()
         hs = [m._ensure_handle()[1].value for m in models]
         arr = (ctypes.c_void_p * max(len(hs), 1))(*hs)
         with torch.cuda.device(self.device):
-            capi.check(self._lib.b2cnn_slide_set_heads(self._s, arr, len(hs), torch.cuda.current_stream().cuda_stream),
-                       "b2cnn_slide_set_heads")
+            st = torch.cuda.current_stream().cuda_stream
+            if shorter_windows:
+                capi.check(self._lib.b2cnn_slide_set_heads_ex(self._s, arr, len(hs), capi.SLIDE_HEADS_SHORTER_WINDOWS, st),
+                           "b2cnn_slide_set_heads_ex")
+            else:
+                capi.check(self._lib.b2cnn_slide_set_heads(self._s, arr, len(hs), st), "b2cnn_slide_set_heads")
         self._heads = models
 
     @torch.no_grad()
@@ -221,7 +265,10 @@ class SlidingScorer:
         first window fills.  After ``admit`` / ``discharge``: NaN for every patient whose window is not complete
         (``samples_seen < W``; a discharged patient's samples are ignored), ``None`` when no patient's window is.
         ``heads=True``: ``Tensor[1 + K, P]`` (or ``None`` as above), row 0 exactly what ``heads=False`` returns, row i
-        the scores of ``heads[i - 1]`` on the same windows and ages, NaN where row 0 is."""
+        the scores of ``heads[i - 1]`` on the same windows and ages, NaN where row 0 is.  With heads of shorter windows
+        (``set_heads(..., shorter_windows=True)``) row i is NaN where that row's own window ``head_windows[i]`` is
+        incomplete, and the result is returned as soon as any row has a complete window for one patient (row 0 may
+        then be all NaN)."""
         if not isinstance(heads, bool):
             raise TypeError(f"heads must be True or False, got {type(heads).__name__}")
         pitch = self.check_samples(samples)
