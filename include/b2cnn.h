@@ -287,6 +287,27 @@ int b2cnn_slide_admit(b2cnn_slide *slide, const int32_t *patients, int32_t n, co
 int b2cnn_slide_discharge(b2cnn_slide *slide, const int32_t *patients, int32_t n, void *stream);
 int b2cnn_slide_samples_seen(b2cnn_slide *slide, int64_t *seen, void *stream);
 
+/* Every sliding window of whole recordings in one call (DESIGN.md §7), each window feature computed once.
+ *   b2cnn_score_record  x: DEVICE [B][C][pitch] samples of `dtype` (channel rows pitch >= N samples apart, recordings
+ *                        C pitch apart; any alignment), N samples per recording.  out: DEVICE float [B][n_w], n_w =
+ *                        (N - W) / stride + 1 (0 when N < W: nothing runs).  out[b][w] is the logit (sigmoid with
+ *                        apply_sigmoid) of the window x[b][:][w stride .. w stride + W - 1], as b2cnn_forward scores it in
+ *                        independent mode.  age: DEVICE float, n_age = 1 or B (one per recording, for all its windows).
+ *                        path: B2CNN_PATH_TENSORCORE (the models b2cnn_slide_create holds; else B2CNN_EARCH),
+ *                        B2CNN_PATH_GENERIC (every model, exact fp32: logits bit-identical to b2cnn_forward with path =
+ *                        generic and small_kernel = 0 on the windows) or B2CNN_PATH_AUTO (tensor cores where they hold).
+ *                        stride: a positive multiple of the feature stride pool_s^2 (4 on the tensor-core path); it may
+ *                        exceed W.  A fixed number of launches whatever B, N and stride; nothing allocated, nothing
+ *                        synchronised.  Every check runs before the first launch: B2CNN_EINVAL for a bad stride, shape,
+ *                        dtype, path, pitch < N, n_age or more than 2^25 rows (B n_w, or B times the folded rows per
+ *                        recording); B2CNN_ESTATE for a workspace that is missing, not 256-byte aligned or smaller than
+ *                        b2cnn_record_workspace_bytes; B2CNN_EARCH as above.
+ *   b2cnn_record_workspace_bytes  DEVICE workspace of that call (-1 for bad arguments, with b2cnn_last_error). */
+int64_t b2cnn_record_workspace_bytes(b2cnn_handle *h, int64_t B, int64_t N, int64_t pitch, int64_t stride, int dtype, int path);
+int b2cnn_score_record(b2cnn_handle *h, const void *x, int dtype, int64_t B, int64_t N, int64_t pitch, int64_t stride, int path,
+                       const float *age, int64_t n_age, int apply_sigmoid, float *out, void *workspace, int64_t workspace_bytes,
+                       void *stream);
+
 /* Export and import of patients (a restart, beds moved to another scorer or GPU, new LSTM / head weights).  A
  * patient's state is its current window's L features in window order, raw and unmasked (for a complete window
  * bit-identical to its b2cnn_slide_features row), its T-sample tail (the stream's last T samples per channel, fp32;

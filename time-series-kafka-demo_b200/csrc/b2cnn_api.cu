@@ -810,6 +810,46 @@ extern "C" int b2cnn_slide_import(b2cnn_slide *o, const int32_t *patients, int32
     return rc == B2CNN_OK ? rc : fail(rc, std::string("b2cnn_slide_import: ") + err);
 }
 
+// ---- every sliding window of whole recordings (b2cnn_slide.cu) ----
+// the path of a record call (B2CNN_OK) or the error: auto takes the tensor-core path where it holds the model, as a scorer
+static int record_path(const char *fn, const b2cnn_handle *h, int dtype, int path, bool *use_tc) {
+    if (!h) return fail(B2CNN_EINVAL, std::string(fn) + ": null argument");
+    if (!h->weights_set) return fail(B2CNN_ESTATE, std::string(fn) + ": weights not set (call b2cnn_set_weights)");
+    if (dtype != B2CNN_DTYPE_F32 && dtype != B2CNN_DTYPE_BF16) return fail(B2CNN_EINVAL, std::string(fn) + ": dtype must be f32 (0) or bf16 (1)");
+    if (path != B2CNN_PATH_TENSORCORE && path != B2CNN_PATH_GENERIC && path != B2CNN_PATH_AUTO)
+        return fail(B2CNN_EINVAL, std::string(fn) + ": path must be B2CNN_PATH_AUTO, B2CNN_PATH_GENERIC or B2CNN_PATH_TENSORCORE");
+    if (path == B2CNN_PATH_TENSORCORE && !h->tc.fused)
+        return fail(B2CNN_EARCH, std::string(fn) + ": the tensor-core path covers the streaming tensor-core geometries only (MyCNN5 or "
+                                                   "MyCNN2/3/4 conv/pool, 1 to 3 channels, tanh, no affine)");
+    *use_tc = path == B2CNN_PATH_TENSORCORE || (path == B2CNN_PATH_AUTO && h->tc.fused);
+    return B2CNN_OK;
+}
+
+extern "C" int64_t b2cnn_record_workspace_bytes(b2cnn_handle *h, int64_t B, int64_t N, int64_t pitch, int64_t stride, int dtype, int path) {
+    bool tc = false;
+    if (record_path("b2cnn_record_workspace_bytes", h, dtype, path, &tc) != B2CNN_OK) return -1;
+    if (pitch < N) { fail(B2CNN_EINVAL, "b2cnn_record_workspace_bytes: pitch must be >= the recording length"); return -1; }
+    const char *err = "";
+    const int64_t n = record_workspace_bytes(h->d, h->tc, tc, B, N, stride, dtype, &err);
+    if (n < 0) fail(B2CNN_EINVAL, std::string("b2cnn_record_workspace_bytes: ") + err);
+    return n;
+}
+
+extern "C" int b2cnn_score_record(b2cnn_handle *h, const void *x, int dtype, int64_t B, int64_t N, int64_t pitch, int64_t stride, int path,
+                                  const float *age, int64_t n_age, int apply_sigmoid, float *out, void *workspace, int64_t workspace_bytes,
+                                  void *stream) {
+    bool tc = false;
+    if (int rc = record_path("b2cnn_score_record", h, dtype, path, &tc)) return rc;
+    if (!x || !age || !out) return fail(B2CNN_EINVAL, "b2cnn_score_record: null argument");
+    DEVICE_GUARD(h->device);
+    const char *err = "";
+    const int rc = score_record(h->d, h->cw, h->hw, h->tc, tc, h->num_sms, x, dtype, B, N, pitch, stride, age, n_age, apply_sigmoid, out,
+                                workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream), &err);
+    if (rc != B2CNN_OK) return fail(rc, std::string("b2cnn_score_record: ") + err);
+    h->last_path = tc ? B2CNN_PATH_TENSORCORE : B2CNN_PATH_GENERIC;
+    return B2CNN_OK;
+}
+
 // ---- host-pointer entry: chunked H2D overlapped with compute -----------------------------
 static int ensure_host_staging(b2cnn_handle *h, size_t x_chunk_bytes, int64_t B, size_t ws_bytes) {
     if (!h->s_copy) {

@@ -44,12 +44,16 @@ void launch_transpose_wih(const float *wih0, float *wih0T, int L, cudaStream_t s
 // ---------------------------------------------------------------------------------------
 constexpr int kPM = 64, kPK = 32, kFsStride = 68;
 
-// kRing: F is a sliding scorer's position-major feature ring (sB = 1, sP = its row pitch) whose cap >= L slots hold
-// window position k in slot (head + k) mod cap; otherwise position k of window b is F[b sB + k sP].  The tiles, the zero padding
-// and the summation order are the same either way.
-template <bool kRing>
+// kProjRing: F is a sliding scorer's position-major feature ring (sB = 1, sP = its row pitch) whose cap >= L slots hold
+// window position k in slot (head + k) mod cap; kProjRecord: row b is window w = b mod n_w of recording r = b / n_w,
+// position k at F[r sB + w step + k] (sP = 1: a recording's features, record-major); otherwise (kProjRows) position k of
+// window b is F[b sB + k sP].  The tiles, the zero padding and the summation order are the same in every mode.
+constexpr int kProjRows = 0, kProjRing = 1, kProjRecord = 2;
+template <int kMode>
 __device__ __forceinline__ void proj_body(const float *__restrict__ F, int64_t sB, int64_t sP, int head, int cap,
-                                          const float *__restrict__ WT, float *__restrict__ part, int B, int L, int k_per_split) {
+                                          const float *__restrict__ WT, float *__restrict__ part, int B, int L, int k_per_split,
+                                          int n_w = 1, int64_t step = 0) {
+    constexpr bool kRing = kMode == kProjRing;
     __shared__ __align__(16) float Fs[kPK][kFsStride];
     __shared__ __align__(16) float Ws[kPK][kGates];
     const int tid = threadIdx.x;
@@ -76,7 +80,14 @@ __device__ __forceinline__ void proj_body(const float *__restrict__ F, int64_t s
                 slot = head + k;
                 if (slot >= cap) slot -= cap;
             }
-            Fs[kk][m] = (b < B && k < kend) ? __ldg(F + (int64_t)b * sB + (int64_t)slot * sP) : 0.f;
+            int64_t row_off;
+            if constexpr (kMode == kProjRecord) {
+                const int r = b / n_w;
+                row_off = (int64_t)r * sB + (int64_t)(b - r * n_w) * step;
+            } else {
+                row_off = (int64_t)b * sB;
+            }
+            Fs[kk][m] = (b < B && k < kend) ? __ldg(F + row_off + (int64_t)slot * sP) : 0.f;
         }
 #pragma unroll
         for (int it = 0; it < (kPK * kGates) / 256; ++it) {
@@ -112,7 +123,7 @@ __device__ __forceinline__ void proj_body(const float *__restrict__ F, int64_t s
 __global__ void __launch_bounds__(256)
 proj_kernel(const float *__restrict__ F, int64_t sB, int64_t sP, const float *__restrict__ WT,
             float *__restrict__ part, int B, int L, int k_per_split) {
-    proj_body<false>(F, sB, sP, 0, L, WT, part, B, L, k_per_split);
+    proj_body<kProjRows>(F, sB, sP, 0, L, WT, part, B, L, k_per_split);
 }
 
 // the sliding scorer's projection over its feature ring of cap slots (b2cnn_slide.cu, generic path): head in [0, cap),
@@ -120,7 +131,15 @@ proj_kernel(const float *__restrict__ F, int64_t sB, int64_t sP, const float *__
 __global__ void __launch_bounds__(256)
 ring_proj_kernel(const float *__restrict__ ring, int64_t pitch, int head, int cap, const float *__restrict__ WT,
                  float *__restrict__ part, int B, int L, int k_per_split) {
-    proj_body<true>(ring, 1, pitch, head, cap, WT, part, B, L, k_per_split);
+    proj_body<kProjRing>(ring, 1, pitch, head, cap, WT, part, B, L, k_per_split);
+}
+
+// whole recordings (b2cnn_slide.cu, b2cnn_score_record): row b = window b mod n_w of recording b / n_w, whose features
+// start at feats[(b / n_w) rec_pitch + (b mod n_w) step]
+__global__ void __launch_bounds__(256)
+record_proj_kernel(const float *__restrict__ feats, int64_t rec_pitch, int n_w, int64_t step, const float *__restrict__ WT,
+                   float *__restrict__ part, int B, int L, int k_per_split) {
+    proj_body<kProjRecord>(feats, rec_pitch, 1, 0, L, WT, part, B, L, k_per_split, n_w, step);
 }
 
 // gates[b][g] = (sum_ks partial[ks][b][g] + b_ih[g]) + b_hh[g]
@@ -335,6 +354,22 @@ int launch_ring_head(const Dims &d, const HeadWeights &hw, const float *ring, in
     int n = launch_reduce_gates(partial_ws, ks_eff, B, hw, gates_ws, st, err);
     if (n < 0) return -1;
     n = launch_lstm_head(d, hw, gates_ws, B, age, n_age, B2CNN_MODE_INDEPENDENT, apply_sigmoid, out, st, err);
+    return n < 0 ? -1 : 3;
+}
+
+// launch_head of the windows of whole recordings: window w of recording r is row r n_w + w of out and of age
+int launch_record_head(const Dims &d, const HeadWeights &hw, const float *feats, int64_t rec_pitch, int n_w, int64_t step, int64_t rows,
+                       const float *age, int64_t n_age, int apply_sigmoid, float *out, float *gates_ws, float *partial_ws,
+                       cudaStream_t st, const char **err) {
+    int ks_eff;
+    const int kps = proj_split(d.L, choose_ksplit(d.L), &ks_eff);
+    record_proj_kernel<<<dim3((unsigned)((rows + kPM - 1) / kPM), ks_eff), 256, 0, st>>>(feats, rec_pitch, n_w, step, hw.wih0T,
+                                                                                        partial_ws, (int)rows, d.L, kps);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) { *err = cudaGetErrorString(e); return -1; }
+    int n = launch_reduce_gates(partial_ws, ks_eff, rows, hw, gates_ws, st, err);
+    if (n < 0) return -1;
+    n = launch_lstm_head(d, hw, gates_ws, rows, age, n_age, B2CNN_MODE_INDEPENDENT, apply_sigmoid, out, st, err);
     return n < 0 ? -1 : 3;
 }
 

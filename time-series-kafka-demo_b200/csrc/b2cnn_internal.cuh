@@ -133,6 +133,13 @@ int launch_ring_head(const Dims &d, const HeadWeights &hw, const float *ring, in
                      const float *age, int64_t n_age, int apply_sigmoid, float *out, float *gates_ws, float *partial_ws,
                      cudaStream_t st, const char **err);
 
+// launch_head of the n_w windows of each whole recording (b2cnn_slide.cu, b2cnn_score_record, generic path): row b =
+// window b mod n_w of recording b / n_w, position k at feats[(b / n_w) rec_pitch + (b mod n_w) step + k]; rows =
+// recordings x n_w; the same tiles and summation order as launch_head
+int launch_record_head(const Dims &d, const HeadWeights &hw, const float *feats, int64_t rec_pitch, int n_w, int64_t step, int64_t rows,
+                       const float *age, int64_t n_age, int apply_sigmoid, float *out, float *gates_ws, float *partial_ws,
+                       cudaStream_t st, const char **err);
+
 // b2cnn_small.cu: whole forward pass of short windows in one launch (independent windows only)
 bool small_supported(const Dims &d);
 int launch_small_forward(const Dims &d, const ConvWeights &cw, const HeadWeights &hw, const void *x, int dtype, int64_t B,

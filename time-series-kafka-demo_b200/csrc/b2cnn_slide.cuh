@@ -51,4 +51,13 @@ int slide_export(const Slide *s, const ConvWeights &cw, const int *patients, int
 int slide_import(Slide *s, const ConvWeights &cw, const int *patients, int64_t k, const b2cnn_slide_state_header &hdr, const float *feats,
                  const float *tails, const int64_t *seen_host, void *ws, int64_t ws_bytes, cudaStream_t st, const char **err);
 
+// whole recordings (b2cnn_score_record): x [B][C][pitch], out [B][n_w], n_w = (N - W) / stride + 1 (0 for N < W).
+// use_tc: the tensor-core path (the caller has checked that the handle's TcState holds the model).  The workspace size
+// is -1 (with *err) for bad arguments.
+int64_t record_workspace_bytes(const Dims &d, const TcState &tc, bool use_tc, int64_t B, int64_t N, int64_t stride, int dtype,
+                               const char **err);
+int score_record(const Dims &d, const ConvWeights &cw, const HeadWeights &hw, const TcState &tc, bool use_tc, int num_sms, const void *x,
+                 int dtype, int64_t B, int64_t N, int64_t pitch, int64_t stride, const float *age, int64_t n_age, int apply_sigmoid,
+                 float *out, void *ws, int64_t ws_bytes, cudaStream_t st, const char **err);
+
 }  // namespace b2cnn

@@ -449,4 +449,39 @@ int tc_ring_features(const TcState &s, const Dims &dseg, const ConvWeights &cw, 
     return 2;
 }
 
+// Whole recordings (b2cnn_score_record): `rows` staged rows, each of dseg.W samples (first feature at sample 0) and
+// dseg.L features, into feats[row * sB + position] (sB >= dseg.L), then the exact re-computation of every row the
+// tensor-core kernel flagged.  flags [rows] (zeroed by the caller) | list [rows] | count.  Returns the launch count.
+int tc_row_features(const TcState &s, const Dims &dseg, const ConvWeights &cw, const void *x, int64_t pitch, int dtype,
+                    int64_t rows, float *feats, int64_t sB, int *flags, int num_sms, cudaStream_t st, const char **err) {
+    const bool f32 = dtype == B2CNN_DTYPE_F32;
+    CUtensorMap tm;
+    if (make_tmap(dseg, x, pitch, rows, f32, &tm, err) != 0) return -1;
+    TcFusedParams p;
+    memset(&p, 0, sizeof p);
+    p.feats = feats; p.sB = sB; p.sP = 1; p.nanflag = flags;
+    p.bmats = reinterpret_cast<const uint8_t *>(s.d_bmats);
+    p.B = (int)rows; p.W = dseg.W; p.L = dseg.L;
+    p.tiles_per_cta = tiles_per_cta_for(dseg);
+    p.feats_per_cta = 2 * kTcBlocks * p.tiles_per_cta - 4;
+    fill_epilogue(p, dseg, cw);
+    dim3 grid((unsigned)((rows + kTcM - 1) / kTcM), (dseg.L + p.feats_per_cta - 1) / p.feats_per_cta);
+    const int key = dseg.C * 100 + (f32 ? 10 : 0) + (dseg.K1 == 10 ? 0 : 1);
+    cudaError_t e;
+    switch (key) {
+#define ROW_CASE(CC, FF, AA) case CC * 100 + FF * 10 + AA: e = launch_stream<CC, FF ? 1 : 3, AA, FF == 1, kOutFeatures>(tm, p, grid, st); break;
+        ROW_CASE(1, 0, 0) ROW_CASE(2, 0, 0) ROW_CASE(3, 0, 0) ROW_CASE(1, 0, 1) ROW_CASE(2, 0, 1) ROW_CASE(3, 0, 1)
+        ROW_CASE(1, 1, 0) ROW_CASE(2, 1, 0) ROW_CASE(3, 1, 0) ROW_CASE(1, 1, 1) ROW_CASE(2, 1, 1) ROW_CASE(3, 1, 1)
+#undef ROW_CASE
+        default: *err = "no feature-row instantiation for this channel count"; return -1;
+    }
+    if (e != cudaSuccess) { *err = cudaGetErrorString(e); return -1; }
+    int *list = flags + rows, *count = list + rows;
+    tc_compact_flags_kernel<<<(unsigned)((rows + 255) / 256), 256, 0, st>>>(flags, (int)rows, list, count);
+    if (cudaGetLastError() != cudaSuccess) { *err = "flag compaction launch"; return -1; }
+    // flagged rows (a NaN or inf sample): every feature of the row again, exact fp32 (the generic front end)
+    const int n = launch_frontend_generic_listed(dseg, cw, x, dtype, rows, feats, sB, 1, list, count, st, num_sms, err);
+    return n < 0 ? n : 2 + n;
+}
+
 }  // namespace b2cnn

@@ -17,6 +17,7 @@ libb2cnn.so (hand-written sm_90a kernels) through ctypes.  No CUDA device -> Run
 from __future__ import annotations
 
 import ctypes
+import operator
 from typing import Optional
 
 import torch
@@ -353,6 +354,77 @@ class B200MyCNN(nn.Module):
         if age.numel() not in (1, B):
             raise RuntimeError(f"age must be a scalar or have {B} elements")
         return self._run(window_tensor, age, m, return_prob)
+
+    def check_record_args(self, records, stride, age=None, path: str = "auto"):
+        """Validates ``predict_record``'s arguments without touching the library; returns ``(stride, age)`` with age a
+        float32 vector of 1 or B elements."""
+        C = self.arch.in_channels
+        if not torch.is_tensor(records) or records.dim() != 3 or records.shape[1] != C:
+            got = tuple(records.shape) if torch.is_tensor(records) else type(records).__name__
+            raise ValueError(f"expected records [B, {C}, N], got {got}")
+        if records.dtype not in (torch.float32, torch.bfloat16):
+            raise ValueError(f"records must be float32 or bfloat16, got {records.dtype}")
+        if records.shape[0] < 1:
+            raise ValueError("records must hold at least one recording")
+        if path not in _PATHS:
+            raise ValueError(f"path must be one of {sorted(_PATHS)}, got {path!r}")
+        if isinstance(stride, bool) or not isinstance(stride, int):
+            try:
+                stride = operator.index(stride)
+            except TypeError:
+                raise ValueError(f"stride must be an integer, got {type(stride).__name__}") from None
+        F = 4 if path == "tensorcore" else self.arch.pool_s ** 2          # the feature stride in samples
+        if stride < 1 or stride % F:
+            raise ValueError(f"stride must be a positive multiple of the feature stride {F}, got {stride}")
+        if age is None:
+            age = 65.0
+        age = (age if torch.is_tensor(age) else torch.tensor(age, dtype=torch.float32)).detach().reshape(-1).float()
+        if age.numel() not in (1, records.shape[0]):
+            raise ValueError(f"age must be a scalar or have {records.shape[0]} elements (one per recording), got {age.numel()}")
+        return stride, age
+
+    @torch.no_grad()
+    def predict_record(self, records: torch.Tensor, stride: int, age=None, return_prob: bool = False,
+                       path: str = "auto") -> torch.Tensor:
+        """Every window of whole recordings in one call: ``records`` ``[B, C, N]`` (float32 or bfloat16; contiguous or
+        a row-padded view), windows of the model's W samples starting every ``stride`` samples.  Returns ``[B, n_w]``,
+        ``n_w = (N - W) // stride + 1`` (0 when N < W): element ``[b, w]`` is ``predict(records[b, :, w*stride :
+        w*stride + W], age[b])`` (the probability with ``return_prob``).  ``age``: a scalar or one per recording
+        (default 65.0).  Each window feature is computed once, however many windows share it.
+
+        ``path``: ``"tensorcore"`` (the models a tensor-core ``SlidingScorer`` holds), ``"generic"`` (every model; its
+        logits are bit-identical to ``predict()`` with ``path="generic"`` and ``small_kernel=0``) or ``"auto"``.
+        ``stride`` must be a multiple of the feature stride ``pool_s ** 2`` (4 on the tensor-core path); it may exceed
+        W.  ``bin/utils.py``'s ``create_batch`` drops the last window when ``(N - W) % stride == 0``: ``out[:, :-1]`` is
+        its set then."""
+        stride, age = self.check_record_args(records, stride, age, path)
+        B, N, W = records.shape[0], records.shape[2], self.arch.window
+        lib, h = self._ensure_handle()
+        dev = self._handle_device
+        n_w = (N - W) // stride + 1 if N >= W else 0
+        if n_w == 0:
+            return torch.empty(B, 0, dtype=torch.float32, device=dev)
+        if records.device != dev:
+            records = records.to(dev)
+        age = age.to(dev).contiguous()
+        C = self.arch.in_channels
+        if records.is_contiguous():
+            pitch = N
+        elif records.stride(2) == 1 and records.stride(1) >= N and (B == 1 or records.stride(0) == C * records.stride(1)):
+            pitch = records.stride(1)                            # a row-padded view, read in place
+        else:
+            records, pitch = records.contiguous(), N
+        dtype = capi.DTYPE_BF16 if records.dtype == torch.bfloat16 else capi.DTYPE_F32
+        out = torch.empty(B, n_w, dtype=torch.float32, device=dev)
+        with torch.cuda.device(dev):
+            need = int(lib.b2cnn_record_workspace_bytes(h, B, N, pitch, stride, dtype, _PATHS[path]))
+            if need < 0:
+                raise RuntimeError(capi.last_error())
+            ws = torch.empty(max(need, 256), dtype=torch.uint8, device=dev)
+            capi.check(lib.b2cnn_score_record(h, records.data_ptr(), dtype, B, N, pitch, stride, _PATHS[path], age.data_ptr(),
+                                              age.numel(), int(return_prob), out.data_ptr(), ws.data_ptr(), ws.numel(),
+                                              torch.cuda.current_stream().cuda_stream), "b2cnn_score_record")
+        return out
 
     def call_plan(self, window_tensor: torch.Tensor, age: torch.Tensor, mode: str = "independent",
                   return_prob: bool = False):
