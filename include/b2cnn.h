@@ -302,11 +302,28 @@ int b2cnn_slide_samples_seen(b2cnn_slide *slide, int64_t *seen, void *stream);
  *                        dtype, path, pitch < N, n_age or more than 2^25 rows (B n_w, or B times the folded rows per
  *                        recording); B2CNN_ESTATE for a workspace that is missing, not 256-byte aligned or smaller than
  *                        b2cnn_record_workspace_bytes; B2CNN_EARCH as above.
- *   b2cnn_record_workspace_bytes  DEVICE workspace of that call (-1 for bad arguments, with b2cnn_last_error). */
+ *   b2cnn_record_workspace_bytes  DEVICE workspace of that call (-1 for bad arguments, with b2cnn_last_error).
+ *   b2cnn_score_record_ex  the same call with a batch mode.  mode = B2CNN_MODE_INDEPENDENT: exactly b2cnn_score_record.
+ *                        mode = B2CNN_MODE_SEQUENCE: out[b] is what model(windows_b, age_b) returns, windows_b the n_w
+ *                        windows of recording b in order -- the LSTM carried across a recording's windows (batch as
+ *                        sequence, as bin/utils.py run_model scores one recording), from the zero state at each
+ *                        recording's first window and never from one recording to the next.  The scan is causal:
+ *                        out[b][0 .. k-1] do not depend on windows k and later, and a NaN window makes its own and
+ *                        every later output of its recording NaN.  On the generic path each row is bit-identical to
+ *                        b2cnn_forward (path = generic, small_kernel = 0, mode = sequence) on the recording's windows.
+ *                        A fixed number of launches whatever B, N and stride; nothing allocated, nothing synchronised.
+ *                        Every check of b2cnn_score_record runs before the first launch, and a mode that is neither
+ *                        value is B2CNN_EINVAL.  Tensor-core sequence mode needs B n_w x 256 bytes more workspace than
+ *                        independent mode: size it with b2cnn_record_workspace_bytes_ex and the same mode. */
 int64_t b2cnn_record_workspace_bytes(b2cnn_handle *h, int64_t B, int64_t N, int64_t pitch, int64_t stride, int dtype, int path);
 int b2cnn_score_record(b2cnn_handle *h, const void *x, int dtype, int64_t B, int64_t N, int64_t pitch, int64_t stride, int path,
                        const float *age, int64_t n_age, int apply_sigmoid, float *out, void *workspace, int64_t workspace_bytes,
                        void *stream);
+int64_t b2cnn_record_workspace_bytes_ex(b2cnn_handle *h, int64_t B, int64_t N, int64_t pitch, int64_t stride, int dtype, int path,
+                                        int mode);
+int b2cnn_score_record_ex(b2cnn_handle *h, const void *x, int dtype, int64_t B, int64_t N, int64_t pitch, int64_t stride, int path,
+                          int mode, const float *age, int64_t n_age, int apply_sigmoid, float *out, void *workspace,
+                          int64_t workspace_bytes, void *stream);
 
 /* Export and import of patients (a restart, beds moved to another scorer or GPU, new LSTM / head weights).  A
  * patient's state is its current window's L features in window order, raw and unmasked (for a complete window

@@ -33,7 +33,7 @@ SYMBOLS = ("b2cnn_l_out", "b2cnn_weight_count", "b2cnn_create", "b2cnn_destroy",
            "b2cnn_slide_create_path", "b2cnn_slide_path",
            "b2cnn_slide_describe_state", "b2cnn_slide_state_workspace_bytes", "b2cnn_slide_export", "b2cnn_slide_import",
            "b2cnn_slide_set_heads", "b2cnn_slide_set_heads_ex", "b2cnn_slide_n_heads", "b2cnn_slide_push_heads",
-           "b2cnn_record_workspace_bytes", "b2cnn_score_record",
+           "b2cnn_record_workspace_bytes", "b2cnn_score_record", "b2cnn_record_workspace_bytes_ex", "b2cnn_score_record_ex",
            "b2cnn_decode_sample_messages", "b2cnn_decode_array_messages", "b2cnn_parse_decimal", "b2cnn_frame_check")
 
 
@@ -161,6 +161,11 @@ def load_library() -> ctypes.CDLL:
     lib.b2cnn_record_workspace_bytes.restype = c_i64
     lib.b2cnn_score_record.argtypes = [c_vp, c_vp, c_int, c_i64, c_i64, c_i64, c_i64, c_int, c_vp, c_i64, c_int, c_vp, c_vp, c_i64, c_vp]
     lib.b2cnn_score_record.restype = c_int
+    lib.b2cnn_record_workspace_bytes_ex.argtypes = [c_vp, c_i64, c_i64, c_i64, c_i64, c_int, c_int, c_int]
+    lib.b2cnn_record_workspace_bytes_ex.restype = c_i64
+    lib.b2cnn_score_record_ex.argtypes = [c_vp, c_vp, c_int, c_i64, c_i64, c_i64, c_i64, c_int, c_int, c_vp, c_i64, c_int, c_vp, c_vp,
+                                          c_i64, c_vp]
+    lib.b2cnn_score_record_ex.restype = c_int
     lib.b2cnn_decode_sample_messages.argtypes = [c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_i64, c_i32, c_vp, c_vp]
     lib.b2cnn_decode_sample_messages.restype = c_int
     lib.b2cnn_decode_array_messages.argtypes = [c_vp, c_vp, c_i64, c_i32, c_vp, c_vp, c_vp, c_vp]

@@ -825,29 +825,53 @@ static int record_path(const char *fn, const b2cnn_handle *h, int dtype, int pat
     return B2CNN_OK;
 }
 
-extern "C" int64_t b2cnn_record_workspace_bytes(b2cnn_handle *h, int64_t B, int64_t N, int64_t pitch, int64_t stride, int dtype, int path) {
+static int64_t record_workspace(const char *fn, b2cnn_handle *h, int64_t B, int64_t N, int64_t pitch, int64_t stride, int dtype, int path,
+                                int mode) {
     bool tc = false;
-    if (record_path("b2cnn_record_workspace_bytes", h, dtype, path, &tc) != B2CNN_OK) return -1;
-    if (pitch < N) { fail(B2CNN_EINVAL, "b2cnn_record_workspace_bytes: pitch must be >= the recording length"); return -1; }
+    if (record_path(fn, h, dtype, path, &tc) != B2CNN_OK) return -1;
+    if (pitch < N) { fail(B2CNN_EINVAL, std::string(fn) + ": pitch must be >= the recording length"); return -1; }
     const char *err = "";
-    const int64_t n = record_workspace_bytes(h->d, h->tc, tc, B, N, stride, dtype, &err);
-    if (n < 0) fail(B2CNN_EINVAL, std::string("b2cnn_record_workspace_bytes: ") + err);
+    const int64_t n = record_workspace_bytes(h->d, h->tc, tc, B, N, stride, dtype, mode, &err);
+    if (n < 0) fail(B2CNN_EINVAL, std::string(fn) + ": " + err);
     return n;
+}
+
+extern "C" int64_t b2cnn_record_workspace_bytes(b2cnn_handle *h, int64_t B, int64_t N, int64_t pitch, int64_t stride, int dtype, int path) {
+    return record_workspace("b2cnn_record_workspace_bytes", h, B, N, pitch, stride, dtype, path, B2CNN_MODE_INDEPENDENT);
+}
+
+extern "C" int64_t b2cnn_record_workspace_bytes_ex(b2cnn_handle *h, int64_t B, int64_t N, int64_t pitch, int64_t stride, int dtype, int path,
+                                                   int mode) {
+    return record_workspace("b2cnn_record_workspace_bytes_ex", h, B, N, pitch, stride, dtype, path, mode);
+}
+
+static int record_score(const char *fn, b2cnn_handle *h, const void *x, int dtype, int64_t B, int64_t N, int64_t pitch, int64_t stride,
+                        int path, int mode, const float *age, int64_t n_age, int apply_sigmoid, float *out, void *workspace,
+                        int64_t workspace_bytes, void *stream) {
+    bool tc = false;
+    if (int rc = record_path(fn, h, dtype, path, &tc)) return rc;
+    if (!x || !age || !out) return fail(B2CNN_EINVAL, std::string(fn) + ": null argument");
+    DEVICE_GUARD(h->device);
+    const char *err = "";
+    const int rc = score_record(h->d, h->cw, h->hw, h->tc, tc, h->num_sms, x, dtype, B, N, pitch, stride, mode, age, n_age, apply_sigmoid,
+                                out, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream), &err);
+    if (rc != B2CNN_OK) return fail(rc, std::string(fn) + ": " + err);
+    h->last_path = tc ? B2CNN_PATH_TENSORCORE : B2CNN_PATH_GENERIC;
+    return B2CNN_OK;
 }
 
 extern "C" int b2cnn_score_record(b2cnn_handle *h, const void *x, int dtype, int64_t B, int64_t N, int64_t pitch, int64_t stride, int path,
                                   const float *age, int64_t n_age, int apply_sigmoid, float *out, void *workspace, int64_t workspace_bytes,
                                   void *stream) {
-    bool tc = false;
-    if (int rc = record_path("b2cnn_score_record", h, dtype, path, &tc)) return rc;
-    if (!x || !age || !out) return fail(B2CNN_EINVAL, "b2cnn_score_record: null argument");
-    DEVICE_GUARD(h->device);
-    const char *err = "";
-    const int rc = score_record(h->d, h->cw, h->hw, h->tc, tc, h->num_sms, x, dtype, B, N, pitch, stride, age, n_age, apply_sigmoid, out,
-                                workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream), &err);
-    if (rc != B2CNN_OK) return fail(rc, std::string("b2cnn_score_record: ") + err);
-    h->last_path = tc ? B2CNN_PATH_TENSORCORE : B2CNN_PATH_GENERIC;
-    return B2CNN_OK;
+    return record_score("b2cnn_score_record", h, x, dtype, B, N, pitch, stride, path, B2CNN_MODE_INDEPENDENT, age, n_age, apply_sigmoid,
+                        out, workspace, workspace_bytes, stream);
+}
+
+extern "C" int b2cnn_score_record_ex(b2cnn_handle *h, const void *x, int dtype, int64_t B, int64_t N, int64_t pitch, int64_t stride, int path,
+                                     int mode, const float *age, int64_t n_age, int apply_sigmoid, float *out, void *workspace,
+                                     int64_t workspace_bytes, void *stream) {
+    return record_score("b2cnn_score_record_ex", h, x, dtype, B, N, pitch, stride, path, mode, age, n_age, apply_sigmoid, out, workspace,
+                        workspace_bytes, stream);
 }
 
 // ---- host-pointer entry: chunked H2D overlapped with compute -----------------------------

@@ -5,8 +5,9 @@
 //   proj_kernel          [B x L] x [L x 64] fp32 tiled GEMM with split-K partials
 //   reduce_gates_kernel  sums the split-K partials in fixed order (deterministic) + biases
 //   head_independent     one thread per window, LSTM from the zero state (predictStream.py:157)
-//   head_sequence        one warp scans the batch axis carrying (h, c) -- the reference's
-//                        model(x_batch) semantics for B > 1 (models.py:29-30, utils.py:249)
+//   head_sequence        one warp per segment scans its rows carrying (h, c) -- the reference's
+//                        model(x_batch) semantics for B > 1 (models.py:29-30, utils.py:249), over
+//                        the whole batch or over each recording's windows (utils.py:671-692)
 #include "b2cnn_internal.cuh"
 #include "b2cnn_head_dev.cuh"
 
@@ -238,13 +239,19 @@ head_reduce_independent_kernel(const float *__restrict__ part, int slices, HeadW
     }
 }
 
-// One warp scans the B rows sequentially.  Lane l owns gate rows l and l+32 of every weight
-// matrix (registers); units' (h, c) are held twice, by lanes u and u+16.
+// One warp (one CTA) per segment: CTA s scans rows s seg_len .. s seg_len + seg_len - 1 of gates0, age (n_age > 1) and
+// out sequentially from the zero state.  forward's sequence mode is one segment of B rows; b2cnn_score_record's is one
+// segment per recording, of its n_w windows.  Lane l owns gate rows l and l+32 of every weight matrix (registers); units'
+// (h, c) are held twice, by lanes u and u+16.
 __global__ void __launch_bounds__(32)
 head_sequence_kernel(const float *__restrict__ gates0, HeadWeights hw, const float *__restrict__ age,
-                     int64_t n_age, float coef, int apply_sigmoid, float *__restrict__ out, int64_t B) {
+                     int64_t n_age, float coef, int apply_sigmoid, float *__restrict__ out, int64_t seg_len) {
     const int l = threadIdx.x, u = l & 15;
     const bool lo = l < 16;
+    const int64_t row0 = (int64_t)blockIdx.x * seg_len, B = seg_len;
+    gates0 += row0 * kGates;
+    out += row0;
+    if (n_age != 1) age += row0;
     float whh0a[kHidden], whh0b[kHidden], wih1a[kHidden], wih1b[kHidden], whh1a[kHidden], whh1b[kHidden];
 #pragma unroll
     for (int k = 0; k < kHidden; ++k) {
@@ -357,9 +364,10 @@ int launch_ring_head(const Dims &d, const HeadWeights &hw, const float *ring, in
     return n < 0 ? -1 : 3;
 }
 
-// launch_head of the windows of whole recordings: window w of recording r is row r n_w + w of out and of age
+// launch_head of the windows of whole recordings: window w of recording r is row r n_w + w of out and of age; in
+// sequence mode each recording's n_w rows are one LSTM scan
 int launch_record_head(const Dims &d, const HeadWeights &hw, const float *feats, int64_t rec_pitch, int n_w, int64_t step, int64_t rows,
-                       const float *age, int64_t n_age, int apply_sigmoid, float *out, float *gates_ws, float *partial_ws,
+                       const float *age, int64_t n_age, int mode, int apply_sigmoid, float *out, float *gates_ws, float *partial_ws,
                        cudaStream_t st, const char **err) {
     int ks_eff;
     const int kps = proj_split(d.L, choose_ksplit(d.L), &ks_eff);
@@ -369,7 +377,9 @@ int launch_record_head(const Dims &d, const HeadWeights &hw, const float *feats,
     if (e != cudaSuccess) { *err = cudaGetErrorString(e); return -1; }
     int n = launch_reduce_gates(partial_ws, ks_eff, rows, hw, gates_ws, st, err);
     if (n < 0) return -1;
-    n = launch_lstm_head(d, hw, gates_ws, rows, age, n_age, B2CNN_MODE_INDEPENDENT, apply_sigmoid, out, st, err);
+    n = mode == B2CNN_MODE_SEQUENCE
+            ? launch_sequence_segments(d, hw, gates_ws, rows / n_w, n_w, age, n_age, apply_sigmoid, out, st, err)
+            : launch_lstm_head(d, hw, gates_ws, rows, age, n_age, B2CNN_MODE_INDEPENDENT, apply_sigmoid, out, st, err);
     return n < 0 ? -1 : 3;
 }
 
@@ -402,8 +412,17 @@ int launch_lstm_head(const Dims &d, const HeadWeights &hw, const float *gates, i
         head_independent_kernel<<<(unsigned)((B + 127) / 128), 128, 0, st>>>(gates, hw, age, n_age, d.age_coef,
                                                                              apply_sigmoid, out, B);
     } else {
-        head_sequence_kernel<<<1, 32, 0, st>>>(gates, hw, age, n_age, d.age_coef, apply_sigmoid, out, B);
+        return launch_sequence_segments(d, hw, gates, 1, B, age, n_age, apply_sigmoid, out, st, err);
     }
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) { *err = cudaGetErrorString(e); return -1; }
+    return 1;
+}
+
+// n_seg independent LSTM scans of seg_len consecutive rows each, one warp per segment
+int launch_sequence_segments(const Dims &d, const HeadWeights &hw, const float *gates, int64_t n_seg, int64_t seg_len, const float *age,
+                             int64_t n_age, int apply_sigmoid, float *out, cudaStream_t st, const char **err) {
+    head_sequence_kernel<<<(unsigned)n_seg, 32, 0, st>>>(gates, hw, age, n_age, d.age_coef, apply_sigmoid, out, seg_len);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) { *err = cudaGetErrorString(e); return -1; }
     return 1;

@@ -118,6 +118,10 @@ int launch_reduce_gates(const float *partial, int slices, int64_t B, const HeadW
                         cudaStream_t st, const char **err);
 int launch_lstm_head(const Dims &d, const HeadWeights &hw, const float *gates, int64_t B, const float *age,
                      int64_t n_age, int mode, int apply_sigmoid, float *out, cudaStream_t st, const char **err);
+// sequence mode over n_seg segments of seg_len consecutive rows of gates [n_seg seg_len][64], age (n_age = 1 or n_seg
+// seg_len) and out, each scanned from the zero state; launch_lstm_head's sequence mode is one segment of B rows
+int launch_sequence_segments(const Dims &d, const HeadWeights &hw, const float *gates, int64_t n_seg, int64_t seg_len, const float *age,
+                             int64_t n_age, int apply_sigmoid, float *out, cudaStream_t st, const char **err);
 
 int launch_reduce_lstm_head(const Dims &d, const HeadWeights &hw, const float *partial, int slices, int64_t B,
                             const float *age, int64_t n_age, int apply_sigmoid, float *out, cudaStream_t st, const char **err,
@@ -135,9 +139,10 @@ int launch_ring_head(const Dims &d, const HeadWeights &hw, const float *ring, in
 
 // launch_head of the n_w windows of each whole recording (b2cnn_slide.cu, b2cnn_score_record, generic path): row b =
 // window b mod n_w of recording b / n_w, position k at feats[(b / n_w) rec_pitch + (b mod n_w) step + k]; rows =
-// recordings x n_w; the same tiles and summation order as launch_head
+// recordings x n_w; the same tiles and summation order as launch_head.  mode B2CNN_MODE_SEQUENCE: one LSTM scan per
+// recording over its n_w windows (launch_sequence_segments) instead of independent windows
 int launch_record_head(const Dims &d, const HeadWeights &hw, const float *feats, int64_t rec_pitch, int n_w, int64_t step, int64_t rows,
-                       const float *age, int64_t n_age, int apply_sigmoid, float *out, float *gates_ws, float *partial_ws,
+                       const float *age, int64_t n_age, int mode, int apply_sigmoid, float *out, float *gates_ws, float *partial_ws,
                        cudaStream_t st, const char **err);
 
 // b2cnn_small.cu: whole forward pass of short windows in one launch (independent windows only)

@@ -1323,28 +1323,35 @@ int slide_import(Slide *s, const ConvWeights &cw, const int *patients, int64_t k
 //     slide_record_proj_kernel, the arithmetic of slide_ring_proj_kernel per window with 128 windows per CTA sharing
 //     each W_ih chunk; generic path: launch_record_head (proj_body with a per-row base), predict()'s tiles and order.
 //   * head: launch_reduce_lstm_head (tensor cores) or reduce_gates + head_independent (generic) over the M rows, with
-//     each recording's age repeated over its windows.
+//     each recording's age repeated over its windows.  Sequence mode (the LSTM carried over each recording's windows,
+//     utils.run_model's batch-as-sequence call per recording): reduce_gates over the same partials (tc.n_ranges slices
+//     on the tensor-core path, as forward's tensor-core sequence mode sums them), then head_sequence with one warp per
+//     recording scanning its n_w gate rows.
 // Launches per call: stage, tensor-core front end, flag compaction, exact re-computation, age, projection, head
-// (tensor-core path, plus the flag memset) or stage, front end, age, projection, reduction, head (generic path) --
-// whatever B, N and S.
+// (tensor-core path, plus the flag memset; reduction + scan in sequence mode) or stage, front end, age, projection,
+// reduction, head (generic path) -- whatever B, N and S.
 constexpr int64_t kRecRowFeats = 4096;
 
 struct RecordPlan {
-    bool tc;
+    bool tc, seq;
     int F, R, ranges;
     int64_t n_w, L_N, K, nr, rows, Lp, row_len, Kp, step, M;
     size_t stage, feats, flags, partial, gates, age, total;
 };
 
 // the plan of a call; false with *err and *code when an argument is out of range
-static bool record_plan(const Dims &d, const TcState &tc, bool use_tc, int64_t B, int64_t N, int64_t stride, int dtype, RecordPlan *o,
-                        int *code, const char **err) {
+static bool record_plan(const Dims &d, const TcState &tc, bool use_tc, int64_t B, int64_t N, int64_t stride, int dtype, int mode,
+                        RecordPlan *o, int *code, const char **err) {
     RecordPlan &p = *o;
     memset(&p, 0, sizeof p);
     p.tc = use_tc;
+    p.seq = mode == B2CNN_MODE_SEQUENCE;
     p.F = d.PS * d.PS;
     p.R = d.PS * (d.PK + d.K2 - 2) + d.PK + d.K1 - 1;
     *code = B2CNN_EINVAL;
+    if (mode != B2CNN_MODE_INDEPENDENT && mode != B2CNN_MODE_SEQUENCE) {
+        *err = "mode must be B2CNN_MODE_INDEPENDENT or B2CNN_MODE_SEQUENCE"; return false;
+    }
     if (B < 1 || B > 0x7fffffff) { *err = "the recording count must be in [1, 2^31)"; return false; }
     if (N < 0) { *err = "the recording length must be >= 0"; return false; }
     if (stride < 1 || stride % p.F != 0) {
@@ -1378,7 +1385,7 @@ static bool record_plan(const Dims &d, const TcState &tc, bool use_tc, int64_t B
     p.feats = al256(sizeof(float) * (size_t)(B * p.Lp));
     p.flags = use_tc ? al256(sizeof(int) * (size_t)(2 * p.rows + 1)) : 0;
     p.partial = al256(sizeof(float) * (size_t)p.ranges * (size_t)p.M * kGates);
-    p.gates = use_tc ? 0 : al256(sizeof(float) * (size_t)p.M * kGates);
+    p.gates = use_tc && !p.seq ? 0 : al256(sizeof(float) * (size_t)p.M * kGates);   // the fused tensor-core head sums in registers
     p.age = al256(sizeof(float) * (size_t)p.M);
     p.total = p.stage + p.feats + p.flags + p.partial + p.gates + p.age;
     *code = B2CNN_OK;
@@ -1527,20 +1534,20 @@ __global__ void __launch_bounds__(kRpThreads) slide_record_proj_kernel(const __g
         }
 }
 
-int64_t record_workspace_bytes(const Dims &d, const TcState &tc, bool use_tc, int64_t B, int64_t N, int64_t stride, int dtype,
+int64_t record_workspace_bytes(const Dims &d, const TcState &tc, bool use_tc, int64_t B, int64_t N, int64_t stride, int dtype, int mode,
                                const char **err) {
     RecordPlan p;
     int code;
-    if (!record_plan(d, tc, use_tc, B, N, stride, dtype, &p, &code, err)) return -1;
+    if (!record_plan(d, tc, use_tc, B, N, stride, dtype, mode, &p, &code, err)) return -1;
     return (int64_t)p.total;
 }
 
 int score_record(const Dims &d, const ConvWeights &cw, const HeadWeights &hw, const TcState &tc, bool use_tc, int num_sms, const void *x,
-                 int dtype, int64_t B, int64_t N, int64_t pitch, int64_t stride, const float *age, int64_t n_age, int apply_sigmoid,
+                 int dtype, int64_t B, int64_t N, int64_t pitch, int64_t stride, int mode, const float *age, int64_t n_age, int apply_sigmoid,
                  float *out, void *ws, int64_t ws_bytes, cudaStream_t st, const char **err) {
     RecordPlan p;
     int code;
-    if (!record_plan(d, tc, use_tc, B, N, stride, dtype, &p, &code, err)) return code;
+    if (!record_plan(d, tc, use_tc, B, N, stride, dtype, mode, &p, &code, err)) return code;
     if (pitch < N || pitch < 1) { *err = "pitch must be >= the recording length"; return B2CNN_EINVAL; }
     if (n_age != 1 && n_age != B) { *err = "age must have 1 or B elements"; return B2CNN_EINVAL; }
     if (p.n_w == 0) return B2CNN_OK;
@@ -1589,7 +1596,7 @@ int score_record(const Dims &d, const ConvWeights &cw, const HeadWeights &hw, co
     if (cudaGetLastError() != cudaSuccess) { *err = "age launch"; return B2CNN_ECUDA; }
     // ---- projection + head over the B n_w windows
     if (!use_tc) {
-        if (launch_record_head(d, hw, feats, p.Lp, (int)p.n_w, p.step, p.M, ages, p.M, apply_sigmoid, out, gates, partial, st, err) < 0)
+        if (launch_record_head(d, hw, feats, p.Lp, (int)p.n_w, p.step, p.M, ages, p.M, mode, apply_sigmoid, out, gates, partial, st, err) < 0)
             return B2CNN_ECUDA;
         return B2CNN_OK;
     }
@@ -1603,6 +1610,12 @@ int score_record(const Dims &d, const ConvWeights &cw, const HeadWeights &hw, co
     }
     slide_record_proj_kernel<<<dim3((unsigned)((p.M + kRpM - 1) / kRpM), (unsigned)tc.n_ranges), kRpThreads, kRecProjSmem, st>>>(rp);
     if (cudaGetLastError() != cudaSuccess) { *err = "projection launch"; return B2CNN_ECUDA; }
+    if (p.seq) {
+        if (launch_reduce_gates(partial, tc.n_ranges, p.M, hw, gates, st, err) < 0 ||
+            launch_sequence_segments(d, hw, gates, B, p.n_w, ages, p.M, apply_sigmoid, out, st, err) < 0)
+            return B2CNN_ECUDA;
+        return B2CNN_OK;
+    }
     if (launch_reduce_lstm_head(d, hw, partial, tc.n_ranges, p.M, ages, p.M, apply_sigmoid, out, st, err) < 0) return B2CNN_ECUDA;
     return B2CNN_OK;
 }

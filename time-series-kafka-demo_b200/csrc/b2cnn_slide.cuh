@@ -53,11 +53,12 @@ int slide_import(Slide *s, const ConvWeights &cw, const int *patients, int64_t k
 
 // whole recordings (b2cnn_score_record): x [B][C][pitch], out [B][n_w], n_w = (N - W) / stride + 1 (0 for N < W).
 // use_tc: the tensor-core path (the caller has checked that the handle's TcState holds the model).  The workspace size
-// is -1 (with *err) for bad arguments.
-int64_t record_workspace_bytes(const Dims &d, const TcState &tc, bool use_tc, int64_t B, int64_t N, int64_t stride, int dtype,
+// is -1 (with *err) for bad arguments.  mode: B2CNN_MODE_INDEPENDENT (every window from the zero LSTM state) or
+// B2CNN_MODE_SEQUENCE (the LSTM carried over each recording's windows in order, from the zero state per recording).
+int64_t record_workspace_bytes(const Dims &d, const TcState &tc, bool use_tc, int64_t B, int64_t N, int64_t stride, int dtype, int mode,
                                const char **err);
 int score_record(const Dims &d, const ConvWeights &cw, const HeadWeights &hw, const TcState &tc, bool use_tc, int num_sms, const void *x,
-                 int dtype, int64_t B, int64_t N, int64_t pitch, int64_t stride, const float *age, int64_t n_age, int apply_sigmoid,
+                 int dtype, int64_t B, int64_t N, int64_t pitch, int64_t stride, int mode, const float *age, int64_t n_age, int apply_sigmoid,
                  float *out, void *ws, int64_t ws_bytes, cudaStream_t st, const char **err);
 
 }  // namespace b2cnn

@@ -355,9 +355,11 @@ class B200MyCNN(nn.Module):
             raise RuntimeError(f"age must be a scalar or have {B} elements")
         return self._run(window_tensor, age, m, return_prob)
 
-    def check_record_args(self, records, stride, age=None, path: str = "auto"):
+    def check_record_args(self, records, stride, age=None, path: str = "auto", mode: str = "independent"):
         """Validates ``predict_record``'s arguments without touching the library; returns ``(stride, age)`` with age a
         float32 vector of 1 or B elements."""
+        if not isinstance(mode, str) or mode not in ("independent", "sequence"):
+            raise ValueError(f"mode must be 'independent' or 'sequence', got {mode!r}")
         C = self.arch.in_channels
         if not torch.is_tensor(records) or records.dim() != 3 or records.shape[1] != C:
             got = tuple(records.shape) if torch.is_tensor(records) else type(records).__name__
@@ -385,19 +387,25 @@ class B200MyCNN(nn.Module):
 
     @torch.no_grad()
     def predict_record(self, records: torch.Tensor, stride: int, age=None, return_prob: bool = False,
-                       path: str = "auto") -> torch.Tensor:
+                       path: str = "auto", mode: str = "independent") -> torch.Tensor:
         """Every window of whole recordings in one call: ``records`` ``[B, C, N]`` (float32 or bfloat16; contiguous or
         a row-padded view), windows of the model's W samples starting every ``stride`` samples.  Returns ``[B, n_w]``,
         ``n_w = (N - W) // stride + 1`` (0 when N < W): element ``[b, w]`` is ``predict(records[b, :, w*stride :
         w*stride + W], age[b])`` (the probability with ``return_prob``).  ``age``: a scalar or one per recording
         (default 65.0).  Each window feature is computed once, however many windows share it.
 
+        ``mode="sequence"``: row ``b`` is instead ``model(windows_b, age_b)``, ``windows_b`` the recording's ``n_w``
+        windows in order -- the LSTM carried across one recording's windows, as ``bin/utils.py``'s ``run_model`` scores
+        a recording; the state starts at zero for every recording and never passes from one to the next.  The scan is
+        causal (the first k outputs do not depend on later windows), and a NaN window makes its own and every later
+        output of its recording NaN.
+
         ``path``: ``"tensorcore"`` (the models a tensor-core ``SlidingScorer`` holds), ``"generic"`` (every model; its
-        logits are bit-identical to ``predict()`` with ``path="generic"`` and ``small_kernel=0``) or ``"auto"``.
-        ``stride`` must be a multiple of the feature stride ``pool_s ** 2`` (4 on the tensor-core path); it may exceed
-        W.  ``bin/utils.py``'s ``create_batch`` drops the last window when ``(N - W) % stride == 0``: ``out[:, :-1]`` is
-        its set then."""
-        stride, age = self.check_record_args(records, stride, age, path)
+        logits are bit-identical to ``predict()`` with ``path="generic"`` and ``small_kernel=0``, per recording with
+        ``mode="sequence"`` in sequence mode) or ``"auto"``.  ``stride`` must be a multiple of the feature stride
+        ``pool_s ** 2`` (4 on the tensor-core path); it may exceed W.  ``bin/utils.py``'s ``create_batch`` drops the
+        last window when ``(N - W) % stride == 0``: ``out[:, :-1]`` is its set then, in either mode."""
+        stride, age = self.check_record_args(records, stride, age, path, mode)
         B, N, W = records.shape[0], records.shape[2], self.arch.window
         lib, h = self._ensure_handle()
         dev = self._handle_device
@@ -416,14 +424,15 @@ class B200MyCNN(nn.Module):
             records, pitch = records.contiguous(), N
         dtype = capi.DTYPE_BF16 if records.dtype == torch.bfloat16 else capi.DTYPE_F32
         out = torch.empty(B, n_w, dtype=torch.float32, device=dev)
+        m = capi.MODE_SEQUENCE if mode == "sequence" else capi.MODE_INDEPENDENT
         with torch.cuda.device(dev):
-            need = int(lib.b2cnn_record_workspace_bytes(h, B, N, pitch, stride, dtype, _PATHS[path]))
+            need = int(lib.b2cnn_record_workspace_bytes_ex(h, B, N, pitch, stride, dtype, _PATHS[path], m))
             if need < 0:
                 raise RuntimeError(capi.last_error())
             ws = torch.empty(max(need, 256), dtype=torch.uint8, device=dev)
-            capi.check(lib.b2cnn_score_record(h, records.data_ptr(), dtype, B, N, pitch, stride, _PATHS[path], age.data_ptr(),
-                                              age.numel(), int(return_prob), out.data_ptr(), ws.data_ptr(), ws.numel(),
-                                              torch.cuda.current_stream().cuda_stream), "b2cnn_score_record")
+            capi.check(lib.b2cnn_score_record_ex(h, records.data_ptr(), dtype, B, N, pitch, stride, _PATHS[path], m, age.data_ptr(),
+                                                 age.numel(), int(return_prob), out.data_ptr(), ws.data_ptr(), ws.numel(),
+                                                 torch.cuda.current_stream().cuda_stream), "b2cnn_score_record_ex")
         return out
 
     def call_plan(self, window_tensor: torch.Tensor, age: torch.Tensor, mode: str = "independent",
