@@ -8,10 +8,11 @@
 // two m64n32k16 row halves x C channels x SPLITS weight pieces, A in registers (one ldmatrix.x4 per row half and
 // channel of the block's 16-sample slice of the TMA tile: 32-sample boxes, SWIZZLE_64B, 3 blocks per tile, shared by
 // the SPLITS pieces), B = the band-matrix piece, D in registers.  The accumulator fragment (two windows x 16 values
-// per thread) is turned into thread == window through an 18 KB shared-memory transpose; the next block's MMAs run
-// while the epilogue of this one computes.  About 100 KB of shared memory and 128 registers per thread at launch let
-// two CTAs share an SM, so each SM sub-partition has two consumer warps to interleave; setmaxnreg then gives the
-// consumer warpgroup 216 of them and the producer warpgroup 40.  fp32 windows (F32IN) evaluate conv1 in exact fp32
+// per thread) is turned into thread == window through a 16 KB shared-memory transpose (XOR-swizzled, conflict-free
+// both ways); the next block's MMAs run while the epilogue of this one computes.  The three blocks of a tile are
+// unrolled, so their addresses are the tile's plus immediates.  About 100 KB of shared memory and 128 registers per
+// thread at launch let two CTAs share an SM, so each SM sub-partition has two consumer warps to interleave;
+// setmaxnreg then gives the consumer warpgroup 232 of them and the producer warpgroup 24.  fp32 windows (F32IN) evaluate conv1 in exact fp32
 // FMAs straight from the tile instead (the same 32-sample boxes as 128-byte SWIZZLE_128B rows; one CTA per SM).
 //
 // Epilogue, thread == window: each thread streams through its window's positions in order, so pool1 -> tanh ->
@@ -34,9 +35,13 @@ namespace b2cnn {
 // bf16 windows: two full warpgroups, so that setmaxnreg can move registers from the producer warpgroup (warps 4-7,
 // 6 and 7 idle) to the consumer one; fp32 windows: 192 threads
 __host__ __device__ constexpr int hp_threads(bool f32in) { return f32in ? 192 : 256; }
-constexpr int kHpProducerRegs = 40, kHpConsumerRegs = 216;   // 128 x 40 + 128 x 216 = 256 x 128: two CTAs per SM
-constexpr int kHpTStride = 36;                    // floats per window row of the accumulator transpose (conflict-free float4 reads)
+constexpr int kHpProducerRegs = 24, kHpConsumerRegs = 232;   // 128 x 24 + 128 x 232 = 256 x 128: two CTAs per SM
+// accumulator transpose: 32 floats per window row, 16-byte chunk q of row r stored at chunk q ^ hp_tswz(r).  The
+// rotation makes both sides conflict-free: the 8 rows an LDS.128 quarter-warp reads get 8 distinct masks, and the
+// 4 rows x 2 chunks an STS.64 half-warp writes (rows 0-3 or 4-7 of a group of 8: even or odd masks) 8 distinct chunks.
+constexpr int kHpTStride = 32;
 constexpr int kHpTBytes = kTcM * kHpTStride * 4;
+__device__ __forceinline__ uint32_t hp_tswz(uint32_t r) { return ((r << 1) | ((r >> 2) & 1u)) & 7u; }   // r % 8 rotated left
 constexpr int kHpPieceBytes = kTcM * 16 * 2;      // one bf16 piece of the projection A operand
 constexpr int kFuWChunkBytes = 3 * 64 * 16 * 2;   // 3 pieces x (64 gates x 16 positions) bf16
 // kOutRing: the features of a sliding-window scorer's new segment (b2cnn_slide.cu) into its position-major
@@ -156,6 +161,12 @@ tc_stream_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant
         const bool row_ok = b < p.B;
         // 16-byte chunk k of a row sits at chunk k ^ swz: SWIZZLE_64B (bf16) k ^ (row / 2) % 4, SWIZZLE_128B (fp32) k ^ row % 8
         const uint32_t swz = F32IN ? (uint32_t)(row & 7) : (uint32_t)((row >> 1) & 3);
+        // transpose addresses.  Rows are 128 bytes, so a chunk mask only flips bits 4-6 of an address.  Writes: this
+        // thread's rows (all == lane / 4 mod 8) at 8 (lane & 1) bytes of chunk (2 E + (lane >> 1) % 2) ^ mask, i.e.
+        // t_w ^ 32 E, plus 128 bytes per row; reads: its own row's chunk q at t_r ^ 16 q.
+        const uint32_t t_w = smem_u32(sT) + (uint32_t)(16 * warp + (lane >> 2)) * (kHpTStride * 4) + 8 * (lane & 1) +
+                             16 * (((lane >> 1) & 1) ^ hp_tswz((uint32_t)lane >> 2));
+        const uint32_t t_r = smem_u32(sT) + (uint32_t)row * (kHpTStride * 4) + 16 * hp_tswz((uint32_t)row);
         float acc[2][16];                             // conv1 accumulators of one block (two m64 row halves)
         float gacc[2][32];                            // gate pre-activations (two m64 row halves)
 #pragma unroll
@@ -182,10 +193,14 @@ tc_stream_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant
         uint32_t afr[2][C][4];
         const uint32_t a_lane = smem_u32(sA) + (uint32_t)(16 * warp + (lane & 7) + 8 * ((lane >> 3) & 1)) * kARow;
         const uint32_t a_swz = (lane >> 1) & 3, a_k = lane >> 4;
+        // chunk (n + a_k) ^ a_swz of a 64-byte row: blocks 0 and 2 at a_b02 ^ 16 n, block 1 ((1 + a_k) == 1 << a_k) at a_b1
+        const uint32_t a_b02 = a_lane | ((a_k ^ a_swz) << 4), a_b1 = a_lane | (((1u << a_k) ^ a_swz) << 4);
+        // tap 9 of block n: chunk (n + 1) ^ swz of this thread's row, t9_row ^ 16 (n + 1)
+        const uint32_t t9_row = smem_u32(sA) + (uint32_t)(row * kARow) + (swz << 4);
         // B descriptor built once: a block's MMAs only add (start address offset) >> 4 to it
         const uint64_t bdesc0 = gdesc_none_kmajor(smem_u32(sBm), 128, 256);
         auto issue_conv1 = [&](int s, int n) {
-            const uint32_t a_sn = a_lane + (uint32_t)(s * C * kABytes) + ((((uint32_t)n + a_k) ^ a_swz) << 4);
+            const uint32_t a_sn = (n == 1 ? a_b1 : a_b02 ^ (uint32_t)(16 * n)) + (uint32_t)(s * C * kABytes);
 #pragma unroll
             for (int h = 0; h < 2; ++h)
 #pragma unroll
@@ -205,17 +220,18 @@ tc_stream_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant
             issue_conv1(0, 0);
         }
 
-#pragma unroll 1
-        for (int j = 0; j < J; ++j) {
-            const int i = j / kBlocks, n = j - i * kBlocks, s = i & 1;
+        // step j = kBlocks i + n: block n of tile i (stage i & 1).  bf16 windows run the blocks of a tile unrolled, n a
+        // compile-time constant, so a block's tile, ldmatrix and tap-9 addresses are the tile's plus immediates.
+        auto step = [&](const int j, const int i, const int n) {
+            const int s = i & 1;
             float D[32];                              // conv1 pre-activations of block j: D[shift * 4 + out channel]
             if constexpr (!F32IN) {
                 if constexpr (ARCH == 0) {
                     // tap 9 of the previous block's position 7: sample 8n + 8 of this tile
 #pragma unroll
                     for (int c = 0; c < C; ++c) {
-                        const uint16_t raw = *reinterpret_cast<const uint16_t *>(sA_of(s, c) + row * kARow + (((uint32_t)(n + 1) ^ swz) << 4));
-                        const float xv = __uint_as_float((uint32_t)raw << 16);
+                        const uint32_t raw = ld_shared_u16((t9_row ^ (uint32_t)(16 * (n + 1))) + (uint32_t)((s * C + c) * kABytes));
+                        const float xv = __uint_as_float(raw << 16);
 #pragma unroll
                         for (int o = 0; o < kCMid; ++o) pm7[o] = fmaf(p.w9[c][o], xv, pm7[o]);
                     }
@@ -228,21 +244,20 @@ tc_stream_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant
 #pragma unroll
                 for (int h = 0; h < 2; ++h)
 #pragma unroll
-                    for (int e = 0; e < 16; e += 2) {
-                        const int r = 64 * h + 16 * warp + (lane >> 2) + 8 * ((e >> 1) & 1);
-                        const int col = 8 * (e >> 2) + 2 * (lane & 3);
-                        *reinterpret_cast<float2 *>(sT + r * kHpTStride + col) = make_float2(acc[h][e], acc[h][e + 1]);
-                    }
+                    for (int e = 0; e < 16; e += 2)   // row 64 h + 16 warp + lane / 4 + 8 ((e / 2) % 2), column 8 (e / 4) + 2 (lane % 4)
+                        st_shared_v2((t_w ^ (uint32_t)(32 * (e >> 2))) + (uint32_t)((64 * h + 8 * ((e >> 1) & 1)) * kHpTStride * 4),
+                                     acc[h][e], acc[h][e + 1]);
                 wg_bar();
                 if (n == kBlocks - 1 && lane == 0) mbar_arrive(bar_empty + 8 * s);   // stage fully consumed
-                if (j + 1 < J) {                      // the next block's MMAs overlap this block's epilogue
-                    const int i2 = (j + 1) / kBlocks, n2 = j + 1 - i2 * kBlocks;
-                    if (n2 == 0) mbar_wait(bar_full + 8 * (i2 & 1), (i2 >> 1) & 1);
-                    issue_conv1(i2 & 1, n2);
+                if (n < kBlocks - 1) {                // the next block's MMAs overlap this block's epilogue
+                    issue_conv1(s, n + 1);
+                } else if (i + 1 < ntiles) {          // (J is a whole number of tiles)
+                    mbar_wait(bar_full + 8 * (s ^ 1), ((i + 1) >> 1) & 1);
+                    issue_conv1(s ^ 1, 0);
                 }
 #pragma unroll
                 for (int k = 0; k < 32; k += 4) {
-                    const float4 v = *reinterpret_cast<const float4 *>(sT + row * kHpTStride + k);
+                    const float4 v = ld_shared_v4(t_r ^ (uint32_t)(4 * k));
                     D[k] = v.x; D[k + 1] = v.y; D[k + 2] = v.z; D[k + 3] = v.w;
                 }
                 wg_bar();                             // transpose buffer free for the next block
@@ -375,6 +390,15 @@ tc_stream_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant
                     wg_bar();                         // A tiles free for the next chunk
                 }
             }
+        };
+        if constexpr (F32IN) {
+#pragma unroll 1
+            for (int j = 0; j < J; ++j) step(j, j / kBlocks, j % kBlocks);
+        } else {
+#pragma unroll 1
+            for (int i = 0; i < ntiles; ++i)
+#pragma unroll
+                for (int n = 0; n < kBlocks; ++n) step(kBlocks * i + n, i, n);
         }
 
         if constexpr (OUT != kOutGates) {

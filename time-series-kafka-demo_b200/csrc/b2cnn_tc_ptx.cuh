@@ -55,6 +55,21 @@ __device__ __forceinline__ void wg_bar() { asm volatile("bar.sync 1, 128;" ::: "
 // generic-proxy shared-memory writes -> visible to the async proxy (wgmma operand reads)
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
+// shared-memory accesses by 32-bit shared address (for addresses built with XOR swizzles)
+__device__ __forceinline__ void st_shared_v2(uint32_t addr, float x, float y) {
+    asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(x), "f"(y) : "memory");
+}
+__device__ __forceinline__ uint32_t ld_shared_u16(uint32_t addr) {
+    uint16_t v;
+    asm volatile("ld.shared.u16 %0, [%1];" : "=h"(v) : "r"(addr) : "memory");
+    return v;
+}
+__device__ __forceinline__ float4 ld_shared_v4(uint32_t addr) {
+    float4 v;
+    asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr) : "memory");
+    return v;
+}
+
 // max_nan: b2cnn_internal.cuh
 __device__ __forceinline__ float max3_nan(float a, float b, float c) { return max_nan(max_nan(a, b), c); }
 // tanh(m + bias) with bias pre-multiplied by 2 log2 e:  1 - 2 / (1 + 2^(2 log2e (m + bias)))
