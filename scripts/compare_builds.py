@@ -6,6 +6,12 @@ inputs, with seed-0 MyCNN5 weights:
   * predict() logits at [--batch, 3, 75000] bf16 (the bench.py workload: the fused streaming kernel, gates out);
   * model.features() at [--feat-batch, 3, 75000] bf16 (the feature-row kernel);
   * one SlidingScorer push after a full window of pushes (the feature-ring kernel), logits and the ring's features;
+  * push(heads=True) with three heads, one of a shorter window (the ring projection with two rows per CTA, its
+    padding row, and one row alone), and export() of a few patients;
+  * a tensor-core scorer at W = 7502 (phase 2, so an admission's history is staged): a full-history admit of three
+    patients, then one push;
+  * a generic-path scorer (C = 10, bf16) after a full window of pushes;
+  * predict_record() on the tensor-core and generic paths, independent and sequence modes;
 then compares every array bit for bit.
 
     python scripts/compare_builds.py --baseline-lib /path/to/parent/libb2cnn.so [--lib /path/to/libb2cnn.so]
@@ -46,6 +52,59 @@ def dump(path: str, batch: int, feat_batch: int, patients: int) -> None:
         seg = tskd_b200.synth.make_windows(patients, C, S, "normal", seed=200 + i, dtype=torch.bfloat16, device=dev)
         got = sc.push(seg.contiguous(), pages)
     out["slide_logits"] = got
+    out["slide_features"] = sc.features()
+
+    # heads: rows 0-2 share the window W (a pair and a padded pair), row 3 has a shorter one and runs alone
+    conv = {k: v for k, v in m.state_dict().items() if k.startswith("conv")}
+    heads = []
+    for i, Wk in enumerate((W, W, W // 2)):
+        ha = O.stretched(O.ARCH_MYCNN5, C, Wk)
+        hm = tskd_b200.B200MyCNN(tskd_b200.ARCH_PRESETS["mycnn5"].with_shape(C, Wk), has_out12=ha.has_out12).to(dev)
+        sd = O.make_ref(ha, seed=20 + i).state_dict()
+        sd.update(conv)
+        hm.load_state_dict(sd)
+        heads.append(hm)
+    sc.set_heads(heads, shorter_windows=True)
+    seg = tskd_b200.synth.make_windows(patients, C, S, "normal", seed=300, dtype=torch.bfloat16, device=dev)
+    out["heads_logits"] = sc.push(seg.contiguous(), pages, heads=True)
+    st = sc.export([0, 5, 17, patients - 1])
+    out["export_features"], out["export_tail"], out["export_seen"] = st["features"], st["tail"], st["seen"]
+    del sc, heads
+
+    # admission with a full history at phase 2: staged before the tensor-core front end
+    Wa, Sa, Pa = 7502, 1876, 64
+    aa = O.stretched(O.ARCH_MYCNN5, C, Wa)
+    ma = tskd_b200.B200MyCNN(tskd_b200.ARCH_PRESETS["mycnn5"].with_shape(C, Wa), has_out12=aa.has_out12).to(dev)
+    ma.load_state_dict(O.make_ref(aa, seed=1).state_dict())
+    sa = tskd_b200.SlidingScorer(ma, Pa, Sa)
+    aages = tskd_b200.synth.make_ages(Pa, seed=10, device=dev)
+    for i in range(Wa // Sa + 1):
+        sa.push(tskd_b200.synth.make_windows(Pa, C, Sa, "normal", seed=400 + i, dtype=torch.bfloat16, device=dev), aages)
+    sa.admit([3, 10, 40], tskd_b200.synth.make_windows(3, C, Wa, "normal", seed=410, dtype=torch.bfloat16, device=dev))
+    out["admit_logits"] = sa.push(tskd_b200.synth.make_windows(Pa, C, Sa, "normal", seed=411, dtype=torch.bfloat16, device=dev),
+                                  aages)
+    out["admit_features"] = sa.features()
+    del sa
+
+    # the generic path: 10 channels have no tensor-core kernel
+    Wg, Sg, Pg, Cg = 1200, 120, 256, 10
+    ag = O.stretched(O.ARCH_MYCNN5, Cg, Wg)
+    mg = tskd_b200.B200MyCNN(tskd_b200.ARCH_PRESETS["mycnn5"].with_shape(Cg, Wg), has_out12=ag.has_out12).to(dev)
+    mg.load_state_dict(O.make_ref(ag, seed=2).state_dict())
+    sg = tskd_b200.SlidingScorer(mg, Pg, Sg, path="generic")
+    gages = tskd_b200.synth.make_ages(Pg, seed=11, device=dev)
+    for i in range(Wg // Sg + 1):
+        got = sg.push(tskd_b200.synth.make_windows(Pg, Cg, Sg, "normal", seed=500 + i, dtype=torch.bfloat16, device=dev), gages)
+    out["generic_slide_logits"] = got
+    out["generic_slide_features"] = sg.features()
+    del sg
+
+    # whole recordings
+    rec = tskd_b200.synth.make_windows(4, C, 4 * W, "normal", seed=600, dtype=torch.bfloat16, device=dev)
+    recg = tskd_b200.synth.make_windows(8, Cg, 20 * Wg, "normal", seed=601, dtype=torch.bfloat16, device=dev)
+    for mode in ("independent", "sequence"):
+        out[f"record_tc_{mode}"] = m.predict_record(rec, S, 60.0, path="tensorcore", mode=mode)
+        out[f"record_generic_{mode}"] = mg.predict_record(recg, Sg, 60.0, path="generic", mode=mode)
     torch.cuda.synchronize()
     np.savez(path, **{k: (v.cpu().numpy() if hasattr(v, "cpu") else v) for k, v in out.items()})
 
@@ -80,7 +139,7 @@ def main() -> int:
         same = a.shape == b.shape and a.dtype == b.dtype and a.tobytes() == b.tobytes()
         ok &= same
         extra = "" if a.dtype.kind == "U" else f", max |diff| {np.abs(a.astype(np.float64) - b.astype(np.float64)).max():.3g}" if a.shape == b.shape else ""
-        print(f"{k:16s} {str(a.shape):16s} {'byte-identical' if same else 'DIFFERENT'}{extra}  {a.ravel()[:1]}")
+        print(f"{k:26s} {str(a.shape):16s} {'byte-identical' if same else 'DIFFERENT'}{extra}  {a.ravel()[:1]}")
     print("all byte-identical" if ok else "builds differ")
     return 0 if ok else 1
 

@@ -9,12 +9,12 @@ from collections import namedtuple
 
 R_OF = {"mycnn5": 24, "mycnn3": 16}          # receptive field of a feature in samples (slide_create: s->R)
 FOFF_OF = {"mycnn5": 3, "mycnn3": 2}         # step j of the stream emits features 2j - foff, 2j - foff + 1
-SPLIT = 32                                   # slide_push / slide_admit: Q >= 32 features run on the tensor cores
+SPLIT = 32                                   # tc_ring_block (slide_push / slide_admit): Q >= 32 features run on tensor cores
 W_OF_PHI = {0: 1532, 3: 1533, 2: 1530, 1: 1531}
 
 
 def fdiv4(a):
-    """fdiv4 / fdiv(a, 4): floor division"""
+    """fdiv(a, 4): floor division"""
     return a // 4
 
 
@@ -24,7 +24,7 @@ def cdiv4(a):
 
 
 def phi_of(W):
-    """slide_create: s->phi = (4 - W % 4) % 4, stream feature g starts at sample 4 g + phi"""
+    """slide_create: s->phi = (F - W % F) % F with F = 4, stream feature g starts at sample 4 g + phi"""
     return (4 - W % 4) % 4
 
 

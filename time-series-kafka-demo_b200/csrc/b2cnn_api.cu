@@ -9,6 +9,7 @@
 #include <vector>
 
 #include "b2cnn_internal.cuh"
+#include "b2cnn_proj_tc.cuh"
 #include "b2cnn_slide.cuh"
 #include "b2cnn_tc.cuh"
 
@@ -611,8 +612,8 @@ static int slide_create_on(const char *fn, b2cnn_handle *h, int32_t n_patients, 
     // auto: the tensor-core path where it holds the model (slide_create refuses everything else with B2CNN_EARCH; its
     // geometries have F = 4, so a stride it refuses the generic path refuses too), else the generic path
     const bool tc = path == B2CNN_PATH_TENSORCORE || (path == B2CNN_PATH_AUTO && h->tc.fused);
-    const int rc = tc ? slide_create(h->d, h->tc, n_patients, stride, dtype, h->device, &s, &err)
-                      : slide_create_generic(h->d, n_patients, stride, dtype, h->device, h->num_sms, &s, &err);
+    const int rc = slide_create(h->d, h->tc, tc ? B2CNN_PATH_TENSORCORE : B2CNN_PATH_GENERIC, n_patients, stride, dtype, h->device,
+                                h->num_sms, &s, &err);
     if (rc != B2CNN_OK) return fail(rc, std::string(fn) + ": " + err);
     b2cnn_slide *o = new (std::nothrow) b2cnn_slide{s, h, h->weight_gen, weights_digest(s, h->cw)};
     if (!o) { slide_destroy(s); return fail(B2CNN_ESTATE, "out of host memory"); }

@@ -135,7 +135,7 @@ ring_proj_kernel(const float *__restrict__ ring, int64_t pitch, int head, int ca
     proj_body<kProjRing>(ring, 1, pitch, head, cap, WT, part, B, L, k_per_split);
 }
 
-// whole recordings (b2cnn_slide.cu, b2cnn_score_record): row b = window b mod n_w of recording b / n_w, whose features
+// whole recordings (b2cnn_record.cu, b2cnn_score_record): row b = window b mod n_w of recording b / n_w, whose features
 // start at feats[(b / n_w) rec_pitch + (b mod n_w) step]
 __global__ void __launch_bounds__(256)
 record_proj_kernel(const float *__restrict__ feats, int64_t rec_pitch, int n_w, int64_t step, const float *__restrict__ WT,

@@ -137,7 +137,7 @@ int launch_ring_head(const Dims &d, const HeadWeights &hw, const float *ring, in
                      const float *age, int64_t n_age, int apply_sigmoid, float *out, float *gates_ws, float *partial_ws,
                      cudaStream_t st, const char **err);
 
-// launch_head of the n_w windows of each whole recording (b2cnn_slide.cu, b2cnn_score_record, generic path): row b =
+// launch_head of the n_w windows of each whole recording (b2cnn_record.cu, b2cnn_score_record, generic path): row b =
 // window b mod n_w of recording b / n_w, position k at feats[(b / n_w) rec_pitch + (b mod n_w) step + k]; rows =
 // recordings x n_w; the same tiles and summation order as launch_head.  mode B2CNN_MODE_SEQUENCE: one LSTM scan per
 // recording over its n_w windows (launch_sequence_segments) instead of independent windows

@@ -30,16 +30,17 @@
 // P patients; slide_live_kernel advances seen and writes NaN for patients without a complete window.  None of this
 // runs for a scorer that never admitted or discharged a patient since its last reset.
 //
-// All of the above is the tensor-core path.  The generic path (slide_create_generic, "generic path" below) runs the
-// same ring and lifecycle for every geometry on exact CUDA-core kernels, with F = pool_s^2 in place of 4.
+// All of the above is the tensor-core path.  The generic path (slide_create with B2CNN_PATH_GENERIC, "generic path"
+// below) runs the same ring and lifecycle for every geometry on exact CUDA-core kernels, with F = pool_s^2 in place of
+// 4.  slide_push and slide_admit are shared; only the step that computes the features differs between the paths.
 #include <algorithm>
 #include <cstring>
 #include <new>
 #include <type_traits>
 #include <vector>
 
+#include "b2cnn_proj_tc.cuh"
 #include "b2cnn_slide.cuh"
-#include "b2cnn_tc_ptx.cuh"
 
 namespace b2cnn {
 
@@ -86,7 +87,6 @@ struct Slide {
     std::vector<SlideHead> heads;    // extra heads, rows 1.. of a push with heads
 };
 
-static int64_t fdiv4(int64_t a) { return a >= 0 ? a / 4 : -((-a + 3) / 4); }
 static int64_t fdiv(int64_t a, int64_t m) { return a >= 0 ? a / m : -((-a + m - 1) / m); }
 // a mod m in [0, m): stream features before sample 0 (negative g) exist once a patient is admitted with history
 __host__ __device__ __forceinline__ int64_t mod_nn(int64_t a, int64_t m) {
@@ -181,17 +181,6 @@ __global__ void __launch_bounds__(128) slide_exact_kernel(const __grid_constant_
     for (int wi = blockIdx.y; wi < nwin; wi += gridDim.y) store(p.list[wi], gi);
 }
 
-// new tail = the last kSlideTail samples of (old tail | segment)
-template <typename Tin>
-__global__ void slide_tail_kernel(const Tin *__restrict__ x, int64_t pitch, int S, const float *__restrict__ tin,
-                                  float *__restrict__ tout, int64_t rows) {
-    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (e >= rows * kSlideTail) return;
-    const int64_t r = e / kSlideTail;
-    const int u = S + (int)(e % kSlideTail);
-    tout[e] = u < kSlideTail ? tin[r * kSlideTail + u] : ld_sample<Tin>(x + r * pitch + (u - kSlideTail));
-}
-
 // segment rows shifted by phi into 16-byte aligned rows of Sp samples (tail zero-filled)
 template <typename T>
 __global__ void slide_stage_kernel(const T *__restrict__ src, int64_t sp, int phi, int n, T *__restrict__ dst, int64_t dp,
@@ -208,17 +197,11 @@ __global__ void slide_stage_kernel(const T *__restrict__ src, int64_t sp, int ph
 // n_ranges, all from L only), so the packed W_ih chunks of tc_prepare serve unchanged: chunk m of range r holds the
 // weights of window positions r F + 16 m - foff + k (k < 16), zero outside the range.  A row's window (L positions,
 // its first in slot `head`) may be a suffix of the ring's (cap >= L slots): a head with a shorter window.
-// CTA = (128 patients, range):
+// CTA = (128 patients, range), the chunk arithmetic of b2cnn_proj_tc.cuh:
 //   warp 4: TMA producer -- per chunk one {128 patients x 16 slots} fp32 box of the ring at the chunk's first slot and,
 //           when the 16 slots wrap past cap, a second box at slot 0; plus the 6 KB W_ih chunk (bulk copy); two stages;
-//   warps 0-3: thread == patient: the chunk's 16 features (0 outside the range) split into three bf16 pieces written
-//           as the K-major A tile, then 2 row halves x 6 m64n64k16 piece pairs (hh hm mh hl lh mm, fp32-equivalent
-//           products, as the fused kernel) accumulating partial[range][patient][64] in registers.
-constexpr int kRpThreads = 160;
-constexpr int kRpM = 128;                            // patients per CTA
+//   warps 0-3: thread == patient, its features read from the ring boxes.
 constexpr int kRpBox = 16 * kRpM * 4;                // one TMA box: 16 slots x 128 patients fp32
-constexpr int kRpWChunk = 3 * 64 * 16 * 2;           // a packed W_ih chunk (tc_pack_wih_kernel, kFuWChunkBytes)
-constexpr int kRpPiece = kRpM * 16 * 2;              // one bf16 piece of the A tile
 // HP: heads per CTA, each with its own W_ih chunk slot per stage (HP = 1: the scorer's own model alone)
 template <int HP>
 constexpr size_t kRpSmemHP = 1024 + 2 * 2 * kRpBox + 2 * HP * kRpWChunk + 3 * kRpPiece + 64;
@@ -316,39 +299,17 @@ slide_ring_proj_kernel(const __grid_constant__ CUtensorMap tm, const __grid_cons
         mbar_wait(bar_full + 8 * u, (m >> 1) & 1);
         const int s0 = first_slot(m), q0 = lo + 16 * m - p.foff;
         const float *fa = sF + (size_t)u * 2 * 16 * kRpM, *fb = fa + 16 * kRpM;
-        auto feat = [&](int k) {
+        rp_split_row(arow, [&](int k) {
             const int q = q0 + k;
             if (q < lo || q >= hi) return 0.f;
             return s0 + k < p.cap ? fa[k * kRpM + row] : fb[(s0 + k - p.cap) * kRpM + row];
-        };
-#pragma unroll
-        for (int kk = 0; kk < 8; ++kk) {
-            const float f0 = feat(2 * kk), f1 = feat(2 * kk + 1);
-            const uint32_t h = pack_bf16x2(f0, f1);
-            const float r1x = f0 - __uint_as_float(h << 16), r1y = f1 - __uint_as_float(h & 0xffff0000u);
-            const uint32_t md = pack_bf16x2(r1x, r1y);
-            const uint32_t lw = pack_bf16x2(r1x - __uint_as_float(md << 16), r1y - __uint_as_float(md & 0xffff0000u));
-            const int off = (kk >> 2) * 128 + (kk & 3) * 4;
-            *reinterpret_cast<uint32_t *>(arow + off) = h;
-            *reinterpret_cast<uint32_t *>(arow + kRpPiece + off) = md;
-            *reinterpret_cast<uint32_t *>(arow + 2 * kRpPiece + off) = lw;
-        }
+        });
         fence_proxy_async();
         wg_bar();
         const uint32_t pa = smem_u32(sPc);
         wgmma_fence();
 #pragma unroll
-        for (int j = 0; j < HP; ++j) {
-            const uint32_t pw = smem_u32(sW + (u * HP + j) * kRpWChunk);
-#pragma unroll
-            for (int hh = 0; hh < 2; ++hh) {
-                constexpr int kAp[6] = {0, 0, 1, 0, 2, 1}, kWp[6] = {0, 1, 0, 2, 0, 1};
-#pragma unroll
-                for (int q = 0; q < 6; ++q)
-                    wgmma_m64n64(gacc[j][hh], gdesc_none_kmajor(pa + kAp[q] * kRpPiece + hh * 2048, 128, 256),
-                                 gdesc_none_kmajor(pw + kWp[q] * 2048, 128, 256));
-            }
-        }
+        for (int j = 0; j < HP; ++j) rp_mma_chunk(gacc[j], pa, smem_u32(sW + (u * HP + j) * kRpWChunk));
         wgmma_commit();
         wgmma_wait<0>();
         __syncwarp();
@@ -359,18 +320,7 @@ slide_ring_proj_kernel(const __grid_constant__ CUtensorMap tm, const __grid_cons
     for (int j = 0; j < HP; ++j) {
         float *const part = partial_of(j);
         if (HP > 1 && !part) continue;
-#pragma unroll
-        for (int hh = 0; hh < 2; ++hh)
-#pragma unroll
-            for (int e2 = 0; e2 < 2; ++e2) {
-                const int bb = b0 + 64 * hh + 16 * warp + (lane >> 2) + 8 * e2;
-                if (bb < p.P) {
-                    float *dst = part + ((int64_t)blockIdx.y * p.P + bb) * kGates + 2 * (lane & 3);
-#pragma unroll
-                    for (int e = 2 * e2; e < 32; e += 4)
-                        *reinterpret_cast<float2 *>(dst + 8 * (e >> 2)) = make_float2(gacc[j][hh][e], gacc[j][hh][e + 1]);
-                }
-            }
+        rp_store_partial(part, blockIdx.y, p.P, b0, warp, lane, gacc[j]);
     }
 }
 
@@ -395,19 +345,6 @@ __global__ void slide_scatter_kernel(const float *__restrict__ scratch, int64_t 
     }
 }
 
-// tail rows of the admitted patients = the last kSlideTail samples of their history [k][C][pitch] (zeros in front of
-// a shorter one: they only reach features that start before the history, which no valid window holds)
-template <typename Tin>
-__global__ void slide_admit_tail_kernel(const Tin *__restrict__ h, int64_t pitch, int64_t H, const int *__restrict__ idx, int k,
-                                        int C, float *__restrict__ tail) {
-    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (e >= (int64_t)k * C * kSlideTail) return;
-    const int64_t r = e / kSlideTail;                     // history row j * C + c
-    const int u = (int)(e % kSlideTail);
-    const int64_t t = H - kSlideTail + u;
-    tail[((int64_t)idx[r / C] * C + r % C) * kSlideTail + u] = t >= 0 ? ld_sample<Tin>(h + r * pitch + t) : 0.f;
-}
-
 // seen[b] += adv for admitted patients (seen >= 0); then row b of x [P][len] = NaN unless seen[b] >= W.
 // adv != 0 only with gridDim.y == 1 (one thread per patient reads and writes seen).
 __global__ void slide_live_kernel(int64_t *__restrict__ seen, int P, int64_t adv, int64_t W, float *__restrict__ x, int64_t len) {
@@ -426,11 +363,11 @@ __global__ void slide_nan_rows_kernel(float *__restrict__ out, int P, unsigned r
     if (b < P && ((rows >> blockIdx.y) & 1u)) out[(int64_t)blockIdx.y * P + b] = __int_as_float(0x7fc00000);
 }
 
-// ---- generic path kernels: tails of any length T ------------------------------------------------------------------
+// ---- tails of T samples per patient and channel (T = kSlideTail on the tensor-core path, R - 1 on the generic one) ----
 // new tail = the last T samples of (old tail | segment)
 template <typename Tin>
-__global__ void slide_gtail_kernel(const Tin *__restrict__ x, int64_t pitch, int S, int T, const float *__restrict__ tin,
-                                   float *__restrict__ tout, int64_t rows) {
+__global__ void slide_shift_tail_kernel(const Tin *__restrict__ x, int64_t pitch, int S, int T, const float *__restrict__ tin,
+                                        float *__restrict__ tout, int64_t rows) {
     const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (e >= rows * T) return;
     const int64_t r = e / T;
@@ -438,7 +375,20 @@ __global__ void slide_gtail_kernel(const Tin *__restrict__ x, int64_t pitch, int
     tout[e] = u < T ? tin[r * T + u] : ld_sample<Tin>(x + r * pitch + (u - T));
 }
 
-// seam rows [rows][T + n] fp32: the tail's T samples, then the segment's first n
+// tail rows of the admitted patients = the last T samples of their history [k][C][pitch] (zeros in front of a shorter
+// one: they only reach features that start before the history, which no valid window holds)
+template <typename Tin>
+__global__ void slide_seed_tail_kernel(const Tin *__restrict__ h, int64_t pitch, int64_t H, const int *__restrict__ idx, int k,
+                                       int C, int T, float *__restrict__ tail) {
+    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= (int64_t)k * C * T) return;
+    const int64_t r = e / T;                               // history row j * C + c
+    const int64_t u = e % T;
+    const int64_t t = H - T + u;
+    tail[((int64_t)idx[r / C] * C + r % C) * T + u] = t >= 0 ? ld_sample<Tin>(h + r * pitch + t) : 0.f;
+}
+
+// seam rows [rows][T + n] fp32 (generic path): the tail's T samples, then the segment's first n
 template <typename Tin>
 __global__ void slide_seam_rows_kernel(const Tin *__restrict__ x, int64_t pitch, const float *__restrict__ tail, int T, int n,
                                        float *__restrict__ dst, int64_t rows) {
@@ -447,18 +397,6 @@ __global__ void slide_seam_rows_kernel(const Tin *__restrict__ x, int64_t pitch,
         const int64_t r = e / w, i = e - r * w;
         dst[e] = i < T ? tail[r * T + i] : ld_sample<Tin>(x + r * pitch + (i - T));
     }
-}
-
-// tail rows of the admitted patients = the last T samples of their history (zeros in front of a shorter one)
-template <typename Tin>
-__global__ void slide_admit_gtail_kernel(const Tin *__restrict__ h, int64_t pitch, int64_t H, const int *__restrict__ idx, int k,
-                                         int C, int T, float *__restrict__ tail) {
-    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (e >= (int64_t)k * C * T) return;
-    const int64_t r = e / T;                               // history row j * C + c
-    const int64_t u = e % T;
-    const int64_t t = H - T + u;
-    tail[((int64_t)idx[r / C] * C + r % C) * T + u] = t >= 0 ? ld_sample<Tin>(h + r * pitch + t) : 0.f;
 }
 
 // ------------------------------------------------------------------------------------------
@@ -485,17 +423,6 @@ static int launch_exact_p(SlideExactParams p, const Slide &s, int64_t ng, cudaSt
     }
     if (cudaGetLastError() != cudaSuccess) { *err = "exact feature kernel launch"; return -1; }
     return 1;
-}
-
-// features [g0, g0 + ng) of the pushed segment exactly into the scorer's ring: of every patient (list == nullptr) or
-// of the listed ones
-static int launch_exact(const Slide &s, const ConvWeights &cw, const void *x, int64_t pitch, const float *tail, int64_t g0,
-                        int64_t ng, const int *list, const int *count, cudaStream_t st, const char **err) {
-    SlideExactParams p;
-    memset(&p, 0, sizeof p);
-    p.x = x; p.pitch = pitch; p.tail = tail; p.ring = s.ring; p.ring_pitch = s.ring_pitch; p.cap = s.d.L; p.P = s.P;
-    p.g0 = g0; p.seg0 = s.n * s.S; p.phi = s.phi; p.list = list; p.count = count; p.cw = cw;
-    return launch_exact_p(p, s, ng, st, err);
 }
 
 // ---- generic path: every geometry, exact fp32 on CUDA cores --------------------------------------------------------
@@ -530,120 +457,117 @@ static int ring_front(const Slide &s, const ConvWeights &cw, const void *x, int 
     return 1;
 }
 
-int slide_create_generic(const Dims &d, int n_patients, int stride, int dtype, int device, int num_sms, Slide **out,
-                         const char **err) {
+// ---- the per-path step of a push: ring slots [g_lo, g_hi] -------------------------------------------------------
+// Tensor-core path: features [p.g0, p.g0 + Q) of p.P rows [p.P][C][p.pitch] holding stream samples [p.seg0, p.seg0 +
+// len) into p.ring, slot g mod p.cap.  From Q >= 32 on, tc_ring_features from the rows (first copied into `stage` rows
+// of sp samples, shifted to start at feature p.g0, where it does not start them or they are not 16-byte aligned), then
+// the rows it flagged in `flags` [2 p.P + 1] exactly; below that every row exactly.
+static int tc_ring_block(const Slide &s, const TcState &tc, SlideExactParams p, int64_t Q, int64_t len, void *stage, int64_t sp,
+                         int *flags, cudaStream_t st, const char **err) {
+    if (Q >= 32) {
+        const int64_t esz = s.dtype == B2CNN_DTYPE_BF16 ? 2 : 4, rows = (int64_t)p.P * s.d.C;
+        const int64_t off = s.F * p.g0 + p.phi - p.seg0;               // the row sample feature p.g0 starts at
+        const void *xin = p.x;
+        int64_t xp = p.pitch;
+        if (off != 0 || p.pitch % (16 / esz) != 0 || (reinterpret_cast<uintptr_t>(p.x) & 15) != 0) {
+            const unsigned blocks = (unsigned)std::min<int64_t>((rows * sp + 255) / 256, 65536);
+            if (esz == 2)
+                slide_stage_kernel<uint16_t><<<blocks, 256, 0, st>>>(static_cast<const uint16_t *>(p.x), p.pitch, (int)off, (int)(len - off),
+                                                                     static_cast<uint16_t *>(stage), sp, rows);
+            else
+                slide_stage_kernel<float><<<blocks, 256, 0, st>>>(static_cast<const float *>(p.x), p.pitch, (int)off, (int)(len - off),
+                                                                  static_cast<float *>(stage), sp, rows);
+            if (cudaGetLastError() != cudaSuccess) { *err = "staging launch"; return -1; }
+            xin = stage; xp = sp;
+        }
+        Dims dseg = s.d;
+        dseg.W = (int)(len - off); dseg.L = (int)Q; dseg.XP = (int)xp;
+        if (cudaMemsetAsync(flags, 0, sizeof(int) * (size_t)(2 * p.P + 1), st) != cudaSuccess) { *err = "memset flags"; return -1; }
+        if (tc_ring_features(tc, dseg, p.cw, xin, xp, s.dtype, p.P, p.ring, p.ring_pitch, p.cap, (int)mod_nn(p.g0, p.cap), flags, st,
+                             err) < 0)
+            return -1;
+        p.list = flags + p.P; p.count = flags + 2 * p.P;
+    }
+    return launch_exact_p(p, s, Q, st, err);
+}
+
+// tensor-core path: main features [g_m0, g_hi] from the segment (tc_ring_block), seam features [g_lo, min(g_hi, g_m0 -
+// 1)] exactly, their receptive field starting in the tail
+static int push_features_tc(Slide *s, const ConvWeights &cw, const TcState &tc, const void *x, int64_t pitch, const float *tail_in,
+                            int64_t g_lo, int64_t g_m0, int64_t g_hi, cudaStream_t st, const char **err) {
+    SlideExactParams p;
+    memset(&p, 0, sizeof p);
+    p.x = x; p.pitch = pitch; p.tail = tail_in; p.ring = s->ring; p.ring_pitch = s->ring_pitch; p.cap = s->d.L; p.P = s->P;
+    p.g0 = g_m0; p.seg0 = s->n * s->S; p.phi = s->phi; p.cw = cw;
+    if (tc_ring_block(*s, tc, p, g_hi - g_m0 + 1, s->S, s->stage, s->Sp, s->flags, st, err) < 0) return -1;
+    p.g0 = g_lo;
+    return launch_exact_p(p, *s, std::min(g_hi, g_m0 - 1) - g_lo + 1, st, err);
+}
+
+// generic path: main features [g_m0, g_hi] straight from the segment (feature g_m0 starts at its sample phi), seam
+// features [g_lo, min(g_hi, g_m0 - 1)] from seam rows: they start in the last T samples before the segment and end in
+// its first min(S, T) (F g_lo + phi >= seg0 - T: g_lo - 1 is at most the last feature complete before this push)
+static int push_features_generic(Slide *s, const ConvWeights &cw, const void *x, int64_t pitch, const float *tail_in, int64_t g_lo,
+                                 int64_t g_m0, int64_t g_hi, cudaStream_t st, const char **err) {
+    const int64_t P = s->P, T = s->T, seg0 = s->n * s->S;
+    if (g_hi >= g_m0 &&
+        ring_front(*s, cw, x, s->dtype, pitch, P, s->phi, g_m0, g_hi - g_m0 + 1, s->ring, s->ring_pitch, s->d.L, st, err) < 0)
+        return -1;
+    const int64_t seam_hi = std::min(g_hi, g_m0 - 1);
+    if (seam_hi < g_lo) return 1;
+    const int64_t rows = P * s->d.C, total = rows * s->Sp;
+    const unsigned blocks = (unsigned)std::min<int64_t>((total + 255) / 256, 65536);
+    const int nseg = (int)(s->Sp - T);
+    if (s->dtype == B2CNN_DTYPE_BF16)
+        slide_seam_rows_kernel<__nv_bfloat16><<<blocks, 256, 0, st>>>(reinterpret_cast<const __nv_bfloat16 *>(x), pitch, tail_in, (int)T,
+                                                                      nseg, reinterpret_cast<float *>(s->stage), rows);
+    else
+        slide_seam_rows_kernel<float><<<blocks, 256, 0, st>>>(reinterpret_cast<const float *>(x), pitch, tail_in, (int)T, nseg,
+                                                              reinterpret_cast<float *>(s->stage), rows);
+    if (cudaGetLastError() != cudaSuccess) { *err = "seam rows launch"; return -1; }
+    return ring_front(*s, cw, s->stage, B2CNN_DTYPE_F32, s->Sp, P, s->F * g_lo + s->phi - seg0 + T, g_lo, seam_hi - g_lo + 1, s->ring,
+                      s->ring_pitch, s->d.L, st, err);
+}
+
+int slide_create(const Dims &d, const TcState &tc, int path, int n_patients, int stride, int dtype, int device, int num_sms, Slide **out,
+                 const char **err) {
     *out = nullptr;
+    const bool tcp = path == B2CNN_PATH_TENSORCORE;
     if (dtype != B2CNN_DTYPE_F32 && dtype != B2CNN_DTYPE_BF16) { *err = "dtype must be f32 (0) or bf16 (1)"; return B2CNN_EINVAL; }
     if (n_patients < 1 || n_patients > (1 << 24)) { *err = "n_patients out of range"; return B2CNN_EINVAL; }
     if (stride < 1 || stride > d.W) { *err = "stride must be in [1, window]"; return B2CNN_EINVAL; }
     const int F = d.PS * d.PS, R = d.PS * (d.PK + d.K2 - 2) + d.PK + d.K1 - 1;
-    if (stride % F != 0) { *err = "stride must be a multiple of the feature stride (pool_s^2 samples)"; return B2CNN_EINVAL; }
+    if (stride % F != 0) {
+        *err = tcp ? "stride must be a multiple of the feature stride (4 samples)"
+                   : "stride must be a multiple of the feature stride (pool_s^2 samples)";
+        return B2CNN_EINVAL;
+    }
+    if (tcp && !tc.fused) {
+        *err = "the sliding-window scorer covers the streaming tensor-core geometries only (MyCNN5 or MyCNN2/3/4 conv/pool, "
+               "1 to 3 channels, tanh, no affine)";
+        return B2CNN_EARCH;
+    }
     if (d.W < R || d.L != (d.W - R) / F + 1) { *err = "the feature lattice does not match the window's feature count"; return B2CNN_EARCH; }
-    if (!frontend_generic_fits(d)) {
+    if (!tcp && !frontend_generic_fits(d)) {
         *err = "the generic front end's tile does not fit shared memory (in_channels * pool_s^2 too large for this window length)";
         return B2CNN_EARCH;
     }
     Slide *s = new (std::nothrow) Slide();
     if (!s) { *err = "out of host memory"; return B2CNN_ESTATE; }
-    s->device = device; s->d = d; s->P = n_patients; s->S = stride; s->dtype = dtype;
-    s->path = B2CNN_PATH_GENERIC; s->F = F; s->R = R; s->T = std::max(R - 1, 1); s->num_sms = num_sms;
+    s->device = device; s->d = d; s->P = n_patients; s->S = stride; s->dtype = dtype; s->num_sms = num_sms;
+    s->path = tcp ? B2CNN_PATH_TENSORCORE : B2CNN_PATH_GENERIC; s->F = F; s->R = R;
+    s->T = tcp ? kSlideTail : std::max(R - 1, 1);
     s->phi = (F - d.W % F) % F;
-    s->ranges = proj_slices(d.L);
+    s->ranges = tcp ? tc.n_ranges : proj_slices(d.L);
     s->ring_pitch = (n_patients + 3) & ~3;
-    s->Sp = s->T + std::min(stride, s->T);
-    const int64_t P = n_patients;
+    // staging rows: tensor-core path, the segment shifted by phi in the window dtype; generic path, fp32 seam rows
+    s->Sp = tcp ? (stride + 7) & ~7 : s->T + std::min(stride, s->T);
+    const int64_t P = n_patients, esz = tcp && dtype == B2CNN_DTYPE_BF16 ? 2 : 4;
     bool ok = cudaMalloc(&s->ring, sizeof(float) * (size_t)d.L * s->ring_pitch) == cudaSuccess &&
               cudaMalloc(&s->tail, sizeof(float) * (size_t)2 * P * d.C * s->T) == cudaSuccess &&
               cudaMalloc(&s->partial, sizeof(float) * (size_t)s->ranges * P * kGates) == cudaSuccess &&
-              cudaMalloc(&s->gates, sizeof(float) * (size_t)P * kGates) == cudaSuccess &&
-              cudaMalloc(&s->stage, sizeof(float) * (size_t)(P * d.C * s->Sp)) == cudaSuccess &&
-              cudaMalloc(&s->seen, sizeof(int64_t) * (size_t)P) == cudaSuccess;
-    if (!ok) { (void)cudaGetLastError(); slide_destroy(s); *err = "cudaMalloc(scorer state)"; return B2CNN_ECUDA; }
-    *out = s;
-    return B2CNN_OK;
-}
-
-static int score_windows(Slide *s, const HeadWeights &hw, const TcState *tc, const float *age, int64_t n_age, int apply_sigmoid,
-                         float *out, bool heads, int *emitted, int64_t *window_index, cudaEvent_t *ev, cudaStream_t st, const char **err);
-
-static int slide_push_generic(Slide *s, const ConvWeights &cw, const HeadWeights &hw, const void *x, int64_t pitch, const float *age,
-                              int64_t n_age, int apply_sigmoid, float *out, bool heads, int *emitted, int64_t *window_index,
-                              cudaEvent_t *ev, cudaStream_t st, const char **err) {
-    const Dims &d = s->d;
-    const int64_t P = s->P, S = s->S, T = s->T;
-    if (pitch < S || pitch > 0x7fffffff) { *err = "pitch must be in [stride, 2^31)"; return B2CNN_EINVAL; }
-    if (n_age != 1 && n_age != P) { *err = "age must have 1 or n_patients elements"; return B2CNN_EINVAL; }
-    const int64_t n1 = s->n + 1, seg0 = s->n * S;
-    const int64_t g_hi = fdiv(n1 * S - s->R - s->phi, s->F);   // last feature whose samples have all arrived
-    const int64_t g_m0 = seg0 / s->F;                           // first feature that starts inside the segment
-    const int64_t g_lo = std::max(s->g_done + 1, window_head(*s, n1));   // earlier features never enter a window
-    const float *tail_in = s->tail + (size_t)s->tail_cur * P * d.C * T;
-    float *tail_out = s->tail + (size_t)(s->tail_cur ^ 1) * P * d.C * T;
-    if (ev && cudaEventRecord(ev[0], st) != cudaSuccess) { *err = "cudaEventRecord"; return B2CNN_ECUDA; }
-    // ---- main features [g_m0, g_hi], straight from the segment (feature g_m0 starts at its sample phi)
-    if (g_hi >= g_m0 &&
-        ring_front(*s, cw, x, s->dtype, pitch, P, s->phi, g_m0, g_hi - g_m0 + 1, s->ring, s->ring_pitch, d.L, st, err) < 0)
-        return B2CNN_ECUDA;
-    // ---- seam features [g_lo, min(g_hi, g_m0 - 1)]: they start in the last T samples before the segment and end in its
-    // first min(S, T) (F g_lo + phi >= seg0 - T: g_lo - 1 is at most the last feature complete before this push)
-    const int64_t seam_hi = std::min(g_hi, g_m0 - 1);
-    if (seam_hi >= g_lo) {
-        const int64_t rows = P * d.C, total = rows * s->Sp;
-        const unsigned blocks = (unsigned)std::min<int64_t>((total + 255) / 256, 65536);
-        const int nseg = (int)(s->Sp - T);
-        if (s->dtype == B2CNN_DTYPE_BF16)
-            slide_seam_rows_kernel<__nv_bfloat16><<<blocks, 256, 0, st>>>(reinterpret_cast<const __nv_bfloat16 *>(x), pitch, tail_in,
-                                                                          (int)T, nseg, reinterpret_cast<float *>(s->stage), rows);
-        else
-            slide_seam_rows_kernel<float><<<blocks, 256, 0, st>>>(reinterpret_cast<const float *>(x), pitch, tail_in, (int)T, nseg,
-                                                                  reinterpret_cast<float *>(s->stage), rows);
-        if (cudaGetLastError() != cudaSuccess) { *err = "seam rows launch"; return B2CNN_ECUDA; }
-        if (ring_front(*s, cw, s->stage, B2CNN_DTYPE_F32, s->Sp, P, s->F * g_lo + s->phi - seg0 + T, g_lo, seam_hi - g_lo + 1, s->ring,
-                       s->ring_pitch, d.L, st, err) < 0)
-            return B2CNN_ECUDA;
-    }
-    {
-        const int64_t rows = P * d.C, total = rows * T;
-        if (s->dtype == B2CNN_DTYPE_BF16)
-            slide_gtail_kernel<__nv_bfloat16><<<(unsigned)((total + 255) / 256), 256, 0, st>>>(
-                reinterpret_cast<const __nv_bfloat16 *>(x), pitch, (int)S, (int)T, tail_in, tail_out, rows);
-        else
-            slide_gtail_kernel<float><<<(unsigned)((total + 255) / 256), 256, 0, st>>>(reinterpret_cast<const float *>(x), pitch, (int)S,
-                                                                                     (int)T, tail_in, tail_out, rows);
-        if (cudaGetLastError() != cudaSuccess) { *err = "tail launch"; return B2CNN_ECUDA; }
-    }
-    if (ev && cudaEventRecord(ev[1], st) != cudaSuccess) { *err = "cudaEventRecord"; return B2CNN_ECUDA; }
-    s->n = n1;
-    if (g_hi >= g_lo) s->g_done = g_hi;
-    s->tail_cur ^= 1;
-    return score_windows(s, hw, nullptr, age, n_age, apply_sigmoid, out, heads, emitted, window_index, ev, st, err);
-}
-
-int slide_create(const Dims &d, const TcState &tc, int n_patients, int stride, int dtype, int device, Slide **out,
-                 const char **err) {
-    *out = nullptr;
-    if (dtype != B2CNN_DTYPE_F32 && dtype != B2CNN_DTYPE_BF16) { *err = "dtype must be f32 (0) or bf16 (1)"; return B2CNN_EINVAL; }
-    if (n_patients < 1 || n_patients > (1 << 24)) { *err = "n_patients out of range"; return B2CNN_EINVAL; }
-    if (stride < 1 || stride > d.W) { *err = "stride must be in [1, window]"; return B2CNN_EINVAL; }
-    if (stride % 4 != 0) { *err = "stride must be a multiple of the feature stride (4 samples)"; return B2CNN_EINVAL; }
-    if (!tc.fused) {
-        *err = "the sliding-window scorer covers the streaming tensor-core geometries only (MyCNN5 or MyCNN2/3/4 conv/pool, "
-               "1 to 3 channels, tanh, no affine)";
-        return B2CNN_EARCH;
-    }
-    Slide *s = new (std::nothrow) Slide();
-    if (!s) { *err = "out of host memory"; return B2CNN_ESTATE; }
-    s->device = device; s->d = d; s->P = n_patients; s->S = stride; s->dtype = dtype;
-    s->R = d.K1 == 10 ? 24 : 16;
-    s->phi = (4 - d.W % 4) % 4;
-    s->ranges = tc.n_ranges;
-    s->ring_pitch = (n_patients + 3) & ~3;
-    s->Sp = (stride + 7) & ~7;
-    const int64_t P = n_patients, esz = dtype == B2CNN_DTYPE_BF16 ? 2 : 4;
-    bool ok = cudaMalloc(&s->ring, sizeof(float) * (size_t)d.L * s->ring_pitch) == cudaSuccess &&
-              cudaMalloc(&s->tail, sizeof(float) * (size_t)2 * P * d.C * kSlideTail) == cudaSuccess &&
-              cudaMalloc(&s->partial, sizeof(float) * (size_t)s->ranges * P * kGates) == cudaSuccess &&
-              cudaMalloc(&s->flags, sizeof(int) * (size_t)(2 * P + 1)) == cudaSuccess &&
+              (tcp ? cudaMalloc(&s->flags, sizeof(int) * (size_t)(2 * P + 1)) : cudaMalloc(&s->gates, sizeof(float) * (size_t)P * kGates)) ==
+                  cudaSuccess &&
               cudaMalloc(&s->stage, (size_t)(P * d.C * s->Sp * esz)) == cudaSuccess &&
               cudaMalloc(&s->seen, sizeof(int64_t) * (size_t)P) == cudaSuccess;
     if (!ok) { (void)cudaGetLastError(); slide_destroy(s); *err = "cudaMalloc(scorer state)"; return B2CNN_ECUDA; }
@@ -690,71 +614,42 @@ static int advance_seen(Slide *s, float *out, cudaStream_t st, const char **err)
     return 1;
 }
 
+
+static int score_windows(Slide *s, const HeadWeights &hw, const TcState *tc, const float *age, int64_t n_age, int apply_sigmoid,
+                         float *out, bool heads, int *emitted, int64_t *window_index, cudaEvent_t *ev, cudaStream_t st, const char **err);
+
 int slide_push(Slide *s, const ConvWeights &cw, const HeadWeights &hw, const TcState &tc, const void *x, int64_t pitch,
                const float *age, int64_t n_age, int apply_sigmoid, float *out, bool heads, int *emitted, int64_t *window_index,
                cudaEvent_t *ev, cudaStream_t st, const char **err) {
-    if (s->path == B2CNN_PATH_GENERIC)
-        return slide_push_generic(s, cw, hw, x, pitch, age, n_age, apply_sigmoid, out, heads, emitted, window_index, ev, st, err);
     const Dims &d = s->d;
-    const int64_t P = s->P, S = s->S, esz = s->dtype == B2CNN_DTYPE_BF16 ? 2 : 4;
-    if (pitch < S) { *err = "pitch must be >= stride"; return B2CNN_EINVAL; }
+    const bool tcp = s->path == B2CNN_PATH_TENSORCORE;
+    const int64_t P = s->P, S = s->S, T = s->T;
+    if (pitch < S || pitch > 0x7fffffff) { *err = "pitch must be in [stride, 2^31)"; return B2CNN_EINVAL; }
     if (n_age != 1 && n_age != P) { *err = "age must have 1 or n_patients elements"; return B2CNN_EINVAL; }
-    if (tc.n_ranges != s->ranges) { *err = "the handle's position ranges changed since create"; return B2CNN_ESTATE; }
+    if (tcp && tc.n_ranges != s->ranges) { *err = "the handle's position ranges changed since create"; return B2CNN_ESTATE; }
     const int64_t n1 = s->n + 1;
-    const int64_t g_hi = fdiv4(n1 * S - s->R - s->phi);      // last feature whose samples have all arrived
-    const int64_t g_m0 = s->n * S / 4;                        // first feature that starts inside the segment
-    int64_t g_lo = s->g_done + 1;
-    const int64_t G = window_head(*s, n1);
-    if (g_lo < G) g_lo = G;                                   // earlier features never enter a window
-    const float *tail_in = s->tail + (size_t)s->tail_cur * P * d.C * kSlideTail;
-    float *tail_out = s->tail + (size_t)(s->tail_cur ^ 1) * P * d.C * kSlideTail;
+    const int64_t g_hi = fdiv(n1 * S - s->R - s->phi, s->F);   // last feature whose samples have all arrived
+    const int64_t g_m0 = s->n * S / s->F;                       // first feature that starts inside the segment
+    const int64_t g_lo = std::max(s->g_done + 1, window_head(*s, n1));   // earlier features never enter a window
+    const float *tail_in = s->tail + (size_t)s->tail_cur * P * d.C * T;
+    float *tail_out = s->tail + (size_t)(s->tail_cur ^ 1) * P * d.C * T;
     if (ev && cudaEventRecord(ev[0], st) != cudaSuccess) { *err = "cudaEventRecord"; return B2CNN_ECUDA; }
-
-    // ---- main features [g_m0, g_hi]: tensor cores from the segment, exact re-computation of flagged patients
-    const int64_t Q = g_hi - g_m0 + 1;
-    if (Q >= 32) {
-        const int unit = 16 / (int)esz;
-        const void *xin = x;
-        int64_t xp = pitch;
-        if (s->phi != 0 || pitch % unit != 0 || (reinterpret_cast<uintptr_t>(x) & 15) != 0) {
-            const int64_t rows = P * d.C;
-            const unsigned blocks = (unsigned)((rows * s->Sp + 255) / 256 < 65536 ? (rows * s->Sp + 255) / 256 : 65536);
-            if (esz == 2)
-                slide_stage_kernel<uint16_t><<<blocks, 256, 0, st>>>(reinterpret_cast<const uint16_t *>(x), pitch, s->phi, (int)(S - s->phi),
-                                                                     reinterpret_cast<uint16_t *>(s->stage), s->Sp, rows);
-            else
-                slide_stage_kernel<float><<<blocks, 256, 0, st>>>(reinterpret_cast<const float *>(x), pitch, s->phi, (int)(S - s->phi),
-                                                                  reinterpret_cast<float *>(s->stage), s->Sp, rows);
-            if (cudaGetLastError() != cudaSuccess) { *err = "staging launch"; return B2CNN_ECUDA; }
-            xin = s->stage; xp = s->Sp;
-        }
-        Dims dseg = d;
-        dseg.W = (int)(S - s->phi); dseg.L = (int)Q; dseg.XP = (int)xp;
-        if (cudaMemsetAsync(s->flags, 0, sizeof(int) * (size_t)(2 * P + 1), st) != cudaSuccess) { *err = "memset flags"; return B2CNN_ECUDA; }
-        if (tc_ring_features(tc, dseg, cw, xin, xp, s->dtype, P, s->ring, s->ring_pitch, d.L, (int)(g_m0 % d.L), s->flags, st, err) < 0)
-            return B2CNN_ECUDA;
-        if (launch_exact(*s, cw, x, pitch, tail_in, g_m0, Q, s->flags + P, s->flags + 2 * P, st, err) < 0) return B2CNN_ECUDA;
-    } else if (launch_exact(*s, cw, x, pitch, tail_in, g_m0, Q, nullptr, nullptr, st, err) < 0) {
-        return B2CNN_ECUDA;
-    }
-    // ---- seam features [g_lo, g_m0 - 1]: receptive field starts in the previous push
-    const int64_t seam_hi = g_hi < g_m0 - 1 ? g_hi : g_m0 - 1;
-    if (launch_exact(*s, cw, x, pitch, tail_in, g_lo, seam_hi - g_lo + 1, nullptr, nullptr, st, err) < 0) return B2CNN_ECUDA;
-    {
-        const int64_t rows = P * d.C, total = rows * kSlideTail;
-        if (esz == 2)
-            slide_tail_kernel<__nv_bfloat16><<<(unsigned)((total + 255) / 256), 256, 0, st>>>(
-                reinterpret_cast<const __nv_bfloat16 *>(x), pitch, (int)S, tail_in, tail_out, rows);
-        else
-            slide_tail_kernel<float><<<(unsigned)((total + 255) / 256), 256, 0, st>>>(reinterpret_cast<const float *>(x), pitch, (int)S,
-                                                                                    tail_in, tail_out, rows);
-        if (cudaGetLastError() != cudaSuccess) { *err = "tail launch"; return B2CNN_ECUDA; }
-    }
+    const int rc = tcp ? push_features_tc(s, cw, tc, x, pitch, tail_in, g_lo, g_m0, g_hi, st, err)
+                       : push_features_generic(s, cw, x, pitch, tail_in, g_lo, g_m0, g_hi, st, err);
+    if (rc < 0) return B2CNN_ECUDA;
+    const int64_t rows = P * d.C, blocks = (rows * T + 255) / 256;
+    if (s->dtype == B2CNN_DTYPE_BF16)
+        slide_shift_tail_kernel<__nv_bfloat16><<<(unsigned)blocks, 256, 0, st>>>(reinterpret_cast<const __nv_bfloat16 *>(x), pitch, (int)S,
+                                                                                 (int)T, tail_in, tail_out, rows);
+    else
+        slide_shift_tail_kernel<float><<<(unsigned)blocks, 256, 0, st>>>(reinterpret_cast<const float *>(x), pitch, (int)S, (int)T, tail_in,
+                                                                         tail_out, rows);
+    if (cudaGetLastError() != cudaSuccess) { *err = "tail launch"; return B2CNN_ECUDA; }
     if (ev && cudaEventRecord(ev[1], st) != cudaSuccess) { *err = "cudaEventRecord"; return B2CNN_ECUDA; }
     s->n = n1;
     if (g_hi >= g_lo) s->g_done = g_hi;
     s->tail_cur ^= 1;
-    return score_windows(s, hw, &tc, age, n_age, apply_sigmoid, out, heads, emitted, window_index, ev, st, err);
+    return score_windows(s, hw, tcp ? &tc : nullptr, age, n_age, apply_sigmoid, out, heads, emitted, window_index, ev, st, err);
 }
 
 // one row of a push: the scorer's model (row 0) or head r - 1, with what its projection and head need
@@ -928,7 +823,6 @@ struct AdmitLayout {
     int64_t kp, cap, hp;
     size_t scratch, flags, idx, stage, total;
 };
-static size_t al256(size_t b) { return (b + 255) & ~(size_t)255; }
 static AdmitLayout admit_layout(const Slide &s, int64_t k, int64_t H) {
     AdmitLayout a;
     const int64_t esz = s.dtype == B2CNN_DTYPE_BF16 ? 2 : 4;
@@ -972,7 +866,6 @@ int slide_admit(Slide *s, const ConvWeights &cw, const TcState &tc, const int *p
     if (cudaMemcpyAsync(idx, patients, sizeof(int) * (size_t)k, cudaMemcpyHostToDevice, st) != cudaSuccess) {
         *err = "copy of the patient indices"; return B2CNN_ECUDA;
     }
-    const int64_t esz = s->dtype == B2CNN_DTYPE_BF16 ? 2 : 4;
     // the history is stream samples [nS - H, nS): the features wholly inside it that lie in the current window n
     // (features() may read it before the next push) or can still enter a later one
     const int64_t nS = s->n * s->S;
@@ -984,36 +877,11 @@ int slide_admit(Slide *s, const ConvWeights &cw, const TcState &tc, const int *p
         const int rc2 = ring_front(*s, cw, hist, s->dtype, pitch, k, s->F * g_lo + s->phi - (nS - H), g_lo, Q, scratch, a.kp, Q, st, err);
         if (rc2 < 0) return rc2 == kLaunchArch ? B2CNN_EARCH : B2CNN_ECUDA;
     } else if (H > 0 && Q > 0) {
-        const int cap = (int)Q;                                        // Q <= a.cap
-        const int64_t off = 4 * g_lo + s->phi - (nS - H);               // (H - W) mod 4 + 4 (g_lo - first feature inside)
-        SlideExactParams p;
+        SlideExactParams p;                                            // into the scratch ring, slot g mod Q (Q <= a.cap)
         memset(&p, 0, sizeof p);
-        p.x = hist; p.pitch = pitch; p.tail = s->tail; p.ring = scratch; p.ring_pitch = a.kp; p.cap = cap; p.P = (int)k;
+        p.x = hist; p.pitch = pitch; p.tail = s->tail; p.ring = scratch; p.ring_pitch = a.kp; p.cap = (int)Q; p.P = (int)k;
         p.g0 = g_lo; p.seg0 = nS - H; p.phi = s->phi; p.cw = cw;
-        if (Q >= 32) {
-            const int unit = 16 / (int)esz;
-            const void *xin = hist;
-            int64_t xp = pitch;
-            if (off != 0 || pitch % unit != 0 || (reinterpret_cast<uintptr_t>(hist) & 15) != 0) {
-                const int64_t rows = k * d.C;
-                const unsigned blocks = (unsigned)std::min<int64_t>((rows * a.hp + 255) / 256, 65536);
-                if (esz == 2)
-                    slide_stage_kernel<uint16_t><<<blocks, 256, 0, st>>>(reinterpret_cast<const uint16_t *>(hist), pitch, (int)off,
-                                                                         (int)(H - off), reinterpret_cast<uint16_t *>(stage), a.hp, rows);
-                else
-                    slide_stage_kernel<float><<<blocks, 256, 0, st>>>(reinterpret_cast<const float *>(hist), pitch, (int)off,
-                                                                      (int)(H - off), reinterpret_cast<float *>(stage), a.hp, rows);
-                if (cudaGetLastError() != cudaSuccess) { *err = "staging launch"; return B2CNN_ECUDA; }
-                xin = stage; xp = a.hp;
-            }
-            Dims dh = d;
-            dh.W = (int)(H - off); dh.L = cap; dh.XP = (int)xp;
-            if (cudaMemsetAsync(flags, 0, sizeof(int) * (size_t)(2 * k + 1), st) != cudaSuccess) { *err = "memset flags"; return B2CNN_ECUDA; }
-            if (tc_ring_features(tc, dh, cw, xin, xp, s->dtype, k, scratch, a.kp, cap, (int)mod_nn(g_lo, cap), flags, st, err) < 0)
-                return B2CNN_ECUDA;
-            p.list = flags + k; p.count = flags + 2 * k;                // flagged histories: exact, over all Q features
-        }
-        if (launch_exact_p(p, *s, Q, st, err) < 0) return B2CNN_ECUDA;
+        if (tc_ring_block(*s, tc, p, Q, H, stage, a.hp, flags, st, err) < 0) return B2CNN_ECUDA;
     }
     if (H > 0 && Q > 0) {
         const unsigned gy = (unsigned)std::min<int64_t>(Q, 1024);
@@ -1023,20 +891,13 @@ int slide_admit(Slide *s, const ConvWeights &cw, const TcState &tc, const int *p
     }
     // the next push's seam features read the history's last samples from the current tail
     float *tail = s->tail + (size_t)s->tail_cur * s->P * d.C * s->T;
-    const int64_t total = k * d.C * s->T;
-    if (s->path == B2CNN_PATH_GENERIC) {
-        if (esz == 2)
-            slide_admit_gtail_kernel<__nv_bfloat16><<<(unsigned)((total + 255) / 256), 256, 0, st>>>(
-                reinterpret_cast<const __nv_bfloat16 *>(hist), pitch, H, idx, (int)k, d.C, s->T, tail);
-        else
-            slide_admit_gtail_kernel<float><<<(unsigned)((total + 255) / 256), 256, 0, st>>>(reinterpret_cast<const float *>(hist), pitch,
-                                                                                             H, idx, (int)k, d.C, s->T, tail);
-    } else if (esz == 2)
-        slide_admit_tail_kernel<__nv_bfloat16><<<(unsigned)((total + 255) / 256), 256, 0, st>>>(
-            reinterpret_cast<const __nv_bfloat16 *>(hist), pitch, H, idx, (int)k, d.C, tail);
+    const int64_t blocks = (k * d.C * s->T + 255) / 256;
+    if (s->dtype == B2CNN_DTYPE_BF16)
+        slide_seed_tail_kernel<__nv_bfloat16><<<(unsigned)blocks, 256, 0, st>>>(reinterpret_cast<const __nv_bfloat16 *>(hist), pitch, H, idx,
+                                                                                (int)k, d.C, s->T, tail);
     else
-        slide_admit_tail_kernel<float><<<(unsigned)((total + 255) / 256), 256, 0, st>>>(reinterpret_cast<const float *>(hist), pitch, H,
-                                                                                        idx, (int)k, d.C, tail);
+        slide_seed_tail_kernel<float><<<(unsigned)blocks, 256, 0, st>>>(reinterpret_cast<const float *>(hist), pitch, H, idx, (int)k, d.C,
+                                                                        s->T, tail);
     if (cudaGetLastError() != cudaSuccess) { *err = "tail launch"; return B2CNN_ECUDA; }
     std::vector<int64_t> next = next_seen(*s, patients, k, H);
     if ((rc = commit_seen(s, next, st, err)) != B2CNN_OK) return rc;
@@ -1306,317 +1167,6 @@ int slide_import(Slide *s, const ConvWeights &cw, const int *patients, int64_t k
     // as after an admission with a full history: the next push computes the seam features from the window's last one on
     const int64_t g_hi = fdiv(s->n * s->S - s->R - s->phi, s->F);
     if (g_hi < s->g_done) s->g_done = g_hi;
-    return B2CNN_OK;
-}
-
-// ---- whole recordings (b2cnn_score_record) ------------------------------------------------------------------------
-// A recording of N samples has L_N = (N - R) / F + 1 features on one lattice: feature g reads samples F g .. F g + R - 1.
-// Every window starts at a multiple of S (S % F == 0), so window w (samples w S .. w S + W - 1) is features w S / F ..
-// w S / F + L - 1 of that lattice (phase 0), and each feature is computed once however many windows hold it.
-//   * fold: each recording is cut into nr rows of K features; row r carries samples r K F .. r K F + F (K - 1) + R - 1
-//     (the R - F sample halo), copied into 16-byte aligned staging rows [B nr][C][Kp] (zeros past the recording's end).
-//     The front end runs once over all B nr rows and stores row (b, r) at feats[b Lp + r K + j], Lp = nr K: one
-//     record-major buffer [B][Lp].  Tensor-core path: tc_row_features, K = ceil(L_N / nr) rounded up to 8 with nr =
-//     ceil(L_N / kRecRowFeats), so that one 24 h recording still gives ~660 rows; a NaN / inf sample flags (and sends
-//     through the exact kernel) its row only.  Generic path: launch_frontend_generic with K = L, predict()'s tile.
-//   * projection: the B n_w (recording, window) pairs are the M rows of one launch.  Tensor-core path:
-//     slide_record_proj_kernel, the arithmetic of slide_ring_proj_kernel per window with 128 windows per CTA sharing
-//     each W_ih chunk; generic path: launch_record_head (proj_body with a per-row base), predict()'s tiles and order.
-//   * head: launch_reduce_lstm_head (tensor cores) or reduce_gates + head_independent (generic) over the M rows, with
-//     each recording's age repeated over its windows.  Sequence mode (the LSTM carried over each recording's windows,
-//     utils.run_model's batch-as-sequence call per recording): reduce_gates over the same partials (tc.n_ranges slices
-//     on the tensor-core path, as forward's tensor-core sequence mode sums them), then head_sequence with one warp per
-//     recording scanning its n_w gate rows.
-// Launches per call: stage, tensor-core front end, flag compaction, exact re-computation, age, projection, head
-// (tensor-core path, plus the flag memset; reduction + scan in sequence mode) or stage, front end, age, projection,
-// reduction, head (generic path) -- whatever B, N and S.
-constexpr int64_t kRecRowFeats = 4096;
-
-struct RecordPlan {
-    bool tc, seq;
-    int F, R, ranges;
-    int64_t n_w, L_N, K, nr, rows, Lp, row_len, Kp, step, M;
-    size_t stage, feats, flags, partial, gates, age, total;
-};
-
-// the plan of a call; false with *err and *code when an argument is out of range
-static bool record_plan(const Dims &d, const TcState &tc, bool use_tc, int64_t B, int64_t N, int64_t stride, int dtype, int mode,
-                        RecordPlan *o, int *code, const char **err) {
-    RecordPlan &p = *o;
-    memset(&p, 0, sizeof p);
-    p.tc = use_tc;
-    p.seq = mode == B2CNN_MODE_SEQUENCE;
-    p.F = d.PS * d.PS;
-    p.R = d.PS * (d.PK + d.K2 - 2) + d.PK + d.K1 - 1;
-    *code = B2CNN_EINVAL;
-    if (mode != B2CNN_MODE_INDEPENDENT && mode != B2CNN_MODE_SEQUENCE) {
-        *err = "mode must be B2CNN_MODE_INDEPENDENT or B2CNN_MODE_SEQUENCE"; return false;
-    }
-    if (B < 1 || B > 0x7fffffff) { *err = "the recording count must be in [1, 2^31)"; return false; }
-    if (N < 0) { *err = "the recording length must be >= 0"; return false; }
-    if (stride < 1 || stride % p.F != 0) {
-        *err = use_tc ? "stride must be a positive multiple of the feature stride (4 samples)"
-                      : "stride must be a positive multiple of the feature stride (pool_s^2 samples)";
-        return false;
-    }
-    p.n_w = N >= d.W ? (N - d.W) / stride + 1 : 0;
-    if (p.n_w == 0) return true;
-    p.L_N = (N - p.R) / p.F + 1;
-    p.step = stride / p.F;
-    if (use_tc) {
-        p.nr = (p.L_N + kRecRowFeats - 1) / kRecRowFeats;
-        p.K = ((p.L_N + p.nr - 1) / p.nr + 7) & ~(int64_t)7;
-    } else {
-        p.K = d.L;
-        p.nr = (p.L_N + p.K - 1) / p.K;
-    }
-    p.rows = B * p.nr;
-    p.M = B * p.n_w;
-    // the kernels index rows, windows and their gate rows with 32-bit integers
-    if (p.rows > 0x7fffffff / kGates || p.M > 0x7fffffff / kGates) {
-        *err = "too many rows: recordings x windows (or x folded rows) must stay below 2^25"; return false;
-    }
-    p.Lp = p.nr * p.K;
-    p.row_len = p.F * (p.K - 1) + p.R;
-    p.Kp = (p.row_len + 7) & ~(int64_t)7;
-    p.ranges = use_tc ? tc.n_ranges : proj_slices(d.L);
-    const int64_t esz = dtype == B2CNN_DTYPE_BF16 ? 2 : 4;
-    p.stage = al256((size_t)(p.rows * d.C * p.Kp * esz));
-    p.feats = al256(sizeof(float) * (size_t)(B * p.Lp));
-    p.flags = use_tc ? al256(sizeof(int) * (size_t)(2 * p.rows + 1)) : 0;
-    p.partial = al256(sizeof(float) * (size_t)p.ranges * (size_t)p.M * kGates);
-    p.gates = use_tc && !p.seq ? 0 : al256(sizeof(float) * (size_t)p.M * kGates);   // the fused tensor-core head sums in registers
-    p.age = al256(sizeof(float) * (size_t)p.M);
-    p.total = p.stage + p.feats + p.flags + p.partial + p.gates + p.age;
-    *code = B2CNN_OK;
-    return true;
-}
-
-// staging rows: row (b, r) channel c = samples r step_s .. r step_s + row_len - 1 of recording b's channel c, zeros past
-// N and past row_len up to Kp; blockIdx.y strides the B nr C row-channels.  A thread writes 16 bytes (Kp % 8 == 0: every
-// staging row is 16-byte aligned) from element loads, which take any alignment of the recording.
-template <typename T>
-__global__ void record_stage_kernel(const T *__restrict__ x, int64_t pitch, int C, int64_t N, int64_t nr, int64_t step_s, int64_t row_len,
-                                    int64_t Kp, T *__restrict__ dst, int64_t row_channels) {
-    constexpr int V = 16 / sizeof(T);
-    for (int64_t rc = blockIdx.y; rc < row_channels; rc += gridDim.y) {
-        const int64_t row = rc / C, c = rc - row * C, b = row / nr, r = row - b * nr;
-        const T *src = x + (b * C + c) * pitch + r * step_s;
-        const int64_t n = min(row_len, N - r * step_s);
-        T *out = dst + rc * Kp;
-        for (int64_t i0 = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) * V; i0 < Kp; i0 += (int64_t)gridDim.x * blockDim.x * V) {
-            union { uint4 u; T e[V]; } v;
-#pragma unroll
-            for (int j = 0; j < V; ++j) v.e[j] = i0 + j < n ? __ldg(src + i0 + j) : T(0);
-            *reinterpret_cast<uint4 *>(out + i0) = v.u;
-        }
-    }
-}
-
-// age of row m = recording m / n_w's
-__global__ void record_age_kernel(const float *__restrict__ age, int64_t n_age, int64_t n_w, int64_t M, float *__restrict__ dst) {
-    const int64_t m = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (m < M) dst[m] = age[n_age == 1 ? 0 : m / n_w];
-}
-
-// The tensor-core projection of whole recordings.  CTA = (128 (recording, window) rows, range); per window the
-// arithmetic of slide_ring_proj_kernel (HP = 1): the same ranges, 16-position chunks in the same order, A pieces and 12
-// MMAs per chunk with the handle's packed W_ih chunks -- which the CTA's 128 windows share.  A window's features start
-// at any float offset (w S / F), so instead of TMA boxes each consumer thread loads its window's 16 consecutive floats
-// of the chunk (whole sectors), one chunk ahead: the loads of chunk m + 1 are in flight during chunk m's MMAs.
-//   warp 4: the W_ih chunks (bulk copies, two stages); warps 0-3: thread == window.
-struct RecordProjParams {
-    const float *feats;              // [B][rec_pitch]
-    const uint8_t *wpack;            // [n_ranges][chunks_per_cta][kRpWChunk]
-    float *partial;                  // [n_ranges][M][64]
-    int64_t rec_pitch, step;         // recording pitch and window step in features
-    int M, n_w, L, feats_per_cta, chunks_per_cta, foff;
-};
-constexpr size_t kRecProjSmem = 1024 + 2 * kRpWChunk + 3 * kRpPiece + 64;
-
-__global__ void __launch_bounds__(kRpThreads) slide_record_proj_kernel(const __grid_constant__ RecordProjParams p) {
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t *smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-    uint8_t *sW = smem;                                            // [2 stages][6 KB]
-    uint8_t *sPc = sW + 2 * kRpWChunk;                             // [3 pieces][4 KB]
-    uint64_t *bars = reinterpret_cast<uint64_t *>(sPc + 3 * kRpPiece);
-    const uint32_t bar_full = smem_u32(bars + 0), bar_empty = smem_u32(bars + 2);
-    const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);
-    const int lane = threadIdx.x & 31;
-    const int b0 = blockIdx.x * kRpM;
-    const int lo = blockIdx.y * p.feats_per_cta, hi = min(p.L, lo + p.feats_per_cta);
-    const int nch = p.chunks_per_cta;
-    if (threadIdx.x == 0) {
-        for (int i = 0; i < 2; ++i) { mbar_init(bar_full + 8 * i, 1); mbar_init(bar_empty + 8 * i, 4); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncthreads();
-    if (warp == 4) {
-        if (lane == 0) {
-            for (int m = 0; m < nch; ++m) {
-                const int u = m & 1;
-                mbar_wait(bar_empty + 8 * u, ((m >> 1) & 1) ^ 1);
-                mbar_expect_tx(bar_full + 8 * u, kRpWChunk);
-                bulk_load_1d(smem_u32(sW + u * kRpWChunk), p.wpack + ((size_t)blockIdx.y * nch + m) * kRpWChunk, kRpWChunk, bar_full + 8 * u);
-            }
-        }
-        return;
-    }
-    const int row = threadIdx.x, b = b0 + row;
-    const bool row_ok = b < p.M;
-    const float *fr = p.feats;
-    if (row_ok) {
-        const int r = b / p.n_w;
-        fr += (int64_t)r * p.rec_pitch + (int64_t)(b - r * p.n_w) * p.step;
-    }
-    float gacc[2][32];
-#pragma unroll
-    for (int h = 0; h < 2; ++h)
-#pragma unroll
-        for (int i = 0; i < 32; ++i) gacc[h][i] = 0.f;
-    uint8_t *arow = sPc + (row >> 3) * 256 + (row & 7) * 16;
-    float v[16];
-    auto load = [&](int m) {
-        const int q0 = lo + 16 * m - p.foff;
-#pragma unroll
-        for (int k = 0; k < 16; ++k) {
-            const int q = q0 + k;
-            v[k] = row_ok && q >= lo && q < hi ? __ldg(fr + q) : 0.f;
-        }
-    };
-    load(0);
-#pragma unroll 1
-    for (int m = 0; m < nch; ++m) {
-        const int u = m & 1;
-#pragma unroll
-        for (int kk = 0; kk < 8; ++kk) {
-            const float f0 = v[2 * kk], f1 = v[2 * kk + 1];
-            const uint32_t h = pack_bf16x2(f0, f1);
-            const float r1x = f0 - __uint_as_float(h << 16), r1y = f1 - __uint_as_float(h & 0xffff0000u);
-            const uint32_t md = pack_bf16x2(r1x, r1y);
-            const uint32_t lw = pack_bf16x2(r1x - __uint_as_float(md << 16), r1y - __uint_as_float(md & 0xffff0000u));
-            const int off = (kk >> 2) * 128 + (kk & 3) * 4;
-            *reinterpret_cast<uint32_t *>(arow + off) = h;
-            *reinterpret_cast<uint32_t *>(arow + kRpPiece + off) = md;
-            *reinterpret_cast<uint32_t *>(arow + 2 * kRpPiece + off) = lw;
-        }
-        fence_proxy_async();
-        wg_bar();
-        mbar_wait(bar_full + 8 * u, (m >> 1) & 1);
-        const uint32_t pa = smem_u32(sPc), pw = smem_u32(sW + u * kRpWChunk);
-        wgmma_fence();
-#pragma unroll
-        for (int hh = 0; hh < 2; ++hh) {
-            constexpr int kAp[6] = {0, 0, 1, 0, 2, 1}, kWp[6] = {0, 1, 0, 2, 0, 1};
-#pragma unroll
-            for (int q = 0; q < 6; ++q)
-                wgmma_m64n64(gacc[hh], gdesc_none_kmajor(pa + kAp[q] * kRpPiece + hh * 2048, 128, 256),
-                             gdesc_none_kmajor(pw + kWp[q] * 2048, 128, 256));
-        }
-        wgmma_commit();
-        if (m + 1 < nch) load(m + 1);                              // in flight during the MMAs
-        wgmma_wait<0>();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(bar_empty + 8 * u);
-        wg_bar();                                                  // A tile free for the next chunk
-    }
-#pragma unroll
-    for (int hh = 0; hh < 2; ++hh)
-#pragma unroll
-        for (int e2 = 0; e2 < 2; ++e2) {
-            const int bb = b0 + 64 * hh + 16 * warp + (lane >> 2) + 8 * e2;
-            if (bb < p.M) {
-                float *dst = p.partial + ((int64_t)blockIdx.y * p.M + bb) * kGates + 2 * (lane & 3);
-#pragma unroll
-                for (int e = 2 * e2; e < 32; e += 4)
-                    *reinterpret_cast<float2 *>(dst + 8 * (e >> 2)) = make_float2(gacc[hh][e], gacc[hh][e + 1]);
-            }
-        }
-}
-
-int64_t record_workspace_bytes(const Dims &d, const TcState &tc, bool use_tc, int64_t B, int64_t N, int64_t stride, int dtype, int mode,
-                               const char **err) {
-    RecordPlan p;
-    int code;
-    if (!record_plan(d, tc, use_tc, B, N, stride, dtype, mode, &p, &code, err)) return -1;
-    return (int64_t)p.total;
-}
-
-int score_record(const Dims &d, const ConvWeights &cw, const HeadWeights &hw, const TcState &tc, bool use_tc, int num_sms, const void *x,
-                 int dtype, int64_t B, int64_t N, int64_t pitch, int64_t stride, int mode, const float *age, int64_t n_age, int apply_sigmoid,
-                 float *out, void *ws, int64_t ws_bytes, cudaStream_t st, const char **err) {
-    RecordPlan p;
-    int code;
-    if (!record_plan(d, tc, use_tc, B, N, stride, dtype, mode, &p, &code, err)) return code;
-    if (pitch < N || pitch < 1) { *err = "pitch must be >= the recording length"; return B2CNN_EINVAL; }
-    if (n_age != 1 && n_age != B) { *err = "age must have 1 or B elements"; return B2CNN_EINVAL; }
-    if (p.n_w == 0) return B2CNN_OK;
-    if (!ws || ws_bytes < (int64_t)p.total || (reinterpret_cast<uintptr_t>(ws) & 255) != 0) {
-        *err = "workspace missing, not 256-byte aligned or smaller than b2cnn_record_workspace_bytes()"; return B2CNN_ESTATE;
-    }
-    Dims dr = d;                                                   // one folded row
-    dr.L = (int)p.K; dr.W = (int)p.row_len; dr.XP = (int)p.Kp;
-    if (!use_tc && !frontend_generic_fits(dr)) {
-        *err = "the generic front end's tile does not fit shared memory (in_channels * pool_s^2 too large for this window length)";
-        return B2CNN_EARCH;
-    }
-    char *base = static_cast<char *>(ws);
-    void *stage = base;
-    float *feats = reinterpret_cast<float *>(base + p.stage);
-    int *flags = reinterpret_cast<int *>(base + p.stage + p.feats);
-    float *partial = reinterpret_cast<float *>(base + p.stage + p.feats + p.flags);
-    float *gates = reinterpret_cast<float *>(base + p.stage + p.feats + p.flags + p.partial);
-    float *ages = reinterpret_cast<float *>(base + p.stage + p.feats + p.flags + p.partial + p.gates);
-    // ---- fold: staging rows
-    {
-        const int64_t rc = p.rows * d.C;
-        const int64_t per_block = 256 * (dtype == B2CNN_DTYPE_BF16 ? 8 : 4);
-        const dim3 grid((unsigned)std::min<int64_t>((p.Kp + per_block - 1) / per_block, 16), (unsigned)std::min<int64_t>(rc, 65535));
-        const int64_t step_s = p.K * p.F;
-        if (dtype == B2CNN_DTYPE_BF16)
-            record_stage_kernel<uint16_t><<<grid, 256, 0, st>>>(static_cast<const uint16_t *>(x), pitch, d.C, N, p.nr, step_s, p.row_len, p.Kp,
-                                                                 static_cast<uint16_t *>(stage), rc);
-        else
-            record_stage_kernel<float><<<grid, 256, 0, st>>>(static_cast<const float *>(x), pitch, d.C, N, p.nr, step_s, p.row_len, p.Kp,
-                                                              static_cast<float *>(stage), rc);
-        if (cudaGetLastError() != cudaSuccess) { *err = "staging launch"; return B2CNN_ECUDA; }
-    }
-    // ---- front end: every row's K features into feats[b Lp + r K + j]
-    if (use_tc) {
-        if (cudaMemsetAsync(flags, 0, sizeof(int) * (size_t)(2 * p.rows + 1), st) != cudaSuccess) { *err = "memset flags"; return B2CNN_ECUDA; }
-        if (tc_row_features(tc, dr, cw, stage, p.Kp, dtype, p.rows, feats, p.K, flags, num_sms, st, err) < 0) return B2CNN_ECUDA;
-    } else {
-        // the rows hold at most L features, often one tile: four times predict()'s CTAs per SM keep the SMs busy (the
-        // grid does not change what a CTA computes)
-        const int rc = launch_frontend_generic(dr, cw, stage, dtype, p.rows, feats, p.K, 1, st, 4 * num_sms, err);
-        if (rc < 0) return rc == kLaunchArch ? B2CNN_EARCH : B2CNN_ECUDA;
-    }
-    // ---- each recording's age over its windows
-    record_age_kernel<<<(unsigned)((p.M + 255) / 256), 256, 0, st>>>(age, n_age, p.n_w, p.M, ages);
-    if (cudaGetLastError() != cudaSuccess) { *err = "age launch"; return B2CNN_ECUDA; }
-    // ---- projection + head over the B n_w windows
-    if (!use_tc) {
-        if (launch_record_head(d, hw, feats, p.Lp, (int)p.n_w, p.step, p.M, ages, p.M, mode, apply_sigmoid, out, gates, partial, st, err) < 0)
-            return B2CNN_ECUDA;
-        return B2CNN_OK;
-    }
-    RecordProjParams rp;
-    rp.feats = feats; rp.wpack = reinterpret_cast<const uint8_t *>(tc.d_wpack); rp.partial = partial;
-    rp.rec_pitch = p.Lp; rp.step = p.step;
-    rp.M = (int)p.M; rp.n_w = (int)p.n_w; rp.L = d.L;
-    rp.feats_per_cta = tc.feats_per_cta; rp.chunks_per_cta = tc.chunks_per_cta; rp.foff = d.K1 == 10 ? 3 : 2;
-    if (cudaFuncSetAttribute(slide_record_proj_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kRecProjSmem) != cudaSuccess) {
-        *err = "projection smem attribute"; return B2CNN_ECUDA;
-    }
-    slide_record_proj_kernel<<<dim3((unsigned)((p.M + kRpM - 1) / kRpM), (unsigned)tc.n_ranges), kRpThreads, kRecProjSmem, st>>>(rp);
-    if (cudaGetLastError() != cudaSuccess) { *err = "projection launch"; return B2CNN_ECUDA; }
-    if (p.seq) {
-        if (launch_reduce_gates(partial, tc.n_ranges, p.M, hw, gates, st, err) < 0 ||
-            launch_sequence_segments(d, hw, gates, B, p.n_w, ages, p.M, apply_sigmoid, out, st, err) < 0)
-            return B2CNN_ECUDA;
-        return B2CNN_OK;
-    }
-    if (launch_reduce_lstm_head(d, hw, partial, tc.n_ranges, p.M, ages, p.M, apply_sigmoid, out, st, err) < 0) return B2CNN_ECUDA;
     return B2CNN_OK;
 }
 

@@ -5,13 +5,12 @@
 namespace b2cnn {
 
 struct Slide;
-// `d`: the model's geometry; the scorer keeps a copy.  Checks stride and geometry, allocates all device state.
-int slide_create(const Dims &d, const TcState &tc, int n_patients, int stride, int dtype, int device, Slide **out,
+// `d`: the model's geometry; the scorer keeps a copy.  Checks stride and geometry, allocates all device state.  path:
+// B2CNN_PATH_TENSORCORE (the geometries `tc` holds in its streaming kernels, else B2CNN_EARCH) or B2CNN_PATH_GENERIC
+// (exact CUDA-core kernels for any geometry b2cnn_create accepts; B2CNN_EARCH, before allocating anything, where the
+// generic front end's tile does not fit shared memory, with num_sms sizing its grid); stride % pool_s^2 == 0
+int slide_create(const Dims &d, const TcState &tc, int path, int n_patients, int stride, int dtype, int device, int num_sms, Slide **out,
                  const char **err);
-// the generic path: exact CUDA-core kernels for any geometry b2cnn_create accepts (B2CNN_EARCH, before allocating
-// anything, where the generic front end's tile does not fit shared memory); stride % pool_s^2 == 0
-int slide_create_generic(const Dims &d, int n_patients, int stride, int dtype, int device, int num_sms, Slide **out,
-                         const char **err);
 int slide_path(const Slide *s);   // B2CNN_PATH_TENSORCORE or B2CNN_PATH_GENERIC
 void slide_destroy(Slide *s);
 int slide_device(const Slide *s);
@@ -50,15 +49,5 @@ int slide_export(const Slide *s, const ConvWeights &cw, const int *patients, int
                  b2cnn_slide_state_header *hdr, void *ws, int64_t ws_bytes, cudaStream_t st, const char **err);
 int slide_import(Slide *s, const ConvWeights &cw, const int *patients, int64_t k, const b2cnn_slide_state_header &hdr, const float *feats,
                  const float *tails, const int64_t *seen_host, void *ws, int64_t ws_bytes, cudaStream_t st, const char **err);
-
-// whole recordings (b2cnn_score_record): x [B][C][pitch], out [B][n_w], n_w = (N - W) / stride + 1 (0 for N < W).
-// use_tc: the tensor-core path (the caller has checked that the handle's TcState holds the model).  The workspace size
-// is -1 (with *err) for bad arguments.  mode: B2CNN_MODE_INDEPENDENT (every window from the zero LSTM state) or
-// B2CNN_MODE_SEQUENCE (the LSTM carried over each recording's windows in order, from the zero state per recording).
-int64_t record_workspace_bytes(const Dims &d, const TcState &tc, bool use_tc, int64_t B, int64_t N, int64_t stride, int dtype, int mode,
-                               const char **err);
-int score_record(const Dims &d, const ConvWeights &cw, const HeadWeights &hw, const TcState &tc, bool use_tc, int num_sms, const void *x,
-                 int dtype, int64_t B, int64_t N, int64_t pitch, int64_t stride, int mode, const float *age, int64_t n_age, int apply_sigmoid,
-                 float *out, void *ws, int64_t ws_bytes, cudaStream_t st, const char **err);
 
 }  // namespace b2cnn

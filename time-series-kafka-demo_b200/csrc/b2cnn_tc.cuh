@@ -53,7 +53,7 @@ int tc_features(TcState &s, const Dims &d, const ConvWeights &cw, const void *x,
 int tc_ring_features(const TcState &s, const Dims &dseg, const ConvWeights &cw, const void *x, int64_t pitch, int dtype,
                      int64_t P, float *ring, int64_t ring_pitch, int cap, int slot0, int *flags, cudaStream_t st, const char **err);
 int tc_ring_tmap(const float *ring, int64_t P, int64_t pitch, int L, CUtensorMap *tm, const char **err);
-// whole recordings (b2cnn_slide.cu, b2cnn_score_record): the features of `rows` staged rows into feats[row sB + j],
+// whole recordings (b2cnn_record.cu, b2cnn_score_record): the features of `rows` staged rows into feats[row sB + j],
 // flagged rows recomputed exactly
 int tc_row_features(const TcState &s, const Dims &dseg, const ConvWeights &cw, const void *x, int64_t pitch, int dtype,
                     int64_t rows, float *feats, int64_t sB, int *flags, int num_sms, cudaStream_t st, const char **err);
