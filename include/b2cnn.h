@@ -474,7 +474,12 @@ const char *b2cnn_version(void);
  *   mask1 [B][4][P1], mask2 [B][L_out]: the two nn.Dropout(0.1) masks of bin/models.py:25,28 ALREADY scaled by 1/(1-p)
  *                   (torch's Philox stream cannot be reproduced here, so the caller draws them); NULL = no dropout
  *   loss_out        one float: the mean BCE-with-logits loss of this batch (before the update)
- * The call allocates nothing and is asynchronous on `stream`. */
+ * The call allocates nothing and is asynchronous on `stream`.
+ * workspace: b2cnn_train_workspace_bytes(cfg, B) bytes; a smaller one is B2CNN_ESTATE before any launch.  The layout
+ * follows the kernels the shape runs, chosen from L_out alone: below 1024 features one CTA per window with every
+ * intermediate in the workspace (about 8 floats per input position and window); from 1024 features on position tiles
+ * that recompute the conv backward in shared memory, and the workspace holds f, d f, the LSTM records and one region
+ * of partial sums (about 2 * 4 * B * L_out bytes).  On that path the gradients are the same bits from run to run. */
 typedef struct b2cnn_adam {
     float lr, beta1, beta2, eps;   /* torch defaults: 1e-3, 0.9, 0.999, 1e-8 */
 } b2cnn_adam;
@@ -504,6 +509,13 @@ int b2cnn_train_forward(const b2cnn_config *cfg, const float *params, const floa
 int b2cnn_train_backward(const b2cnn_config *cfg, const float *params, const float *x, int64_t B, const float *age,
                          int mode, const float *mask1, const float *mask2, const float *dz, float *grads,
                          float *dx, float *dage, void *workspace, int64_t workspace_bytes, void *stream);
+/* b2cnn_train_backward with flags (0 = b2cnn_train_backward).  B2CNN_TRAIN_FROZEN_CONV: neither conv1 / conv2 nor the
+ * input needs a gradient (fine-tuning the LSTM head on a fixed front end): d f and the whole convolutional backward
+ * are skipped, the conv entries of grads are zero, and dx must be NULL. */
+#define B2CNN_TRAIN_FROZEN_CONV 1
+int b2cnn_train_backward_ex(const b2cnn_config *cfg, const float *params, const float *x, int64_t B, const float *age,
+                            int mode, const float *mask1, const float *mask2, const float *dz, float *grads,
+                            float *dx, float *dage, int flags, void *workspace, int64_t workspace_bytes, void *stream);
 
 #ifdef __cplusplus
 }

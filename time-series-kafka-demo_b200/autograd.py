@@ -11,9 +11,10 @@ with ``criterion = nn.BCEWithLogitsLoss(pos_weight=pos_weight)`` and ``optim.Ada
 (bin/explore_torch.ipynb:3170,3204-3205).  :class:`B200TrainableMyCNN` is a :class:`B200MyCNN` whose parameters
 take part in that loop unchanged: in ``train()`` mode its forward is ``b2cnn_train_forward`` (the training kernels of
 csrc/b2cnn_train.cu, keeping the activations the backward pass needs) and autograd's backward is
-``b2cnn_train_backward`` (BPTT over the batch axis, pooling / conv backward, and the input gradient) driven by whatever
-upstream gradient the loss produces.  In ``eval()`` mode it is the inference path of :class:`B200MyCNN`; optimizer
-steps edit the parameters in place, so the next inference call re-uploads them.
+``b2cnn_train_backward_ex`` (BPTT over the batch axis, pooling / conv backward, and the input gradient) driven by whatever
+upstream gradient the loss produces.  With ``conv1`` / ``conv2`` frozen (``requires_grad_(False)``) and an input that
+needs no gradient, the convolutional backward is skipped altogether.  In ``eval()`` mode it is the inference path of
+:class:`B200MyCNN`; optimizer steps edit the parameters in place, so the next inference call re-uploads them.
 
 :func:`mycnn_train_forward` is the same computation as a function of explicit parameters and dropout masks.
 """
@@ -66,10 +67,12 @@ class _TrainForward(torch.autograd.Function):
         grads = torch.empty_like(blob)
         dx = torch.empty_like(x) if ctx.needs_input_grad[1] else None
         dage = torch.empty_like(age) if ctx.needs_input_grad[2] else None
+        # conv1 / conv2 frozen and no input gradient wanted (fine-tuning the head): the library skips the conv backward
+        frozen = dx is None and not any(ctx.needs_input_grad[3:7])
         st = torch.cuda.current_stream(x.device).cuda_stream
-        rc = call.lib.b2cnn_train_backward(ctypes.byref(call.cfg), _ptr(blob), _ptr(x), B, _ptr(age), call.mode, _ptr(call.mask1),
-                                           _ptr(call.mask2), _ptr(dz), _ptr(grads), _ptr(dx), _ptr(dage), _ptr(ws), ws.numel(),
-                                           ctypes.c_void_p(st))
+        rc = call.lib.b2cnn_train_backward_ex(ctypes.byref(call.cfg), _ptr(blob), _ptr(x), B, _ptr(age), call.mode, _ptr(call.mask1),
+                                              _ptr(call.mask2), _ptr(dz), _ptr(grads), _ptr(dx), _ptr(dage),
+                                              capi.TRAIN_FROZEN_CONV if frozen else 0, _ptr(ws), ws.numel(), ctypes.c_void_p(st))
         capi.check(rc, "b2cnn_train_backward")
         out, at = [], 0
         for shape, need in zip(ctx.shapes, ctx.needs_input_grad[3:]):

@@ -16,6 +16,7 @@ _LIB_PATH = os.environ.get("B2CNN_LIB") or os.path.join(_HERE, "lib", "libb2cnn.
 OK, EINVAL, EARCH, EVIEW, ECUDA, ESTATE = range(6)
 DTYPE_F32, DTYPE_BF16 = 0, 1
 MODE_INDEPENDENT, MODE_SEQUENCE = 0, 1
+TRAIN_FROZEN_CONV = 1          # b2cnn_train_backward_ex flag (include/b2cnn.h)
 PATH_AUTO, PATH_GENERIC, PATH_TENSORCORE = 0, 1, 2
 FLAG_AFFINE = 1
 SAMPLES_ADC16, SAMPLES_F64, SAMPLES_GRID = 0, 1, 2
@@ -25,7 +26,7 @@ SYMBOLS = ("b2cnn_l_out", "b2cnn_weight_count", "b2cnn_create", "b2cnn_destroy",
            "b2cnn_set_weights", "b2cnn_workspace_bytes", "b2cnn_workspace_bytes_for", "b2cnn_forward", "b2cnn_forward_pitched", "b2cnn_forward_host",
            "b2cnn_features", "b2cnn_set_option", "b2cnn_get_option", "b2cnn_last_launch_count",
            "b2cnn_last_path", "b2cnn_last_stage_ms", "b2cnn_last_error", "b2cnn_version", "b2cnn_train_workspace_bytes", "b2cnn_train_step",
-           "b2cnn_train_step_weighted", "b2cnn_train_forward", "b2cnn_train_backward",
+           "b2cnn_train_step_weighted", "b2cnn_train_forward", "b2cnn_train_backward", "b2cnn_train_backward_ex",
            "b2cnn_prep_window_count", "b2cnn_prep_workspace_bytes", "b2cnn_prep_windows",
            "b2cnn_ring_create", "b2cnn_ring_destroy", "b2cnn_ring_reset", "b2cnn_ring_set_signals", "b2cnn_ring_push",
            "b2cnn_slide_create", "b2cnn_slide_destroy", "b2cnn_slide_reset", "b2cnn_slide_push", "b2cnn_slide_features",
@@ -184,6 +185,8 @@ def load_library() -> ctypes.CDLL:
     lib.b2cnn_train_forward.restype = c_int
     lib.b2cnn_train_backward.argtypes = [cfgp, c_vp, c_vp, c_i64, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp]
     lib.b2cnn_train_backward.restype = c_int
+    lib.b2cnn_train_backward_ex.argtypes = [cfgp, c_vp, c_vp, c_i64, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_i64, c_vp]
+    lib.b2cnn_train_backward_ex.restype = c_int
     lib.b2cnn_last_error.argtypes = []; lib.b2cnn_last_error.restype = ctypes.c_char_p
     lib.b2cnn_version.argtypes = []; lib.b2cnn_version.restype = ctypes.c_char_p
     _lib = lib

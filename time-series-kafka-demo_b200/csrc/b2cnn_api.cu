@@ -161,13 +161,18 @@ extern "C" int b2cnn_train_forward(const b2cnn_config *cfg, const float *params,
                                  reinterpret_cast<cudaStream_t>(stream), &err);
     return rc == B2CNN_OK ? rc : fail(rc, std::string("b2cnn_train_forward: ") + err);
 }
+extern "C" int b2cnn_train_backward_ex(const b2cnn_config *cfg, const float *params, const float *x, int64_t B, const float *age, int mode,
+                                       const float *mask1, const float *mask2, const float *dz, float *grads, float *dx, float *dage,
+                                       int flags, void *workspace, int64_t workspace_bytes, void *stream) {
+    const char *err = "";
+    const int rc = train_backward(cfg, params, x, B, age, mode, mask1, mask2, dz, grads, dx, dage, flags, workspace, workspace_bytes,
+                                  reinterpret_cast<cudaStream_t>(stream), &err);
+    return rc == B2CNN_OK ? rc : fail(rc, std::string("b2cnn_train_backward: ") + err);
+}
 extern "C" int b2cnn_train_backward(const b2cnn_config *cfg, const float *params, const float *x, int64_t B, const float *age, int mode,
                                     const float *mask1, const float *mask2, const float *dz, float *grads, float *dx, float *dage,
                                     void *workspace, int64_t workspace_bytes, void *stream) {
-    const char *err = "";
-    const int rc = train_backward(cfg, params, x, B, age, mode, mask1, mask2, dz, grads, dx, dage, workspace, workspace_bytes,
-                                  reinterpret_cast<cudaStream_t>(stream), &err);
-    return rc == B2CNN_OK ? rc : fail(rc, std::string("b2cnn_train_backward: ") + err);
+    return b2cnn_train_backward_ex(cfg, params, x, B, age, mode, mask1, mask2, dz, grads, dx, dage, 0, workspace, workspace_bytes, stream);
 }
 
 // ---- preprocessing + window assembly (b2cnn_prep.cu) ----

@@ -192,8 +192,8 @@ int train_step(const b2cnn_config *cfg, float *params, float *adam_m, float *ada
 int train_forward(const b2cnn_config *cfg, const float *params, const float *x, int64_t B, const float *age, int mode, const float *mask1,
                   const float *mask2, float *z_out, void *workspace, int64_t ws_bytes, cudaStream_t st, const char **err);
 int train_backward(const b2cnn_config *cfg, const float *params, const float *x, int64_t B, const float *age, int mode,
-                   const float *mask1, const float *mask2, const float *dz, float *grads, float *dx, float *dage, void *workspace,
-                   int64_t ws_bytes, cudaStream_t st, const char **err);
+                   const float *mask1, const float *mask2, const float *dz, float *grads, float *dx, float *dage, int flags,
+                   void *workspace, int64_t ws_bytes, cudaStream_t st, const char **err);
 
 void launch_transpose_wih(const float *wih0, float *wih0T, int L, cudaStream_t st);
 

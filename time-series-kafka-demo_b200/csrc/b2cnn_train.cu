@@ -21,8 +21,22 @@
 //   train_adam       torch.optim.Adam (no amsgrad, weight_decay 0) on the packed parameter blob
 // The head of the two LSTM kernels is a template parameter (Head): the fused step's BCE, BCE with pos_weight, or logits
 // only, with d loss / d z supplied by the caller (b2cnn_train_forward / b2cnn_train_backward, driven by torch autograd).
-// These are launch-latency kernels for the training shape [B,10,120] (44 k MAC per window); they take any geometry the
-// forward path takes (all intermediates live in the caller's workspace), but are not tuned for the stretched windows.
+// Those are launch-latency kernels for the training shape [B,10,120] (44 k MAC per window): one CTA per window, every
+// intermediate in the caller's workspace.  train_plan() sends windows with L >= kLongMinL features (the waveform windows,
+// [B,3,75000] -> L = 18745) to a second set, chosen from L alone so that a window's arithmetic never depends on its batch:
+//   train_conv_fwd_tiled   grid (position tiles x B): a CTA stages the x span of kLongT final features in shared memory,
+//                          runs conv_tile() there and writes only f (bit-identical to train_conv_fwd's)
+//   train_pre0_partial / train_pre0_reduce   layer-0 pre-activations f . W_ih_l0^T as a split-K GEMM, partials added
+//                          in slice order; train_lstm_fwd takes them through a pointer
+//   train_wih0_grad_tiled / train_sum_chunks  dW_ih_l0 = da0^T f with f read once: a thread owns a position and all 64
+//                          gate rows, the batch is split into chunks, chunk partials are added in chunk order
+//   train_dfeat_tiled      d f with a thread's 64 W_ih_l0 values in registers (train_dfeat's summation order)
+//   train_conv_bwd_tiled   grid (position tiles x groups of kLongWin windows): recomputes c1 / d1 / c2 with conv_tile(),
+//                          back-propagates the gradients of ITS OWN kLongT features through its receptive span in shared
+//                          memory, keeps the conv weight-gradient partials of its windows and adds d x into a zeroed array
+//   train_conv_grad_reduce sums the per-CTA partials in a fixed order (no atomics: gradients repeat bit for bit)
+// Everything below f is linear in d f, so the sum over tiles of what each tile back-propagates from its own features is
+// the full gradient; no halo is exchanged and dc1 / dd1 / dc2 never reach global memory.
 #include <cfloat>
 #include <cstring>
 
@@ -62,9 +76,60 @@ static BlobOff blob_offsets(const TrainDims &d) {
 
 // workspace layout (floats)
 struct TrainWs {
-    int64_t c1, p1, c2, f, acts, cs, hs, lin, z, da0, dfeat, dc2, dd1, dc1, total;
+    int64_t c1, p1, c2, f, acts, cs, hs, lin, z, da0, dfeat, dc2, dd1, dc1, pre0, part, total;
 };
-static TrainWs train_ws(const TrainDims &d, int64_t B) {
+
+// ---- the tiled kernels' constants ----
+constexpr int kLongMinL = 1024;     // L >= this: the tiled kernels
+constexpr int kLongT = 128;         // final features per tile
+constexpr int kLongThreads = 256;
+constexpr int kLongWin = 8;         // windows per CTA of the tiled conv backward (one weight-gradient partial per CTA)
+constexpr int kPre0Slice = 1024;    // positions per split-K slice of the pre-activation GEMM
+constexpr int kWihChunks = 16;      // at most this many batch chunks in dW_ih_l0
+constexpr int kRowBatch = 64;       // da0 rows staged per pass of train_dfeat_tiled / train_wih0_grad_tiled
+
+// float offsets of a conv tile's buffers in dynamic shared memory; xp / pp are the row pitches of x and d1 / dd1
+struct TileSmem {
+    int w1, b1, w2, b2, x, xp, c1, d1, pp, c2, df, dc2, dd1, dc1, g, total;
+};
+// The largest tile: kLongT features plus the few positions the last tile takes on beyond its last pooling window.
+__host__ __device__ inline TileSmem tile_smem(const TrainDims &d, bool backward) {
+    const int n2 = d.PS * (kLongT - 1) + d.PK + d.PS - 1, np1 = n2 + d.K2 - 1, n1 = d.PS * (np1 - 1) + d.PK + d.PS - 1, nx = n1 + d.K1 - 1;
+    TileSmem s;
+    int p = 0;
+    auto take = [&](int n) { int at = p; p += (n + 3) / 4 * 4; return at; };
+    s.w1 = take(kCMid * d.C * d.K1);      // [c][k][oc]
+    s.b1 = take(kCMid);
+    s.w2 = take(kCMid * d.K2);
+    s.b2 = take(1);
+    s.xp = (nx + 3) / 4 * 4;
+    s.x = take(d.C * s.xp);
+    s.c1 = take(kCMid * n1);              // [position][oc]
+    s.pp = (np1 + 3) / 4 * 4;
+    s.d1 = take(kCMid * s.pp);            // tanh(pool(c1)) * mask1
+    s.c2 = take(n2);
+    s.df = s.dc2 = s.dd1 = s.dc1 = s.g = 0;
+    if (backward) {
+        s.df = take(kLongT);
+        s.dc2 = take(n2);
+        s.dd1 = take(kCMid * s.pp);
+        s.dc1 = take(kCMid * n1);         // [position][oc]
+        s.g = take(kCMid * d.C * d.K1 + kCMid + kCMid * d.K2 + 1);
+    }
+    s.total = p;
+    return s;
+}
+
+// Which kernels a shape runs and what they need; read by every entry point and by the workspace query.
+struct TrainPlan {
+    bool tiled;
+    TrainWs w;
+    int tiles, slices, wih_chunk, wih_chunks, groups, n_conv;
+    int64_t part_rows;                  // per-CTA conv weight-gradient partials
+    size_t smem_fwd, smem_bwd;
+};
+
+static TrainWs train_ws_short(const TrainDims &d, int64_t B) {
     TrainWs w;
     int64_t p = 0;
     auto take = [&](int64_t n) { int64_t at = p; p += (n + 63) / 64 * 64; return at; };
@@ -82,8 +147,47 @@ static TrainWs train_ws(const TrainDims &d, int64_t B) {
     w.dc2 = take(B * d.L2);
     w.dd1 = take(B * kCMid * d.P1);
     w.dc1 = take(B * kCMid * d.L1);
+    w.pre0 = w.part = 0;
     w.total = p;
     return w;
+}
+
+static TrainPlan train_plan(const TrainDims &d, int64_t B) {
+    TrainPlan pl{};
+    pl.tiled = d.L >= kLongMinL;
+    if (!pl.tiled) {
+        pl.w = train_ws_short(d, B);
+        return pl;
+    }
+    pl.tiles = (d.L + kLongT - 1) / kLongT;
+    pl.slices = (d.L + kPre0Slice - 1) / kPre0Slice;
+    pl.wih_chunk = (int)((B + kWihChunks - 1) / kWihChunks);
+    pl.wih_chunks = (int)((B + pl.wih_chunk - 1) / pl.wih_chunk);
+    pl.groups = (int)((B + kLongWin - 1) / kLongWin);
+    pl.n_conv = kCMid * d.C * d.K1 + kCMid + kCMid * d.K2 + 1;
+    pl.part_rows = (int64_t)pl.tiles * pl.groups;
+    pl.smem_fwd = sizeof(float) * tile_smem(d, false).total;
+    pl.smem_bwd = sizeof(float) * tile_smem(d, true).total;
+    TrainWs &w = pl.w;
+    w = TrainWs{};
+    int64_t p = 0;
+    auto take = [&](int64_t n) { int64_t at = p; p += (n + 63) / 64 * 64; return at; };
+    w.f = take(B * d.L);
+    w.pre0 = take(B * kGates);          // f . W_ih_l0^T
+    w.acts = take(B * 2 * kGates);
+    w.cs = take(B * 2 * kHidden);
+    w.hs = take(B * 2 * kHidden);
+    w.lin = take(B);
+    w.z = take(B);
+    w.da0 = take(B * kGates);
+    w.dfeat = take(B * d.L);
+    // one region for the partial sums of three reductions that never overlap in time
+    int64_t part = (int64_t)pl.slices * B * kGates;
+    if ((int64_t)pl.wih_chunks * kGates * d.L > part) part = (int64_t)pl.wih_chunks * kGates * d.L;
+    if (pl.part_rows * pl.n_conv > part) part = pl.part_rows * pl.n_conv;
+    w.part = take(part);
+    w.total = p;
+    return pl;
 }
 
 __device__ __forceinline__ float sigmoidf_(float v) { return 1.0f / (1.0f + expf(-v)); }
@@ -146,12 +250,13 @@ train_conv_fwd(const float *__restrict__ x, const float *__restrict__ prm, BlobO
 
 // ------------------------------------------------------------------------------------------------------------------
 // LSTM forward over the batch axis with everything the backward pass needs kept; logits and loss.
-// One CTA of 64 threads: thread r owns gate row r of every matrix.  sequence == 0: every step starts from the zero state
+// One CTA of 64 threads: thread r owns gate row r of every matrix.  pre0 != NULL: W_ih_l0 f_t was computed before the
+// scan (pre0[t][r]); NULL: the thread computes its dot product at every step.  sequence == 0: every step starts from the zero state
 // (independent windows).  HEAD == kHeadLogits: target and loss_out are not used.
 // ------------------------------------------------------------------------------------------------------------------
 template <int HEAD>
 __global__ void __launch_bounds__(64)
-train_lstm_fwd(const float *__restrict__ f, const float *__restrict__ prm, BlobOff o, TrainDims d, int64_t B, int sequence,
+train_lstm_fwd(const float *__restrict__ f, const float *__restrict__ pre0, const float *__restrict__ prm, BlobOff o, TrainDims d, int64_t B, int sequence,
                const float *__restrict__ age, const float *__restrict__ target, float pos_weight, float *__restrict__ acts,
                float *__restrict__ cs, float *__restrict__ hs, float *__restrict__ lin, float *__restrict__ z,
                float *__restrict__ loss_out) {
@@ -167,10 +272,14 @@ train_lstm_fwd(const float *__restrict__ f, const float *__restrict__ prm, BlobO
         }
         // ---- layer 0: g = (W_ih f_t + b_ih) + (W_hh h_{t-1} + b_hh)
         {
-            const float *ft = f + t * d.L;
-            const float *wr = prm + o.wih0 + (int64_t)r * d.L;
             float a = 0.f;
-            for (int p = 0; p < d.L; ++p) a = fmaf(wr[p], ft[p], a);
+            if (pre0) {
+                a = pre0[t * kGates + r];
+            } else {
+                const float *ft = f + t * d.L;
+                const float *wr = prm + o.wih0 + (int64_t)r * d.L;
+                for (int p = 0; p < d.L; ++p) a = fmaf(wr[p], ft[p], a);
+            }
             float rr = 0.f;
             for (int k = 0; k < kHidden; ++k) rr = fmaf(prm[o.whh0 + r * kHidden + k], h0[k], rr);
             g[r] = (a + prm[o.bih0 + r]) + (rr + prm[o.bhh0 + r]);
@@ -490,6 +599,342 @@ __global__ void train_dx(const float *__restrict__ dc1, const float *__restrict_
     dx[e] = a;
 }
 
+// ------------------------------------------------------------------------------------------------------------------
+// The tiled kernels (L >= kLongMinL).
+// Tile `tile` of a window owns final features [i0, i0 + nf).  Their receptive span starts at c2 / p1 position
+// s2 = PS i0 and at c1 / x position s1 = PS s2 and holds n2 / np1 / n1 / nx positions of c2 / p1 / c1 / x.  The last tile
+// also takes the positions after the last pooling window (a geometry may leave a few): they get no gradient, but a NaN
+// there reaches d tanh as it does in train_conv_bwd.
+// ------------------------------------------------------------------------------------------------------------------
+struct Tile {
+    int i0, nf, s2, s1, n2, np1, n1, nx;
+};
+__device__ __forceinline__ Tile tile_of(const TrainDims &d, int tile) {
+    Tile t;
+    t.i0 = tile * kLongT;
+    t.nf = min(kLongT, d.L - t.i0);
+    t.s2 = d.PS * t.i0;
+    t.s1 = d.PS * t.s2;
+    const bool last = t.i0 + t.nf == d.L;
+    t.n2 = last ? d.L2 - t.s2 : d.PS * (t.nf - 1) + d.PK;
+    t.np1 = last ? d.P1 - t.s2 : t.n2 + d.K2 - 1;
+    t.n1 = last ? d.L1 - t.s1 : d.PS * (t.np1 - 1) + d.PK;
+    t.nx = last ? d.W - t.s1 : t.n1 + d.K1 - 1;
+    return t;
+}
+
+// conv weights into shared memory; conv1's as [c][k][oc], so one 16-byte load feeds the four output channels of a tap
+__device__ __forceinline__ void tile_stage_weights(const float *__restrict__ prm, const BlobOff &o, const TrainDims &d, const TileSmem &s,
+                                                   float *sm, int tid) {
+    const int ck = d.C * d.K1;
+    for (int e = tid; e < kCMid * ck; e += kLongThreads) sm[s.w1 + (e % ck) * kCMid + e / ck] = prm[o.w1 + e];
+    if (tid < kCMid) sm[s.b1 + tid] = prm[o.b1 + tid];
+    for (int e = tid; e < kCMid * d.K2; e += kLongThreads) sm[s.w2 + e] = prm[o.w2 + e];
+    if (tid == 0) sm[s.b2] = prm[o.b2];
+}
+
+// One tile of one window, everything in shared memory: x span -> c1 -> pool -> tanh -> mask1 (d1) -> c2.  Every sum in
+// train_conv_fwd's order (bias first, channels outer, taps inner, fmaf), so c1, d1 and c2 are the values it computes.
+// xb / m1b: the window's x [C][W] and its mask1 [4][P1] (or NULL).  Ends with a barrier.
+__device__ __forceinline__ void conv_tile(const float *__restrict__ xb, const float *__restrict__ m1b, const TrainDims &d, const Tile &t,
+                                          const TileSmem &s, float *sm, int tid) {
+    for (int c = 0; c < d.C; ++c)
+        for (int j = tid; j < t.nx; j += kLongThreads) sm[s.x + c * s.xp + j] = xb[(int64_t)c * d.W + t.s1 + j];
+    __syncthreads();
+    for (int j = tid; j < t.n1; j += kLongThreads) {
+        float4 acc = *reinterpret_cast<const float4 *>(sm + s.b1);
+        for (int c = 0; c < d.C; ++c) {
+            const float *xr = sm + s.x + c * s.xp + j;
+            const float4 *wr = reinterpret_cast<const float4 *>(sm + s.w1) + c * d.K1;
+            for (int k = 0; k < d.K1; ++k) {
+                const float4 w = wr[k];
+                const float xv = xr[k];
+                acc.x = fmaf(w.x, xv, acc.x); acc.y = fmaf(w.y, xv, acc.y); acc.z = fmaf(w.z, xv, acc.z); acc.w = fmaf(w.w, xv, acc.w);
+            }
+        }
+        *reinterpret_cast<float4 *>(sm + s.c1 + 4 * j) = acc;
+    }
+    __syncthreads();
+    for (int e = tid; e < kCMid * t.np1; e += kLongThreads) {
+        const int oc = e / t.np1, i = e % t.np1;
+        const float *col = sm + s.c1 + oc;
+        float m = col[4 * d.PS * i];
+        for (int j = 1; j < d.PK; ++j) m = max_nan(m, col[4 * (d.PS * i + j)]);
+        sm[s.d1 + oc * s.pp + i] = tanhf(m) * (m1b ? m1b[(int64_t)oc * d.P1 + t.s2 + i] : 1.0f);
+    }
+    __syncthreads();
+    for (int j = tid; j < t.n2; j += kLongThreads) {
+        float acc = sm[s.b2];
+        for (int oc = 0; oc < kCMid; ++oc)
+            for (int k = 0; k < d.K2; ++k) acc = fmaf(sm[s.w2 + oc * d.K2 + k], sm[s.d1 + oc * s.pp + j + k], acc);
+        sm[s.c2 + j] = acc;
+    }
+    __syncthreads();
+}
+
+// grid: B x tiles CTAs, window-major
+__global__ void __launch_bounds__(kLongThreads)
+train_conv_fwd_tiled(const float *__restrict__ x, const float *__restrict__ prm, BlobOff o, TrainDims d, int tiles,
+                     const float *__restrict__ mask1, const float *__restrict__ mask2, float *__restrict__ f) {
+    extern __shared__ __align__(16) float sm[];
+    const TileSmem s = tile_smem(d, false);
+    const int tid = threadIdx.x;
+    const int64_t b = blockIdx.x / tiles;
+    const Tile t = tile_of(d, blockIdx.x % tiles);
+    tile_stage_weights(prm, o, d, s, sm, tid);
+    conv_tile(x + b * d.C * d.W, mask1 ? mask1 + b * kCMid * d.P1 : nullptr, d, t, s, sm, tid);
+    for (int i = tid; i < t.nf; i += kLongThreads) {
+        float m = sm[s.c2 + d.PS * i];
+        for (int j = 1; j < d.PK; ++j) m = max_nan(m, sm[s.c2 + d.PS * i + j]);
+        f[b * d.L + t.i0 + i] = tanhf(m) * (mask2 ? mask2[b * d.L + t.i0 + i] : 1.0f);
+    }
+}
+
+// pre0 partial[slice][b][g] = sum over the slice's positions of f[b][p] W_ih_l0[g][p]: 64 windows x 64 gates per CTA,
+// K chunks of 32, a 4 x 4 register tile per thread (the tiling of the inference projection, reading W_ih_l0 as stored)
+constexpr int kGemmK = 32, kGemmStride = 68;
+__global__ void __launch_bounds__(256)
+train_pre0_partial(const float *__restrict__ f, const float *__restrict__ wih0, int64_t B, int L, float *__restrict__ part) {
+    __shared__ __align__(16) float Fs[kGemmK][kGemmStride];
+    __shared__ __align__(16) float Ws[kGemmK][kGemmStride];
+    const int tid = threadIdx.x, tm = tid >> 4, tn = tid & 15;
+    const int64_t b0 = (int64_t)blockIdx.x * 64;
+    const int kbeg = blockIdx.y * kPre0Slice, kend = min(L, kbeg + kPre0Slice);
+    float acc[4][4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
+    for (int k0 = kbeg; k0 < kend; k0 += kGemmK) {
+#pragma unroll
+        for (int it = 0; it < 8; ++it) {
+            const int e = tid + it * 256, m = e >> 5, kk = e & 31, k = k0 + kk;
+            Fs[kk][m] = (b0 + m < B && k < kend) ? f[(b0 + m) * L + k] : 0.f;
+            Ws[kk][m] = k < kend ? wih0[(int64_t)m * L + k] : 0.f;
+        }
+        __syncthreads();
+#pragma unroll
+        for (int kk = 0; kk < kGemmK; ++kk) {
+            const float4 a = *reinterpret_cast<const float4 *>(&Fs[kk][4 * tm]);
+            const float4 w = *reinterpret_cast<const float4 *>(&Ws[kk][4 * tn]);
+            const float av[4] = {a.x, a.y, a.z, a.w}, wv[4] = {w.x, w.y, w.z, w.w};
+#pragma unroll
+            for (int i = 0; i < 4; ++i)
+#pragma unroll
+                for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(av[i], wv[j], acc[i][j]);
+        }
+        __syncthreads();
+    }
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        const int64_t b = b0 + 4 * tm + i;
+        if (b < B) *reinterpret_cast<float4 *>(part + ((int64_t)blockIdx.y * B + b) * kGates + 4 * tn) = make_float4(acc[i][0], acc[i][1], acc[i][2], acc[i][3]);
+    }
+}
+
+// out[e] = part[0][e] + part[1][e] + ... in that order (split-K slices of pre0, batch chunks of dW_ih_l0)
+__global__ void train_sum_chunks(const float *__restrict__ part, int n_chunks, int64_t n, float *__restrict__ out) {
+    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= n) return;
+    float a = part[e];
+    for (int c = 1; c < n_chunks; ++c) a += part[(int64_t)c * n + e];
+    out[e] = a;
+}
+
+// dW_ih_l0 partial[chunk][g][p] = sum over the chunk's windows t (ascending) of da0[t][g] f[t][p].  Thread = position p
+// with the 64 gate rows' sums in registers, so f is read once; grid (position tiles of 128, batch chunks).
+__global__ void __launch_bounds__(128)
+train_wih0_grad_tiled(const float *__restrict__ da0, const float *__restrict__ f, int64_t B, int L, int chunk, float *__restrict__ part) {
+    __shared__ __align__(16) float sda[kRowBatch * kGates];
+    const int p = blockIdx.x * 128 + threadIdx.x;
+    const int64_t t0 = (int64_t)blockIdx.y * chunk, t1 = min(B, t0 + chunk);
+    float acc[kGates];
+#pragma unroll
+    for (int g = 0; g < kGates; ++g) acc[g] = 0.f;
+    for (int64_t tb = t0; tb < t1; tb += kRowBatch) {
+        const int rows = (int)min((int64_t)kRowBatch, t1 - tb);
+        __syncthreads();
+        for (int e = threadIdx.x; e < rows * kGates; e += 128) sda[e] = da0[tb * kGates + e];
+        __syncthreads();
+        if (p < L)
+            for (int r = 0; r < rows; ++r) {
+                const float fv = f[(tb + r) * L + p];
+#pragma unroll
+                for (int g4 = 0; g4 < kGates / 4; ++g4) {
+                    const float4 a = *reinterpret_cast<const float4 *>(sda + r * kGates + 4 * g4);
+                    acc[4 * g4 + 0] = fmaf(a.x, fv, acc[4 * g4 + 0]); acc[4 * g4 + 1] = fmaf(a.y, fv, acc[4 * g4 + 1]);
+                    acc[4 * g4 + 2] = fmaf(a.z, fv, acc[4 * g4 + 2]); acc[4 * g4 + 3] = fmaf(a.w, fv, acc[4 * g4 + 3]);
+                }
+            }
+    }
+    if (p < L)
+#pragma unroll
+        for (int g = 0; g < kGates; ++g) part[((int64_t)blockIdx.y * kGates + g) * L + p] = acc[g];
+}
+
+// d f[t][p] = sum_g da0[t][g] W_ih_l0[g][p] in train_dfeat's order; thread = position p with its 64 weights in
+// registers, grid (position tiles of 128, groups of kRowBatch windows)
+__global__ void __launch_bounds__(128)
+train_dfeat_tiled(const float *__restrict__ da0, const float *__restrict__ wih0, int64_t B, int L, float *__restrict__ dfeat) {
+    __shared__ __align__(16) float sda[kRowBatch * kGates];
+    const int p = blockIdx.x * 128 + threadIdx.x;
+    const int64_t t0 = (int64_t)blockIdx.y * kRowBatch;
+    const int rows = (int)min((int64_t)kRowBatch, B - t0);
+    for (int e = threadIdx.x; e < rows * kGates; e += 128) sda[e] = da0[t0 * kGates + e];
+    __syncthreads();
+    if (p >= L) return;
+    float w[kGates];
+#pragma unroll
+    for (int g = 0; g < kGates; ++g) w[g] = wih0[(int64_t)g * L + p];
+    for (int r = 0; r < rows; ++r) {
+        float a = 0.f;
+#pragma unroll
+        for (int g4 = 0; g4 < kGates / 4; ++g4) {
+            const float4 v = *reinterpret_cast<const float4 *>(sda + r * kGates + 4 * g4);
+            a = fmaf(v.x, w[4 * g4 + 0], a); a = fmaf(v.y, w[4 * g4 + 1], a); a = fmaf(v.z, w[4 * g4 + 2], a); a = fmaf(v.w, w[4 * g4 + 3], a);
+        }
+        dfeat[(t0 + r) * L + p] = a;
+    }
+}
+
+// pool_argmax over every `stride`-th float (c1 is kept position-major in a tile)
+__device__ __forceinline__ int pool_argmax_strided(const float *v, int stride, int start, int pk) {
+    int best = start;
+    float m = v[start * stride];
+    for (int j = 1; j < pk; ++j) {
+        const float c = v[(start + j) * stride];
+        if (c > m || c != c) { m = c; best = start + j; }
+    }
+    return best;
+}
+__device__ __forceinline__ float warp_sum(float v) {
+#pragma unroll
+    for (int sft = 16; sft > 0; sft >>= 1) v += __shfl_xor_sync(0xffffffffu, v, sft);
+    return v;
+}
+
+// The conv backward of one tile for kLongWin consecutive windows; grid: groups x tiles CTAs, group-major.  Per window:
+// conv_tile() again (same masks, so the pool arg-max is the forward's), then train_conv_bwd's steps on the tile's own
+// features in shared memory.  A warp owns each weight's partial sum (lanes stride the positions, one shuffle tree) and
+// adds it to the CTA's running sum in window order; the CTA writes one row of part[groups x tiles][n_conv].
+// dx != NULL: d x of the tile's span is added into the zeroed dx; adjacent spans overlap by less than a tile's stride
+// (checked by the host), so a sample has at most two contributions and their sum does not depend on the order.
+__global__ void __launch_bounds__(kLongThreads)
+train_conv_bwd_tiled(const float *__restrict__ x, const float *__restrict__ prm, BlobOff o, TrainDims d, int tiles, int64_t B,
+                     const float *__restrict__ mask1, const float *__restrict__ mask2, const float *__restrict__ dfeat,
+                     float *__restrict__ part, float *__restrict__ dx) {
+    extern __shared__ __align__(16) float sm[];
+    const TileSmem s = tile_smem(d, true);
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    constexpr int kWarps = kLongThreads / 32;
+    const Tile t = tile_of(d, blockIdx.x % tiles);
+    const int64_t b0 = (int64_t)(blockIdx.x / tiles) * kLongWin, b1 = min(B, b0 + kLongWin);
+    const int ck = d.C * d.K1, n_conv = kCMid * ck + kCMid + kCMid * d.K2 + 1;
+    tile_stage_weights(prm, o, d, s, sm, tid);
+    for (int e = tid; e < n_conv; e += kLongThreads) sm[s.g + e] = 0.f;
+    for (int64_t b = b0; b < b1; ++b) {
+        const float *m1b = mask1 ? mask1 + b * kCMid * d.P1 : nullptr;
+        __syncthreads();                                       // the previous window's readers are done
+        for (int i = tid; i < t.nf; i += kLongThreads) sm[s.df + i] = dfeat[b * d.L + t.i0 + i] * (mask2 ? mask2[b * d.L + t.i0 + i] : 1.0f);
+        conv_tile(x + b * d.C * d.W, m1b, d, t, s, sm, tid);
+        // ---- dropout 2 + pool 2 + tanh, gather form over the tile's own features
+        for (int j = tid; j < t.n2; j += kLongThreads) {
+            float a = 0.f;
+            int i_lo = (j - d.PK + d.PS) / d.PS;
+            if (j - d.PK + 1 <= 0) i_lo = 0;
+            for (int i = i_lo; i <= j / d.PS && i < t.nf; ++i)
+                if (pool_argmax(sm + s.c2, d.PS * i, d.PK) == j) a += sm[s.df + i];
+            sm[s.dc2 + j] = a * dtanhf_(sm[s.c2 + j]);
+        }
+        __syncthreads();
+        // ---- conv2: weight / bias partials, d d1
+        for (int e = warp; e < kCMid * d.K2 + 1; e += kWarps) {
+            float a = 0.f;
+            if (e < kCMid * d.K2) {
+                const float *dr = sm + s.d1 + (e / d.K2) * s.pp + e % d.K2;
+                for (int j = lane; j < t.n2; j += 32) a = fmaf(sm[s.dc2 + j], dr[j], a);
+            } else {
+                for (int j = lane; j < t.n2; j += 32) a += sm[s.dc2 + j];
+            }
+            a = warp_sum(a);
+            if (lane == 0) sm[s.g + (e < kCMid * d.K2 ? o.w2 + e : o.b2)] += a;
+        }
+        for (int e = tid; e < kCMid * t.np1; e += kLongThreads) {
+            const int oc = e / t.np1, u = e % t.np1;
+            float a = 0.f;
+            for (int k = 0; k < d.K2; ++k) {
+                const int j = u - k;
+                if (j >= 0 && j < t.n2) a = fmaf(sm[s.w2 + oc * d.K2 + k], sm[s.dc2 + j], a);
+            }
+            sm[s.dd1 + oc * s.pp + u] = a * (m1b ? m1b[(int64_t)oc * d.P1 + t.s2 + u] : 1.0f);
+        }
+        __syncthreads();
+        // ---- pool 1 + tanh
+        for (int e = tid; e < kCMid * t.n1; e += kLongThreads) {
+            const int j = e >> 2, oc = e & 3;
+            const float *col = sm + s.c1 + oc;
+            float a = 0.f;
+            int i_lo = (j - d.PK + d.PS) / d.PS;
+            if (j - d.PK + 1 <= 0) i_lo = 0;
+            for (int i = i_lo; i <= j / d.PS && i < t.np1; ++i)
+                if (pool_argmax_strided(col, kCMid, d.PS * i, d.PK) == j) a += sm[s.dd1 + oc * s.pp + i];
+            sm[s.dc1 + e] = a * dtanhf_(sm[s.c1 + e]);
+        }
+        __syncthreads();
+        // ---- conv1: a warp per (channel, tap) with the four output channels' sums, then the biases
+        for (int e = warp; e < ck + 1; e += kWarps) {
+            float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (e < ck) {
+                const float *xr = sm + s.x + (e / d.K1) * s.xp + e % d.K1;
+                for (int j = lane; j < t.n1; j += 32) {
+                    const float4 g = *reinterpret_cast<const float4 *>(sm + s.dc1 + 4 * j);
+                    const float xv = xr[j];
+                    a.x = fmaf(g.x, xv, a.x); a.y = fmaf(g.y, xv, a.y); a.z = fmaf(g.z, xv, a.z); a.w = fmaf(g.w, xv, a.w);
+                }
+            } else {
+                for (int j = lane; j < t.n1; j += 32) {
+                    const float4 g = *reinterpret_cast<const float4 *>(sm + s.dc1 + 4 * j);
+                    a.x += g.x; a.y += g.y; a.z += g.z; a.w += g.w;
+                }
+            }
+            a.x = warp_sum(a.x); a.y = warp_sum(a.y); a.z = warp_sum(a.z); a.w = warp_sum(a.w);
+            if (lane == 0) {
+                const float av[4] = {a.x, a.y, a.z, a.w};
+                for (int oc = 0; oc < kCMid; ++oc) sm[s.g + (e < ck ? o.w1 + oc * ck + e : o.b1 + oc)] += av[oc];
+            }
+        }
+        if (dx) {
+            for (int e = tid; e < d.C * t.nx; e += kLongThreads) {
+                const int c = e / t.nx, u = e % t.nx;
+                const int k_lo = max(0, u - (t.n1 - 1)), k_hi = min(d.K1 - 1, u);
+                float a = 0.f;
+                for (int oc = 0; oc < kCMid; ++oc)
+                    for (int k = k_lo; k <= k_hi; ++k) a = fmaf(sm[s.w1 + (c * d.K1 + k) * kCMid + oc], sm[s.dc1 + 4 * (u - k) + oc], a);
+                atomicAdd(dx + (b * d.C + c) * d.W + t.s1 + u, a);
+            }
+        }
+    }
+    __syncthreads();
+    for (int e = tid; e < n_conv; e += kLongThreads) part[(int64_t)blockIdx.x * n_conv + e] = sm[s.g + e];
+}
+
+// grad[e] = the sum of part[.][e] over all rows in a fixed order: one CTA per conv parameter, thread i adds rows
+// i, i + 256, ... in order, then the block's tree
+__global__ void __launch_bounds__(256)
+train_conv_grad_reduce(const float *__restrict__ part, int64_t rows, int n_conv, float *__restrict__ grad) {
+    __shared__ float red[256];
+    const int e = blockIdx.x, tid = threadIdx.x;
+    float a = 0.f;
+    for (int64_t r = tid; r < rows; r += 256) a += part[r * n_conv + e];
+    red[tid] = a;
+    __syncthreads();
+    for (int sft = 128; sft > 0; sft >>= 1) {
+        if (tid < sft) red[tid] += red[tid + sft];
+        __syncthreads();
+    }
+    if (tid == 0) grad[e] = red[0];
+}
+
 // torch.optim.Adam, single-tensor form: exp_avg.lerp_(grad, 1-b1); exp_avg_sq = b2*v + (1-b2) g^2;
 // denom = sqrt(v) / sqrt(1 - b2^t) + eps; param -= (lr / (1 - b1^t)) * m / denom
 __global__ void train_adam(float *__restrict__ prm, float *__restrict__ m, float *__restrict__ v, const float *__restrict__ grad, int64_t n,
@@ -523,7 +968,7 @@ int64_t train_workspace_bytes(const b2cnn_config *cfg, int64_t B) {
     TrainDims d;
     const char *err = "";
     if (!cfg || B < 1 || !train_dims(*cfg, d, &err)) return -1;
-    return train_ws(d, B).total * (int64_t)sizeof(float);
+    return train_plan(d, B).w.total * (int64_t)sizeof(float);
 }
 
 // Sets cfg->device current for the launches of one call (when it is >= 0) and restores the caller's device afterwards.
@@ -538,20 +983,63 @@ struct DeviceScope {
     }
 };
 
-// everything after d(head): d W_ih_l0, d f, the convolutional backward into `grads` (zeroed by the caller: conv weight
-// gradients are added atomically) and, when dx != NULL, the input gradient
-static void launch_backward_tail(const TrainDims &d, const BlobOff &o, const TrainWs &w, float *ws, const float *params,
-                                 const float *x, int64_t B, const float *mask1, const float *mask2, float *grads, float *dx,
-                                 cudaStream_t st) {
-    const int64_t n1 = (int64_t)kGates * d.L, n2 = B * d.L;
-    train_wih0_grad<<<(unsigned)((n1 + 255) / 256), 256, 0, st>>>(ws + w.da0, ws + w.f, B, d.L, grads + o.wih0);
-    train_dfeat<<<(unsigned)((n2 + 255) / 256), 256, 0, st>>>(ws + w.da0, params + o.wih0, B, d.L, ws + w.dfeat);
-    train_conv_bwd<<<(unsigned)B, 256, 0, st>>>(x, params, o, d, mask1, mask2, ws + w.c1, ws + w.p1, ws + w.c2, ws + w.dfeat, ws + w.dc2,
-                                               ws + w.dd1, ws + w.dc1, grads);
-    if (dx) {
-        const int64_t n = B * d.C * d.W;
-        train_dx<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(ws + w.dc1, params, o, d, B, dx);
+// what the tiled kernels need beyond a valid geometry; no CUDA call
+static bool tiled_args_ok(const TrainDims &d, const TrainPlan &pl, int64_t B, const char **err) {
+    if (pl.smem_bwd > 227 * 1024) { *err = "training: too many input channels for a conv tile's shared memory"; return false; }
+    // a tile's x span against the tiles' stride: d x relies on at most two tiles touching a sample
+    const int np1 = d.PS * (kLongT - 1) + d.PK + d.K2 - 1, span = d.PS * (np1 - 1) + d.PK + d.K1 - 1, stride = d.PS * d.PS * kLongT;
+    if (span > 2 * stride) { *err = "training: receptive field longer than a conv tile"; return false; }
+    if ((int64_t)pl.tiles * B > INT32_MAX) { *err = "training: batch too large"; return false; }
+    return true;
+}
+
+// conv forward into ws.f and, on the tiled plan, the layer-0 pre-activations; returns what train_lstm_fwd takes as pre0
+static const float *launch_conv_forward(const TrainDims &d, const BlobOff &o, const TrainPlan &pl, float *ws, const float *params,
+                                        const float *x, int64_t B, const float *mask1, const float *mask2, cudaStream_t st) {
+    const TrainWs &w = pl.w;
+    if (!pl.tiled) {
+        train_conv_fwd<<<(unsigned)B, 256, 0, st>>>(x, params, o, d, mask1, mask2, ws + w.c1, ws + w.p1, ws + w.c2, ws + w.f);
+        return nullptr;
     }
+    if (pl.smem_fwd > 48 * 1024) cudaFuncSetAttribute(train_conv_fwd_tiled, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.smem_fwd);
+    train_conv_fwd_tiled<<<(unsigned)(B * pl.tiles), kLongThreads, pl.smem_fwd, st>>>(x, params, o, d, pl.tiles, mask1, mask2, ws + w.f);
+    train_pre0_partial<<<dim3((unsigned)((B + 63) / 64), (unsigned)pl.slices), 256, 0, st>>>(ws + w.f, params + o.wih0, B, d.L, ws + w.part);
+    const int64_t n = B * kGates;
+    train_sum_chunks<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(ws + w.part, pl.slices, n, ws + w.pre0);
+    return ws + w.pre0;
+}
+
+// everything after d(head): d W_ih_l0 and, unless the front end is frozen, d f, the convolutional backward into `grads`
+// (zeroed by the caller: the one-CTA-per-window kernel adds its conv weight gradients atomically) and, when dx != NULL,
+// the input gradient
+static bool launch_backward_tail(const TrainDims &d, const BlobOff &o, const TrainPlan &pl, float *ws, const float *params,
+                                 const float *x, int64_t B, const float *mask1, const float *mask2, float *grads, float *dx,
+                                 bool frozen_conv, cudaStream_t st) {
+    const TrainWs &w = pl.w;
+    const int64_t n1 = (int64_t)kGates * d.L, n2 = B * d.L;
+    if (!pl.tiled) {
+        train_wih0_grad<<<(unsigned)((n1 + 255) / 256), 256, 0, st>>>(ws + w.da0, ws + w.f, B, d.L, grads + o.wih0);
+        if (frozen_conv) return true;
+        train_dfeat<<<(unsigned)((n2 + 255) / 256), 256, 0, st>>>(ws + w.da0, params + o.wih0, B, d.L, ws + w.dfeat);
+        train_conv_bwd<<<(unsigned)B, 256, 0, st>>>(x, params, o, d, mask1, mask2, ws + w.c1, ws + w.p1, ws + w.c2, ws + w.dfeat, ws + w.dc2,
+                                                   ws + w.dd1, ws + w.dc1, grads);
+        if (dx) {
+            const int64_t n = B * d.C * d.W;
+            train_dx<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(ws + w.dc1, params, o, d, B, dx);
+        }
+        return true;
+    }
+    const unsigned ptiles = (unsigned)((d.L + 127) / 128);
+    train_wih0_grad_tiled<<<dim3(ptiles, (unsigned)pl.wih_chunks), 128, 0, st>>>(ws + w.da0, ws + w.f, B, d.L, pl.wih_chunk, ws + w.part);
+    train_sum_chunks<<<(unsigned)((n1 + 255) / 256), 256, 0, st>>>(ws + w.part, pl.wih_chunks, n1, grads + o.wih0);
+    if (frozen_conv) return true;
+    train_dfeat_tiled<<<dim3(ptiles, (unsigned)((B + kRowBatch - 1) / kRowBatch)), 128, 0, st>>>(ws + w.da0, params + o.wih0, B, d.L, ws + w.dfeat);
+    if (dx && cudaMemsetAsync(dx, 0, sizeof(float) * B * d.C * d.W, st) != cudaSuccess) return false;
+    if (pl.smem_bwd > 48 * 1024) cudaFuncSetAttribute(train_conv_bwd_tiled, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.smem_bwd);
+    train_conv_bwd_tiled<<<(unsigned)pl.part_rows, kLongThreads, pl.smem_bwd, st>>>(x, params, o, d, pl.tiles, B, mask1, mask2, ws + w.dfeat,
+                                                                                   ws + w.part, dx);
+    train_conv_grad_reduce<<<(unsigned)pl.n_conv, 256, 0, st>>>(ws + w.part, pl.part_rows, pl.n_conv, grads);
+    return true;
 }
 
 int train_step(const b2cnn_config *cfg, float *params, float *adam_m, float *adam_v, float *grads, int64_t step, float lr, float beta1,
@@ -563,24 +1051,26 @@ int train_step(const b2cnn_config *cfg, float *params, float *adam_m, float *ada
     if (!params || !grads || !x || !age || !target || !loss_out || !workspace || B < 1 || step < 1) { *err = "training: null argument / bad step"; return B2CNN_EINVAL; }
     if (apply_update && (!adam_m || !adam_v)) { *err = "training: Adam state missing"; return B2CNN_EINVAL; }
     if (weighted && !(pos_weight > 0.f && pos_weight <= FLT_MAX)) { *err = "training: pos_weight must be positive and finite"; return B2CNN_EINVAL; }
-    const TrainWs w = train_ws(d, B);
+    const TrainPlan pl = train_plan(d, B);
+    const TrainWs &w = pl.w;
+    if (pl.tiled && !tiled_args_ok(d, pl, B, err)) return B2CNN_EINVAL;
     if (ws_bytes < w.total * (int64_t)sizeof(float)) { *err = "training: workspace smaller than b2cnn_train_workspace_bytes()"; return B2CNN_ESTATE; }
     const BlobOff o = blob_offsets(d);
     float *ws = reinterpret_cast<float *>(workspace);
     if (cudaMemsetAsync(grads, 0, sizeof(float) * o.total, st) != cudaSuccess) { *err = "memset grads"; return B2CNN_ECUDA; }
-    train_conv_fwd<<<(unsigned)B, 256, 0, st>>>(x, params, o, d, mask1, mask2, ws + w.c1, ws + w.p1, ws + w.c2, ws + w.f);
+    const float *pre0 = launch_conv_forward(d, o, pl, ws, params, x, B, mask1, mask2, st);
     if (weighted) {
-        train_lstm_fwd<kHeadBcePw><<<1, 64, 0, st>>>(ws + w.f, params, o, d, B, sequence, age, target, pos_weight, ws + w.acts, ws + w.cs,
+        train_lstm_fwd<kHeadBcePw><<<1, 64, 0, st>>>(ws + w.f, pre0, params, o, d, B, sequence, age, target, pos_weight, ws + w.acts, ws + w.cs,
                                                      ws + w.hs, ws + w.lin, ws + w.z, loss_out);
         train_lstm_bwd<kHeadBcePw><<<1, 64, 0, st>>>(params, o, d, B, sequence, age, target, pos_weight, nullptr, ws + w.acts, ws + w.cs,
                                                      ws + w.hs, ws + w.lin, ws + w.z, ws + w.da0, grads, nullptr);
     } else {
-        train_lstm_fwd<kHeadBce><<<1, 64, 0, st>>>(ws + w.f, params, o, d, B, sequence, age, target, 1.f, ws + w.acts, ws + w.cs,
+        train_lstm_fwd<kHeadBce><<<1, 64, 0, st>>>(ws + w.f, pre0, params, o, d, B, sequence, age, target, 1.f, ws + w.acts, ws + w.cs,
                                                    ws + w.hs, ws + w.lin, ws + w.z, loss_out);
         train_lstm_bwd<kHeadBce><<<1, 64, 0, st>>>(params, o, d, B, sequence, age, target, 1.f, nullptr, ws + w.acts, ws + w.cs,
                                                    ws + w.hs, ws + w.lin, ws + w.z, ws + w.da0, grads, nullptr);
     }
-    launch_backward_tail(d, o, w, ws, params, x, B, mask1, mask2, grads, nullptr, st);
+    if (!launch_backward_tail(d, o, pl, ws, params, x, B, mask1, mask2, grads, nullptr, false, st)) { *err = "memset dx"; return B2CNN_ECUDA; }
     if (apply_update) {
         const float bc1 = 1.f - powf(beta1, (float)step), bc2 = 1.f - powf(beta2, (float)step);
         train_adam<<<(unsigned)((o.total + 255) / 256), 256, 0, st>>>(params, adam_m, adam_v, grads, o.total, lr, beta1, beta2, eps, bc1, sqrtf(bc2));
@@ -591,29 +1081,31 @@ int train_step(const b2cnn_config *cfg, float *params, float *adam_m, float *ada
 }
 
 // the checks b2cnn_train_forward and b2cnn_train_backward share; no CUDA call
-static int autograd_args(const b2cnn_config *cfg, int64_t B, int mode, int64_t ws_bytes, bool ptrs_ok, TrainDims &d, TrainWs &w,
+static int autograd_args(const b2cnn_config *cfg, int64_t B, int mode, int64_t ws_bytes, bool ptrs_ok, TrainDims &d, TrainPlan &pl,
                          const char **err) {
     if (!cfg || !train_dims(*cfg, d, err)) return B2CNN_EINVAL;
     if (mode != B2CNN_MODE_INDEPENDENT && mode != B2CNN_MODE_SEQUENCE) { *err = "training: bad mode"; return B2CNN_EINVAL; }
     if (!ptrs_ok || B < 1) { *err = "training: null argument / bad batch"; return B2CNN_EINVAL; }
-    w = train_ws(d, B);
-    if (ws_bytes < w.total * (int64_t)sizeof(float)) { *err = "training: workspace smaller than b2cnn_train_workspace_bytes()"; return B2CNN_ESTATE; }
+    pl = train_plan(d, B);
+    if (pl.tiled && !tiled_args_ok(d, pl, B, err)) return B2CNN_EINVAL;
+    if (ws_bytes < pl.w.total * (int64_t)sizeof(float)) { *err = "training: workspace smaller than b2cnn_train_workspace_bytes()"; return B2CNN_ESTATE; }
     return B2CNN_OK;
 }
 
 int train_forward(const b2cnn_config *cfg, const float *params, const float *x, int64_t B, const float *age, int mode, const float *mask1,
                   const float *mask2, float *z_out, void *workspace, int64_t ws_bytes, cudaStream_t st, const char **err) {
     TrainDims d;
-    TrainWs w;
-    const int rc = autograd_args(cfg, B, mode, ws_bytes, params && x && age && z_out && workspace, d, w, err);
+    TrainPlan pl;
+    const int rc = autograd_args(cfg, B, mode, ws_bytes, params && x && age && z_out && workspace, d, pl, err);
     if (rc != B2CNN_OK) return rc;
     DeviceScope dev(cfg->device);
     if (!dev.ok) { *err = "cudaSetDevice"; return B2CNN_ECUDA; }
+    const TrainWs &w = pl.w;
     const BlobOff o = blob_offsets(d);
     const int sequence = mode == B2CNN_MODE_SEQUENCE ? 1 : 0;
     float *ws = reinterpret_cast<float *>(workspace);
-    train_conv_fwd<<<(unsigned)B, 256, 0, st>>>(x, params, o, d, mask1, mask2, ws + w.c1, ws + w.p1, ws + w.c2, ws + w.f);
-    train_lstm_fwd<kHeadLogits><<<1, 64, 0, st>>>(ws + w.f, params, o, d, B, sequence, age, nullptr, 1.f, ws + w.acts, ws + w.cs,
+    const float *pre0 = launch_conv_forward(d, o, pl, ws, params, x, B, mask1, mask2, st);
+    train_lstm_fwd<kHeadLogits><<<1, 64, 0, st>>>(ws + w.f, pre0, params, o, d, B, sequence, age, nullptr, 1.f, ws + w.acts, ws + w.cs,
                                                   ws + w.hs, ws + w.lin, z_out, nullptr);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) { *err = cudaGetErrorString(e); return B2CNN_ECUDA; }
@@ -621,21 +1113,25 @@ int train_forward(const b2cnn_config *cfg, const float *params, const float *x, 
 }
 
 int train_backward(const b2cnn_config *cfg, const float *params, const float *x, int64_t B, const float *age, int mode,
-                   const float *mask1, const float *mask2, const float *dz, float *grads, float *dx, float *dage, void *workspace,
-                   int64_t ws_bytes, cudaStream_t st, const char **err) {
+                   const float *mask1, const float *mask2, const float *dz, float *grads, float *dx, float *dage, int flags,
+                   void *workspace, int64_t ws_bytes, cudaStream_t st, const char **err) {
     TrainDims d;
-    TrainWs w;
-    const int rc = autograd_args(cfg, B, mode, ws_bytes, params && x && age && dz && grads && workspace, d, w, err);
+    TrainPlan pl;
+    const int rc = autograd_args(cfg, B, mode, ws_bytes, params && x && age && dz && grads && workspace, d, pl, err);
     if (rc != B2CNN_OK) return rc;
+    if (flags & ~B2CNN_TRAIN_FROZEN_CONV) { *err = "training: unknown flag"; return B2CNN_EINVAL; }
+    const bool frozen_conv = (flags & B2CNN_TRAIN_FROZEN_CONV) != 0;
+    if (frozen_conv && dx) { *err = "training: B2CNN_TRAIN_FROZEN_CONV computes no input gradient (dx must be NULL)"; return B2CNN_EINVAL; }
     DeviceScope dev(cfg->device);
     if (!dev.ok) { *err = "cudaSetDevice"; return B2CNN_ECUDA; }
+    const TrainWs &w = pl.w;
     const BlobOff o = blob_offsets(d);
     const int sequence = mode == B2CNN_MODE_SEQUENCE ? 1 : 0;
     float *ws = reinterpret_cast<float *>(workspace);
     if (cudaMemsetAsync(grads, 0, sizeof(float) * o.total, st) != cudaSuccess) { *err = "memset grads"; return B2CNN_ECUDA; }
     train_lstm_bwd<kHeadLogits><<<1, 64, 0, st>>>(params, o, d, B, sequence, age, nullptr, 1.f, dz, ws + w.acts, ws + w.cs, ws + w.hs,
                                                   ws + w.lin, nullptr, ws + w.da0, grads, dage);
-    launch_backward_tail(d, o, w, ws, params, x, B, mask1, mask2, grads, dx, st);
+    if (!launch_backward_tail(d, o, pl, ws, params, x, B, mask1, mask2, grads, dx, frozen_conv, st)) { *err = "memset dx"; return B2CNN_ECUDA; }
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) { *err = cudaGetErrorString(e); return B2CNN_ECUDA; }
     return B2CNN_OK;

@@ -12,7 +12,7 @@ hand-written forward-with-saved-activations, BPTT over the batch axis, pooling/c
 :class:`B200MyCNN`'s parameters::
 
     trainer = B200Trainer(model, lr=1e-5, pos_weight=13.5)
-    for x, age, y in loader:                       # x [B,10,120], age [B], y [B] in {0,1}
+    for x, age, y in loader:                       # x [B,10,120] or waveform windows [B,3,75000]; age [B], y [B] in {0,1}
         loss = trainer.step(x, age, y)             # == the five reference lines above
     model.predict(...)                             # scores with the updated weights
 
