@@ -475,11 +475,12 @@ const char *b2cnn_version(void);
  *                   (torch's Philox stream cannot be reproduced here, so the caller draws them); NULL = no dropout
  *   loss_out        one float: the mean BCE-with-logits loss of this batch (before the update)
  * The call allocates nothing and is asynchronous on `stream`.
- * workspace: b2cnn_train_workspace_bytes(cfg, B) bytes; a smaller one is B2CNN_ESTATE before any launch.  The layout
- * follows the kernels the shape runs, chosen from L_out alone: below 1024 features one CTA per window with every
- * intermediate in the workspace (about 8 floats per input position and window); from 1024 features on position tiles
- * that recompute the conv backward in shared memory, and the workspace holds f, d f, the LSTM records and one region
- * of partial sums (about 2 * 4 * B * L_out bytes).  On that path the gradients are the same bits from run to run. */
+ * workspace: b2cnn_train_workspace_bytes(cfg, B) bytes; a smaller one is B2CNN_ESTATE before any launch.  The conv
+ * layers run on position tiles of 128 window features that recompute the conv backward in shared memory, so the
+ * workspace holds f, d f, the LSTM records and one region of partial sums (about 2 * 4 * B * L_out bytes plus the
+ * per-window records).  The gradients are the same bits from run to run.  A geometry whose conv tile does not fit
+ * shared memory (hundreds of input channels at W = 120, 83 or more from L_out = 128 on for the MyCNN5 layer stack)
+ * is B2CNN_EINVAL. */
 typedef struct b2cnn_adam {
     float lr, beta1, beta2, eps;   /* torch defaults: 1e-3, 0.9, 0.999, 1e-8 */
 } b2cnn_adam;

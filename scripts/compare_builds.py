@@ -12,7 +12,10 @@ inputs, with seed-0 MyCNN5 weights:
     patients, then one push;
   * a generic-path scorer (C = 10, bf16) after a full window of pushes;
   * predict_record() on the tensor-core and generic paths, independent and sequence modes;
-then compares every array bit for bit.
+  * training: one B200Trainer.step (sequence, dropout masks given) at [2048, 10, 120] and at [256, 3, 75000], with the
+    loss, the gradients and the updated parameters; and one autograd forward and backward at [257, 10, 120] with the
+    logits, every parameter gradient, d x and d age;
+then compares every array bit for bit and prints each array's status and max |diff|.
 
     python scripts/compare_builds.py --baseline-lib /path/to/parent/libb2cnn.so [--lib /path/to/libb2cnn.so]
 """
@@ -105,6 +108,44 @@ def dump(path: str, batch: int, feat_batch: int, patients: int) -> None:
     for mode in ("independent", "sequence"):
         out[f"record_tc_{mode}"] = m.predict_record(rec, S, 60.0, path="tensorcore", mode=mode)
         out[f"record_generic_{mode}"] = mg.predict_record(recg, Sg, 60.0, path="generic", mode=mode)
+    del m, mg, rec, recg
+
+    # training
+    from tskd_b200.arch import BLOB_KEYS
+    from tskd_b200.trainer import B200Trainer
+
+    def train_inputs(Ct, Wt, Bt, seed):
+        ta = O.stretched(O.ARCH_MYCNN5, Ct, Wt)
+        g = torch.Generator(device=dev).manual_seed(seed)
+        xt = torch.randn(Bt, Ct, Wt, generator=g, device=dev)
+        at = torch.rand(Bt, generator=g, device=dev) * 60 + 20
+        yt = (torch.rand(Bt, generator=g, device=dev) > 0.5).float()
+        m1 = torch.bernoulli(torch.full((Bt, ta.c_mid, ta.p1), 0.9, device=dev), generator=g) / 0.9
+        m2 = torch.bernoulli(torch.full((Bt, ta.l_out), 0.9, device=dev), generator=g) / 0.9
+        return ta, xt, at, yt, m1, m2
+
+    for Ct, Wt, Bt in ((10, 120, 2048), (3, 75000, 256)):
+        ta, xt, at, yt, m1, m2 = train_inputs(Ct, Wt, Bt, 12)
+        tm = tskd_b200.B200MyCNN(tskd_b200.ARCH_PRESETS["mycnn5"].with_shape(Ct, Wt), has_out12=ta.has_out12).to(dev)
+        tm.load_state_dict(O.make_ref(ta, seed=3).state_dict())
+        tr = B200Trainer(tm, mode="sequence", dropout=0.1)
+        tag = f"train_step_{Bt}x{Ct}x{Wt}"
+        out[tag + "_loss"] = tr.step(xt, at, yt, masks=(m1, m2)).reshape(1)
+        out.update({f"{tag}_grad_{k}": v.clone() for k, v in tr.grads().items()})
+        sd = tm.state_dict()
+        out.update({f"{tag}_param_{k}": sd[k].clone() for k in BLOB_KEYS})
+        del tr, tm, xt
+    ta, xt, at, _, m1, m2 = train_inputs(10, 120, 257, 13)
+    sd = O.make_ref(ta, seed=4).state_dict()
+    params = [sd[k].to(dev).clone().requires_grad_() for k in BLOB_KEYS]
+    xt.requires_grad_()
+    at.requires_grad_()
+    z = tskd_b200.mycnn_train_forward(xt, at, params, tskd_b200.ARCH_PRESETS["mycnn5"], "sequence", m1, m2)
+    z.backward(torch.randn(257, generator=torch.Generator(device=dev).manual_seed(14), device=dev))
+    tag = "train_autograd_257x10x120"
+    out[tag + "_z"] = z.detach()
+    out.update({f"{tag}_grad_{k}": p.grad for k, p in zip(BLOB_KEYS, params)})
+    out[tag + "_dx"], out[tag + "_dage"] = xt.grad, at.grad
     torch.cuda.synchronize()
     np.savez(path, **{k: (v.cpu().numpy() if hasattr(v, "cpu") else v) for k, v in out.items()})
 
@@ -139,7 +180,7 @@ def main() -> int:
         same = a.shape == b.shape and a.dtype == b.dtype and a.tobytes() == b.tobytes()
         ok &= same
         extra = "" if a.dtype.kind == "U" else f", max |diff| {np.abs(a.astype(np.float64) - b.astype(np.float64)).max():.3g}" if a.shape == b.shape else ""
-        print(f"{k:26s} {str(a.shape):16s} {'byte-identical' if same else 'DIFFERENT'}{extra}  {a.ravel()[:1]}")
+        print(f"{k:56s} {str(a.shape):16s} {'byte-identical' if same else 'DIFFERENT'}{extra}  {a.ravel()[:1]}")
     print("all byte-identical" if ok else "builds differ")
     return 0 if ok else 1
 

@@ -134,7 +134,7 @@ CASES = [
     ("pool23-b5-seq", "pool23", None, None, 5, "sequence", 0.1, 13),
     ("mycnn5-b2048-seq", "mycnn5", 10, 120, 2048, "sequence", 0.1, 14),      # the benchmarked size, the long BPTT chain
 ]
-# at B >= 257 the conv gradients are sums of B per-window atomics in run-dependent order, and those sums cancel
+# at B >= 257 the conv gradients are sums over B x L1 >= 28 000 positions, and those long sums cancel
 BIG_B_BETA = {k: 4e-6 for k in ("conv1.weight", "conv1.bias", "conv2.weight", "conv2.bias")}
 
 

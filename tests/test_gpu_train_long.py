@@ -1,7 +1,7 @@
-"""GPU: the tiled training kernels of csrc/b2cnn_train.cu (windows with L_out >= 1024: position tiles of 128 final
-features, the conv backward recomputed per tile, W_ih_l0 products as GEMMs) element by element against the float64
-reference of oracle/train_ref.py, at the existing allowance (tests/test_gpu_train_edges.py: _check) with the two named
-differences of _check and LONG_SUM_BETA below.
+"""GPU: the training kernels of csrc/b2cnn_train.cu at long windows (position tiles of 128 final features, the conv
+backward recomputed per tile, W_ih_l0 products as GEMMs) element by element against the float64 reference of
+oracle/train_ref.py, at the existing allowance (tests/test_gpu_train_edges.py: _check) with the two named differences of
+_check and LONG_SUM_BETA below.
 
 Inputs are drawn until no pooling window holds a near-tie (oracle/train_ref.py::pool_gaps): with hundreds of thousands
 of pooling windows per batch a random input has one now and then, and there a float32 kernel may legitimately route a
@@ -30,8 +30,7 @@ from test_gpu_train_edges import TIE_GAP, _arch, _check as _check_per_tensor, _d
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
-T = 128                    # final features per tile (kLongT)
-LONG_MIN_L = 1024          # the plan's boundary (kLongMinL)
+T = 128                    # final features per tile (kT)
 POS_WEIGHT = 13.5
 CONV_KEYS = BLOB_KEYS[:4]
 # The grant tests/test_gpu_train_edges.py gives the conv gradients from B = 257 on (BIG_B_BETA: long cancelling sums), for
@@ -101,7 +100,6 @@ CASES = [
 @pytest.mark.parametrize("kind,C,W,B,mode,p,pos_weight", CASES)
 def test_fused_step_and_autograd_match_float64(kind, C, W, B, mode, p, pos_weight):
     oarch = O.stretched(O.ARCHS[kind], C, W)
-    assert oarch.l_out >= LONG_MIN_L
     ref = O.make_ref(oarch, seed=B + W)
     x, age, y, dz, m1, m2 = _clean_inputs(oarch, ref, B, B + W, p)
     truth, ref32 = _refs(ref, x, age, mode, m1, m2, dz=dz, target=y, pos_weight=pos_weight)
@@ -111,10 +109,11 @@ def test_fused_step_and_autograd_match_float64(kind, C, W, B, mode, p, pos_weigh
 
 
 # ------------------------------------------------------------------ tile seams
-@pytest.mark.parametrize("L", [LONG_MIN_L - 1, LONG_MIN_L, LONG_MIN_L + 1, LONG_MIN_L + T, LONG_MIN_L + T + 5])
+@pytest.mark.parametrize("L", [1023, 1024, 1025, 1152, 1157])
 def test_tile_seams_and_the_plan_boundary(L):
-    """L = 1023 runs the one-CTA-per-window kernels, 1024 and 1152 are whole tiles, 1025 leaves a last tile of one
-    feature; every one against float64, d x included"""
+    """L = 1023 ends on a last tile of 127 features, 1024 and 1152 are whole tiles, 1025 leaves a last tile of one
+    feature, and 1024 / 1025 straddle the point where the pre-activation GEMM takes a second slice of 1024 positions;
+    every one against float64, d x included"""
     oarch = O.stretched(O.ARCH_MYCNN5, 3, _window_for("mycnn5", L))
     assert oarch.l_out == L
     ref = O.make_ref(oarch, seed=L)
@@ -286,8 +285,8 @@ print(json.dumps(lists))
 """
 
 
-@pytest.mark.parametrize("C,W,conv_bwd,dfeat", [(3, 7504, "train_conv_bwd_tiled", "train_dfeat_tiled"), (10, 120, "train_conv_bwd(", "train_dfeat(")])
-def test_frozen_conv_launches_no_conv_backward(C, W, conv_bwd, dfeat):
+@pytest.mark.parametrize("C,W", [(3, 7504), (10, 120)])
+def test_frozen_conv_launches_no_conv_backward(C, W):
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     env = dict(os.environ, PYTHONPATH=os.pathsep.join([root] + [p for p in [os.environ.get("PYTHONPATH")] if p]))
     cmd = [sys.executable] + (["-s"] if sys.flags.no_user_site else []) + ["-c", _LAUNCH_LIST, str(C), str(W)]
@@ -295,18 +294,18 @@ def test_frozen_conv_launches_no_conv_backward(C, W, conv_bwd, dfeat):
     assert r.returncode == 0, r.stderr[-3000:]
     full, frozen = [collections.Counter(d) for d in json.loads(r.stdout.strip().splitlines()[-1])]
     has = lambda c, name: any(name in k for k in c)
-    assert has(full, conv_bwd) and has(full, dfeat), full
-    assert not has(frozen, conv_bwd) and not has(frozen, dfeat) and not has(frozen, "train_dx") and not has(frozen, "grad_reduce"), frozen
+    assert has(full, "train_conv_bwd(") and has(full, "train_dfeat(") and has(full, "grad_reduce"), full
+    assert has(full, "train_conv_fwd(") and has(full, "train_pre0_partial") and not has(full, "train_dx"), full
+    assert not has(frozen, "train_conv_bwd") and not has(frozen, "train_dfeat") and not has(frozen, "grad_reduce"), frozen
     assert has(frozen, "train_lstm_bwd") and has(frozen, "train_wih0_grad"), frozen
-    if W > 120:                                                           # the tiled plan runs none of the per-window kernels
-        assert not has(full, "train_conv_fwd(") and not has(full, "train_conv_bwd(") and has(full, "train_pre0_partial"), full
 
 
 # ------------------------------------------------------------------ run-to-run, the eval path, Adam
-def test_two_runs_give_the_same_bits():
-    oarch = O.stretched(O.ARCH_MYCNN5, 3, 7504)
+def _two_runs(C, W, B):
+    """two fused sequence steps with dropout, then autograd with d x and d age, twice from the same state: equal bits"""
+    oarch = O.stretched(O.ARCH_MYCNN5, C, W)
     ref = O.make_ref(oarch, seed=7)
-    x, age, y, dz, m1, m2 = _inputs(oarch, 40, 7, 0.1)
+    x, age, y, dz, m1, m2 = _inputs(oarch, B, 7, 0.1)
     runs = []
     for _ in range(2):
         model = tskd_b200.B200MyCNN(_arch(oarch), has_out12=oarch.has_out12).to(DEV)
@@ -320,6 +319,16 @@ def test_two_runs_give_the_same_bits():
     for k in BLOB_KEYS:
         assert torch.equal(ga[k], gb[k]) and torch.equal(pa[k], pb[k]) and torch.equal(da["grads"][k], db["grads"][k]), k
     assert torch.equal(da["dx"], db["dx"]) and torch.equal(da["dage"], db["dage"])
+
+
+def test_two_runs_give_the_same_bits():
+    _two_runs(3, 7504, 40)
+
+
+@pytest.mark.parametrize("B", [257, 2048])
+def test_two_runs_give_the_same_bits_at_the_training_shape(B):
+    """[B,10,120]: one tile per window, 257 / 1024 conv-backward CTAs"""
+    _two_runs(10, 120, B)
 
 
 @pytest.mark.parametrize("mode", ["sequence", "independent"])

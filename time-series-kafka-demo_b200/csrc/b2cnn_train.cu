@@ -11,32 +11,32 @@
 //   loss = mean_b( max(z,0) - z y + log(1 + exp(-|z|)) )
 //
 // Dropout cannot share torch's Philox stream, so the two masks are INPUTS (already scaled by 1/(1-p), or NULL = no
-// dropout); everything else is bit-for-bit the same graph, differentiated by hand:
-//   train_conv_fwd   per window: c1, p1, c2, f (kept for the backward pass)
-//   train_lstm_fwd   one CTA scans the batch axis, keeps gate activations / cell / hidden states, logits, loss
-//   train_lstm_bwd   BPTT over the batch axis: gradients of the head and of every recurrent matrix, d(gates of layer 0)
-//   train_wih0_grad  dW_ih_l0 = d(gates0)^T x f            train_dfeat   d f = d(gates0) x W_ih_l0
-//   train_conv_bwd   per window: dropout / pool (argmax routing, first maximum like ATen) / tanh / conv2 / conv1 backward
-//   train_dx         d x (the input gradient), gather form: one thread per input sample
-//   train_adam       torch.optim.Adam (no amsgrad, weight_decay 0) on the packed parameter blob
+// dropout); everything else is bit-for-bit the same graph, differentiated by hand.  The conv layers work on position
+// tiles of kT = 128 final features of one window (a window with fewer features, such as the training shape [B,10,120]
+// with L = 25, is one tile; the waveform window [B,3,75000] has L = 18745, 147 tiles):
+//   train_conv_fwd         grid (position tiles x B): a CTA stages its tile's x span in shared memory, runs conv_tile()
+//                          there and writes only f
+//   train_pre0_partial     layer-0 pre-activations f . W_ih_l0^T as a split-K GEMM over slices of kPre0Slice positions;
+//                          with more than one slice train_sum_chunks adds the partials in slice order
+//   train_lstm_fwd         one CTA scans the batch axis from those pre-activations, keeps gate activations / cell /
+//                          hidden states, logits, loss
+//   train_lstm_bwd         BPTT over the batch axis: gradients of the head and of every recurrent matrix, d(gates of
+//                          layer 0) = da0
+//   train_wih0_grad        dW_ih_l0 = da0^T f with f read once: a thread owns a position and all 64 gate rows, the batch
+//                          is split into chunks, and train_sum_chunks adds the chunk partials in chunk order
+//   train_dfeat            d f = da0 W_ih_l0 with a thread's 64 W_ih_l0 values in registers
+//   train_conv_bwd         grid (position tiles x groups of windows): recomputes c1 / d1 / c2 with conv_tile(), back-
+//                          propagates the gradients of ITS OWN features through its receptive span in shared memory
+//                          (dropout / pool with first-maximum routing like ATen / tanh / conv2 / conv1), keeps the conv
+//                          weight-gradient partials of its windows and adds d x into a zeroed array
+//   train_conv_grad_reduce sums the per-CTA partials in a fixed order (no atomic on a parameter gradient: gradients
+//                          repeat bit for bit)
+//   train_adam             torch.optim.Adam (no amsgrad, weight_decay 0) on the packed parameter blob
 // The head of the two LSTM kernels is a template parameter (Head): the fused step's BCE, BCE with pos_weight, or logits
 // only, with d loss / d z supplied by the caller (b2cnn_train_forward / b2cnn_train_backward, driven by torch autograd).
-// Those are launch-latency kernels for the training shape [B,10,120] (44 k MAC per window): one CTA per window, every
-// intermediate in the caller's workspace.  train_plan() sends windows with L >= kLongMinL features (the waveform windows,
-// [B,3,75000] -> L = 18745) to a second set, chosen from L alone so that a window's arithmetic never depends on its batch:
-//   train_conv_fwd_tiled   grid (position tiles x B): a CTA stages the x span of kLongT final features in shared memory,
-//                          runs conv_tile() there and writes only f (bit-identical to train_conv_fwd's)
-//   train_pre0_partial / train_pre0_reduce   layer-0 pre-activations f . W_ih_l0^T as a split-K GEMM, partials added
-//                          in slice order; train_lstm_fwd takes them through a pointer
-//   train_wih0_grad_tiled / train_sum_chunks  dW_ih_l0 = da0^T f with f read once: a thread owns a position and all 64
-//                          gate rows, the batch is split into chunks, chunk partials are added in chunk order
-//   train_dfeat_tiled      d f with a thread's 64 W_ih_l0 values in registers (train_dfeat's summation order)
-//   train_conv_bwd_tiled   grid (position tiles x groups of kLongWin windows): recomputes c1 / d1 / c2 with conv_tile(),
-//                          back-propagates the gradients of ITS OWN kLongT features through its receptive span in shared
-//                          memory, keeps the conv weight-gradient partials of its windows and adds d x into a zeroed array
-//   train_conv_grad_reduce sums the per-CTA partials in a fixed order (no atomics: gradients repeat bit for bit)
 // Everything below f is linear in d f, so the sum over tiles of what each tile back-propagates from its own features is
-// the full gradient; no halo is exchanged and dc1 / dd1 / dc2 never reach global memory.
+// the full gradient; no halo is exchanged and dc1 / dd1 / dc2 never reach global memory.  A window's values depend on
+// its geometry alone; the batch sets only the order in which conv-gradient partials and dW_ih_l0's chunks are added.
 #include <cfloat>
 #include <cstring>
 
@@ -76,25 +76,25 @@ static BlobOff blob_offsets(const TrainDims &d) {
 
 // workspace layout (floats)
 struct TrainWs {
-    int64_t c1, p1, c2, f, acts, cs, hs, lin, z, da0, dfeat, dc2, dd1, dc1, pre0, part, total;
+    int64_t f, pre0, acts, cs, hs, lin, z, da0, dfeat, part, total;
 };
 
-// ---- the tiled kernels' constants ----
-constexpr int kLongMinL = 1024;     // L >= this: the tiled kernels
-constexpr int kLongT = 128;         // final features per tile
-constexpr int kLongThreads = 256;
-constexpr int kLongWin = 8;         // windows per CTA of the tiled conv backward (one weight-gradient partial per CTA)
+constexpr int kT = 128;             // final features per tile
+constexpr int kThreads = 256;       // threads of a conv tile's CTA
+constexpr int kWin = 8;             // at most this many windows per CTA of the conv backward (one partial row per CTA)
+constexpr int kBwdCtas = 1024;      // the conv backward puts several windows in a CTA only beyond this many CTAs
 constexpr int kPre0Slice = 1024;    // positions per split-K slice of the pre-activation GEMM
 constexpr int kWihChunks = 16;      // at most this many batch chunks in dW_ih_l0
-constexpr int kRowBatch = 64;       // da0 rows staged per pass of train_dfeat_tiled / train_wih0_grad_tiled
+constexpr int kRowBatch = 64;       // da0 rows staged per pass of train_dfeat / train_wih0_grad
 
 // float offsets of a conv tile's buffers in dynamic shared memory; xp / pp are the row pitches of x and d1 / dd1
 struct TileSmem {
     int w1, b1, w2, b2, x, xp, c1, d1, pp, c2, df, dc2, dd1, dc1, g, total;
 };
-// The largest tile: kLongT features plus the few positions the last tile takes on beyond its last pooling window.
+// The largest tile: min(kT, L) features plus the few positions the last tile takes on beyond its last pooling window.
 __host__ __device__ inline TileSmem tile_smem(const TrainDims &d, bool backward) {
-    const int n2 = d.PS * (kLongT - 1) + d.PK + d.PS - 1, np1 = n2 + d.K2 - 1, n1 = d.PS * (np1 - 1) + d.PK + d.PS - 1, nx = n1 + d.K1 - 1;
+    const int T = d.L < kT ? d.L : kT;
+    const int n2 = d.PS * (T - 1) + d.PK + d.PS - 1, np1 = n2 + d.K2 - 1, n1 = d.PS * (np1 - 1) + d.PK + d.PS - 1, nx = n1 + d.K1 - 1;
     TileSmem s;
     int p = 0;
     auto take = [&](int n) { int at = p; p += (n + 3) / 4 * 4; return at; };
@@ -110,7 +110,7 @@ __host__ __device__ inline TileSmem tile_smem(const TrainDims &d, bool backward)
     s.c2 = take(n2);
     s.df = s.dc2 = s.dd1 = s.dc1 = s.g = 0;
     if (backward) {
-        s.df = take(kLongT);
+        s.df = take(T);
         s.dc2 = take(n2);
         s.dd1 = take(kCMid * s.pp);
         s.dc1 = take(kCMid * n1);         // [position][oc]
@@ -120,66 +120,39 @@ __host__ __device__ inline TileSmem tile_smem(const TrainDims &d, bool backward)
     return s;
 }
 
-// Which kernels a shape runs and what they need; read by every entry point and by the workspace query.
+// The grids and the workspace of a shape; read by every entry point and by the workspace query.
 struct TrainPlan {
-    bool tiled;
     TrainWs w;
-    int tiles, slices, wih_chunk, wih_chunks, groups, n_conv;
+    int tiles, slices, wih_chunk, wih_chunks, win, groups, n_conv;
     int64_t part_rows;                  // per-CTA conv weight-gradient partials
     size_t smem_fwd, smem_bwd;
 };
 
-static TrainWs train_ws_short(const TrainDims &d, int64_t B) {
-    TrainWs w;
+static TrainPlan train_plan(const TrainDims &d, int64_t B) {
+    TrainPlan pl{};
+    pl.tiles = (d.L + kT - 1) / kT;
+    pl.slices = (d.L + kPre0Slice - 1) / kPre0Slice;
+    pl.wih_chunk = (int)((B + kWihChunks - 1) / kWihChunks);
+    pl.wih_chunks = (int)((B + pl.wih_chunk - 1) / pl.wih_chunk);
+    // windows per conv-backward CTA: ceil(B x tiles / kBwdCtas) within [1, kWin], from the shape alone, never the device
+    const int64_t bt = B * pl.tiles, win = (bt + kBwdCtas - 1) / kBwdCtas;
+    pl.win = (int)(win < 1 ? 1 : win > kWin ? kWin : win);
+    pl.groups = (int)((B + pl.win - 1) / pl.win);
+    pl.n_conv = kCMid * d.C * d.K1 + kCMid + kCMid * d.K2 + 1;
+    pl.part_rows = (int64_t)pl.tiles * pl.groups;
+    pl.smem_fwd = sizeof(float) * tile_smem(d, false).total;
+    pl.smem_bwd = sizeof(float) * tile_smem(d, true).total;
+    TrainWs &w = pl.w;
     int64_t p = 0;
     auto take = [&](int64_t n) { int64_t at = p; p += (n + 63) / 64 * 64; return at; };
-    w.c1 = take(B * kCMid * d.L1);
-    w.p1 = take(B * kCMid * d.P1);
-    w.c2 = take(B * d.L2);
     w.f = take(B * d.L);
+    w.pre0 = take(B * kGates);          // f . W_ih_l0^T
     w.acts = take(B * 2 * kGates);      // [t][layer][i f g o] post-activation
     w.cs = take(B * 2 * kHidden);       // [t][layer] cell state
     w.hs = take(B * 2 * kHidden);       // [t][layer] hidden state
     w.lin = take(B);                    // out(h1) before the age scale (d age needs it)
     w.z = take(B);
     w.da0 = take(B * kGates);           // d loss / d (layer-0 gate pre-activations)
-    w.dfeat = take(B * d.L);
-    w.dc2 = take(B * d.L2);
-    w.dd1 = take(B * kCMid * d.P1);
-    w.dc1 = take(B * kCMid * d.L1);
-    w.pre0 = w.part = 0;
-    w.total = p;
-    return w;
-}
-
-static TrainPlan train_plan(const TrainDims &d, int64_t B) {
-    TrainPlan pl{};
-    pl.tiled = d.L >= kLongMinL;
-    if (!pl.tiled) {
-        pl.w = train_ws_short(d, B);
-        return pl;
-    }
-    pl.tiles = (d.L + kLongT - 1) / kLongT;
-    pl.slices = (d.L + kPre0Slice - 1) / kPre0Slice;
-    pl.wih_chunk = (int)((B + kWihChunks - 1) / kWihChunks);
-    pl.wih_chunks = (int)((B + pl.wih_chunk - 1) / pl.wih_chunk);
-    pl.groups = (int)((B + kLongWin - 1) / kLongWin);
-    pl.n_conv = kCMid * d.C * d.K1 + kCMid + kCMid * d.K2 + 1;
-    pl.part_rows = (int64_t)pl.tiles * pl.groups;
-    pl.smem_fwd = sizeof(float) * tile_smem(d, false).total;
-    pl.smem_bwd = sizeof(float) * tile_smem(d, true).total;
-    TrainWs &w = pl.w;
-    w = TrainWs{};
-    int64_t p = 0;
-    auto take = [&](int64_t n) { int64_t at = p; p += (n + 63) / 64 * 64; return at; };
-    w.f = take(B * d.L);
-    w.pre0 = take(B * kGates);          // f . W_ih_l0^T
-    w.acts = take(B * 2 * kGates);
-    w.cs = take(B * 2 * kHidden);
-    w.hs = take(B * 2 * kHidden);
-    w.lin = take(B);
-    w.z = take(B);
-    w.da0 = take(B * kGates);
     w.dfeat = take(B * d.L);
     // one region for the partial sums of three reductions that never overlap in time
     int64_t part = (int64_t)pl.slices * B * kGates;
@@ -204,59 +177,14 @@ __device__ __forceinline__ float dtanhf_(float v) {
 enum Head : int { kHeadLogits = 0, kHeadBce = 1, kHeadBcePw = 2 };
 
 // ------------------------------------------------------------------------------------------------------------------
-// forward, convolutional part: one CTA per window
-// ------------------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256)
-train_conv_fwd(const float *__restrict__ x, const float *__restrict__ prm, BlobOff o, TrainDims d, const float *__restrict__ mask1,
-               const float *__restrict__ mask2, float *__restrict__ c1, float *__restrict__ p1, float *__restrict__ c2,
-               float *__restrict__ f) {
-    const int b = blockIdx.x, tid = threadIdx.x;
-    const float *xb = x + (int64_t)b * d.C * d.W;
-    float *c1b = c1 + (int64_t)b * kCMid * d.L1, *p1b = p1 + (int64_t)b * kCMid * d.P1;
-    float *c2b = c2 + (int64_t)b * d.L2, *fb = f + (int64_t)b * d.L;
-    // conv1: same summation order as the inference kernels (channels outer, taps inner, fmaf chain from the bias)
-    for (int e = tid; e < kCMid * d.L1; e += blockDim.x) {
-        const int oc = e / d.L1, t = e % d.L1;
-        float acc = prm[o.b1 + oc];
-        for (int c = 0; c < d.C; ++c)
-            for (int k = 0; k < d.K1; ++k) acc = fmaf(prm[o.w1 + ((int64_t)oc * d.C + c) * d.K1 + k], xb[(int64_t)c * d.W + t + k], acc);
-        c1b[e] = acc;
-    }
-    __syncthreads();
-    for (int e = tid; e < kCMid * d.P1; e += blockDim.x) {
-        const int oc = e / d.P1, i = e % d.P1;
-        float m = c1b[oc * d.L1 + d.PS * i];
-        for (int j = 1; j < d.PK; ++j) m = max_nan(m, c1b[oc * d.L1 + d.PS * i + j]);
-        p1b[e] = tanhf(m);                  // pooling before tanh: tanh is monotone, and a NaN in the window wins either way
-    }
-    __syncthreads();
-    for (int t = tid; t < d.L2; t += blockDim.x) {
-        float acc = prm[o.b2];
-        for (int oc = 0; oc < kCMid; ++oc)
-            for (int k = 0; k < d.K2; ++k) {
-                const int64_t at = (int64_t)oc * d.P1 + t + k;
-                const float dv = p1b[at] * (mask1 ? mask1[(int64_t)b * kCMid * d.P1 + at] : 1.0f);
-                acc = fmaf(prm[o.w2 + oc * d.K2 + k], dv, acc);
-            }
-        c2b[t] = acc;
-    }
-    __syncthreads();
-    for (int i = tid; i < d.L; i += blockDim.x) {
-        float m = c2b[d.PS * i];
-        for (int j = 1; j < d.PK; ++j) m = max_nan(m, c2b[d.PS * i + j]);
-        fb[i] = tanhf(m) * (mask2 ? mask2[(int64_t)b * d.L + i] : 1.0f);
-    }
-}
-
-// ------------------------------------------------------------------------------------------------------------------
 // LSTM forward over the batch axis with everything the backward pass needs kept; logits and loss.
-// One CTA of 64 threads: thread r owns gate row r of every matrix.  pre0 != NULL: W_ih_l0 f_t was computed before the
-// scan (pre0[t][r]); NULL: the thread computes its dot product at every step.  sequence == 0: every step starts from the zero state
-// (independent windows).  HEAD == kHeadLogits: target and loss_out are not used.
+// One CTA of 64 threads: thread r owns gate row r of every matrix; W_ih_l0 f_t was computed before the scan (pre0[t][r]).
+// sequence == 0: every step starts from the zero state (independent windows).  HEAD == kHeadLogits: target and loss_out
+// are not used.
 // ------------------------------------------------------------------------------------------------------------------
 template <int HEAD>
 __global__ void __launch_bounds__(64)
-train_lstm_fwd(const float *__restrict__ f, const float *__restrict__ pre0, const float *__restrict__ prm, BlobOff o, TrainDims d, int64_t B, int sequence,
+train_lstm_fwd(const float *__restrict__ pre0, const float *__restrict__ prm, BlobOff o, TrainDims d, int64_t B, int sequence,
                const float *__restrict__ age, const float *__restrict__ target, float pos_weight, float *__restrict__ acts,
                float *__restrict__ cs, float *__restrict__ hs, float *__restrict__ lin, float *__restrict__ z,
                float *__restrict__ loss_out) {
@@ -272,14 +200,7 @@ train_lstm_fwd(const float *__restrict__ f, const float *__restrict__ pre0, cons
         }
         // ---- layer 0: g = (W_ih f_t + b_ih) + (W_hh h_{t-1} + b_hh)
         {
-            float a = 0.f;
-            if (pre0) {
-                a = pre0[t * kGates + r];
-            } else {
-                const float *ft = f + t * d.L;
-                const float *wr = prm + o.wih0 + (int64_t)r * d.L;
-                for (int p = 0; p < d.L; ++p) a = fmaf(wr[p], ft[p], a);
-            }
+            const float a = pre0[t * kGates + r];
             float rr = 0.f;
             for (int k = 0; k < kHidden; ++k) rr = fmaf(prm[o.whh0 + r * kHidden + k], h0[k], rr);
             g[r] = (a + prm[o.bih0 + r]) + (rr + prm[o.bhh0 + r]);
@@ -464,155 +385,20 @@ train_lstm_bwd(const float *__restrict__ prm, BlobOff o, TrainDims d, int64_t B,
     if (r == 0) grad[o.bo] = gbo;
 }
 
-// dW_ih_l0[g][p] = sum_t da0[t][g] f[t][p]
-__global__ void train_wih0_grad(const float *__restrict__ da0, const float *__restrict__ f, int64_t B, int L, float *__restrict__ gw) {
-    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (e >= (int64_t)kGates * L) return;
-    const int g = (int)(e / L), p = (int)(e % L);
-    float a = 0.f;
-    for (int64_t t = 0; t < B; ++t) a = fmaf(da0[t * kGates + g], f[t * L + p], a);
-    gw[e] = a;
-}
-// d f[t][p] = sum_g da0[t][g] W_ih_l0[g][p]
-__global__ void train_dfeat(const float *__restrict__ da0, const float *__restrict__ wih0, int64_t B, int L, float *__restrict__ dfeat) {
-    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (e >= B * L) return;
-    const int64_t t = e / L;
-    const int p = (int)(e % L);
-    float a = 0.f;
-    for (int g = 0; g < kGates; ++g) a = fmaf(da0[t * kGates + g], wih0[(int64_t)g * L + p], a);
-    dfeat[e] = a;
-}
-
-// first maximum of a pooling window, like ATen's max_pool1d ((v > m) || isnan(v) replaces).  This is the first maximum
-// of the pre-activation; the reference pools after tanh and takes the first maximum there.  The two differ only where
-// tanhf maps distinct pre-activations to one float: this choice is the one exact arithmetic makes.
-__device__ __forceinline__ int pool_argmax(const float *v, int start, int pk) {
-    int best = start;
-    float m = v[start];
-    for (int j = 1; j < pk; ++j) {
-        const float c = v[start + j];
-        if (c > m || c != c) { m = c; best = start + j; }
-    }
-    return best;
-}
-
 // ------------------------------------------------------------------------------------------------------------------
-// backward, convolutional part: one CTA per window; conv weight gradients are reduced per CTA and added atomically
-// ------------------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256)
-train_conv_bwd(const float *__restrict__ x, const float *__restrict__ prm, BlobOff o, TrainDims d, const float *__restrict__ mask1,
-               const float *__restrict__ mask2, const float *__restrict__ c1, const float *__restrict__ p1,
-               const float *__restrict__ c2, const float *__restrict__ dfeat, float *__restrict__ dc2, float *__restrict__ dd1,
-               float *__restrict__ dc1, float *__restrict__ grad) {
-    const int b = blockIdx.x, tid = threadIdx.x;
-    const float *xb = x + (int64_t)b * d.C * d.W;
-    const float *c1b = c1 + (int64_t)b * kCMid * d.L1, *p1b = p1 + (int64_t)b * kCMid * d.P1, *c2b = c2 + (int64_t)b * d.L2;
-    const float *dfb = dfeat + (int64_t)b * d.L;
-    float *dc2b = dc2 + (int64_t)b * d.L2, *dd1b = dd1 + (int64_t)b * kCMid * d.P1, *dc1b = dc1 + (int64_t)b * kCMid * d.L1;
-    __shared__ float red[256];
-    // ---- dropout 2 + pool 2 + tanh: gather form -- position t collects from the (overlapping) windows whose maximum it is
-    for (int t = tid; t < d.L2; t += blockDim.x) {
-        float a = 0.f;
-        int i_lo = (t - d.PK + d.PS) / d.PS;                   // ceil((t - PK + 1) / PS)
-        if (t - d.PK + 1 <= 0) i_lo = 0;
-        for (int i = i_lo; i <= t / d.PS && i < d.L; ++i)
-            if (pool_argmax(c2b, d.PS * i, d.PK) == t) a += dfb[i] * (mask2 ? mask2[(int64_t)b * d.L + i] : 1.0f);
-        dc2b[t] = a * dtanhf_(c2b[t]);
-    }
-    __syncthreads();
-    // ---- conv2: weight / bias gradients (block reduction, one atomic per value and CTA), d d1
-    for (int e = 0; e < kCMid * d.K2 + 1; ++e) {
-        float part = 0.f;
-        if (e < kCMid * d.K2) {
-            const int oc = e / d.K2, k = e % d.K2;
-            for (int t = tid; t < d.L2; t += blockDim.x) {
-                const int64_t at = (int64_t)oc * d.P1 + t + k;
-                part = fmaf(dc2b[t], p1b[at] * (mask1 ? mask1[(int64_t)b * kCMid * d.P1 + at] : 1.0f), part);
-            }
-        } else {
-            for (int t = tid; t < d.L2; t += blockDim.x) part += dc2b[t];
-        }
-        red[tid] = part;
-        __syncthreads();
-        for (int sft = 128; sft > 0; sft >>= 1) {
-            if (tid < sft) red[tid] += red[tid + sft];
-            __syncthreads();
-        }
-        if (tid == 0) atomicAdd(grad + (e < kCMid * d.K2 ? o.w2 + e : o.b2), red[0]);
-        __syncthreads();
-    }
-    for (int e = tid; e < kCMid * d.P1; e += blockDim.x) {
-        const int oc = e / d.P1, uu = e % d.P1;
-        float a = 0.f;
-        for (int k = 0; k < d.K2; ++k) {
-            const int t = uu - k;
-            if (t >= 0 && t < d.L2) a = fmaf(prm[o.w2 + oc * d.K2 + k], dc2b[t], a);
-        }
-        dd1b[e] = a * (mask1 ? mask1[(int64_t)b * kCMid * d.P1 + e] : 1.0f);     // through dropout 1: d p1
-    }
-    __syncthreads();
-    // ---- pool 1 + tanh
-    for (int e = tid; e < kCMid * d.L1; e += blockDim.x) {
-        const int oc = e / d.L1, t = e % d.L1;
-        const float *row = c1b + oc * d.L1;
-        float a = 0.f;
-        int i_lo = (t - d.PK + d.PS) / d.PS;
-        if (t - d.PK + 1 <= 0) i_lo = 0;
-        for (int i = i_lo; i <= t / d.PS && i < d.P1; ++i)
-            if (pool_argmax(row, d.PS * i, d.PK) == t) a += dd1b[oc * d.P1 + i];
-        dc1b[e] = a * dtanhf_(row[t]);
-    }
-    __syncthreads();
-    // ---- conv1: one thread per weight, a dot product over the positions
-    for (int e = tid; e < kCMid * d.C * d.K1 + kCMid; e += blockDim.x) {
-        float a = 0.f;
-        if (e < kCMid * d.C * d.K1) {
-            const int oc = e / (d.C * d.K1), c = (e / d.K1) % d.C, k = e % d.K1;
-            const float *dr = dc1b + oc * d.L1, *xr = xb + (int64_t)c * d.W + k;
-            for (int t = 0; t < d.L1; ++t) a = fmaf(dr[t], xr[t], a);
-            atomicAdd(grad + o.w1 + e, a);
-        } else {
-            const int oc = e - kCMid * d.C * d.K1;
-            const float *dr = dc1b + oc * d.L1;
-            for (int t = 0; t < d.L1; ++t) a += dr[t];
-            atomicAdd(grad + o.b1 + oc, a);
-        }
-    }
-}
-
-// d x[b][c][t] = sum_oc sum_k w1[oc][c][k] * dc1[b][oc][t-k] over the valid t-k in [0, L1): conv1's input gradient in
-// gather form, one thread per input sample (no atomics)
-__global__ void train_dx(const float *__restrict__ dc1, const float *__restrict__ prm, BlobOff o, TrainDims d, int64_t B,
-                         float *__restrict__ dx) {
-    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (e >= B * d.C * d.W) return;
-    const int t = (int)(e % d.W), c = (int)((e / d.W) % d.C);
-    const int64_t b = e / ((int64_t)d.C * d.W);
-    const int k_lo = max(0, t - (d.L1 - 1)), k_hi = min(d.K1 - 1, t);
-    float a = 0.f;
-    for (int oc = 0; oc < kCMid; ++oc) {
-        const float *wr = prm + o.w1 + ((int64_t)oc * d.C + c) * d.K1;
-        const float *dr = dc1 + (b * kCMid + oc) * d.L1 + t;
-        for (int k = k_lo; k <= k_hi; ++k) a = fmaf(wr[k], dr[-k], a);
-    }
-    dx[e] = a;
-}
-
-// ------------------------------------------------------------------------------------------------------------------
-// The tiled kernels (L >= kLongMinL).
+// Position tiles.
 // Tile `tile` of a window owns final features [i0, i0 + nf).  Their receptive span starts at c2 / p1 position
 // s2 = PS i0 and at c1 / x position s1 = PS s2 and holds n2 / np1 / n1 / nx positions of c2 / p1 / c1 / x.  The last tile
 // also takes the positions after the last pooling window (a geometry may leave a few): they get no gradient, but a NaN
-// there reaches d tanh as it does in train_conv_bwd.
+// there reaches d tanh and so the conv gradients, as in the reference.
 // ------------------------------------------------------------------------------------------------------------------
 struct Tile {
     int i0, nf, s2, s1, n2, np1, n1, nx;
 };
 __device__ __forceinline__ Tile tile_of(const TrainDims &d, int tile) {
     Tile t;
-    t.i0 = tile * kLongT;
-    t.nf = min(kLongT, d.L - t.i0);
+    t.i0 = tile * kT;
+    t.nf = min(kT, d.L - t.i0);
     t.s2 = d.PS * t.i0;
     t.s1 = d.PS * t.s2;
     const bool last = t.i0 + t.nf == d.L;
@@ -627,21 +413,22 @@ __device__ __forceinline__ Tile tile_of(const TrainDims &d, int tile) {
 __device__ __forceinline__ void tile_stage_weights(const float *__restrict__ prm, const BlobOff &o, const TrainDims &d, const TileSmem &s,
                                                    float *sm, int tid) {
     const int ck = d.C * d.K1;
-    for (int e = tid; e < kCMid * ck; e += kLongThreads) sm[s.w1 + (e % ck) * kCMid + e / ck] = prm[o.w1 + e];
+    for (int e = tid; e < kCMid * ck; e += kThreads) sm[s.w1 + (e % ck) * kCMid + e / ck] = prm[o.w1 + e];
     if (tid < kCMid) sm[s.b1 + tid] = prm[o.b1 + tid];
-    for (int e = tid; e < kCMid * d.K2; e += kLongThreads) sm[s.w2 + e] = prm[o.w2 + e];
+    for (int e = tid; e < kCMid * d.K2; e += kThreads) sm[s.w2 + e] = prm[o.w2 + e];
     if (tid == 0) sm[s.b2] = prm[o.b2];
 }
 
 // One tile of one window, everything in shared memory: x span -> c1 -> pool -> tanh -> mask1 (d1) -> c2.  Every sum in
-// train_conv_fwd's order (bias first, channels outer, taps inner, fmaf), so c1, d1 and c2 are the values it computes.
+// the inference kernels' order (an fmaf chain from the bias, channels outer, taps inner), so a value does not depend on
+// the tile that computes it.  Pooling comes before tanh: tanh is monotone, and a NaN in the window wins either way.
 // xb / m1b: the window's x [C][W] and its mask1 [4][P1] (or NULL).  Ends with a barrier.
 __device__ __forceinline__ void conv_tile(const float *__restrict__ xb, const float *__restrict__ m1b, const TrainDims &d, const Tile &t,
                                           const TileSmem &s, float *sm, int tid) {
     for (int c = 0; c < d.C; ++c)
-        for (int j = tid; j < t.nx; j += kLongThreads) sm[s.x + c * s.xp + j] = xb[(int64_t)c * d.W + t.s1 + j];
+        for (int j = tid; j < t.nx; j += kThreads) sm[s.x + c * s.xp + j] = xb[(int64_t)c * d.W + t.s1 + j];
     __syncthreads();
-    for (int j = tid; j < t.n1; j += kLongThreads) {
+    for (int j = tid; j < t.n1; j += kThreads) {
         float4 acc = *reinterpret_cast<const float4 *>(sm + s.b1);
         for (int c = 0; c < d.C; ++c) {
             const float *xr = sm + s.x + c * s.xp + j;
@@ -655,7 +442,7 @@ __device__ __forceinline__ void conv_tile(const float *__restrict__ xb, const fl
         *reinterpret_cast<float4 *>(sm + s.c1 + 4 * j) = acc;
     }
     __syncthreads();
-    for (int e = tid; e < kCMid * t.np1; e += kLongThreads) {
+    for (int e = tid; e < kCMid * t.np1; e += kThreads) {
         const int oc = e / t.np1, i = e % t.np1;
         const float *col = sm + s.c1 + oc;
         float m = col[4 * d.PS * i];
@@ -663,7 +450,7 @@ __device__ __forceinline__ void conv_tile(const float *__restrict__ xb, const fl
         sm[s.d1 + oc * s.pp + i] = tanhf(m) * (m1b ? m1b[(int64_t)oc * d.P1 + t.s2 + i] : 1.0f);
     }
     __syncthreads();
-    for (int j = tid; j < t.n2; j += kLongThreads) {
+    for (int j = tid; j < t.n2; j += kThreads) {
         float acc = sm[s.b2];
         for (int oc = 0; oc < kCMid; ++oc)
             for (int k = 0; k < d.K2; ++k) acc = fmaf(sm[s.w2 + oc * d.K2 + k], sm[s.d1 + oc * s.pp + j + k], acc);
@@ -673,9 +460,9 @@ __device__ __forceinline__ void conv_tile(const float *__restrict__ xb, const fl
 }
 
 // grid: B x tiles CTAs, window-major
-__global__ void __launch_bounds__(kLongThreads)
-train_conv_fwd_tiled(const float *__restrict__ x, const float *__restrict__ prm, BlobOff o, TrainDims d, int tiles,
-                     const float *__restrict__ mask1, const float *__restrict__ mask2, float *__restrict__ f) {
+__global__ void __launch_bounds__(kThreads)
+train_conv_fwd(const float *__restrict__ x, const float *__restrict__ prm, BlobOff o, TrainDims d, int tiles,
+               const float *__restrict__ mask1, const float *__restrict__ mask2, float *__restrict__ f) {
     extern __shared__ __align__(16) float sm[];
     const TileSmem s = tile_smem(d, false);
     const int tid = threadIdx.x;
@@ -683,7 +470,7 @@ train_conv_fwd_tiled(const float *__restrict__ x, const float *__restrict__ prm,
     const Tile t = tile_of(d, blockIdx.x % tiles);
     tile_stage_weights(prm, o, d, s, sm, tid);
     conv_tile(x + b * d.C * d.W, mask1 ? mask1 + b * kCMid * d.P1 : nullptr, d, t, s, sm, tid);
-    for (int i = tid; i < t.nf; i += kLongThreads) {
+    for (int i = tid; i < t.nf; i += kThreads) {
         float m = sm[s.c2 + d.PS * i];
         for (int j = 1; j < d.PK; ++j) m = max_nan(m, sm[s.c2 + d.PS * i + j]);
         f[b * d.L + t.i0 + i] = tanhf(m) * (mask2 ? mask2[b * d.L + t.i0 + i] : 1.0f);
@@ -744,7 +531,7 @@ __global__ void train_sum_chunks(const float *__restrict__ part, int n_chunks, i
 // dW_ih_l0 partial[chunk][g][p] = sum over the chunk's windows t (ascending) of da0[t][g] f[t][p].  Thread = position p
 // with the 64 gate rows' sums in registers, so f is read once; grid (position tiles of 128, batch chunks).
 __global__ void __launch_bounds__(128)
-train_wih0_grad_tiled(const float *__restrict__ da0, const float *__restrict__ f, int64_t B, int L, int chunk, float *__restrict__ part) {
+train_wih0_grad(const float *__restrict__ da0, const float *__restrict__ f, int64_t B, int L, int chunk, float *__restrict__ part) {
     __shared__ __align__(16) float sda[kRowBatch * kGates];
     const int p = blockIdx.x * 128 + threadIdx.x;
     const int64_t t0 = (int64_t)blockIdx.y * chunk, t1 = min(B, t0 + chunk);
@@ -772,10 +559,10 @@ train_wih0_grad_tiled(const float *__restrict__ da0, const float *__restrict__ f
         for (int g = 0; g < kGates; ++g) part[((int64_t)blockIdx.y * kGates + g) * L + p] = acc[g];
 }
 
-// d f[t][p] = sum_g da0[t][g] W_ih_l0[g][p] in train_dfeat's order; thread = position p with its 64 weights in
-// registers, grid (position tiles of 128, groups of kRowBatch windows)
+// d f[t][p] = sum_g da0[t][g] W_ih_l0[g][p], g ascending; thread = position p with its 64 weights in registers, grid
+// (position tiles of 128, groups of kRowBatch windows)
 __global__ void __launch_bounds__(128)
-train_dfeat_tiled(const float *__restrict__ da0, const float *__restrict__ wih0, int64_t B, int L, float *__restrict__ dfeat) {
+train_dfeat(const float *__restrict__ da0, const float *__restrict__ wih0, int64_t B, int L, float *__restrict__ dfeat) {
     __shared__ __align__(16) float sda[kRowBatch * kGates];
     const int p = blockIdx.x * 128 + threadIdx.x;
     const int64_t t0 = (int64_t)blockIdx.y * kRowBatch;
@@ -797,8 +584,11 @@ train_dfeat_tiled(const float *__restrict__ da0, const float *__restrict__ wih0,
     }
 }
 
-// pool_argmax over every `stride`-th float (c1 is kept position-major in a tile)
-__device__ __forceinline__ int pool_argmax_strided(const float *v, int stride, int start, int pk) {
+// first maximum of a pooling window over every `stride`-th float (c1 is kept position-major in a tile), like ATen's
+// max_pool1d ((v > m) || isnan(v) replaces).  This is the first maximum of the pre-activation; the reference pools after
+// tanh and takes the first maximum there.  The two differ only where tanhf maps distinct pre-activations to one float:
+// this choice is the one exact arithmetic makes.
+__device__ __forceinline__ int pool_argmax(const float *v, int stride, int start, int pk) {
     int best = start;
     float m = v[start * stride];
     for (int j = 1; j < pk; ++j) {
@@ -813,37 +603,38 @@ __device__ __forceinline__ float warp_sum(float v) {
     return v;
 }
 
-// The conv backward of one tile for kLongWin consecutive windows; grid: groups x tiles CTAs, group-major.  Per window:
-// conv_tile() again (same masks, so the pool arg-max is the forward's), then train_conv_bwd's steps on the tile's own
-// features in shared memory.  A warp owns each weight's partial sum (lanes stride the positions, one shuffle tree) and
-// adds it to the CTA's running sum in window order; the CTA writes one row of part[groups x tiles][n_conv].
+// The conv backward of one tile for `win` consecutive windows; grid: groups x tiles CTAs, group-major.  Per window:
+// conv_tile() again (same masks, so the pool arg-max is the forward's), then dropout 2 / pool 2 / tanh / conv2 / pool 1 /
+// tanh / conv1 backward over the tile's own features in shared memory.  A warp owns each weight's partial sum (lanes
+// stride the positions, one shuffle tree) and adds it to the CTA's running sum in window order; the CTA writes one row
+// of part[groups x tiles][n_conv].
 // dx != NULL: d x of the tile's span is added into the zeroed dx; adjacent spans overlap by less than a tile's stride
 // (checked by the host), so a sample has at most two contributions and their sum does not depend on the order.
-__global__ void __launch_bounds__(kLongThreads)
-train_conv_bwd_tiled(const float *__restrict__ x, const float *__restrict__ prm, BlobOff o, TrainDims d, int tiles, int64_t B,
-                     const float *__restrict__ mask1, const float *__restrict__ mask2, const float *__restrict__ dfeat,
-                     float *__restrict__ part, float *__restrict__ dx) {
+__global__ void __launch_bounds__(kThreads)
+train_conv_bwd(const float *__restrict__ x, const float *__restrict__ prm, BlobOff o, TrainDims d, int tiles, int win, int64_t B,
+               const float *__restrict__ mask1, const float *__restrict__ mask2, const float *__restrict__ dfeat,
+               float *__restrict__ part, float *__restrict__ dx) {
     extern __shared__ __align__(16) float sm[];
     const TileSmem s = tile_smem(d, true);
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    constexpr int kWarps = kLongThreads / 32;
+    constexpr int kWarps = kThreads / 32;
     const Tile t = tile_of(d, blockIdx.x % tiles);
-    const int64_t b0 = (int64_t)(blockIdx.x / tiles) * kLongWin, b1 = min(B, b0 + kLongWin);
+    const int64_t b0 = (int64_t)(blockIdx.x / tiles) * win, b1 = min(B, b0 + win);
     const int ck = d.C * d.K1, n_conv = kCMid * ck + kCMid + kCMid * d.K2 + 1;
     tile_stage_weights(prm, o, d, s, sm, tid);
-    for (int e = tid; e < n_conv; e += kLongThreads) sm[s.g + e] = 0.f;
+    for (int e = tid; e < n_conv; e += kThreads) sm[s.g + e] = 0.f;
     for (int64_t b = b0; b < b1; ++b) {
         const float *m1b = mask1 ? mask1 + b * kCMid * d.P1 : nullptr;
         __syncthreads();                                       // the previous window's readers are done
-        for (int i = tid; i < t.nf; i += kLongThreads) sm[s.df + i] = dfeat[b * d.L + t.i0 + i] * (mask2 ? mask2[b * d.L + t.i0 + i] : 1.0f);
+        for (int i = tid; i < t.nf; i += kThreads) sm[s.df + i] = dfeat[b * d.L + t.i0 + i] * (mask2 ? mask2[b * d.L + t.i0 + i] : 1.0f);
         conv_tile(x + b * d.C * d.W, m1b, d, t, s, sm, tid);
         // ---- dropout 2 + pool 2 + tanh, gather form over the tile's own features
-        for (int j = tid; j < t.n2; j += kLongThreads) {
+        for (int j = tid; j < t.n2; j += kThreads) {
             float a = 0.f;
             int i_lo = (j - d.PK + d.PS) / d.PS;
             if (j - d.PK + 1 <= 0) i_lo = 0;
             for (int i = i_lo; i <= j / d.PS && i < t.nf; ++i)
-                if (pool_argmax(sm + s.c2, d.PS * i, d.PK) == j) a += sm[s.df + i];
+                if (pool_argmax(sm + s.c2, 1, d.PS * i, d.PK) == j) a += sm[s.df + i];
             sm[s.dc2 + j] = a * dtanhf_(sm[s.c2 + j]);
         }
         __syncthreads();
@@ -859,7 +650,7 @@ train_conv_bwd_tiled(const float *__restrict__ x, const float *__restrict__ prm,
             a = warp_sum(a);
             if (lane == 0) sm[s.g + (e < kCMid * d.K2 ? o.w2 + e : o.b2)] += a;
         }
-        for (int e = tid; e < kCMid * t.np1; e += kLongThreads) {
+        for (int e = tid; e < kCMid * t.np1; e += kThreads) {
             const int oc = e / t.np1, u = e % t.np1;
             float a = 0.f;
             for (int k = 0; k < d.K2; ++k) {
@@ -870,14 +661,14 @@ train_conv_bwd_tiled(const float *__restrict__ x, const float *__restrict__ prm,
         }
         __syncthreads();
         // ---- pool 1 + tanh
-        for (int e = tid; e < kCMid * t.n1; e += kLongThreads) {
+        for (int e = tid; e < kCMid * t.n1; e += kThreads) {
             const int j = e >> 2, oc = e & 3;
             const float *col = sm + s.c1 + oc;
             float a = 0.f;
             int i_lo = (j - d.PK + d.PS) / d.PS;
             if (j - d.PK + 1 <= 0) i_lo = 0;
             for (int i = i_lo; i <= j / d.PS && i < t.np1; ++i)
-                if (pool_argmax_strided(col, kCMid, d.PS * i, d.PK) == j) a += sm[s.dd1 + oc * s.pp + i];
+                if (pool_argmax(col, kCMid, d.PS * i, d.PK) == j) a += sm[s.dd1 + oc * s.pp + i];
             sm[s.dc1 + e] = a * dtanhf_(sm[s.c1 + e]);
         }
         __syncthreads();
@@ -904,7 +695,7 @@ train_conv_bwd_tiled(const float *__restrict__ x, const float *__restrict__ prm,
             }
         }
         if (dx) {
-            for (int e = tid; e < d.C * t.nx; e += kLongThreads) {
+            for (int e = tid; e < d.C * t.nx; e += kThreads) {
                 const int c = e / t.nx, u = e % t.nx;
                 const int k_lo = max(0, u - (t.n1 - 1)), k_hi = min(d.K1 - 1, u);
                 float a = 0.f;
@@ -915,7 +706,7 @@ train_conv_bwd_tiled(const float *__restrict__ x, const float *__restrict__ prm,
         }
     }
     __syncthreads();
-    for (int e = tid; e < n_conv; e += kLongThreads) part[(int64_t)blockIdx.x * n_conv + e] = sm[s.g + e];
+    for (int e = tid; e < n_conv; e += kThreads) part[(int64_t)blockIdx.x * n_conv + e] = sm[s.g + e];
 }
 
 // grad[e] = the sum of part[.][e] over all rows in a fixed order: one CTA per conv parameter, thread i adds rows
@@ -983,61 +774,48 @@ struct DeviceScope {
     }
 };
 
-// what the tiled kernels need beyond a valid geometry; no CUDA call
-static bool tiled_args_ok(const TrainDims &d, const TrainPlan &pl, int64_t B, const char **err) {
+// what the kernels need beyond a valid geometry; no CUDA call
+static bool plan_fits(const TrainDims &d, const TrainPlan &pl, int64_t B, const char **err) {
     if (pl.smem_bwd > 227 * 1024) { *err = "training: too many input channels for a conv tile's shared memory"; return false; }
     // a tile's x span against the tiles' stride: d x relies on at most two tiles touching a sample
-    const int np1 = d.PS * (kLongT - 1) + d.PK + d.K2 - 1, span = d.PS * (np1 - 1) + d.PK + d.K1 - 1, stride = d.PS * d.PS * kLongT;
-    if (span > 2 * stride) { *err = "training: receptive field longer than a conv tile"; return false; }
+    const int np1 = d.PS * (kT - 1) + d.PK + d.K2 - 1, span = d.PS * (np1 - 1) + d.PK + d.K1 - 1, stride = d.PS * d.PS * kT;
+    if (pl.tiles > 1 && span > 2 * stride) { *err = "training: receptive field longer than a conv tile"; return false; }
     if ((int64_t)pl.tiles * B > INT32_MAX) { *err = "training: batch too large"; return false; }
     return true;
 }
 
-// conv forward into ws.f and, on the tiled plan, the layer-0 pre-activations; returns what train_lstm_fwd takes as pre0
-static const float *launch_conv_forward(const TrainDims &d, const BlobOff &o, const TrainPlan &pl, float *ws, const float *params,
-                                        const float *x, int64_t B, const float *mask1, const float *mask2, cudaStream_t st) {
+// conv forward into ws.f and the layer-0 pre-activations into ws.pre0 (one slice is the whole sum: no reduction)
+static void launch_conv_forward(const TrainDims &d, const BlobOff &o, const TrainPlan &pl, float *ws, const float *params,
+                                const float *x, int64_t B, const float *mask1, const float *mask2, cudaStream_t st) {
     const TrainWs &w = pl.w;
-    if (!pl.tiled) {
-        train_conv_fwd<<<(unsigned)B, 256, 0, st>>>(x, params, o, d, mask1, mask2, ws + w.c1, ws + w.p1, ws + w.c2, ws + w.f);
-        return nullptr;
+    if (pl.smem_fwd > 48 * 1024) cudaFuncSetAttribute(train_conv_fwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.smem_fwd);
+    train_conv_fwd<<<(unsigned)(B * pl.tiles), kThreads, pl.smem_fwd, st>>>(x, params, o, d, pl.tiles, mask1, mask2, ws + w.f);
+    train_pre0_partial<<<dim3((unsigned)((B + 63) / 64), (unsigned)pl.slices), 256, 0, st>>>(ws + w.f, params + o.wih0, B, d.L,
+                                                                                            ws + (pl.slices > 1 ? w.part : w.pre0));
+    if (pl.slices > 1) {
+        const int64_t n = B * kGates;
+        train_sum_chunks<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(ws + w.part, pl.slices, n, ws + w.pre0);
     }
-    if (pl.smem_fwd > 48 * 1024) cudaFuncSetAttribute(train_conv_fwd_tiled, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.smem_fwd);
-    train_conv_fwd_tiled<<<(unsigned)(B * pl.tiles), kLongThreads, pl.smem_fwd, st>>>(x, params, o, d, pl.tiles, mask1, mask2, ws + w.f);
-    train_pre0_partial<<<dim3((unsigned)((B + 63) / 64), (unsigned)pl.slices), 256, 0, st>>>(ws + w.f, params + o.wih0, B, d.L, ws + w.part);
-    const int64_t n = B * kGates;
-    train_sum_chunks<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(ws + w.part, pl.slices, n, ws + w.pre0);
-    return ws + w.pre0;
 }
 
 // everything after d(head): d W_ih_l0 and, unless the front end is frozen, d f, the convolutional backward into `grads`
-// (zeroed by the caller: the one-CTA-per-window kernel adds its conv weight gradients atomically) and, when dx != NULL,
-// the input gradient
+// and, when dx != NULL, the input gradient (added into dx, zeroed here)
 static bool launch_backward_tail(const TrainDims &d, const BlobOff &o, const TrainPlan &pl, float *ws, const float *params,
                                  const float *x, int64_t B, const float *mask1, const float *mask2, float *grads, float *dx,
                                  bool frozen_conv, cudaStream_t st) {
     const TrainWs &w = pl.w;
-    const int64_t n1 = (int64_t)kGates * d.L, n2 = B * d.L;
-    if (!pl.tiled) {
-        train_wih0_grad<<<(unsigned)((n1 + 255) / 256), 256, 0, st>>>(ws + w.da0, ws + w.f, B, d.L, grads + o.wih0);
-        if (frozen_conv) return true;
-        train_dfeat<<<(unsigned)((n2 + 255) / 256), 256, 0, st>>>(ws + w.da0, params + o.wih0, B, d.L, ws + w.dfeat);
-        train_conv_bwd<<<(unsigned)B, 256, 0, st>>>(x, params, o, d, mask1, mask2, ws + w.c1, ws + w.p1, ws + w.c2, ws + w.dfeat, ws + w.dc2,
-                                                   ws + w.dd1, ws + w.dc1, grads);
-        if (dx) {
-            const int64_t n = B * d.C * d.W;
-            train_dx<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(ws + w.dc1, params, o, d, B, dx);
-        }
-        return true;
-    }
+    const int64_t n1 = (int64_t)kGates * d.L;
     const unsigned ptiles = (unsigned)((d.L + 127) / 128);
-    train_wih0_grad_tiled<<<dim3(ptiles, (unsigned)pl.wih_chunks), 128, 0, st>>>(ws + w.da0, ws + w.f, B, d.L, pl.wih_chunk, ws + w.part);
-    train_sum_chunks<<<(unsigned)((n1 + 255) / 256), 256, 0, st>>>(ws + w.part, pl.wih_chunks, n1, grads + o.wih0);
+    train_wih0_grad<<<dim3(ptiles, (unsigned)pl.wih_chunks), 128, 0, st>>>(ws + w.da0, ws + w.f, B, d.L, pl.wih_chunk,
+                                                                           pl.wih_chunks > 1 ? ws + w.part : grads + o.wih0);
+    if (pl.wih_chunks > 1)
+        train_sum_chunks<<<(unsigned)((n1 + 255) / 256), 256, 0, st>>>(ws + w.part, pl.wih_chunks, n1, grads + o.wih0);
     if (frozen_conv) return true;
-    train_dfeat_tiled<<<dim3(ptiles, (unsigned)((B + kRowBatch - 1) / kRowBatch)), 128, 0, st>>>(ws + w.da0, params + o.wih0, B, d.L, ws + w.dfeat);
+    train_dfeat<<<dim3(ptiles, (unsigned)((B + kRowBatch - 1) / kRowBatch)), 128, 0, st>>>(ws + w.da0, params + o.wih0, B, d.L, ws + w.dfeat);
     if (dx && cudaMemsetAsync(dx, 0, sizeof(float) * B * d.C * d.W, st) != cudaSuccess) return false;
-    if (pl.smem_bwd > 48 * 1024) cudaFuncSetAttribute(train_conv_bwd_tiled, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.smem_bwd);
-    train_conv_bwd_tiled<<<(unsigned)pl.part_rows, kLongThreads, pl.smem_bwd, st>>>(x, params, o, d, pl.tiles, B, mask1, mask2, ws + w.dfeat,
-                                                                                   ws + w.part, dx);
+    if (pl.smem_bwd > 48 * 1024) cudaFuncSetAttribute(train_conv_bwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.smem_bwd);
+    train_conv_bwd<<<(unsigned)pl.part_rows, kThreads, pl.smem_bwd, st>>>(x, params, o, d, pl.tiles, pl.win, B, mask1, mask2, ws + w.dfeat,
+                                                                          ws + w.part, dx);
     train_conv_grad_reduce<<<(unsigned)pl.n_conv, 256, 0, st>>>(ws + w.part, pl.part_rows, pl.n_conv, grads);
     return true;
 }
@@ -1053,19 +831,19 @@ int train_step(const b2cnn_config *cfg, float *params, float *adam_m, float *ada
     if (weighted && !(pos_weight > 0.f && pos_weight <= FLT_MAX)) { *err = "training: pos_weight must be positive and finite"; return B2CNN_EINVAL; }
     const TrainPlan pl = train_plan(d, B);
     const TrainWs &w = pl.w;
-    if (pl.tiled && !tiled_args_ok(d, pl, B, err)) return B2CNN_EINVAL;
+    if (!plan_fits(d, pl, B, err)) return B2CNN_EINVAL;
     if (ws_bytes < w.total * (int64_t)sizeof(float)) { *err = "training: workspace smaller than b2cnn_train_workspace_bytes()"; return B2CNN_ESTATE; }
     const BlobOff o = blob_offsets(d);
     float *ws = reinterpret_cast<float *>(workspace);
     if (cudaMemsetAsync(grads, 0, sizeof(float) * o.total, st) != cudaSuccess) { *err = "memset grads"; return B2CNN_ECUDA; }
-    const float *pre0 = launch_conv_forward(d, o, pl, ws, params, x, B, mask1, mask2, st);
+    launch_conv_forward(d, o, pl, ws, params, x, B, mask1, mask2, st);
     if (weighted) {
-        train_lstm_fwd<kHeadBcePw><<<1, 64, 0, st>>>(ws + w.f, pre0, params, o, d, B, sequence, age, target, pos_weight, ws + w.acts, ws + w.cs,
+        train_lstm_fwd<kHeadBcePw><<<1, 64, 0, st>>>(ws + w.pre0, params, o, d, B, sequence, age, target, pos_weight, ws + w.acts, ws + w.cs,
                                                      ws + w.hs, ws + w.lin, ws + w.z, loss_out);
         train_lstm_bwd<kHeadBcePw><<<1, 64, 0, st>>>(params, o, d, B, sequence, age, target, pos_weight, nullptr, ws + w.acts, ws + w.cs,
                                                      ws + w.hs, ws + w.lin, ws + w.z, ws + w.da0, grads, nullptr);
     } else {
-        train_lstm_fwd<kHeadBce><<<1, 64, 0, st>>>(ws + w.f, pre0, params, o, d, B, sequence, age, target, 1.f, ws + w.acts, ws + w.cs,
+        train_lstm_fwd<kHeadBce><<<1, 64, 0, st>>>(ws + w.pre0, params, o, d, B, sequence, age, target, 1.f, ws + w.acts, ws + w.cs,
                                                    ws + w.hs, ws + w.lin, ws + w.z, loss_out);
         train_lstm_bwd<kHeadBce><<<1, 64, 0, st>>>(params, o, d, B, sequence, age, target, 1.f, nullptr, ws + w.acts, ws + w.cs,
                                                    ws + w.hs, ws + w.lin, ws + w.z, ws + w.da0, grads, nullptr);
@@ -1087,7 +865,7 @@ static int autograd_args(const b2cnn_config *cfg, int64_t B, int mode, int64_t w
     if (mode != B2CNN_MODE_INDEPENDENT && mode != B2CNN_MODE_SEQUENCE) { *err = "training: bad mode"; return B2CNN_EINVAL; }
     if (!ptrs_ok || B < 1) { *err = "training: null argument / bad batch"; return B2CNN_EINVAL; }
     pl = train_plan(d, B);
-    if (pl.tiled && !tiled_args_ok(d, pl, B, err)) return B2CNN_EINVAL;
+    if (!plan_fits(d, pl, B, err)) return B2CNN_EINVAL;
     if (ws_bytes < pl.w.total * (int64_t)sizeof(float)) { *err = "training: workspace smaller than b2cnn_train_workspace_bytes()"; return B2CNN_ESTATE; }
     return B2CNN_OK;
 }
@@ -1104,8 +882,8 @@ int train_forward(const b2cnn_config *cfg, const float *params, const float *x, 
     const BlobOff o = blob_offsets(d);
     const int sequence = mode == B2CNN_MODE_SEQUENCE ? 1 : 0;
     float *ws = reinterpret_cast<float *>(workspace);
-    const float *pre0 = launch_conv_forward(d, o, pl, ws, params, x, B, mask1, mask2, st);
-    train_lstm_fwd<kHeadLogits><<<1, 64, 0, st>>>(ws + w.f, pre0, params, o, d, B, sequence, age, nullptr, 1.f, ws + w.acts, ws + w.cs,
+    launch_conv_forward(d, o, pl, ws, params, x, B, mask1, mask2, st);
+    train_lstm_fwd<kHeadLogits><<<1, 64, 0, st>>>(ws + w.pre0, params, o, d, B, sequence, age, nullptr, 1.f, ws + w.acts, ws + w.cs,
                                                   ws + w.hs, ws + w.lin, z_out, nullptr);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) { *err = cudaGetErrorString(e); return B2CNN_ECUDA; }
@@ -1128,6 +906,7 @@ int train_backward(const b2cnn_config *cfg, const float *params, const float *x,
     const BlobOff o = blob_offsets(d);
     const int sequence = mode == B2CNN_MODE_SEQUENCE ? 1 : 0;
     float *ws = reinterpret_cast<float *>(workspace);
+    // zeroed: a frozen front end leaves the conv entries as they are
     if (cudaMemsetAsync(grads, 0, sizeof(float) * o.total, st) != cudaSuccess) { *err = "memset grads"; return B2CNN_ECUDA; }
     train_lstm_bwd<kHeadLogits><<<1, 64, 0, st>>>(params, o, d, B, sequence, age, nullptr, 1.f, dz, ws + w.acts, ws + w.cs, ws + w.hs,
                                                   ws + w.lin, nullptr, ws + w.da0, grads, dage);
