@@ -474,7 +474,8 @@ const char *b2cnn_version(void);
  *   mask1 [B][4][P1], mask2 [B][L_out]: the two nn.Dropout(0.1) masks of bin/models.py:25,28 ALREADY scaled by 1/(1-p)
  *                   (torch's Philox stream cannot be reproduced here, so the caller draws them); NULL = no dropout
  *   loss_out        one float: the mean BCE-with-logits loss of this batch (before the update)
- * The call allocates nothing and is asynchronous on `stream`.
+ * The call allocates nothing and is asynchronous on `stream`.  Like every training call it checks all its arguments
+ * before any CUDA call, then runs on cfg->device (the current device for -1) and restores the caller's device.
  * workspace: b2cnn_train_workspace_bytes(cfg, B) bytes; a smaller one is B2CNN_ESTATE before any launch.  The conv
  * layers run on position tiles of 128 window features that recompute the conv backward in shared memory, so the
  * workspace holds f, d f, the LSTM records and one region of partial sums (about 2 * 4 * B * L_out bytes plus the

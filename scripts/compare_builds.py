@@ -14,7 +14,8 @@ inputs, with seed-0 MyCNN5 weights:
   * predict_record() on the tensor-core and generic paths, independent and sequence modes;
   * training: one B200Trainer.step (sequence, dropout masks given) at [2048, 10, 120] and at [256, 3, 75000], with the
     loss, the gradients and the updated parameters; and one autograd forward and backward at [257, 10, 120] with the
-    logits, every parameter gradient, d x and d age;
+    logits, every parameter gradient, d x and d age; and the dropout masks B200Trainer(seed=0).draw_masks(64) and
+    B200TrainableMyCNN.draw_masks(64) after torch.manual_seed(0);
 then compares every array bit for bit and prints each array's status and max |diff|.
 
     python scripts/compare_builds.py --baseline-lib /path/to/parent/libb2cnn.so [--lib /path/to/libb2cnn.so]
@@ -146,6 +147,11 @@ def dump(path: str, batch: int, feat_batch: int, patients: int) -> None:
     out[tag + "_z"] = z.detach()
     out.update({f"{tag}_grad_{k}": p.grad for k, p in zip(BLOB_KEYS, params)})
     out[tag + "_dx"], out[tag + "_dage"] = xt.grad, at.grad
+    # dropout masks: the trainer's seeded generator, and torch's default generator under autograd
+    dm = tskd_b200.B200TrainableMyCNN(tskd_b200.ARCH_PRESETS["mycnn5"]).to(dev)
+    out["masks_trainer_mask1"], out["masks_trainer_mask2"] = B200Trainer(dm, seed=0).draw_masks(64)
+    torch.manual_seed(0)
+    out["masks_autograd_mask1"], out["masks_autograd_mask2"] = dm.draw_masks(64)
     torch.cuda.synchronize()
     np.savez(path, **{k: (v.cpu().numpy() if hasattr(v, "cpu") else v) for k, v in out.items()})
 

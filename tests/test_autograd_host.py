@@ -56,6 +56,20 @@ def test_weighted_step_rejects_bad_arguments_before_cuda():
     assert step(ws=need - 1) == capi.ESTATE and "workspace" in capi.last_error()
 
 
+def test_training_calls_check_arguments_before_the_device():
+    """cfg->device is made current only once every other argument has passed: a device that does not exist is not
+    what a bad argument reports"""
+    lib = capi.load_library()
+    cfg = capi.make_config(tskd_b200.ARCH_PRESETS["mycnn5"], device=1000)
+    opt = capi.Adam(1e-5, 0.9, 0.999, 1e-8)
+    p = ctypes.c_void_p(1)
+    assert _fwd(lib, ctypes.byref(cfg), mode=7) == capi.EINVAL and "mode" in capi.last_error()
+    assert _bwd(lib, ctypes.byref(cfg), ptr=0) == capi.EINVAL and "null" in capi.last_error()
+    rc = lib.b2cnn_train_step_weighted(ctypes.byref(cfg), p, p, p, p, 1, ctypes.byref(opt), 1, p, 4, p, p, 0.0, capi.MODE_SEQUENCE,
+                                       None, None, p, p, 1 << 30, None)
+    assert rc == capi.EINVAL and "pos_weight" in capi.last_error()
+
+
 def test_trainable_model_contract_without_a_gpu():
     plain = tskd_b200.B200MyCNN(tskd_b200.ARCH_PRESETS["mycnn5"])
     m = tskd_b200.B200TrainableMyCNN(tskd_b200.ARCH_PRESETS["mycnn5"])

@@ -53,6 +53,11 @@ class ArchConfig:
         return (self.l2 - self.pool_k) // self.pool_s + 1
 
     @property
+    def receptive_field(self) -> int:
+        """Samples one feature reads; features start pool_s ** 2 samples apart, so l_out = (window - R) // pool_s ** 2 + 1."""
+        return self.pool_s * (self.pool_k + self.k2 - 2) + self.pool_k + self.k1 - 1
+
+    @property
     def act_id(self) -> int:
         return _ACT_NAMES[self.act]
 

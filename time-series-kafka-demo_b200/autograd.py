@@ -38,6 +38,37 @@ def _ptr(t: Optional[torch.Tensor]):
     return ctypes.c_void_p(t.data_ptr()) if t is not None else None
 
 
+def check_trainable(arch: ArchConfig) -> None:
+    """The training kernels cover the reference's tanh layer stack without the affine variant."""
+    if arch.affine or arch.act_id != 0:
+        raise NotImplementedError("training covers the reference's tanh stack (bin/models.py:23,26) without the affine variant")
+
+
+def draw_masks(arch: ArchConfig, B: int, p: float, device, generator: Optional[torch.Generator] = None):
+    """The two nn.Dropout masks of bin/models.py:25,28 for B windows, scaled by 1/(1-p) like torch's dropout; (None, None)
+    for p = 0.  Drawn from ``generator``, or from torch's default generator of the device when None."""
+    if not 0.0 <= p < 1.0:
+        raise ValueError("dropout p must be in [0, 1)")
+    if p == 0.0:
+        return None, None
+    keep = 1.0 - p
+    m1 = torch.bernoulli(torch.full((B, arch.c_mid, arch.p1), keep, device=device), generator=generator).div_(keep)
+    m2 = torch.bernoulli(torch.full((B, arch.l_out), keep, device=device), generator=generator).div_(keep)
+    return m1, m2
+
+
+def check_masks(arch: ArchConfig, B: int, device, mask1: Optional[torch.Tensor], mask2: Optional[torch.Tensor]):
+    """The two dropout masks as contiguous fp32 tensors on ``device``: each None or of shape [B, c_mid, P1] / [B, L_out]."""
+    out = []
+    for i, (m, shape) in enumerate(((mask1, (B, arch.c_mid, arch.p1)), (mask2, (B, arch.l_out))), 1):
+        if m is not None:
+            m = m.detach().to(device, torch.float32).contiguous()
+            if tuple(m.shape) != shape:
+                raise RuntimeError(f"dropout mask {i} must be {shape}, got {tuple(m.shape)}")
+        out.append(m)
+    return out
+
+
 class _TrainForward(torch.autograd.Function):
     """Inputs: a :class:`_Call` (non-tensor), x [B,C,W] fp32, age [B] fp32, then the 14 ``BLOB_KEYS`` tensors."""
 
@@ -106,8 +137,7 @@ def mycnn_train_forward(x: torch.Tensor, age: torch.Tensor, params: Sequence[tor
     to fp32), ``age`` 1 or B values.  ``mode``: "sequence" (the LSTM scans the batch axis, as ``model(x, age)`` does in
     the reference) or "independent" (every window from the zero state).  ``mask1`` [B, c_mid, P1] / ``mask2``
     [B, L_out]: the two dropout masks, already scaled by 1/(1-p); None = no dropout."""
-    if arch.affine or arch.act_id != 0:
-        raise NotImplementedError("training covers the reference's tanh stack (bin/models.py:23,26) without the affine variant")
+    check_trainable(arch)
     if mode not in _MODES:
         raise ValueError("mode must be 'sequence' or 'independent'")
     if len(params) != len(BLOB_KEYS):
@@ -133,15 +163,7 @@ def mycnn_train_forward(x: torch.Tensor, age: torch.Tensor, params: Sequence[tor
     if age.numel() != B:
         raise RuntimeError(f"age must have 1 or {B} elements, got {age.numel()}")
     age = age.contiguous()
-    p1 = arch.p1
-    masks = []
-    for m, shape in ((mask1, (B, arch.c_mid, p1)), (mask2, (B, arch.l_out))):
-        if m is not None:
-            m = m.detach().to(dev, torch.float32).contiguous()
-            if tuple(m.shape) != shape:
-                raise RuntimeError(f"dropout mask must be {shape}, got {tuple(m.shape)}")
-        masks.append(m)
-    call = _Call(arch, dev, _MODES[mode], *masks)
+    call = _Call(arch, dev, _MODES[mode], *check_masks(arch, B, dev, mask1, mask2))
     return _TrainForward.apply(call, x, age, *params)
 
 
@@ -160,8 +182,7 @@ class B200TrainableMyCNN(B200MyCNN):
     drawn on the device with ``p = self.dropout.p`` from torch's default CUDA generator."""
 
     def __init__(self, arch: ArchConfig = ArchConfig(), *a, **kw):
-        if arch.affine or arch.act_id != 0:
-            raise NotImplementedError("training covers the reference's tanh stack (bin/models.py:23,26) without the affine variant")
+        check_trainable(arch)
         super().__init__(arch, *a, **kw)
         self.requires_grad_(True)
 
@@ -169,16 +190,8 @@ class B200TrainableMyCNN(B200MyCNN):
         return nn.Module.train(self, mode)
 
     def draw_masks(self, B: int):
-        """The two nn.Dropout masks of bin/models.py:25,28, scaled by 1/(1-p) like torch's dropout; (None, None) for p = 0."""
-        p = float(self.dropout.p)
-        if not 0.0 <= p < 1.0:
-            raise ValueError("dropout.p must be in [0, 1)")
-        if p == 0.0:
-            return None, None
-        keep, dev, a = 1.0 - p, self._device(), self.arch
-        m1 = torch.bernoulli(torch.full((B, a.c_mid, a.p1), keep, device=dev)).div_(keep)
-        m2 = torch.bernoulli(torch.full((B, a.l_out), keep, device=dev)).div_(keep)
-        return m1, m2
+        """The two nn.Dropout masks of bin/models.py:25,28 with ``p = self.dropout.p``, from torch's default generator."""
+        return draw_masks(self.arch, B, float(self.dropout.p), self._device())
 
     def forward(self, x: torch.Tensor, age: torch.Tensor) -> torch.Tensor:
         """``model(x, age)`` (bin/models.py:22-36): differentiable in train mode, the inference path in eval mode."""

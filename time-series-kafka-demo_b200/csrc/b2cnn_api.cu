@@ -25,27 +25,17 @@ static int cuda_fail(cudaError_t e, const char *what) {
     g_err = std::string(what) + ": " + cudaGetErrorString(e);
     return B2CNN_ECUDA;
 }
+// rc, with the internal call's message under the entry point's name when rc is an error
+static int finish(const char *fn, int rc, const char *err) {
+    return rc == B2CNN_OK ? rc : fail(rc, std::string(fn) + ": " + err);
+}
 #define CU_TRY(expr)                                         \
     do {                                                     \
         cudaError_t e__ = (expr);                            \
         if (e__ != cudaSuccess) return cuda_fail(e__, #expr); \
     } while (0)
 
-// Every entry point that touches the handle's device switches to it for the duration of the call only and
-// restores the caller's current device on every exit path (a forward on cuda:1 must not leave the calling
-// thread on cuda:1 -- later `device="cuda"` allocations of the host framework would land on the wrong GPU).
-struct DeviceGuard {
-    int prev = -1;
-    cudaError_t err = cudaSuccess;
-    explicit DeviceGuard(int dev) {
-        err = cudaGetDevice(&prev);
-        if (err != cudaSuccess) { prev = -1; return; }
-        if (prev != dev) err = cudaSetDevice(dev); else prev = -1;     // nothing to restore
-    }
-    ~DeviceGuard() { if (prev >= 0) cudaSetDevice(prev); }
-    DeviceGuard(const DeviceGuard &) = delete;
-    DeviceGuard &operator=(const DeviceGuard &) = delete;
-};
+// Every entry point that touches the handle's device switches to it for the duration of the call only (DeviceGuard).
 #define DEVICE_GUARD(dev)                   \
     DeviceGuard guard__(dev);               \
     if (guard__.err != cudaSuccess) return cuda_fail(guard__.err, "cudaSetDevice")
@@ -84,19 +74,6 @@ struct b2cnn_handle {
 
 static int64_t align_up(int64_t v, int64_t a) { return (v + a - 1) / a * a; }
 
-static bool derive_dims(const b2cnn_config &c, Dims &d) {
-    d.C = c.in_channels; d.K1 = c.k1; d.K2 = c.k2; d.PK = c.pool_k; d.PS = c.pool_s; d.W = c.window;
-    d.act = c.act; d.has_affine = (c.flags & B2CNN_FLAG_AFFINE) ? 1 : 0; d.age_coef = c.age_coef; d.XP = c.window;
-    if (d.C < 1 || d.K1 < 1 || d.K2 < 1 || d.PK < 1 || d.PS < 1 || d.W < 1) return false;
-    d.L1 = d.W - d.K1 + 1;
-    if (d.L1 < d.PK) return false;
-    d.P1 = (d.L1 - d.PK) / d.PS + 1;
-    d.L2 = d.P1 - d.K2 + 1;
-    if (d.L2 < d.PK) return false;
-    d.L = (d.L2 - d.PK) / d.PS + 1;
-    return d.L >= 1;
-}
-
 extern "C" int64_t b2cnn_l_out(const b2cnn_config *cfg) {
     Dims d;
     if (!cfg || !derive_dims(*cfg, d)) return -1;
@@ -106,12 +83,7 @@ extern "C" int64_t b2cnn_l_out(const b2cnn_config *cfg) {
 extern "C" int64_t b2cnn_weight_count(const b2cnn_config *cfg) {
     Dims d;
     if (!cfg || !derive_dims(*cfg, d)) return -1;
-    int64_t n = (int64_t)kCMid * d.C * d.K1 + kCMid + kCMid * d.K2 + 1;
-    n += (int64_t)kGates * d.L + kGates * kHidden + 2 * kGates;   // layer 0
-    n += 2 * kGates * kHidden + 2 * kGates;                       // layer 1
-    n += kHidden + 1;                                             // out
-    if (d.has_affine) n += 2 * kCMid + 2;
-    return n;
+    return blob_offsets(d).total;
 }
 
 extern "C" const char *b2cnn_last_error(void) { return g_err.c_str(); }
@@ -127,17 +99,11 @@ static int train_step_api(const char *name, const b2cnn_config *cfg, float *para
                           const float *target, int weighted, float pos_weight, int mode, const float *mask1, const float *mask2,
                           float *loss_out, void *workspace, int64_t workspace_bytes, void *stream) {
     if (!cfg || !opt) return fail(B2CNN_EINVAL, std::string(name) + ": null configuration");
-    if (mode != B2CNN_MODE_INDEPENDENT && mode != B2CNN_MODE_SEQUENCE) return fail(B2CNN_EINVAL, std::string(name) + ": bad mode");
-    int prev = -1;
-    if (cfg->device >= 0) {
-        if (cudaGetDevice(&prev) != cudaSuccess || cudaSetDevice(cfg->device) != cudaSuccess) return fail(B2CNN_ECUDA, std::string(name) + ": cudaSetDevice");
-    }
     const char *err = "";
     const int rc = train_step(cfg, params, adam_m, adam_v, grads, step, opt->lr, opt->beta1, opt->beta2, opt->eps, apply_update, x, B, age,
-                              target, weighted, pos_weight, mode == B2CNN_MODE_SEQUENCE ? 1 : 0, mask1, mask2, loss_out, workspace,
-                              workspace_bytes, reinterpret_cast<cudaStream_t>(stream), &err);
-    if (prev >= 0) cudaSetDevice(prev);
-    return rc == B2CNN_OK ? rc : fail(rc, std::string(name) + ": " + err);
+                              target, weighted, pos_weight, mode, mask1, mask2, loss_out, workspace, workspace_bytes,
+                              reinterpret_cast<cudaStream_t>(stream), &err);
+    return finish(name, rc, err);
 }
 extern "C" int b2cnn_train_step(const b2cnn_config *cfg, float *params, float *adam_m, float *adam_v, float *grads, int64_t step,
                                 const b2cnn_adam *opt, int apply_update, const float *x, int64_t B, const float *age,
@@ -159,7 +125,7 @@ extern "C" int b2cnn_train_forward(const b2cnn_config *cfg, const float *params,
     const char *err = "";
     const int rc = train_forward(cfg, params, x, B, age, mode, mask1, mask2, z_out, workspace, workspace_bytes,
                                  reinterpret_cast<cudaStream_t>(stream), &err);
-    return rc == B2CNN_OK ? rc : fail(rc, std::string("b2cnn_train_forward: ") + err);
+    return finish("b2cnn_train_forward", rc, err);
 }
 extern "C" int b2cnn_train_backward_ex(const b2cnn_config *cfg, const float *params, const float *x, int64_t B, const float *age, int mode,
                                        const float *mask1, const float *mask2, const float *dz, float *grads, float *dx, float *dage,
@@ -167,7 +133,7 @@ extern "C" int b2cnn_train_backward_ex(const b2cnn_config *cfg, const float *par
     const char *err = "";
     const int rc = train_backward(cfg, params, x, B, age, mode, mask1, mask2, dz, grads, dx, dage, flags, workspace, workspace_bytes,
                                   reinterpret_cast<cudaStream_t>(stream), &err);
-    return rc == B2CNN_OK ? rc : fail(rc, std::string("b2cnn_train_backward: ") + err);
+    return finish("b2cnn_train_backward", rc, err);
 }
 extern "C" int b2cnn_train_backward(const b2cnn_config *cfg, const float *params, const float *x, int64_t B, const float *age, int mode,
                                     const float *mask1, const float *mask2, const float *dz, float *grads, float *dx, float *dage,
@@ -192,7 +158,7 @@ extern "C" int b2cnn_prep_windows(const int16_t *raw, int64_t n_samples, int32_t
     const char *err = "";
     const int rc = prep_windows(raw, n_samples, n_sig, sel, n_sel, gains, baselines, fs, cfg, x_out, dtype, t0_out, workspace,
                                 workspace_bytes, reinterpret_cast<cudaStream_t>(stream), &err);
-    return rc == B2CNN_OK ? rc : fail(rc, std::string("b2cnn_prep_windows: ") + err);
+    return finish("b2cnn_prep_windows", rc, err);
 }
 // ---- streaming form: per-patient device ring buffers (b2cnn_prep.cu) ----
 struct b2cnn_ring { Ring *r; int device; };
@@ -207,7 +173,7 @@ extern "C" int b2cnn_ring_create(const b2cnn_prep_config *cfg, int32_t n_patient
     const char *err = "";
     Ring *r = nullptr;
     const int rc = ring_create(cfg, n_patients, n_sig, fs, dev, &r, &err);
-    if (rc != B2CNN_OK) return fail(rc, std::string("b2cnn_ring_create: ") + err);
+    if (rc != B2CNN_OK) return finish("b2cnn_ring_create", rc, err);
     b2cnn_ring *h = new (std::nothrow) b2cnn_ring{r, dev};
     if (!h) { ring_destroy(r); return fail(B2CNN_ESTATE, "out of host memory"); }
     *out = h;
@@ -224,7 +190,7 @@ extern "C" int b2cnn_ring_reset(b2cnn_ring *h, void *stream) {
     DEVICE_GUARD(h->device);
     const char *err = "";
     const int rc = ring_reset(h->r, reinterpret_cast<cudaStream_t>(stream), &err);
-    return rc == B2CNN_OK ? rc : fail(rc, std::string("b2cnn_ring_reset: ") + err);
+    return finish("b2cnn_ring_reset", rc, err);
 }
 extern "C" int b2cnn_ring_set_signals(b2cnn_ring *h, int32_t patient, const int32_t *sel, int32_t n_sel, const double *gains,
                                       const double *baselines, void *stream) {
@@ -232,7 +198,7 @@ extern "C" int b2cnn_ring_set_signals(b2cnn_ring *h, int32_t patient, const int3
     DEVICE_GUARD(h->device);
     const char *err = "";
     const int rc = ring_set_signals(h->r, patient, sel, n_sel, gains, baselines, reinterpret_cast<cudaStream_t>(stream), &err);
-    return rc == B2CNN_OK ? rc : fail(rc, std::string("b2cnn_ring_set_signals: ") + err);
+    return finish("b2cnn_ring_set_signals", rc, err);
 }
 extern "C" int b2cnn_ring_push(b2cnn_ring *h, const void *new_samples, int sample_kind, int64_t n_new, void *x_out, int dtype,
                                int32_t *emitted, int64_t *window_index, double *t0_seconds, void *stream) {
@@ -244,7 +210,7 @@ extern "C" int b2cnn_ring_push(b2cnn_ring *h, const void *new_samples, int sampl
     int em = 0;
     const int rc = ring_push(h->r, new_samples, sample_kind, n_new, x_out, dtype, &em, window_index,
                              t0_seconds, reinterpret_cast<cudaStream_t>(stream), &err);
-    if (rc != B2CNN_OK) return fail(rc, std::string("b2cnn_ring_push: ") + err);
+    if (rc != B2CNN_OK) return finish("b2cnn_ring_push", rc, err);
     if (emitted) *emitted = em;
     return B2CNN_OK;
 }
@@ -256,14 +222,14 @@ extern "C" int b2cnn_decode_sample_messages(const void *bytes, const int64_t *of
     const char *err = "";
     const int rc = wire_decode_pairs(reinterpret_cast<const uint8_t *>(bytes), offsets, n_msgs, idx_out, val_out, row_of_msg, frame,
                                      frame_rows, n_sig, n_bad, reinterpret_cast<cudaStream_t>(stream), &err);
-    return rc == B2CNN_OK ? rc : fail(rc, std::string("b2cnn_decode_sample_messages: ") + err);
+    return finish("b2cnn_decode_sample_messages", rc, err);
 }
 extern "C" int b2cnn_decode_array_messages(const void *bytes, const int64_t *offsets, int64_t n_msgs, int32_t max_vals, double *vals_out,
                                            int32_t *counts_out, int32_t *n_bad, void *stream) {
     const char *err = "";
     const int rc = wire_decode_arrays(reinterpret_cast<const uint8_t *>(bytes), offsets, n_msgs, max_vals, vals_out, counts_out, n_bad,
                                       reinterpret_cast<cudaStream_t>(stream), &err);
-    return rc == B2CNN_OK ? rc : fail(rc, std::string("b2cnn_decode_array_messages: ") + err);
+    return finish("b2cnn_decode_array_messages", rc, err);
 }
 extern "C" int b2cnn_frame_check(const void *frame, int64_t bytes, b2cnn_frame_header *header_out, int64_t *ids_offset,
                                  int64_t *samples_offset) {
@@ -362,20 +328,19 @@ extern "C" int b2cnn_set_weights(b2cnn_handle *h, const float *blob, int64_t n, 
     ++h->weight_gen;
     CU_TRY(cudaMemcpyAsync(h->d_blob, blob, sizeof(float) * n, on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, st));
     // conv weights + affine -> host copy for the kernel-parameter constant bank
-    const int64_t n_conv = (int64_t)kCMid * d.C * d.K1 + kCMid + kCMid * d.K2 + 1;
-    std::vector<float> conv(n_conv), aff(2 * kCMid + 2, 0.f);
-    const int64_t aff_off = n - (2 * kCMid + 2);
+    const BlobOff off = blob_offsets(d);
+    std::vector<float> conv(off.wih0), aff(2 * kCMid + 2, 0.f);
     if (on_device) {
-        CU_TRY(cudaMemcpyAsync(conv.data(), blob, sizeof(float) * n_conv, cudaMemcpyDeviceToHost, st));
-        if (d.has_affine) CU_TRY(cudaMemcpyAsync(aff.data(), blob + aff_off, sizeof(float) * aff.size(), cudaMemcpyDeviceToHost, st));
+        CU_TRY(cudaMemcpyAsync(conv.data(), blob, sizeof(float) * conv.size(), cudaMemcpyDeviceToHost, st));
+        if (d.has_affine) CU_TRY(cudaMemcpyAsync(aff.data(), blob + off.affine, sizeof(float) * aff.size(), cudaMemcpyDeviceToHost, st));
         CU_TRY(cudaStreamSynchronize(st));
     } else {
-        memcpy(conv.data(), blob, sizeof(float) * n_conv);
-        if (d.has_affine) memcpy(aff.data(), blob + aff_off, sizeof(float) * aff.size());
+        memcpy(conv.data(), blob, sizeof(float) * conv.size());
+        if (d.has_affine) memcpy(aff.data(), blob + off.affine, sizeof(float) * aff.size());
     }
     ConvWeights &cw = h->cw;
     memset(&cw, 0, sizeof cw);
-    const float *w1 = conv.data(), *b1 = w1 + (int64_t)kCMid * d.C * d.K1, *w2 = b1 + kCMid, *b2 = w2 + kCMid * d.K2;
+    const float *w1 = conv.data() + off.w1, *b1 = conv.data() + off.b1, *w2 = conv.data() + off.w2, *b2 = conv.data() + off.b2;
     for (int o = 0; o < kCMid; ++o)
         for (int c = 0; c < d.C; ++c)
             for (int k = 0; k < d.K1; ++k) cw.w1[(c * d.K1 + k) * kCMid + o] = w1[((int64_t)o * d.C + c) * d.K1 + k];
@@ -386,18 +351,9 @@ extern "C" int b2cnn_set_weights(b2cnn_handle *h, const float *blob, int64_t n, 
     cw.s2 = d.has_affine ? aff[2 * kCMid] : 1.f;
     cw.t2 = d.has_affine ? aff[2 * kCMid + 1] : 0.f;
     // head pointers into the device blob
-    const float *p = h->d_blob + n_conv;
-    const float *wih0 = p; p += (int64_t)kGates * d.L;
-    h->hw.whh0 = p; p += kGates * kHidden;
-    h->hw.bih0 = p; p += kGates;
-    h->hw.bhh0 = p; p += kGates;
-    h->hw.wih1 = p; p += kGates * kHidden;
-    h->hw.whh1 = p; p += kGates * kHidden;
-    h->hw.bih1 = p; p += kGates;
-    h->hw.bhh1 = p; p += kGates;
-    h->hw.wo = p; p += kHidden;
-    h->hw.bo = p;
-    h->hw.wih0T = h->d_wih0T;
+    const float *p = h->d_blob, *wih0 = p + off.wih0;
+    h->hw = HeadWeights{h->d_wih0T, p + off.whh0, p + off.bih0, p + off.bhh0, p + off.wih1, p + off.whh1, p + off.bih1, p + off.bhh1,
+                        p + off.wo, p + off.bo};
     launch_transpose_wih(wih0, h->d_wih0T, d.L, st);
     CU_TRY(cudaGetLastError());
     int rc = tc_prepare(h->tc, d, cw, wih0, (int)h->opt_tc_splits, st);
@@ -470,6 +426,13 @@ extern "C" int64_t b2cnn_workspace_bytes_for(b2cnn_handle *h, int64_t B, int mod
     return call_layout(h, h->d, B, front_end(h, h->d, dtype)).total;
 }
 
+// the events b2cnn_last_stage_ms reads, created by the first profiled call
+static int create_stage_events(b2cnn_handle *h) {
+    for (int i = 0; i < 3; ++i)
+        if (!h->ev_stage[i]) CU_TRY(cudaEventCreate(&h->ev_stage[i]));
+    return B2CNN_OK;
+}
+
 static int forward_device(b2cnn_handle *h, const void *x, int dtype, int64_t B, int64_t xpitch, const float *age, int64_t n_age,
                           int mode, int apply_sigmoid, float *out, void *ws, int64_t ws_bytes, cudaStream_t st) {
     Dims d = h->d;
@@ -489,8 +452,7 @@ static int forward_device(b2cnn_handle *h, const void *x, int dtype, int64_t B, 
     void *tc_ws = base;
     const bool prof = h->opt_profile != 0;
     if (prof) {
-        for (int i = 0; i < 3; ++i)
-            if (!h->ev_stage[i]) CU_TRY(cudaEventCreate(&h->ev_stage[i]));
+        if (int rc = create_stage_events(h)) return rc;
         CU_TRY(cudaEventRecord(h->ev_stage[0], st));
     }
     // stage 0: the front end, or the short-window kernel that does the whole call
@@ -605,11 +567,22 @@ static uint64_t weights_digest(const Slide *s, const ConvWeights &cw) {
     return hdr.frontend_digest;
 }
 
+// B2CNN_ESTATE when the handle's weights changed since the scorer's last reset, else B2CNN_OK
+static int check_fresh(const char *fn, const b2cnn_slide *o,
+                       const char *why = "the handle's weights changed since the scorer's last reset (stored features are stale)") {
+    return o->gen == o->h->weight_gen ? B2CNN_OK : fail(B2CNN_ESTATE, std::string(fn) + ": " + why);
+}
+
+// B2CNN_EINVAL unless path is B2CNN_PATH_AUTO, B2CNN_PATH_GENERIC or B2CNN_PATH_TENSORCORE
+static int check_path(const char *fn, int path) {
+    if (path == B2CNN_PATH_TENSORCORE || path == B2CNN_PATH_GENERIC || path == B2CNN_PATH_AUTO) return B2CNN_OK;
+    return fail(B2CNN_EINVAL, std::string(fn) + ": path must be B2CNN_PATH_AUTO, B2CNN_PATH_GENERIC or B2CNN_PATH_TENSORCORE");
+}
+
 static int slide_create_on(const char *fn, b2cnn_handle *h, int32_t n_patients, int32_t stride, int dtype, int path, b2cnn_slide **out) {
     if (!h || !out) return fail(B2CNN_EINVAL, std::string(fn) + ": null argument");
     *out = nullptr;
-    if (path != B2CNN_PATH_TENSORCORE && path != B2CNN_PATH_GENERIC && path != B2CNN_PATH_AUTO)
-        return fail(B2CNN_EINVAL, std::string(fn) + ": path must be B2CNN_PATH_AUTO, B2CNN_PATH_GENERIC or B2CNN_PATH_TENSORCORE");
+    if (int rc = check_path(fn, path)) return rc;
     if (!h->weights_set) return fail(B2CNN_ESTATE, std::string(fn) + ": weights not set (call b2cnn_set_weights)");
     DEVICE_GUARD(h->device);
     const char *err = "";
@@ -619,7 +592,7 @@ static int slide_create_on(const char *fn, b2cnn_handle *h, int32_t n_patients, 
     const bool tc = path == B2CNN_PATH_TENSORCORE || (path == B2CNN_PATH_AUTO && h->tc.fused);
     const int rc = slide_create(h->d, h->tc, tc ? B2CNN_PATH_TENSORCORE : B2CNN_PATH_GENERIC, n_patients, stride, dtype, h->device,
                                 h->num_sms, &s, &err);
-    if (rc != B2CNN_OK) return fail(rc, std::string(fn) + ": " + err);
+    if (rc != B2CNN_OK) return finish(fn, rc, err);
     b2cnn_slide *o = new (std::nothrow) b2cnn_slide{s, h, h->weight_gen, weights_digest(s, h->cw)};
     if (!o) { slide_destroy(s); return fail(B2CNN_ESTATE, "out of host memory"); }
     if (slide_reset(s, nullptr, &err) != B2CNN_OK || cudaStreamSynchronize(nullptr) != cudaSuccess) {
@@ -647,7 +620,7 @@ extern "C" int b2cnn_slide_reset(b2cnn_slide *o, void *stream) {
     DEVICE_GUARD(slide_device(o->s));
     const char *err = "";
     const int rc = slide_reset(o->s, reinterpret_cast<cudaStream_t>(stream), &err);
-    if (rc != B2CNN_OK) return fail(rc, std::string("b2cnn_slide_reset: ") + err);
+    if (rc != B2CNN_OK) return finish("b2cnn_slide_reset", rc, err);
     o->gen = o->h->weight_gen;
     o->digest = weights_digest(o->s, o->h->cw);
     return B2CNN_OK;
@@ -656,8 +629,7 @@ static int slide_push_api(const char *fn, b2cnn_slide *o, const void *new_sample
                           int apply_sigmoid, float *out, bool heads, int32_t *emitted, int64_t *window_index, void *stream) {
     if (!o || !new_samples || !age || !out || !emitted || !window_index) return fail(B2CNN_EINVAL, std::string(fn) + ": null argument");
     b2cnn_handle *h = o->h;
-    if (o->gen != h->weight_gen)
-        return fail(B2CNN_ESTATE, std::string(fn) + ": the handle's weights changed since the scorer's last reset (stored features are stale)");
+    if (int rc = check_fresh(fn, o)) return rc;
     const int stale = heads ? slide_stale_head(o->s, o->digest) : -1;
     if (stale >= 0)
         return fail(B2CNN_ESTATE, std::string(fn) + ": head " + std::to_string(stale) +
@@ -666,8 +638,7 @@ static int slide_push_api(const char *fn, b2cnn_slide *o, const void *new_sample
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     cudaEvent_t *ev = nullptr;
     if (h->opt_profile) {
-        for (int i = 0; i < 3; ++i)
-            if (!h->ev_stage[i]) CU_TRY(cudaEventCreate(&h->ev_stage[i]));
+        if (int rc = create_stage_events(h)) return rc;
         ev = h->ev_stage;
     }
     const char *err = "";
@@ -675,7 +646,7 @@ static int slide_push_api(const char *fn, b2cnn_slide *o, const void *new_sample
     int64_t widx = -1;
     const int rc = slide_push(o->s, h->cw, h->hw, h->tc, new_samples, pitch, age, n_age, apply_sigmoid, out, heads, &em, &widx, ev, st,
                               &err);
-    if (rc != B2CNN_OK) return fail(rc, std::string(fn) + ": " + err);
+    if (rc != B2CNN_OK) return finish(fn, rc, err);
     h->ev_valid = ev != nullptr;
     *emitted = em;
     if (em) *window_index = widx;
@@ -692,66 +663,62 @@ extern "C" int b2cnn_slide_push_heads(b2cnn_slide *o, const void *new_samples, i
 }
 extern "C" int b2cnn_slide_n_heads(const b2cnn_slide *o) { return o ? slide_n_heads(o->s) : -1; }
 static int slide_set_heads_api(const char *fn, b2cnn_slide *o, b2cnn_handle *const *heads, int32_t n, int32_t flags, void *stream) {
-    if (!o || (n > 0 && !heads)) return fail(B2CNN_EINVAL, std::string(fn) + "null argument");
-    if (flags & ~B2CNN_SLIDE_HEADS_SHORTER_WINDOWS) return fail(B2CNN_EINVAL, std::string(fn) + "unknown flag bits");
+    const std::string pre = std::string(fn) + ": ";
+    if (!o || (n > 0 && !heads)) return fail(B2CNN_EINVAL, pre + "null argument");
+    if (flags & ~B2CNN_SLIDE_HEADS_SHORTER_WINDOWS) return fail(B2CNN_EINVAL, pre + "unknown flag bits");
     if (n < 0 || n > B2CNN_SLIDE_MAX_HEADS)
-        return fail(B2CNN_EINVAL, std::string(fn) + "n must be in [0, " + std::to_string(B2CNN_SLIDE_MAX_HEADS) + "]");
+        return fail(B2CNN_EINVAL, pre + "n must be in [0, " + std::to_string(B2CNN_SLIDE_MAX_HEADS) + "]");
     const b2cnn_handle *h = o->h;
     const b2cnn_config &c = h->cfg;
     const bool shorter = flags & B2CNN_SLIDE_HEADS_SHORTER_WINDOWS;
-    b2cnn_slide_state_header mine;
-    slide_describe_state(o->s, h->cw, &mine);
-    const int F = mine.feature_stride;
-    const int R = c.pool_s * (c.pool_k + c.k2 - 2) + c.pool_k + c.k1 - 1;     // the receptive field of one feature
+    const int F = h->d.feature_stride(), R = h->d.receptive_field();
     std::vector<SlideHeadSource> src((size_t)n);
     for (int i = 0; i < n; ++i) {
         const b2cnn_handle *x = heads[i];
         const std::string which = "head " + std::to_string(i) + ": ";
-        if (!x) return fail(B2CNN_EINVAL, fn + which + "null handle");
-        if (!x->weights_set) return fail(B2CNN_EINVAL, fn + which + "weights not set (call b2cnn_set_weights)");
-        if (x->device != h->device) return fail(B2CNN_EINVAL, fn + which + "on another device than the scorer");
+        if (!x) return fail(B2CNN_EINVAL, pre + which + "null handle");
+        if (!x->weights_set) return fail(B2CNN_EINVAL, pre + which + "weights not set (call b2cnn_set_weights)");
+        if (x->device != h->device) return fail(B2CNN_EINVAL, pre + which + "on another device than the scorer");
         const b2cnn_config &e = x->cfg;
         if (e.in_channels != c.in_channels || e.k1 != c.k1 || e.c_mid != c.c_mid || e.k2 != c.k2 || e.pool_k != c.pool_k ||
             e.pool_s != c.pool_s || e.hidden != c.hidden || e.layers != c.layers || e.act != c.act || e.flags != c.flags ||
             (!shorter && (e.window != c.window || e.lstm_input != c.lstm_input)))
-            return fail(B2CNN_EARCH, fn + which + (shorter ? "another architecture than the scorer's model (only window, lstm_input and age_coef may differ)"
-                                                           : "another architecture than the scorer's model (only age_coef may differ)"));
-        if (e.window > c.window) return fail(B2CNN_EARCH, fn + which + "a longer window than the scorer's");
+            return fail(B2CNN_EARCH, pre + which + (shorter ? "another architecture than the scorer's model (only window, lstm_input and age_coef may differ)"
+                                                            : "another architecture than the scorer's model (only age_coef may differ)"));
+        if (e.window > c.window) return fail(B2CNN_EARCH, pre + which + "a longer window than the scorer's");
         if ((c.window - e.window) % F != 0)
-            return fail(B2CNN_EARCH, fn + which + "the scorer's window minus the head's is not a multiple of the feature stride " +
-                                         std::to_string(F) + " (another feature lattice)");
+            return fail(B2CNN_EARCH, pre + which + "the scorer's window minus the head's is not a multiple of the feature stride " +
+                                          std::to_string(F) + " (another feature lattice)");
         if (e.window < R || e.lstm_input != (e.window - R) / F + 1)
-            return fail(B2CNN_EARCH, fn + which + "lstm_input is not the feature count of the head's window");
+            return fail(B2CNN_EARCH, pre + which + "lstm_input is not the feature count of the head's window");
         if (slide_path(o->s) == B2CNN_PATH_TENSORCORE &&
             (!x->tc.fused || (e.window == c.window && (x->tc.n_ranges != h->tc.n_ranges || x->tc.chunks_per_cta != h->tc.chunks_per_cta))))
-            return fail(B2CNN_EARCH, fn + which + (e.window == c.window ? "no packed W_ih chunks of the scorer's layout"
-                                                                        : "no packed W_ih chunks of the streaming kernels for its window"));
+            return fail(B2CNN_EARCH, pre + which + (e.window == c.window ? "no packed W_ih chunks of the scorer's layout"
+                                                                         : "no packed W_ih chunks of the streaming kernels for its window"));
         src[i] = SlideHeadSource{x->hw, &x->tc, x->d.age_coef, weights_digest(o->s, x->cw), e.window, e.lstm_input};
     }
-    if (o->gen != h->weight_gen)
-        return fail(B2CNN_ESTATE, std::string(fn) + "the scorer's handle's weights changed since its last reset (call reset first)");
+    if (int rc = check_fresh(fn, o, "the scorer's handle's weights changed since its last reset (call reset first)")) return rc;
     for (int i = 0; i < n; ++i)
         if (src[i].digest != o->digest)
-            return fail(B2CNN_ESTATE, fn + ("head " + std::to_string(i)) + ": other front-end (conv / affine) weights than the scorer's");
+            return fail(B2CNN_ESTATE, pre + ("head " + std::to_string(i)) + ": other front-end (conv / affine) weights than the scorer's");
     DEVICE_GUARD(h->device);
     const char *err = "";
     const int rc = slide_set_heads(o->s, src.data(), n, reinterpret_cast<cudaStream_t>(stream), &err);
-    return rc == B2CNN_OK ? rc : fail(rc, fn + std::string(err));
+    return finish(fn, rc, err);
 }
 extern "C" int b2cnn_slide_set_heads(b2cnn_slide *o, b2cnn_handle *const *heads, int32_t n, void *stream) {
-    return slide_set_heads_api("b2cnn_slide_set_heads: ", o, heads, n, 0, stream);
+    return slide_set_heads_api("b2cnn_slide_set_heads", o, heads, n, 0, stream);
 }
 extern "C" int b2cnn_slide_set_heads_ex(b2cnn_slide *o, b2cnn_handle *const *heads, int32_t n, int32_t flags, void *stream) {
-    return slide_set_heads_api("b2cnn_slide_set_heads_ex: ", o, heads, n, flags, stream);
+    return slide_set_heads_api("b2cnn_slide_set_heads_ex", o, heads, n, flags, stream);
 }
 extern "C" int b2cnn_slide_features(b2cnn_slide *o, float *feats, void *stream) {
     if (!o || !feats) return fail(B2CNN_EINVAL, "b2cnn_slide_features: null argument");
-    if (o->gen != o->h->weight_gen)
-        return fail(B2CNN_ESTATE, "b2cnn_slide_features: the handle's weights changed since the scorer's last reset (stored features are stale)");
+    if (int rc = check_fresh("b2cnn_slide_features", o)) return rc;
     DEVICE_GUARD(slide_device(o->s));
     const char *err = "";
     const int rc = slide_features(o->s, feats, reinterpret_cast<cudaStream_t>(stream), &err);
-    return rc == B2CNN_OK ? rc : fail(rc, std::string("b2cnn_slide_features: ") + err);
+    return finish("b2cnn_slide_features", rc, err);
 }
 
 extern "C" int64_t b2cnn_slide_admit_workspace_bytes(b2cnn_slide *o, int32_t n, int64_t history_len) {
@@ -761,28 +728,27 @@ extern "C" int b2cnn_slide_admit(b2cnn_slide *o, const int32_t *patients, int32_
                                  int64_t pitch, int dtype, void *workspace, int64_t workspace_bytes, void *stream) {
     if (!o) return fail(B2CNN_EINVAL, "b2cnn_slide_admit: null argument");
     if (dtype != slide_dtype(o->s)) return fail(B2CNN_EINVAL, "b2cnn_slide_admit: the history's dtype is not the scorer's");
-    if (o->gen != o->h->weight_gen)
-        return fail(B2CNN_ESTATE, "b2cnn_slide_admit: the handle's weights changed since the scorer's last reset (stored features are stale)");
+    if (int rc = check_fresh("b2cnn_slide_admit", o)) return rc;
     b2cnn_handle *h = o->h;
     DEVICE_GUARD(h->device);
     const char *err = "";
     const int rc = slide_admit(o->s, h->cw, h->tc, patients, n, history, history_len, pitch, workspace, workspace_bytes,
                                reinterpret_cast<cudaStream_t>(stream), &err);
-    return rc == B2CNN_OK ? rc : fail(rc, std::string("b2cnn_slide_admit: ") + err);
+    return finish("b2cnn_slide_admit", rc, err);
 }
 extern "C" int b2cnn_slide_discharge(b2cnn_slide *o, const int32_t *patients, int32_t n, void *stream) {
     if (!o) return fail(B2CNN_EINVAL, "b2cnn_slide_discharge: null argument");
     DEVICE_GUARD(slide_device(o->s));
     const char *err = "";
     const int rc = slide_discharge(o->s, patients, n, reinterpret_cast<cudaStream_t>(stream), &err);
-    return rc == B2CNN_OK ? rc : fail(rc, std::string("b2cnn_slide_discharge: ") + err);
+    return finish("b2cnn_slide_discharge", rc, err);
 }
 extern "C" int b2cnn_slide_samples_seen(b2cnn_slide *o, int64_t *seen, void *stream) {
     if (!o || !seen) return fail(B2CNN_EINVAL, "b2cnn_slide_samples_seen: null argument");
     DEVICE_GUARD(slide_device(o->s));
     const char *err = "";
     const int rc = slide_samples_seen(o->s, seen, reinterpret_cast<cudaStream_t>(stream), &err);
-    return rc == B2CNN_OK ? rc : fail(rc, std::string("b2cnn_slide_samples_seen: ") + err);
+    return finish("b2cnn_slide_samples_seen", rc, err);
 }
 extern "C" int b2cnn_slide_describe_state(b2cnn_slide *o, b2cnn_slide_state_header *out) {
     if (!o || !out) return fail(B2CNN_EINVAL, "b2cnn_slide_describe_state: null argument");
@@ -795,25 +761,23 @@ extern "C" int64_t b2cnn_slide_state_workspace_bytes(b2cnn_slide *o, int32_t n) 
 extern "C" int b2cnn_slide_export(b2cnn_slide *o, const int32_t *patients, int32_t n, float *features, float *tails, int64_t *seen_host,
                                   b2cnn_slide_state_header *header, void *workspace, int64_t workspace_bytes, void *stream) {
     if (!o || !header) return fail(B2CNN_EINVAL, "b2cnn_slide_export: null argument");
-    if (o->gen != o->h->weight_gen)
-        return fail(B2CNN_ESTATE, "b2cnn_slide_export: the handle's weights changed since the scorer's last reset (stored features are stale)");
+    if (int rc = check_fresh("b2cnn_slide_export", o)) return rc;
     DEVICE_GUARD(slide_device(o->s));
     const char *err = "";
     const int rc = slide_export(o->s, o->h->cw, patients, n, features, tails, seen_host, header, workspace, workspace_bytes,
                                 reinterpret_cast<cudaStream_t>(stream), &err);
-    return rc == B2CNN_OK ? rc : fail(rc, std::string("b2cnn_slide_export: ") + err);
+    return finish("b2cnn_slide_export", rc, err);
 }
 extern "C" int b2cnn_slide_import(b2cnn_slide *o, const int32_t *patients, int32_t n, const b2cnn_slide_state_header *header,
                                   const float *features, const float *tails, const int64_t *seen_host, void *workspace,
                                   int64_t workspace_bytes, void *stream) {
     if (!o || !header) return fail(B2CNN_EINVAL, "b2cnn_slide_import: null argument");
-    if (o->gen != o->h->weight_gen)
-        return fail(B2CNN_ESTATE, "b2cnn_slide_import: the handle's weights changed since the scorer's last reset (stored features are stale)");
+    if (int rc = check_fresh("b2cnn_slide_import", o)) return rc;
     DEVICE_GUARD(slide_device(o->s));
     const char *err = "";
     const int rc = slide_import(o->s, o->h->cw, patients, n, *header, features, tails, seen_host, workspace, workspace_bytes,
                                 reinterpret_cast<cudaStream_t>(stream), &err);
-    return rc == B2CNN_OK ? rc : fail(rc, std::string("b2cnn_slide_import: ") + err);
+    return finish("b2cnn_slide_import", rc, err);
 }
 
 // ---- every sliding window of whole recordings (b2cnn_slide.cu) ----
@@ -822,8 +786,7 @@ static int record_path(const char *fn, const b2cnn_handle *h, int dtype, int pat
     if (!h) return fail(B2CNN_EINVAL, std::string(fn) + ": null argument");
     if (!h->weights_set) return fail(B2CNN_ESTATE, std::string(fn) + ": weights not set (call b2cnn_set_weights)");
     if (dtype != B2CNN_DTYPE_F32 && dtype != B2CNN_DTYPE_BF16) return fail(B2CNN_EINVAL, std::string(fn) + ": dtype must be f32 (0) or bf16 (1)");
-    if (path != B2CNN_PATH_TENSORCORE && path != B2CNN_PATH_GENERIC && path != B2CNN_PATH_AUTO)
-        return fail(B2CNN_EINVAL, std::string(fn) + ": path must be B2CNN_PATH_AUTO, B2CNN_PATH_GENERIC or B2CNN_PATH_TENSORCORE");
+    if (int rc = check_path(fn, path)) return rc;
     if (path == B2CNN_PATH_TENSORCORE && !h->tc.fused)
         return fail(B2CNN_EARCH, std::string(fn) + ": the tensor-core path covers the streaming tensor-core geometries only (MyCNN5 or "
                                                    "MyCNN2/3/4 conv/pool, 1 to 3 channels, tanh, no affine)");
@@ -861,7 +824,7 @@ static int record_score(const char *fn, b2cnn_handle *h, const void *x, int dtyp
     const char *err = "";
     const int rc = score_record(h->d, h->cw, h->hw, h->tc, tc, h->num_sms, x, dtype, B, N, pitch, stride, mode, age, n_age, apply_sigmoid,
                                 out, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream), &err);
-    if (rc != B2CNN_OK) return fail(rc, std::string(fn) + ": " + err);
+    if (rc != B2CNN_OK) return finish(fn, rc, err);
     h->last_path = tc ? B2CNN_PATH_TENSORCORE : B2CNN_PATH_GENERIC;
     return B2CNN_OK;
 }

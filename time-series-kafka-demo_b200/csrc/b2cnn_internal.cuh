@@ -27,6 +27,69 @@ struct Dims {
     float age_coef;
     int XP;                  // row pitch of x in elements (>= W): channel rows start XP apart, windows C*XP apart.
                              // == W for a contiguous [B][C][W] tensor; set per call (b2cnn_forward_pitched)
+
+    // consecutive features start F = pool_s^2 samples apart and each reads R samples, so L = (W - R) / F + 1
+    int feature_stride() const { return PS * PS; }
+    int receptive_field() const { return PS * (PK + K2 - 2) + PK + K1 - 1; }
+};
+
+// false when a size is below 1 or the window is too short for the conv/pool stack
+inline bool derive_dims(const b2cnn_config &c, Dims &d) {
+    d.C = c.in_channels; d.K1 = c.k1; d.K2 = c.k2; d.PK = c.pool_k; d.PS = c.pool_s; d.W = c.window;
+    d.act = c.act; d.has_affine = (c.flags & B2CNN_FLAG_AFFINE) ? 1 : 0; d.age_coef = c.age_coef; d.XP = c.window;
+    if (d.C < 1 || d.K1 < 1 || d.K2 < 1 || d.PK < 1 || d.PS < 1 || d.W < 1) return false;
+    d.L1 = d.W - d.K1 + 1;
+    if (d.L1 < d.PK) return false;
+    d.P1 = (d.L1 - d.PK) / d.PS + 1;
+    d.L2 = d.P1 - d.K2 + 1;
+    if (d.L2 < d.PK) return false;
+    d.L = (d.L2 - d.PK) / d.PS + 1;
+    return d.L >= 1;
+}
+
+// Offsets (floats) of the tensors in the packed weight blob (include/b2cnn.h: b2cnn_weight_count is total): the conv
+// parameters [w1, wih0), the LSTM and the output layer, then with has_affine the conv-epilogue affine block
+// [affine, total) = s1[4], t1[4], s2, t2.
+struct BlobOff {
+    int64_t w1, b1, w2, b2, wih0, whh0, bih0, bhh0, wih1, whh1, bih1, bhh1, wo, bo, affine, total;
+};
+__host__ __device__ inline BlobOff blob_offsets(const Dims &d) {
+    BlobOff o;
+    int64_t p = 0;
+    o.w1 = p; p += (int64_t)kCMid * d.C * d.K1;
+    o.b1 = p; p += kCMid;
+    o.w2 = p; p += kCMid * d.K2;
+    o.b2 = p; p += 1;
+    o.wih0 = p; p += (int64_t)kGates * d.L;
+    o.whh0 = p; p += kGates * kHidden;
+    o.bih0 = p; p += kGates;
+    o.bhh0 = p; p += kGates;
+    o.wih1 = p; p += kGates * kHidden;
+    o.whh1 = p; p += kGates * kHidden;
+    o.bih1 = p; p += kGates;
+    o.bhh1 = p; p += kGates;
+    o.wo = p; p += kHidden;
+    o.bo = p; p += 1;
+    o.affine = p; if (d.has_affine) p += 2 * kCMid + 2;
+    o.total = p;
+    return o;
+}
+
+// Makes `device` current for the guard's lifetime and restores the caller's device on every exit path (a call on cuda:1
+// must not leave the calling thread on cuda:1: later `device="cuda"` allocations of the host framework would land on the
+// wrong GPU).  A negative device leaves the current device as it is.
+struct DeviceGuard {
+    int prev = -1;
+    cudaError_t err = cudaSuccess;
+    explicit DeviceGuard(int dev) {
+        if (dev < 0) return;
+        err = cudaGetDevice(&prev);
+        if (err != cudaSuccess) { prev = -1; return; }
+        if (prev != dev) err = cudaSetDevice(dev); else prev = -1;     // nothing to restore
+    }
+    ~DeviceGuard() { if (prev >= 0) cudaSetDevice(prev); }
+    DeviceGuard(const DeviceGuard &) = delete;
+    DeviceGuard &operator=(const DeviceGuard &) = delete;
 };
 
 // Conv weights travel as a by-value kernel parameter: they land in the constant bank, so the
@@ -181,14 +244,15 @@ int wire_decode_arrays(const uint8_t *bytes, const int64_t *offsets, int64_t n_m
                        int *n_bad, cudaStream_t st, const char **err);
 double wire_parse_decimal_host(const char *s, int64_t len, int *status);
 
-// b2cnn_train.cu: one training step (row f4)
+// b2cnn_train.cu: one training step (row f4).  mode is B2CNN_MODE_*; every entry point checks all its arguments before
+// any CUDA call, then makes cfg->device current for the call (a negative device: the current one)
 int64_t train_workspace_bytes(const b2cnn_config *cfg, int64_t B);
 // weighted != 0: BCEWithLogitsLoss(pos_weight=pos_weight), else plain BCEWithLogitsLoss
 int train_step(const b2cnn_config *cfg, float *params, float *adam_m, float *adam_v, float *grads, int64_t step, float lr, float beta1,
                float beta2, float eps, int apply_update, const float *x, int64_t B, const float *age, const float *target,
-               int weighted, float pos_weight, int sequence, const float *mask1, const float *mask2, float *loss_out, void *workspace,
+               int weighted, float pos_weight, int mode, const float *mask1, const float *mask2, float *loss_out, void *workspace,
                int64_t ws_bytes, cudaStream_t st, const char **err);
-// the autograd seam: mode is B2CNN_MODE_*; both check every argument before any CUDA call and set cfg->device themselves
+// the autograd seam
 int train_forward(const b2cnn_config *cfg, const float *params, const float *x, int64_t B, const float *age, int mode, const float *mask1,
                   const float *mask2, float *z_out, void *workspace, int64_t ws_bytes, cudaStream_t st, const char **err);
 int train_backward(const b2cnn_config *cfg, const float *params, const float *x, int64_t B, const float *age, int mode,

@@ -43,8 +43,8 @@ static bool record_plan(const Dims &d, const TcState &tc, bool use_tc, int64_t B
     memset(&p, 0, sizeof p);
     p.tc = use_tc;
     p.seq = mode == B2CNN_MODE_SEQUENCE;
-    p.F = d.PS * d.PS;
-    p.R = d.PS * (d.PK + d.K2 - 2) + d.PK + d.K1 - 1;
+    p.F = d.feature_stride();
+    p.R = d.receptive_field();
     *code = B2CNN_EINVAL;
     if (mode != B2CNN_MODE_INDEPENDENT && mode != B2CNN_MODE_SEQUENCE) {
         *err = "mode must be B2CNN_MODE_INDEPENDENT or B2CNN_MODE_SEQUENCE"; return false;

@@ -426,8 +426,8 @@ static int launch_exact_p(SlideExactParams p, const Slide &s, int64_t ng, cudaSt
 }
 
 // ---- generic path: every geometry, exact fp32 on CUDA cores --------------------------------------------------------
-// Lattice of a conv/pool geometry: feature stride F = pool_s^2, receptive field R = pool_s (pool_k + k2 - 2) + pool_k +
-// k1 - 1 (L = (W - R) / F + 1), phase phi = (-W) mod F; stream feature g reads samples F g + phi .. F g + phi + R - 1.
+// Lattice of a conv/pool geometry: feature stride F = pool_s^2, receptive field R (Dims::receptive_field; L = (W - R) /
+// F + 1), phase phi = (-W) mod F; stream feature g reads samples F g + phi .. F g + phi + R - 1.
 // Every feature comes from the generic front end predict() runs on whole windows (launch_frontend_generic: the
 // templated frontend_kernel or frontend_any_kernel, the same arithmetic term for term), pointed at the first feature's
 // sample with the window's row pitch and writing straight into ring slots:
@@ -536,7 +536,7 @@ int slide_create(const Dims &d, const TcState &tc, int path, int n_patients, int
     if (dtype != B2CNN_DTYPE_F32 && dtype != B2CNN_DTYPE_BF16) { *err = "dtype must be f32 (0) or bf16 (1)"; return B2CNN_EINVAL; }
     if (n_patients < 1 || n_patients > (1 << 24)) { *err = "n_patients out of range"; return B2CNN_EINVAL; }
     if (stride < 1 || stride > d.W) { *err = "stride must be in [1, window]"; return B2CNN_EINVAL; }
-    const int F = d.PS * d.PS, R = d.PS * (d.PK + d.K2 - 2) + d.PK + d.K1 - 1;
+    const int F = d.feature_stride(), R = d.receptive_field();
     if (stride % F != 0) {
         *err = tcp ? "stride must be a multiple of the feature stride (4 samples)"
                    : "stride must be a multiple of the feature stride (pool_s^2 samples)";

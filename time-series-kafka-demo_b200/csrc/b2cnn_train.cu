@@ -44,36 +44,6 @@
 
 namespace b2cnn {
 
-struct TrainDims {
-    int C, K1, K2, PK, PS, W, L1, P1, L2, L;
-    float age_coef;
-};
-
-// offsets (floats) of the tensors inside the packed parameter blob (include/b2cnn.h: b2cnn_weight_count)
-struct BlobOff {
-    int64_t w1, b1, w2, b2, wih0, whh0, bih0, bhh0, wih1, whh1, bih1, bhh1, wo, bo, total;
-};
-static BlobOff blob_offsets(const TrainDims &d) {
-    BlobOff o;
-    int64_t p = 0;
-    o.w1 = p; p += (int64_t)kCMid * d.C * d.K1;
-    o.b1 = p; p += kCMid;
-    o.w2 = p; p += kCMid * d.K2;
-    o.b2 = p; p += 1;
-    o.wih0 = p; p += (int64_t)kGates * d.L;
-    o.whh0 = p; p += kGates * kHidden;
-    o.bih0 = p; p += kGates;
-    o.bhh0 = p; p += kGates;
-    o.wih1 = p; p += kGates * kHidden;
-    o.whh1 = p; p += kGates * kHidden;
-    o.bih1 = p; p += kGates;
-    o.bhh1 = p; p += kGates;
-    o.wo = p; p += kHidden;
-    o.bo = p; p += 1;
-    o.total = p;
-    return o;
-}
-
 // workspace layout (floats)
 struct TrainWs {
     int64_t f, pre0, acts, cs, hs, lin, z, da0, dfeat, part, total;
@@ -92,7 +62,7 @@ struct TileSmem {
     int w1, b1, w2, b2, x, xp, c1, d1, pp, c2, df, dc2, dd1, dc1, g, total;
 };
 // The largest tile: min(kT, L) features plus the few positions the last tile takes on beyond its last pooling window.
-__host__ __device__ inline TileSmem tile_smem(const TrainDims &d, bool backward) {
+__host__ __device__ inline TileSmem tile_smem(const Dims &d, bool backward) {
     const int T = d.L < kT ? d.L : kT;
     const int n2 = d.PS * (T - 1) + d.PK + d.PS - 1, np1 = n2 + d.K2 - 1, n1 = d.PS * (np1 - 1) + d.PK + d.PS - 1, nx = n1 + d.K1 - 1;
     TileSmem s;
@@ -114,7 +84,7 @@ __host__ __device__ inline TileSmem tile_smem(const TrainDims &d, bool backward)
         s.dc2 = take(n2);
         s.dd1 = take(kCMid * s.pp);
         s.dc1 = take(kCMid * n1);         // [position][oc]
-        s.g = take(kCMid * d.C * d.K1 + kCMid + kCMid * d.K2 + 1);
+        s.g = take((int)blob_offsets(d).wih0);   // the conv parameters' gradient sums
     }
     s.total = p;
     return s;
@@ -128,7 +98,7 @@ struct TrainPlan {
     size_t smem_fwd, smem_bwd;
 };
 
-static TrainPlan train_plan(const TrainDims &d, int64_t B) {
+static TrainPlan train_plan(const Dims &d, int64_t B) {
     TrainPlan pl{};
     pl.tiles = (d.L + kT - 1) / kT;
     pl.slices = (d.L + kPre0Slice - 1) / kPre0Slice;
@@ -138,7 +108,7 @@ static TrainPlan train_plan(const TrainDims &d, int64_t B) {
     const int64_t bt = B * pl.tiles, win = (bt + kBwdCtas - 1) / kBwdCtas;
     pl.win = (int)(win < 1 ? 1 : win > kWin ? kWin : win);
     pl.groups = (int)((B + pl.win - 1) / pl.win);
-    pl.n_conv = kCMid * d.C * d.K1 + kCMid + kCMid * d.K2 + 1;
+    pl.n_conv = (int)blob_offsets(d).wih0;
     pl.part_rows = (int64_t)pl.tiles * pl.groups;
     pl.smem_fwd = sizeof(float) * tile_smem(d, false).total;
     pl.smem_bwd = sizeof(float) * tile_smem(d, true).total;
@@ -184,7 +154,7 @@ enum Head : int { kHeadLogits = 0, kHeadBce = 1, kHeadBcePw = 2 };
 // ------------------------------------------------------------------------------------------------------------------
 template <int HEAD>
 __global__ void __launch_bounds__(64)
-train_lstm_fwd(const float *__restrict__ pre0, const float *__restrict__ prm, BlobOff o, TrainDims d, int64_t B, int sequence,
+train_lstm_fwd(const float *__restrict__ pre0, const float *__restrict__ prm, BlobOff o, Dims d, int64_t B, int sequence,
                const float *__restrict__ age, const float *__restrict__ target, float pos_weight, float *__restrict__ acts,
                float *__restrict__ cs, float *__restrict__ hs, float *__restrict__ lin, float *__restrict__ z,
                float *__restrict__ loss_out) {
@@ -272,7 +242,7 @@ train_lstm_fwd(const float *__restrict__ pre0, const float *__restrict__ prm, Bl
 // ------------------------------------------------------------------------------------------------------------------
 template <int HEAD>
 __global__ void __launch_bounds__(64)
-train_lstm_bwd(const float *__restrict__ prm, BlobOff o, TrainDims d, int64_t B, int sequence, const float *__restrict__ age,
+train_lstm_bwd(const float *__restrict__ prm, BlobOff o, Dims d, int64_t B, int sequence, const float *__restrict__ age,
                const float *__restrict__ target, float pos_weight, const float *__restrict__ dz_in, const float *__restrict__ acts,
                const float *__restrict__ cs, const float *__restrict__ hs, const float *__restrict__ lin, const float *__restrict__ z,
                float *__restrict__ da0, float *__restrict__ grad, float *__restrict__ dage) {
@@ -395,7 +365,7 @@ train_lstm_bwd(const float *__restrict__ prm, BlobOff o, TrainDims d, int64_t B,
 struct Tile {
     int i0, nf, s2, s1, n2, np1, n1, nx;
 };
-__device__ __forceinline__ Tile tile_of(const TrainDims &d, int tile) {
+__device__ __forceinline__ Tile tile_of(const Dims &d, int tile) {
     Tile t;
     t.i0 = tile * kT;
     t.nf = min(kT, d.L - t.i0);
@@ -410,7 +380,7 @@ __device__ __forceinline__ Tile tile_of(const TrainDims &d, int tile) {
 }
 
 // conv weights into shared memory; conv1's as [c][k][oc], so one 16-byte load feeds the four output channels of a tap
-__device__ __forceinline__ void tile_stage_weights(const float *__restrict__ prm, const BlobOff &o, const TrainDims &d, const TileSmem &s,
+__device__ __forceinline__ void tile_stage_weights(const float *__restrict__ prm, const BlobOff &o, const Dims &d, const TileSmem &s,
                                                    float *sm, int tid) {
     const int ck = d.C * d.K1;
     for (int e = tid; e < kCMid * ck; e += kThreads) sm[s.w1 + (e % ck) * kCMid + e / ck] = prm[o.w1 + e];
@@ -423,7 +393,7 @@ __device__ __forceinline__ void tile_stage_weights(const float *__restrict__ prm
 // the inference kernels' order (an fmaf chain from the bias, channels outer, taps inner), so a value does not depend on
 // the tile that computes it.  Pooling comes before tanh: tanh is monotone, and a NaN in the window wins either way.
 // xb / m1b: the window's x [C][W] and its mask1 [4][P1] (or NULL).  Ends with a barrier.
-__device__ __forceinline__ void conv_tile(const float *__restrict__ xb, const float *__restrict__ m1b, const TrainDims &d, const Tile &t,
+__device__ __forceinline__ void conv_tile(const float *__restrict__ xb, const float *__restrict__ m1b, const Dims &d, const Tile &t,
                                           const TileSmem &s, float *sm, int tid) {
     for (int c = 0; c < d.C; ++c)
         for (int j = tid; j < t.nx; j += kThreads) sm[s.x + c * s.xp + j] = xb[(int64_t)c * d.W + t.s1 + j];
@@ -461,7 +431,7 @@ __device__ __forceinline__ void conv_tile(const float *__restrict__ xb, const fl
 
 // grid: B x tiles CTAs, window-major
 __global__ void __launch_bounds__(kThreads)
-train_conv_fwd(const float *__restrict__ x, const float *__restrict__ prm, BlobOff o, TrainDims d, int tiles,
+train_conv_fwd(const float *__restrict__ x, const float *__restrict__ prm, BlobOff o, Dims d, int tiles,
                const float *__restrict__ mask1, const float *__restrict__ mask2, float *__restrict__ f) {
     extern __shared__ __align__(16) float sm[];
     const TileSmem s = tile_smem(d, false);
@@ -611,7 +581,7 @@ __device__ __forceinline__ float warp_sum(float v) {
 // dx != NULL: d x of the tile's span is added into the zeroed dx; adjacent spans overlap by less than a tile's stride
 // (checked by the host), so a sample has at most two contributions and their sum does not depend on the order.
 __global__ void __launch_bounds__(kThreads)
-train_conv_bwd(const float *__restrict__ x, const float *__restrict__ prm, BlobOff o, TrainDims d, int tiles, int win, int64_t B,
+train_conv_bwd(const float *__restrict__ x, const float *__restrict__ prm, BlobOff o, Dims d, int tiles, int win, int64_t B,
                const float *__restrict__ mask1, const float *__restrict__ mask2, const float *__restrict__ dfeat,
                float *__restrict__ part, float *__restrict__ dx) {
     extern __shared__ __align__(16) float sm[];
@@ -740,42 +710,26 @@ __global__ void train_adam(float *__restrict__ prm, float *__restrict__ m, float
     prm[e] = prm[e] - (lr / bc1) * (mm / denom);
 }
 
-static bool train_dims(const b2cnn_config &c, TrainDims &d, const char **err) {
-    d.C = c.in_channels; d.K1 = c.k1; d.K2 = c.k2; d.PK = c.pool_k; d.PS = c.pool_s; d.W = c.window; d.age_coef = c.age_coef;
+// the geometry of a configuration, refusing what the training kernels do not cover; no CUDA call
+static bool train_geometry(const b2cnn_config *cfg, Dims &d, const char **err) {
+    if (!cfg) { *err = "training: null configuration"; return false; }
+    const b2cnn_config &c = *cfg;
     if (c.c_mid != kCMid || c.hidden != kHidden || c.layers != 2) { *err = "training: c_mid / hidden / layers must be 4 / 16 / 2"; return false; }
     if (c.act != B2CNN_ACT_TANH || (c.flags & B2CNN_FLAG_AFFINE)) { *err = "training: tanh activations without affine only (bin/models.py:23,26)"; return false; }
-    if (d.C < 1 || d.K1 < 1 || d.K2 < 1 || d.PK < 1 || d.PS < 1 || d.W < 1) { *err = "training: bad geometry"; return false; }
-    d.L1 = d.W - d.K1 + 1;
-    if (d.L1 < d.PK) { *err = "training: window too short"; return false; }
-    d.P1 = (d.L1 - d.PK) / d.PS + 1;
-    d.L2 = d.P1 - d.K2 + 1;
-    if (d.L2 < d.PK) { *err = "training: window too short"; return false; }
-    d.L = (d.L2 - d.PK) / d.PS + 1;
+    if (!derive_dims(c, d)) { *err = "training: bad geometry or window too short for the conv/pool stack"; return false; }
     if (d.L != c.lstm_input) { *err = "training: L_out(window) != lstm_input (x.view(-1, MAGICNUM) would straddle windows)"; return false; }
     return true;
 }
 
 int64_t train_workspace_bytes(const b2cnn_config *cfg, int64_t B) {
-    TrainDims d;
+    Dims d;
     const char *err = "";
-    if (!cfg || B < 1 || !train_dims(*cfg, d, &err)) return -1;
+    if (B < 1 || !train_geometry(cfg, d, &err)) return -1;
     return train_plan(d, B).w.total * (int64_t)sizeof(float);
 }
 
-// Sets cfg->device current for the launches of one call (when it is >= 0) and restores the caller's device afterwards.
-struct DeviceScope {
-    int prev = -1;
-    bool ok = true;
-    explicit DeviceScope(int device) {
-        if (device >= 0) ok = cudaGetDevice(&prev) == cudaSuccess && cudaSetDevice(device) == cudaSuccess;
-    }
-    ~DeviceScope() {
-        if (prev >= 0) cudaSetDevice(prev);
-    }
-};
-
 // what the kernels need beyond a valid geometry; no CUDA call
-static bool plan_fits(const TrainDims &d, const TrainPlan &pl, int64_t B, const char **err) {
+static bool plan_fits(const Dims &d, const TrainPlan &pl, int64_t B, const char **err) {
     if (pl.smem_bwd > 227 * 1024) { *err = "training: too many input channels for a conv tile's shared memory"; return false; }
     // a tile's x span against the tiles' stride: d x relies on at most two tiles touching a sample
     const int np1 = d.PS * (kT - 1) + d.PK + d.K2 - 1, span = d.PS * (np1 - 1) + d.PK + d.K1 - 1, stride = d.PS * d.PS * kT;
@@ -785,7 +739,7 @@ static bool plan_fits(const TrainDims &d, const TrainPlan &pl, int64_t B, const 
 }
 
 // conv forward into ws.f and the layer-0 pre-activations into ws.pre0 (one slice is the whole sum: no reduction)
-static void launch_conv_forward(const TrainDims &d, const BlobOff &o, const TrainPlan &pl, float *ws, const float *params,
+static void launch_conv_forward(const Dims &d, const BlobOff &o, const TrainPlan &pl, float *ws, const float *params,
                                 const float *x, int64_t B, const float *mask1, const float *mask2, cudaStream_t st) {
     const TrainWs &w = pl.w;
     if (pl.smem_fwd > 48 * 1024) cudaFuncSetAttribute(train_conv_fwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.smem_fwd);
@@ -800,7 +754,7 @@ static void launch_conv_forward(const TrainDims &d, const BlobOff &o, const Trai
 
 // everything after d(head): d W_ih_l0 and, unless the front end is frozen, d f, the convolutional backward into `grads`
 // and, when dx != NULL, the input gradient (added into dx, zeroed here)
-static bool launch_backward_tail(const TrainDims &d, const BlobOff &o, const TrainPlan &pl, float *ws, const float *params,
+static bool launch_backward_tail(const Dims &d, const BlobOff &o, const TrainPlan &pl, float *ws, const float *params,
                                  const float *x, int64_t B, const float *mask1, const float *mask2, float *grads, float *dx,
                                  bool frozen_conv, cudaStream_t st) {
     const TrainWs &w = pl.w;
@@ -820,20 +774,35 @@ static bool launch_backward_tail(const TrainDims &d, const BlobOff &o, const Tra
     return true;
 }
 
+// The checks every training entry point shares, before any CUDA call: the configuration, the mode, the pointers the call
+// needs (ptrs_ok) and the batch, what the kernels hold, and the workspace size.
+static int train_args(const b2cnn_config *cfg, int64_t B, int mode, bool ptrs_ok, int64_t ws_bytes, Dims &d, TrainPlan &pl,
+                      const char **err) {
+    if (!train_geometry(cfg, d, err)) return B2CNN_EINVAL;
+    if (mode != B2CNN_MODE_INDEPENDENT && mode != B2CNN_MODE_SEQUENCE) { *err = "training: bad mode"; return B2CNN_EINVAL; }
+    if (!ptrs_ok || B < 1) { *err = "training: null argument / bad batch"; return B2CNN_EINVAL; }
+    pl = train_plan(d, B);
+    if (!plan_fits(d, pl, B, err)) return B2CNN_EINVAL;
+    if (ws_bytes < pl.w.total * (int64_t)sizeof(float)) { *err = "training: workspace smaller than b2cnn_train_workspace_bytes()"; return B2CNN_ESTATE; }
+    return B2CNN_OK;
+}
+
 int train_step(const b2cnn_config *cfg, float *params, float *adam_m, float *adam_v, float *grads, int64_t step, float lr, float beta1,
                float beta2, float eps, int apply_update, const float *x, int64_t B, const float *age, const float *target,
-               int weighted, float pos_weight, int sequence, const float *mask1, const float *mask2, float *loss_out, void *workspace,
+               int weighted, float pos_weight, int mode, const float *mask1, const float *mask2, float *loss_out, void *workspace,
                int64_t ws_bytes, cudaStream_t st, const char **err) {
-    TrainDims d;
-    if (!cfg || !train_dims(*cfg, d, err)) return B2CNN_EINVAL;
-    if (!params || !grads || !x || !age || !target || !loss_out || !workspace || B < 1 || step < 1) { *err = "training: null argument / bad step"; return B2CNN_EINVAL; }
+    Dims d;
+    TrainPlan pl;
+    const int rc = train_args(cfg, B, mode, params && grads && x && age && target && loss_out && workspace, ws_bytes, d, pl, err);
+    if (rc != B2CNN_OK) return rc;
+    if (step < 1) { *err = "training: step must be >= 1"; return B2CNN_EINVAL; }
     if (apply_update && (!adam_m || !adam_v)) { *err = "training: Adam state missing"; return B2CNN_EINVAL; }
     if (weighted && !(pos_weight > 0.f && pos_weight <= FLT_MAX)) { *err = "training: pos_weight must be positive and finite"; return B2CNN_EINVAL; }
-    const TrainPlan pl = train_plan(d, B);
+    DeviceGuard dev(cfg->device);
+    if (dev.err != cudaSuccess) { *err = "cudaSetDevice"; return B2CNN_ECUDA; }
     const TrainWs &w = pl.w;
-    if (!plan_fits(d, pl, B, err)) return B2CNN_EINVAL;
-    if (ws_bytes < w.total * (int64_t)sizeof(float)) { *err = "training: workspace smaller than b2cnn_train_workspace_bytes()"; return B2CNN_ESTATE; }
     const BlobOff o = blob_offsets(d);
+    const int sequence = mode == B2CNN_MODE_SEQUENCE ? 1 : 0;
     float *ws = reinterpret_cast<float *>(workspace);
     if (cudaMemsetAsync(grads, 0, sizeof(float) * o.total, st) != cudaSuccess) { *err = "memset grads"; return B2CNN_ECUDA; }
     launch_conv_forward(d, o, pl, ws, params, x, B, mask1, mask2, st);
@@ -858,26 +827,14 @@ int train_step(const b2cnn_config *cfg, float *params, float *adam_m, float *ada
     return B2CNN_OK;
 }
 
-// the checks b2cnn_train_forward and b2cnn_train_backward share; no CUDA call
-static int autograd_args(const b2cnn_config *cfg, int64_t B, int mode, int64_t ws_bytes, bool ptrs_ok, TrainDims &d, TrainPlan &pl,
-                         const char **err) {
-    if (!cfg || !train_dims(*cfg, d, err)) return B2CNN_EINVAL;
-    if (mode != B2CNN_MODE_INDEPENDENT && mode != B2CNN_MODE_SEQUENCE) { *err = "training: bad mode"; return B2CNN_EINVAL; }
-    if (!ptrs_ok || B < 1) { *err = "training: null argument / bad batch"; return B2CNN_EINVAL; }
-    pl = train_plan(d, B);
-    if (!plan_fits(d, pl, B, err)) return B2CNN_EINVAL;
-    if (ws_bytes < pl.w.total * (int64_t)sizeof(float)) { *err = "training: workspace smaller than b2cnn_train_workspace_bytes()"; return B2CNN_ESTATE; }
-    return B2CNN_OK;
-}
-
 int train_forward(const b2cnn_config *cfg, const float *params, const float *x, int64_t B, const float *age, int mode, const float *mask1,
                   const float *mask2, float *z_out, void *workspace, int64_t ws_bytes, cudaStream_t st, const char **err) {
-    TrainDims d;
+    Dims d;
     TrainPlan pl;
-    const int rc = autograd_args(cfg, B, mode, ws_bytes, params && x && age && z_out && workspace, d, pl, err);
+    const int rc = train_args(cfg, B, mode, params && x && age && z_out && workspace, ws_bytes, d, pl, err);
     if (rc != B2CNN_OK) return rc;
-    DeviceScope dev(cfg->device);
-    if (!dev.ok) { *err = "cudaSetDevice"; return B2CNN_ECUDA; }
+    DeviceGuard dev(cfg->device);
+    if (dev.err != cudaSuccess) { *err = "cudaSetDevice"; return B2CNN_ECUDA; }
     const TrainWs &w = pl.w;
     const BlobOff o = blob_offsets(d);
     const int sequence = mode == B2CNN_MODE_SEQUENCE ? 1 : 0;
@@ -893,15 +850,15 @@ int train_forward(const b2cnn_config *cfg, const float *params, const float *x, 
 int train_backward(const b2cnn_config *cfg, const float *params, const float *x, int64_t B, const float *age, int mode,
                    const float *mask1, const float *mask2, const float *dz, float *grads, float *dx, float *dage, int flags,
                    void *workspace, int64_t ws_bytes, cudaStream_t st, const char **err) {
-    TrainDims d;
+    Dims d;
     TrainPlan pl;
-    const int rc = autograd_args(cfg, B, mode, ws_bytes, params && x && age && dz && grads && workspace, d, pl, err);
+    const int rc = train_args(cfg, B, mode, params && x && age && dz && grads && workspace, ws_bytes, d, pl, err);
     if (rc != B2CNN_OK) return rc;
     if (flags & ~B2CNN_TRAIN_FROZEN_CONV) { *err = "training: unknown flag"; return B2CNN_EINVAL; }
     const bool frozen_conv = (flags & B2CNN_TRAIN_FROZEN_CONV) != 0;
     if (frozen_conv && dx) { *err = "training: B2CNN_TRAIN_FROZEN_CONV computes no input gradient (dx must be NULL)"; return B2CNN_EINVAL; }
-    DeviceScope dev(cfg->device);
-    if (!dev.ok) { *err = "cudaSetDevice"; return B2CNN_ECUDA; }
+    DeviceGuard dev(cfg->device);
+    if (dev.err != cudaSuccess) { *err = "cudaSetDevice"; return B2CNN_ECUDA; }
     const TrainWs &w = pl.w;
     const BlobOff o = blob_offsets(d);
     const int sequence = mode == B2CNN_MODE_SEQUENCE ? 1 : 0;

@@ -223,7 +223,7 @@ class SlidingScorer:
         the head's LSTM input size the feature count of W_k"""
         a = self.model.arch
         F = a.pool_s ** 2                                         # 4 on the tensor-core path's geometries too
-        R = a.pool_s * (a.pool_k + a.k2 - 2) + a.pool_k + a.k1 - 1   # samples one feature reads
+        R = a.receptive_field
         Wk = arch.window
         if Wk > self.window:
             raise ValueError(f"heads[{i}]'s window {Wk} is longer than the scorer's, {self.window}")

@@ -33,6 +33,7 @@ import torch
 
 from . import capi
 from .arch import BLOB_KEYS
+from .autograd import check_masks, check_trainable, draw_masks
 from .model import B200MyCNN
 
 
@@ -41,8 +42,7 @@ class B200Trainer:
                  mode: str = "sequence", dropout: float = 0.1, seed: int = 0, pos_weight: Optional[float] = None):
         """``pos_weight``: the class weight of ``nn.BCEWithLogitsLoss(pos_weight=...)`` (a positive number; None = the
         unweighted loss)."""
-        if model.arch.affine or model.arch.act_id != 0:
-            raise NotImplementedError("training covers the reference's tanh stack (bin/models.py:23,26) without the affine variant")
+        check_trainable(model.arch)
         if mode not in ("sequence", "independent"):
             raise ValueError("mode must be 'sequence' or 'independent'")
         if not 0.0 <= float(dropout) < 1.0:
@@ -67,8 +67,6 @@ class B200Trainer:
         self._gen = torch.Generator(device=dev)
         self._gen.manual_seed(seed)
         self.steps = 0
-        a = model.arch
-        self._p1 = ((a.window - a.k1 + 1) - a.pool_k) // a.pool_s + 1
 
     # ------------------------------------------------------------------
     def _views(self, flat: torch.Tensor) -> Dict[str, torch.Tensor]:
@@ -84,14 +82,9 @@ class B200Trainer:
         return self._views(self._grads)
 
     def draw_masks(self, B: int) -> Tuple[Optional[torch.Tensor], Optional[torch.Tensor]]:
-        """The two nn.Dropout masks of bin/models.py:25,28, scaled by 1/(1-p) like torch's dropout."""
-        if self.dropout <= 0.0:
-            return None, None
-        keep = 1.0 - self.dropout
-        dev = self._params.device
-        m1 = torch.bernoulli(torch.full((B, self.model.arch.c_mid, self._p1), keep, device=dev), generator=self._gen) / keep
-        m2 = torch.bernoulli(torch.full((B, self.model.arch.l_out), keep, device=dev), generator=self._gen) / keep
-        return m1, m2
+        """The two nn.Dropout masks of bin/models.py:25,28, scaled by 1/(1-p) like torch's dropout, from the trainer's
+        seeded generator."""
+        return draw_masks(self.model.arch, B, self.dropout, self._params.device, self._gen)
 
     def step(self, x: torch.Tensor, age: torch.Tensor, target: torch.Tensor,
              masks: Optional[Tuple[Optional[torch.Tensor], Optional[torch.Tensor]]] = None, update: bool = True) -> torch.Tensor:
@@ -107,15 +100,7 @@ class B200Trainer:
         target = target.to(dev, torch.float32).reshape(-1).contiguous()
         if age.numel() != B or target.numel() != B:
             raise RuntimeError("age and target must have one entry per window")
-        m1, m2 = masks if masks is not None else self.draw_masks(B)
-        if m1 is not None:
-            m1 = m1.to(dev, torch.float32).contiguous()
-            if tuple(m1.shape) != (B, a.c_mid, self._p1):
-                raise RuntimeError(f"dropout mask 1 must be {(B, a.c_mid, self._p1)}, got {tuple(m1.shape)}")
-        if m2 is not None:
-            m2 = m2.to(dev, torch.float32).contiguous()
-            if tuple(m2.shape) != (B, a.l_out):
-                raise RuntimeError(f"dropout mask 2 must be {(B, a.l_out)}, got {tuple(m2.shape)}")
+        m1, m2 = check_masks(a, B, dev, *(masks if masks is not None else self.draw_masks(B)))
         need = self._lib.b2cnn_train_workspace_bytes(ctypes.byref(self._cfg), B)
         if need < 0:
             capi.check(capi.EINVAL, "b2cnn_train_workspace_bytes")
