@@ -24,7 +24,9 @@
 // Projection: the two features of a step are split into three bf16 pieces and stored into a [128 x 16]
 // K-major A tile per piece; every 16 positions the warpgroup issues 2 row halves x 6 m64n64k16 MMAs (piece
 // pairs hh hm mh hl lh mm: fp32-equivalent products) against the packed W_ih chunk, accumulating the 64 gate
-// pre-activations in registers over the CTA's whole range.  They leave once, as partial[range][window][64].
+// pre-activations in registers over the CTA's whole range.  They leave once, as partial[range][window][64].  The A
+// tiles are double-buffered, so a chunk's MMAs are retired a block later by the wait that retires the next conv1,
+// instead of draining the tensor pipe at every chunk.
 //
 // CTA = 256 threads for bf16 windows, 192 for fp32: warps 0-3 the consumer warpgroup, warp 4 the TMA producer of the
 // window tiles, warp 5 the producer of the W_ih chunks (1-D bulk copies), warps 6-7 (bf16) idle.
@@ -69,7 +71,7 @@ struct TcFusedParams {
 
 __host__ __device__ constexpr size_t hp_smem_bytes(int C, int SPLITS, bool f32in, int out) {
     return 1024 + (size_t)2 * C * kTcM * (f32in ? kTcF32ARow : kTcARow) + (f32in ? 0 : (size_t)C * SPLITS * kTcBBytes + kHpTBytes) +
-           (out == kOutGates ? (size_t)2 * kFuWChunkBytes + 3 * kHpPieceBytes : 0) + 8 * 8;
+           (out == kOutGates ? (size_t)2 * kFuWChunkBytes + 2 * 3 * kHpPieceBytes : 0) + 8 * 8;
 }
 
 // ARCH 0: MyCNN5 geometry (K1=10, pool(3,2)) -- bin/models.py.
@@ -85,7 +87,7 @@ tc_stream_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant
     constexpr int kABytes = kTcM * kARow;             // one channel of one stage
     constexpr int FOFF = ARCH == 0 ? 3 : 2;           // step j emits features 2j-FOFF, 2j-FOFF+1
     extern __shared__ uint8_t smem_raw[];
-    // [2 stages][C][8 KB bf16 | 16 KB fp32] | bands | transpose | W ring [2][6 KB] | A pieces [3][4 KB] | barriers
+    // [2 stages][C][8 KB bf16 | 16 KB fp32] | bands | transpose | W ring [2][6 KB] | A pieces [2][3][4 KB] | barriers
     // aligned by an offset from smem_raw, not by rounding the generic address as an integer: the compiler then still
     // knows every pointer below is shared memory and emits 32-bit LDS / STS instead of 64-bit generic LD / ST
     uint8_t *smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -94,7 +96,7 @@ tc_stream_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant
     float *sT = reinterpret_cast<float *>(sBm + (F32IN ? 0 : C * SPLITS * kTcBBytes));
     uint8_t *sW = reinterpret_cast<uint8_t *>(sT) + (F32IN ? 0 : kHpTBytes);
     uint8_t *sPc = sW + (OUT == kOutGates ? 2 * kFuWChunkBytes : 0);
-    uint64_t *bars = reinterpret_cast<uint64_t *>(sPc + (OUT == kOutGates ? 3 * kHpPieceBytes : 0));
+    uint64_t *bars = reinterpret_cast<uint64_t *>(sPc + (OUT == kOutGates ? 2 * 3 * kHpPieceBytes : 0));
     const uint32_t bar_full = smem_u32(bars + 0), bar_empty = smem_u32(bars + 2);
     const uint32_t bar_wfull = smem_u32(bars + 4), bar_wempty = smem_u32(bars + 6);
     auto sA_of = [&](int s, int c) -> uint8_t * { return sA + (size_t)(s * C + c) * kABytes; };
@@ -215,6 +217,42 @@ tc_stream_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant
                         wgmma_m64n32_rs(acc[h], afr[h][c], bdesc0 + (uint64_t)((c * SPLITS + sp) * (kTcBBytes >> 4)), (c | sp) != 0);
             wgmma_commit();
         };
+        // the projection of chunk m (A pieces in buffer m & 1, W_ih in ring slot m & 1).  Its K-major no-swizzle
+        // descriptors (LBO 128, SBO 256 bytes) differ only in the start-address field of their low word, so an MMA
+        // adds its buffer, piece, row half and W slot offsets (>> 4) to one 32-bit base.  The caller has made every
+        // warp's pieces visible.
+        auto issue_proj = [&](int m) {
+            const int u = m & 1;
+            mbar_wait(bar_wfull + 8 * u, (m >> 1) & 1);
+            const uint32_t pa = smem_u32(sPc) + u * 3 * kHpPieceBytes, pw = smem_u32(sW) + u * kFuWChunkBytes;
+            auto desc = [](uint32_t addr) { return ((uint64_t)(256 >> 4) << 32) | ((addr >> 4) + (uint32_t)((128 >> 4) << 16)); };
+            wgmma_fence();
+#pragma unroll
+            for (int hh = 0; hh < 2; ++hh) {
+                // piece pairs (feature piece, weight piece) with fp + wp <= 2: hh hm mh hl lh mm
+                constexpr int kAp[6] = {0, 0, 1, 0, 2, 1}, kWp[6] = {0, 1, 0, 2, 0, 1};
+#pragma unroll
+                for (int q = 0; q < 6; ++q)
+                    wgmma_m64n64(gacc[hh], desc(pa + (uint32_t)(kAp[q] * kHpPieceBytes + hh * 2048)), desc(pw + (uint32_t)(kWp[q] * 2048)));
+            }
+            wgmma_commit();
+        };
+        // A chunk that ends at step jc inside the range is projected without draining the tensor pipe: bf16 windows issue
+        // it at step jc + 1 behind that step's transpose barrier and before its conv1, and the wait of step jc + 2 retires
+        // both; fp32 windows issue it at the end of step jc and retire it at step jc + 1, after the CUDA-core conv1.  The
+        // step that retires it gives its W slot back.  The range's last chunk is projected after the loop.
+        constexpr int kLag = F32IN ? 1 : 2;
+        // word col of this window's row of the three A tiles of buffer u
+        uint8_t *const prow = sPc + (row >> 3) * 256 + (row & 7) * 16;
+        auto put_pieces = [&](int u, int col, uint32_t w0, uint32_t w1, uint32_t w2) {
+            uint8_t *const a = prow + u * 3 * kHpPieceBytes + (col >> 2) * 128 + (col & 3) * 4;
+            *reinterpret_cast<uint32_t *>(a) = w0;
+            *reinterpret_cast<uint32_t *>(a + kHpPieceBytes) = w1;
+            *reinterpret_cast<uint32_t *>(a + 2 * kHpPieceBytes) = w2;
+        };
+        auto release_w = [&](int j) {
+            if (OUT == kOutGates && j >= kLag && ((j - kLag) & 7) == 7 && lane == 0) mbar_arrive(bar_wempty + 8 * (((j - kLag) >> 3) & 1));
+        };
         if (!F32IN) {
             mbar_wait(bar_full, 0);
             issue_conv1(0, 0);
@@ -236,11 +274,12 @@ tc_stream_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant
                         for (int o = 0; o < kCMid; ++o) pm7[o] = fmaf(p.w9[c][o], xv, pm7[o]);
                     }
                 }
-                wgmma_wait<0>();
+                wgmma_wait<0>();                      // conv1 of this block (and the projection issued at step j - 1)
 #pragma unroll
                 for (int h = 0; h < 2; ++h)
 #pragma unroll
                     for (int c = 0; c < C; ++c) wgmma_keep(afr[h][c]);
+                release_w(j);
 #pragma unroll
                 for (int h = 0; h < 2; ++h)
 #pragma unroll
@@ -249,6 +288,9 @@ tc_stream_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant
                                      acc[h][e], acc[h][e + 1]);
                 wg_bar();
                 if (n == kBlocks - 1 && lane == 0) mbar_arrive(bar_empty + 8 * s);   // stage fully consumed
+                // the chunk that ended at step j - 1, its pieces published by the barrier above, ahead of the next conv1
+                // (behind it, measured no faster than draining)
+                if (OUT == kOutGates && (j & 7) == 0 && j > 0) issue_proj((j >> 3) - 1);
                 if (n < kBlocks - 1) {                // the next block's MMAs overlap this block's epilogue
                     issue_conv1(s, n + 1);
                 } else if (i + 1 < ntiles) {          // (J is a whole number of tiles)
@@ -286,6 +328,10 @@ tc_stream_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant
 #pragma unroll
                                 for (int o = 0; o < kCMid; ++o) D[sft * 4 + o] = fmaf(p.w1[c][k][o], xs[sft + k], D[sft * 4 + o]);
                             }
+                }
+                if constexpr (OUT == kOutGates) {
+                    wgmma_wait<0>();                  // the projection issued at the end of step j - 1, if any
+                    release_w(j);
                 }
                 if (n == kBlocks - 1) {
                     __syncwarp();
@@ -353,41 +399,21 @@ tc_stream_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant
                     if (pr0 + 1 >= 0 && pr0 + 1 < nfeat) p.feats[(int64_t)slot * p.sP + b] = f1;
                 }
             } else {
-                // three bf16 pieces of (f0, f1) -> word kk of this window's row of the A tiles
-                const int kk = j & 7, m = j >> 3, u = m & 1;
+                // three bf16 pieces of (f0, f1) -> word kk of this window's row of chunk m's A tiles (buffer m & 1)
+                const int kk = j & 7, m = j >> 3;
                 const uint32_t h = pack_bf16x2(f0, f1);
                 const float r1x = f0 - __uint_as_float(h << 16), r1y = f1 - __uint_as_float(h & 0xffff0000u);
                 const uint32_t md = pack_bf16x2(r1x, r1y);
                 const uint32_t lo = pack_bf16x2(r1x - __uint_as_float(md << 16), r1y - __uint_as_float(md & 0xffff0000u));
-                uint8_t *arow = sPc + (row >> 3) * 256 + (row & 7) * 16;
-                auto put = [&](int col, uint32_t w0, uint32_t w1, uint32_t w2) {
-                    const int off = (col >> 2) * 128 + (col & 3) * 4;
-                    *reinterpret_cast<uint32_t *>(arow + off) = w0;
-                    *reinterpret_cast<uint32_t *>(arow + kHpPieceBytes + off) = w1;
-                    *reinterpret_cast<uint32_t *>(arow + 2 * kHpPieceBytes + off) = w2;
-                };
-                put(kk, h, md, lo);
-                if (kk == 7 || j == J - 1) {
-                    for (int z = kk + 1; z < 8; ++z) put(z, 0u, 0u, 0u);
+                // chunk m's buffer was last read by chunk m - 2's projection, which every warp retired before it passed the
+                // barrier that published chunk m - 1, so the pieces need no barrier after the MMAs
+                put_pieces(m & 1, kk, h, md, lo);
+                if (kk == 7) {
                     fence_proxy_async();
-                    wg_bar();
-                    mbar_wait(bar_wfull + 8 * u, (m >> 1) & 1);
-                    const uint32_t pa = smem_u32(sPc), pw = smem_u32(sW + u * kFuWChunkBytes);
-                    wgmma_fence();
-#pragma unroll
-                    for (int hh = 0; hh < 2; ++hh) {
-                        // piece pairs (feature piece, weight piece) with fp + wp <= 2: hh hm mh hl lh mm
-                        constexpr int kAp[6] = {0, 0, 1, 0, 2, 1}, kWp[6] = {0, 1, 0, 2, 0, 1};
-#pragma unroll
-                        for (int q = 0; q < 6; ++q)
-                            wgmma_m64n64(gacc[hh], gdesc_none_kmajor(pa + kAp[q] * kHpPieceBytes + hh * 2048, 128, 256),
-                                         gdesc_none_kmajor(pw + kWp[q] * 2048, 128, 256));
+                    if (F32IN && j < J - 1) {
+                        wg_bar();
+                        issue_proj(m);
                     }
-                    wgmma_commit();
-                    wgmma_wait<0>();
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(bar_wempty + 8 * u);
-                    wg_bar();                         // A tiles free for the next chunk
                 }
             }
         };
@@ -404,6 +430,12 @@ tc_stream_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant
         if constexpr (OUT != kOutGates) {
             if (row_ok && nan_probe != nan_probe) p.nanflag[b] = 1;
         } else {
+            // the range's last chunk, whole or partial: zero the words of the steps it does not have
+            for (int z = ((J - 1) & 7) + 1; z < 8; ++z) put_pieces(((J - 1) >> 3) & 1, z, 0u, 0u, 0u);
+            fence_proxy_async();
+            wg_bar();
+            issue_proj((J - 1) >> 3);
+            wgmma_wait<0>();
             // gate pre-activations of this CTA's position range -> partial[range][window][64].  A NaN feature (a NaN / inf
             // sample met a zero of the band matrix, or a real NaN) makes every gate it is multiplied into NaN -- zero weights
             // included -- so the sums themselves are the probe.
