@@ -287,6 +287,28 @@ int b2cnn_slide_admit(b2cnn_slide *slide, const int32_t *patients, int32_t n, co
 int b2cnn_slide_discharge(b2cnn_slide *slide, const int32_t *patients, int32_t n, void *stream);
 int b2cnn_slide_samples_seen(b2cnn_slide *slide, int64_t *seen, void *stream);
 
+/* Sequence mode: every patient scored as the reference's run_model scores a recording (bin/utils.py:671-692, the LSTM
+ * running along the batch axis, bin/models.py:29-30), live.  Each patient p keeps its LSTM state (h and c of both
+ * layers, 256 bytes) on the device, carried from its previous scored window to the next.
+ *   b2cnn_slide_create_ex  b2cnn_slide_create_path with a batch mode.  mode = B2CNN_MODE_INDEPENDENT: exactly
+ *                        b2cnn_slide_create_path.  mode = B2CNN_MODE_SEQUENCE: after a push, out[p] is what
+ *                        model(windows_p, age) returns for the last row, windows_p all of p's windows scored since its
+ *                        admission (or since the last reset), in order: one LSTM step per push from p's stored state.
+ *                        On the generic path out[p] is bit-identical to b2cnn_score_record_ex (generic, sequence) over
+ *                        those windows.  Any other mode: B2CNN_EINVAL.
+ *   b2cnn_slide_mode     B2CNN_MODE_INDEPENDENT or B2CNN_MODE_SEQUENCE (-1 for NULL).
+ * The state starts at zero at create, b2cnn_slide_reset, b2cnn_slide_admit (with or without history: the history's own
+ * window is not scored, the first step is at the first push with seen[p] >= W) and b2cnn_slide_discharge, and is not
+ * advanced for a patient whose output is NaN because its window is incomplete or it is discharged.  The age enters the
+ * output scale only, never the state.  A NaN sample makes its patient's output NaN from the first window holding it on
+ * (the state is poisoned, as in run_model) without touching the other patients; b2cnn_slide_admit starts it again.  A
+ * sequence-mode scorer takes no extra heads: b2cnn_slide_set_heads{,_ex} with n > 0 is B2CNN_EINVAL and changes
+ * nothing (n == 0 and b2cnn_slide_push_heads with no heads work).  A push runs the launches of an independent-mode
+ * push with one step kernel in place of the head's launches, allocates nothing, and its results do not depend on P
+ * or on the run. */
+int b2cnn_slide_create_ex(b2cnn_handle *h, int32_t n_patients, int32_t stride, int dtype, int path, int mode, b2cnn_slide **out);
+int b2cnn_slide_mode(const b2cnn_slide *slide);
+
 /* Every sliding window of whole recordings in one call (DESIGN.md §7), each window feature computed once.
  *   b2cnn_score_record  x: DEVICE [B][C][pitch] samples of `dtype` (channel rows pitch >= N samples apart, recordings
  *                        C pitch apart; any alignment), N samples per recording.  out: DEVICE float [B][n_w], n_w =
@@ -368,6 +390,18 @@ int b2cnn_slide_export(b2cnn_slide *slide, const int32_t *patients, int32_t n, f
 int b2cnn_slide_import(b2cnn_slide *slide, const int32_t *patients, int32_t n, const b2cnn_slide_state_header *header,
                        const float *features, const float *tails, const int64_t *seen_host, void *workspace,
                        int64_t workspace_bytes, void *stream);
+/* The same calls with a sequence-mode scorer's LSTM state (b2cnn_slide_create_ex): lstm is NULL or a DEVICE fp32
+ * array [n][2 layers][h, c][16 units].
+ *   b2cnn_slide_export_ex  b2cnn_slide_export, plus the listed patients' state rows into lstm when it is not NULL.
+ *   b2cnn_slide_import_ex  b2cnn_slide_import, plus the listed patients' state rows from lstm; with lstm == NULL (and
+ *                        with b2cnn_slide_import) a sequence-mode scorer zeroes them, as an admission does.
+ * A non-NULL lstm for an independent-mode scorer is B2CNN_EINVAL.  Every check runs before the first write, and the
+ * header, the workspace and the other arrays are those of b2cnn_slide_export / _import. */
+int b2cnn_slide_export_ex(b2cnn_slide *slide, const int32_t *patients, int32_t n, float *features, float *tails, int64_t *seen_host,
+                          float *lstm, b2cnn_slide_state_header *header, void *workspace, int64_t workspace_bytes, void *stream);
+int b2cnn_slide_import_ex(b2cnn_slide *slide, const int32_t *patients, int32_t n, const b2cnn_slide_state_header *header,
+                          const float *features, const float *tails, const int64_t *seen_host, const float *lstm, void *workspace,
+                          int64_t workspace_bytes, void *stream);
 
 /* Extra heads over one scorer's features (shadow scoring a retrained head, ensembles of heads over one front end).
  * The stored ring holds everything a head needs, so K extra heads cost one projection over the ring each (on the

@@ -34,6 +34,7 @@ SYMBOLS = ("b2cnn_l_out", "b2cnn_weight_count", "b2cnn_create", "b2cnn_destroy",
            "b2cnn_slide_create_path", "b2cnn_slide_path",
            "b2cnn_slide_describe_state", "b2cnn_slide_state_workspace_bytes", "b2cnn_slide_export", "b2cnn_slide_import",
            "b2cnn_slide_set_heads", "b2cnn_slide_set_heads_ex", "b2cnn_slide_n_heads", "b2cnn_slide_push_heads",
+           "b2cnn_slide_create_ex", "b2cnn_slide_mode", "b2cnn_slide_export_ex", "b2cnn_slide_import_ex",
            "b2cnn_record_workspace_bytes", "b2cnn_score_record", "b2cnn_record_workspace_bytes_ex", "b2cnn_score_record_ex",
            "b2cnn_decode_sample_messages", "b2cnn_decode_array_messages", "b2cnn_parse_decimal", "b2cnn_frame_check")
 
@@ -158,6 +159,13 @@ def load_library() -> ctypes.CDLL:
     lib.b2cnn_slide_set_heads_ex.argtypes = [c_vp, c_vp, c_i32, c_i32, c_vp]; lib.b2cnn_slide_set_heads_ex.restype = c_int
     lib.b2cnn_slide_n_heads.argtypes = [c_vp]; lib.b2cnn_slide_n_heads.restype = c_int
     lib.b2cnn_slide_push_heads.argtypes = lib.b2cnn_slide_push.argtypes; lib.b2cnn_slide_push_heads.restype = c_int
+    lib.b2cnn_slide_create_ex.argtypes = [c_vp, c_i32, c_i32, c_int, c_int, c_int, ctypes.POINTER(c_vp)]
+    lib.b2cnn_slide_create_ex.restype = c_int
+    lib.b2cnn_slide_mode.argtypes = [c_vp]; lib.b2cnn_slide_mode.restype = c_int
+    lib.b2cnn_slide_export_ex.argtypes = [c_vp, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp, hdrp, c_vp, c_i64, c_vp]
+    lib.b2cnn_slide_export_ex.restype = c_int
+    lib.b2cnn_slide_import_ex.argtypes = [c_vp, c_vp, c_i32, hdrp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp]
+    lib.b2cnn_slide_import_ex.restype = c_int
     lib.b2cnn_record_workspace_bytes.argtypes = [c_vp, c_i64, c_i64, c_i64, c_i64, c_int, c_int]
     lib.b2cnn_record_workspace_bytes.restype = c_i64
     lib.b2cnn_score_record.argtypes = [c_vp, c_vp, c_int, c_i64, c_i64, c_i64, c_i64, c_int, c_vp, c_i64, c_int, c_vp, c_vp, c_i64, c_vp]

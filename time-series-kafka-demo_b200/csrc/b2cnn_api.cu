@@ -579,10 +579,13 @@ static int check_path(const char *fn, int path) {
     return fail(B2CNN_EINVAL, std::string(fn) + ": path must be B2CNN_PATH_AUTO, B2CNN_PATH_GENERIC or B2CNN_PATH_TENSORCORE");
 }
 
-static int slide_create_on(const char *fn, b2cnn_handle *h, int32_t n_patients, int32_t stride, int dtype, int path, b2cnn_slide **out) {
+static int slide_create_on(const char *fn, b2cnn_handle *h, int32_t n_patients, int32_t stride, int dtype, int path, int mode,
+                           b2cnn_slide **out) {
     if (!h || !out) return fail(B2CNN_EINVAL, std::string(fn) + ": null argument");
     *out = nullptr;
     if (int rc = check_path(fn, path)) return rc;
+    if (mode != B2CNN_MODE_INDEPENDENT && mode != B2CNN_MODE_SEQUENCE)
+        return fail(B2CNN_EINVAL, std::string(fn) + ": mode must be B2CNN_MODE_INDEPENDENT or B2CNN_MODE_SEQUENCE");
     if (!h->weights_set) return fail(B2CNN_ESTATE, std::string(fn) + ": weights not set (call b2cnn_set_weights)");
     DEVICE_GUARD(h->device);
     const char *err = "";
@@ -590,8 +593,8 @@ static int slide_create_on(const char *fn, b2cnn_handle *h, int32_t n_patients, 
     // auto: the tensor-core path where it holds the model (slide_create refuses everything else with B2CNN_EARCH; its
     // geometries have F = 4, so a stride it refuses the generic path refuses too), else the generic path
     const bool tc = path == B2CNN_PATH_TENSORCORE || (path == B2CNN_PATH_AUTO && h->tc.fused);
-    const int rc = slide_create(h->d, h->tc, tc ? B2CNN_PATH_TENSORCORE : B2CNN_PATH_GENERIC, n_patients, stride, dtype, h->device,
-                                h->num_sms, &s, &err);
+    const int rc = slide_create(h->d, h->tc, tc ? B2CNN_PATH_TENSORCORE : B2CNN_PATH_GENERIC, mode, n_patients, stride, dtype,
+                                h->device, h->num_sms, &s, &err);
     if (rc != B2CNN_OK) return finish(fn, rc, err);
     b2cnn_slide *o = new (std::nothrow) b2cnn_slide{s, h, h->weight_gen, weights_digest(s, h->cw)};
     if (!o) { slide_destroy(s); return fail(B2CNN_ESTATE, "out of host memory"); }
@@ -603,12 +606,16 @@ static int slide_create_on(const char *fn, b2cnn_handle *h, int32_t n_patients, 
     return B2CNN_OK;
 }
 extern "C" int b2cnn_slide_create(b2cnn_handle *h, int32_t n_patients, int32_t stride, int dtype, b2cnn_slide **out) {
-    return slide_create_on("b2cnn_slide_create", h, n_patients, stride, dtype, B2CNN_PATH_TENSORCORE, out);
+    return slide_create_on("b2cnn_slide_create", h, n_patients, stride, dtype, B2CNN_PATH_TENSORCORE, B2CNN_MODE_INDEPENDENT, out);
 }
 extern "C" int b2cnn_slide_create_path(b2cnn_handle *h, int32_t n_patients, int32_t stride, int dtype, int path, b2cnn_slide **out) {
-    return slide_create_on("b2cnn_slide_create_path", h, n_patients, stride, dtype, path, out);
+    return slide_create_on("b2cnn_slide_create_path", h, n_patients, stride, dtype, path, B2CNN_MODE_INDEPENDENT, out);
+}
+extern "C" int b2cnn_slide_create_ex(b2cnn_handle *h, int32_t n_patients, int32_t stride, int dtype, int path, int mode, b2cnn_slide **out) {
+    return slide_create_on("b2cnn_slide_create_ex", h, n_patients, stride, dtype, path, mode, out);
 }
 extern "C" int b2cnn_slide_path(const b2cnn_slide *o) { return o ? slide_path(o->s) : -1; }
+extern "C" int b2cnn_slide_mode(const b2cnn_slide *o) { return o ? slide_mode(o->s) : -1; }
 extern "C" void b2cnn_slide_destroy(b2cnn_slide *o) {
     if (!o) return;
     DeviceGuard guard(slide_device(o->s));
@@ -668,6 +675,8 @@ static int slide_set_heads_api(const char *fn, b2cnn_slide *o, b2cnn_handle *con
     if (flags & ~B2CNN_SLIDE_HEADS_SHORTER_WINDOWS) return fail(B2CNN_EINVAL, pre + "unknown flag bits");
     if (n < 0 || n > B2CNN_SLIDE_MAX_HEADS)
         return fail(B2CNN_EINVAL, pre + "n must be in [0, " + std::to_string(B2CNN_SLIDE_MAX_HEADS) + "]");
+    if (n > 0 && slide_mode(o->s) == B2CNN_MODE_SEQUENCE)
+        return fail(B2CNN_EINVAL, pre + "a sequence-mode scorer takes no extra heads");
     const b2cnn_handle *h = o->h;
     const b2cnn_config &c = h->cfg;
     const bool shorter = flags & B2CNN_SLIDE_HEADS_SHORTER_WINDOWS;
@@ -758,26 +767,49 @@ extern "C" int b2cnn_slide_describe_state(b2cnn_slide *o, b2cnn_slide_state_head
 extern "C" int64_t b2cnn_slide_state_workspace_bytes(b2cnn_slide *o, int32_t n) {
     return o ? slide_state_workspace_bytes(o->s, n) : -1;
 }
-extern "C" int b2cnn_slide_export(b2cnn_slide *o, const int32_t *patients, int32_t n, float *features, float *tails, int64_t *seen_host,
-                                  b2cnn_slide_state_header *header, void *workspace, int64_t workspace_bytes, void *stream) {
-    if (!o || !header) return fail(B2CNN_EINVAL, "b2cnn_slide_export: null argument");
-    if (int rc = check_fresh("b2cnn_slide_export", o)) return rc;
+static int slide_export_api(const char *fn, b2cnn_slide *o, const int32_t *patients, int32_t n, float *features, float *tails,
+                            int64_t *seen_host, float *lstm, b2cnn_slide_state_header *header, void *workspace, int64_t workspace_bytes,
+                            void *stream) {
+    if (!o || !header) return fail(B2CNN_EINVAL, std::string(fn) + ": null argument");
+    if (int rc = check_fresh(fn, o)) return rc;
     DEVICE_GUARD(slide_device(o->s));
     const char *err = "";
-    const int rc = slide_export(o->s, o->h->cw, patients, n, features, tails, seen_host, header, workspace, workspace_bytes,
+    const int rc = slide_export(o->s, o->h->cw, patients, n, features, tails, seen_host, lstm, header, workspace, workspace_bytes,
                                 reinterpret_cast<cudaStream_t>(stream), &err);
-    return finish("b2cnn_slide_export", rc, err);
+    return finish(fn, rc, err);
+}
+static int slide_import_api(const char *fn, b2cnn_slide *o, const int32_t *patients, int32_t n, const b2cnn_slide_state_header *header,
+                            const float *features, const float *tails, const int64_t *seen_host, const float *lstm, void *workspace,
+                            int64_t workspace_bytes, void *stream) {
+    if (!o || !header) return fail(B2CNN_EINVAL, std::string(fn) + ": null argument");
+    if (int rc = check_fresh(fn, o)) return rc;
+    DEVICE_GUARD(slide_device(o->s));
+    const char *err = "";
+    const int rc = slide_import(o->s, o->h->cw, patients, n, *header, features, tails, seen_host, lstm, workspace, workspace_bytes,
+                                reinterpret_cast<cudaStream_t>(stream), &err);
+    return finish(fn, rc, err);
+}
+extern "C" int b2cnn_slide_export(b2cnn_slide *o, const int32_t *patients, int32_t n, float *features, float *tails, int64_t *seen_host,
+                                  b2cnn_slide_state_header *header, void *workspace, int64_t workspace_bytes, void *stream) {
+    return slide_export_api("b2cnn_slide_export", o, patients, n, features, tails, seen_host, nullptr, header, workspace, workspace_bytes,
+                            stream);
+}
+extern "C" int b2cnn_slide_export_ex(b2cnn_slide *o, const int32_t *patients, int32_t n, float *features, float *tails, int64_t *seen_host,
+                                     float *lstm, b2cnn_slide_state_header *header, void *workspace, int64_t workspace_bytes, void *stream) {
+    return slide_export_api("b2cnn_slide_export_ex", o, patients, n, features, tails, seen_host, lstm, header, workspace, workspace_bytes,
+                            stream);
 }
 extern "C" int b2cnn_slide_import(b2cnn_slide *o, const int32_t *patients, int32_t n, const b2cnn_slide_state_header *header,
                                   const float *features, const float *tails, const int64_t *seen_host, void *workspace,
                                   int64_t workspace_bytes, void *stream) {
-    if (!o || !header) return fail(B2CNN_EINVAL, "b2cnn_slide_import: null argument");
-    if (int rc = check_fresh("b2cnn_slide_import", o)) return rc;
-    DEVICE_GUARD(slide_device(o->s));
-    const char *err = "";
-    const int rc = slide_import(o->s, o->h->cw, patients, n, *header, features, tails, seen_host, workspace, workspace_bytes,
-                                reinterpret_cast<cudaStream_t>(stream), &err);
-    return finish("b2cnn_slide_import", rc, err);
+    return slide_import_api("b2cnn_slide_import", o, patients, n, header, features, tails, seen_host, nullptr, workspace, workspace_bytes,
+                            stream);
+}
+extern "C" int b2cnn_slide_import_ex(b2cnn_slide *o, const int32_t *patients, int32_t n, const b2cnn_slide_state_header *header,
+                                     const float *features, const float *tails, const int64_t *seen_host, const float *lstm, void *workspace,
+                                     int64_t workspace_bytes, void *stream) {
+    return slide_import_api("b2cnn_slide_import_ex", o, patients, n, header, features, tails, seen_host, lstm, workspace, workspace_bytes,
+                            stream);
 }
 
 // ---- every sliding window of whole recordings (b2cnn_slide.cu) ----

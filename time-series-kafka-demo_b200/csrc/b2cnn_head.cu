@@ -241,70 +241,63 @@ head_reduce_independent_kernel(const float *__restrict__ part, int slices, HeadW
 
 // One warp (one CTA) per segment: CTA s scans rows s seg_len .. s seg_len + seg_len - 1 of gates0, age (n_age > 1) and
 // out sequentially from the zero state.  forward's sequence mode is one segment of B rows; b2cnn_score_record's is one
-// segment per recording, of its n_w windows.  Lane l owns gate rows l and l+32 of every weight matrix (registers); units'
-// (h, c) are held twice, by lanes u and u+16.
+// segment per recording, of its n_w windows.  Each row is one seq_step (b2cnn_head_dev.cuh).
 __global__ void __launch_bounds__(32)
 head_sequence_kernel(const float *__restrict__ gates0, HeadWeights hw, const float *__restrict__ age,
                      int64_t n_age, float coef, int apply_sigmoid, float *__restrict__ out, int64_t seg_len) {
-    const int l = threadIdx.x, u = l & 15;
-    const bool lo = l < 16;
+    const int l = threadIdx.x;
     const int64_t row0 = (int64_t)blockIdx.x * seg_len, B = seg_len;
     gates0 += row0 * kGates;
     out += row0;
     if (n_age != 1) age += row0;
-    float whh0a[kHidden], whh0b[kHidden], wih1a[kHidden], wih1b[kHidden], whh1a[kHidden], whh1b[kHidden];
-#pragma unroll
-    for (int k = 0; k < kHidden; ++k) {
-        whh0a[k] = hw.whh0[l * kHidden + k]; whh0b[k] = hw.whh0[(l + 32) * kHidden + k];
-        wih1a[k] = hw.wih1[l * kHidden + k]; wih1b[k] = hw.wih1[(l + 32) * kHidden + k];
-        whh1a[k] = hw.whh1[l * kHidden + k]; whh1b[k] = hw.whh1[(l + 32) * kHidden + k];
-    }
-    const float bih1a = hw.bih1[l], bih1b = hw.bih1[l + 32], bhh1a = hw.bhh1[l], bhh1b = hw.bhh1[l + 32];
-    const float wo = hw.wo[u], bo = hw.bo[0];
-    float h0 = 0.f, c0 = 0.f, h1 = 0.f, c1 = 0.f;
+    SeqLaneWeights w;
+    seq_load_weights(hw, l, w);
+    SeqState s = {0.f, 0.f, 0.f, 0.f};
     float na = gates0[l], nb = gates0[l + 32];
     for (int64_t t = 0; t < B; ++t) {
-        float ga = na, gb = nb;
+        const float ga = na, gb = nb;                      // (W_ih x + b_ih) + b_hh
         if (t + 1 < B) { na = gates0[(t + 1) * kGates + l]; nb = gates0[(t + 1) * kGates + l + 32]; }
-        // ---- layer 0: gates0 already holds (W_ih x + b_ih) + b_hh; add W_hh h_{t-1}
-        float ra = 0.f, rb = 0.f;
-#pragma unroll
-        for (int k = 0; k < kHidden; ++k) {
-            const float hk = __shfl_sync(0xffffffffu, h0, k);
-            ra = fmaf(whh0a[k], hk, ra); rb = fmaf(whh0b[k], hk, rb);
+        seq_step(w, s, ga, gb, l, age + (n_age == 1 ? 0 : t), coef, apply_sigmoid, out + t);
+    }
+}
+
+// A sequence-mode sliding scorer's head (b2cnn_slide.cu): one seq_step per live patient from its stored state
+// state[p] = {h0, c0, h1, c1} (16 units each), written back.  Its layer-0 pre-activations are summed from the range
+// partials [slices][P][64] in reduce_gates_kernel's order, (sum_k part[k][p][g] + b_ih[g]) + b_hh[g], so that a
+// patient's steps are those of head_sequence_kernel over its windows.  Warp w takes patients w, w + warps, ...: the
+// weights are loaded once per warp.  seen: nullptr (every patient live) or the counts before the push advances them;
+// patient p is live when seen[p] >= 0 && seen[p] + S >= W, and the state of any other patient is left as it is.
+constexpr int kSeqStepThreads = 128, kSeqStepPerWarp = 4;
+__global__ void __launch_bounds__(kSeqStepThreads)
+slide_seq_step_kernel(const float *__restrict__ part, int slices, int64_t P, HeadWeights hw, const float *__restrict__ age,
+                      int64_t n_age, float coef, int apply_sigmoid, float *__restrict__ out, float *__restrict__ state,
+                      const int64_t *__restrict__ seen, int64_t S, int64_t W) {
+    constexpr int kIn = B2CNN_HEAD_INFLIGHT;
+    const int l = threadIdx.x & 31, u = l & 15;
+    SeqLaneWeights w;
+    seq_load_weights(hw, l, w);
+    const float bih0a = hw.bih0[l], bih0b = hw.bih0[l + 32], bhh0a = hw.bhh0[l], bhh0b = hw.bhh0[l + 32];
+    const int64_t warps = (int64_t)gridDim.x * (blockDim.x >> 5), slice = P * kGates;
+    for (int64_t p = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); p < P; p += warps) {
+        if (seen) {
+            const int64_t v = seen[p];
+            if (v < 0 || v + S < W) continue;                      // warp-uniform
         }
-        ga += ra; gb += rb;
-        float A = sigmoid_acc(ga);                         // lanes <16: i ; lanes >=16: f
-        float Bv = lo ? tanhf(gb) : sigmoid_acc(gb);       // lanes <16: g ; lanes >=16: o
-        float ig = __shfl_sync(0xffffffffu, A, u), fg = __shfl_sync(0xffffffffu, A, u + 16);
-        float gg = __shfl_sync(0xffffffffu, Bv, u), og = __shfl_sync(0xffffffffu, Bv, u + 16);
-        c0 = fg * c0 + ig * gg;
-        h0 = og * tanhf(c0);
-        // ---- layer 1: input h0 (new), recurrent h1 (old)
-        float sa = 0.f, sb = 0.f; ra = 0.f; rb = 0.f;
+        const float *row = part + p * kGates + l;
+        float sa = 0.f, sb = 0.f;
+        int k = 0;
+        for (; k + kIn <= slices; k += kIn) {
+            float va[kIn], vb[kIn];
 #pragma unroll
-        for (int k = 0; k < kHidden; ++k) {
-            const float xk = __shfl_sync(0xffffffffu, h0, k);
-            const float hk = __shfl_sync(0xffffffffu, h1, k);
-            sa = fmaf(wih1a[k], xk, sa); sb = fmaf(wih1b[k], xk, sb);
-            ra = fmaf(whh1a[k], hk, ra); rb = fmaf(whh1b[k], hk, rb);
-        }
-        ga = (sa + bih1a) + (ra + bhh1a);
-        gb = (sb + bih1b) + (rb + bhh1b);
-        A = sigmoid_acc(ga);
-        Bv = lo ? tanhf(gb) : sigmoid_acc(gb);
-        ig = __shfl_sync(0xffffffffu, A, u); fg = __shfl_sync(0xffffffffu, A, u + 16);
-        gg = __shfl_sync(0xffffffffu, Bv, u); og = __shfl_sync(0xffffffffu, Bv, u + 16);
-        c1 = fg * c1 + ig * gg;
-        h1 = og * tanhf(c1);
-        // ---- Linear(16->1) + age scale
-        float y = lo ? wo * h1 : 0.f;
+            for (int j = 0; j < kIn; ++j) { va[j] = __ldcg(row + (k + j) * slice); vb[j] = __ldcg(row + (k + j) * slice + 32); }
 #pragma unroll
-        for (int off = 8; off >= 1; off >>= 1) y += __shfl_xor_sync(0xffffffffu, y, off);
-        if (l == 0) {
-            y = (y + bo) * age_scale(age[n_age == 1 ? 0 : t], coef);
-            out[t] = apply_sigmoid ? sigmoid_acc(y) : y;
+            for (int j = 0; j < kIn; ++j) { sa += va[j]; sb += vb[j]; }
         }
+        for (; k < slices; ++k) { sa += __ldcg(row + k * slice); sb += __ldcg(row + k * slice + 32); }
+        float *st = state + p * kGates;
+        SeqState s = {st[u], st[kHidden + u], st[2 * kHidden + u], st[3 * kHidden + u]};
+        seq_step(w, s, (sa + bih0a) + bhh0a, (sb + bih0b) + bhh0b, l, age + (n_age == 1 ? 0 : p), coef, apply_sigmoid, out + p);
+        if (l < kHidden) { st[u] = s.h0; st[kHidden + u] = s.c0; st[2 * kHidden + u] = s.h1; st[3 * kHidden + u] = s.c1; }
     }
 }
 
@@ -349,8 +342,7 @@ int launch_head(const Dims &d, const HeadWeights &hw, const float *feats, int64_
 }
 
 // launch_head of independent windows over a feature ring: window b's position k in ring[((head + k) mod cap) pitch + b]
-int launch_ring_head(const Dims &d, const HeadWeights &hw, const float *ring, int64_t pitch, int cap, int head, int64_t B,
-                     const float *age, int64_t n_age, int apply_sigmoid, float *out, float *gates_ws, float *partial_ws,
+int launch_ring_proj(const Dims &d, const HeadWeights &hw, const float *ring, int64_t pitch, int cap, int head, int64_t B, float *partial_ws,
                      cudaStream_t st, const char **err) {
     int ks_eff;
     const int kps = proj_split(d.L, choose_ksplit(d.L), &ks_eff);
@@ -358,6 +350,14 @@ int launch_ring_head(const Dims &d, const HeadWeights &hw, const float *ring, in
                                                                                     d.L, kps);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) { *err = cudaGetErrorString(e); return -1; }
+    return ks_eff;
+}
+
+int launch_ring_head(const Dims &d, const HeadWeights &hw, const float *ring, int64_t pitch, int cap, int head, int64_t B,
+                     const float *age, int64_t n_age, int apply_sigmoid, float *out, float *gates_ws, float *partial_ws,
+                     cudaStream_t st, const char **err) {
+    const int ks_eff = launch_ring_proj(d, hw, ring, pitch, cap, head, B, partial_ws, st, err);
+    if (ks_eff < 0) return -1;
     int n = launch_reduce_gates(partial_ws, ks_eff, B, hw, gates_ws, st, err);
     if (n < 0) return -1;
     n = launch_lstm_head(d, hw, gates_ws, B, age, n_age, B2CNN_MODE_INDEPENDENT, apply_sigmoid, out, st, err);
@@ -423,6 +423,17 @@ int launch_lstm_head(const Dims &d, const HeadWeights &hw, const float *gates, i
 int launch_sequence_segments(const Dims &d, const HeadWeights &hw, const float *gates, int64_t n_seg, int64_t seg_len, const float *age,
                              int64_t n_age, int apply_sigmoid, float *out, cudaStream_t st, const char **err) {
     head_sequence_kernel<<<(unsigned)n_seg, 32, 0, st>>>(gates, hw, age, n_age, d.age_coef, apply_sigmoid, out, seg_len);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) { *err = cudaGetErrorString(e); return -1; }
+    return 1;
+}
+
+// one LSTM step per live patient of a sequence-mode scorer from its range partials and state (slide_seq_step_kernel)
+int launch_seq_step(const Dims &d, const HeadWeights &hw, const float *partial, int slices, int64_t P, const float *age, int64_t n_age,
+                    int apply_sigmoid, float *out, float *state, const int64_t *seen, int64_t S, cudaStream_t st, const char **err) {
+    constexpr int64_t per_cta = (kSeqStepThreads / 32) * kSeqStepPerWarp;
+    slide_seq_step_kernel<<<(unsigned)((P + per_cta - 1) / per_cta), kSeqStepThreads, 0, st>>>(partial, slices, P, hw, age, n_age, d.age_coef,
+                                                                                            apply_sigmoid, out, state, seen, S, d.W);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) { *err = cudaGetErrorString(e); return -1; }
     return 1;

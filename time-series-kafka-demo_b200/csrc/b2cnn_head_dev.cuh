@@ -3,6 +3,7 @@
 // streaming kernel was built and removed: its registers spilled the streaming loop, see DESIGN.md).  bin/models.py:30-34 from the zero state:
 //   gates0[g] = (sum_k partial[k][b][g] + b_ih[g]) + b_hh[g]      slices summed in FIXED order
 //   layer 0, layer 1 (W_hh * h and f * c vanish but are kept as written), Linear(16 -> 1), age scale, optional sigmoid
+// and (seq_step, below) one step of the LSTM carried across windows, on a whole warp.
 #pragma once
 #include "b2cnn_internal.cuh"
 
@@ -77,6 +78,76 @@ __device__ __forceinline__ float head_window16(const float4 *__restrict__ row, i
     y += __ldg(hw.bo);
     y *= head_age_scale(age, coef);
     return apply_sigmoid ? sigmoid_acc(y) : y;
+}
+
+// ---- one step of the LSTM carried from window to window (sequence mode), one warp per sequence ----
+// Shared by head_sequence_kernel (a scan over consecutive rows) and slide_seq_step_kernel (one step per patient of a
+// sliding scorer from its stored state), so that both run the same instructions.  Lane l owns gate rows l and l + 32
+// of every weight matrix (registers); units' (h, c) are held twice, by lanes u and u + 16.
+struct SeqLaneWeights {
+    float whh0a[kHidden], whh0b[kHidden], wih1a[kHidden], wih1b[kHidden], whh1a[kHidden], whh1b[kHidden];
+    float bih1a, bih1b, bhh1a, bhh1b, wo, bo;
+};
+
+__device__ __forceinline__ void seq_load_weights(const HeadWeights &hw, int l, SeqLaneWeights &w) {
+#pragma unroll
+    for (int k = 0; k < kHidden; ++k) {
+        w.whh0a[k] = hw.whh0[l * kHidden + k]; w.whh0b[k] = hw.whh0[(l + 32) * kHidden + k];
+        w.wih1a[k] = hw.wih1[l * kHidden + k]; w.wih1b[k] = hw.wih1[(l + 32) * kHidden + k];
+        w.whh1a[k] = hw.whh1[l * kHidden + k]; w.whh1b[k] = hw.whh1[(l + 32) * kHidden + k];
+    }
+    w.bih1a = hw.bih1[l]; w.bih1b = hw.bih1[l + 32]; w.bhh1a = hw.bhh1[l]; w.bhh1b = hw.bhh1[l + 32];
+    w.wo = hw.wo[l & 15]; w.bo = hw.bo[0];
+}
+
+struct SeqState { float h0, c0, h1, c1; };   // lane l: unit l & 15
+
+// All 32 lanes call this together (full-mask shuffles).  ga, gb: the window's layer-0 pre-activations (W_ih x + b_ih)
+// + b_hh of gate rows l and l + 32.  Advances s by one window (bin/models.py:30); lane 0 then reads *age and writes
+// *out = (Linear(h1) + b) * relu(age coef + 1), or its sigmoid (models.py:31-34).
+__device__ __forceinline__ void seq_step(const SeqLaneWeights &w, SeqState &s, float ga, float gb, int l, const float *age, float coef,
+                                         int apply_sigmoid, float *out) {
+    const int u = l & 15;
+    const bool lo = l < 16;
+    // ---- layer 0: add W_hh h_{t-1}
+    float ra = 0.f, rb = 0.f;
+#pragma unroll
+    for (int k = 0; k < kHidden; ++k) {
+        const float hk = __shfl_sync(0xffffffffu, s.h0, k);
+        ra = fmaf(w.whh0a[k], hk, ra); rb = fmaf(w.whh0b[k], hk, rb);
+    }
+    ga += ra; gb += rb;
+    float A = sigmoid_acc(ga);                         // lanes <16: i ; lanes >=16: f
+    float Bv = lo ? tanhf(gb) : sigmoid_acc(gb);       // lanes <16: g ; lanes >=16: o
+    float ig = __shfl_sync(0xffffffffu, A, u), fg = __shfl_sync(0xffffffffu, A, u + 16);
+    float gg = __shfl_sync(0xffffffffu, Bv, u), og = __shfl_sync(0xffffffffu, Bv, u + 16);
+    s.c0 = fg * s.c0 + ig * gg;
+    s.h0 = og * tanhf(s.c0);
+    // ---- layer 1: input h0 (new), recurrent h1 (old)
+    float sa = 0.f, sb = 0.f; ra = 0.f; rb = 0.f;
+#pragma unroll
+    for (int k = 0; k < kHidden; ++k) {
+        const float xk = __shfl_sync(0xffffffffu, s.h0, k);
+        const float hk = __shfl_sync(0xffffffffu, s.h1, k);
+        sa = fmaf(w.wih1a[k], xk, sa); sb = fmaf(w.wih1b[k], xk, sb);
+        ra = fmaf(w.whh1a[k], hk, ra); rb = fmaf(w.whh1b[k], hk, rb);
+    }
+    ga = (sa + w.bih1a) + (ra + w.bhh1a);
+    gb = (sb + w.bih1b) + (rb + w.bhh1b);
+    A = sigmoid_acc(ga);
+    Bv = lo ? tanhf(gb) : sigmoid_acc(gb);
+    ig = __shfl_sync(0xffffffffu, A, u); fg = __shfl_sync(0xffffffffu, A, u + 16);
+    gg = __shfl_sync(0xffffffffu, Bv, u); og = __shfl_sync(0xffffffffu, Bv, u + 16);
+    s.c1 = fg * s.c1 + ig * gg;
+    s.h1 = og * tanhf(s.c1);
+    // ---- Linear(16->1) + age scale
+    float y = lo ? w.wo * s.h1 : 0.f;
+#pragma unroll
+    for (int off = 8; off >= 1; off >>= 1) y += __shfl_xor_sync(0xffffffffu, y, off);
+    if (l == 0) {
+        y = (y + w.bo) * head_age_scale(*age, coef);
+        *out = apply_sigmoid ? sigmoid_acc(y) : y;
+    }
 }
 
 }  // namespace b2cnn

@@ -185,6 +185,11 @@ int launch_lstm_head(const Dims &d, const HeadWeights &hw, const float *gates, i
 // seg_len) and out, each scanned from the zero state; launch_lstm_head's sequence mode is one segment of B rows
 int launch_sequence_segments(const Dims &d, const HeadWeights &hw, const float *gates, int64_t n_seg, int64_t seg_len, const float *age,
                              int64_t n_age, int apply_sigmoid, float *out, cudaStream_t st, const char **err);
+// a sequence-mode sliding scorer's head: for every live patient p (all with seen == nullptr, else seen[p] >= 0 &&
+// seen[p] + S >= d.W, the counts before the push advances them), one LSTM step from state[p] [64] = h0 | c0 | h1 | c1,
+// its layer-0 gates summed from partial [slices][P][64] as launch_reduce_gates does; out[p] and state[p] written
+int launch_seq_step(const Dims &d, const HeadWeights &hw, const float *partial, int slices, int64_t P, const float *age, int64_t n_age,
+                    int apply_sigmoid, float *out, float *state, const int64_t *seen, int64_t S, cudaStream_t st, const char **err);
 
 int launch_reduce_lstm_head(const Dims &d, const HeadWeights &hw, const float *partial, int slices, int64_t B,
                             const float *age, int64_t n_age, int apply_sigmoid, float *out, cudaStream_t st, const char **err,
@@ -198,6 +203,9 @@ int proj_slices(int L);       // split-K slices launch_head's projection writes 
 // ring's); the same tiles and summation order as launch_head
 int launch_ring_head(const Dims &d, const HeadWeights &hw, const float *ring, int64_t pitch, int cap, int head, int64_t B,
                      const float *age, int64_t n_age, int apply_sigmoid, float *out, float *gates_ws, float *partial_ws,
+                     cudaStream_t st, const char **err);
+// launch_ring_head's projection alone: partial_ws [slices][B][64]; returns slices (-1 on error)
+int launch_ring_proj(const Dims &d, const HeadWeights &hw, const float *ring, int64_t pitch, int cap, int head, int64_t B, float *partial_ws,
                      cudaStream_t st, const char **err);
 
 // launch_head of the n_w windows of each whole recording (b2cnn_record.cu, b2cnn_score_record, generic path): row b =

@@ -22,6 +22,8 @@
 //     partial[range][P][64]; then the head kernel of the independent forward sums the ranges in fixed order and runs
 //     the LSTM cells, Linear, age scale and sigmoid.  Extra heads (b2cnn_slide_set_heads_ex) may have a shorter window
 //     W_k ending at nS: window positions d .. L - 1 of the scorer's, d = (W - W_k) / F, with their own ranges.
+//     In sequence mode (slide_create with B2CNN_MODE_SEQUENCE) slide_seq_step_kernel takes the head's place: one LSTM
+//     step per live patient from its state in `lstm`, carried from push to push (utils.run_model over its windows).
 //
 // Per-patient lifecycle (b2cnn_slide_admit / _discharge): seen[p] counts patient p's samples since its admission (-1:
 // discharged); its window after a push is the last W samples of (history | pushes since admission), defined once
@@ -84,6 +86,9 @@ struct Slide {
     bool lifecycle = false;          // set by the first admit / discharge since the last reset
     int64_t *seen = nullptr;         // [P] on the device: samples since admission, -1: discharged (while lifecycle)
     std::vector<int64_t> seen_h;     // its host mirror, equal to it in stream order
+    int mode = B2CNN_MODE_INDEPENDENT;   // or B2CNN_MODE_SEQUENCE: each patient's LSTM state carried from push to push
+    float *lstm = nullptr;           // sequence mode: [P][64] fp32 on the device, h0 | c0 | h1 | c1 of 16 units each
+    int *lidx = nullptr;             // sequence mode: [P] device indices of a discharge's patients (their rows zeroed)
     std::vector<SlideHead> heads;    // extra heads, rows 1.. of a push with heads
 };
 
@@ -356,6 +361,14 @@ __global__ void slide_live_kernel(int64_t *__restrict__ seen, int P, int64_t adv
     for (int64_t j = blockIdx.y; j < len; j += gridDim.y) x[b * len + j] = __int_as_float(0x7fc00000);
 }
 
+// rows idx[j] (j < k) of dst [P][ct] = 0: the LSTM state of a sequence-mode scorer's admitted or discharged patients
+__global__ void slide_zero_rows_kernel(float *__restrict__ dst, const int *__restrict__ idx, int64_t k, int64_t ct) {
+    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= k * ct) return;
+    const int64_t j = e / ct;
+    dst[(int64_t)idx[j] * ct + (e - j * ct)] = 0.f;
+}
+
 // out[r][P] = NaN for every row r with bit r of `rows` set (blockIdx.y = r): the rows of a push with heads whose window
 // no patient has complete yet (a scorer without lifecycle calls; with them slide_live_kernel masks those rows whole)
 __global__ void slide_nan_rows_kernel(float *__restrict__ out, int P, unsigned rows) {
@@ -529,10 +542,13 @@ static int push_features_generic(Slide *s, const ConvWeights &cw, const void *x,
                       s->ring_pitch, s->d.L, st, err);
 }
 
-int slide_create(const Dims &d, const TcState &tc, int path, int n_patients, int stride, int dtype, int device, int num_sms, Slide **out,
-                 const char **err) {
+int slide_create(const Dims &d, const TcState &tc, int path, int mode, int n_patients, int stride, int dtype, int device, int num_sms,
+                 Slide **out, const char **err) {
     *out = nullptr;
     const bool tcp = path == B2CNN_PATH_TENSORCORE;
+    if (mode != B2CNN_MODE_INDEPENDENT && mode != B2CNN_MODE_SEQUENCE) {
+        *err = "mode must be B2CNN_MODE_INDEPENDENT (0) or B2CNN_MODE_SEQUENCE (1)"; return B2CNN_EINVAL;
+    }
     if (dtype != B2CNN_DTYPE_F32 && dtype != B2CNN_DTYPE_BF16) { *err = "dtype must be f32 (0) or bf16 (1)"; return B2CNN_EINVAL; }
     if (n_patients < 1 || n_patients > (1 << 24)) { *err = "n_patients out of range"; return B2CNN_EINVAL; }
     if (stride < 1 || stride > d.W) { *err = "stride must be in [1, window]"; return B2CNN_EINVAL; }
@@ -570,6 +586,10 @@ int slide_create(const Dims &d, const TcState &tc, int path, int n_patients, int
                   cudaSuccess &&
               cudaMalloc(&s->stage, (size_t)(P * d.C * s->Sp * esz)) == cudaSuccess &&
               cudaMalloc(&s->seen, sizeof(int64_t) * (size_t)P) == cudaSuccess;
+    s->mode = mode;
+    if (ok && mode == B2CNN_MODE_SEQUENCE)
+        ok = cudaMalloc(&s->lstm, sizeof(float) * (size_t)P * kGates) == cudaSuccess &&
+             cudaMalloc(&s->lidx, sizeof(int) * (size_t)P) == cudaSuccess;
     if (!ok) { (void)cudaGetLastError(); slide_destroy(s); *err = "cudaMalloc(scorer state)"; return B2CNN_ECUDA; }
     *out = s;
     return B2CNN_OK;
@@ -578,7 +598,7 @@ int slide_create(const Dims &d, const TcState &tc, int path, int n_patients, int
 void slide_destroy(Slide *s) {
     if (!s) return;
     cudaFree(s->ring); cudaFree(s->tail); cudaFree(s->partial); cudaFree(s->gates); cudaFree(s->flags); cudaFree(s->stage);
-    cudaFree(s->seen);
+    cudaFree(s->seen); cudaFree(s->lstm); cudaFree(s->lidx);
     for (SlideHead &hd : s->heads) cudaFree(hd.mem);
     delete s;
 }
@@ -586,12 +606,24 @@ void slide_destroy(Slide *s) {
 int slide_device(const Slide *s) { return s->device; }
 int slide_dtype(const Slide *s) { return s->dtype; }
 int slide_path(const Slide *s) { return s->path; }
+int slide_mode(const Slide *s) { return s->mode; }
 
 int slide_reset(Slide *s, cudaStream_t st, const char **err) {
     s->n = 0; s->g_done = -1; s->tail_cur = 0; s->lifecycle = false;
     if (cudaMemsetAsync(s->tail, 0, sizeof(float) * (size_t)2 * s->P * s->d.C * s->T, st) != cudaSuccess) {
         *err = "memset tail"; return B2CNN_ECUDA;
     }
+    if (s->lstm && cudaMemsetAsync(s->lstm, 0, sizeof(float) * (size_t)s->P * kGates, st) != cudaSuccess) {
+        *err = "memset LSTM state"; return B2CNN_ECUDA;
+    }
+    return B2CNN_OK;
+}
+
+// a sequence-mode scorer: the LSTM state rows of the k patients whose device indices are idx = 0 (else nothing)
+static int zero_lstm_rows(const Slide &s, const int *idx, int64_t k, cudaStream_t st, const char **err) {
+    if (!s.lstm || k == 0) return B2CNN_OK;
+    slide_zero_rows_kernel<<<(unsigned)((k * kGates + 255) / 256), 256, 0, st>>>(s.lstm, idx, k, kGates);
+    if (cudaGetLastError() != cudaSuccess) { *err = "LSTM state launch"; return B2CNN_ECUDA; }
     return B2CNN_OK;
 }
 
@@ -701,10 +733,20 @@ static int score_windows(Slide *s, const HeadWeights &hw, const TcState *tc, con
         if (ev && cudaEventRecord(ev[2], st) != cudaSuccess) { *err = "cudaEventRecord"; return B2CNN_ECUDA; }
         return B2CNN_OK;
     }
+    // sequence mode (no heads): row 0's head is one LSTM step per live patient from its state, before seen advances
+    const bool seq = s->mode == B2CNN_MODE_SEQUENCE;
+    const int64_t *seen_now = s->lifecycle ? s->seen : nullptr;
     if (!tc) {
         // each row: the same kernels over the same ring with its own W_ih^T, LSTM, Linear and age coefficient
         for (int r = 0; r < rows; ++r) {
             if (!((live >> r) & 1u)) continue;
+            if (r == 0 && seq) {
+                const int slices = launch_ring_proj(d, hw, s->ring, s->ring_pitch, d.L, row[0].head, P, s->partial, st, err);
+                if (slices < 0 ||
+                    launch_seq_step(d, hw, s->partial, slices, P, age, n_age, apply_sigmoid, out, s->lstm, seen_now, S, st, err) < 0)
+                    return B2CNN_ECUDA;
+                continue;
+            }
             if (launch_ring_head(row[r].d, *row[r].hw, s->ring, s->ring_pitch, d.L, row[r].head, P, age, n_age, apply_sigmoid, out + r * P,
                                  s->gates, s->partial, st, err) < 0)
                 return B2CNN_ECUDA;
@@ -751,6 +793,11 @@ static int score_windows(Slide *s, const HeadWeights &hw, const TcState *tc, con
         }
         for (int r = 0; r < rows; ++r) {
             if (!((live >> r) & 1u)) continue;
+            if (r == 0 && seq) {
+                if (launch_seq_step(d, hw, s->partial, s->ranges, P, age, n_age, apply_sigmoid, out, s->lstm, seen_now, S, st, err) < 0)
+                    return B2CNN_ECUDA;
+                continue;
+            }
             if (launch_reduce_lstm_head(row[r].d, *row[r].hw, row[r].partial, row[r].ranges, P, age, n_age, apply_sigmoid, out + r * P, st,
                                         err) < 0)
                 return B2CNN_ECUDA;
@@ -899,6 +946,7 @@ int slide_admit(Slide *s, const ConvWeights &cw, const TcState &tc, const int *p
         slide_seed_tail_kernel<float><<<(unsigned)blocks, 256, 0, st>>>(reinterpret_cast<const float *>(hist), pitch, H, idx, (int)k, d.C,
                                                                         s->T, tail);
     if (cudaGetLastError() != cudaSuccess) { *err = "tail launch"; return B2CNN_ECUDA; }
+    if ((rc = zero_lstm_rows(*s, idx, k, st, err)) != B2CNN_OK) return rc;   // sequence mode: the LSTM starts again
     std::vector<int64_t> next = next_seen(*s, patients, k, H);
     if ((rc = commit_seen(s, next, st, err)) != B2CNN_OK) return rc;
     // features from the history's last complete one on are seam features of the next push, for every patient (before
@@ -908,8 +956,14 @@ int slide_admit(Slide *s, const ConvWeights &cw, const TcState &tc, const int *p
 }
 
 int slide_discharge(Slide *s, const int *patients, int64_t k, cudaStream_t st, const char **err) {
-    const int rc = check_patients(*s, patients, k, err);
+    int rc = check_patients(*s, patients, k, err);
     if (rc != B2CNN_OK || k == 0) return rc;
+    if (s->lstm) {
+        if (cudaMemcpyAsync(s->lidx, patients, sizeof(int) * (size_t)k, cudaMemcpyHostToDevice, st) != cudaSuccess) {
+            *err = "copy of the patient indices"; return B2CNN_ECUDA;
+        }
+        if ((rc = zero_lstm_rows(*s, s->lidx, k, st, err)) != B2CNN_OK) return rc;
+    }
     std::vector<int64_t> next = next_seen(*s, patients, k, -1);
     return commit_seen(s, next, st, err);
 }
@@ -1096,10 +1150,12 @@ int64_t slide_state_workspace_bytes(const Slide *s, int64_t k) {
     return (int64_t)al256(sizeof(int) * (size_t)k);
 }
 
-// the indices into the workspace, then the feature tile kernel and the tail kernel in one direction
+// the indices into the workspace, then the feature tile kernel and the tail kernel in one direction; a sequence-mode
+// scorer's LSTM state rows [k][64] too: exported into dst_lstm when it is given, imported from src_lstm, or zeroed (an
+// import without them starts the patients' LSTM again, as an admission does)
 template <bool kExport>
 static int launch_state(const Slide &s, const int *patients, int64_t k, const float *src_rows, float *dst_rows, const float *src_tails,
-                        float *dst_tails, void *ws, cudaStream_t st, const char **err) {
+                        float *dst_tails, const float *src_lstm, float *dst_lstm, void *ws, cudaStream_t st, const char **err) {
     int *idx = static_cast<int *>(ws);
     if (cudaMemcpyAsync(idx, patients, sizeof(int) * (size_t)k, cudaMemcpyHostToDevice, st) != cudaSuccess) {
         *err = "copy of the patient indices"; return B2CNN_ECUDA;
@@ -1114,13 +1170,22 @@ static int launch_state(const Slide &s, const int *patients, int64_t k, const fl
     if constexpr (kExport) slide_state_tail_kernel<true><<<(unsigned)blocks, 256, 0, st>>>(tail, dst_tails, idx, k, ct);
     else slide_state_tail_kernel<false><<<(unsigned)blocks, 256, 0, st>>>(src_tails, tail, idx, k, ct);
     if (cudaGetLastError() != cudaSuccess) { *err = "state tail launch"; return B2CNN_ECUDA; }
+    const unsigned lblocks = (unsigned)((k * kGates + 255) / 256);
+    if constexpr (kExport) {
+        if (dst_lstm) slide_state_tail_kernel<true><<<lblocks, 256, 0, st>>>(s.lstm, dst_lstm, idx, k, kGates);
+    } else {
+        if (s.lstm && src_lstm) slide_state_tail_kernel<false><<<lblocks, 256, 0, st>>>(src_lstm, s.lstm, idx, k, kGates);
+        else if (zero_lstm_rows(s, idx, k, st, err) != B2CNN_OK) return B2CNN_ECUDA;
+    }
+    if (cudaGetLastError() != cudaSuccess) { *err = "LSTM state launch"; return B2CNN_ECUDA; }
     return B2CNN_OK;
 }
 
 static int check_state_args(const Slide &s, const int *patients, int64_t k, const void *feats, const void *tails, const void *seen,
-                            void *ws, int64_t ws_bytes, const char **err) {
+                            const void *lstm, void *ws, int64_t ws_bytes, const char **err) {
     const int rc = check_patients(s, patients, k, err);
     if (rc != B2CNN_OK) return rc;
+    if (lstm && s.mode != B2CNN_MODE_SEQUENCE) { *err = "an LSTM state array for an independent-mode scorer"; return B2CNN_EINVAL; }
     if (k > 0 && (!feats || !tails || !seen)) { *err = "null feature, tail or count array with patients listed"; return B2CNN_EINVAL; }
     if (k > 0 && (!ws || ws_bytes < slide_state_workspace_bytes(&s, k))) {
         *err = "workspace missing or smaller than b2cnn_slide_state_workspace_bytes()"; return B2CNN_ESTATE;
@@ -1129,10 +1194,11 @@ static int check_state_args(const Slide &s, const int *patients, int64_t k, cons
 }
 
 int slide_export(const Slide *s, const ConvWeights &cw, const int *patients, int64_t k, float *feats, float *tails, int64_t *seen_host,
-                 b2cnn_slide_state_header *hdr, void *ws, int64_t ws_bytes, cudaStream_t st, const char **err) {
-    int rc = check_state_args(*s, patients, k, feats, tails, seen_host, ws, ws_bytes, err);
+                 float *lstm, b2cnn_slide_state_header *hdr, void *ws, int64_t ws_bytes, cudaStream_t st, const char **err) {
+    int rc = check_state_args(*s, patients, k, feats, tails, seen_host, lstm, ws, ws_bytes, err);
     if (rc != B2CNN_OK) return rc;
-    if (k > 0 && (rc = launch_state<true>(*s, patients, k, nullptr, feats, nullptr, tails, ws, st, err)) != B2CNN_OK) return rc;
+    if (k > 0 && (rc = launch_state<true>(*s, patients, k, nullptr, feats, nullptr, tails, nullptr, lstm, ws, st, err)) != B2CNN_OK)
+        return rc;
     // the host mirror: the counts need no device read (before any lifecycle call every patient has seen n S samples)
     for (int64_t j = 0; j < k; ++j) seen_host[j] = s->lifecycle ? s->seen_h[patients[j]] : s->n * s->S;
     slide_describe_state(s, cw, hdr);
@@ -1140,7 +1206,8 @@ int slide_export(const Slide *s, const ConvWeights &cw, const int *patients, int
 }
 
 int slide_import(Slide *s, const ConvWeights &cw, const int *patients, int64_t k, const b2cnn_slide_state_header &hdr, const float *feats,
-                 const float *tails, const int64_t *seen_host, void *ws, int64_t ws_bytes, cudaStream_t st, const char **err) {
+                 const float *tails, const int64_t *seen_host, const float *lstm, void *ws, int64_t ws_bytes, cudaStream_t st,
+                 const char **err) {
     if (hdr.magic != B2CNN_SLIDE_STATE_MAGIC || hdr.version != B2CNN_SLIDE_STATE_VERSION) {
         *err = "not a scorer state header of this version (magic, version)"; return B2CNN_EINVAL;
     }
@@ -1155,12 +1222,12 @@ int slide_import(Slide *s, const ConvWeights &cw, const int *patients, int64_t k
         *err = "the state's features come from other front-end weights than the handle's (conv / affine digest differs)";
         return B2CNN_ESTATE;
     }
-    int rc = check_state_args(*s, patients, k, feats, tails, seen_host, ws, ws_bytes, err);
+    int rc = check_state_args(*s, patients, k, feats, tails, seen_host, lstm, ws, ws_bytes, err);
     if (rc != B2CNN_OK) return rc;
     for (int64_t j = 0; j < k; ++j)
         if (seen_host[j] < -1) { *err = "a sample count below -1"; return B2CNN_EINVAL; }
     if (k == 0) return B2CNN_OK;
-    if ((rc = launch_state<false>(*s, patients, k, feats, nullptr, tails, nullptr, ws, st, err)) != B2CNN_OK) return rc;
+    if ((rc = launch_state<false>(*s, patients, k, feats, nullptr, tails, nullptr, lstm, nullptr, ws, st, err)) != B2CNN_OK) return rc;
     std::vector<int64_t> next = next_seen(*s, patients, 0, 0);
     for (int64_t j = 0; j < k; ++j) next[patients[j]] = seen_host[j];
     if ((rc = commit_seen(s, next, st, err)) != B2CNN_OK) return rc;

@@ -9,9 +9,12 @@ struct Slide;
 // B2CNN_PATH_TENSORCORE (the geometries `tc` holds in its streaming kernels, else B2CNN_EARCH) or B2CNN_PATH_GENERIC
 // (exact CUDA-core kernels for any geometry b2cnn_create accepts; B2CNN_EARCH, before allocating anything, where the
 // generic front end's tile does not fit shared memory, with num_sms sizing its grid); stride % pool_s^2 == 0
-int slide_create(const Dims &d, const TcState &tc, int path, int n_patients, int stride, int dtype, int device, int num_sms, Slide **out,
-                 const char **err);
+// mode: B2CNN_MODE_INDEPENDENT, or B2CNN_MODE_SEQUENCE (each patient's LSTM state [64] fp32 on the device, carried
+// from push to push; zeroed at reset, admit, discharge and an import without state); anything else B2CNN_EINVAL
+int slide_create(const Dims &d, const TcState &tc, int path, int mode, int n_patients, int stride, int dtype, int device, int num_sms,
+                 Slide **out, const char **err);
 int slide_path(const Slide *s);   // B2CNN_PATH_TENSORCORE or B2CNN_PATH_GENERIC
+int slide_mode(const Slide *s);   // B2CNN_MODE_INDEPENDENT or B2CNN_MODE_SEQUENCE
 void slide_destroy(Slide *s);
 int slide_device(const Slide *s);
 int slide_reset(Slide *s, cudaStream_t st, const char **err);
@@ -42,12 +45,15 @@ int slide_admit(Slide *s, const ConvWeights &cw, const TcState &tc, const int *p
 int slide_discharge(Slide *s, const int *patients, int64_t k, cudaStream_t st, const char **err);
 int slide_samples_seen(Slide *s, int64_t *out, cudaStream_t st, const char **err);
 int slide_dtype(const Slide *s);
-// export / import of patients (b2cnn_slide_export / _import): `cw` the handle's current conv weights (the digest)
+// export / import of patients (b2cnn_slide_export / _import): `cw` the handle's current conv weights (the digest);
+// lstm: nullptr or [k][64] device fp32 LSTM state rows (sequence mode only, else B2CNN_EINVAL); an import into a
+// sequence-mode scorer without them zeroes the patients' rows
 void slide_describe_state(const Slide *s, const ConvWeights &cw, b2cnn_slide_state_header *out);
 int64_t slide_state_workspace_bytes(const Slide *s, int64_t k);
 int slide_export(const Slide *s, const ConvWeights &cw, const int *patients, int64_t k, float *feats, float *tails, int64_t *seen_host,
-                 b2cnn_slide_state_header *hdr, void *ws, int64_t ws_bytes, cudaStream_t st, const char **err);
+                 float *lstm, b2cnn_slide_state_header *hdr, void *ws, int64_t ws_bytes, cudaStream_t st, const char **err);
 int slide_import(Slide *s, const ConvWeights &cw, const int *patients, int64_t k, const b2cnn_slide_state_header &hdr, const float *feats,
-                 const float *tails, const int64_t *seen_host, void *ws, int64_t ws_bytes, cudaStream_t st, const char **err);
+                 const float *tails, const int64_t *seen_host, const float *lstm, void *ws, int64_t ws_bytes, cudaStream_t st,
+                 const char **err);
 
 }  // namespace b2cnn

@@ -32,6 +32,20 @@ With ``shorter_windows=True`` a head may have a shorter window than the scorer's
     scorer = SlidingScorer(m600, n_patients=P, stride=7500)          # W = 75000: 600 s at 125 Hz
     scorer.set_heads([m60, m300], shorter_windows=True)              # W_k = 7500 and 37500, the same conv weights
     out = scorer.push(samples, age=ages, heads=True)                 # [3, P] once the 60 s window is complete
+
+``mode="sequence"`` scores every patient as ``utils.run_model`` scores a recording, live: the LSTM runs along the
+patient's windows, its state (h and c of both layers, 256 bytes per patient) carried on the device from one scored
+window to the next, so each push costs one LSTM step per patient however long the stay::
+
+    scorer = SlidingScorer(model, n_patients=P, stride=7500, mode="sequence")
+    for samples in triggers:
+        logits = scorer.push(samples, age=ages)                      # model(windows since admission, age)[-1] per patient
+
+For a patient whose stream is ``s`` (history first), with ``s0`` its ``samples_seen`` at the first push with
+``samples_seen >= W`` and ``o = s0 - W``, the push at ``samples_seen == s0 + j * stride`` returns
+``predict_record(s[:, :, o : s0 + j * stride], stride, age, mode="sequence")[:, j]`` -- bit for bit on the generic
+path.  The state starts at zero at ``reset()``, ``admit()`` and ``discharge()``; a NaN sample poisons its patient's
+state (NaN at every later push, as in ``run_model``) until ``admit()`` starts it again.
 """
 from __future__ import annotations
 
@@ -63,18 +77,33 @@ class SlidingScorer:
     ``push(..., heads=True)`` returns ``Tensor[1 + K, P]``, row 0 what ``push`` returns and row i ``heads[i - 1]``'s
     logits of the same windows.  ``heads`` is the tuple attached.  ``set_heads(models, shorter_windows=True)`` also
     takes heads whose window ``W_k <= W`` ends where the scorer's does (``W - W_k`` a multiple of the feature stride);
-    ``head_windows`` lists each row's window."""
+    ``head_windows`` lists each row's window.
+
+    ``mode``: ``"independent"`` (the default) scores every window from the zero LSTM state, the reference's per-window
+    call (bin/predictStream.py:157).  ``"sequence"`` carries each patient's LSTM state from its previous scored window,
+    as ``model(windows, age)`` with the windows as the batch (bin/models.py:29-30, ``utils.run_model``) and as
+    ``B200Trainer`` trains by default: ``push`` returns, for patient p, the output ``model(windows_p, age)`` gives for
+    its last row, ``windows_p`` all of p's windows scored since its admission (or ``reset()``), in order.  The state
+    is zeroed at ``reset()``, ``admit()`` and ``discharge()`` and does not advance while p's score is NaN for an
+    incomplete window; the age scales the output only.  A sequence scorer takes no extra heads.  ``scorer.mode``
+    tells which one runs."""
 
     ARCH_FIELDS = ("in_channels", "window", "k1", "k2", "pool_k", "pool_s", "act", "affine", "l_out", "c_mid", "hidden", "layers")
 
     PATHS = {"tensorcore": capi.PATH_TENSORCORE, "generic": capi.PATH_GENERIC, "auto": capi.PATH_AUTO}
+    MODES = {"independent": capi.MODE_INDEPENDENT, "sequence": capi.MODE_SEQUENCE}
+    LSTM_STATE = (2, 2, 16)                                             # [layer][h | c][unit] per patient
+    mode = "independent"                                                # the instance's, set at construction
     STATE_HEADER = tuple(n for n, _ in capi.SlideStateHeader._fields_)
 
-    def __init__(self, model, n_patients: int, stride: int, dtype=torch.bfloat16, path: str = "tensorcore"):
+    def __init__(self, model, n_patients: int, stride: int, dtype=torch.bfloat16, path: str = "tensorcore",
+                 mode: str = "independent"):
         if dtype not in (torch.bfloat16, torch.float32):
             raise ValueError("dtype must be torch.bfloat16 or torch.float32")
         if path not in self.PATHS:
             raise ValueError(f"path must be one of {sorted(self.PATHS)}, got {path!r}")
+        if not isinstance(mode, str) or mode not in self.MODES:
+            raise ValueError(f"mode must be one of {sorted(self.MODES)}, got {mode!r}")
         n_patients, stride = int(n_patients), int(stride)
         if n_patients < 1:
             raise ValueError(f"n_patients must be >= 1, got {n_patients}")
@@ -89,12 +118,16 @@ class SlidingScorer:
         self.device = model._handle_device
         s = ctypes.c_void_p()
         with torch.cuda.device(self.device):
-            if path == "tensorcore":
+            if mode == "sequence":
+                capi.check(self._lib.b2cnn_slide_create_ex(h, n_patients, stride, self._dt(), self.PATHS[path], capi.MODE_SEQUENCE,
+                                                           ctypes.byref(s)), "b2cnn_slide_create_ex")
+            elif path == "tensorcore":
                 capi.check(self._lib.b2cnn_slide_create(h, n_patients, stride, self._dt(), ctypes.byref(s)), "b2cnn_slide_create")
             else:
                 capi.check(self._lib.b2cnn_slide_create_path(h, n_patients, stride, self._dt(), self.PATHS[path], ctypes.byref(s)),
                            "b2cnn_slide_create_path")
         self._s = s
+        self.mode = mode
         self._heads = ()
         self.path = "generic" if self._lib.b2cnn_slide_path(s) == capi.PATH_GENERIC else "tensorcore"
         self.window_index = -1
@@ -246,6 +279,8 @@ class SlidingScorer:
         ones of the stored window, and its row equals what a scorer of that model at its own window and the same
         stride computes from the same pushes, NaN for a patient whose ``samples_seen`` is below its window."""
         models = self.check_heads(models, shorter_windows)
+        if models and self.mode == "sequence":
+            raise ValueError("a sequence-mode SlidingScorer takes no extra heads")
         self._handle()
         hs = [m._ensure_handle()[1].value for m in models]
         arr = (ctypes.c_void_p * max(len(hs), 1))(*hs)
@@ -265,7 +300,10 @@ class SlidingScorer:
         first window fills.  After ``admit`` / ``discharge``: NaN for every patient whose window is not complete
         (``samples_seen < W``; a discharged patient's samples are ignored), ``None`` when no patient's window is.
         ``heads=True``: ``Tensor[1 + K, P]`` (or ``None`` as above), row 0 exactly what ``heads=False`` returns, row i
-        the scores of ``heads[i - 1]`` on the same windows and ages, NaN where row 0 is.  With heads of shorter windows
+        the scores of ``heads[i - 1]`` on the same windows and ages, NaN where row 0 is.  In sequence mode each
+        patient's row is ``model(windows, age)``'s last row over its windows since admission (the class docstring
+        states the identity with ``predict_record(mode="sequence")``), and its state advances only where the result
+        is not NaN for an incomplete window.  With heads of shorter windows
         (``set_heads(..., shorter_windows=True)``) row i is NaN where that row's own window ``head_windows[i]`` is
         incomplete, and the result is returned as soon as any row has a complete window for one patient (row 0 may
         then be all NaN)."""
@@ -365,7 +403,8 @@ class SlidingScorer:
         a complete window has no NaN mask here), ``tail`` [k, C, T] fp32 (the stream's last T samples per channel),
         both on the scorer's device, ``seen`` [k] CPU int64 (``samples_seen``), and the header fields (path, dtype,
         C, W, L, feature stride F, T and a digest of the conv weights).  Changes nothing in the scorer.
-        ``window_index`` is not part of it: it counts this scorer's own pushes."""
+        ``window_index`` is not part of it: it counts this scorer's own pushes.  A sequence-mode scorer adds ``lstm``
+        [k, 2, 2, 16] fp32 on its device, each patient's LSTM state as [layer][h | c][unit]."""
         idx = self.check_patients(patients)
         k = len(idx)
         self._handle()
@@ -378,16 +417,29 @@ class SlidingScorer:
         with torch.cuda.device(self.device):
             nbytes = int(self._lib.b2cnn_slide_state_workspace_bytes(self._s, k))
             ws = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=self.device)
-            capi.check(self._lib.b2cnn_slide_export(self._s, arr, k, feats.data_ptr(), tail.data_ptr(), seen.data_ptr(), ctypes.byref(hdr),
-                                                    ws.data_ptr(), nbytes, torch.cuda.current_stream().cuda_stream), "b2cnn_slide_export")
+            st = torch.cuda.current_stream().cuda_stream
+            if self.mode == "sequence":
+                lstm = torch.empty((k,) + self.LSTM_STATE, dtype=torch.float32, device=self.device)
+                capi.check(self._lib.b2cnn_slide_export_ex(self._s, arr, k, feats.data_ptr(), tail.data_ptr(), seen.data_ptr(),
+                                                           lstm.data_ptr(), ctypes.byref(hdr), ws.data_ptr(), nbytes, st),
+                           "b2cnn_slide_export_ex")
+            else:
+                capi.check(self._lib.b2cnn_slide_export(self._s, arr, k, feats.data_ptr(), tail.data_ptr(), seen.data_ptr(), ctypes.byref(hdr),
+                                                        ws.data_ptr(), nbytes, st), "b2cnn_slide_export")
         state = {"features": feats, "tail": tail, "seen": seen}
+        if self.mode == "sequence":
+            state["lstm"] = lstm
         state.update({n: int(getattr(hdr, n)) for n in self.STATE_HEADER})
         return state
 
     def check_state(self, state, k: int):
-        """Validates a state of k patients (``export``'s dict) against this scorer; returns (features, tail, seen)."""
+        """Validates a state of k patients (``export``'s dict) against this scorer; returns (features, tail, seen).  The
+        state holds ``lstm`` exactly when the scorer is in sequence mode."""
         if not isinstance(state, dict):
             raise ValueError(f"expected the dict of SlidingScorer.export(), got {type(state).__name__}")
+        if ("lstm" in state) != (self.mode == "sequence"):
+            raise ValueError(f"the state was exported in another mode than this scorer's ({self.mode}): it "
+                             + ("lacks" if self.mode == "sequence" else "holds") + " 'lstm'")
         missing = [n for n in ("features", "tail", "seen") + self.STATE_HEADER if n not in state]
         if missing:
             raise ValueError(f"the state lacks {missing}")
@@ -404,6 +456,8 @@ class SlidingScorer:
                              + ", ".join(f"{n}: {a}" for n, a in bad.items()))
         L, T = self._state_fields["lstm_input"], self._state_fields["tail_len"]
         want = {"features": ((k, L), torch.float32), "tail": ((k, self.channels, T), torch.float32), "seen": ((k,), torch.int64)}
+        if self.mode == "sequence":
+            want["lstm"] = ((k,) + self.LSTM_STATE, torch.float32)
         for n, (shape, dtype) in want.items():
             t = state[n]
             if not torch.is_tensor(t) or tuple(t.shape) != shape or t.dtype != dtype:
@@ -421,10 +475,13 @@ class SlidingScorer:
         a patient with ``samples_seen >= W`` is in ``features()`` at once and scored from the next push on, exactly as
         the exporting scorer would have scored it on the same samples; one exported discharged stays discharged.  The
         state must come from a scorer of the same path, dtype, C, W and conv weights (the LSTM and head weights may
-        differ: change them, ``reset()``, then restore).  Errors leave the scorer unchanged."""
+        differ: change them, ``reset()``, then restore).  A sequence-mode scorer takes only a sequence-mode state (with
+        ``lstm``), from which the patients' LSTM continues; an independent one only an independent state.  Errors
+        leave the scorer unchanged."""
         idx = self.check_patients(patients)
         k = len(idx)
         feats, tail, seen = self.check_state(state, k)
+        lstm = state.get("lstm")
         self._handle()
         feats = feats.to(self.device).contiguous()
         tail = tail.to(self.device).contiguous()
@@ -434,5 +491,12 @@ class SlidingScorer:
         with torch.cuda.device(self.device):
             nbytes = int(self._lib.b2cnn_slide_state_workspace_bytes(self._s, k))
             ws = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=self.device)
-            capi.check(self._lib.b2cnn_slide_import(self._s, arr, k, ctypes.byref(hdr), feats.data_ptr(), tail.data_ptr(), seen.data_ptr(),
-                                                    ws.data_ptr(), nbytes, torch.cuda.current_stream().cuda_stream), "b2cnn_slide_import")
+            st = torch.cuda.current_stream().cuda_stream
+            if lstm is not None:
+                lstm = lstm.to(self.device).contiguous()
+                capi.check(self._lib.b2cnn_slide_import_ex(self._s, arr, k, ctypes.byref(hdr), feats.data_ptr(), tail.data_ptr(),
+                                                           seen.data_ptr(), lstm.data_ptr(), ws.data_ptr(), nbytes, st),
+                           "b2cnn_slide_import_ex")
+            else:
+                capi.check(self._lib.b2cnn_slide_import(self._s, arr, k, ctypes.byref(hdr), feats.data_ptr(), tail.data_ptr(), seen.data_ptr(),
+                                                        ws.data_ptr(), nbytes, st), "b2cnn_slide_import")
