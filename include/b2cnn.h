@@ -114,6 +114,20 @@ int b2cnn_forward_pitched(b2cnn_handle *h, const void *x, int dtype, int64_t B, 
                           int64_t n_age, int mode, int apply_sigmoid, float *out, void *workspace,
                           int64_t workspace_bytes, void *stream);
 
+/* Many sequences in one sequence-mode call: the B windows are n_seq consecutive sequences of seq_lengths[0], ...,
+ * seq_lengths[n_seq - 1] windows (a HOST array; every length >= 1, the lengths add up to B), and the LSTM scans each
+ * sequence from the zero state, no state crossing from one to the next -- what one b2cnn_forward(mode =
+ * B2CNN_MODE_SEQUENCE) call per sequence returns, row for row, with the front end run once for the whole batch.
+ * {B} is B2CNN_MODE_SEQUENCE over the batch, {1, ..., 1} is B2CNN_MODE_INDEPENDENT.  x, x_pitch, age, n_age,
+ * apply_sigmoid and out as in b2cnn_forward_pitched.  Bad lengths (NULL, n_seq < 1, a length below 1, a sum other
+ * than B) are B2CNN_EINVAL before any CUDA call.  workspace: b2cnn_workspace_bytes_seq() bytes, which is
+ * b2cnn_workspace_bytes(h, B) plus a region the call copies the sequence offsets into (from the host array, on
+ * `stream`); a smaller one is B2CNN_ESTATE before any launch.  The call allocates nothing. */
+int64_t b2cnn_workspace_bytes_seq(b2cnn_handle *h, int64_t B, const int64_t *seq_lengths, int64_t n_seq);
+int b2cnn_forward_seq(b2cnn_handle *h, const void *x, int dtype, int64_t B, int64_t x_pitch, const float *age, int64_t n_age,
+                      const int64_t *seq_lengths, int64_t n_seq, int apply_sigmoid, float *out, void *workspace,
+                      int64_t workspace_bytes, void *stream);
+
 /* Same call with HOST pointers (ideally pinned): chunked H2D copy of x overlapped with
  * compute, D2H of the B results; synchronous on return.  Uses library-owned staging. */
 int b2cnn_forward_host(b2cnn_handle *h, const void *x_host, int dtype, int64_t B,
@@ -552,6 +566,35 @@ int b2cnn_train_backward(const b2cnn_config *cfg, const float *params, const flo
 int b2cnn_train_backward_ex(const b2cnn_config *cfg, const float *params, const float *x, int64_t B, const float *age,
                             int mode, const float *mask1, const float *mask2, const float *dz, float *grads,
                             float *dx, float *dage, int flags, void *workspace, int64_t workspace_bytes, void *stream);
+
+/* ---- Many patients' window sequences in one training call ----
+ * The _seq variants take a HOST array of sequence lengths in place of `mode`: the batch is n_seq consecutive sequences
+ * of seq_lengths[0], ..., seq_lengths[n_seq - 1] windows (every length >= 1, the lengths add up to B), each scanned by
+ * the LSTM from the zero state, no state crossing a sequence boundary.  The logits are those of one model(x_s, age_s)
+ * call per sequence, concatenated; the loss is the mean over all B windows, as in b2cnn_train_step.  {B} is
+ * B2CNN_MODE_SEQUENCE (the same bits) and {1, ..., 1} is B2CNN_MODE_INDEPENDENT.  Bad lengths (NULL, n_seq < 1, a
+ * length below 1, a sum other than B) are B2CNN_EINVAL before any CUDA call.  The workspace is
+ * b2cnn_train_workspace_bytes_seq() bytes: the call copies the sequence offsets into it (from the host array, on
+ * `stream`), and one sized by b2cnn_train_workspace_bytes() is B2CNN_ESTATE before any launch.  Up to 256 sequences
+ * are scanned one CTA each; beyond that a CTA scans ceil(n_seq / 256) consecutive sequences, a grouping taken from
+ * (B, n_seq) alone.  Each CTA writes its head-gradient and loss partials as one row, and the rows are summed in
+ * sequence order (no atomics): the gradients are the same bits from run to run.  With one sequence no row is
+ * written and nothing is summed.
+ * b2cnn_train_step_seq: b2cnn_train_step, or with pos_weight != NULL (one host float, > 0 and finite)
+ * b2cnn_train_step_weighted.  b2cnn_train_forward_seq / b2cnn_train_backward_seq: the autograd pair, the backward with
+ * the flags of b2cnn_train_backward_ex; the backward takes the lengths its forward took. */
+int64_t b2cnn_train_workspace_bytes_seq(const b2cnn_config *cfg, int64_t B, const int64_t *seq_lengths, int64_t n_seq);
+int b2cnn_train_step_seq(const b2cnn_config *cfg, float *params, float *adam_m, float *adam_v, float *grads, int64_t step,
+                         const b2cnn_adam *opt, int apply_update, const float *x, int64_t B, const float *age, const float *target,
+                         const float *pos_weight, const int64_t *seq_lengths, int64_t n_seq, const float *mask1, const float *mask2,
+                         float *loss_out, void *workspace, int64_t workspace_bytes, void *stream);
+int b2cnn_train_forward_seq(const b2cnn_config *cfg, const float *params, const float *x, int64_t B, const float *age,
+                            const int64_t *seq_lengths, int64_t n_seq, const float *mask1, const float *mask2, float *z_out,
+                            void *workspace, int64_t workspace_bytes, void *stream);
+int b2cnn_train_backward_seq(const b2cnn_config *cfg, const float *params, const float *x, int64_t B, const float *age,
+                             const int64_t *seq_lengths, int64_t n_seq, const float *mask1, const float *mask2, const float *dz,
+                             float *grads, float *dx, float *dage, int flags, void *workspace, int64_t workspace_bytes,
+                             void *stream);
 
 #ifdef __cplusplus
 }

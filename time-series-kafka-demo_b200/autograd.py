@@ -80,8 +80,12 @@ class _TrainForward(torch.autograd.Function):
         ws = torch.empty(call.workspace_bytes(B), dtype=torch.uint8, device=dev)
         z = torch.empty(B, dtype=torch.float32, device=dev)
         st = torch.cuda.current_stream(dev).cuda_stream
-        rc = call.lib.b2cnn_train_forward(ctypes.byref(call.cfg), _ptr(blob), _ptr(x), B, _ptr(age), call.mode,
-                                          _ptr(call.mask1), _ptr(call.mask2), _ptr(z), _ptr(ws), ws.numel(), ctypes.c_void_p(st))
+        if call.lens is None:
+            rc = call.lib.b2cnn_train_forward(ctypes.byref(call.cfg), _ptr(blob), _ptr(x), B, _ptr(age), call.mode,
+                                              _ptr(call.mask1), _ptr(call.mask2), _ptr(z), _ptr(ws), ws.numel(), ctypes.c_void_p(st))
+        else:
+            rc = call.lib.b2cnn_train_forward_seq(ctypes.byref(call.cfg), _ptr(blob), _ptr(x), B, _ptr(age), call.lens, len(call.lens),
+                                                  _ptr(call.mask1), _ptr(call.mask2), _ptr(z), _ptr(ws), ws.numel(), ctypes.c_void_p(st))
         capi.check(rc, "b2cnn_train_forward")
         ctx.call, ctx.blob, ctx.ws = call, blob, ws
         ctx.shapes = [p.shape for p in params]
@@ -101,9 +105,15 @@ class _TrainForward(torch.autograd.Function):
         # conv1 / conv2 frozen and no input gradient wanted (fine-tuning the head): the library skips the conv backward
         frozen = dx is None and not any(ctx.needs_input_grad[3:7])
         st = torch.cuda.current_stream(x.device).cuda_stream
-        rc = call.lib.b2cnn_train_backward_ex(ctypes.byref(call.cfg), _ptr(blob), _ptr(x), B, _ptr(age), call.mode, _ptr(call.mask1),
-                                              _ptr(call.mask2), _ptr(dz), _ptr(grads), _ptr(dx), _ptr(dage),
-                                              capi.TRAIN_FROZEN_CONV if frozen else 0, _ptr(ws), ws.numel(), ctypes.c_void_p(st))
+        flags = capi.TRAIN_FROZEN_CONV if frozen else 0
+        if call.lens is None:
+            rc = call.lib.b2cnn_train_backward_ex(ctypes.byref(call.cfg), _ptr(blob), _ptr(x), B, _ptr(age), call.mode, _ptr(call.mask1),
+                                                  _ptr(call.mask2), _ptr(dz), _ptr(grads), _ptr(dx), _ptr(dage), flags, _ptr(ws),
+                                                  ws.numel(), ctypes.c_void_p(st))
+        else:
+            rc = call.lib.b2cnn_train_backward_seq(ctypes.byref(call.cfg), _ptr(blob), _ptr(x), B, _ptr(age), call.lens, len(call.lens),
+                                                   _ptr(call.mask1), _ptr(call.mask2), _ptr(dz), _ptr(grads), _ptr(dx), _ptr(dage), flags,
+                                                   _ptr(ws), ws.numel(), ctypes.c_void_p(st))
         capi.check(rc, "b2cnn_train_backward")
         out, at = [], 0
         for shape, need in zip(ctx.shapes, ctx.needs_input_grad[3:]):
@@ -114,15 +124,19 @@ class _TrainForward(torch.autograd.Function):
 
 
 class _Call:
-    """What one forward / backward pair shares besides tensors: the library, its configuration, mode and masks."""
+    """What one forward / backward pair shares besides tensors: the library, its configuration, mode, masks and sequence
+    lengths (the host array of the _seq calls, or None)."""
 
-    def __init__(self, arch: ArchConfig, device: torch.device, mode: int, mask1, mask2):
+    def __init__(self, arch: ArchConfig, device: torch.device, mode: int, mask1, mask2, lens=None):
         self.lib = capi.load_library()
         self.cfg = capi.make_config(arch, device.index if device.index is not None else torch.cuda.current_device())
-        self.mode, self.mask1, self.mask2 = mode, mask1, mask2
+        self.mode, self.mask1, self.mask2, self.lens = mode, mask1, mask2, lens
 
     def workspace_bytes(self, B: int) -> int:
-        need = int(self.lib.b2cnn_train_workspace_bytes(ctypes.byref(self.cfg), B))
+        if self.lens is None:
+            need = int(self.lib.b2cnn_train_workspace_bytes(ctypes.byref(self.cfg), B))
+        else:
+            need = int(self.lib.b2cnn_train_workspace_bytes_seq(ctypes.byref(self.cfg), B, self.lens, len(self.lens)))
         if need < 0:
             capi.check(capi.EINVAL, "b2cnn_train_workspace_bytes")
         return need
@@ -130,16 +144,20 @@ class _Call:
 
 def mycnn_train_forward(x: torch.Tensor, age: torch.Tensor, params: Sequence[torch.Tensor], arch: ArchConfig,
                         mode: str = "sequence", mask1: Optional[torch.Tensor] = None,
-                        mask2: Optional[torch.Tensor] = None) -> torch.Tensor:
+                        mask2: Optional[torch.Tensor] = None, seq_lengths=None) -> torch.Tensor:
     """Logits [B] of the model in train() mode (bin/models.py:22-36), differentiable in ``x``, ``age`` and ``params``.
 
     ``params``: the 14 tensors of ``BLOB_KEYS`` in that order, on one CUDA device.  ``x`` [B,C,W] (fp32 or bf16; cast
     to fp32), ``age`` 1 or B values.  ``mode``: "sequence" (the LSTM scans the batch axis, as ``model(x, age)`` does in
     the reference) or "independent" (every window from the zero state).  ``mask1`` [B, c_mid, P1] / ``mask2``
-    [B, L_out]: the two dropout masks, already scaled by 1/(1-p); None = no dropout."""
+    [B, L_out]: the two dropout masks, already scaled by 1/(1-p); None = no dropout.  ``seq_lengths`` (mode "sequence"
+    only; a list, tuple or integer tensor, each >= 1, adding up to B): the batch is that many consecutive sequences, each
+    scanned from the zero LSTM state, as ``torch.cat([model(x[o:o+n], age[o:o+n]) for ...])``."""
     check_trainable(arch)
     if mode not in _MODES:
         raise ValueError("mode must be 'sequence' or 'independent'")
+    if seq_lengths is not None and mode != "sequence":
+        raise ValueError("seq_lengths is only accepted with mode='sequence'")
     if len(params) != len(BLOB_KEYS):
         raise ValueError(f"expected the {len(BLOB_KEYS)} tensors of BLOB_KEYS, got {len(params)}")
     shapes = arch.param_shapes()
@@ -156,6 +174,11 @@ def mycnn_train_forward(x: torch.Tensor, age: torch.Tensor, params: Sequence[tor
     B = x.shape[0]
     if B < 1:
         raise RuntimeError("expected at least one window")
+    lens = None
+    if seq_lengths is not None:
+        lens = capi.seq_lengths_array(seq_lengths, B)
+        if torch.as_tensor(age).dim() > 1:
+            raise ValueError(f"with seq_lengths, age must have 1 or {B} elements (one per window), got shape {tuple(torch.as_tensor(age).shape)}")
     x = x.to(dev, torch.float32).contiguous()
     age = torch.as_tensor(age).to(dev, torch.float32).reshape(-1)
     if age.numel() == 1:
@@ -163,7 +186,7 @@ def mycnn_train_forward(x: torch.Tensor, age: torch.Tensor, params: Sequence[tor
     if age.numel() != B:
         raise RuntimeError(f"age must have 1 or {B} elements, got {age.numel()}")
     age = age.contiguous()
-    call = _Call(arch, dev, _MODES[mode], *check_masks(arch, B, dev, mask1, mask2))
+    call = _Call(arch, dev, _MODES[mode], *check_masks(arch, B, dev, mask1, mask2), lens=lens)
     return _TrainForward.apply(call, x, age, *params)
 
 
@@ -193,14 +216,20 @@ class B200TrainableMyCNN(B200MyCNN):
         """The two nn.Dropout masks of bin/models.py:25,28 with ``p = self.dropout.p``, from torch's default generator."""
         return draw_masks(self.arch, B, float(self.dropout.p), self._device())
 
-    def forward(self, x: torch.Tensor, age: torch.Tensor) -> torch.Tensor:
-        """``model(x, age)`` (bin/models.py:22-36): differentiable in train mode, the inference path in eval mode."""
+    def forward(self, x: torch.Tensor, age: torch.Tensor, seq_lengths=None) -> torch.Tensor:
+        """``model(x, age)`` (bin/models.py:22-36): differentiable in train mode, the inference path in eval mode.
+        ``seq_lengths``: the batch is that many consecutive sequences, each from the zero LSTM state, in either mode
+        (``batch_mode == "sequence"`` only; see :func:`mycnn_train_forward`)."""
+        if seq_lengths is not None and self.batch_mode != "sequence":
+            raise ValueError("seq_lengths needs batch_mode == 'sequence'")
         if not self.training:
-            return super().forward(x, age)
+            return super().forward(x, age, seq_lengths)
         if self._device().type != "cuda":
             raise RuntimeError("B200TrainableMyCNN needs the model on a CUDA device to train (there is no CPU fallback)")
         B = x.shape[0]
-        mode = "sequence" if (self.batch_mode == "sequence" and B > 1) else "independent"
+        if seq_lengths is not None:
+            capi.seq_lengths_array(seq_lengths, B)          # refused before the masks are drawn
+        mode = "sequence" if (self.batch_mode == "sequence" and (B > 1 or seq_lengths is not None)) else "independent"
         m1, m2 = self.draw_masks(B)
         named = dict(self.named_parameters())
-        return mycnn_train_forward(x, age, [named[k] for k in BLOB_KEYS], self.arch, mode, m1, m2)
+        return mycnn_train_forward(x, age, [named[k] for k in BLOB_KEYS], self.arch, mode, m1, m2, seq_lengths)

@@ -27,6 +27,8 @@ SYMBOLS = ("b2cnn_l_out", "b2cnn_weight_count", "b2cnn_create", "b2cnn_destroy",
            "b2cnn_features", "b2cnn_set_option", "b2cnn_get_option", "b2cnn_last_launch_count",
            "b2cnn_last_path", "b2cnn_last_stage_ms", "b2cnn_last_error", "b2cnn_version", "b2cnn_train_workspace_bytes", "b2cnn_train_step",
            "b2cnn_train_step_weighted", "b2cnn_train_forward", "b2cnn_train_backward", "b2cnn_train_backward_ex",
+           "b2cnn_train_workspace_bytes_seq", "b2cnn_train_step_seq", "b2cnn_train_forward_seq", "b2cnn_train_backward_seq",
+           "b2cnn_workspace_bytes_seq", "b2cnn_forward_seq",
            "b2cnn_prep_window_count", "b2cnn_prep_workspace_bytes", "b2cnn_prep_windows",
            "b2cnn_ring_create", "b2cnn_ring_destroy", "b2cnn_ring_reset", "b2cnn_ring_set_signals", "b2cnn_ring_push",
            "b2cnn_slide_create", "b2cnn_slide_destroy", "b2cnn_slide_reset", "b2cnn_slide_push", "b2cnn_slide_features",
@@ -195,6 +197,18 @@ def load_library() -> ctypes.CDLL:
     lib.b2cnn_train_backward.restype = c_int
     lib.b2cnn_train_backward_ex.argtypes = [cfgp, c_vp, c_vp, c_i64, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_i64, c_vp]
     lib.b2cnn_train_backward_ex.restype = c_int
+    lib.b2cnn_train_workspace_bytes_seq.argtypes = [cfgp, c_i64, c_vp, c_i64]; lib.b2cnn_train_workspace_bytes_seq.restype = c_i64
+    lib.b2cnn_train_step_seq.argtypes = [cfgp, c_vp, c_vp, c_vp, c_vp, c_i64, ctypes.POINTER(Adam), c_int, c_vp, c_i64, c_vp, c_vp,
+                                         c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp]
+    lib.b2cnn_train_step_seq.restype = c_int
+    lib.b2cnn_train_forward_seq.argtypes = [cfgp, c_vp, c_vp, c_i64, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp]
+    lib.b2cnn_train_forward_seq.restype = c_int
+    lib.b2cnn_train_backward_seq.argtypes = [cfgp, c_vp, c_vp, c_i64, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_vp,
+                                             c_i64, c_vp]
+    lib.b2cnn_train_backward_seq.restype = c_int
+    lib.b2cnn_workspace_bytes_seq.argtypes = [c_vp, c_i64, c_vp, c_i64]; lib.b2cnn_workspace_bytes_seq.restype = c_i64
+    lib.b2cnn_forward_seq.argtypes = [c_vp, c_vp, c_int, c_i64, c_i64, c_vp, c_i64, c_vp, c_i64, c_int, c_vp, c_vp, c_i64, c_vp]
+    lib.b2cnn_forward_seq.restype = c_int
     lib.b2cnn_last_error.argtypes = []; lib.b2cnn_last_error.restype = ctypes.c_char_p
     lib.b2cnn_version.argtypes = []; lib.b2cnn_version.restype = ctypes.c_char_p
     _lib = lib
@@ -209,6 +223,40 @@ def check(rc: int, what: str) -> None:
     """The reference raises RuntimeError on shape mismatches; so does the drop-in."""
     if rc != OK:
         raise RuntimeError(f"{what}: {last_error()} (b2cnn error {rc})")
+
+
+def seq_lengths_array(seq_lengths, B: int):
+    """``seq_lengths`` (a list, tuple or integer tensor of N >= 1 lengths, each >= 1, adding up to B) as the host int64
+    array the ``_seq`` entry points take; ValueError for anything else.  Sequence s is rows o_s .. o_s + n_s - 1 of the
+    batch, o_s = n_0 + ... + n_{s-1}."""
+    import operator
+
+    import torch
+    if isinstance(seq_lengths, (list, tuple)):
+        vals = list(seq_lengths)
+    elif torch.is_tensor(seq_lengths):
+        if seq_lengths.dim() != 1 or seq_lengths.dtype.is_floating_point or seq_lengths.dtype.is_complex \
+                or seq_lengths.dtype == torch.bool:
+            raise ValueError(f"seq_lengths must be a 1-d integer tensor, got {seq_lengths.dtype} of shape {tuple(seq_lengths.shape)}")
+        vals = seq_lengths.tolist()
+    else:
+        raise ValueError(f"seq_lengths must be a list, tuple or integer tensor, got {type(seq_lengths).__name__}")
+    if not vals:
+        raise ValueError("seq_lengths must hold at least one sequence")
+    out = []
+    for i, v in enumerate(vals):
+        if isinstance(v, bool):
+            raise ValueError(f"seq_lengths[{i}] must be an integer, got bool")
+        try:
+            v = operator.index(v)
+        except TypeError:
+            raise ValueError(f"seq_lengths[{i}] must be an integer, got {type(v).__name__}") from None
+        if v < 1:
+            raise ValueError(f"seq_lengths[{i}] = {v}: every sequence needs at least one window")
+        out.append(v)
+    if sum(out) != B:
+        raise ValueError(f"seq_lengths add up to {sum(out)}, the batch has {B} windows")
+    return (ctypes.c_int64 * len(out))(*out)
 
 
 def make_config(arch, device: int = -1) -> Config:

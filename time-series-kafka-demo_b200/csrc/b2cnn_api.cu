@@ -89,19 +89,26 @@ extern "C" int64_t b2cnn_weight_count(const b2cnn_config *cfg) {
 extern "C" const char *b2cnn_last_error(void) { return g_err.c_str(); }
 
 // ---- one training step (b2cnn_train.cu) ----
+static constexpr SeqLengths kNoSeq{false, nullptr, 0};
+
 extern "C" int64_t b2cnn_train_workspace_bytes(const b2cnn_config *cfg, int64_t B) {
-    const int64_t n = train_workspace_bytes(cfg, B);
+    const int64_t n = train_workspace_bytes(cfg, B, kNoSeq);
     if (n < 0) fail(B2CNN_EINVAL, "b2cnn_train_workspace_bytes: bad configuration / batch");
+    return n;
+}
+extern "C" int64_t b2cnn_train_workspace_bytes_seq(const b2cnn_config *cfg, int64_t B, const int64_t *seq_lengths, int64_t n_seq) {
+    const int64_t n = train_workspace_bytes(cfg, B, SeqLengths{true, seq_lengths, n_seq});
+    if (n < 0) fail(B2CNN_EINVAL, "b2cnn_train_workspace_bytes_seq: bad configuration / batch / sequence lengths");
     return n;
 }
 static int train_step_api(const char *name, const b2cnn_config *cfg, float *params, float *adam_m, float *adam_v, float *grads,
                           int64_t step, const b2cnn_adam *opt, int apply_update, const float *x, int64_t B, const float *age,
-                          const float *target, int weighted, float pos_weight, int mode, const float *mask1, const float *mask2,
-                          float *loss_out, void *workspace, int64_t workspace_bytes, void *stream) {
+                          const float *target, int weighted, float pos_weight, int mode, const SeqLengths &sl, const float *mask1,
+                          const float *mask2, float *loss_out, void *workspace, int64_t workspace_bytes, void *stream) {
     if (!cfg || !opt) return fail(B2CNN_EINVAL, std::string(name) + ": null configuration");
     const char *err = "";
     const int rc = train_step(cfg, params, adam_m, adam_v, grads, step, opt->lr, opt->beta1, opt->beta2, opt->eps, apply_update, x, B, age,
-                              target, weighted, pos_weight, mode, mask1, mask2, loss_out, workspace, workspace_bytes,
+                              target, weighted, pos_weight, mode, sl, mask1, mask2, loss_out, workspace, workspace_bytes,
                               reinterpret_cast<cudaStream_t>(stream), &err);
     return finish(name, rc, err);
 }
@@ -110,28 +117,45 @@ extern "C" int b2cnn_train_step(const b2cnn_config *cfg, float *params, float *a
                                 const float *target, int mode, const float *mask1, const float *mask2, float *loss_out,
                                 void *workspace, int64_t workspace_bytes, void *stream) {
     return train_step_api("b2cnn_train_step", cfg, params, adam_m, adam_v, grads, step, opt, apply_update, x, B, age, target, 0, 1.f, mode,
-                          mask1, mask2, loss_out, workspace, workspace_bytes, stream);
+                          kNoSeq, mask1, mask2, loss_out, workspace, workspace_bytes, stream);
 }
 extern "C" int b2cnn_train_step_weighted(const b2cnn_config *cfg, float *params, float *adam_m, float *adam_v, float *grads, int64_t step,
                                          const b2cnn_adam *opt, int apply_update, const float *x, int64_t B, const float *age,
                                          const float *target, float pos_weight, int mode, const float *mask1, const float *mask2,
                                          float *loss_out, void *workspace, int64_t workspace_bytes, void *stream) {
     return train_step_api("b2cnn_train_step_weighted", cfg, params, adam_m, adam_v, grads, step, opt, apply_update, x, B, age, target, 1,
-                          pos_weight, mode, mask1, mask2, loss_out, workspace, workspace_bytes, stream);
+                          pos_weight, mode, kNoSeq, mask1, mask2, loss_out, workspace, workspace_bytes, stream);
+}
+extern "C" int b2cnn_train_step_seq(const b2cnn_config *cfg, float *params, float *adam_m, float *adam_v, float *grads, int64_t step,
+                                    const b2cnn_adam *opt, int apply_update, const float *x, int64_t B, const float *age,
+                                    const float *target, const float *pos_weight, const int64_t *seq_lengths, int64_t n_seq,
+                                    const float *mask1, const float *mask2, float *loss_out, void *workspace, int64_t workspace_bytes,
+                                    void *stream) {
+    return train_step_api("b2cnn_train_step_seq", cfg, params, adam_m, adam_v, grads, step, opt, apply_update, x, B, age, target,
+                          pos_weight ? 1 : 0, pos_weight ? *pos_weight : 1.f, B2CNN_MODE_SEQUENCE, SeqLengths{true, seq_lengths, n_seq},
+                          mask1, mask2, loss_out, workspace, workspace_bytes, stream);
 }
 extern "C" int b2cnn_train_forward(const b2cnn_config *cfg, const float *params, const float *x, int64_t B, const float *age, int mode,
                                    const float *mask1, const float *mask2, float *z_out, void *workspace, int64_t workspace_bytes,
                                    void *stream) {
     const char *err = "";
-    const int rc = train_forward(cfg, params, x, B, age, mode, mask1, mask2, z_out, workspace, workspace_bytes,
+    const int rc = train_forward(cfg, params, x, B, age, mode, kNoSeq, mask1, mask2, z_out, workspace, workspace_bytes,
                                  reinterpret_cast<cudaStream_t>(stream), &err);
     return finish("b2cnn_train_forward", rc, err);
+}
+extern "C" int b2cnn_train_forward_seq(const b2cnn_config *cfg, const float *params, const float *x, int64_t B, const float *age,
+                                       const int64_t *seq_lengths, int64_t n_seq, const float *mask1, const float *mask2, float *z_out,
+                                       void *workspace, int64_t workspace_bytes, void *stream) {
+    const char *err = "";
+    const int rc = train_forward(cfg, params, x, B, age, B2CNN_MODE_SEQUENCE, SeqLengths{true, seq_lengths, n_seq}, mask1, mask2, z_out,
+                                 workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream), &err);
+    return finish("b2cnn_train_forward_seq", rc, err);
 }
 extern "C" int b2cnn_train_backward_ex(const b2cnn_config *cfg, const float *params, const float *x, int64_t B, const float *age, int mode,
                                        const float *mask1, const float *mask2, const float *dz, float *grads, float *dx, float *dage,
                                        int flags, void *workspace, int64_t workspace_bytes, void *stream) {
     const char *err = "";
-    const int rc = train_backward(cfg, params, x, B, age, mode, mask1, mask2, dz, grads, dx, dage, flags, workspace, workspace_bytes,
+    const int rc = train_backward(cfg, params, x, B, age, mode, kNoSeq, mask1, mask2, dz, grads, dx, dage, flags, workspace, workspace_bytes,
                                   reinterpret_cast<cudaStream_t>(stream), &err);
     return finish("b2cnn_train_backward", rc, err);
 }
@@ -139,6 +163,15 @@ extern "C" int b2cnn_train_backward(const b2cnn_config *cfg, const float *params
                                     const float *mask1, const float *mask2, const float *dz, float *grads, float *dx, float *dage,
                                     void *workspace, int64_t workspace_bytes, void *stream) {
     return b2cnn_train_backward_ex(cfg, params, x, B, age, mode, mask1, mask2, dz, grads, dx, dage, 0, workspace, workspace_bytes, stream);
+}
+extern "C" int b2cnn_train_backward_seq(const b2cnn_config *cfg, const float *params, const float *x, int64_t B, const float *age,
+                                        const int64_t *seq_lengths, int64_t n_seq, const float *mask1, const float *mask2, const float *dz,
+                                        float *grads, float *dx, float *dage, int flags, void *workspace, int64_t workspace_bytes,
+                                        void *stream) {
+    const char *err = "";
+    const int rc = train_backward(cfg, params, x, B, age, B2CNN_MODE_SEQUENCE, SeqLengths{true, seq_lengths, n_seq}, mask1, mask2, dz, grads,
+                                  dx, dage, flags, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream), &err);
+    return finish("b2cnn_train_backward_seq", rc, err);
 }
 
 // ---- preprocessing + window assembly (b2cnn_prep.cu) ----
@@ -433,8 +466,10 @@ static int create_stage_events(b2cnn_handle *h) {
     return B2CNN_OK;
 }
 
+// seq_off / n_seq: b2cnn_forward_seq's sequences (device memory, n_seq + 1 offsets; mode is B2CNN_MODE_SEQUENCE), else NULL / 0
 static int forward_device(b2cnn_handle *h, const void *x, int dtype, int64_t B, int64_t xpitch, const float *age, int64_t n_age,
-                          int mode, int apply_sigmoid, float *out, void *ws, int64_t ws_bytes, cudaStream_t st) {
+                          int mode, int apply_sigmoid, float *out, void *ws, int64_t ws_bytes, cudaStream_t st,
+                          const int64_t *seq_off = nullptr, int64_t n_seq = 0) {
     Dims d = h->d;
     if (xpitch < d.W || xpitch > 0x7fffffff) return fail(B2CNN_EINVAL, "b2cnn_forward: x_pitch must be >= window");
     d.XP = (int)xpitch;
@@ -488,12 +523,13 @@ static int forward_device(b2cnn_handle *h, const void *x, int dtype, int64_t B, 
         // the head kernel is the last reader of the call's exception list: it also puts the handle's flag state back to zero
         const bool cleans = to_gates && indep && h->tc.cur_own;
         if (!to_gates)
-            n = launch_head(d, h->hw, feats, sB, sP, B, age, n_age, mode, apply_sigmoid, out, gates, partial, choose_ksplit(d.L), st, &err);
+            n = launch_head(d, h->hw, feats, sB, sP, B, age, n_age, mode, apply_sigmoid, out, gates, partial, choose_ksplit(d.L), st, &err,
+                            seq_off, n_seq);
         else if (indep)
             n = launch_reduce_lstm_head(d, h->hw, partial, h->tc.n_ranges, B, age, n_age, apply_sigmoid, out, st, &err,
                                         cleans ? h->tc.cur_count : nullptr, h->tc.cur_flags, h->tc.cur_list);
         else
-            n = launch_lstm_head(d, h->hw, gates, B, age, n_age, mode, apply_sigmoid, out, st, &err);
+            n = launch_lstm_head(d, h->hw, gates, B, age, n_age, mode, apply_sigmoid, out, st, &err, seq_off, n_seq);
         if (n < 0) return fail(B2CNN_ECUDA, std::string("head: ") + err);
         if (cleans) h->tc.flags_clean = true;
         launches += n;
@@ -536,6 +572,38 @@ extern "C" int b2cnn_forward_pitched(b2cnn_handle *h, const void *x, int dtype, 
     if (rc) return rc;
     DEVICE_GUARD(h->device);
     return forward_device(h, x, dtype, B, x_pitch, age, n_age, mode, apply_sigmoid, out, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+// The sequence offsets of b2cnn_forward_seq sit after what b2cnn_workspace_bytes(h, B) covers.
+static int64_t seq_ws_base(b2cnn_handle *h, int64_t B) { return ws_layout(h, B, true, true).total; }
+
+extern "C" int64_t b2cnn_workspace_bytes_seq(b2cnn_handle *h, int64_t B, const int64_t *seq_lengths, int64_t n_seq) {
+    std::vector<int64_t> off;
+    const char *err = "";
+    if (!h || B < 1) { fail(B2CNN_EINVAL, "b2cnn_workspace_bytes_seq: null handle / bad batch"); return -1; }
+    if (!seq_offsets(SeqLengths{true, seq_lengths, n_seq}, B, off, &err)) {
+        fail(B2CNN_EINVAL, std::string("b2cnn_workspace_bytes_seq: ") + err);
+        return -1;
+    }
+    return seq_ws_base(h, B) + align_up(8 * (n_seq + 1), 256);
+}
+
+extern "C" int b2cnn_forward_seq(b2cnn_handle *h, const void *x, int dtype, int64_t B, int64_t x_pitch, const float *age, int64_t n_age,
+                                 const int64_t *seq_lengths, int64_t n_seq, int apply_sigmoid, float *out, void *workspace,
+                                 int64_t workspace_bytes, void *stream) {
+    int rc = check_call(h, x, dtype, B, age, n_age, B2CNN_MODE_SEQUENCE, out);
+    if (rc) return rc;
+    std::vector<int64_t> off;
+    const char *err = "";
+    if (!seq_offsets(SeqLengths{true, seq_lengths, n_seq}, B, off, &err)) return fail(B2CNN_EINVAL, std::string("b2cnn_forward_seq: ") + err);
+    const int64_t base = seq_ws_base(h, B);
+    if (!workspace || workspace_bytes < base + align_up(8 * (n_seq + 1), 256))
+        return fail(B2CNN_ESTATE, "b2cnn_forward_seq: workspace missing or smaller than b2cnn_workspace_bytes_seq()");
+    DEVICE_GUARD(h->device);
+    cudaStream_t st = (cudaStream_t)stream;
+    int64_t *doff = reinterpret_cast<int64_t *>((char *)workspace + base);
+    CU_TRY(cudaMemcpyAsync(doff, off.data(), sizeof(int64_t) * off.size(), cudaMemcpyHostToDevice, st));
+    return forward_device(h, x, dtype, B, x_pitch, age, n_age, B2CNN_MODE_SEQUENCE, apply_sigmoid, out, workspace, base, st, doff, n_seq);
 }
 
 extern "C" int b2cnn_features(b2cnn_handle *h, const void *x, int dtype, int64_t B, float *feats, void *stream) {

@@ -7,7 +7,8 @@
 //   head_independent     one thread per window, LSTM from the zero state (predictStream.py:157)
 //   head_sequence        one warp per segment scans its rows carrying (h, c) -- the reference's
 //                        model(x_batch) semantics for B > 1 (models.py:29-30, utils.py:249), over
-//                        the whole batch or over each recording's windows (utils.py:671-692)
+//                        the whole batch, over each sequence of b2cnn_forward_seq or over each
+//                        recording's windows (utils.py:671-692)
 #include "b2cnn_internal.cuh"
 #include "b2cnn_head_dev.cuh"
 
@@ -240,13 +241,16 @@ head_reduce_independent_kernel(const float *__restrict__ part, int slices, HeadW
 }
 
 // One warp (one CTA) per segment: CTA s scans rows s seg_len .. s seg_len + seg_len - 1 of gates0, age (n_age > 1) and
-// out sequentially from the zero state.  forward's sequence mode is one segment of B rows; b2cnn_score_record's is one
-// segment per recording, of its n_w windows.  Each row is one seq_step (b2cnn_head_dev.cuh).
+// out sequentially from the zero state, or with seg_off rows seg_off[s] .. seg_off[s + 1] - 1.  forward's sequence mode
+// is one segment of B rows, or one per sequence of b2cnn_forward_seq; b2cnn_score_record's is one segment per recording,
+// of its n_w windows.  Each row is one seq_step (b2cnn_head_dev.cuh).
 __global__ void __launch_bounds__(32)
 head_sequence_kernel(const float *__restrict__ gates0, HeadWeights hw, const float *__restrict__ age,
-                     int64_t n_age, float coef, int apply_sigmoid, float *__restrict__ out, int64_t seg_len) {
+                     int64_t n_age, float coef, int apply_sigmoid, float *__restrict__ out, int64_t seg_len,
+                     const int64_t *__restrict__ seg_off) {
     const int l = threadIdx.x;
-    const int64_t row0 = (int64_t)blockIdx.x * seg_len, B = seg_len;
+    const int64_t row0 = seg_off ? seg_off[blockIdx.x] : (int64_t)blockIdx.x * seg_len;
+    const int64_t B = seg_off ? seg_off[blockIdx.x + 1] - row0 : seg_len;
     gates0 += row0 * kGates;
     out += row0;
     if (n_age != 1) age += row0;
@@ -326,7 +330,7 @@ int proj_slices(int L) {
 int launch_head(const Dims &d, const HeadWeights &hw, const float *feats, int64_t sB, int64_t sP,
                 int64_t B, const float *age, int64_t n_age, int mode, int apply_sigmoid,
                 float *out, float *gates_ws, float *partial_ws, int ksplit, cudaStream_t st,
-                const char **err) {
+                const char **err, const int64_t *seq_off, int64_t n_seq) {
     int launches = 0;
     int ks_eff;
     const int kps = proj_split(d.L, ksplit, &ks_eff);
@@ -336,7 +340,7 @@ int launch_head(const Dims &d, const HeadWeights &hw, const float *feats, int64_
     int n = launch_reduce_gates(partial_ws, ks_eff, B, hw, gates_ws, st, err);
     if (n < 0) return -1;
     launches += n;
-    n = launch_lstm_head(d, hw, gates_ws, B, age, n_age, mode, apply_sigmoid, out, st, err);
+    n = launch_lstm_head(d, hw, gates_ws, B, age, n_age, mode, apply_sigmoid, out, st, err, seq_off, n_seq);
     if (n < 0) return -1;
     return launches + n;
 }
@@ -407,12 +411,14 @@ int launch_reduce_lstm_head(const Dims &d, const HeadWeights &hw, const float *p
 
 // LSTM cells + Linear + age scale from layer-0 gate pre-activations (bin/models.py:30-34)
 int launch_lstm_head(const Dims &d, const HeadWeights &hw, const float *gates, int64_t B, const float *age,
-                     int64_t n_age, int mode, int apply_sigmoid, float *out, cudaStream_t st, const char **err) {
+                     int64_t n_age, int mode, int apply_sigmoid, float *out, cudaStream_t st, const char **err,
+                     const int64_t *seq_off, int64_t n_seq) {
     if (mode == B2CNN_MODE_INDEPENDENT) {
         head_independent_kernel<<<(unsigned)((B + 127) / 128), 128, 0, st>>>(gates, hw, age, n_age, d.age_coef,
                                                                              apply_sigmoid, out, B);
     } else {
-        return launch_sequence_segments(d, hw, gates, 1, B, age, n_age, apply_sigmoid, out, st, err);
+        return seq_off ? launch_sequence_segments(d, hw, gates, n_seq, 0, age, n_age, apply_sigmoid, out, st, err, seq_off)
+                       : launch_sequence_segments(d, hw, gates, 1, B, age, n_age, apply_sigmoid, out, st, err);
     }
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) { *err = cudaGetErrorString(e); return -1; }
@@ -421,8 +427,8 @@ int launch_lstm_head(const Dims &d, const HeadWeights &hw, const float *gates, i
 
 // n_seg independent LSTM scans of seg_len consecutive rows each, one warp per segment
 int launch_sequence_segments(const Dims &d, const HeadWeights &hw, const float *gates, int64_t n_seg, int64_t seg_len, const float *age,
-                             int64_t n_age, int apply_sigmoid, float *out, cudaStream_t st, const char **err) {
-    head_sequence_kernel<<<(unsigned)n_seg, 32, 0, st>>>(gates, hw, age, n_age, d.age_coef, apply_sigmoid, out, seg_len);
+                             int64_t n_age, int apply_sigmoid, float *out, cudaStream_t st, const char **err, const int64_t *seg_off) {
+    head_sequence_kernel<<<(unsigned)n_seg, 32, 0, st>>>(gates, hw, age, n_age, d.age_coef, apply_sigmoid, out, seg_len, seg_off);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) { *err = cudaGetErrorString(e); return -1; }
     return 1;

@@ -9,6 +9,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <vector>
+
 #include "../../include/b2cnn.h"
 
 namespace b2cnn {
@@ -73,6 +75,28 @@ __host__ __device__ inline BlobOff blob_offsets(const Dims &d) {
     o.affine = p; if (d.has_affine) p += 2 * kCMid + 2;
     o.total = p;
     return o;
+}
+
+// The sequence lengths of a _seq call (include/b2cnn.h): a host array of n lengths; on == false for the calls that take
+// a mode instead
+struct SeqLengths {
+    bool on;
+    const int64_t *len;
+    int64_t n;
+};
+// off = the n + 1 offsets 0, n_0, n_0 + n_1, ..., B of lengths that are each >= 1 and sum to B; false (with the reason in
+// err) for a NULL array, n < 1, a length below 1 or a sum that is not B.  No CUDA call.
+inline bool seq_offsets(const SeqLengths &sl, int64_t B, std::vector<int64_t> &off, const char **err) {
+    if (!sl.len || sl.n < 1 || sl.n > B) { *err = "seq_lengths: NULL, or n_seq not in [1, B]"; return false; }
+    off.resize((size_t)sl.n + 1);
+    off[0] = 0;
+    for (int64_t s = 0; s < sl.n; ++s) {
+        const int64_t v = sl.len[s];
+        if (v < 1 || v > B - off[s]) { *err = v < 1 ? "seq_lengths: every length must be >= 1" : "seq_lengths: the lengths add up to more than B"; return false; }
+        off[s + 1] = off[s] + v;
+    }
+    if (off[sl.n] != B) { *err = "seq_lengths: the lengths add up to less than B"; return false; }
+    return true;
 }
 
 // Makes `device` current for the guard's lifetime and restores the caller's device on every exit path (a call on cuda:1
@@ -172,19 +196,24 @@ int launch_frontend_generic_gates_listed(const Dims &d, const ConvWeights &cw, c
                                          const float *wih0T, float *gate_part, int gate_slices, const int *win_list,
                                          const int *win_count, cudaStream_t st, int num_sms, const char **err);
 
+// seq_off / n_seq (sequence mode only): the scan runs over n_seq sequences, rows [seq_off[s], seq_off[s + 1]) of the
+// batch (device memory), instead of over all B rows
 int launch_head(const Dims &d, const HeadWeights &hw, const float *feats, int64_t sB, int64_t sP,
                 int64_t B, const float *age, int64_t n_age, int mode, int apply_sigmoid,
                 float *out, float *gates_ws, float *partial_ws, int ksplit, cudaStream_t st,
-                const char **err);
+                const char **err, const int64_t *seq_off = nullptr, int64_t n_seq = 0);
 
 int launch_reduce_gates(const float *partial, int slices, int64_t B, const HeadWeights &hw, float *gates,
                         cudaStream_t st, const char **err);
 int launch_lstm_head(const Dims &d, const HeadWeights &hw, const float *gates, int64_t B, const float *age,
-                     int64_t n_age, int mode, int apply_sigmoid, float *out, cudaStream_t st, const char **err);
+                     int64_t n_age, int mode, int apply_sigmoid, float *out, cudaStream_t st, const char **err,
+                     const int64_t *seq_off = nullptr, int64_t n_seq = 0);
 // sequence mode over n_seg segments of seg_len consecutive rows of gates [n_seg seg_len][64], age (n_age = 1 or n_seg
-// seg_len) and out, each scanned from the zero state; launch_lstm_head's sequence mode is one segment of B rows
+// seg_len) and out, each scanned from the zero state; launch_lstm_head's sequence mode is one segment of B rows.
+// seg_off != nullptr (device memory, n_seg + 1 offsets): segment s is rows [seg_off[s], seg_off[s + 1]) instead
 int launch_sequence_segments(const Dims &d, const HeadWeights &hw, const float *gates, int64_t n_seg, int64_t seg_len, const float *age,
-                             int64_t n_age, int apply_sigmoid, float *out, cudaStream_t st, const char **err);
+                             int64_t n_age, int apply_sigmoid, float *out, cudaStream_t st, const char **err,
+                             const int64_t *seg_off = nullptr);
 // a sequence-mode sliding scorer's head: for every live patient p (all with seen == nullptr, else seen[p] >= 0 &&
 // seen[p] + S >= d.W, the counts before the push advances them), one LSTM step from state[p] [64] = h0 | c0 | h1 | c1,
 // its layer-0 gates summed from partial [slices][P][64] as launch_reduce_gates does; out[p] and state[p] written
@@ -254,16 +283,17 @@ double wire_parse_decimal_host(const char *s, int64_t len, int *status);
 
 // b2cnn_train.cu: one training step (row f4).  mode is B2CNN_MODE_*; every entry point checks all its arguments before
 // any CUDA call, then makes cfg->device current for the call (a negative device: the current one)
-int64_t train_workspace_bytes(const b2cnn_config *cfg, int64_t B);
+// sl: the sequence lengths of a _seq call (mode is then B2CNN_MODE_SEQUENCE), or {false} for the calls that take a mode
+int64_t train_workspace_bytes(const b2cnn_config *cfg, int64_t B, const SeqLengths &sl);
 // weighted != 0: BCEWithLogitsLoss(pos_weight=pos_weight), else plain BCEWithLogitsLoss
 int train_step(const b2cnn_config *cfg, float *params, float *adam_m, float *adam_v, float *grads, int64_t step, float lr, float beta1,
                float beta2, float eps, int apply_update, const float *x, int64_t B, const float *age, const float *target,
-               int weighted, float pos_weight, int mode, const float *mask1, const float *mask2, float *loss_out, void *workspace,
-               int64_t ws_bytes, cudaStream_t st, const char **err);
+               int weighted, float pos_weight, int mode, const SeqLengths &sl, const float *mask1, const float *mask2, float *loss_out,
+               void *workspace, int64_t ws_bytes, cudaStream_t st, const char **err);
 // the autograd seam
-int train_forward(const b2cnn_config *cfg, const float *params, const float *x, int64_t B, const float *age, int mode, const float *mask1,
-                  const float *mask2, float *z_out, void *workspace, int64_t ws_bytes, cudaStream_t st, const char **err);
-int train_backward(const b2cnn_config *cfg, const float *params, const float *x, int64_t B, const float *age, int mode,
+int train_forward(const b2cnn_config *cfg, const float *params, const float *x, int64_t B, const float *age, int mode, const SeqLengths &sl,
+                  const float *mask1, const float *mask2, float *z_out, void *workspace, int64_t ws_bytes, cudaStream_t st, const char **err);
+int train_backward(const b2cnn_config *cfg, const float *params, const float *x, int64_t B, const float *age, int mode, const SeqLengths &sl,
                    const float *mask1, const float *mask2, const float *dz, float *grads, float *dx, float *dage, int flags,
                    void *workspace, int64_t ws_bytes, cudaStream_t st, const char **err);
 

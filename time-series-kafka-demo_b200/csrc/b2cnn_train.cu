@@ -18,10 +18,13 @@
 //                          there and writes only f
 //   train_pre0_partial     layer-0 pre-activations f . W_ih_l0^T as a split-K GEMM over slices of kPre0Slice positions;
 //                          with more than one slice train_sum_chunks adds the partials in slice order
-//   train_lstm_fwd         one CTA scans the batch axis from those pre-activations, keeps gate activations / cell /
-//                          hidden states, logits, loss
-//   train_lstm_bwd         BPTT over the batch axis: gradients of the head and of every recurrent matrix, d(gates of
-//                          layer 0) = da0
+//   train_lstm_fwd         scans the batch axis from those pre-activations, keeps gate activations / cell / hidden
+//                          states, logits, loss; one CTA, or with seq_lengths (the _seq entry points) one CTA per group
+//                          of consecutive sequences, each sequence from the zero state
+//   train_lstm_bwd         BPTT over the batch axis (over each CTA's sequences): gradients of the head and of every
+//                          recurrent matrix, d(gates of layer 0) = da0
+//   train_head_reduce      with more than one scan CTA: sums the CTAs' head-gradient and loss rows in CTA (= sequence)
+//                          order
 //   train_wih0_grad        dW_ih_l0 = da0^T f with f read once: a thread owns a position and all 64 gate rows, the batch
 //                          is split into chunks, and train_sum_chunks adds the chunk partials in chunk order
 //   train_dfeat            d f = da0 W_ih_l0 with a thread's 64 W_ih_l0 values in registers
@@ -39,6 +42,7 @@
 // its geometry alone; the batch sets only the order in which conv-gradient partials and dW_ih_l0's chunks are added.
 #include <cfloat>
 #include <cstring>
+#include <vector>
 
 #include "b2cnn_internal.cuh"
 
@@ -46,7 +50,7 @@ namespace b2cnn {
 
 // workspace layout (floats)
 struct TrainWs {
-    int64_t f, pre0, acts, cs, hs, lin, z, da0, dfeat, part, total;
+    int64_t f, pre0, acts, cs, hs, lin, z, da0, dfeat, part, off, total;
 };
 
 constexpr int kT = 128;             // final features per tile
@@ -56,6 +60,10 @@ constexpr int kBwdCtas = 1024;      // the conv backward puts several windows in
 constexpr int kPre0Slice = 1024;    // positions per split-K slice of the pre-activation GEMM
 constexpr int kWihChunks = 16;      // at most this many batch chunks in dW_ih_l0
 constexpr int kRowBatch = 64;       // da0 rows staged per pass of train_dfeat / train_wih0_grad
+constexpr int kSeqCtas = 256;       // at most this many CTAs scan the sequences of a batch (one partial row per CTA)
+
+// The head's gradients (blob entries [o.whh0, o.bo], contiguous) and, after them, a loss sum: one scan CTA's partial row
+__host__ __device__ inline int64_t head_row_len(const BlobOff &o) { return o.bo + 1 - o.whh0 + 1; }
 
 // float offsets of a conv tile's buffers in dynamic shared memory; xp / pp are the row pitches of x and d1 / dd1
 struct TileSmem {
@@ -96,10 +104,15 @@ struct TrainPlan {
     int tiles, slices, wih_chunk, wih_chunks, win, groups, n_conv;
     int64_t part_rows;                  // per-CTA conv weight-gradient partials
     size_t smem_fwd, smem_bwd;
+    int seq_per, seq_ctas;              // sequences per scan CTA, scan CTAs
 };
 
-static TrainPlan train_plan(const Dims &d, int64_t B) {
+// n_seq: the number of sequences of a _seq call, 0 for the calls that take a mode (their layout has no offsets region)
+static TrainPlan train_plan(const Dims &d, int64_t B, int64_t n_seq = 0) {
     TrainPlan pl{};
+    // consecutive sequences per scan CTA: ceil(n_seq / kSeqCtas), from (B, n_seq) alone, never the device
+    pl.seq_per = n_seq > kSeqCtas ? (int)((n_seq + kSeqCtas - 1) / kSeqCtas) : 1;
+    pl.seq_ctas = n_seq > 0 ? (int)((n_seq + pl.seq_per - 1) / pl.seq_per) : 1;
     pl.tiles = (d.L + kT - 1) / kT;
     pl.slices = (d.L + kPre0Slice - 1) / kPre0Slice;
     pl.wih_chunk = (int)((B + kWihChunks - 1) / kWihChunks);
@@ -128,7 +141,10 @@ static TrainPlan train_plan(const Dims &d, int64_t B) {
     int64_t part = (int64_t)pl.slices * B * kGates;
     if ((int64_t)pl.wih_chunks * kGates * d.L > part) part = (int64_t)pl.wih_chunks * kGates * d.L;
     if (pl.part_rows * pl.n_conv > part) part = pl.part_rows * pl.n_conv;
+    // the scan CTAs' head rows: written by the LSTM kernels and summed before any other reduction uses the region
+    if (pl.seq_ctas > 1 && pl.seq_ctas * head_row_len(blob_offsets(d)) > part) part = pl.seq_ctas * head_row_len(blob_offsets(d));
     w.part = take(part);
+    w.off = n_seq > 0 ? take(2 * (n_seq + 1)) : 0;     // int64 sequence offsets [n_seq + 1], copied in by every _seq call
     w.total = p;
     return pl;
 }
@@ -146,24 +162,40 @@ __device__ __forceinline__ float dtanhf_(float v) {
 // backward kernel.  kHeadBce: BCEWithLogitsLoss (mean).  kHeadBcePw: BCEWithLogitsLoss(pos_weight=pw) (mean).
 enum Head : int { kHeadLogits = 0, kHeadBce = 1, kHeadBcePw = 2 };
 
+// The sequences of a batch.  off == nullptr: one sequence of all B rows (with sequence == 0: B sequences of one row),
+// scanned by one CTA.  Otherwise sequence s is rows [off[s], off[s + 1]) and CTA c scans sequences [c per, min(n, (c + 1)
+// per)) in order, each from the zero state.  rows == nullptr: the (only) CTA writes the head's gradients into grad and the
+// mean loss into loss_out; otherwise CTA c writes row c of rows [CTAs][head_row_len(o)] (its gradients of blob entries
+// [o.whh0, o.bo], then its loss sum), which train_head_reduce adds up.
+struct SeqSpan {
+    const int64_t *off;
+    int64_t n;
+    int per;
+    float *rows;
+};
+
 // ------------------------------------------------------------------------------------------------------------------
 // LSTM forward over the batch axis with everything the backward pass needs kept; logits and loss.
-// One CTA of 64 threads: thread r owns gate row r of every matrix; W_ih_l0 f_t was computed before the scan (pre0[t][r]).
-// sequence == 0: every step starts from the zero state (independent windows).  HEAD == kHeadLogits: target and loss_out
-// are not used.
+// A CTA of 64 threads per group of sequences (SeqSpan): thread r owns gate row r of every matrix; W_ih_l0 f_t was
+// computed before the scan (pre0[t][r]).  sequence == 0: every step starts from the zero state (independent windows).
+// HEAD == kHeadLogits: target and loss_out are not used.
 // ------------------------------------------------------------------------------------------------------------------
 template <int HEAD>
 __global__ void __launch_bounds__(64)
-train_lstm_fwd(const float *__restrict__ pre0, const float *__restrict__ prm, BlobOff o, Dims d, int64_t B, int sequence,
+train_lstm_fwd(const float *__restrict__ pre0, const float *__restrict__ prm, BlobOff o, Dims d, int64_t B, int sequence, SeqSpan sq,
                const float *__restrict__ age, const float *__restrict__ target, float pos_weight, float *__restrict__ acts,
                float *__restrict__ cs, float *__restrict__ hs, float *__restrict__ lin, float *__restrict__ z,
                float *__restrict__ loss_out) {
     __shared__ float g[kGates], h0[kHidden], c0[kHidden], h1[kHidden], c1s[kHidden];
     const int r = threadIdx.x;
-    if (r < kHidden) { h0[r] = c0[r] = h1[r] = c1s[r] = 0.f; }
+    // this CTA's sequences [s0, s1); one sequence of all B rows without offsets
+    const int64_t s0 = sq.off ? (int64_t)blockIdx.x * sq.per : 0, s1 = sq.off ? min(sq.n, s0 + sq.per) : 1;
     float loss = 0.f;
+    for (int64_t sid = s0; sid < s1; ++sid) {            // the body is the single-sequence scan, over rows [t0, t1)
+    const int64_t t0 = sq.off ? sq.off[sid] : 0, t1 = sq.off ? sq.off[sid + 1] : B;
+    if (r < kHidden) { h0[r] = c0[r] = h1[r] = c1s[r] = 0.f; }
     __syncthreads();
-    for (int64_t t = 0; t < B; ++t) {
+    for (int64_t t = t0; t < t1; ++t) {
         if (!sequence) {
             if (r < kHidden) { h0[r] = c0[r] = h1[r] = c1s[r] = 0.f; }
             __syncthreads();
@@ -231,35 +263,44 @@ train_lstm_fwd(const float *__restrict__ pre0, const float *__restrict__ prm, Bl
         }
         __syncthreads();
     }
-    if (HEAD != kHeadLogits && r == 0) *loss_out = loss / (float)B;
+    }
+    if (HEAD != kHeadLogits && r == 0) {
+        if (sq.rows) sq.rows[blockIdx.x * head_row_len(o) + head_row_len(o) - 1] = loss;
+        else *loss_out = loss / (float)B;
+    }
 }
 
 // ------------------------------------------------------------------------------------------------------------------
-// BPTT over the batch axis.  64 threads: thread r owns gate row r.  Gradients of the recurrent matrices, biases and of
-// the head are accumulated in registers / shared memory and written once; d(gates of layer 0) goes to da0[t][64].
+// BPTT over the batch axis (over each CTA's sequences, SeqSpan).  64 threads: thread r owns gate row r.  Gradients of
+// the recurrent matrices, biases and of the head are accumulated in registers / shared memory and written once (into
+// grad, or as the CTA's row of sq.rows); d(gates of layer 0) goes to da0[t][64].
 // HEAD == kHeadLogits: d loss / d z is dz_in[t] and, when dage != NULL, d loss / d age goes to dage[t] (torch's relu
 // backward: zero where relu(age * coef + 1) is not positive); otherwise dz comes from z and target, dage is not written.
 // ------------------------------------------------------------------------------------------------------------------
 template <int HEAD>
-__global__ void __launch_bounds__(64)
-train_lstm_bwd(const float *__restrict__ prm, BlobOff o, Dims d, int64_t B, int sequence, const float *__restrict__ age,
+__global__ void __launch_bounds__(64, 1)   // the 48 gradient sums stay in registers: no spill
+train_lstm_bwd(const float *__restrict__ prm, BlobOff o, Dims d, int64_t B, int sequence, SeqSpan sq, const float *__restrict__ age,
                const float *__restrict__ target, float pos_weight, const float *__restrict__ dz_in, const float *__restrict__ acts,
                const float *__restrict__ cs, const float *__restrict__ hs, const float *__restrict__ lin, const float *__restrict__ z,
                float *__restrict__ da0, float *__restrict__ grad, float *__restrict__ dage) {
     __shared__ float da[kGates], dh0c[kHidden], dc0c[kHidden], dh1c[kHidden], dc1c[kHidden], dh0ext[kHidden], dh1ext[kHidden];
     const int r = threadIdx.x, u = r & 15, q = r >> 4;
+    // this CTA's sequences [s0, s1), walked last to first; one sequence of all B rows without offsets
+    const int64_t s0 = sq.off ? (int64_t)blockIdx.x * sq.per : 0, s1 = sq.off ? min(sq.n, s0 + sq.per) : 1;
     float gWhh0[kHidden], gWih1[kHidden], gWhh1[kHidden];
 #pragma unroll
     for (int k = 0; k < kHidden; ++k) gWhh0[k] = gWih1[k] = gWhh1[k] = 0.f;
     float gb0 = 0.f, gb1 = 0.f, gwo = 0.f, gbo = 0.f;
+    for (int64_t sid = s1 - 1; sid >= s0; --sid) {       // the body is the single-sequence walk, over rows [t0, t1)
+    const int64_t t0 = sq.off ? sq.off[sid] : 0, t1 = sq.off ? sq.off[sid + 1] : B;
     if (r < kHidden) dh0c[r] = dc0c[r] = dh1c[r] = dc1c[r] = 0.f;
     __syncthreads();
-    for (int64_t t = B - 1; t >= 0; --t) {
+    for (int64_t t = t1 - 1; t >= t0; --t) {
         if (!sequence) {
             if (r < kHidden) dh0c[r] = dc0c[r] = dh1c[r] = dc1c[r] = 0.f;
             __syncthreads();
         }
-        const bool first = !sequence || t == 0;               // no previous step: h_{t-1} = c_{t-1} = 0
+        const bool first = !sequence || t == t0;              // no previous step: h_{t-1} = c_{t-1} = 0
         // ---- head: z = (wo . h1 + bo) * s
         float s = __fadd_rn(__fmul_rn(age[t], d.age_coef), 1.0f);
         s = (s > 0.f || s != s) ? s : 0.f;
@@ -343,16 +384,32 @@ train_lstm_bwd(const float *__restrict__ prm, BlobOff o, Dims d, int64_t B, int 
         }
         __syncthreads();
     }
+    }
+    // blob entry e of the head goes to grad[e], or to entry e - o.whh0 of this CTA's row
+    float *const gout = sq.rows ? sq.rows + blockIdx.x * head_row_len(o) : grad;
+    const int64_t base = sq.rows ? o.whh0 : 0;
 #pragma unroll
     for (int k = 0; k < kHidden; ++k) {
-        grad[o.whh0 + r * kHidden + k] = gWhh0[k];
-        grad[o.wih1 + r * kHidden + k] = gWih1[k];
-        grad[o.whh1 + r * kHidden + k] = gWhh1[k];
+        gout[o.whh0 - base + r * kHidden + k] = gWhh0[k];
+        gout[o.wih1 - base + r * kHidden + k] = gWih1[k];
+        gout[o.whh1 - base + r * kHidden + k] = gWhh1[k];
     }
-    grad[o.bih0 + r] = gb0; grad[o.bhh0 + r] = gb0;
-    grad[o.bih1 + r] = gb1; grad[o.bhh1 + r] = gb1;
-    if (r < kHidden) grad[o.wo + r] = gwo;
-    if (r == 0) grad[o.bo] = gbo;
+    gout[o.bih0 - base + r] = gb0; gout[o.bhh0 - base + r] = gb0;
+    gout[o.bih1 - base + r] = gb1; gout[o.bhh1 - base + r] = gb1;
+    if (r < kHidden) gout[o.wo - base + r] = gwo;
+    if (r == 0) gout[o.bo - base] = gbo;
+}
+
+// grad[o.whh0 + e] = the sum of rows[c][e] over the scan CTAs c in order, i.e. in sequence order (no atomic: gradients
+// repeat bit for bit); the rows' last column is the loss sum, and loss_out (when not NULL) gets that sum / B
+__global__ void __launch_bounds__(256)
+train_head_reduce(const float *__restrict__ rows, int n_rows, BlobOff o, int64_t B, float *__restrict__ grad, float *__restrict__ loss_out) {
+    const int64_t len = head_row_len(o), e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= len) return;
+    float a = rows[e];
+    for (int c = 1; c < n_rows; ++c) a += rows[c * len + e];
+    if (e < len - 1) grad[o.whh0 + e] = a;
+    else if (loss_out) *loss_out = a / (float)B;
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -721,11 +778,12 @@ static bool train_geometry(const b2cnn_config *cfg, Dims &d, const char **err) {
     return true;
 }
 
-int64_t train_workspace_bytes(const b2cnn_config *cfg, int64_t B) {
+int64_t train_workspace_bytes(const b2cnn_config *cfg, int64_t B, const SeqLengths &sl) {
     Dims d;
     const char *err = "";
-    if (B < 1 || !train_geometry(cfg, d, &err)) return -1;
-    return train_plan(d, B).w.total * (int64_t)sizeof(float);
+    std::vector<int64_t> off;
+    if (B < 1 || !train_geometry(cfg, d, &err) || (sl.on && !seq_offsets(sl, B, off, &err))) return -1;
+    return train_plan(d, B, sl.on ? sl.n : 0).w.total * (int64_t)sizeof(float);
 }
 
 // what the kernels need beyond a valid geometry; no CUDA call
@@ -775,25 +833,49 @@ static bool launch_backward_tail(const Dims &d, const BlobOff &o, const TrainPla
 }
 
 // The checks every training entry point shares, before any CUDA call: the configuration, the mode, the pointers the call
-// needs (ptrs_ok) and the batch, what the kernels hold, and the workspace size.
-static int train_args(const b2cnn_config *cfg, int64_t B, int mode, bool ptrs_ok, int64_t ws_bytes, Dims &d, TrainPlan &pl,
-                      const char **err) {
+// needs (ptrs_ok) and the batch, the sequence lengths of a _seq call (into off), what the kernels hold, and the workspace
+// size.
+static int train_args(const b2cnn_config *cfg, int64_t B, int mode, const SeqLengths &sl, bool ptrs_ok, int64_t ws_bytes, Dims &d,
+                      TrainPlan &pl, std::vector<int64_t> &off, const char **err) {
     if (!train_geometry(cfg, d, err)) return B2CNN_EINVAL;
     if (mode != B2CNN_MODE_INDEPENDENT && mode != B2CNN_MODE_SEQUENCE) { *err = "training: bad mode"; return B2CNN_EINVAL; }
     if (!ptrs_ok || B < 1) { *err = "training: null argument / bad batch"; return B2CNN_EINVAL; }
-    pl = train_plan(d, B);
+    if (sl.on && !seq_offsets(sl, B, off, err)) return B2CNN_EINVAL;
+    pl = train_plan(d, B, sl.on ? sl.n : 0);
     if (!plan_fits(d, pl, B, err)) return B2CNN_EINVAL;
-    if (ws_bytes < pl.w.total * (int64_t)sizeof(float)) { *err = "training: workspace smaller than b2cnn_train_workspace_bytes()"; return B2CNN_ESTATE; }
+    if (ws_bytes < pl.w.total * (int64_t)sizeof(float)) {
+        *err = sl.on ? "training: workspace smaller than b2cnn_train_workspace_bytes_seq()" : "training: workspace smaller than b2cnn_train_workspace_bytes()";
+        return B2CNN_ESTATE;
+    }
     return B2CNN_OK;
+}
+
+// The scan's SeqSpan; a _seq call first copies its offsets into the workspace (from pageable memory: the copy has read
+// `off` when it returns)
+static bool seq_span(const TrainPlan &pl, const std::vector<int64_t> &off, float *ws, cudaStream_t st, SeqSpan &sq) {
+    sq = SeqSpan{nullptr, 0, 1, nullptr};
+    if (off.empty()) return true;
+    int64_t *doff = reinterpret_cast<int64_t *>(ws + pl.w.off);
+    if (cudaMemcpyAsync(doff, off.data(), sizeof(int64_t) * off.size(), cudaMemcpyHostToDevice, st) != cudaSuccess) return false;
+    sq = SeqSpan{doff, (int64_t)off.size() - 1, pl.seq_per, pl.seq_ctas > 1 ? ws + pl.w.part : nullptr};
+    return true;
+}
+
+// with more than one scan CTA: the head's gradients (and, with loss_out, the mean loss) from the CTAs' rows
+static void launch_head_reduce(const TrainPlan &pl, const BlobOff &o, const SeqSpan &sq, int64_t B, float *grads, float *loss_out,
+                               cudaStream_t st) {
+    if (!sq.rows) return;
+    train_head_reduce<<<(unsigned)((head_row_len(o) + 255) / 256), 256, 0, st>>>(sq.rows, pl.seq_ctas, o, B, grads, loss_out);
 }
 
 int train_step(const b2cnn_config *cfg, float *params, float *adam_m, float *adam_v, float *grads, int64_t step, float lr, float beta1,
                float beta2, float eps, int apply_update, const float *x, int64_t B, const float *age, const float *target,
-               int weighted, float pos_weight, int mode, const float *mask1, const float *mask2, float *loss_out, void *workspace,
-               int64_t ws_bytes, cudaStream_t st, const char **err) {
+               int weighted, float pos_weight, int mode, const SeqLengths &sl, const float *mask1, const float *mask2, float *loss_out,
+               void *workspace, int64_t ws_bytes, cudaStream_t st, const char **err) {
     Dims d;
     TrainPlan pl;
-    const int rc = train_args(cfg, B, mode, params && grads && x && age && target && loss_out && workspace, ws_bytes, d, pl, err);
+    std::vector<int64_t> off;
+    const int rc = train_args(cfg, B, mode, sl, params && grads && x && age && target && loss_out && workspace, ws_bytes, d, pl, off, err);
     if (rc != B2CNN_OK) return rc;
     if (step < 1) { *err = "training: step must be >= 1"; return B2CNN_EINVAL; }
     if (apply_update && (!adam_m || !adam_v)) { *err = "training: Adam state missing"; return B2CNN_EINVAL; }
@@ -804,19 +886,23 @@ int train_step(const b2cnn_config *cfg, float *params, float *adam_m, float *ada
     const BlobOff o = blob_offsets(d);
     const int sequence = mode == B2CNN_MODE_SEQUENCE ? 1 : 0;
     float *ws = reinterpret_cast<float *>(workspace);
+    SeqSpan sq;
+    if (!seq_span(pl, off, ws, st, sq)) { *err = "copy sequence offsets"; return B2CNN_ECUDA; }
     if (cudaMemsetAsync(grads, 0, sizeof(float) * o.total, st) != cudaSuccess) { *err = "memset grads"; return B2CNN_ECUDA; }
     launch_conv_forward(d, o, pl, ws, params, x, B, mask1, mask2, st);
+    const unsigned scans = (unsigned)pl.seq_ctas;
     if (weighted) {
-        train_lstm_fwd<kHeadBcePw><<<1, 64, 0, st>>>(ws + w.pre0, params, o, d, B, sequence, age, target, pos_weight, ws + w.acts, ws + w.cs,
-                                                     ws + w.hs, ws + w.lin, ws + w.z, loss_out);
-        train_lstm_bwd<kHeadBcePw><<<1, 64, 0, st>>>(params, o, d, B, sequence, age, target, pos_weight, nullptr, ws + w.acts, ws + w.cs,
-                                                     ws + w.hs, ws + w.lin, ws + w.z, ws + w.da0, grads, nullptr);
+        train_lstm_fwd<kHeadBcePw><<<scans, 64, 0, st>>>(ws + w.pre0, params, o, d, B, sequence, sq, age, target, pos_weight, ws + w.acts,
+                                                         ws + w.cs, ws + w.hs, ws + w.lin, ws + w.z, loss_out);
+        train_lstm_bwd<kHeadBcePw><<<scans, 64, 0, st>>>(params, o, d, B, sequence, sq, age, target, pos_weight, nullptr, ws + w.acts,
+                                                         ws + w.cs, ws + w.hs, ws + w.lin, ws + w.z, ws + w.da0, grads, nullptr);
     } else {
-        train_lstm_fwd<kHeadBce><<<1, 64, 0, st>>>(ws + w.pre0, params, o, d, B, sequence, age, target, 1.f, ws + w.acts, ws + w.cs,
-                                                   ws + w.hs, ws + w.lin, ws + w.z, loss_out);
-        train_lstm_bwd<kHeadBce><<<1, 64, 0, st>>>(params, o, d, B, sequence, age, target, 1.f, nullptr, ws + w.acts, ws + w.cs,
-                                                   ws + w.hs, ws + w.lin, ws + w.z, ws + w.da0, grads, nullptr);
+        train_lstm_fwd<kHeadBce><<<scans, 64, 0, st>>>(ws + w.pre0, params, o, d, B, sequence, sq, age, target, 1.f, ws + w.acts, ws + w.cs,
+                                                       ws + w.hs, ws + w.lin, ws + w.z, loss_out);
+        train_lstm_bwd<kHeadBce><<<scans, 64, 0, st>>>(params, o, d, B, sequence, sq, age, target, 1.f, nullptr, ws + w.acts, ws + w.cs,
+                                                       ws + w.hs, ws + w.lin, ws + w.z, ws + w.da0, grads, nullptr);
     }
+    launch_head_reduce(pl, o, sq, B, grads, loss_out, st);
     if (!launch_backward_tail(d, o, pl, ws, params, x, B, mask1, mask2, grads, nullptr, false, st)) { *err = "memset dx"; return B2CNN_ECUDA; }
     if (apply_update) {
         const float bc1 = 1.f - powf(beta1, (float)step), bc2 = 1.f - powf(beta2, (float)step);
@@ -827,11 +913,12 @@ int train_step(const b2cnn_config *cfg, float *params, float *adam_m, float *ada
     return B2CNN_OK;
 }
 
-int train_forward(const b2cnn_config *cfg, const float *params, const float *x, int64_t B, const float *age, int mode, const float *mask1,
-                  const float *mask2, float *z_out, void *workspace, int64_t ws_bytes, cudaStream_t st, const char **err) {
+int train_forward(const b2cnn_config *cfg, const float *params, const float *x, int64_t B, const float *age, int mode, const SeqLengths &sl,
+                  const float *mask1, const float *mask2, float *z_out, void *workspace, int64_t ws_bytes, cudaStream_t st, const char **err) {
     Dims d;
     TrainPlan pl;
-    const int rc = train_args(cfg, B, mode, params && x && age && z_out && workspace, ws_bytes, d, pl, err);
+    std::vector<int64_t> off;
+    const int rc = train_args(cfg, B, mode, sl, params && x && age && z_out && workspace, ws_bytes, d, pl, off, err);
     if (rc != B2CNN_OK) return rc;
     DeviceGuard dev(cfg->device);
     if (dev.err != cudaSuccess) { *err = "cudaSetDevice"; return B2CNN_ECUDA; }
@@ -839,20 +926,23 @@ int train_forward(const b2cnn_config *cfg, const float *params, const float *x, 
     const BlobOff o = blob_offsets(d);
     const int sequence = mode == B2CNN_MODE_SEQUENCE ? 1 : 0;
     float *ws = reinterpret_cast<float *>(workspace);
+    SeqSpan sq;
+    if (!seq_span(pl, off, ws, st, sq)) { *err = "copy sequence offsets"; return B2CNN_ECUDA; }
     launch_conv_forward(d, o, pl, ws, params, x, B, mask1, mask2, st);
-    train_lstm_fwd<kHeadLogits><<<1, 64, 0, st>>>(ws + w.pre0, params, o, d, B, sequence, age, nullptr, 1.f, ws + w.acts, ws + w.cs,
-                                                  ws + w.hs, ws + w.lin, z_out, nullptr);
+    train_lstm_fwd<kHeadLogits><<<(unsigned)pl.seq_ctas, 64, 0, st>>>(ws + w.pre0, params, o, d, B, sequence, sq, age, nullptr, 1.f, ws + w.acts,
+                                                                     ws + w.cs, ws + w.hs, ws + w.lin, z_out, nullptr);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) { *err = cudaGetErrorString(e); return B2CNN_ECUDA; }
     return B2CNN_OK;
 }
 
-int train_backward(const b2cnn_config *cfg, const float *params, const float *x, int64_t B, const float *age, int mode,
+int train_backward(const b2cnn_config *cfg, const float *params, const float *x, int64_t B, const float *age, int mode, const SeqLengths &sl,
                    const float *mask1, const float *mask2, const float *dz, float *grads, float *dx, float *dage, int flags,
                    void *workspace, int64_t ws_bytes, cudaStream_t st, const char **err) {
     Dims d;
     TrainPlan pl;
-    const int rc = train_args(cfg, B, mode, params && x && age && dz && grads && workspace, ws_bytes, d, pl, err);
+    std::vector<int64_t> off;
+    const int rc = train_args(cfg, B, mode, sl, params && x && age && dz && grads && workspace, ws_bytes, d, pl, off, err);
     if (rc != B2CNN_OK) return rc;
     if (flags & ~B2CNN_TRAIN_FROZEN_CONV) { *err = "training: unknown flag"; return B2CNN_EINVAL; }
     const bool frozen_conv = (flags & B2CNN_TRAIN_FROZEN_CONV) != 0;
@@ -863,10 +953,13 @@ int train_backward(const b2cnn_config *cfg, const float *params, const float *x,
     const BlobOff o = blob_offsets(d);
     const int sequence = mode == B2CNN_MODE_SEQUENCE ? 1 : 0;
     float *ws = reinterpret_cast<float *>(workspace);
+    SeqSpan sq;
+    if (!seq_span(pl, off, ws, st, sq)) { *err = "copy sequence offsets"; return B2CNN_ECUDA; }
     // zeroed: a frozen front end leaves the conv entries as they are
     if (cudaMemsetAsync(grads, 0, sizeof(float) * o.total, st) != cudaSuccess) { *err = "memset grads"; return B2CNN_ECUDA; }
-    train_lstm_bwd<kHeadLogits><<<1, 64, 0, st>>>(params, o, d, B, sequence, age, nullptr, 1.f, dz, ws + w.acts, ws + w.cs, ws + w.hs,
-                                                  ws + w.lin, nullptr, ws + w.da0, grads, dage);
+    train_lstm_bwd<kHeadLogits><<<(unsigned)pl.seq_ctas, 64, 0, st>>>(params, o, d, B, sequence, sq, age, nullptr, 1.f, dz, ws + w.acts, ws + w.cs,
+                                                                     ws + w.hs, ws + w.lin, nullptr, ws + w.da0, grads, dage);
+    launch_head_reduce(pl, o, sq, B, grads, nullptr, st);
     if (!launch_backward_tail(d, o, pl, ws, params, x, B, mask1, mask2, grads, dx, frozen_conv, st)) { *err = "memset dx"; return B2CNN_ECUDA; }
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) { *err = cudaGetErrorString(e); return B2CNN_ECUDA; }

@@ -314,9 +314,50 @@ class B200MyCNN(nn.Module):
             capi.check(rc, "b2cnn_forward")
         return out
 
+    def _seq_args(self, x: torch.Tensor, age, seq_lengths):
+        """Validates a many-sequence call before anything runs: (x, age as 1 or B float32 values, the host length array)."""
+        x = self._check_x(x)
+        B = x.shape[0]
+        age = (age if torch.is_tensor(age) else torch.tensor(age, dtype=torch.float32)).detach()
+        if age.dim() > 1 or age.numel() not in (1, B):
+            raise ValueError(f"with seq_lengths, age must have 1 or {B} elements (one per window), got shape {tuple(age.shape)}")
+        return x, age.reshape(-1).float().contiguous(), capi.seq_lengths_array(seq_lengths, B)
+
+    def _run_seq(self, x: torch.Tensor, age, seq_lengths, sigmoid: bool) -> torch.Tensor:
+        """Sequence mode over the consecutive sequences ``seq_lengths`` of the batch (b2cnn_forward_seq)."""
+        x, age, lens = self._seq_args(x, age, seq_lengths)
+        lib, h = self._ensure_handle()
+        dev = self._handle_device
+        x, age = x.to(dev), age.to(dev)
+        B = x.shape[0]
+        pitch = 0 if x.is_contiguous() else self._row_pitch(x)
+        if not x.is_contiguous() and not pitch:
+            x = x.contiguous()
+        dtype = capi.DTYPE_BF16 if x.dtype == torch.bfloat16 else capi.DTYPE_F32
+        out = torch.empty(B, dtype=torch.float32, device=dev)
+        with torch.cuda.device(dev):
+            need = int(lib.b2cnn_workspace_bytes_seq(h, B, lens, len(lens)))
+            if need < 0:
+                capi.check(capi.EINVAL, "b2cnn_workspace_bytes_seq")
+            ws = self._ws
+            if ws is None or ws.numel() < need or ws.device != dev:
+                ws = self._ws = torch.empty(need, dtype=torch.uint8, device=dev)
+            capi.check(lib.b2cnn_forward_seq(h, x.data_ptr(), dtype, B, pitch or self.arch.window, age.data_ptr(), age.numel(), lens,
+                                             len(lens), int(sigmoid), out.data_ptr(), ws.data_ptr(), ws.numel(),
+                                             torch.cuda.current_stream().cuda_stream), "b2cnn_forward_seq")
+        return out
+
     @torch.no_grad()
-    def forward(self, x: torch.Tensor, age: torch.Tensor) -> torch.Tensor:
-        """``model(x, age)`` with the reference's semantics (bin/models.py:22-36)."""
+    def forward(self, x: torch.Tensor, age: torch.Tensor, seq_lengths=None) -> torch.Tensor:
+        """``model(x, age)`` with the reference's semantics (bin/models.py:22-36).
+
+        ``seq_lengths`` [n_0, ..., n_{N-1}] (a list, tuple or integer tensor; each >= 1, adding up to B): the batch is N
+        consecutive sequences, each scanned from the zero LSTM state -- ``torch.cat([model(x[o:o+n], age[o:o+n]) for
+        ...])`` in one call.  Sequence mode only (``batch_mode == "sequence"``); age then has 1 or B elements."""
+        if seq_lengths is not None:
+            if self.batch_mode != "sequence":
+                raise ValueError("seq_lengths needs batch_mode == 'sequence'")
+            return self._run_seq(x, age, seq_lengths, False)
         mode = capi.MODE_SEQUENCE if (self.batch_mode == "sequence" and x.shape[0] > 1) else capi.MODE_INDEPENDENT
         B = x.shape[0]
         if age.dim() == 1 and age.numel() in (1, B):
@@ -330,14 +371,21 @@ class B200MyCNN(nn.Module):
         return (y.unsqueeze(1) * age_scale).squeeze(1)
 
     @torch.no_grad()
-    def predict(self, window_tensor: torch.Tensor, age=None, mode: str = "independent",
+    def predict(self, window_tensor: torch.Tensor, age=None, mode: str = "independent", seq_lengths=None,
                 return_prob: bool = False) -> torch.Tensor:
         """Batched dispatch for predictStream's per-row loop (bin/predictStream.py:70-162):
         ``window_tensor`` [B, C, W]; ``age`` scalar / [B] (default 65.0, predictStream.py:149);
-        returns logits [B] or, with ``return_prob``, ``sigmoid(logit)`` (predictStream.py:160)."""
+        returns logits [B] or, with ``return_prob``, ``sigmoid(logit)`` (predictStream.py:160).
+
+        ``mode="sequence", seq_lengths=[n_0, ...]``: the batch is consecutive sequences (each >= 1 window, adding up to
+        B), each scored like ``predict(x_s, age_s, mode="sequence")`` in one call (see :meth:`forward`)."""
         if window_tensor.dim() == 2:
             window_tensor = window_tensor.unsqueeze(0)
         B = window_tensor.shape[0]
+        if seq_lengths is not None:
+            if mode != "sequence":
+                raise ValueError("seq_lengths is only accepted with mode='sequence'")
+            return self._run_seq(window_tensor, 65.0 if age is None else age, seq_lengths, return_prob)
         if age is None:
             age = 65.0
         if not torch.is_tensor(age):

@@ -87,21 +87,35 @@ class B200Trainer:
         return draw_masks(self.model.arch, B, self.dropout, self._params.device, self._gen)
 
     def step(self, x: torch.Tensor, age: torch.Tensor, target: torch.Tensor,
-             masks: Optional[Tuple[Optional[torch.Tensor], Optional[torch.Tensor]]] = None, update: bool = True) -> torch.Tensor:
+             masks: Optional[Tuple[Optional[torch.Tensor], Optional[torch.Tensor]]] = None, update: bool = True,
+             seq_lengths=None) -> torch.Tensor:
         """zero_grad + forward + BCEWithLogitsLoss(pos_weight) + backward + Adam step; returns the batch loss (a 0-d device
-        tensor)."""
+        tensor).
+
+        ``seq_lengths`` [n_0, ..., n_{N-1}] (sequence mode only; a list, tuple or integer tensor, each >= 1, adding up to
+        B): the batch is N consecutive sequences -- one patient's windows each -- and the LSTM starts every one from the
+        zero state, as ``torch.cat([model(x[o:o+n], age[o:o+n]) for ...])`` would; the loss is still the mean over all B
+        windows and one Adam step updates the parameters."""
         dev = self._params.device
         a = self.model.arch
         if x.dim() != 3 or x.shape[1] != a.in_channels or x.shape[2] != a.window:
             raise RuntimeError(f"expected x of shape [B, {a.in_channels}, {a.window}], got {tuple(x.shape)}")
         B = x.shape[0]
+        lens = None
+        if seq_lengths is not None:
+            if self.mode != "sequence":
+                raise ValueError("seq_lengths needs a trainer in mode='sequence'")
+            lens = capi.seq_lengths_array(seq_lengths, B)
         x = x.to(dev, torch.float32).contiguous()
         age = age.to(dev, torch.float32).reshape(-1).contiguous()
         target = target.to(dev, torch.float32).reshape(-1).contiguous()
         if age.numel() != B or target.numel() != B:
             raise RuntimeError("age and target must have one entry per window")
         m1, m2 = check_masks(a, B, dev, *(masks if masks is not None else self.draw_masks(B)))
-        need = self._lib.b2cnn_train_workspace_bytes(ctypes.byref(self._cfg), B)
+        if lens is None:
+            need = self._lib.b2cnn_train_workspace_bytes(ctypes.byref(self._cfg), B)
+        else:
+            need = self._lib.b2cnn_train_workspace_bytes_seq(ctypes.byref(self._cfg), B, lens, len(lens))
         if need < 0:
             capi.check(capi.EINVAL, "b2cnn_train_workspace_bytes")
         if self._ws is None or self._ws.numel() < need:
@@ -112,7 +126,10 @@ class B200Trainer:
                 ctypes.byref(self._opt), 1 if update else 0, ptr(x), B, ptr(age), ptr(target))
         tail = (capi.MODE_SEQUENCE if self.mode == "sequence" else capi.MODE_INDEPENDENT, ptr(m1), ptr(m2), ptr(self._loss),
                 ptr(self._ws), need, ctypes.c_void_p(st))
-        if self.pos_weight is None:
+        if lens is not None:
+            pw = None if self.pos_weight is None else ctypes.byref(ctypes.c_float(self.pos_weight))
+            capi.check(self._lib.b2cnn_train_step_seq(*head, pw, lens, len(lens), *tail[1:]), "b2cnn_train_step_seq")
+        elif self.pos_weight is None:
             capi.check(self._lib.b2cnn_train_step(*head, *tail), "b2cnn_train_step")
         else:
             capi.check(self._lib.b2cnn_train_step_weighted(*head, self.pos_weight, *tail), "b2cnn_train_step_weighted")
