@@ -596,6 +596,40 @@ int b2cnn_train_backward_seq(const b2cnn_config *cfg, const float *params, const
                              float *grads, float *dx, float *dage, int flags, void *workspace, int64_t workspace_bytes,
                              void *stream);
 
+/* ---- Training on whole recordings ----
+ * The _record variants take `records` [B][C][N] (contiguous fp32, N >= the window W) in place of windows, a window
+ * stride `stride` S (a positive multiple of the feature stride pool_s^2) and a HOST array window_counts[B]: recording b
+ * contributes its windows w = 0 .. window_counts[b] - 1, window w being samples [w S, w S + W).  Every count lies in
+ * [0, n_w], n_w = (N - W) / S + 1 (0 when N < W), and the counts add up to M >= 1.  The M windows are the rows, in
+ * recording-major, window order: age[M], target[M], z_out[M], dz[M] and dage[M] are per window.
+ * mode B2CNN_MODE_SEQUENCE: each recording's windows are one sequence, the LSTM starting from the zero state (the _seq
+ * calls with the non-zero counts as lengths); B2CNN_MODE_INDEPENDENT: every window alone.  The dropout masks belong to
+ * the recording: mask1 [B][4][P1(N)] and mask2 [B][L(N)], the geometry of a window of N samples, and window w uses
+ * mask1[b][:][w S / pool_s + i] and mask2[b][w S / pool_s^2 + j], so a feature two windows share is dropped in both or
+ * in neither.  The logits, the loss and the LSTM / Linear gradients (W_ih_l0 included) are the bits of the _seq /
+ * independent call on the windows cut out of the recordings with their masks cut the same way; the conv gradients and
+ * d_records sum each shared feature's gradient over its windows before the conv backward, so they match those sums up
+ * to rounding.  Samples no counted window reads (a recording's tail, the gaps when S > W, a recording with count 0)
+ * change nothing: NaN or inf there gives the bits that zeros give, and d_records[B][C][N] (or NULL) is 0 there.
+ * Bad strides, counts or lengths are B2CNN_EINVAL before any CUDA call; the workspace is
+ * b2cnn_train_workspace_bytes_record() bytes (a smaller one is B2CNN_ESTATE before any launch), and the calls copy the
+ * counts' offsets into it on `stream`.  b2cnn_train_step_record: pos_weight NULL or one host float (> 0 and finite).
+ * b2cnn_train_backward_record takes the arguments its forward took and the flags of b2cnn_train_backward_ex. */
+int64_t b2cnn_train_workspace_bytes_record(const b2cnn_config *cfg, int64_t B, int64_t N, int64_t stride, const int64_t *window_counts,
+                                           int mode);
+int b2cnn_train_step_record(const b2cnn_config *cfg, float *params, float *adam_m, float *adam_v, float *grads, int64_t step,
+                            const b2cnn_adam *opt, int apply_update, const float *records, int64_t B, int64_t N, int64_t stride,
+                            const int64_t *window_counts, int mode, const float *age, const float *target, const float *pos_weight,
+                            const float *mask1, const float *mask2, float *loss_out, void *workspace, int64_t workspace_bytes,
+                            void *stream);
+int b2cnn_train_forward_record(const b2cnn_config *cfg, const float *params, const float *records, int64_t B, int64_t N, int64_t stride,
+                               const int64_t *window_counts, int mode, const float *age, const float *mask1, const float *mask2,
+                               float *z_out, void *workspace, int64_t workspace_bytes, void *stream);
+int b2cnn_train_backward_record(const b2cnn_config *cfg, const float *params, const float *records, int64_t B, int64_t N, int64_t stride,
+                                const int64_t *window_counts, int mode, const float *age, const float *mask1, const float *mask2,
+                                const float *dz, float *grads, float *d_records, float *dage, int flags, void *workspace,
+                                int64_t workspace_bytes, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

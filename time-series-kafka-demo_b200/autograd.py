@@ -16,11 +16,14 @@ upstream gradient the loss produces.  With ``conv1`` / ``conv2`` frozen (``requi
 needs no gradient, the convolutional backward is skipped altogether.  In ``eval()`` mode it is the inference path of
 :class:`B200MyCNN`; optimizer steps edit the parameters in place, so the next inference call re-uploads them.
 
-:func:`mycnn_train_forward` is the same computation as a function of explicit parameters and dropout masks.
+:func:`mycnn_train_forward` is the same computation as a function of explicit parameters and dropout masks, and
+:func:`mycnn_train_record_forward` the same over every sliding window of whole recordings ``[B, C, N]``, each window
+feature computed and back-propagated once.
 """
 from __future__ import annotations
 
 import ctypes
+import operator
 from typing import Optional, Sequence
 
 import torch
@@ -69,8 +72,70 @@ def check_masks(arch: ArchConfig, B: int, device, mask1: Optional[torch.Tensor],
     return out
 
 
+def check_record_batch(arch: ArchConfig, records: torch.Tensor, stride, age, window_counts):
+    """The arguments of a whole-recording training call, refused (ValueError) before anything runs: ``records``
+    [B, C, N] float32 / bfloat16, ``stride`` a positive multiple of the feature stride ``pool_s ** 2``, ``age`` a scalar
+    or one value per recording, ``window_counts`` as :func:`capi.window_counts_array` takes it.  Returns ``(stride, age,
+    counts, M, rarch)``: age flattened (still differentiable), the host counts array, the number of windows and the
+    geometry of a window of N samples (the dropout masks' shape)."""
+    C = arch.in_channels
+    if not torch.is_tensor(records) or records.dim() != 3 or records.shape[1] != C:
+        got = tuple(records.shape) if torch.is_tensor(records) else type(records).__name__
+        raise ValueError(f"expected records [B, {C}, N], got {got}")
+    if records.dtype not in (torch.float32, torch.bfloat16):
+        raise ValueError(f"records must be float32 or bfloat16, got {records.dtype}")
+    B, N = records.shape[0], records.shape[2]
+    if B < 1:
+        raise ValueError("records must hold at least one recording")
+    if isinstance(stride, bool):
+        raise ValueError("stride must be an integer, got bool")
+    try:
+        stride = operator.index(stride)
+    except TypeError:
+        raise ValueError(f"stride must be an integer, got {type(stride).__name__}") from None
+    F = arch.pool_s ** 2
+    if stride < 1 or stride % F:
+        raise ValueError(f"stride must be a positive multiple of the feature stride {F}, got {stride}")
+    counts, M = capi.window_counts_array(window_counts, B, N, arch.window, stride)
+    age = (age if torch.is_tensor(age) else torch.tensor(age, dtype=torch.float32)).reshape(-1)
+    if age.numel() not in (1, B):
+        raise ValueError(f"age must be a scalar or have {B} elements (one per recording), got {age.numel()}")
+    return stride, age, counts, M, arch.with_shape(C, N)
+
+
+def window_ages(age: torch.Tensor, counts, M: int, device) -> torch.Tensor:
+    """One age per window [M] from one per recording (or a scalar): every window of recording b takes age[b]
+    (``get_arr``).  Differentiable, so autograd sums d age over each recording's windows."""
+    age = age.to(device, torch.float32)
+    if age.numel() == 1:
+        return age.expand(M).contiguous()
+    return age.repeat_interleave(torch.tensor(list(counts), device=device), output_size=M).contiguous()
+
+
+def cut_record_windows(records: torch.Tensor, window: int, stride: int, counts, pool_s: int, mask1=None, mask2=None):
+    """The windows the ``_record`` training calls train on, cut out as copies: ``[M, C, W]`` (recording-major, window
+    order, ``counts[b]`` windows of recording b) and the recording's dropout masks cut the same way (window w of
+    recording b: ``mask1[b, :, wS/pool_s : wS/pool_s + P1]`` and ``mask2[b, wS/pool_s**2 : wS/pool_s**2 + L]``), or None
+    where a mask is None.  ``B200Trainer.step`` on these equals ``step_record`` on the recordings."""
+    counts = [int(c) for c in counts]
+    sel = [(b, w) for b, n in enumerate(counts) for w in range(n)]
+    bi = torch.tensor([b for b, _ in sel], device=records.device)
+    wi = torch.tensor([w for _, w in sel], device=records.device)
+    x = records.unfold(2, window, stride)[bi, :, wi]
+    out = [x.contiguous()]
+    for m, unit in ((mask1, pool_s), (mask2, pool_s ** 2)):
+        if m is None:
+            out.append(None)
+            continue
+        P = m.shape[-1] - (records.shape[2] - window) // unit          # the window's P1 / L
+        cut = m.unfold(-1, P, stride // unit)
+        out.append((cut[bi, :, wi] if m.dim() == 3 else cut[bi, wi]).contiguous())
+    return tuple(out)
+
+
 class _TrainForward(torch.autograd.Function):
-    """Inputs: a :class:`_Call` (non-tensor), x [B,C,W] fp32, age [B] fp32, then the 14 ``BLOB_KEYS`` tensors."""
+    """Inputs: a :class:`_Call` (non-tensor), x [B,C,W] fp32 (with a record call the recordings [B,C,N]), age [rows]
+    fp32, then the 14 ``BLOB_KEYS`` tensors."""
 
     @staticmethod
     def forward(ctx, call, x, age, *params):
@@ -78,9 +143,13 @@ class _TrainForward(torch.autograd.Function):
         blob = torch.cat([p.detach().reshape(-1) for p in params])               # the packed blob (include/b2cnn.h)
         B = x.shape[0]
         ws = torch.empty(call.workspace_bytes(B), dtype=torch.uint8, device=dev)
-        z = torch.empty(B, dtype=torch.float32, device=dev)
+        z = torch.empty(age.numel(), dtype=torch.float32, device=dev)
         st = torch.cuda.current_stream(dev).cuda_stream
-        if call.lens is None:
+        if call.rec is not None:
+            N, S, counts, _ = call.rec
+            rc = call.lib.b2cnn_train_forward_record(ctypes.byref(call.cfg), _ptr(blob), _ptr(x), B, N, S, counts, call.mode, _ptr(age),
+                                                     _ptr(call.mask1), _ptr(call.mask2), _ptr(z), _ptr(ws), ws.numel(), ctypes.c_void_p(st))
+        elif call.lens is None:
             rc = call.lib.b2cnn_train_forward(ctypes.byref(call.cfg), _ptr(blob), _ptr(x), B, _ptr(age), call.mode,
                                               _ptr(call.mask1), _ptr(call.mask2), _ptr(z), _ptr(ws), ws.numel(), ctypes.c_void_p(st))
         else:
@@ -106,7 +175,12 @@ class _TrainForward(torch.autograd.Function):
         frozen = dx is None and not any(ctx.needs_input_grad[3:7])
         st = torch.cuda.current_stream(x.device).cuda_stream
         flags = capi.TRAIN_FROZEN_CONV if frozen else 0
-        if call.lens is None:
+        if call.rec is not None:
+            N, S, counts, _ = call.rec
+            rc = call.lib.b2cnn_train_backward_record(ctypes.byref(call.cfg), _ptr(blob), _ptr(x), B, N, S, counts, call.mode, _ptr(age),
+                                                      _ptr(call.mask1), _ptr(call.mask2), _ptr(dz), _ptr(grads), _ptr(dx), _ptr(dage), flags,
+                                                      _ptr(ws), ws.numel(), ctypes.c_void_p(st))
+        elif call.lens is None:
             rc = call.lib.b2cnn_train_backward_ex(ctypes.byref(call.cfg), _ptr(blob), _ptr(x), B, _ptr(age), call.mode, _ptr(call.mask1),
                                                   _ptr(call.mask2), _ptr(dz), _ptr(grads), _ptr(dx), _ptr(dage), flags, _ptr(ws),
                                                   ws.numel(), ctypes.c_void_p(st))
@@ -124,22 +198,41 @@ class _TrainForward(torch.autograd.Function):
 
 
 class _Call:
-    """What one forward / backward pair shares besides tensors: the library, its configuration, mode, masks and sequence
-    lengths (the host array of the _seq calls, or None)."""
+    """What one forward / backward pair shares besides tensors: the library, its configuration, mode, masks, sequence
+    lengths (the host array of the _seq calls, or None) and, for the _record calls, (N, stride, counts array, M)."""
 
-    def __init__(self, arch: ArchConfig, device: torch.device, mode: int, mask1, mask2, lens=None):
+    def __init__(self, arch: ArchConfig, device: torch.device, mode: int, mask1, mask2, lens=None, rec=None):
         self.lib = capi.load_library()
         self.cfg = capi.make_config(arch, device.index if device.index is not None else torch.cuda.current_device())
-        self.mode, self.mask1, self.mask2, self.lens = mode, mask1, mask2, lens
+        self.mode, self.mask1, self.mask2, self.lens, self.rec = mode, mask1, mask2, lens, rec
 
     def workspace_bytes(self, B: int) -> int:
-        if self.lens is None:
+        if self.rec is not None:
+            N, S, counts, _ = self.rec
+            need = int(self.lib.b2cnn_train_workspace_bytes_record(ctypes.byref(self.cfg), B, N, S, counts, self.mode))
+        elif self.lens is None:
             need = int(self.lib.b2cnn_train_workspace_bytes(ctypes.byref(self.cfg), B))
         else:
             need = int(self.lib.b2cnn_train_workspace_bytes_seq(ctypes.byref(self.cfg), B, self.lens, len(self.lens)))
         if need < 0:
             capi.check(capi.EINVAL, "b2cnn_train_workspace_bytes")
         return need
+
+
+def _check_params(params: Sequence[torch.Tensor], arch: ArchConfig) -> torch.device:
+    """The 14 ``BLOB_KEYS`` tensors of ``arch``: float32, on one CUDA device (returned)."""
+    if len(params) != len(BLOB_KEYS):
+        raise ValueError(f"expected the {len(BLOB_KEYS)} tensors of BLOB_KEYS, got {len(params)}")
+    shapes = arch.param_shapes()
+    for k, p in zip(BLOB_KEYS, params):
+        if tuple(p.shape) != shapes[k]:
+            raise RuntimeError(f"{k}: expected shape {shapes[k]}, got {tuple(p.shape)}")
+    dev = params[0].device
+    if dev.type != "cuda" or any(p.device != dev for p in params):
+        raise RuntimeError("training on the device needs every parameter on one CUDA device (there is no CPU fallback)")
+    if any(p.dtype != torch.float32 for p in params):
+        raise RuntimeError("training on the device needs float32 parameters")
+    return dev
 
 
 def mycnn_train_forward(x: torch.Tensor, age: torch.Tensor, params: Sequence[torch.Tensor], arch: ArchConfig,
@@ -158,17 +251,7 @@ def mycnn_train_forward(x: torch.Tensor, age: torch.Tensor, params: Sequence[tor
         raise ValueError("mode must be 'sequence' or 'independent'")
     if seq_lengths is not None and mode != "sequence":
         raise ValueError("seq_lengths is only accepted with mode='sequence'")
-    if len(params) != len(BLOB_KEYS):
-        raise ValueError(f"expected the {len(BLOB_KEYS)} tensors of BLOB_KEYS, got {len(params)}")
-    shapes = arch.param_shapes()
-    for k, p in zip(BLOB_KEYS, params):
-        if tuple(p.shape) != shapes[k]:
-            raise RuntimeError(f"{k}: expected shape {shapes[k]}, got {tuple(p.shape)}")
-    dev = params[0].device
-    if dev.type != "cuda" or any(p.device != dev for p in params):
-        raise RuntimeError("training on the device needs every parameter on one CUDA device (there is no CPU fallback)")
-    if any(p.dtype != torch.float32 for p in params):
-        raise RuntimeError("training on the device needs float32 parameters")
+    dev = _check_params(params, arch)
     if x.dim() != 3 or x.shape[1] != arch.in_channels or x.shape[2] != arch.window:
         raise RuntimeError(f"expected x of shape [B, {arch.in_channels}, {arch.window}], got {tuple(x.shape)}")
     B = x.shape[0]
@@ -188,6 +271,35 @@ def mycnn_train_forward(x: torch.Tensor, age: torch.Tensor, params: Sequence[tor
     age = age.contiguous()
     call = _Call(arch, dev, _MODES[mode], *check_masks(arch, B, dev, mask1, mask2), lens=lens)
     return _TrainForward.apply(call, x, age, *params)
+
+
+def mycnn_train_record_forward(records: torch.Tensor, stride: int, age, params: Sequence[torch.Tensor], arch: ArchConfig,
+                               mode: str = "sequence", mask1: Optional[torch.Tensor] = None, mask2: Optional[torch.Tensor] = None,
+                               window_counts=None) -> torch.Tensor:
+    """Logits [M] of every counted window of whole recordings in train() mode, differentiable in ``records``, ``age``
+    and ``params``; each window feature is computed, and back-propagated, once however many windows share it.
+
+    ``records`` [B, C, N] (fp32 or bf16; cast to fp32); window w of recording b is ``records[b, :, w*stride :
+    w*stride + W]``, for w < ``window_counts[b]`` (default: all n_w = (N - W) // stride + 1 of them; a count may be
+    smaller, down to 0, so recordings of different lengths can be padded to one N).  The logits are recording-major, in
+    window order.  ``stride``: a positive multiple of the feature stride ``pool_s ** 2``.  ``age``: a scalar or one value
+    per recording, every window of recording b taking age[b] (its gradient sums over the recording's windows).
+    ``mode``: "sequence" (each recording's windows one sequence, the LSTM from the zero state -- ``seq_lengths`` = the
+    non-zero counts) or "independent".  ``mask1`` [B, c_mid, P1(N)] / ``mask2`` [B, L(N)]: the recording's dropout
+    masks, the geometry of a window of N samples (``arch.with_shape(C, N)``); window w uses the slices at its own
+    positions, so a feature two windows share is dropped in both or in neither (the one difference from cutting the
+    windows first and drawing their masks independently).  Samples no counted window reads change nothing, NaN
+    included, and get a zero gradient."""
+    check_trainable(arch)
+    if mode not in _MODES:
+        raise ValueError("mode must be 'sequence' or 'independent'")
+    dev = _check_params(params, arch)
+    stride, age, counts, M, rarch = check_record_batch(arch, records, stride, age, window_counts)
+    B, N = records.shape[0], records.shape[2]
+    masks = check_masks(rarch, B, dev, mask1, mask2)
+    records = records.to(dev, torch.float32).contiguous()
+    call = _Call(arch, dev, _MODES[mode], *masks, rec=(N, stride, counts, M))
+    return _TrainForward.apply(call, records, window_ages(age, counts, M, dev), *params)
 
 
 class B200TrainableMyCNN(B200MyCNN):
@@ -212,9 +324,11 @@ class B200TrainableMyCNN(B200MyCNN):
     def train(self, mode: bool = True):
         return nn.Module.train(self, mode)
 
-    def draw_masks(self, B: int):
-        """The two nn.Dropout masks of bin/models.py:25,28 with ``p = self.dropout.p``, from torch's default generator."""
-        return draw_masks(self.arch, B, float(self.dropout.p), self._device())
+    def draw_masks(self, B: int, n_samples: Optional[int] = None):
+        """The two nn.Dropout masks of bin/models.py:25,28 with ``p = self.dropout.p``, from torch's default generator;
+        with ``n_samples``, those of B recordings of that many samples (:meth:`forward_record`)."""
+        arch = self.arch if n_samples is None else self.arch.with_shape(self.arch.in_channels, n_samples)
+        return draw_masks(arch, B, float(self.dropout.p), self._device())
 
     def forward(self, x: torch.Tensor, age: torch.Tensor, seq_lengths=None) -> torch.Tensor:
         """``model(x, age)`` (bin/models.py:22-36): differentiable in train mode, the inference path in eval mode.
@@ -233,3 +347,20 @@ class B200TrainableMyCNN(B200MyCNN):
         m1, m2 = self.draw_masks(B)
         named = dict(self.named_parameters())
         return mycnn_train_forward(x, age, [named[k] for k in BLOB_KEYS], self.arch, mode, m1, m2, seq_lengths)
+
+    def forward_record(self, records: torch.Tensor, stride: int, age, window_counts=None) -> torch.Tensor:
+        """Logits [M] of every counted window of whole recordings ``[B, C, N]`` (see :func:`mycnn_train_record_forward`),
+        recording-major: in train mode differentiable, with the dropout masks drawn at the recording's geometry and the
+        LSTM over each recording's windows (``batch_mode == "sequence"``) or every window alone; in eval mode
+        ``predict_record(records, stride, age, mode=batch_mode)`` with each row cut to its count."""
+        stride, _, counts, M, _ = check_record_batch(self.arch, records, stride, age, window_counts)
+        if not self.training:
+            out = self.predict_record(records, stride, age, mode=self.batch_mode)
+            keep = torch.arange(out.shape[1], device=out.device) < torch.tensor(list(counts), device=out.device)[:, None]
+            return out[keep]
+        if self._device().type != "cuda":
+            raise RuntimeError("B200TrainableMyCNN needs the model on a CUDA device to train (there is no CPU fallback)")
+        m1, m2 = self.draw_masks(records.shape[0], records.shape[2])
+        named = dict(self.named_parameters())
+        return mycnn_train_record_forward(records, stride, age, [named[k] for k in BLOB_KEYS], self.arch, self.batch_mode, m1, m2,
+                                          window_counts)

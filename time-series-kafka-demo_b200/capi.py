@@ -29,6 +29,7 @@ SYMBOLS = ("b2cnn_l_out", "b2cnn_weight_count", "b2cnn_create", "b2cnn_destroy",
            "b2cnn_train_step_weighted", "b2cnn_train_forward", "b2cnn_train_backward", "b2cnn_train_backward_ex",
            "b2cnn_train_workspace_bytes_seq", "b2cnn_train_step_seq", "b2cnn_train_forward_seq", "b2cnn_train_backward_seq",
            "b2cnn_workspace_bytes_seq", "b2cnn_forward_seq",
+           "b2cnn_train_workspace_bytes_record", "b2cnn_train_step_record", "b2cnn_train_forward_record", "b2cnn_train_backward_record",
            "b2cnn_prep_window_count", "b2cnn_prep_workspace_bytes", "b2cnn_prep_windows",
            "b2cnn_ring_create", "b2cnn_ring_destroy", "b2cnn_ring_reset", "b2cnn_ring_set_signals", "b2cnn_ring_push",
            "b2cnn_slide_create", "b2cnn_slide_destroy", "b2cnn_slide_reset", "b2cnn_slide_push", "b2cnn_slide_features",
@@ -206,6 +207,16 @@ def load_library() -> ctypes.CDLL:
     lib.b2cnn_train_backward_seq.argtypes = [cfgp, c_vp, c_vp, c_i64, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_vp,
                                              c_i64, c_vp]
     lib.b2cnn_train_backward_seq.restype = c_int
+    lib.b2cnn_train_workspace_bytes_record.argtypes = [cfgp, c_i64, c_i64, c_i64, c_vp, c_int]
+    lib.b2cnn_train_workspace_bytes_record.restype = c_i64
+    lib.b2cnn_train_step_record.argtypes = [cfgp, c_vp, c_vp, c_vp, c_vp, c_i64, ctypes.POINTER(Adam), c_int, c_vp, c_i64, c_i64, c_i64, c_vp,
+                                            c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp]
+    lib.b2cnn_train_step_record.restype = c_int
+    lib.b2cnn_train_forward_record.argtypes = [cfgp, c_vp, c_vp, c_i64, c_i64, c_i64, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp]
+    lib.b2cnn_train_forward_record.restype = c_int
+    lib.b2cnn_train_backward_record.argtypes = [cfgp, c_vp, c_vp, c_i64, c_i64, c_i64, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
+                                                c_int, c_vp, c_i64, c_vp]
+    lib.b2cnn_train_backward_record.restype = c_int
     lib.b2cnn_workspace_bytes_seq.argtypes = [c_vp, c_i64, c_vp, c_i64]; lib.b2cnn_workspace_bytes_seq.restype = c_i64
     lib.b2cnn_forward_seq.argtypes = [c_vp, c_vp, c_int, c_i64, c_i64, c_vp, c_i64, c_vp, c_i64, c_int, c_vp, c_vp, c_i64, c_vp]
     lib.b2cnn_forward_seq.restype = c_int
@@ -257,6 +268,49 @@ def seq_lengths_array(seq_lengths, B: int):
     if sum(out) != B:
         raise ValueError(f"seq_lengths add up to {sum(out)}, the batch has {B} windows")
     return (ctypes.c_int64 * len(out))(*out)
+
+
+def record_window_count(N: int, W: int, stride: int) -> int:
+    """n_w: the windows of W samples every ``stride`` samples that fit in N samples, (N - W) // stride + 1 (0 when N < W)."""
+    return (N - W) // stride + 1 if N >= W else 0
+
+
+def window_counts_array(window_counts, B: int, N: int, W: int, stride: int):
+    """``window_counts`` (None for every recording's n_w windows; else a list, tuple or 1-d integer tensor of B counts,
+    each in [0, n_w], adding up to at least 1) as the host int64 array the ``_record`` training calls take, and their sum
+    M; ValueError for anything else.  Recording b contributes its windows 0 .. count_b - 1."""
+    import operator
+
+    import torch
+    n_w = record_window_count(N, W, stride)
+    if window_counts is None:
+        vals = [n_w] * B
+    elif isinstance(window_counts, (list, tuple)):
+        vals = list(window_counts)
+    elif torch.is_tensor(window_counts):
+        if window_counts.dim() != 1 or window_counts.dtype.is_floating_point or window_counts.dtype.is_complex \
+                or window_counts.dtype == torch.bool:
+            raise ValueError(f"window_counts must be a 1-d integer tensor, got {window_counts.dtype} of shape {tuple(window_counts.shape)}")
+        vals = window_counts.tolist()
+    else:
+        raise ValueError(f"window_counts must be a list, tuple or integer tensor, got {type(window_counts).__name__}")
+    if len(vals) != B:
+        raise ValueError(f"window_counts has {len(vals)} entries, the batch has {B} recordings")
+    out = []
+    for i, v in enumerate(vals):
+        if isinstance(v, bool):
+            raise ValueError(f"window_counts[{i}] must be an integer, got bool")
+        try:
+            v = operator.index(v)
+        except TypeError:
+            raise ValueError(f"window_counts[{i}] must be an integer, got {type(v).__name__}") from None
+        if not 0 <= v <= n_w:
+            raise ValueError(f"window_counts[{i}] = {v}: a recording of N = {N} samples holds 0 .. {n_w} windows of W = {W} "
+                             f"every {stride} samples")
+        out.append(v)
+    if sum(out) < 1:
+        raise ValueError(f"the recordings hold no window (N = {N}, W = {W}, stride = {stride}, counts add up to 0)")
+    return (ctypes.c_int64 * B)(*out), sum(out)
 
 
 def make_config(arch, device: int = -1) -> Config:

@@ -90,25 +90,26 @@ extern "C" const char *b2cnn_last_error(void) { return g_err.c_str(); }
 
 // ---- one training step (b2cnn_train.cu) ----
 static constexpr SeqLengths kNoSeq{false, nullptr, 0};
+static constexpr RecordArgs kNoRec{false, 0, 0, nullptr};
 
 extern "C" int64_t b2cnn_train_workspace_bytes(const b2cnn_config *cfg, int64_t B) {
-    const int64_t n = train_workspace_bytes(cfg, B, kNoSeq);
+    const int64_t n = train_workspace_bytes(cfg, B, kNoSeq, kNoRec, B2CNN_MODE_SEQUENCE);
     if (n < 0) fail(B2CNN_EINVAL, "b2cnn_train_workspace_bytes: bad configuration / batch");
     return n;
 }
 extern "C" int64_t b2cnn_train_workspace_bytes_seq(const b2cnn_config *cfg, int64_t B, const int64_t *seq_lengths, int64_t n_seq) {
-    const int64_t n = train_workspace_bytes(cfg, B, SeqLengths{true, seq_lengths, n_seq});
+    const int64_t n = train_workspace_bytes(cfg, B, SeqLengths{true, seq_lengths, n_seq}, kNoRec, B2CNN_MODE_SEQUENCE);
     if (n < 0) fail(B2CNN_EINVAL, "b2cnn_train_workspace_bytes_seq: bad configuration / batch / sequence lengths");
     return n;
 }
 static int train_step_api(const char *name, const b2cnn_config *cfg, float *params, float *adam_m, float *adam_v, float *grads,
                           int64_t step, const b2cnn_adam *opt, int apply_update, const float *x, int64_t B, const float *age,
-                          const float *target, int weighted, float pos_weight, int mode, const SeqLengths &sl, const float *mask1,
-                          const float *mask2, float *loss_out, void *workspace, int64_t workspace_bytes, void *stream) {
+                          const float *target, int weighted, float pos_weight, int mode, const SeqLengths &sl, const RecordArgs &ra,
+                          const float *mask1, const float *mask2, float *loss_out, void *workspace, int64_t workspace_bytes, void *stream) {
     if (!cfg || !opt) return fail(B2CNN_EINVAL, std::string(name) + ": null configuration");
     const char *err = "";
     const int rc = train_step(cfg, params, adam_m, adam_v, grads, step, opt->lr, opt->beta1, opt->beta2, opt->eps, apply_update, x, B, age,
-                              target, weighted, pos_weight, mode, sl, mask1, mask2, loss_out, workspace, workspace_bytes,
+                              target, weighted, pos_weight, mode, sl, ra, mask1, mask2, loss_out, workspace, workspace_bytes,
                               reinterpret_cast<cudaStream_t>(stream), &err);
     return finish(name, rc, err);
 }
@@ -117,14 +118,14 @@ extern "C" int b2cnn_train_step(const b2cnn_config *cfg, float *params, float *a
                                 const float *target, int mode, const float *mask1, const float *mask2, float *loss_out,
                                 void *workspace, int64_t workspace_bytes, void *stream) {
     return train_step_api("b2cnn_train_step", cfg, params, adam_m, adam_v, grads, step, opt, apply_update, x, B, age, target, 0, 1.f, mode,
-                          kNoSeq, mask1, mask2, loss_out, workspace, workspace_bytes, stream);
+                          kNoSeq, kNoRec, mask1, mask2, loss_out, workspace, workspace_bytes, stream);
 }
 extern "C" int b2cnn_train_step_weighted(const b2cnn_config *cfg, float *params, float *adam_m, float *adam_v, float *grads, int64_t step,
                                          const b2cnn_adam *opt, int apply_update, const float *x, int64_t B, const float *age,
                                          const float *target, float pos_weight, int mode, const float *mask1, const float *mask2,
                                          float *loss_out, void *workspace, int64_t workspace_bytes, void *stream) {
     return train_step_api("b2cnn_train_step_weighted", cfg, params, adam_m, adam_v, grads, step, opt, apply_update, x, B, age, target, 1,
-                          pos_weight, mode, kNoSeq, mask1, mask2, loss_out, workspace, workspace_bytes, stream);
+                          pos_weight, mode, kNoSeq, kNoRec, mask1, mask2, loss_out, workspace, workspace_bytes, stream);
 }
 extern "C" int b2cnn_train_step_seq(const b2cnn_config *cfg, float *params, float *adam_m, float *adam_v, float *grads, int64_t step,
                                     const b2cnn_adam *opt, int apply_update, const float *x, int64_t B, const float *age,
@@ -133,13 +134,13 @@ extern "C" int b2cnn_train_step_seq(const b2cnn_config *cfg, float *params, floa
                                     void *stream) {
     return train_step_api("b2cnn_train_step_seq", cfg, params, adam_m, adam_v, grads, step, opt, apply_update, x, B, age, target,
                           pos_weight ? 1 : 0, pos_weight ? *pos_weight : 1.f, B2CNN_MODE_SEQUENCE, SeqLengths{true, seq_lengths, n_seq},
-                          mask1, mask2, loss_out, workspace, workspace_bytes, stream);
+                          kNoRec, mask1, mask2, loss_out, workspace, workspace_bytes, stream);
 }
 extern "C" int b2cnn_train_forward(const b2cnn_config *cfg, const float *params, const float *x, int64_t B, const float *age, int mode,
                                    const float *mask1, const float *mask2, float *z_out, void *workspace, int64_t workspace_bytes,
                                    void *stream) {
     const char *err = "";
-    const int rc = train_forward(cfg, params, x, B, age, mode, kNoSeq, mask1, mask2, z_out, workspace, workspace_bytes,
+    const int rc = train_forward(cfg, params, x, B, age, mode, kNoSeq, kNoRec, mask1, mask2, z_out, workspace, workspace_bytes,
                                  reinterpret_cast<cudaStream_t>(stream), &err);
     return finish("b2cnn_train_forward", rc, err);
 }
@@ -147,7 +148,7 @@ extern "C" int b2cnn_train_forward_seq(const b2cnn_config *cfg, const float *par
                                        const int64_t *seq_lengths, int64_t n_seq, const float *mask1, const float *mask2, float *z_out,
                                        void *workspace, int64_t workspace_bytes, void *stream) {
     const char *err = "";
-    const int rc = train_forward(cfg, params, x, B, age, B2CNN_MODE_SEQUENCE, SeqLengths{true, seq_lengths, n_seq}, mask1, mask2, z_out,
+    const int rc = train_forward(cfg, params, x, B, age, B2CNN_MODE_SEQUENCE, SeqLengths{true, seq_lengths, n_seq}, kNoRec, mask1, mask2, z_out,
                                  workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream), &err);
     return finish("b2cnn_train_forward_seq", rc, err);
 }
@@ -155,7 +156,7 @@ extern "C" int b2cnn_train_backward_ex(const b2cnn_config *cfg, const float *par
                                        const float *mask1, const float *mask2, const float *dz, float *grads, float *dx, float *dage,
                                        int flags, void *workspace, int64_t workspace_bytes, void *stream) {
     const char *err = "";
-    const int rc = train_backward(cfg, params, x, B, age, mode, kNoSeq, mask1, mask2, dz, grads, dx, dage, flags, workspace, workspace_bytes,
+    const int rc = train_backward(cfg, params, x, B, age, mode, kNoSeq, kNoRec, mask1, mask2, dz, grads, dx, dage, flags, workspace, workspace_bytes,
                                   reinterpret_cast<cudaStream_t>(stream), &err);
     return finish("b2cnn_train_backward", rc, err);
 }
@@ -169,9 +170,41 @@ extern "C" int b2cnn_train_backward_seq(const b2cnn_config *cfg, const float *pa
                                         float *grads, float *dx, float *dage, int flags, void *workspace, int64_t workspace_bytes,
                                         void *stream) {
     const char *err = "";
-    const int rc = train_backward(cfg, params, x, B, age, B2CNN_MODE_SEQUENCE, SeqLengths{true, seq_lengths, n_seq}, mask1, mask2, dz, grads,
+    const int rc = train_backward(cfg, params, x, B, age, B2CNN_MODE_SEQUENCE, SeqLengths{true, seq_lengths, n_seq}, kNoRec, mask1, mask2, dz, grads,
                                   dx, dage, flags, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream), &err);
     return finish("b2cnn_train_backward_seq", rc, err);
+}
+extern "C" int64_t b2cnn_train_workspace_bytes_record(const b2cnn_config *cfg, int64_t B, int64_t N, int64_t stride,
+                                                     const int64_t *window_counts, int mode) {
+    const int64_t n = train_workspace_bytes(cfg, B, kNoSeq, RecordArgs{true, N, stride, window_counts}, mode);
+    if (n < 0) fail(B2CNN_EINVAL, "b2cnn_train_workspace_bytes_record: bad configuration / batch / stride / window counts / mode");
+    return n;
+}
+extern "C" int b2cnn_train_step_record(const b2cnn_config *cfg, float *params, float *adam_m, float *adam_v, float *grads, int64_t step,
+                                       const b2cnn_adam *opt, int apply_update, const float *records, int64_t B, int64_t N, int64_t stride,
+                                       const int64_t *window_counts, int mode, const float *age, const float *target,
+                                       const float *pos_weight, const float *mask1, const float *mask2, float *loss_out, void *workspace,
+                                       int64_t workspace_bytes, void *stream) {
+    return train_step_api("b2cnn_train_step_record", cfg, params, adam_m, adam_v, grads, step, opt, apply_update, records, B, age, target,
+                          pos_weight ? 1 : 0, pos_weight ? *pos_weight : 1.f, mode, kNoSeq, RecordArgs{true, N, stride, window_counts},
+                          mask1, mask2, loss_out, workspace, workspace_bytes, stream);
+}
+extern "C" int b2cnn_train_forward_record(const b2cnn_config *cfg, const float *params, const float *records, int64_t B, int64_t N,
+                                          int64_t stride, const int64_t *window_counts, int mode, const float *age, const float *mask1,
+                                          const float *mask2, float *z_out, void *workspace, int64_t workspace_bytes, void *stream) {
+    const char *err = "";
+    const int rc = train_forward(cfg, params, records, B, age, mode, kNoSeq, RecordArgs{true, N, stride, window_counts}, mask1, mask2, z_out,
+                                 workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream), &err);
+    return finish("b2cnn_train_forward_record", rc, err);
+}
+extern "C" int b2cnn_train_backward_record(const b2cnn_config *cfg, const float *params, const float *records, int64_t B, int64_t N,
+                                           int64_t stride, const int64_t *window_counts, int mode, const float *age, const float *mask1,
+                                           const float *mask2, const float *dz, float *grads, float *d_records, float *dage, int flags,
+                                           void *workspace, int64_t workspace_bytes, void *stream) {
+    const char *err = "";
+    const int rc = train_backward(cfg, params, records, B, age, mode, kNoSeq, RecordArgs{true, N, stride, window_counts}, mask1, mask2, dz,
+                                  grads, d_records, dage, flags, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream), &err);
+    return finish("b2cnn_train_backward_record", rc, err);
 }
 
 // ---- preprocessing + window assembly (b2cnn_prep.cu) ----

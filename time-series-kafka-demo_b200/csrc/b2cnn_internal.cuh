@@ -99,6 +99,14 @@ inline bool seq_offsets(const SeqLengths &sl, int64_t B, std::vector<int64_t> &o
     return true;
 }
 
+// The windows of a _record training call (include/b2cnn.h): B recordings of N samples, windows of the configuration's W
+// samples every S samples, counts[b] of them (a host array) from recording b; on == false for every other call
+struct RecordArgs {
+    bool on;
+    int64_t N, S;
+    const int64_t *counts;
+};
+
 // Makes `device` current for the guard's lifetime and restores the caller's device on every exit path (a call on cuda:1
 // must not leave the calling thread on cuda:1: later `device="cuda"` allocations of the host framework would land on the
 // wrong GPU).  A negative device leaves the current device as it is.
@@ -284,17 +292,17 @@ double wire_parse_decimal_host(const char *s, int64_t len, int *status);
 // b2cnn_train.cu: one training step (row f4).  mode is B2CNN_MODE_*; every entry point checks all its arguments before
 // any CUDA call, then makes cfg->device current for the call (a negative device: the current one)
 // sl: the sequence lengths of a _seq call (mode is then B2CNN_MODE_SEQUENCE), or {false} for the calls that take a mode
-int64_t train_workspace_bytes(const b2cnn_config *cfg, int64_t B, const SeqLengths &sl);
+int64_t train_workspace_bytes(const b2cnn_config *cfg, int64_t B, const SeqLengths &sl, const RecordArgs &ra, int mode);
 // weighted != 0: BCEWithLogitsLoss(pos_weight=pos_weight), else plain BCEWithLogitsLoss
 int train_step(const b2cnn_config *cfg, float *params, float *adam_m, float *adam_v, float *grads, int64_t step, float lr, float beta1,
                float beta2, float eps, int apply_update, const float *x, int64_t B, const float *age, const float *target,
-               int weighted, float pos_weight, int mode, const SeqLengths &sl, const float *mask1, const float *mask2, float *loss_out,
-               void *workspace, int64_t ws_bytes, cudaStream_t st, const char **err);
+               int weighted, float pos_weight, int mode, const SeqLengths &sl, const RecordArgs &ra, const float *mask1, const float *mask2,
+               float *loss_out, void *workspace, int64_t ws_bytes, cudaStream_t st, const char **err);
 // the autograd seam
 int train_forward(const b2cnn_config *cfg, const float *params, const float *x, int64_t B, const float *age, int mode, const SeqLengths &sl,
-                  const float *mask1, const float *mask2, float *z_out, void *workspace, int64_t ws_bytes, cudaStream_t st, const char **err);
+                  const RecordArgs &ra, const float *mask1, const float *mask2, float *z_out, void *workspace, int64_t ws_bytes, cudaStream_t st, const char **err);
 int train_backward(const b2cnn_config *cfg, const float *params, const float *x, int64_t B, const float *age, int mode, const SeqLengths &sl,
-                   const float *mask1, const float *mask2, const float *dz, float *grads, float *dx, float *dage, int flags,
+                   const RecordArgs &ra, const float *mask1, const float *mask2, const float *dz, float *grads, float *dx, float *dage, int flags,
                    void *workspace, int64_t ws_bytes, cudaStream_t st, const char **err);
 
 void launch_transpose_wih(const float *wih0, float *wih0T, int L, cudaStream_t st);

@@ -28,6 +28,7 @@
 //   train_wih0_grad        dW_ih_l0 = da0^T f with f read once: a thread owns a position and all 64 gate rows, the batch
 //                          is split into chunks, and train_sum_chunks adds the chunk partials in chunk order
 //   train_dfeat            d f = da0 W_ih_l0 with a thread's 64 W_ih_l0 values in registers
+//   train_dfeat_fold       (whole recordings only) d f of each recording feature = the sum of its covering windows' d f
 //   train_conv_bwd         grid (position tiles x groups of windows): recomputes c1 / d1 / c2 with conv_tile(), back-
 //                          propagates the gradients of ITS OWN features through its receptive span in shared memory
 //                          (dropout / pool with first-maximum routing like ATen / tanh / conv2 / conv1), keeps the conv
@@ -40,6 +41,14 @@
 // Everything below f is linear in d f, so the sum over tiles of what each tile back-propagates from its own features is
 // the full gradient; no halo is exchanged and dc1 / dd1 / dc2 never reach global memory.  A window's values depend on
 // its geometry alone; the batch sets only the order in which conv-gradient partials and dW_ih_l0's chunks are added.
+//
+// Whole recordings (the _record entry points and the *_record kernels, whose bodies are the window kernels' with
+// REC = true): the rows of the scans are the counted windows of
+// B recordings [B][C][N].  The conv kernels run over each recording's geometry (a "window" of N samples, L_N features,
+// one grid row per recording), the projection and dW_ih_l0 read window w of recording b as features [w S/F, w S/F + L)
+// of the recording's row, and train_dfeat_fold sums the windows' d f onto the recording before the conv backward.  A
+// tile that no counted window reaches does no conv work, and the conv backward zeroes every staged sample that no counted
+// window reads, so NaN / inf there cannot reach a gradient.
 #include <cfloat>
 #include <cstring>
 #include <vector>
@@ -50,7 +59,7 @@ namespace b2cnn {
 
 // workspace layout (floats)
 struct TrainWs {
-    int64_t f, pre0, acts, cs, hs, lin, z, da0, dfeat, part, off, total;
+    int64_t f, pre0, acts, cs, hs, lin, z, da0, dfeat, part, off, dfw, roff, total;
 };
 
 constexpr int kT = 128;             // final features per tile
@@ -107,28 +116,32 @@ struct TrainPlan {
     int seq_per, seq_ctas;              // sequences per scan CTA, scan CTAs
 };
 
-// n_seq: the number of sequences of a _seq call, 0 for the calls that take a mode (their layout has no offsets region)
-static TrainPlan train_plan(const Dims &d, int64_t B, int64_t n_seq = 0) {
+// n_seq: the number of sequences of a _seq call, 0 for the calls that take a mode (their layout has no offsets region).
+// rd: a _record call's recording geometry, whose n_rec recordings the conv kernels run over; B is then the number of
+// counted windows (the scans' rows), and the layout gains the per-window d f [B][L] and the row offsets [n_rec + 1].
+static TrainPlan train_plan(const Dims &d, int64_t B, int64_t n_seq = 0, const Dims *rd = nullptr, int64_t n_rec = 0) {
     TrainPlan pl{};
+    const Dims &cd = rd ? *rd : d;                      // the conv kernels' geometry and rows
+    const int64_t cb = rd ? n_rec : B;
     // consecutive sequences per scan CTA: ceil(n_seq / kSeqCtas), from (B, n_seq) alone, never the device
     pl.seq_per = n_seq > kSeqCtas ? (int)((n_seq + kSeqCtas - 1) / kSeqCtas) : 1;
     pl.seq_ctas = n_seq > 0 ? (int)((n_seq + pl.seq_per - 1) / pl.seq_per) : 1;
-    pl.tiles = (d.L + kT - 1) / kT;
+    pl.tiles = (cd.L + kT - 1) / kT;
     pl.slices = (d.L + kPre0Slice - 1) / kPre0Slice;
     pl.wih_chunk = (int)((B + kWihChunks - 1) / kWihChunks);
     pl.wih_chunks = (int)((B + pl.wih_chunk - 1) / pl.wih_chunk);
     // windows per conv-backward CTA: ceil(B x tiles / kBwdCtas) within [1, kWin], from the shape alone, never the device
-    const int64_t bt = B * pl.tiles, win = (bt + kBwdCtas - 1) / kBwdCtas;
+    const int64_t bt = cb * pl.tiles, win = (bt + kBwdCtas - 1) / kBwdCtas;
     pl.win = (int)(win < 1 ? 1 : win > kWin ? kWin : win);
-    pl.groups = (int)((B + pl.win - 1) / pl.win);
+    pl.groups = (int)((cb + pl.win - 1) / pl.win);
     pl.n_conv = (int)blob_offsets(d).wih0;
     pl.part_rows = (int64_t)pl.tiles * pl.groups;
-    pl.smem_fwd = sizeof(float) * tile_smem(d, false).total;
-    pl.smem_bwd = sizeof(float) * tile_smem(d, true).total;
+    pl.smem_fwd = sizeof(float) * tile_smem(cd, false).total;
+    pl.smem_bwd = sizeof(float) * tile_smem(cd, true).total;
     TrainWs &w = pl.w;
     int64_t p = 0;
     auto take = [&](int64_t n) { int64_t at = p; p += (n + 63) / 64 * 64; return at; };
-    w.f = take(B * d.L);
+    w.f = take(cb * cd.L);
     w.pre0 = take(B * kGates);          // f . W_ih_l0^T
     w.acts = take(B * 2 * kGates);      // [t][layer][i f g o] post-activation
     w.cs = take(B * 2 * kHidden);       // [t][layer] cell state
@@ -136,7 +149,7 @@ static TrainPlan train_plan(const Dims &d, int64_t B, int64_t n_seq = 0) {
     w.lin = take(B);                    // out(h1) before the age scale (d age needs it)
     w.z = take(B);
     w.da0 = take(B * kGates);           // d loss / d (layer-0 gate pre-activations)
-    w.dfeat = take(B * d.L);
+    w.dfeat = take(cb * cd.L);
     // one region for the partial sums of three reductions that never overlap in time
     int64_t part = (int64_t)pl.slices * B * kGates;
     if ((int64_t)pl.wih_chunks * kGates * d.L > part) part = (int64_t)pl.wih_chunks * kGates * d.L;
@@ -145,6 +158,8 @@ static TrainPlan train_plan(const Dims &d, int64_t B, int64_t n_seq = 0) {
     if (pl.seq_ctas > 1 && pl.seq_ctas * head_row_len(blob_offsets(d)) > part) part = pl.seq_ctas * head_row_len(blob_offsets(d));
     w.part = take(part);
     w.off = n_seq > 0 ? take(2 * (n_seq + 1)) : 0;     // int64 sequence offsets [n_seq + 1], copied in by every _seq call
+    w.dfw = rd ? take(B * d.L) : 0;                    // the windows' d f, folded into dfeat
+    w.roff = rd ? take(2 * (n_rec + 1)) : 0;           // int64 row offsets of the recordings, copied in by every _record call
     w.total = p;
     return pl;
 }
@@ -173,6 +188,35 @@ struct SeqSpan {
     int per;
     float *rows;
 };
+
+// The rows of a _record call: recording b holds rows [roff[b], roff[b + 1]) (its counted windows, in order); window w of
+// it starts at sample w S, i.e. at feature w sf (sf = S / F) of the recording's L_N = LN features, and holds Lw of them.
+struct RecRows {
+    const int64_t *roff;
+    int64_t nrec;
+    int S, sf, W, Lw, LN;
+};
+// the recording of row m: the last b with roff[b] <= m (a recording without windows never matches)
+__device__ __forceinline__ int64_t rec_row_base(const RecRows &r, int64_t m) {
+    int64_t lo = 0, hi = r.nrec - 1;
+    while (lo < hi) {
+        const int64_t mid = (lo + hi + 1) >> 1;
+        if (r.roff[mid] <= m) lo = mid; else hi = mid - 1;
+    }
+    return lo * r.LN + (m - r.roff[lo]) * r.sf;          // where the window's features start in f [nrec][LN]
+}
+// the windows [lo, hi] of a recording with n counted windows whose features include recording feature p (empty: lo > hi)
+__device__ __forceinline__ int64_t rec_first_window(const RecRows &r, int p) { return p >= r.Lw ? (p - r.Lw) / r.sf + 1 : 0; }
+__device__ __forceinline__ int64_t rec_last_window(const RecRows &r, int64_t n, int p) { return min(n - 1, (int64_t)(p / r.sf)); }
+// does a counted window hold one of the features [i0, i0 + nf)?
+__device__ __forceinline__ bool rec_covers(const RecRows &r, int64_t n, int i0, int nf) {
+    return rec_first_window(r, i0) <= rec_last_window(r, n, i0 + nf - 1);
+}
+// does a counted window read sample s? (the last window starting at or before s is the one that can)
+__device__ __forceinline__ bool rec_reads(const RecRows &r, int64_t n, int s) {
+    const int64_t w = min(n - 1, (int64_t)(s / r.S));
+    return w >= 0 && s < w * r.S + r.W;
+}
 
 // ------------------------------------------------------------------------------------------------------------------
 // LSTM forward over the batch axis with everything the backward pass needs kept; logits and loss.
@@ -450,10 +494,16 @@ __device__ __forceinline__ void tile_stage_weights(const float *__restrict__ prm
 // the inference kernels' order (an fmaf chain from the bias, channels outer, taps inner), so a value does not depend on
 // the tile that computes it.  Pooling comes before tanh: tanh is monotone, and a NaN in the window wins either way.
 // xb / m1b: the window's x [C][W] and its mask1 [4][P1] (or NULL).  Ends with a barrier.
+// ZERO: xb is a recording with n counted windows (rr), and a sample none of them reads is staged as 0.
+template <bool ZERO = false>
 __device__ __forceinline__ void conv_tile(const float *__restrict__ xb, const float *__restrict__ m1b, const Dims &d, const Tile &t,
-                                          const TileSmem &s, float *sm, int tid) {
+                                          const TileSmem &s, float *sm, int tid, const RecRows *rr = nullptr, int64_t n = 0) {
     for (int c = 0; c < d.C; ++c)
-        for (int j = tid; j < t.nx; j += kThreads) sm[s.x + c * s.xp + j] = xb[(int64_t)c * d.W + t.s1 + j];
+        for (int j = tid; j < t.nx; j += kThreads) {
+            float v = xb[(int64_t)c * d.W + t.s1 + j];
+            if constexpr (ZERO) v = rec_reads(*rr, n, t.s1 + j) ? v : 0.f;
+            sm[s.x + c * s.xp + j] = v;
+        }
     __syncthreads();
     for (int j = tid; j < t.n1; j += kThreads) {
         float4 acc = *reinterpret_cast<const float4 *>(sm + s.b1);
@@ -486,15 +536,19 @@ __device__ __forceinline__ void conv_tile(const float *__restrict__ xb, const fl
     __syncthreads();
 }
 
-// grid: B x tiles CTAs, window-major
-__global__ void __launch_bounds__(kThreads)
-train_conv_fwd(const float *__restrict__ x, const float *__restrict__ prm, BlobOff o, Dims d, int tiles,
-               const float *__restrict__ mask1, const float *__restrict__ mask2, float *__restrict__ f) {
+// grid: B x tiles CTAs, window-major.  REC: d is a recording's geometry, and a tile that no counted window of it reaches
+// writes nothing (f there is never read)
+template <bool REC>
+__device__ __forceinline__ void train_conv_fwd_body(const float *__restrict__ x, const float *__restrict__ prm, BlobOff o, Dims d, int tiles,
+               const float *__restrict__ mask1, const float *__restrict__ mask2, float *__restrict__ f, const RecRows &rr) {
     extern __shared__ __align__(16) float sm[];
     const TileSmem s = tile_smem(d, false);
     const int tid = threadIdx.x;
     const int64_t b = blockIdx.x / tiles;
     const Tile t = tile_of(d, blockIdx.x % tiles);
+    if constexpr (REC) {
+        if (!rec_covers(rr, rr.roff[b + 1] - rr.roff[b], t.i0, t.nf)) return;
+    }
     tile_stage_weights(prm, o, d, s, sm, tid);
     conv_tile(x + b * d.C * d.W, mask1 ? mask1 + b * kCMid * d.P1 : nullptr, d, t, s, sm, tid);
     for (int i = tid; i < t.nf; i += kThreads) {
@@ -503,17 +557,33 @@ train_conv_fwd(const float *__restrict__ x, const float *__restrict__ prm, BlobO
         f[b * d.L + t.i0 + i] = tanhf(m) * (mask2 ? mask2[b * d.L + t.i0 + i] : 1.0f);
     }
 }
+__global__ void __launch_bounds__(kThreads)
+train_conv_fwd(const float *__restrict__ x, const float *__restrict__ prm, BlobOff o, Dims d, int tiles,
+               const float *__restrict__ mask1, const float *__restrict__ mask2, float *__restrict__ f) {
+    train_conv_fwd_body<false>(x, prm, o, d, tiles, mask1, mask2, f, RecRows{});
+}
+__global__ void __launch_bounds__(kThreads)
+train_conv_fwd_record(const float *__restrict__ x, const float *__restrict__ prm, BlobOff o, Dims d, int tiles,
+               const float *__restrict__ mask1, const float *__restrict__ mask2, float *__restrict__ f, RecRows rr) {
+    train_conv_fwd_body<true>(x, prm, o, d, tiles, mask1, mask2, f, rr);
+}
 
 // pre0 partial[slice][b][g] = sum over the slice's positions of f[b][p] W_ih_l0[g][p]: 64 windows x 64 gates per CTA,
 // K chunks of 32, a 4 x 4 register tile per thread (the tiling of the inference projection, reading W_ih_l0 as stored)
+// REC: row b is a window of a recording (rr), read in place from the recording's feature row
 constexpr int kGemmK = 32, kGemmStride = 68;
-__global__ void __launch_bounds__(256)
-train_pre0_partial(const float *__restrict__ f, const float *__restrict__ wih0, int64_t B, int L, float *__restrict__ part) {
+template <bool REC>
+__device__ __forceinline__ void train_pre0_partial_body(const float *__restrict__ f, const float *__restrict__ wih0, int64_t B, int L, float *__restrict__ part, const RecRows &rr) {
     __shared__ __align__(16) float Fs[kGemmK][kGemmStride];
     __shared__ __align__(16) float Ws[kGemmK][kGemmStride];
     const int tid = threadIdx.x, tm = tid >> 4, tn = tid & 15;
     const int64_t b0 = (int64_t)blockIdx.x * 64;
     const int kbeg = blockIdx.y * kPre0Slice, kend = min(L, kbeg + kPre0Slice);
+    [[maybe_unused]] __shared__ int64_t row_at[REC ? 64 : 1];
+    if constexpr (REC) {
+        if (tid < 64 && b0 + tid < B) row_at[tid] = rec_row_base(rr, b0 + tid);
+        __syncthreads();
+    }
     float acc[4][4];
 #pragma unroll
     for (int i = 0; i < 4; ++i)
@@ -523,7 +593,8 @@ train_pre0_partial(const float *__restrict__ f, const float *__restrict__ wih0, 
 #pragma unroll
         for (int it = 0; it < 8; ++it) {
             const int e = tid + it * 256, m = e >> 5, kk = e & 31, k = k0 + kk;
-            Fs[kk][m] = (b0 + m < B && k < kend) ? f[(b0 + m) * L + k] : 0.f;
+            if constexpr (REC) Fs[kk][m] = (b0 + m < B && k < kend) ? f[row_at[m] + k] : 0.f;
+            else Fs[kk][m] = (b0 + m < B && k < kend) ? f[(b0 + m) * L + k] : 0.f;
             Ws[kk][m] = k < kend ? wih0[(int64_t)m * L + k] : 0.f;
         }
         __syncthreads();
@@ -545,6 +616,14 @@ train_pre0_partial(const float *__restrict__ f, const float *__restrict__ wih0, 
         if (b < B) *reinterpret_cast<float4 *>(part + ((int64_t)blockIdx.y * B + b) * kGates + 4 * tn) = make_float4(acc[i][0], acc[i][1], acc[i][2], acc[i][3]);
     }
 }
+__global__ void __launch_bounds__(256)
+train_pre0_partial(const float *__restrict__ f, const float *__restrict__ wih0, int64_t B, int L, float *__restrict__ part) {
+    train_pre0_partial_body<false>(f, wih0, B, L, part, RecRows{});
+}
+__global__ void __launch_bounds__(256)
+train_pre0_partial_record(const float *__restrict__ f, const float *__restrict__ wih0, int64_t B, int L, float *__restrict__ part, RecRows rr) {
+    train_pre0_partial_body<true>(f, wih0, B, L, part, rr);
+}
 
 // out[e] = part[0][e] + part[1][e] + ... in that order (split-K slices of pre0, batch chunks of dW_ih_l0)
 __global__ void train_sum_chunks(const float *__restrict__ part, int n_chunks, int64_t n, float *__restrict__ out) {
@@ -556,10 +635,12 @@ __global__ void train_sum_chunks(const float *__restrict__ part, int n_chunks, i
 }
 
 // dW_ih_l0 partial[chunk][g][p] = sum over the chunk's windows t (ascending) of da0[t][g] f[t][p].  Thread = position p
-// with the 64 gate rows' sums in registers, so f is read once; grid (position tiles of 128, batch chunks).
-__global__ void __launch_bounds__(128)
-train_wih0_grad(const float *__restrict__ da0, const float *__restrict__ f, int64_t B, int L, int chunk, float *__restrict__ part) {
+// with the 64 gate rows' sums in registers, so f is read once; grid (position tiles of 128, batch chunks).  REC: window t
+// is read in place from its recording's feature row (rr).
+template <bool REC>
+__device__ __forceinline__ void train_wih0_grad_body(const float *__restrict__ da0, const float *__restrict__ f, int64_t B, int L, int chunk, float *__restrict__ part, const RecRows &rr) {
     __shared__ __align__(16) float sda[kRowBatch * kGates];
+    [[maybe_unused]] __shared__ int64_t row_at[REC ? kRowBatch : 1];
     const int p = blockIdx.x * 128 + threadIdx.x;
     const int64_t t0 = (int64_t)blockIdx.y * chunk, t1 = min(B, t0 + chunk);
     float acc[kGates];
@@ -569,10 +650,15 @@ train_wih0_grad(const float *__restrict__ da0, const float *__restrict__ f, int6
         const int rows = (int)min((int64_t)kRowBatch, t1 - tb);
         __syncthreads();
         for (int e = threadIdx.x; e < rows * kGates; e += 128) sda[e] = da0[tb * kGates + e];
+        if constexpr (REC) {
+            if (threadIdx.x < rows) row_at[threadIdx.x] = rec_row_base(rr, tb + threadIdx.x);
+        }
         __syncthreads();
         if (p < L)
             for (int r = 0; r < rows; ++r) {
-                const float fv = f[(tb + r) * L + p];
+                float fv;
+                if constexpr (REC) fv = f[row_at[r] + p];
+                else fv = f[(tb + r) * L + p];
 #pragma unroll
                 for (int g4 = 0; g4 < kGates / 4; ++g4) {
                     const float4 a = *reinterpret_cast<const float4 *>(sda + r * kGates + 4 * g4);
@@ -584,6 +670,14 @@ train_wih0_grad(const float *__restrict__ da0, const float *__restrict__ f, int6
     if (p < L)
 #pragma unroll
         for (int g = 0; g < kGates; ++g) part[((int64_t)blockIdx.y * kGates + g) * L + p] = acc[g];
+}
+__global__ void __launch_bounds__(128)
+train_wih0_grad(const float *__restrict__ da0, const float *__restrict__ f, int64_t B, int L, int chunk, float *__restrict__ part) {
+    train_wih0_grad_body<false>(da0, f, B, L, chunk, part, RecRows{});
+}
+__global__ void __launch_bounds__(128)
+train_wih0_grad_record(const float *__restrict__ da0, const float *__restrict__ f, int64_t B, int L, int chunk, float *__restrict__ part, RecRows rr) {
+    train_wih0_grad_body<true>(da0, f, B, L, chunk, part, rr);
 }
 
 // d f[t][p] = sum_g da0[t][g] W_ih_l0[g][p], g ascending; thread = position p with its 64 weights in registers, grid
@@ -609,6 +703,23 @@ train_dfeat(const float *__restrict__ da0, const float *__restrict__ wih0, int64
         }
         dfeat[(t0 + r) * L + p] = a;
     }
+}
+
+// d f of recording b's feature p = the sum of the d f of the counted windows that hold it (dfw [rows][Lw]), in ascending
+// window order, without atomics; 0 where no window holds it.  One thread per recording feature.
+__global__ void __launch_bounds__(256)
+train_dfeat_fold(const float *__restrict__ dfw, RecRows rr, float *__restrict__ dfeat) {
+    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= rr.nrec * rr.LN) return;
+    const int64_t b = e / rr.LN;
+    const int p = (int)(e - b * rr.LN);
+    const int64_t r0 = rr.roff[b], lo = rec_first_window(rr, p), hi = rec_last_window(rr, rr.roff[b + 1] - r0, p);
+    float a = 0.f;
+    for (int64_t w = lo; w <= hi; ++w) {
+        const float v = dfw[(r0 + w) * rr.Lw + p - w * rr.sf];
+        a = w == lo ? v : a + v;
+    }
+    dfeat[e] = a;
 }
 
 // first maximum of a pooling window over every `stride`-th float (c1 is kept position-major in a tile), like ATen's
@@ -637,10 +748,13 @@ __device__ __forceinline__ float warp_sum(float v) {
 // of part[groups x tiles][n_conv].
 // dx != NULL: d x of the tile's span is added into the zeroed dx; adjacent spans overlap by less than a tile's stride
 // (checked by the host), so a sample has at most two contributions and their sum does not depend on the order.
-__global__ void __launch_bounds__(kThreads)
-train_conv_bwd(const float *__restrict__ x, const float *__restrict__ prm, BlobOff o, Dims d, int tiles, int win, int64_t B,
+// REC: the rows are recordings (rr); a tile that no counted window reaches is skipped (its partial row stays 0), and the
+// staged x span is 0 wherever no counted window reads it: a covered feature reads none of those samples, so every
+// uncovered position sees a finite pre-activation times an exact 0 gradient, and no 0 * NaN reaches the partials or d x.
+template <bool REC>
+__device__ __forceinline__ void train_conv_bwd_body(const float *__restrict__ x, const float *__restrict__ prm, BlobOff o, Dims d, int tiles, int win, int64_t B,
                const float *__restrict__ mask1, const float *__restrict__ mask2, const float *__restrict__ dfeat,
-               float *__restrict__ part, float *__restrict__ dx) {
+               float *__restrict__ part, float *__restrict__ dx, const RecRows &rr) {
     extern __shared__ __align__(16) float sm[];
     const TileSmem s = tile_smem(d, true);
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -651,10 +765,15 @@ train_conv_bwd(const float *__restrict__ x, const float *__restrict__ prm, BlobO
     tile_stage_weights(prm, o, d, s, sm, tid);
     for (int e = tid; e < n_conv; e += kThreads) sm[s.g + e] = 0.f;
     for (int64_t b = b0; b < b1; ++b) {
+        [[maybe_unused]] int64_t n = 0;
+        if constexpr (REC) {
+            n = rr.roff[b + 1] - rr.roff[b];
+            if (!rec_covers(rr, n, t.i0, t.nf)) continue;       // the same for the whole CTA
+        }
         const float *m1b = mask1 ? mask1 + b * kCMid * d.P1 : nullptr;
         __syncthreads();                                       // the previous window's readers are done
         for (int i = tid; i < t.nf; i += kThreads) sm[s.df + i] = dfeat[b * d.L + t.i0 + i] * (mask2 ? mask2[b * d.L + t.i0 + i] : 1.0f);
-        conv_tile(x + b * d.C * d.W, m1b, d, t, s, sm, tid);
+        conv_tile<REC>(x + b * d.C * d.W, m1b, d, t, s, sm, tid, &rr, n);
         // ---- dropout 2 + pool 2 + tanh, gather form over the tile's own features
         for (int j = tid; j < t.n2; j += kThreads) {
             float a = 0.f;
@@ -735,6 +854,18 @@ train_conv_bwd(const float *__restrict__ x, const float *__restrict__ prm, BlobO
     __syncthreads();
     for (int e = tid; e < n_conv; e += kThreads) part[(int64_t)blockIdx.x * n_conv + e] = sm[s.g + e];
 }
+__global__ void __launch_bounds__(kThreads)
+train_conv_bwd(const float *__restrict__ x, const float *__restrict__ prm, BlobOff o, Dims d, int tiles, int win, int64_t B,
+               const float *__restrict__ mask1, const float *__restrict__ mask2, const float *__restrict__ dfeat,
+               float *__restrict__ part, float *__restrict__ dx) {
+    train_conv_bwd_body<false>(x, prm, o, d, tiles, win, B, mask1, mask2, dfeat, part, dx, RecRows{});
+}
+__global__ void __launch_bounds__(kThreads)
+train_conv_bwd_record(const float *__restrict__ x, const float *__restrict__ prm, BlobOff o, Dims d, int tiles, int win, int64_t B,
+               const float *__restrict__ mask1, const float *__restrict__ mask2, const float *__restrict__ dfeat,
+               float *__restrict__ part, float *__restrict__ dx, RecRows rr) {
+    train_conv_bwd_body<true>(x, prm, o, d, tiles, win, B, mask1, mask2, dfeat, part, dx, rr);
+}
 
 // grad[e] = the sum of part[.][e] over all rows in a fixed order: one CTA per conv parameter, thread i adds rows
 // i, i + 256, ... in order, then the block's tree
@@ -778,73 +909,142 @@ static bool train_geometry(const b2cnn_config *cfg, Dims &d, const char **err) {
     return true;
 }
 
-int64_t train_workspace_bytes(const b2cnn_config *cfg, int64_t B, const SeqLengths &sl) {
-    Dims d;
-    const char *err = "";
-    std::vector<int64_t> off;
-    if (B < 1 || !train_geometry(cfg, d, &err) || (sl.on && !seq_offsets(sl, B, off, &err))) return -1;
-    return train_plan(d, B, sl.on ? sl.n : 0).w.total * (int64_t)sizeof(float);
+// A _record call after its checks: the recording geometry rd, the window stride S, the row offsets of the recordings (the
+// prefix sums of their window counts) and the rows (counted windows) of the scans.  Without one, rows is the batch.
+struct Rec {
+    bool on = false;
+    Dims rd{};
+    int64_t S = 0, rows = 0;
+    std::vector<int64_t> roff;
+};
+
+// The windows of a _record call (include/b2cnn.h): stride S a positive multiple of the feature stride F, every count in
+// [0, n_w] with n_w = (N - W) / S + 1 (0 when N < W), at least one window in all, and indices the kernels hold.  Fills
+// rec and, in sequence mode, off with the offsets of one sequence per recording with windows.  No CUDA call.
+static bool record_rows(const b2cnn_config &c, const Dims &d, int64_t B, int mode, const RecordArgs &ra, Rec &rec,
+                        std::vector<int64_t> &off, const char **err) {
+    if (!ra.counts) { *err = "training: NULL window_counts"; return false; }
+    if (ra.S < 1 || ra.S % d.feature_stride() || ra.S > INT32_MAX) { *err = "training: stride must be a positive multiple of the feature stride pool_s^2"; return false; }
+    if (ra.N < 1 || ra.N > INT32_MAX) { *err = "training: recording length N must be in [1, 2^31 - 1] (the kernels index samples with int)"; return false; }
+    const int64_t n_w = ra.N >= d.W ? (ra.N - d.W) / ra.S + 1 : 0;
+    rec.roff.assign((size_t)B + 1, 0);
+    off.clear();
+    if (mode == B2CNN_MODE_SEQUENCE) off.push_back(0);
+    for (int64_t b = 0; b < B; ++b) {
+        const int64_t v = ra.counts[b];
+        if (v < 0 || v > n_w) { *err = "training: every window count must lie in [0, (N - W) / stride + 1]"; return false; }
+        rec.roff[b + 1] = rec.roff[b] + v;
+        if (v > 0 && mode == B2CNN_MODE_SEQUENCE) off.push_back(rec.roff[b + 1]);
+    }
+    if (rec.roff[B] < 1) { *err = "training: the window counts add up to 0"; return false; }
+    if (rec.roff[B] > INT32_MAX) { *err = "training: more than 2^31 - 1 windows"; return false; }
+    b2cnn_config rc = c;
+    rc.window = (int)ra.N;
+    derive_dims(rc, rec.rd);                     // N >= W: at least one window fits
+    rec.on = true;
+    rec.S = ra.S;
+    rec.rows = rec.roff[B];
+    return true;
 }
 
-// what the kernels need beyond a valid geometry; no CUDA call
-static bool plan_fits(const Dims &d, const TrainPlan &pl, int64_t B, const char **err) {
+// what the kernels need beyond a valid geometry (cd / B: the conv kernels' geometry and rows); no CUDA call
+static bool plan_fits(const Dims &cd, const TrainPlan &pl, int64_t B, const char **err) {
     if (pl.smem_bwd > 227 * 1024) { *err = "training: too many input channels for a conv tile's shared memory"; return false; }
     // a tile's x span against the tiles' stride: d x relies on at most two tiles touching a sample
-    const int np1 = d.PS * (kT - 1) + d.PK + d.K2 - 1, span = d.PS * (np1 - 1) + d.PK + d.K1 - 1, stride = d.PS * d.PS * kT;
+    const int np1 = cd.PS * (kT - 1) + cd.PK + cd.K2 - 1, span = cd.PS * (np1 - 1) + cd.PK + cd.K1 - 1, stride = cd.PS * cd.PS * kT;
     if (pl.tiles > 1 && span > 2 * stride) { *err = "training: receptive field longer than a conv tile"; return false; }
     if ((int64_t)pl.tiles * B > INT32_MAX) { *err = "training: batch too large"; return false; }
     return true;
 }
 
-// conv forward into ws.f and the layer-0 pre-activations into ws.pre0 (one slice is the whole sum: no reduction)
-static void launch_conv_forward(const Dims &d, const BlobOff &o, const TrainPlan &pl, float *ws, const float *params,
-                                const float *x, int64_t B, const float *mask1, const float *mask2, cudaStream_t st) {
+int64_t train_workspace_bytes(const b2cnn_config *cfg, int64_t B, const SeqLengths &sl, const RecordArgs &ra, int mode) {
+    Dims d;
+    const char *err = "";
+    std::vector<int64_t> off;
+    Rec rec;
+    if (B < 1 || !train_geometry(cfg, d, &err) || (sl.on && !seq_offsets(sl, B, off, &err))) return -1;
+    if (ra.on && ((mode != B2CNN_MODE_INDEPENDENT && mode != B2CNN_MODE_SEQUENCE) || !record_rows(*cfg, d, B, mode, ra, rec, off, &err))) return -1;
+    const TrainPlan pl = train_plan(d, ra.on ? rec.rows : B, off.empty() ? 0 : (int64_t)off.size() - 1, ra.on ? &rec.rd : nullptr, B);
+    if (ra.on && !plan_fits(rec.rd, pl, B, &err)) return -1;      // a shape the _record calls refuse has no workspace
+    return pl.w.total * (int64_t)sizeof(float);
+}
+
+// conv forward into ws.f and the layer-0 pre-activations of the R rows into ws.pre0 (one slice is the whole sum: no
+// reduction).  cd / B: the conv kernels' geometry and rows (the recordings' with REC, else d and the windows)
+template <bool REC>
+static void launch_conv_forward(const Dims &d, const Dims &cd, const BlobOff &o, const TrainPlan &pl, float *ws, const float *params,
+                                const float *x, int64_t B, int64_t R, const float *mask1, const float *mask2, const RecRows &rr,
+                                cudaStream_t st) {
     const TrainWs &w = pl.w;
-    if (pl.smem_fwd > 48 * 1024) cudaFuncSetAttribute(train_conv_fwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.smem_fwd);
-    train_conv_fwd<<<(unsigned)(B * pl.tiles), kThreads, pl.smem_fwd, st>>>(x, params, o, d, pl.tiles, mask1, mask2, ws + w.f);
-    train_pre0_partial<<<dim3((unsigned)((B + 63) / 64), (unsigned)pl.slices), 256, 0, st>>>(ws + w.f, params + o.wih0, B, d.L,
-                                                                                            ws + (pl.slices > 1 ? w.part : w.pre0));
+    const dim3 conv((unsigned)(B * pl.tiles)), proj((unsigned)((R + 63) / 64), (unsigned)pl.slices);
+    float *const pre0 = ws + (pl.slices > 1 ? w.part : w.pre0);
+    if constexpr (REC) {
+        if (pl.smem_fwd > 48 * 1024) cudaFuncSetAttribute(train_conv_fwd_record, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.smem_fwd);
+        train_conv_fwd_record<<<conv, kThreads, pl.smem_fwd, st>>>(x, params, o, cd, pl.tiles, mask1, mask2, ws + w.f, rr);
+        train_pre0_partial_record<<<proj, 256, 0, st>>>(ws + w.f, params + o.wih0, R, d.L, pre0, rr);
+    } else {
+        if (pl.smem_fwd > 48 * 1024) cudaFuncSetAttribute(train_conv_fwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.smem_fwd);
+        train_conv_fwd<<<conv, kThreads, pl.smem_fwd, st>>>(x, params, o, cd, pl.tiles, mask1, mask2, ws + w.f);
+        train_pre0_partial<<<proj, 256, 0, st>>>(ws + w.f, params + o.wih0, R, d.L, pre0);
+    }
     if (pl.slices > 1) {
-        const int64_t n = B * kGates;
+        const int64_t n = R * kGates;
         train_sum_chunks<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(ws + w.part, pl.slices, n, ws + w.pre0);
     }
 }
 
-// everything after d(head): d W_ih_l0 and, unless the front end is frozen, d f, the convolutional backward into `grads`
-// and, when dx != NULL, the input gradient (added into dx, zeroed here)
-static bool launch_backward_tail(const Dims &d, const BlobOff &o, const TrainPlan &pl, float *ws, const float *params,
-                                 const float *x, int64_t B, const float *mask1, const float *mask2, float *grads, float *dx,
-                                 bool frozen_conv, cudaStream_t st) {
+// everything after d(head): d W_ih_l0 and, unless the front end is frozen, d f (with REC folded onto the recordings), the
+// convolutional backward into `grads` and, when dx != NULL, the input gradient (added into dx, zeroed here)
+template <bool REC>
+static bool launch_backward_tail(const Dims &d, const Dims &cd, const BlobOff &o, const TrainPlan &pl, float *ws, const float *params,
+                                 const float *x, int64_t B, int64_t R, const float *mask1, const float *mask2, float *grads, float *dx,
+                                 bool frozen_conv, const RecRows &rr, cudaStream_t st) {
     const TrainWs &w = pl.w;
     const int64_t n1 = (int64_t)kGates * d.L;
     const unsigned ptiles = (unsigned)((d.L + 127) / 128);
-    train_wih0_grad<<<dim3(ptiles, (unsigned)pl.wih_chunks), 128, 0, st>>>(ws + w.da0, ws + w.f, B, d.L, pl.wih_chunk,
-                                                                           pl.wih_chunks > 1 ? ws + w.part : grads + o.wih0);
+    const dim3 wgrid(ptiles, (unsigned)pl.wih_chunks);
+    float *const wout = pl.wih_chunks > 1 ? ws + w.part : grads + o.wih0;
+    if constexpr (REC) train_wih0_grad_record<<<wgrid, 128, 0, st>>>(ws + w.da0, ws + w.f, R, d.L, pl.wih_chunk, wout, rr);
+    else train_wih0_grad<<<wgrid, 128, 0, st>>>(ws + w.da0, ws + w.f, R, d.L, pl.wih_chunk, wout);
     if (pl.wih_chunks > 1)
         train_sum_chunks<<<(unsigned)((n1 + 255) / 256), 256, 0, st>>>(ws + w.part, pl.wih_chunks, n1, grads + o.wih0);
     if (frozen_conv) return true;
-    train_dfeat<<<dim3(ptiles, (unsigned)((B + kRowBatch - 1) / kRowBatch)), 128, 0, st>>>(ws + w.da0, params + o.wih0, B, d.L, ws + w.dfeat);
-    if (dx && cudaMemsetAsync(dx, 0, sizeof(float) * B * d.C * d.W, st) != cudaSuccess) return false;
-    if (pl.smem_bwd > 48 * 1024) cudaFuncSetAttribute(train_conv_bwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.smem_bwd);
-    train_conv_bwd<<<(unsigned)pl.part_rows, kThreads, pl.smem_bwd, st>>>(x, params, o, d, pl.tiles, pl.win, B, mask1, mask2, ws + w.dfeat,
-                                                                          ws + w.part, dx);
+    train_dfeat<<<dim3(ptiles, (unsigned)((R + kRowBatch - 1) / kRowBatch)), 128, 0, st>>>(ws + w.da0, params + o.wih0, R, d.L,
+                                                                                          ws + (REC ? w.dfw : w.dfeat));
+    if (REC) {
+        const int64_t n = B * cd.L;
+        train_dfeat_fold<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(ws + w.dfw, rr, ws + w.dfeat);
+    }
+    if (dx && cudaMemsetAsync(dx, 0, sizeof(float) * B * cd.C * cd.W, st) != cudaSuccess) return false;
+    if constexpr (REC) {
+        if (pl.smem_bwd > 48 * 1024) cudaFuncSetAttribute(train_conv_bwd_record, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.smem_bwd);
+        train_conv_bwd_record<<<(unsigned)pl.part_rows, kThreads, pl.smem_bwd, st>>>(x, params, o, cd, pl.tiles, pl.win, B, mask1, mask2,
+                                                                                     ws + w.dfeat, ws + w.part, dx, rr);
+    } else {
+        if (pl.smem_bwd > 48 * 1024) cudaFuncSetAttribute(train_conv_bwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.smem_bwd);
+        train_conv_bwd<<<(unsigned)pl.part_rows, kThreads, pl.smem_bwd, st>>>(x, params, o, cd, pl.tiles, pl.win, B, mask1, mask2,
+                                                                              ws + w.dfeat, ws + w.part, dx);
+    }
     train_conv_grad_reduce<<<(unsigned)pl.n_conv, 256, 0, st>>>(ws + w.part, pl.part_rows, pl.n_conv, grads);
     return true;
 }
 
 // The checks every training entry point shares, before any CUDA call: the configuration, the mode, the pointers the call
-// needs (ptrs_ok) and the batch, the sequence lengths of a _seq call (into off), what the kernels hold, and the workspace
-// size.
-static int train_args(const b2cnn_config *cfg, int64_t B, int mode, const SeqLengths &sl, bool ptrs_ok, int64_t ws_bytes, Dims &d,
-                      TrainPlan &pl, std::vector<int64_t> &off, const char **err) {
+// needs (ptrs_ok) and the batch, the sequence lengths of a _seq call (into off), the windows of a _record call (into rec
+// and off), what the kernels hold, and the workspace size.
+static int train_args(const b2cnn_config *cfg, int64_t B, int mode, const SeqLengths &sl, const RecordArgs &ra, bool ptrs_ok,
+                      int64_t ws_bytes, Dims &d, TrainPlan &pl, std::vector<int64_t> &off, Rec &rec, const char **err) {
     if (!train_geometry(cfg, d, err)) return B2CNN_EINVAL;
     if (mode != B2CNN_MODE_INDEPENDENT && mode != B2CNN_MODE_SEQUENCE) { *err = "training: bad mode"; return B2CNN_EINVAL; }
     if (!ptrs_ok || B < 1) { *err = "training: null argument / bad batch"; return B2CNN_EINVAL; }
     if (sl.on && !seq_offsets(sl, B, off, err)) return B2CNN_EINVAL;
-    pl = train_plan(d, B, sl.on ? sl.n : 0);
-    if (!plan_fits(d, pl, B, err)) return B2CNN_EINVAL;
+    if (ra.on && !record_rows(*cfg, d, B, mode, ra, rec, off, err)) return B2CNN_EINVAL;
+    if (!ra.on) rec.rows = B;
+    pl = train_plan(d, rec.rows, off.empty() ? 0 : (int64_t)off.size() - 1, ra.on ? &rec.rd : nullptr, B);
+    if (!plan_fits(ra.on ? rec.rd : d, pl, B, err)) return B2CNN_EINVAL;
     if (ws_bytes < pl.w.total * (int64_t)sizeof(float)) {
-        *err = sl.on ? "training: workspace smaller than b2cnn_train_workspace_bytes_seq()" : "training: workspace smaller than b2cnn_train_workspace_bytes()";
+        *err = ra.on ? "training: workspace smaller than b2cnn_train_workspace_bytes_record()"
+             : sl.on ? "training: workspace smaller than b2cnn_train_workspace_bytes_seq()" : "training: workspace smaller than b2cnn_train_workspace_bytes()";
         return B2CNN_ESTATE;
     }
     return B2CNN_OK;
@@ -868,14 +1068,41 @@ static void launch_head_reduce(const TrainPlan &pl, const BlobOff &o, const SeqS
     train_head_reduce<<<(unsigned)((head_row_len(o) + 255) / 256), 256, 0, st>>>(sq.rows, pl.seq_ctas, o, B, grads, loss_out);
 }
 
+// The row addressing of a _record call over its B recordings; it first copies the row offsets into the workspace (from
+// pageable memory, as seq_span does)
+static bool record_span(const TrainPlan &pl, const Rec &rec, const Dims &d, int64_t B, float *ws, cudaStream_t st, RecRows &rr) {
+    rr = RecRows{nullptr, 0, 0, 1, 0, 0, 0};
+    if (!rec.on) return true;
+    int64_t *droff = reinterpret_cast<int64_t *>(ws + pl.w.roff);
+    if (cudaMemcpyAsync(droff, rec.roff.data(), sizeof(int64_t) * rec.roff.size(), cudaMemcpyHostToDevice, st) != cudaSuccess) return false;
+    rr = RecRows{droff, B, (int)rec.S, (int)(rec.S / d.feature_stride()), d.W, d.L, rec.rd.L};
+    return true;
+}
+
+// the conv kernels over the windows, or with a _record call over the recordings
+static void conv_forward(const Dims &d, const Rec &rec, const BlobOff &o, const TrainPlan &pl, float *ws, const float *params,
+                         const float *x, int64_t B, const float *mask1, const float *mask2, const RecRows &rr, cudaStream_t st) {
+    if (rec.on) launch_conv_forward<true>(d, rec.rd, o, pl, ws, params, x, B, rec.rows, mask1, mask2, rr, st);
+    else launch_conv_forward<false>(d, d, o, pl, ws, params, x, B, B, mask1, mask2, rr, st);
+}
+static bool backward_tail(const Dims &d, const Rec &rec, const BlobOff &o, const TrainPlan &pl, float *ws, const float *params,
+                          const float *x, int64_t B, const float *mask1, const float *mask2, float *grads, float *dx, bool frozen_conv,
+                          const RecRows &rr, cudaStream_t st) {
+    if (rec.on) return launch_backward_tail<true>(d, rec.rd, o, pl, ws, params, x, B, rec.rows, mask1, mask2, grads, dx, frozen_conv, rr, st);
+    return launch_backward_tail<false>(d, d, o, pl, ws, params, x, B, B, mask1, mask2, grads, dx, frozen_conv, rr, st);
+}
+
+// B: the windows, or with a _record call (ra.on) the recordings x [B][C][N], whose R counted windows are the rows that age,
+// target and the scans see
 int train_step(const b2cnn_config *cfg, float *params, float *adam_m, float *adam_v, float *grads, int64_t step, float lr, float beta1,
                float beta2, float eps, int apply_update, const float *x, int64_t B, const float *age, const float *target,
-               int weighted, float pos_weight, int mode, const SeqLengths &sl, const float *mask1, const float *mask2, float *loss_out,
-               void *workspace, int64_t ws_bytes, cudaStream_t st, const char **err) {
+               int weighted, float pos_weight, int mode, const SeqLengths &sl, const RecordArgs &ra, const float *mask1, const float *mask2,
+               float *loss_out, void *workspace, int64_t ws_bytes, cudaStream_t st, const char **err) {
     Dims d;
     TrainPlan pl;
     std::vector<int64_t> off;
-    const int rc = train_args(cfg, B, mode, sl, params && grads && x && age && target && loss_out && workspace, ws_bytes, d, pl, off, err);
+    Rec rec;
+    const int rc = train_args(cfg, B, mode, sl, ra, params && grads && x && age && target && loss_out && workspace, ws_bytes, d, pl, off, rec, err);
     if (rc != B2CNN_OK) return rc;
     if (step < 1) { *err = "training: step must be >= 1"; return B2CNN_EINVAL; }
     if (apply_update && (!adam_m || !adam_v)) { *err = "training: Adam state missing"; return B2CNN_EINVAL; }
@@ -885,25 +1112,28 @@ int train_step(const b2cnn_config *cfg, float *params, float *adam_m, float *ada
     const TrainWs &w = pl.w;
     const BlobOff o = blob_offsets(d);
     const int sequence = mode == B2CNN_MODE_SEQUENCE ? 1 : 0;
+    const int64_t R = rec.rows;
     float *ws = reinterpret_cast<float *>(workspace);
     SeqSpan sq;
     if (!seq_span(pl, off, ws, st, sq)) { *err = "copy sequence offsets"; return B2CNN_ECUDA; }
+    RecRows rr;
+    if (!record_span(pl, rec, d, B, ws, st, rr)) { *err = "copy row offsets"; return B2CNN_ECUDA; }
     if (cudaMemsetAsync(grads, 0, sizeof(float) * o.total, st) != cudaSuccess) { *err = "memset grads"; return B2CNN_ECUDA; }
-    launch_conv_forward(d, o, pl, ws, params, x, B, mask1, mask2, st);
+    conv_forward(d, rec, o, pl, ws, params, x, B, mask1, mask2, rr, st);
     const unsigned scans = (unsigned)pl.seq_ctas;
     if (weighted) {
-        train_lstm_fwd<kHeadBcePw><<<scans, 64, 0, st>>>(ws + w.pre0, params, o, d, B, sequence, sq, age, target, pos_weight, ws + w.acts,
+        train_lstm_fwd<kHeadBcePw><<<scans, 64, 0, st>>>(ws + w.pre0, params, o, d, R, sequence, sq, age, target, pos_weight, ws + w.acts,
                                                          ws + w.cs, ws + w.hs, ws + w.lin, ws + w.z, loss_out);
-        train_lstm_bwd<kHeadBcePw><<<scans, 64, 0, st>>>(params, o, d, B, sequence, sq, age, target, pos_weight, nullptr, ws + w.acts,
+        train_lstm_bwd<kHeadBcePw><<<scans, 64, 0, st>>>(params, o, d, R, sequence, sq, age, target, pos_weight, nullptr, ws + w.acts,
                                                          ws + w.cs, ws + w.hs, ws + w.lin, ws + w.z, ws + w.da0, grads, nullptr);
     } else {
-        train_lstm_fwd<kHeadBce><<<scans, 64, 0, st>>>(ws + w.pre0, params, o, d, B, sequence, sq, age, target, 1.f, ws + w.acts, ws + w.cs,
+        train_lstm_fwd<kHeadBce><<<scans, 64, 0, st>>>(ws + w.pre0, params, o, d, R, sequence, sq, age, target, 1.f, ws + w.acts, ws + w.cs,
                                                        ws + w.hs, ws + w.lin, ws + w.z, loss_out);
-        train_lstm_bwd<kHeadBce><<<scans, 64, 0, st>>>(params, o, d, B, sequence, sq, age, target, 1.f, nullptr, ws + w.acts, ws + w.cs,
+        train_lstm_bwd<kHeadBce><<<scans, 64, 0, st>>>(params, o, d, R, sequence, sq, age, target, 1.f, nullptr, ws + w.acts, ws + w.cs,
                                                        ws + w.hs, ws + w.lin, ws + w.z, ws + w.da0, grads, nullptr);
     }
-    launch_head_reduce(pl, o, sq, B, grads, loss_out, st);
-    if (!launch_backward_tail(d, o, pl, ws, params, x, B, mask1, mask2, grads, nullptr, false, st)) { *err = "memset dx"; return B2CNN_ECUDA; }
+    launch_head_reduce(pl, o, sq, R, grads, loss_out, st);
+    if (!backward_tail(d, rec, o, pl, ws, params, x, B, mask1, mask2, grads, nullptr, false, rr, st)) { *err = "memset dx"; return B2CNN_ECUDA; }
     if (apply_update) {
         const float bc1 = 1.f - powf(beta1, (float)step), bc2 = 1.f - powf(beta2, (float)step);
         train_adam<<<(unsigned)((o.total + 255) / 256), 256, 0, st>>>(params, adam_m, adam_v, grads, o.total, lr, beta1, beta2, eps, bc1, sqrtf(bc2));
@@ -914,11 +1144,13 @@ int train_step(const b2cnn_config *cfg, float *params, float *adam_m, float *ada
 }
 
 int train_forward(const b2cnn_config *cfg, const float *params, const float *x, int64_t B, const float *age, int mode, const SeqLengths &sl,
-                  const float *mask1, const float *mask2, float *z_out, void *workspace, int64_t ws_bytes, cudaStream_t st, const char **err) {
+                  const RecordArgs &ra, const float *mask1, const float *mask2, float *z_out, void *workspace, int64_t ws_bytes,
+                  cudaStream_t st, const char **err) {
     Dims d;
     TrainPlan pl;
     std::vector<int64_t> off;
-    const int rc = train_args(cfg, B, mode, sl, params && x && age && z_out && workspace, ws_bytes, d, pl, off, err);
+    Rec rec;
+    const int rc = train_args(cfg, B, mode, sl, ra, params && x && age && z_out && workspace, ws_bytes, d, pl, off, rec, err);
     if (rc != B2CNN_OK) return rc;
     DeviceGuard dev(cfg->device);
     if (dev.err != cudaSuccess) { *err = "cudaSetDevice"; return B2CNN_ECUDA; }
@@ -928,21 +1160,24 @@ int train_forward(const b2cnn_config *cfg, const float *params, const float *x, 
     float *ws = reinterpret_cast<float *>(workspace);
     SeqSpan sq;
     if (!seq_span(pl, off, ws, st, sq)) { *err = "copy sequence offsets"; return B2CNN_ECUDA; }
-    launch_conv_forward(d, o, pl, ws, params, x, B, mask1, mask2, st);
-    train_lstm_fwd<kHeadLogits><<<(unsigned)pl.seq_ctas, 64, 0, st>>>(ws + w.pre0, params, o, d, B, sequence, sq, age, nullptr, 1.f, ws + w.acts,
-                                                                     ws + w.cs, ws + w.hs, ws + w.lin, z_out, nullptr);
+    RecRows rr;
+    if (!record_span(pl, rec, d, B, ws, st, rr)) { *err = "copy row offsets"; return B2CNN_ECUDA; }
+    conv_forward(d, rec, o, pl, ws, params, x, B, mask1, mask2, rr, st);
+    train_lstm_fwd<kHeadLogits><<<(unsigned)pl.seq_ctas, 64, 0, st>>>(ws + w.pre0, params, o, d, rec.rows, sequence, sq, age, nullptr, 1.f,
+                                                                     ws + w.acts, ws + w.cs, ws + w.hs, ws + w.lin, z_out, nullptr);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) { *err = cudaGetErrorString(e); return B2CNN_ECUDA; }
     return B2CNN_OK;
 }
 
 int train_backward(const b2cnn_config *cfg, const float *params, const float *x, int64_t B, const float *age, int mode, const SeqLengths &sl,
-                   const float *mask1, const float *mask2, const float *dz, float *grads, float *dx, float *dage, int flags,
-                   void *workspace, int64_t ws_bytes, cudaStream_t st, const char **err) {
+                   const RecordArgs &ra, const float *mask1, const float *mask2, const float *dz, float *grads, float *dx, float *dage,
+                   int flags, void *workspace, int64_t ws_bytes, cudaStream_t st, const char **err) {
     Dims d;
     TrainPlan pl;
     std::vector<int64_t> off;
-    const int rc = train_args(cfg, B, mode, sl, params && x && age && dz && grads && workspace, ws_bytes, d, pl, off, err);
+    Rec rec;
+    const int rc = train_args(cfg, B, mode, sl, ra, params && x && age && dz && grads && workspace, ws_bytes, d, pl, off, rec, err);
     if (rc != B2CNN_OK) return rc;
     if (flags & ~B2CNN_TRAIN_FROZEN_CONV) { *err = "training: unknown flag"; return B2CNN_EINVAL; }
     const bool frozen_conv = (flags & B2CNN_TRAIN_FROZEN_CONV) != 0;
@@ -955,12 +1190,14 @@ int train_backward(const b2cnn_config *cfg, const float *params, const float *x,
     float *ws = reinterpret_cast<float *>(workspace);
     SeqSpan sq;
     if (!seq_span(pl, off, ws, st, sq)) { *err = "copy sequence offsets"; return B2CNN_ECUDA; }
+    RecRows rr;
+    if (!record_span(pl, rec, d, B, ws, st, rr)) { *err = "copy row offsets"; return B2CNN_ECUDA; }
     // zeroed: a frozen front end leaves the conv entries as they are
     if (cudaMemsetAsync(grads, 0, sizeof(float) * o.total, st) != cudaSuccess) { *err = "memset grads"; return B2CNN_ECUDA; }
-    train_lstm_bwd<kHeadLogits><<<(unsigned)pl.seq_ctas, 64, 0, st>>>(params, o, d, B, sequence, sq, age, nullptr, 1.f, dz, ws + w.acts, ws + w.cs,
-                                                                     ws + w.hs, ws + w.lin, nullptr, ws + w.da0, grads, dage);
-    launch_head_reduce(pl, o, sq, B, grads, nullptr, st);
-    if (!launch_backward_tail(d, o, pl, ws, params, x, B, mask1, mask2, grads, dx, frozen_conv, st)) { *err = "memset dx"; return B2CNN_ECUDA; }
+    train_lstm_bwd<kHeadLogits><<<(unsigned)pl.seq_ctas, 64, 0, st>>>(params, o, d, rec.rows, sequence, sq, age, nullptr, 1.f, dz, ws + w.acts,
+                                                                     ws + w.cs, ws + w.hs, ws + w.lin, nullptr, ws + w.da0, grads, dage);
+    launch_head_reduce(pl, o, sq, rec.rows, grads, nullptr, st);
+    if (!backward_tail(d, rec, o, pl, ws, params, x, B, mask1, mask2, grads, dx, frozen_conv, rr, st)) { *err = "memset dx"; return B2CNN_ECUDA; }
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) { *err = cudaGetErrorString(e); return B2CNN_ECUDA; }
     return B2CNN_OK;

@@ -33,7 +33,7 @@ import torch
 
 from . import capi
 from .arch import BLOB_KEYS
-from .autograd import check_masks, check_trainable, draw_masks
+from .autograd import check_masks, check_record_batch, check_trainable, draw_masks, window_ages
 from .model import B200MyCNN
 
 
@@ -81,10 +81,11 @@ class B200Trainer:
         """d loss / d parameter of the most recent step, keyed like the reference's state_dict."""
         return self._views(self._grads)
 
-    def draw_masks(self, B: int) -> Tuple[Optional[torch.Tensor], Optional[torch.Tensor]]:
+    def draw_masks(self, B: int, n_samples: Optional[int] = None) -> Tuple[Optional[torch.Tensor], Optional[torch.Tensor]]:
         """The two nn.Dropout masks of bin/models.py:25,28, scaled by 1/(1-p) like torch's dropout, from the trainer's
-        seeded generator."""
-        return draw_masks(self.model.arch, B, self.dropout, self._params.device, self._gen)
+        seeded generator: of B windows, or with ``n_samples`` of B recordings of that many samples (:meth:`step_record`)."""
+        arch = self.model.arch if n_samples is None else self.model.arch.with_shape(self.model.arch.in_channels, n_samples)
+        return draw_masks(arch, B, self.dropout, self._params.device, self._gen)
 
     def step(self, x: torch.Tensor, age: torch.Tensor, target: torch.Tensor,
              masks: Optional[Tuple[Optional[torch.Tensor], Optional[torch.Tensor]]] = None, update: bool = True,
@@ -133,6 +134,45 @@ class B200Trainer:
             capi.check(self._lib.b2cnn_train_step(*head, *tail), "b2cnn_train_step")
         else:
             capi.check(self._lib.b2cnn_train_step_weighted(*head, self.pos_weight, *tail), "b2cnn_train_step_weighted")
+        return self._finish(update)
+
+    def step_record(self, records: torch.Tensor, stride: int, age, target: torch.Tensor, window_counts=None,
+                    masks: Optional[Tuple[Optional[torch.Tensor], Optional[torch.Tensor]]] = None, update: bool = True) -> torch.Tensor:
+        """:meth:`step` over every counted window of whole recordings ``[B, C, N]`` (fp32 or bf16), each window feature
+        computed and back-propagated once: window w of recording b is ``records[b, :, w*stride : w*stride + W]`` for
+        w < ``window_counts[b]`` (default: all n_w = (N - W) // stride + 1; fewer, down to 0, pads a ragged batch to one
+        N).  ``stride``: a positive multiple of ``pool_s ** 2``.  ``age``: a scalar or one per recording; ``target``: one
+        per window, recording-major [M].  In sequence mode each recording's windows are one sequence, the LSTM starting
+        from zero (``step(windows, ..., seq_lengths=`` the non-zero counts ``)``); in independent mode every window is
+        alone.  The loss is the mean over the M windows.  ``masks``: the recording's dropout masks [B, c_mid, P1(N)] /
+        [B, L(N)] (default :meth:`draw_masks` ``(B, N)``); window w uses the slices at its own positions, so a feature
+        two windows share is dropped in both or in neither.  Samples no counted window reads (tails, gaps when stride >
+        W, recordings with count 0) change nothing, NaN included."""
+        dev = self._params.device
+        stride, age, counts, M, rarch = check_record_batch(self.model.arch, records, stride, age, window_counts)
+        B, N = records.shape[0], records.shape[2]
+        target = torch.as_tensor(target).detach().to(dev, torch.float32).reshape(-1).contiguous()
+        if target.numel() != M:
+            raise ValueError(f"target must have one entry per window ({M}), got {target.numel()}")
+        m1, m2 = check_masks(rarch, B, dev, *(masks if masks is not None else self.draw_masks(B, N)))
+        mode = capi.MODE_SEQUENCE if self.mode == "sequence" else capi.MODE_INDEPENDENT
+        need = self._lib.b2cnn_train_workspace_bytes_record(ctypes.byref(self._cfg), B, N, stride, counts, mode)
+        if need < 0:
+            capi.check(capi.EINVAL, "b2cnn_train_workspace_bytes_record")
+        records = records.to(dev, torch.float32).contiguous()
+        age = window_ages(age.detach(), counts, M, dev)
+        if self._ws is None or self._ws.numel() < need:
+            self._ws = torch.empty(need, dtype=torch.uint8, device=dev)
+        ptr = lambda t: ctypes.c_void_p(t.data_ptr()) if t is not None else None
+        pw = None if self.pos_weight is None else ctypes.byref(ctypes.c_float(self.pos_weight))
+        st = torch.cuda.current_stream(dev).cuda_stream
+        capi.check(self._lib.b2cnn_train_step_record(ctypes.byref(self._cfg), ptr(self._params), ptr(self._m), ptr(self._v), ptr(self._grads),
+                                                     self.steps + 1, ctypes.byref(self._opt), 1 if update else 0, ptr(records), B, N, stride,
+                                                     counts, mode, ptr(age), ptr(target), pw, ptr(m1), ptr(m2), ptr(self._loss),
+                                                     ptr(self._ws), need, ctypes.c_void_p(st)), "b2cnn_train_step_record")
+        return self._finish(update)
+
+    def _finish(self, update: bool) -> torch.Tensor:
         if update:
             self.steps += 1
             with torch.no_grad():                        # the inference kernels read the module's parameters
