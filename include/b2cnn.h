@@ -323,6 +323,18 @@ int b2cnn_slide_samples_seen(b2cnn_slide *slide, int64_t *seen, void *stream);
 int b2cnn_slide_create_ex(b2cnn_handle *h, int32_t n_patients, int32_t stride, int dtype, int path, int mode, b2cnn_slide **out);
 int b2cnn_slide_mode(const b2cnn_slide *slide);
 
+/* Warm-started admission (DESIGN.md §6, state across calls).  The LSTM state of one patient or recording is 64 floats,
+ * [layer][h | c][unit] = h0 | c0 | h1 | c1 of 16 units each (b2cnn_slide_export_ex's rows, b2cnn_score_record_state's).
+ *   b2cnn_slide_admit_ex  b2cnn_slide_admit plus lstm: DEVICE float [n][64], row j the state patients[j]'s next LSTM step
+ *                        starts from, or NULL to zero the rows as b2cnn_slide_admit does.  A non-NULL lstm on an
+ *                        independent-mode scorer is B2CNN_EINVAL.  Every check of b2cnn_slide_admit runs first; the rows
+ *                        are written before the counts are committed, so a call that fails changes neither.  The
+ *                        handoff from a backtest to a live scorer: admit a stay of T >= W samples with history = its last
+ *                        W samples and lstm = b2cnn_score_record_state's state_out over samples (T - W) mod S .. T - 1;
+ *                        every later push then scores what b2cnn_score_record_state scores over the whole stream. */
+int b2cnn_slide_admit_ex(b2cnn_slide *slide, const int32_t *patients, int32_t n, const void *history, int64_t history_len,
+                         int64_t pitch, int dtype, const float *lstm, void *workspace, int64_t workspace_bytes, void *stream);
+
 /* Every sliding window of whole recordings in one call (DESIGN.md §7), each window feature computed once.
  *   b2cnn_score_record  x: DEVICE [B][C][pitch] samples of `dtype` (channel rows pitch >= N samples apart, recordings
  *                        C pitch apart; any alignment), N samples per recording.  out: DEVICE float [B][n_w], n_w =
@@ -360,6 +372,23 @@ int64_t b2cnn_record_workspace_bytes_ex(b2cnn_handle *h, int64_t B, int64_t N, i
 int b2cnn_score_record_ex(b2cnn_handle *h, const void *x, int dtype, int64_t B, int64_t N, int64_t pitch, int64_t stride, int path,
                           int mode, const float *age, int64_t n_age, int apply_sigmoid, float *out, void *workspace,
                           int64_t workspace_bytes, void *stream);
+
+/* A recording scored in chunks (DESIGN.md §7, state across calls).
+ *   b2cnn_score_record_state  b2cnn_score_record_ex in sequence mode with the LSTM state as an input and an output.
+ *                        state_in: DEVICE float [B][64] (layout above), recording b's scan starts from state_in[b]
+ *                        instead of zero; NULL: the zero state.  state_out: DEVICE float [B][64], recording b's state
+ *                        after its last window, or NULL.  With n_w = 0 no head kernel runs and state_out = state_in (zeros
+ *                        for a NULL state_in).  A NaN in state_in[b] makes recording b's outputs and state_out[b] NaN
+ *                        and no other recording's.  Cutting a recording x at window k into A = x[.., 0 .. (k - 1) S + W)
+ *                        and B = x[.., k S ..] and passing A's state_out as B's state_in gives A's and B's outputs and a
+ *                        final state that are bit-identical to one call over x, on both paths.  mode must be
+ *                        B2CNN_MODE_SEQUENCE (else B2CNN_EINVAL).  state_in and state_out must not overlap (else
+ *                        B2CNN_EINVAL): carry the state between calls in two buffers.  The same workspace as
+ *                        b2cnn_score_record_ex in sequence mode (b2cnn_record_workspace_bytes_ex); every check runs
+ *                        before the first launch. */
+int b2cnn_score_record_state(b2cnn_handle *h, const void *x, int dtype, int64_t B, int64_t N, int64_t pitch, int64_t stride, int path,
+                             int mode, const float *age, int64_t n_age, int apply_sigmoid, float *out, const float *state_in,
+                             float *state_out, void *workspace, int64_t workspace_bytes, void *stream);
 
 /* Export and import of patients (a restart, beds moved to another scorer or GPU, new LSTM / head weights).  A
  * patient's state is its current window's L features in window order, raw and unmasked (for a complete window
@@ -629,6 +658,39 @@ int b2cnn_train_backward_record(const b2cnn_config *cfg, const float *params, co
                                 const int64_t *window_counts, int mode, const float *age, const float *mask1, const float *mask2,
                                 const float *dz, float *grads, float *d_records, float *dage, int flags, void *workspace,
                                 int64_t workspace_bytes, void *stream);
+
+/* Training on chunks of recordings (DESIGN.md §8, state across calls): the _record calls in sequence mode with each
+ * recording's LSTM state, DEVICE float [B][64] = h0 | c0 | h1 | c1 (16 units each; b2cnn_score_record_state's layout).
+ * mode must be B2CNN_MODE_SEQUENCE (else B2CNN_EINVAL); every argument is checked before any CUDA call, and the workspace
+ * is b2cnn_train_workspace_bytes_record()'s for the same arguments (the states live in the caller's memory).  Every
+ * state pointer may be NULL: a NULL state_in is the zero state, and with every state NULL each call computes what its
+ * _record counterpart computes.  No two of a call's state arrays may overlap (B2CNN_EINVAL): the step's backward reads
+ * state_in after its forward has written state_out, so a TBPTT loop carries the state in two buffers, swapped per call.
+ *   b2cnn_train_forward_record_state  recording b's scan starts from state_in[b]; state_out[b] receives its state after
+ *                        its last counted window.  A recording with window_counts[b] == 0 passes it through: state_out[b]
+ *                        = state_in[b] (zeros for a NULL state_in).
+ *   b2cnn_train_backward_record_state  the forward's arguments (state_in included), dz, and d_state_out: the gradient
+ *                        of the loss at state_out (NULL: none).  Writes grads, d_records, dage as
+ *                        b2cnn_train_backward_record does, and d_state_in [B][64]: the gradient at state_in (d_state_out[b]
+ *                        for a recording without windows).  Chaining two forwards through the state and running the
+ *                        backwards in reverse order, d_state_in of the second as d_state_out of the first, gives the
+ *                        gradients of one call over the whole recordings.
+ *   b2cnn_train_step_record_state  b2cnn_train_step_record from state_in, writing state_out: truncated back-propagation
+ *                        through time (no gradient enters through state_out). */
+int b2cnn_train_step_record_state(const b2cnn_config *cfg, float *params, float *adam_m, float *adam_v, float *grads, int64_t step,
+                                  const b2cnn_adam *opt, int apply_update, const float *records, int64_t B, int64_t N, int64_t stride,
+                                  const int64_t *window_counts, int mode, const float *age, const float *target, const float *pos_weight,
+                                  const float *mask1, const float *mask2, const float *state_in, float *state_out, float *loss_out,
+                                  void *workspace, int64_t workspace_bytes, void *stream);
+int b2cnn_train_forward_record_state(const b2cnn_config *cfg, const float *params, const float *records, int64_t B, int64_t N,
+                                     int64_t stride, const int64_t *window_counts, int mode, const float *age, const float *mask1,
+                                     const float *mask2, const float *state_in, float *state_out, float *z_out, void *workspace,
+                                     int64_t workspace_bytes, void *stream);
+int b2cnn_train_backward_record_state(const b2cnn_config *cfg, const float *params, const float *records, int64_t B, int64_t N,
+                                      int64_t stride, const int64_t *window_counts, int mode, const float *age, const float *mask1,
+                                      const float *mask2, const float *state_in, const float *dz, const float *d_state_out, float *grads,
+                                      float *d_records, float *dage, float *d_state_in, int flags, void *workspace, int64_t workspace_bytes,
+                                      void *stream);
 
 #ifdef __cplusplus
 }

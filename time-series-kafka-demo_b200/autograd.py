@@ -32,7 +32,7 @@ from torch.autograd.function import once_differentiable
 
 from . import capi
 from .arch import BLOB_KEYS, ArchConfig
-from .model import B200MyCNN
+from .model import B200MyCNN, check_record_state
 
 _MODES = {"sequence": capi.MODE_SEQUENCE, "independent": capi.MODE_INDEPENDENT}
 
@@ -189,12 +189,65 @@ class _TrainForward(torch.autograd.Function):
                                                    _ptr(call.mask1), _ptr(call.mask2), _ptr(dz), _ptr(grads), _ptr(dx), _ptr(dage), flags,
                                                    _ptr(ws), ws.numel(), ctypes.c_void_p(st))
         capi.check(rc, "b2cnn_train_backward")
-        out, at = [], 0
-        for shape, need in zip(ctx.shapes, ctx.needs_input_grad[3:]):
-            n = shape.numel()
-            out.append(grads[at:at + n].view(shape) if need else None)
-            at += n
-        return (None, dx, dage, *out)
+        return (None, dx, dage, *_param_grads(grads, ctx.shapes, ctx.needs_input_grad[3:]))
+
+
+def _param_grads(grads, shapes, needs):
+    """the packed gradient blob as one tensor per parameter (None where none is needed)"""
+    out, at = [], 0
+    for shape, need in zip(shapes, needs):
+        n = shape.numel()
+        out.append(grads[at:at + n].view(shape) if need else None)
+        at += n
+    return out
+
+
+class _TrainRecordState(torch.autograd.Function):
+    """The sequence-mode ``_record`` call with each recording's LSTM state as an input and an output.  Inputs: a
+    :class:`_Call` with ``rec`` set, the recordings [B,C,N] fp32, age [M] fp32, state [B,2,2,16] fp32 or None (zeros),
+    then the 14 ``BLOB_KEYS`` tensors.  Outputs: the logits [M] and the state after each recording's last counted window
+    [B,2,2,16]; both are differentiable, and so is the input state."""
+
+    @staticmethod
+    def forward(ctx, call, x, age, state, *params):
+        dev = x.device
+        blob = torch.cat([p.detach().reshape(-1) for p in params])
+        B = x.shape[0]
+        N, S, counts, _ = call.rec
+        ws = torch.empty(call.workspace_bytes(B), dtype=torch.uint8, device=dev)
+        z = torch.empty(age.numel(), dtype=torch.float32, device=dev)
+        state_out = torch.empty(B, 2, 2, 16, dtype=torch.float32, device=dev)
+        st = torch.cuda.current_stream(dev).cuda_stream
+        rc = call.lib.b2cnn_train_forward_record_state(ctypes.byref(call.cfg), _ptr(blob), _ptr(x), B, N, S, counts, call.mode, _ptr(age),
+                                                       _ptr(call.mask1), _ptr(call.mask2), _ptr(state), _ptr(state_out), _ptr(z),
+                                                       _ptr(ws), ws.numel(), ctypes.c_void_p(st))
+        capi.check(rc, "b2cnn_train_forward_record_state")
+        ctx.call, ctx.blob, ctx.ws = call, blob, ws
+        ctx.shapes = [p.shape for p in params]
+        ctx.save_for_backward(x, age, state)
+        return z, state_out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dz, dstate):
+        call, blob, ws = ctx.call, ctx.blob, ctx.ws
+        x, age, state = ctx.saved_tensors
+        B = x.shape[0]
+        N, S, counts, _ = call.rec
+        dz = dz.to(torch.float32).contiguous()
+        dstate = dstate.to(torch.float32).contiguous()
+        grads = torch.empty_like(blob)
+        dx = torch.empty_like(x) if ctx.needs_input_grad[1] else None
+        dage = torch.empty_like(age) if ctx.needs_input_grad[2] else None
+        dstate_in = torch.empty_like(dstate) if ctx.needs_input_grad[3] else None
+        frozen = dx is None and not any(ctx.needs_input_grad[4:8])
+        st = torch.cuda.current_stream(x.device).cuda_stream
+        rc = call.lib.b2cnn_train_backward_record_state(ctypes.byref(call.cfg), _ptr(blob), _ptr(x), B, N, S, counts, call.mode, _ptr(age),
+                                                        _ptr(call.mask1), _ptr(call.mask2), _ptr(state), _ptr(dz), _ptr(dstate),
+                                                        _ptr(grads), _ptr(dx), _ptr(dage), _ptr(dstate_in),
+                                                        capi.TRAIN_FROZEN_CONV if frozen else 0, _ptr(ws), ws.numel(), ctypes.c_void_p(st))
+        capi.check(rc, "b2cnn_train_backward_record_state")
+        return (None, dx, dage, dstate_in, *_param_grads(grads, ctx.shapes, ctx.needs_input_grad[4:]))
 
 
 class _Call:
@@ -275,7 +328,7 @@ def mycnn_train_forward(x: torch.Tensor, age: torch.Tensor, params: Sequence[tor
 
 def mycnn_train_record_forward(records: torch.Tensor, stride: int, age, params: Sequence[torch.Tensor], arch: ArchConfig,
                                mode: str = "sequence", mask1: Optional[torch.Tensor] = None, mask2: Optional[torch.Tensor] = None,
-                               window_counts=None) -> torch.Tensor:
+                               window_counts=None, state=None, return_state: bool = False):
     """Logits [M] of every counted window of whole recordings in train() mode, differentiable in ``records``, ``age``
     and ``params``; each window feature is computed, and back-propagated, once however many windows share it.
 
@@ -289,17 +342,30 @@ def mycnn_train_record_forward(records: torch.Tensor, stride: int, age, params: 
     masks, the geometry of a window of N samples (``arch.with_shape(C, N)``); window w uses the slices at its own
     positions, so a feature two windows share is dropped in both or in neither (the one difference from cutting the
     windows first and drawing their masks independently).  Samples no counted window reads change nothing, NaN
-    included, and get a zero gradient."""
+    included, and get a zero gradient.
+
+    State across calls (mode "sequence" only, else ValueError): ``state`` ``[B, 2, 2, 16]``, [recording][layer][h |
+    c][unit] (as ``nn.LSTM``'s tuple: ``h = state[:, :, 0].transpose(0, 1)``, ``c = state[:, :, 1].transpose(0, 1)``), is
+    the state recording b's LSTM starts from (None: zeros); it may require grad.  ``return_state=True`` returns ``(z,
+    state_out)``, ``state_out[b]`` the state after recording b's last counted window (``state[b]`` itself for a count of
+    0), differentiable too: chaining two calls through it and back-propagating once gives the gradients of one call over
+    the whole recordings (full back-propagation through time); ``state_out.detach()`` cuts it (truncated)."""
     check_trainable(arch)
     if mode not in _MODES:
         raise ValueError("mode must be 'sequence' or 'independent'")
     dev = _check_params(params, arch)
     stride, age, counts, M, rarch = check_record_batch(arch, records, stride, age, window_counts)
+    check_record_state(records, mode, state, return_state)
     B, N = records.shape[0], records.shape[2]
     masks = check_masks(rarch, B, dev, mask1, mask2)
     records = records.to(dev, torch.float32).contiguous()
     call = _Call(arch, dev, _MODES[mode], *masks, rec=(N, stride, counts, M))
-    return _TrainForward.apply(call, records, window_ages(age, counts, M, dev), *params)
+    if state is None and not return_state:
+        return _TrainForward.apply(call, records, window_ages(age, counts, M, dev), *params)
+    if state is not None:
+        state = state.to(dev, torch.float32).contiguous()
+    z, state_out = _TrainRecordState.apply(call, records, window_ages(age, counts, M, dev), state, *params)
+    return (z, state_out) if return_state else z
 
 
 class B200TrainableMyCNN(B200MyCNN):
@@ -348,12 +414,20 @@ class B200TrainableMyCNN(B200MyCNN):
         named = dict(self.named_parameters())
         return mycnn_train_forward(x, age, [named[k] for k in BLOB_KEYS], self.arch, mode, m1, m2, seq_lengths)
 
-    def forward_record(self, records: torch.Tensor, stride: int, age, window_counts=None) -> torch.Tensor:
+    def forward_record(self, records: torch.Tensor, stride: int, age, window_counts=None, state=None, return_state: bool = False):
         """Logits [M] of every counted window of whole recordings ``[B, C, N]`` (see :func:`mycnn_train_record_forward`),
         recording-major: in train mode differentiable, with the dropout masks drawn at the recording's geometry and the
         LSTM over each recording's windows (``batch_mode == "sequence"``) or every window alone; in eval mode
-        ``predict_record(records, stride, age, mode=batch_mode)`` with each row cut to its count."""
+        ``predict_record(records, stride, age, mode=batch_mode)`` with each row cut to its count.  ``state`` /
+        ``return_state``: the LSTM state across calls (``batch_mode == "sequence"``; see
+        :func:`mycnn_train_record_forward`); in eval mode ``predict_record``'s, which counts every window."""
         stride, _, counts, M, _ = check_record_batch(self.arch, records, stride, age, window_counts)
+        check_record_state(records, self.batch_mode, state, return_state)
+        if not self.training and (state is not None or return_state):
+            n_w = (records.shape[2] - self.arch.window) // stride + 1 if records.shape[2] >= self.arch.window else 0
+            if any(int(c) != n_w for c in counts):
+                raise ValueError("in eval mode the LSTM state needs every window counted (window_counts=None)")
+            return self.predict_record(records, stride, age, mode=self.batch_mode, state=state, return_state=return_state)
         if not self.training:
             out = self.predict_record(records, stride, age, mode=self.batch_mode)
             keep = torch.arange(out.shape[1], device=out.device) < torch.tensor(list(counts), device=out.device)[:, None]
@@ -363,4 +437,4 @@ class B200TrainableMyCNN(B200MyCNN):
         m1, m2 = self.draw_masks(records.shape[0], records.shape[2])
         named = dict(self.named_parameters())
         return mycnn_train_record_forward(records, stride, age, [named[k] for k in BLOB_KEYS], self.arch, self.batch_mode, m1, m2,
-                                          window_counts)
+                                          window_counts, state, return_state)

@@ -206,6 +206,40 @@ extern "C" int b2cnn_train_backward_record(const b2cnn_config *cfg, const float 
                                   grads, d_records, dage, flags, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream), &err);
     return finish("b2cnn_train_backward_record", rc, err);
 }
+extern "C" int b2cnn_train_step_record_state(const b2cnn_config *cfg, float *params, float *adam_m, float *adam_v, float *grads,
+                                             int64_t step, const b2cnn_adam *opt, int apply_update, const float *records, int64_t B,
+                                             int64_t N, int64_t stride, const int64_t *window_counts, int mode, const float *age,
+                                             const float *target, const float *pos_weight, const float *mask1, const float *mask2,
+                                             const float *state_in, float *state_out, float *loss_out, void *workspace,
+                                             int64_t workspace_bytes, void *stream) {
+    if (mode != B2CNN_MODE_SEQUENCE) return fail(B2CNN_EINVAL, "b2cnn_train_step_record_state: mode must be B2CNN_MODE_SEQUENCE");
+    return train_step_api("b2cnn_train_step_record_state", cfg, params, adam_m, adam_v, grads, step, opt, apply_update, records, B, age,
+                          target, pos_weight ? 1 : 0, pos_weight ? *pos_weight : 1.f, mode, kNoSeq,
+                          RecordArgs{true, N, stride, window_counts, state_in, state_out}, mask1, mask2, loss_out, workspace,
+                          workspace_bytes, stream);
+}
+extern "C" int b2cnn_train_forward_record_state(const b2cnn_config *cfg, const float *params, const float *records, int64_t B, int64_t N,
+                                                int64_t stride, const int64_t *window_counts, int mode, const float *age, const float *mask1,
+                                                const float *mask2, const float *state_in, float *state_out, float *z_out, void *workspace,
+                                                int64_t workspace_bytes, void *stream) {
+    if (mode != B2CNN_MODE_SEQUENCE) return fail(B2CNN_EINVAL, "b2cnn_train_forward_record_state: mode must be B2CNN_MODE_SEQUENCE");
+    const char *err = "";
+    const int rc = train_forward(cfg, params, records, B, age, mode, kNoSeq, RecordArgs{true, N, stride, window_counts, state_in, state_out},
+                                 mask1, mask2, z_out, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream), &err);
+    return finish("b2cnn_train_forward_record_state", rc, err);
+}
+extern "C" int b2cnn_train_backward_record_state(const b2cnn_config *cfg, const float *params, const float *records, int64_t B, int64_t N,
+                                                 int64_t stride, const int64_t *window_counts, int mode, const float *age,
+                                                 const float *mask1, const float *mask2, const float *state_in, const float *dz,
+                                                 const float *d_state_out, float *grads, float *d_records, float *dage, float *d_state_in,
+                                                 int flags, void *workspace, int64_t workspace_bytes, void *stream) {
+    if (mode != B2CNN_MODE_SEQUENCE) return fail(B2CNN_EINVAL, "b2cnn_train_backward_record_state: mode must be B2CNN_MODE_SEQUENCE");
+    const char *err = "";
+    const int rc = train_backward(cfg, params, records, B, age, mode, kNoSeq,
+                                  RecordArgs{true, N, stride, window_counts, state_in, nullptr, d_state_out, d_state_in}, mask1, mask2, dz,
+                                  grads, d_records, dage, flags, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream), &err);
+    return finish("b2cnn_train_backward_record_state", rc, err);
+}
 
 // ---- preprocessing + window assembly (b2cnn_prep.cu) ----
 extern "C" int64_t b2cnn_prep_window_count(int64_t n_samples, double fs, const b2cnn_prep_config *cfg) {
@@ -834,17 +868,27 @@ extern "C" int b2cnn_slide_features(b2cnn_slide *o, float *feats, void *stream) 
 extern "C" int64_t b2cnn_slide_admit_workspace_bytes(b2cnn_slide *o, int32_t n, int64_t history_len) {
     return o ? slide_admit_workspace_bytes(o->s, n, history_len) : -1;
 }
-extern "C" int b2cnn_slide_admit(b2cnn_slide *o, const int32_t *patients, int32_t n, const void *history, int64_t history_len,
-                                 int64_t pitch, int dtype, void *workspace, int64_t workspace_bytes, void *stream) {
-    if (!o) return fail(B2CNN_EINVAL, "b2cnn_slide_admit: null argument");
-    if (dtype != slide_dtype(o->s)) return fail(B2CNN_EINVAL, "b2cnn_slide_admit: the history's dtype is not the scorer's");
-    if (int rc = check_fresh("b2cnn_slide_admit", o)) return rc;
+static int slide_admit_api(const char *fn, b2cnn_slide *o, const int32_t *patients, int32_t n, const void *history, int64_t history_len,
+                           int64_t pitch, int dtype, const float *lstm, void *workspace, int64_t workspace_bytes, void *stream) {
+    if (!o) return fail(B2CNN_EINVAL, std::string(fn) + ": null argument");
+    if (dtype != slide_dtype(o->s)) return fail(B2CNN_EINVAL, std::string(fn) + ": the history's dtype is not the scorer's");
+    if (int rc = check_fresh(fn, o)) return rc;
     b2cnn_handle *h = o->h;
     DEVICE_GUARD(h->device);
     const char *err = "";
-    const int rc = slide_admit(o->s, h->cw, h->tc, patients, n, history, history_len, pitch, workspace, workspace_bytes,
+    const int rc = slide_admit(o->s, h->cw, h->tc, patients, n, history, history_len, pitch, lstm, workspace, workspace_bytes,
                                reinterpret_cast<cudaStream_t>(stream), &err);
-    return finish("b2cnn_slide_admit", rc, err);
+    return finish(fn, rc, err);
+}
+extern "C" int b2cnn_slide_admit(b2cnn_slide *o, const int32_t *patients, int32_t n, const void *history, int64_t history_len,
+                                 int64_t pitch, int dtype, void *workspace, int64_t workspace_bytes, void *stream) {
+    return slide_admit_api("b2cnn_slide_admit", o, patients, n, history, history_len, pitch, dtype, nullptr, workspace, workspace_bytes,
+                           stream);
+}
+extern "C" int b2cnn_slide_admit_ex(b2cnn_slide *o, const int32_t *patients, int32_t n, const void *history, int64_t history_len,
+                                    int64_t pitch, int dtype, const float *lstm, void *workspace, int64_t workspace_bytes, void *stream) {
+    return slide_admit_api("b2cnn_slide_admit_ex", o, patients, n, history, history_len, pitch, dtype, lstm, workspace, workspace_bytes,
+                           stream);
 }
 extern "C" int b2cnn_slide_discharge(b2cnn_slide *o, const int32_t *patients, int32_t n, void *stream) {
     if (!o) return fail(B2CNN_EINVAL, "b2cnn_slide_discharge: null argument");
@@ -949,14 +993,14 @@ extern "C" int64_t b2cnn_record_workspace_bytes_ex(b2cnn_handle *h, int64_t B, i
 
 static int record_score(const char *fn, b2cnn_handle *h, const void *x, int dtype, int64_t B, int64_t N, int64_t pitch, int64_t stride,
                         int path, int mode, const float *age, int64_t n_age, int apply_sigmoid, float *out, void *workspace,
-                        int64_t workspace_bytes, void *stream) {
+                        int64_t workspace_bytes, void *stream, const float *state_in = nullptr, float *state_out = nullptr) {
     bool tc = false;
     if (int rc = record_path(fn, h, dtype, path, &tc)) return rc;
     if (!x || !age || !out) return fail(B2CNN_EINVAL, std::string(fn) + ": null argument");
     DEVICE_GUARD(h->device);
     const char *err = "";
     const int rc = score_record(h->d, h->cw, h->hw, h->tc, tc, h->num_sms, x, dtype, B, N, pitch, stride, mode, age, n_age, apply_sigmoid,
-                                out, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream), &err);
+                                out, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream), &err, state_in, state_out);
     if (rc != B2CNN_OK) return finish(fn, rc, err);
     h->last_path = tc ? B2CNN_PATH_TENSORCORE : B2CNN_PATH_GENERIC;
     return B2CNN_OK;
@@ -974,6 +1018,14 @@ extern "C" int b2cnn_score_record_ex(b2cnn_handle *h, const void *x, int dtype, 
                                      int64_t workspace_bytes, void *stream) {
     return record_score("b2cnn_score_record_ex", h, x, dtype, B, N, pitch, stride, path, mode, age, n_age, apply_sigmoid, out, workspace,
                         workspace_bytes, stream);
+}
+
+extern "C" int b2cnn_score_record_state(b2cnn_handle *h, const void *x, int dtype, int64_t B, int64_t N, int64_t pitch, int64_t stride,
+                                        int path, int mode, const float *age, int64_t n_age, int apply_sigmoid, float *out,
+                                        const float *state_in, float *state_out, void *workspace, int64_t workspace_bytes, void *stream) {
+    if (mode != B2CNN_MODE_SEQUENCE) return fail(B2CNN_EINVAL, "b2cnn_score_record_state: mode must be B2CNN_MODE_SEQUENCE");
+    return record_score("b2cnn_score_record_state", h, x, dtype, B, N, pitch, stride, path, mode, age, n_age, apply_sigmoid, out, workspace,
+                        workspace_bytes, stream, state_in, state_out);
 }
 
 // ---- host-pointer entry: chunked H2D overlapped with compute -----------------------------

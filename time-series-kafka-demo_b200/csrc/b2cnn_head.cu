@@ -241,14 +241,19 @@ head_reduce_independent_kernel(const float *__restrict__ part, int slices, HeadW
 }
 
 // One warp (one CTA) per segment: CTA s scans rows s seg_len .. s seg_len + seg_len - 1 of gates0, age (n_age > 1) and
-// out sequentially from the zero state, or with seg_off rows seg_off[s] .. seg_off[s + 1] - 1.  forward's sequence mode
-// is one segment of B rows, or one per sequence of b2cnn_forward_seq; b2cnn_score_record's is one segment per recording,
-// of its n_w windows.  Each row is one seq_step (b2cnn_head_dev.cuh).
+// out sequentially, or with seg_off rows seg_off[s] .. seg_off[s + 1] - 1.  forward's sequence mode is one segment of B
+// rows, or one per sequence of b2cnn_forward_seq; b2cnn_score_record's is one segment per recording, of its n_w windows.
+// Each row is one seq_step (b2cnn_head_dev.cuh).  The scan starts from the zero state, or from state_in[s] [64] = h0 |
+// c0 | h1 | c1 (16 units each) when state_in is not null; with state_out, segment s's state after its last row goes to
+// state_out[s] in the same layout.  kState == false (every launch without a state) ignores both pointers and compiles to
+// the scan without them.
+template <bool kState>
 __global__ void __launch_bounds__(32)
 head_sequence_kernel(const float *__restrict__ gates0, HeadWeights hw, const float *__restrict__ age,
                      int64_t n_age, float coef, int apply_sigmoid, float *__restrict__ out, int64_t seg_len,
-                     const int64_t *__restrict__ seg_off) {
-    const int l = threadIdx.x;
+                     const int64_t *__restrict__ seg_off, const float *__restrict__ state_in, float *__restrict__ state_out) {
+    if constexpr (!kState) { state_in = nullptr; state_out = nullptr; }
+    const int l = threadIdx.x, u = l & 15;
     const int64_t row0 = seg_off ? seg_off[blockIdx.x] : (int64_t)blockIdx.x * seg_len;
     const int64_t B = seg_off ? seg_off[blockIdx.x + 1] - row0 : seg_len;
     gates0 += row0 * kGates;
@@ -257,11 +262,19 @@ head_sequence_kernel(const float *__restrict__ gates0, HeadWeights hw, const flo
     SeqLaneWeights w;
     seq_load_weights(hw, l, w);
     SeqState s = {0.f, 0.f, 0.f, 0.f};
+    if (state_in) {
+        const float *si = state_in + (int64_t)blockIdx.x * kGates;
+        s = {si[u], si[kHidden + u], si[2 * kHidden + u], si[3 * kHidden + u]};
+    }
     float na = gates0[l], nb = gates0[l + 32];
     for (int64_t t = 0; t < B; ++t) {
         const float ga = na, gb = nb;                      // (W_ih x + b_ih) + b_hh
         if (t + 1 < B) { na = gates0[(t + 1) * kGates + l]; nb = gates0[(t + 1) * kGates + l + 32]; }
         seq_step(w, s, ga, gb, l, age + (n_age == 1 ? 0 : t), coef, apply_sigmoid, out + t);
+    }
+    if (state_out && l < kHidden) {
+        float *so = state_out + (int64_t)blockIdx.x * kGates;
+        so[u] = s.h0; so[kHidden + u] = s.c0; so[2 * kHidden + u] = s.h1; so[3 * kHidden + u] = s.c1;
     }
 }
 
@@ -372,7 +385,7 @@ int launch_ring_head(const Dims &d, const HeadWeights &hw, const float *ring, in
 // sequence mode each recording's n_w rows are one LSTM scan
 int launch_record_head(const Dims &d, const HeadWeights &hw, const float *feats, int64_t rec_pitch, int n_w, int64_t step, int64_t rows,
                        const float *age, int64_t n_age, int mode, int apply_sigmoid, float *out, float *gates_ws, float *partial_ws,
-                       cudaStream_t st, const char **err) {
+                       cudaStream_t st, const char **err, const float *state_in, float *state_out) {
     int ks_eff;
     const int kps = proj_split(d.L, choose_ksplit(d.L), &ks_eff);
     record_proj_kernel<<<dim3((unsigned)((rows + kPM - 1) / kPM), ks_eff), 256, 0, st>>>(feats, rec_pitch, n_w, step, hw.wih0T,
@@ -382,7 +395,7 @@ int launch_record_head(const Dims &d, const HeadWeights &hw, const float *feats,
     int n = launch_reduce_gates(partial_ws, ks_eff, rows, hw, gates_ws, st, err);
     if (n < 0) return -1;
     n = mode == B2CNN_MODE_SEQUENCE
-            ? launch_sequence_segments(d, hw, gates_ws, rows / n_w, n_w, age, n_age, apply_sigmoid, out, st, err)
+            ? launch_sequence_segments(d, hw, gates_ws, rows / n_w, n_w, age, n_age, apply_sigmoid, out, st, err, nullptr, state_in, state_out)
             : launch_lstm_head(d, hw, gates_ws, rows, age, n_age, B2CNN_MODE_INDEPENDENT, apply_sigmoid, out, st, err);
     return n < 0 ? -1 : 3;
 }
@@ -427,8 +440,14 @@ int launch_lstm_head(const Dims &d, const HeadWeights &hw, const float *gates, i
 
 // n_seg independent LSTM scans of seg_len consecutive rows each, one warp per segment
 int launch_sequence_segments(const Dims &d, const HeadWeights &hw, const float *gates, int64_t n_seg, int64_t seg_len, const float *age,
-                             int64_t n_age, int apply_sigmoid, float *out, cudaStream_t st, const char **err, const int64_t *seg_off) {
-    head_sequence_kernel<<<(unsigned)n_seg, 32, 0, st>>>(gates, hw, age, n_age, d.age_coef, apply_sigmoid, out, seg_len, seg_off);
+                             int64_t n_age, int apply_sigmoid, float *out, cudaStream_t st, const char **err, const int64_t *seg_off,
+                             const float *state_in, float *state_out) {
+    if (state_in || state_out)
+        head_sequence_kernel<true><<<(unsigned)n_seg, 32, 0, st>>>(gates, hw, age, n_age, d.age_coef, apply_sigmoid, out, seg_len, seg_off,
+                                                                   state_in, state_out);
+    else
+        head_sequence_kernel<false><<<(unsigned)n_seg, 32, 0, st>>>(gates, hw, age, n_age, d.age_coef, apply_sigmoid, out, seg_len, seg_off,
+                                                                    nullptr, nullptr);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) { *err = cudaGetErrorString(e); return -1; }
     return 1;

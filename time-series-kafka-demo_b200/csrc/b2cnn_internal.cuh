@@ -99,12 +99,37 @@ inline bool seq_offsets(const SeqLengths &sl, int64_t B, std::vector<int64_t> &o
     return true;
 }
 
+// whether the device arrays of `bytes` bytes at a and at b share a byte (false when either is null)
+inline bool overlap(const void *a, const void *b, size_t bytes) {
+    if (!a || !b) return false;
+    const uintptr_t x = reinterpret_cast<uintptr_t>(a), y = reinterpret_cast<uintptr_t>(b);
+    return x < y + bytes && y < x + bytes;
+}
+
 // The windows of a _record training call (include/b2cnn.h): B recordings of N samples, windows of the configuration's W
-// samples every S samples, counts[b] of them (a host array) from recording b; on == false for every other call
+// samples every S samples, counts[b] of them (a host array) from recording b; on == false for every other call.  The
+// _record_state calls (sequence mode) add the LSTM state of each recording, device [B][64] = h0 | c0 | h1 | c1, each
+// pointer may be null: state_in (the scan starts from it instead of zero), state_out (the state after the recording's
+// last counted window), and for the backward d_state_out (the gradient arriving at state_out) and d_state_in (the
+// gradient of state_in).  A recording without windows passes both through.
 struct RecordArgs {
     bool on;
     int64_t N, S;
     const int64_t *counts;
+    const float *state_in = nullptr;
+    float *state_out = nullptr;
+    const float *d_state_out = nullptr;
+    float *d_state_in = nullptr;
+    bool has_state() const { return state_in || state_out || d_state_out || d_state_in; }
+    // whether two of the state arrays of B recordings overlap: an output written while an input is still to be read
+    bool states_overlap(int64_t B) const {
+        const void *p[4] = {state_in, state_out, d_state_out, d_state_in};
+        const size_t bytes = sizeof(float) * 64 * (size_t)B;
+        for (int i = 0; i < 4; ++i)
+            for (int j = i + 1; j < 4; ++j)
+                if (overlap(p[i], p[j], bytes)) return true;
+        return false;
+    }
 };
 
 // Makes `device` current for the guard's lifetime and restores the caller's device on every exit path (a call on cuda:1
@@ -218,10 +243,12 @@ int launch_lstm_head(const Dims &d, const HeadWeights &hw, const float *gates, i
                      const int64_t *seq_off = nullptr, int64_t n_seq = 0);
 // sequence mode over n_seg segments of seg_len consecutive rows of gates [n_seg seg_len][64], age (n_age = 1 or n_seg
 // seg_len) and out, each scanned from the zero state; launch_lstm_head's sequence mode is one segment of B rows.
-// seg_off != nullptr (device memory, n_seg + 1 offsets): segment s is rows [seg_off[s], seg_off[s + 1]) instead
+// seg_off != nullptr (device memory, n_seg + 1 offsets): segment s is rows [seg_off[s], seg_off[s + 1]) instead.
+// state_in / state_out (device memory, [n_seg][64] = h0 | c0 | h1 | c1, each may be null): segment s starts from
+// state_in[s] instead of zero, and its state after its last row is stored to state_out[s]
 int launch_sequence_segments(const Dims &d, const HeadWeights &hw, const float *gates, int64_t n_seg, int64_t seg_len, const float *age,
                              int64_t n_age, int apply_sigmoid, float *out, cudaStream_t st, const char **err,
-                             const int64_t *seg_off = nullptr);
+                             const int64_t *seg_off = nullptr, const float *state_in = nullptr, float *state_out = nullptr);
 // a sequence-mode sliding scorer's head: for every live patient p (all with seen == nullptr, else seen[p] >= 0 &&
 // seen[p] + S >= d.W, the counts before the push advances them), one LSTM step from state[p] [64] = h0 | c0 | h1 | c1,
 // its layer-0 gates summed from partial [slices][P][64] as launch_reduce_gates does; out[p] and state[p] written
@@ -248,10 +275,10 @@ int launch_ring_proj(const Dims &d, const HeadWeights &hw, const float *ring, in
 // launch_head of the n_w windows of each whole recording (b2cnn_record.cu, b2cnn_score_record, generic path): row b =
 // window b mod n_w of recording b / n_w, position k at feats[(b / n_w) rec_pitch + (b mod n_w) step + k]; rows =
 // recordings x n_w; the same tiles and summation order as launch_head.  mode B2CNN_MODE_SEQUENCE: one LSTM scan per
-// recording over its n_w windows (launch_sequence_segments) instead of independent windows
+// recording over its n_w windows (launch_sequence_segments, from state_in and into state_out) instead of independent windows
 int launch_record_head(const Dims &d, const HeadWeights &hw, const float *feats, int64_t rec_pitch, int n_w, int64_t step, int64_t rows,
                        const float *age, int64_t n_age, int mode, int apply_sigmoid, float *out, float *gates_ws, float *partial_ws,
-                       cudaStream_t st, const char **err);
+                       cudaStream_t st, const char **err, const float *state_in = nullptr, float *state_out = nullptr);
 
 // b2cnn_small.cu: whole forward pass of short windows in one launch (independent windows only)
 bool small_supported(const Dims &d);

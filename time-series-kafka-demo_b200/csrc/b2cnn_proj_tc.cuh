@@ -71,11 +71,14 @@ __device__ __forceinline__ void rp_store_partial(float *part, int range, int n_r
 // (0 for N < W).  use_tc: the tensor-core path (the caller has checked that the handle's TcState holds the model).  The
 // workspace size is -1 (with *err) for bad arguments.  mode: B2CNN_MODE_INDEPENDENT (every window from the zero LSTM
 // state) or B2CNN_MODE_SEQUENCE (the LSTM carried over each recording's windows in order, from the zero state per
-// recording).
+// recording, or from state_in[b] when state_in is not null; state_out[b] receives recording b's state after its last
+// window, state_in[b] (or zeros) when it has none).  state_in / state_out: device [B][64] = h0 | c0 | h1 | c1, null
+// or sequence mode only (else B2CNN_EINVAL).
 int64_t record_workspace_bytes(const Dims &d, const TcState &tc, bool use_tc, int64_t B, int64_t N, int64_t stride, int dtype, int mode,
                                const char **err);
 int score_record(const Dims &d, const ConvWeights &cw, const HeadWeights &hw, const TcState &tc, bool use_tc, int num_sms, const void *x,
                  int dtype, int64_t B, int64_t N, int64_t pitch, int64_t stride, int mode, const float *age, int64_t n_age, int apply_sigmoid,
-                 float *out, void *ws, int64_t ws_bytes, cudaStream_t st, const char **err);
+                 float *out, void *ws, int64_t ws_bytes, cudaStream_t st, const char **err, const float *state_in = nullptr,
+                 float *state_out = nullptr);
 
 }  // namespace b2cnn

@@ -211,13 +211,23 @@ int64_t record_workspace_bytes(const Dims &d, const TcState &tc, bool use_tc, in
 
 int score_record(const Dims &d, const ConvWeights &cw, const HeadWeights &hw, const TcState &tc, bool use_tc, int num_sms, const void *x,
                  int dtype, int64_t B, int64_t N, int64_t pitch, int64_t stride, int mode, const float *age, int64_t n_age, int apply_sigmoid,
-                 float *out, void *ws, int64_t ws_bytes, cudaStream_t st, const char **err) {
+                 float *out, void *ws, int64_t ws_bytes, cudaStream_t st, const char **err, const float *state_in, float *state_out) {
     RecordPlan p;
     int code;
     if (!record_plan(d, tc, use_tc, B, N, stride, dtype, mode, &p, &code, err)) return code;
     if (pitch < N || pitch < 1) { *err = "pitch must be >= the recording length"; return B2CNN_EINVAL; }
     if (n_age != 1 && n_age != B) { *err = "age must have 1 or B elements"; return B2CNN_EINVAL; }
-    if (p.n_w == 0) return B2CNN_OK;
+    if ((state_in || state_out) && !p.seq) { *err = "an LSTM state needs sequence mode"; return B2CNN_EINVAL; }
+    if (overlap(state_in, state_out, sizeof(float) * kGates * (size_t)B)) { *err = "state_in and state_out overlap"; return B2CNN_EINVAL; }
+    if (p.n_w == 0) {
+        // no window: the state passes through unchanged
+        const size_t bytes = sizeof(float) * (size_t)B * kGates;
+        if (state_out && (state_in ? cudaMemcpyAsync(state_out, state_in, bytes, cudaMemcpyDeviceToDevice, st)
+                                   : cudaMemsetAsync(state_out, 0, bytes, st)) != cudaSuccess) {
+            *err = "copy of the LSTM state"; return B2CNN_ECUDA;
+        }
+        return B2CNN_OK;
+    }
     if (!ws || ws_bytes < (int64_t)p.total || (reinterpret_cast<uintptr_t>(ws) & 255) != 0) {
         *err = "workspace missing, not 256-byte aligned or smaller than b2cnn_record_workspace_bytes()"; return B2CNN_ESTATE;
     }
@@ -263,7 +273,8 @@ int score_record(const Dims &d, const ConvWeights &cw, const HeadWeights &hw, co
     if (cudaGetLastError() != cudaSuccess) { *err = "age launch"; return B2CNN_ECUDA; }
     // ---- projection + head over the B n_w windows
     if (!use_tc) {
-        if (launch_record_head(d, hw, feats, p.Lp, (int)p.n_w, p.step, p.M, ages, p.M, mode, apply_sigmoid, out, gates, partial, st, err) < 0)
+        if (launch_record_head(d, hw, feats, p.Lp, (int)p.n_w, p.step, p.M, ages, p.M, mode, apply_sigmoid, out, gates, partial, st, err,
+                               state_in, state_out) < 0)
             return B2CNN_ECUDA;
         return B2CNN_OK;
     }
@@ -279,7 +290,7 @@ int score_record(const Dims &d, const ConvWeights &cw, const HeadWeights &hw, co
     if (cudaGetLastError() != cudaSuccess) { *err = "projection launch"; return B2CNN_ECUDA; }
     if (p.seq) {
         if (launch_reduce_gates(partial, tc.n_ranges, p.M, hw, gates, st, err) < 0 ||
-            launch_sequence_segments(d, hw, gates, B, p.n_w, ages, p.M, apply_sigmoid, out, st, err) < 0)
+            launch_sequence_segments(d, hw, gates, B, p.n_w, ages, p.M, apply_sigmoid, out, st, err, nullptr, state_in, state_out) < 0)
             return B2CNN_ECUDA;
         return B2CNN_OK;
     }

@@ -619,10 +619,17 @@ int slide_reset(Slide *s, cudaStream_t st, const char **err) {
     return B2CNN_OK;
 }
 
-// a sequence-mode scorer: the LSTM state rows of the k patients whose device indices are idx = 0 (else nothing)
-static int zero_lstm_rows(const Slide &s, const int *idx, int64_t k, cudaStream_t st, const char **err) {
+template <bool kExport>
+__global__ void slide_state_tail_kernel(const float *__restrict__ src, float *__restrict__ dst, const int *__restrict__ idx, int64_t k,
+                                        int64_t ct);
+
+// a sequence-mode scorer: the LSTM state rows of the k patients whose device indices are idx = 0, or = src [k][64]
+// (device) when src is not null (else nothing)
+static int set_lstm_rows(const Slide &s, const int *idx, int64_t k, const float *src, cudaStream_t st, const char **err) {
     if (!s.lstm || k == 0) return B2CNN_OK;
-    slide_zero_rows_kernel<<<(unsigned)((k * kGates + 255) / 256), 256, 0, st>>>(s.lstm, idx, k, kGates);
+    const unsigned blocks = (unsigned)((k * kGates + 255) / 256);
+    if (src) slide_state_tail_kernel<false><<<blocks, 256, 0, st>>>(src, s.lstm, idx, k, kGates);
+    else slide_zero_rows_kernel<<<blocks, 256, 0, st>>>(s.lstm, idx, k, kGates);
     if (cudaGetLastError() != cudaSuccess) { *err = "LSTM state launch"; return B2CNN_ECUDA; }
     return B2CNN_OK;
 }
@@ -891,10 +898,11 @@ int64_t slide_admit_workspace_bytes(const Slide *s, int64_t k, int64_t H) {
 }
 
 int slide_admit(Slide *s, const ConvWeights &cw, const TcState &tc, const int *patients, int64_t k, const void *hist, int64_t H,
-                int64_t pitch, void *ws, int64_t ws_bytes, cudaStream_t st, const char **err) {
+                int64_t pitch, const float *lstm, void *ws, int64_t ws_bytes, cudaStream_t st, const char **err) {
     const Dims &d = s->d;
     int rc = check_patients(*s, patients, k, err);
     if (rc != B2CNN_OK) return rc;
+    if (lstm && s->mode != B2CNN_MODE_SEQUENCE) { *err = "an LSTM state array for an independent-mode scorer"; return B2CNN_EINVAL; }
     if (H < 0 || H > d.W) { *err = "history length must be in [0, window]"; return B2CNN_EINVAL; }
     if (H > 0 && !hist) { *err = "null history with a positive length"; return B2CNN_EINVAL; }
     if (H > 0 && pitch < H) { *err = "history pitch must be >= its length"; return B2CNN_EINVAL; }
@@ -946,7 +954,8 @@ int slide_admit(Slide *s, const ConvWeights &cw, const TcState &tc, const int *p
         slide_seed_tail_kernel<float><<<(unsigned)blocks, 256, 0, st>>>(reinterpret_cast<const float *>(hist), pitch, H, idx, (int)k, d.C,
                                                                         s->T, tail);
     if (cudaGetLastError() != cudaSuccess) { *err = "tail launch"; return B2CNN_ECUDA; }
-    if ((rc = zero_lstm_rows(*s, idx, k, st, err)) != B2CNN_OK) return rc;   // sequence mode: the LSTM starts again
+    // sequence mode: the LSTM starts again, from zero or from the caller's rows
+    if ((rc = set_lstm_rows(*s, idx, k, lstm, st, err)) != B2CNN_OK) return rc;
     std::vector<int64_t> next = next_seen(*s, patients, k, H);
     if ((rc = commit_seen(s, next, st, err)) != B2CNN_OK) return rc;
     // features from the history's last complete one on are seam features of the next push, for every patient (before
@@ -962,7 +971,7 @@ int slide_discharge(Slide *s, const int *patients, int64_t k, cudaStream_t st, c
         if (cudaMemcpyAsync(s->lidx, patients, sizeof(int) * (size_t)k, cudaMemcpyHostToDevice, st) != cudaSuccess) {
             *err = "copy of the patient indices"; return B2CNN_ECUDA;
         }
-        if ((rc = zero_lstm_rows(*s, s->lidx, k, st, err)) != B2CNN_OK) return rc;
+        if ((rc = set_lstm_rows(*s, s->lidx, k, nullptr, st, err)) != B2CNN_OK) return rc;
     }
     std::vector<int64_t> next = next_seen(*s, patients, k, -1);
     return commit_seen(s, next, st, err);
@@ -1174,8 +1183,7 @@ static int launch_state(const Slide &s, const int *patients, int64_t k, const fl
     if constexpr (kExport) {
         if (dst_lstm) slide_state_tail_kernel<true><<<lblocks, 256, 0, st>>>(s.lstm, dst_lstm, idx, k, kGates);
     } else {
-        if (s.lstm && src_lstm) slide_state_tail_kernel<false><<<lblocks, 256, 0, st>>>(src_lstm, s.lstm, idx, k, kGates);
-        else if (zero_lstm_rows(s, idx, k, st, err) != B2CNN_OK) return B2CNN_ECUDA;
+        if (set_lstm_rows(s, idx, k, src_lstm, st, err) != B2CNN_OK) return B2CNN_ECUDA;
     }
     if (cudaGetLastError() != cudaSuccess) { *err = "LSTM state launch"; return B2CNN_ECUDA; }
     return B2CNN_OK;

@@ -40,8 +40,10 @@ int slide_stale_head(const Slide *s, uint64_t digest);
 int slide_features(const Slide *s, float *feats, cudaStream_t st, const char **err);
 // per-patient lifecycle: `patients` host indices; `hist` [k][C][pitch] device samples in the scorer's dtype
 int64_t slide_admit_workspace_bytes(const Slide *s, int64_t k, int64_t H);
+// lstm: nullptr (a sequence-mode scorer's LSTM state rows of the patients are zeroed) or [k][64] device fp32 rows they
+// start from (sequence mode only, else B2CNN_EINVAL)
 int slide_admit(Slide *s, const ConvWeights &cw, const TcState &tc, const int *patients, int64_t k, const void *hist, int64_t H,
-                int64_t pitch, void *ws, int64_t ws_bytes, cudaStream_t st, const char **err);
+                int64_t pitch, const float *lstm, void *ws, int64_t ws_bytes, cudaStream_t st, const char **err);
 int slide_discharge(Slide *s, const int *patients, int64_t k, cudaStream_t st, const char **err);
 int slide_samples_seen(Slide *s, int64_t *out, cudaStream_t st, const char **err);
 int slide_dtype(const Slide *s);

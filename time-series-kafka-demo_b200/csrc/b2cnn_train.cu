@@ -218,18 +218,41 @@ __device__ __forceinline__ bool rec_reads(const RecRows &r, int64_t n, int s) {
     return w >= 0 && s < w * r.S + r.W;
 }
 
+// The LSTM state of each recording of a _record_state call (RecordArgs), [nrec][64] = h0 | c0 | h1 | c1; every pointer
+// null for every other call.  A scan's sequence is a recording with windows, found from its first row in roff.
+struct ScanState {
+    const float *in;
+    float *out;
+    const float *d_out;
+    float *d_in;
+    const int64_t *roff;
+    int64_t nrec;
+};
+// the recording whose rows start at row m: the last b with roff[b] <= m
+__device__ __forceinline__ int64_t scan_recording(const ScanState &ss, int64_t m) {
+    int64_t lo = 0, hi = ss.nrec - 1;
+    while (lo < hi) {
+        const int64_t mid = (lo + hi + 1) >> 1;
+        if (ss.roff[mid] <= m) lo = mid; else hi = mid - 1;
+    }
+    return lo;
+}
+
 // ------------------------------------------------------------------------------------------------------------------
 // LSTM forward over the batch axis with everything the backward pass needs kept; logits and loss.
 // A CTA of 64 threads per group of sequences (SeqSpan): thread r owns gate row r of every matrix; W_ih_l0 f_t was
 // computed before the scan (pre0[t][r]).  sequence == 0: every step starts from the zero state (independent windows).
-// HEAD == kHeadLogits: target and loss_out are not used.
+// A sequence starts from the zero state, or from its recording's row of ss.in, and with ss.out its final state is
+// stored there (STATE == false: ss is ignored, and the kernel compiles to the scan without it).  HEAD == kHeadLogits:
+// target and loss_out are not used.
 // ------------------------------------------------------------------------------------------------------------------
-template <int HEAD>
+template <int HEAD, bool STATE>
 __global__ void __launch_bounds__(64)
 train_lstm_fwd(const float *__restrict__ pre0, const float *__restrict__ prm, BlobOff o, Dims d, int64_t B, int sequence, SeqSpan sq,
                const float *__restrict__ age, const float *__restrict__ target, float pos_weight, float *__restrict__ acts,
                float *__restrict__ cs, float *__restrict__ hs, float *__restrict__ lin, float *__restrict__ z,
-               float *__restrict__ loss_out) {
+               float *__restrict__ loss_out, ScanState ss) {
+    if constexpr (!STATE) ss = ScanState{};
     __shared__ float g[kGates], h0[kHidden], c0[kHidden], h1[kHidden], c1s[kHidden];
     const int r = threadIdx.x;
     // this CTA's sequences [s0, s1); one sequence of all B rows without offsets
@@ -237,7 +260,15 @@ train_lstm_fwd(const float *__restrict__ pre0, const float *__restrict__ prm, Bl
     float loss = 0.f;
     for (int64_t sid = s0; sid < s1; ++sid) {            // the body is the single-sequence scan, over rows [t0, t1)
     const int64_t t0 = sq.off ? sq.off[sid] : 0, t1 = sq.off ? sq.off[sid + 1] : B;
-    if (r < kHidden) { h0[r] = c0[r] = h1[r] = c1s[r] = 0.f; }
+    const int64_t rec = ss.in || ss.out ? scan_recording(ss, t0) : 0;
+    if (r < kHidden) {
+        if (ss.in) {
+            const float *si = ss.in + rec * kGates;
+            h0[r] = si[r]; c0[r] = si[kHidden + r]; h1[r] = si[2 * kHidden + r]; c1s[r] = si[3 * kHidden + r];
+        } else {
+            h0[r] = c0[r] = h1[r] = c1s[r] = 0.f;
+        }
+    }
     __syncthreads();
     for (int64_t t = t0; t < t1; ++t) {
         if (!sequence) {
@@ -307,6 +338,10 @@ train_lstm_fwd(const float *__restrict__ pre0, const float *__restrict__ prm, Bl
         }
         __syncthreads();
     }
+    if (ss.out && r < kHidden) {                          // each thread stores the units it wrote last
+        float *so = ss.out + rec * kGates;
+        so[r] = h0[r]; so[kHidden + r] = c0[r]; so[2 * kHidden + r] = h1[r]; so[3 * kHidden + r] = c1s[r];
+    }
     }
     if (HEAD != kHeadLogits && r == 0) {
         if (sq.rows) sq.rows[blockIdx.x * head_row_len(o) + head_row_len(o) - 1] = loss;
@@ -320,13 +355,18 @@ train_lstm_fwd(const float *__restrict__ pre0, const float *__restrict__ prm, Bl
 // grad, or as the CTA's row of sq.rows); d(gates of layer 0) goes to da0[t][64].
 // HEAD == kHeadLogits: d loss / d z is dz_in[t] and, when dage != NULL, d loss / d age goes to dage[t] (torch's relu
 // backward: zero where relu(age * coef + 1) is not positive); otherwise dz comes from z and target, dage is not written.
+// With ss.in, a sequence's first step reads its recording's initial state (h_{t-1}, c_{t-1}) there instead of zeros;
+// with ss.d_out, the carried d h / d c start from the gradient arriving at the final state instead of zeros; with
+// ss.d_in, the carries after the first step -- d loss / d (initial state) -- are stored there (STATE == false: as for
+// train_lstm_fwd).
 // ------------------------------------------------------------------------------------------------------------------
-template <int HEAD>
+template <int HEAD, bool STATE>
 __global__ void __launch_bounds__(64, 1)   // the 48 gradient sums stay in registers: no spill
 train_lstm_bwd(const float *__restrict__ prm, BlobOff o, Dims d, int64_t B, int sequence, SeqSpan sq, const float *__restrict__ age,
                const float *__restrict__ target, float pos_weight, const float *__restrict__ dz_in, const float *__restrict__ acts,
                const float *__restrict__ cs, const float *__restrict__ hs, const float *__restrict__ lin, const float *__restrict__ z,
-               float *__restrict__ da0, float *__restrict__ grad, float *__restrict__ dage) {
+               float *__restrict__ da0, float *__restrict__ grad, float *__restrict__ dage, ScanState ss) {
+    if constexpr (!STATE) ss = ScanState{};
     __shared__ float da[kGates], dh0c[kHidden], dc0c[kHidden], dh1c[kHidden], dc1c[kHidden], dh0ext[kHidden], dh1ext[kHidden];
     const int r = threadIdx.x, u = r & 15, q = r >> 4;
     // this CTA's sequences [s0, s1), walked last to first; one sequence of all B rows without offsets
@@ -337,14 +377,23 @@ train_lstm_bwd(const float *__restrict__ prm, BlobOff o, Dims d, int64_t B, int 
     float gb0 = 0.f, gb1 = 0.f, gwo = 0.f, gbo = 0.f;
     for (int64_t sid = s1 - 1; sid >= s0; --sid) {       // the body is the single-sequence walk, over rows [t0, t1)
     const int64_t t0 = sq.off ? sq.off[sid] : 0, t1 = sq.off ? sq.off[sid + 1] : B;
-    if (r < kHidden) dh0c[r] = dc0c[r] = dh1c[r] = dc1c[r] = 0.f;
+    const int64_t rec = ss.in || ss.d_out || ss.d_in ? scan_recording(ss, t0) : 0;
+    const float *const sin = ss.in ? ss.in + rec * kGates : nullptr;      // h0 | c0 | h1 | c1 before step t0
+    if (r < kHidden) {
+        if (ss.d_out) {
+            const float *g = ss.d_out + rec * kGates;
+            dh0c[r] = g[r]; dc0c[r] = g[kHidden + r]; dh1c[r] = g[2 * kHidden + r]; dc1c[r] = g[3 * kHidden + r];
+        } else {
+            dh0c[r] = dc0c[r] = dh1c[r] = dc1c[r] = 0.f;
+        }
+    }
     __syncthreads();
     for (int64_t t = t1 - 1; t >= t0; --t) {
         if (!sequence) {
             if (r < kHidden) dh0c[r] = dc0c[r] = dh1c[r] = dc1c[r] = 0.f;
             __syncthreads();
         }
-        const bool first = !sequence || t == t0;              // no previous step: h_{t-1} = c_{t-1} = 0
+        const bool first = !sequence || t == t0;              // no previous step: h_{t-1}, c_{t-1} = 0 or from sin
         // ---- head: z = (wo . h1 + bo) * s
         float s = __fadd_rn(__fmul_rn(age[t], d.age_coef), 1.0f);
         s = (s > 0.f || s != s) ? s : 0.f;
@@ -369,7 +418,7 @@ train_lstm_bwd(const float *__restrict__ prm, BlobOff o, Dims d, int64_t B, int 
         {
             const float *a = acts + (t * 2 + 1) * kGates;
             const float ct = cs[(t * 2 + 1) * kHidden + u];
-            const float cprev = first ? 0.f : cs[((t - 1) * 2 + 1) * kHidden + u];
+            const float cprev = first ? (sin ? sin[3 * kHidden + u] : 0.f) : cs[((t - 1) * 2 + 1) * kHidden + u];
             const float tc = tanhf(ct);
             const float dh = dh1ext[u] + dh1c[u];
             const float dc = dc1c[u] + dh * a[3 * kHidden + u] * (1.f - tc * tc);
@@ -385,7 +434,7 @@ train_lstm_bwd(const float *__restrict__ prm, BlobOff o, Dims d, int64_t B, int 
 #pragma unroll
             for (int k = 0; k < kHidden; ++k) {
                 gWih1[k] += v * hs[(t * 2 + 0) * kHidden + k];                      // layer-1 input = h0_t
-                gWhh1[k] += v * (first ? 0.f : hs[((t - 1) * 2 + 1) * kHidden + k]);  // v * 0: a NaN v still counts
+                gWhh1[k] += v * (first ? (sin ? sin[2 * kHidden + k] : 0.f) : hs[((t - 1) * 2 + 1) * kHidden + k]);  // v * 0: a NaN v still counts
             }
         }
         __syncthreads();
@@ -403,7 +452,7 @@ train_lstm_bwd(const float *__restrict__ prm, BlobOff o, Dims d, int64_t B, int 
         {
             const float *a = acts + (t * 2 + 0) * kGates;
             const float ct = cs[(t * 2 + 0) * kHidden + u];
-            const float cprev = first ? 0.f : cs[((t - 1) * 2 + 0) * kHidden + u];
+            const float cprev = first ? (sin ? sin[kHidden + u] : 0.f) : cs[((t - 1) * 2 + 0) * kHidden + u];
             const float tc = tanhf(ct);
             const float dh = dh0ext[u] + dh0c[u];
             const float dc = dc0c[u] + dh * a[3 * kHidden + u] * (1.f - tc * tc);
@@ -418,7 +467,7 @@ train_lstm_bwd(const float *__restrict__ prm, BlobOff o, Dims d, int64_t B, int 
             if (q == 0) dc0c[u] = dc * a[kHidden + u];
             gb0 += v;
 #pragma unroll
-            for (int k = 0; k < kHidden; ++k) gWhh0[k] += v * (first ? 0.f : hs[((t - 1) * 2 + 0) * kHidden + k]);
+            for (int k = 0; k < kHidden; ++k) gWhh0[k] += v * (first ? (sin ? sin[k] : 0.f) : hs[((t - 1) * 2 + 0) * kHidden + k]);
         }
         __syncthreads();
         if (r < kHidden) {
@@ -427,6 +476,10 @@ train_lstm_bwd(const float *__restrict__ prm, BlobOff o, Dims d, int64_t B, int 
             dh0c[r] = e;
         }
         __syncthreads();
+    }
+    if (ss.d_in && r < kHidden) {                         // the carries after the first step: d (h0, c0, h1, c1)
+        float *g = ss.d_in + rec * kGates;
+        g[r] = dh0c[r]; g[kHidden + r] = dc0c[r]; g[2 * kHidden + r] = dh1c[r]; g[3 * kHidden + r] = dc1c[r];
     }
     }
     // blob entry e of the head goes to grad[e], or to entry e - o.whh0 of this CTA's row
@@ -1039,6 +1092,8 @@ static int train_args(const b2cnn_config *cfg, int64_t B, int mode, const SeqLen
     if (!ptrs_ok || B < 1) { *err = "training: null argument / bad batch"; return B2CNN_EINVAL; }
     if (sl.on && !seq_offsets(sl, B, off, err)) return B2CNN_EINVAL;
     if (ra.on && !record_rows(*cfg, d, B, mode, ra, rec, off, err)) return B2CNN_EINVAL;
+    if (ra.has_state() && (!ra.on || mode != B2CNN_MODE_SEQUENCE)) { *err = "training: an LSTM state needs sequence mode"; return B2CNN_EINVAL; }
+    if (ra.states_overlap(B)) { *err = "training: the LSTM state arrays overlap"; return B2CNN_EINVAL; }
     if (!ra.on) rec.rows = B;
     pl = train_plan(d, rec.rows, off.empty() ? 0 : (int64_t)off.size() - 1, ra.on ? &rec.rd : nullptr, B);
     if (!plan_fits(ra.on ? rec.rd : d, pl, B, err)) return B2CNN_EINVAL;
@@ -1077,6 +1132,30 @@ static bool record_span(const TrainPlan &pl, const Rec &rec, const Dims &d, int6
     if (cudaMemcpyAsync(droff, rec.roff.data(), sizeof(int64_t) * rec.roff.size(), cudaMemcpyHostToDevice, st) != cudaSuccess) return false;
     rr = RecRows{droff, B, (int)rec.S, (int)(rec.S / d.feature_stride()), d.W, d.L, rec.rd.L};
     return true;
+}
+
+// the scan kernels of one HEAD, the STATE instance for a call with states
+template <int HEAD, typename... A>
+static void lstm_fwd(unsigned grid, cudaStream_t st, bool state, A... a) {
+    if (state) train_lstm_fwd<HEAD, true><<<grid, 64, 0, st>>>(a...);
+    else train_lstm_fwd<HEAD, false><<<grid, 64, 0, st>>>(a...);
+}
+template <int HEAD, typename... A>
+static void lstm_bwd(unsigned grid, cudaStream_t st, bool state, A... a) {
+    if (state) train_lstm_bwd<HEAD, true><<<grid, 64, 0, st>>>(a...);
+    else train_lstm_bwd<HEAD, false><<<grid, 64, 0, st>>>(a...);
+}
+
+// The scans' view of a _record_state call's states (all null otherwise).  Before the scan that writes `dst` (state_out in
+// the forward, d_state_in in the backward), dst = src, or zeros for a null src: the rows of recordings without windows
+// keep that value, the scan overwrites the others.
+static ScanState scan_state(const RecordArgs &ra, const RecRows &rr) {
+    return ScanState{ra.state_in, ra.state_out, ra.d_state_out, ra.d_state_in, rr.roff, rr.nrec};
+}
+static bool pass_state(float *dst, const float *src, int64_t B, cudaStream_t st) {
+    if (!dst) return true;
+    const size_t bytes = sizeof(float) * (size_t)B * kGates;
+    return (src ? cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, st) : cudaMemsetAsync(dst, 0, bytes, st)) == cudaSuccess;
 }
 
 // the conv kernels over the windows, or with a _record call over the recordings
@@ -1121,16 +1200,21 @@ int train_step(const b2cnn_config *cfg, float *params, float *adam_m, float *ada
     if (cudaMemsetAsync(grads, 0, sizeof(float) * o.total, st) != cudaSuccess) { *err = "memset grads"; return B2CNN_ECUDA; }
     conv_forward(d, rec, o, pl, ws, params, x, B, mask1, mask2, rr, st);
     const unsigned scans = (unsigned)pl.seq_ctas;
+    // the fused step is truncated back-propagation through time: no gradient enters through the final state
+    const ScanState ss = scan_state(RecordArgs{ra.on, ra.N, ra.S, ra.counts, ra.state_in, ra.state_out}, rr);
+    if (!pass_state(ra.state_out, ra.state_in, B, st)) { *err = "copy of the LSTM state"; return B2CNN_ECUDA; }
+    const bool on = ra.has_state();
+    const float *const nul = nullptr;
     if (weighted) {
-        train_lstm_fwd<kHeadBcePw><<<scans, 64, 0, st>>>(ws + w.pre0, params, o, d, R, sequence, sq, age, target, pos_weight, ws + w.acts,
-                                                         ws + w.cs, ws + w.hs, ws + w.lin, ws + w.z, loss_out);
-        train_lstm_bwd<kHeadBcePw><<<scans, 64, 0, st>>>(params, o, d, R, sequence, sq, age, target, pos_weight, nullptr, ws + w.acts,
-                                                         ws + w.cs, ws + w.hs, ws + w.lin, ws + w.z, ws + w.da0, grads, nullptr);
+        lstm_fwd<kHeadBcePw>(scans, st, on, ws + w.pre0, params, o, d, R, sequence, sq, age, target, pos_weight, ws + w.acts, ws + w.cs,
+                             ws + w.hs, ws + w.lin, ws + w.z, loss_out, ss);
+        lstm_bwd<kHeadBcePw>(scans, st, on, params, o, d, R, sequence, sq, age, target, pos_weight, nul, ws + w.acts, ws + w.cs, ws + w.hs,
+                             ws + w.lin, ws + w.z, ws + w.da0, grads, (float *)nullptr, ss);
     } else {
-        train_lstm_fwd<kHeadBce><<<scans, 64, 0, st>>>(ws + w.pre0, params, o, d, R, sequence, sq, age, target, 1.f, ws + w.acts, ws + w.cs,
-                                                       ws + w.hs, ws + w.lin, ws + w.z, loss_out);
-        train_lstm_bwd<kHeadBce><<<scans, 64, 0, st>>>(params, o, d, R, sequence, sq, age, target, 1.f, nullptr, ws + w.acts, ws + w.cs,
-                                                       ws + w.hs, ws + w.lin, ws + w.z, ws + w.da0, grads, nullptr);
+        lstm_fwd<kHeadBce>(scans, st, on, ws + w.pre0, params, o, d, R, sequence, sq, age, target, 1.f, ws + w.acts, ws + w.cs, ws + w.hs,
+                           ws + w.lin, ws + w.z, loss_out, ss);
+        lstm_bwd<kHeadBce>(scans, st, on, params, o, d, R, sequence, sq, age, target, 1.f, nul, ws + w.acts, ws + w.cs, ws + w.hs,
+                           ws + w.lin, ws + w.z, ws + w.da0, grads, (float *)nullptr, ss);
     }
     launch_head_reduce(pl, o, sq, R, grads, loss_out, st);
     if (!backward_tail(d, rec, o, pl, ws, params, x, B, mask1, mask2, grads, nullptr, false, rr, st)) { *err = "memset dx"; return B2CNN_ECUDA; }
@@ -1163,8 +1247,10 @@ int train_forward(const b2cnn_config *cfg, const float *params, const float *x, 
     RecRows rr;
     if (!record_span(pl, rec, d, B, ws, st, rr)) { *err = "copy row offsets"; return B2CNN_ECUDA; }
     conv_forward(d, rec, o, pl, ws, params, x, B, mask1, mask2, rr, st);
-    train_lstm_fwd<kHeadLogits><<<(unsigned)pl.seq_ctas, 64, 0, st>>>(ws + w.pre0, params, o, d, rec.rows, sequence, sq, age, nullptr, 1.f,
-                                                                     ws + w.acts, ws + w.cs, ws + w.hs, ws + w.lin, z_out, nullptr);
+    if (!pass_state(ra.state_out, ra.state_in, B, st)) { *err = "copy of the LSTM state"; return B2CNN_ECUDA; }
+    lstm_fwd<kHeadLogits>((unsigned)pl.seq_ctas, st, ra.has_state(), ws + w.pre0, params, o, d, rec.rows, sequence, sq, age,
+                          (const float *)nullptr, 1.f, ws + w.acts, ws + w.cs, ws + w.hs, ws + w.lin, z_out, (float *)nullptr,
+                          scan_state(ra, rr));
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) { *err = cudaGetErrorString(e); return B2CNN_ECUDA; }
     return B2CNN_OK;
@@ -1194,8 +1280,10 @@ int train_backward(const b2cnn_config *cfg, const float *params, const float *x,
     if (!record_span(pl, rec, d, B, ws, st, rr)) { *err = "copy row offsets"; return B2CNN_ECUDA; }
     // zeroed: a frozen front end leaves the conv entries as they are
     if (cudaMemsetAsync(grads, 0, sizeof(float) * o.total, st) != cudaSuccess) { *err = "memset grads"; return B2CNN_ECUDA; }
-    train_lstm_bwd<kHeadLogits><<<(unsigned)pl.seq_ctas, 64, 0, st>>>(params, o, d, rec.rows, sequence, sq, age, nullptr, 1.f, dz, ws + w.acts,
-                                                                     ws + w.cs, ws + w.hs, ws + w.lin, nullptr, ws + w.da0, grads, dage);
+    if (!pass_state(ra.d_state_in, ra.d_state_out, B, st)) { *err = "copy of the LSTM state gradient"; return B2CNN_ECUDA; }
+    lstm_bwd<kHeadLogits>((unsigned)pl.seq_ctas, st, ra.has_state(), params, o, d, rec.rows, sequence, sq, age, (const float *)nullptr, 1.f,
+                          dz, ws + w.acts, ws + w.cs, ws + w.hs, ws + w.lin, (const float *)nullptr, ws + w.da0, grads, dage,
+                          scan_state(ra, rr));
     launch_head_reduce(pl, o, sq, rec.rows, grads, nullptr, st);
     if (!backward_tail(d, rec, o, pl, ws, params, x, B, mask1, mask2, grads, dx, frozen_conv, rr, st)) { *err = "memset dx"; return B2CNN_ECUDA; }
     cudaError_t e = cudaGetLastError();

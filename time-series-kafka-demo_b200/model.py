@@ -32,6 +32,28 @@ _PATH_NAMES = {v: k for k, v in _PATHS.items()}
 _PATH_NAMES[3] = "stream"            # B2CNN_PATH_STREAM: fp32 windows through the streaming kernel
 
 
+LSTM_STATE = (2, 2, 16)              # one recording's or patient's LSTM state: [layer][h | c][unit]
+
+
+def check_lstm_state(state, n: int, name: str, what: str) -> None:
+    """ValueError unless ``state`` is a float tensor ``[n, 2, 2, 16]``, indexed [``what``][layer][h | c][unit]."""
+    want = (n,) + LSTM_STATE
+    if not torch.is_tensor(state) or tuple(state.shape) != want or not state.dtype.is_floating_point:
+        got = (tuple(state.shape), state.dtype) if torch.is_tensor(state) else type(state).__name__
+        raise ValueError(f"{name} must be a float tensor {list(want)} ([{what}][layer][h | c][unit]), got {got}")
+
+
+def check_record_state(records: torch.Tensor, mode: str, state=None, return_state: bool = False) -> None:
+    """The LSTM state arguments of a whole-recording call, refused (ValueError) before anything runs: both need mode
+    "sequence", and ``state`` is None or a float tensor ``[B, 2, 2, 16]``."""
+    if not isinstance(return_state, bool):
+        raise ValueError(f"return_state must be True or False, got {type(return_state).__name__}")
+    if (state is not None or return_state) and mode != "sequence":
+        raise ValueError("state and return_state need mode 'sequence': independent windows carry no LSTM state")
+    if state is not None:
+        check_lstm_state(state, records.shape[0], "state", "recording")
+
+
 class B200MyCNN(nn.Module):
     def __init__(self, arch: ArchConfig = ArchConfig(), has_out12: bool = True,
                  device: Optional[torch.device | str] = None, path: str = "auto", tc_splits: int = 3):
@@ -435,7 +457,7 @@ class B200MyCNN(nn.Module):
 
     @torch.no_grad()
     def predict_record(self, records: torch.Tensor, stride: int, age=None, return_prob: bool = False,
-                       path: str = "auto", mode: str = "independent") -> torch.Tensor:
+                       path: str = "auto", mode: str = "independent", state=None, return_state: bool = False):
         """Every window of whole recordings in one call: ``records`` ``[B, C, N]`` (float32 or bfloat16; contiguous or
         a row-padded view), windows of the model's W samples starting every ``stride`` samples.  Returns ``[B, n_w]``,
         ``n_w = (N - W) // stride + 1`` (0 when N < W): element ``[b, w]`` is ``predict(records[b, :, w*stride :
@@ -452,14 +474,29 @@ class B200MyCNN(nn.Module):
         logits are bit-identical to ``predict()`` with ``path="generic"`` and ``small_kernel=0``, per recording with
         ``mode="sequence"`` in sequence mode) or ``"auto"``.  ``stride`` must be a multiple of the feature stride
         ``pool_s ** 2`` (4 on the tensor-core path); it may exceed W.  ``bin/utils.py``'s ``create_batch`` drops the
-        last window when ``(N - W) % stride == 0``: ``out[:, :-1]`` is its set then, in either mode."""
+        last window when ``(N - W) % stride == 0``: ``out[:, :-1]`` is its set then, in either mode.
+
+        State across calls (``mode="sequence"`` only, else ``ValueError``): ``state`` ``[B, 2, 2, 16]``, indexed
+        [recording][layer][h | c][unit] (``SlidingScorer.export()["lstm"]``'s layout; as ``nn.LSTM``'s tuple, ``h =
+        state[:, :, 0].transpose(0, 1)`` and ``c = state[:, :, 1].transpose(0, 1)``, each ``[2, B, 16]``), is the
+        state recording b's scan starts from (None: zeros; other float dtypes and devices are converted to float32 on
+        the model's device).  ``return_state=True`` returns ``(out, state_out)``, ``state_out[b]`` the state after
+        recording b's last window (``state`` itself, or zeros, when n_w = 0).  A recording cut at window k into ``x[...,
+        :(k - 1) * stride + W]`` and ``x[..., k * stride:]``, the first call's ``state_out`` passed to the second, gives
+        the outputs and final state of one call over the recording, bit for bit on both paths."""
         stride, age = self.check_record_args(records, stride, age, path, mode)
+        check_record_state(records, mode, state, return_state)
         B, N, W = records.shape[0], records.shape[2], self.arch.window
         lib, h = self._ensure_handle()
         dev = self._handle_device
+        if state is not None:
+            state = state.detach().to(device=dev, dtype=torch.float32).contiguous()
         n_w = (N - W) // stride + 1 if N >= W else 0
         if n_w == 0:
-            return torch.empty(B, 0, dtype=torch.float32, device=dev)
+            out = torch.empty(B, 0, dtype=torch.float32, device=dev)
+            if not return_state:
+                return out
+            return out, (state.clone() if state is not None else torch.zeros((B,) + LSTM_STATE, dtype=torch.float32, device=dev))
         if records.device != dev:
             records = records.to(dev)
         age = age.to(dev).contiguous()
@@ -478,10 +515,19 @@ class B200MyCNN(nn.Module):
             if need < 0:
                 raise RuntimeError(capi.last_error())
             ws = torch.empty(max(need, 256), dtype=torch.uint8, device=dev)
-            capi.check(lib.b2cnn_score_record_ex(h, records.data_ptr(), dtype, B, N, pitch, stride, _PATHS[path], m, age.data_ptr(),
-                                                 age.numel(), int(return_prob), out.data_ptr(), ws.data_ptr(), ws.numel(),
-                                                 torch.cuda.current_stream().cuda_stream), "b2cnn_score_record_ex")
-        return out
+            st = torch.cuda.current_stream().cuda_stream
+            if state is None and not return_state:
+                capi.check(lib.b2cnn_score_record_ex(h, records.data_ptr(), dtype, B, N, pitch, stride, _PATHS[path], m, age.data_ptr(),
+                                                     age.numel(), int(return_prob), out.data_ptr(), ws.data_ptr(), ws.numel(), st),
+                           "b2cnn_score_record_ex")
+                return out
+            state_out = torch.empty((B,) + LSTM_STATE, dtype=torch.float32, device=dev) if return_state else None
+            capi.check(lib.b2cnn_score_record_state(h, records.data_ptr(), dtype, B, N, pitch, stride, _PATHS[path], m, age.data_ptr(),
+                                                    age.numel(), int(return_prob), out.data_ptr(),
+                                                    None if state is None else state.data_ptr(),
+                                                    None if state_out is None else state_out.data_ptr(), ws.data_ptr(), ws.numel(), st),
+                       "b2cnn_score_record_state")
+        return (out, state_out) if return_state else out
 
     def call_plan(self, window_tensor: torch.Tensor, age: torch.Tensor, mode: str = "independent",
                   return_prob: bool = False):

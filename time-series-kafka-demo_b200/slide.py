@@ -55,6 +55,7 @@ import operator
 import torch
 
 from . import capi
+from .model import check_lstm_state
 
 
 class SlidingScorer:
@@ -346,19 +347,38 @@ class SlidingScorer:
                        "b2cnn_slide_features")
         return feats
 
+    def check_lstm(self, lstm, k: int):
+        """Validates ``admit``'s ``lstm`` for k patients: None, or a float tensor ``[k, 2, 2, 16]`` on a sequence-mode
+        scorer."""
+        if lstm is None:
+            return None
+        if self.mode != "sequence":
+            raise ValueError("lstm is only accepted by a sequence-mode scorer: independent windows carry no LSTM state")
+        check_lstm_state(lstm, k, "lstm", "patient")
+        return lstm
+
     @torch.no_grad()
-    def admit(self, patients, history=None):
+    def admit(self, patients, history=None, lstm=None):
         """Restart the streams of ``patients`` (distinct indices in [0, P)).  ``history``: None, or ``[k, C, H]`` in
         the scorer's dtype with 0 <= H <= W, the samples just before the next push's (a row-padded or unaligned view is
         read in place).  A patient's window after a later push is the last W samples of (history | pushes since
-        admission); it is scored from the push at which ``samples_seen`` reaches W -- with H = W, the next one."""
+        admission); it is scored from the push at which ``samples_seen`` reaches W -- with H = W, the next one.
+
+        ``lstm`` (sequence mode only, else ``ValueError``): ``[k, 2, 2, 16]``, the LSTM state each patient's next step
+        starts from instead of zeros, in ``export()["lstm"]``'s layout (converted to float32 on the scorer's device).
+        The handoff from a backtest of a stay of T >= W samples: ``admit([p], stay[:, :, T - W:T], lstm=st)`` with ``st
+        = model.predict_record(stay[:, :, (T - W) % S:T], S, age, mode="sequence", return_state=True)[1]``; every later
+        push then scores what ``predict_record(mode="sequence")`` gives over the stay and the pushes."""
         idx = self.check_patients(patients)
         k = len(idx)
+        lstm = self.check_lstm(lstm, k)
         H, pitch = 0, 0
         if history is not None:
             pitch = self.check_history(history, k)
             H = int(history.shape[2])
         self._handle()
+        if lstm is not None:
+            lstm = lstm.detach().to(device=self.device, dtype=torch.float32).contiguous()
         if H:
             if history.device != self.device:
                 history = history.to(self.device)
@@ -372,8 +392,12 @@ class SlidingScorer:
                 raise RuntimeError(f"b2cnn_slide_admit_workspace_bytes: invalid arguments (k={k}, H={H})")
             ws = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=self.device)
             st = torch.cuda.current_stream().cuda_stream
-            capi.check(self._lib.b2cnn_slide_admit(self._s, arr, k, history.data_ptr() if H else None, H, pitch, self._dt(),
-                                                   ws.data_ptr(), nbytes, st), "b2cnn_slide_admit")
+            if lstm is None:
+                capi.check(self._lib.b2cnn_slide_admit(self._s, arr, k, history.data_ptr() if H else None, H, pitch, self._dt(),
+                                                       ws.data_ptr(), nbytes, st), "b2cnn_slide_admit")
+            else:
+                capi.check(self._lib.b2cnn_slide_admit_ex(self._s, arr, k, history.data_ptr() if H else None, H, pitch, self._dt(),
+                                                          lstm.data_ptr(), ws.data_ptr(), nbytes, st), "b2cnn_slide_admit_ex")
 
     def discharge(self, patients):
         """Stop scoring ``patients``: their scores and features are NaN, their samples in later pushes ignored, until

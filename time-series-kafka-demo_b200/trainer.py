@@ -34,7 +34,7 @@ import torch
 from . import capi
 from .arch import BLOB_KEYS
 from .autograd import check_masks, check_record_batch, check_trainable, draw_masks, window_ages
-from .model import B200MyCNN
+from .model import B200MyCNN, check_record_state
 
 
 class B200Trainer:
@@ -137,7 +137,8 @@ class B200Trainer:
         return self._finish(update)
 
     def step_record(self, records: torch.Tensor, stride: int, age, target: torch.Tensor, window_counts=None,
-                    masks: Optional[Tuple[Optional[torch.Tensor], Optional[torch.Tensor]]] = None, update: bool = True) -> torch.Tensor:
+                    masks: Optional[Tuple[Optional[torch.Tensor], Optional[torch.Tensor]]] = None, update: bool = True,
+                    state=None, return_state: bool = False):
         """:meth:`step` over every counted window of whole recordings ``[B, C, N]`` (fp32 or bf16), each window feature
         computed and back-propagated once: window w of recording b is ``records[b, :, w*stride : w*stride + W]`` for
         w < ``window_counts[b]`` (default: all n_w = (N - W) // stride + 1; fewer, down to 0, pads a ragged batch to one
@@ -147,9 +148,15 @@ class B200Trainer:
         alone.  The loss is the mean over the M windows.  ``masks``: the recording's dropout masks [B, c_mid, P1(N)] /
         [B, L(N)] (default :meth:`draw_masks` ``(B, N)``); window w uses the slices at its own positions, so a feature
         two windows share is dropped in both or in neither.  Samples no counted window reads (tails, gaps when stride >
-        W, recordings with count 0) change nothing, NaN included."""
+        W, recordings with count 0) change nothing, NaN included.
+
+        Truncated back-propagation through time (sequence mode only, else ValueError): ``state`` ``[B, 2, 2, 16]``
+        ([recording][layer][h | c][unit]; None: zeros) is the LSTM state each recording starts from, and with
+        ``return_state=True`` the call returns ``(loss, state_out)``, ``state_out`` detached: the state after each
+        recording's last counted window (``state[b]`` for a count of 0), to pass to the step on the next chunk."""
         dev = self._params.device
         stride, age, counts, M, rarch = check_record_batch(self.model.arch, records, stride, age, window_counts)
+        check_record_state(records, self.mode, state, return_state)
         B, N = records.shape[0], records.shape[2]
         target = torch.as_tensor(target).detach().to(dev, torch.float32).reshape(-1).contiguous()
         if target.numel() != M:
@@ -166,11 +173,22 @@ class B200Trainer:
         ptr = lambda t: ctypes.c_void_p(t.data_ptr()) if t is not None else None
         pw = None if self.pos_weight is None else ctypes.byref(ctypes.c_float(self.pos_weight))
         st = torch.cuda.current_stream(dev).cuda_stream
-        capi.check(self._lib.b2cnn_train_step_record(ctypes.byref(self._cfg), ptr(self._params), ptr(self._m), ptr(self._v), ptr(self._grads),
-                                                     self.steps + 1, ctypes.byref(self._opt), 1 if update else 0, ptr(records), B, N, stride,
-                                                     counts, mode, ptr(age), ptr(target), pw, ptr(m1), ptr(m2), ptr(self._loss),
-                                                     ptr(self._ws), need, ctypes.c_void_p(st)), "b2cnn_train_step_record")
-        return self._finish(update)
+        if state is None and not return_state:
+            capi.check(self._lib.b2cnn_train_step_record(ctypes.byref(self._cfg), ptr(self._params), ptr(self._m), ptr(self._v),
+                                                         ptr(self._grads), self.steps + 1, ctypes.byref(self._opt), 1 if update else 0,
+                                                         ptr(records), B, N, stride, counts, mode, ptr(age), ptr(target), pw, ptr(m1), ptr(m2),
+                                                         ptr(self._loss), ptr(self._ws), need, ctypes.c_void_p(st)), "b2cnn_train_step_record")
+            return self._finish(update)
+        if state is not None:
+            state = state.detach().to(dev, torch.float32).contiguous()
+        state_out = torch.empty(B, 2, 2, 16, dtype=torch.float32, device=dev)
+        capi.check(self._lib.b2cnn_train_step_record_state(ctypes.byref(self._cfg), ptr(self._params), ptr(self._m), ptr(self._v),
+                                                           ptr(self._grads), self.steps + 1, ctypes.byref(self._opt), 1 if update else 0,
+                                                           ptr(records), B, N, stride, counts, mode, ptr(age), ptr(target), pw, ptr(m1),
+                                                           ptr(m2), ptr(state), ptr(state_out), ptr(self._loss), ptr(self._ws), need,
+                                                           ctypes.c_void_p(st)), "b2cnn_train_step_record_state")
+        loss = self._finish(update)
+        return (loss, state_out) if return_state else loss
 
     def _finish(self, update: bool) -> torch.Tensor:
         if update:
