@@ -390,6 +390,35 @@ int b2cnn_score_record_state(b2cnn_handle *h, const void *x, int dtype, int64_t 
                              int mode, const float *age, int64_t n_age, int apply_sigmoid, float *out, const float *state_in,
                              float *state_out, void *workspace, int64_t workspace_bytes, void *stream);
 
+/* Candidate heads over whole recordings (DESIGN.md §7, backtesting heads): the model and up to B2CNN_SLIDE_MAX_HEADS
+ * handles that share its front end scored over the same recordings, the features computed once.
+ *   b2cnn_score_record_heads  out: DEVICE float [1 + n_heads][B][n_w].  out[0] is exactly what b2cnn_score_record_state
+ *                        (b2cnn_score_record_ex when both states are NULL) writes with the same arguments; out[i] exactly
+ *                        what that call on heads[i - 1] writes -- its own LSTM, Linear and age_coef, the same records,
+ *                        ages, path and mode.  state_in / state_out: NULL or DEVICE float [1 + n_heads][B][64] (the
+ *                        layout above), row i model i's start and final states; sequence mode only, and they must not
+ *                        overlap.  n_heads = 0 is exactly b2cnn_score_record_state (or _ex): the same launches and bits.
+ *                        Every head needs the model's architecture (b2cnn_config apart from age_coef and device), weights
+ *                        set, the model's device and the model's front-end digest (b2cnn_slide_state_header); on the
+ *                        tensor-core path also its packed W_ih chunks in the model's layout (any handle of the model's
+ *                        b2cnn_config has them).  A head may be the model's own handle.  Stage, front end and ages run
+ *                        once; on the tensor-core path the rows' projections run two per launch (the features split once
+ *                        for both), then each row's head.  Nothing allocated, nothing synchronised.
+ *   b2cnn_record_workspace_bytes_heads  DEVICE workspace of that call: b2cnn_record_workspace_bytes_ex's, plus on the
+ *                        tensor-core path one range-partial buffer (4 * n_ranges * B n_w * 64 bytes, rounded up to 256)
+ *                        when n_heads > 0; -1 for bad arguments or n_heads outside [0, B2CNN_SLIDE_MAX_HEADS].
+ * Every check runs before the first launch.  B2CNN_EINVAL: a NULL handle or argument, n_heads outside [0,
+ * B2CNN_SLIDE_MAX_HEADS], a head without weights or on another device, a state outside sequence mode, overlapping states
+ * and every refusal of b2cnn_score_record_ex.  B2CNN_EARCH: a head of another architecture, or without packed W_ih chunks
+ * of the model's layout on the tensor-core path.  B2CNN_ESTATE: a head with other front-end (conv / affine) weights than
+ * the model's (the message names the head), and the workspace refusals of b2cnn_score_record. */
+int64_t b2cnn_record_workspace_bytes_heads(b2cnn_handle *h, int32_t n_heads, int64_t B, int64_t N, int64_t pitch, int64_t stride,
+                                           int dtype, int path, int mode);
+int b2cnn_score_record_heads(b2cnn_handle *h, b2cnn_handle *const *heads, int32_t n_heads, const void *x, int dtype, int64_t B,
+                             int64_t N, int64_t pitch, int64_t stride, int path, int mode, const float *age, int64_t n_age,
+                             int apply_sigmoid, float *out, const float *state_in, float *state_out, void *workspace,
+                             int64_t workspace_bytes, void *stream);
+
 /* Export and import of patients (a restart, beds moved to another scorer or GPU, new LSTM / head weights).  A
  * patient's state is its current window's L features in window order, raw and unmasked (for a complete window
  * bit-identical to its b2cnn_slide_features row), its T-sample tail (the stream's last T samples per channel, fp32;

@@ -40,7 +40,7 @@ SYMBOLS = ("b2cnn_l_out", "b2cnn_weight_count", "b2cnn_create", "b2cnn_destroy",
            "b2cnn_slide_create_ex", "b2cnn_slide_mode", "b2cnn_slide_export_ex", "b2cnn_slide_import_ex",
            "b2cnn_record_workspace_bytes", "b2cnn_score_record", "b2cnn_record_workspace_bytes_ex", "b2cnn_score_record_ex",
            "b2cnn_score_record_state", "b2cnn_slide_admit_ex", "b2cnn_train_step_record_state", "b2cnn_train_forward_record_state",
-           "b2cnn_train_backward_record_state",
+           "b2cnn_train_backward_record_state", "b2cnn_record_workspace_bytes_heads", "b2cnn_score_record_heads",
            "b2cnn_decode_sample_messages", "b2cnn_decode_array_messages", "b2cnn_parse_decimal", "b2cnn_frame_check")
 
 
@@ -183,6 +183,11 @@ def load_library() -> ctypes.CDLL:
     lib.b2cnn_score_record_state.argtypes = [c_vp, c_vp, c_int, c_i64, c_i64, c_i64, c_i64, c_int, c_int, c_vp, c_i64, c_int, c_vp, c_vp,
                                              c_vp, c_vp, c_i64, c_vp]
     lib.b2cnn_score_record_state.restype = c_int
+    lib.b2cnn_record_workspace_bytes_heads.argtypes = [c_vp, c_i32, c_i64, c_i64, c_i64, c_i64, c_int, c_int, c_int]
+    lib.b2cnn_record_workspace_bytes_heads.restype = c_i64
+    lib.b2cnn_score_record_heads.argtypes = [c_vp, c_vp, c_i32, c_vp, c_int, c_i64, c_i64, c_i64, c_i64, c_int, c_int, c_vp, c_i64, c_int,
+                                             c_vp, c_vp, c_vp, c_vp, c_i64, c_vp]
+    lib.b2cnn_score_record_heads.restype = c_int
     lib.b2cnn_slide_admit_ex.argtypes = [c_vp, c_vp, c_i32, c_vp, c_i64, c_i64, c_int, c_vp, c_vp, c_i64, c_vp]
     lib.b2cnn_slide_admit_ex.restype = c_int
     lib.b2cnn_decode_sample_messages.argtypes = [c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_i64, c_i32, c_vp, c_vp]

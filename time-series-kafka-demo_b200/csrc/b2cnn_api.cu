@@ -972,12 +972,12 @@ static int record_path(const char *fn, const b2cnn_handle *h, int dtype, int pat
 }
 
 static int64_t record_workspace(const char *fn, b2cnn_handle *h, int64_t B, int64_t N, int64_t pitch, int64_t stride, int dtype, int path,
-                                int mode) {
+                                int mode, int n_heads = 0) {
     bool tc = false;
     if (record_path(fn, h, dtype, path, &tc) != B2CNN_OK) return -1;
     if (pitch < N) { fail(B2CNN_EINVAL, std::string(fn) + ": pitch must be >= the recording length"); return -1; }
     const char *err = "";
-    const int64_t n = record_workspace_bytes(h->d, h->tc, tc, B, N, stride, dtype, mode, &err);
+    const int64_t n = record_workspace_bytes(h->d, h->tc, tc, B, N, stride, dtype, mode, &err, n_heads);
     if (n < 0) fail(B2CNN_EINVAL, std::string(fn) + ": " + err);
     return n;
 }
@@ -993,14 +993,42 @@ extern "C" int64_t b2cnn_record_workspace_bytes_ex(b2cnn_handle *h, int64_t B, i
 
 static int record_score(const char *fn, b2cnn_handle *h, const void *x, int dtype, int64_t B, int64_t N, int64_t pitch, int64_t stride,
                         int path, int mode, const float *age, int64_t n_age, int apply_sigmoid, float *out, void *workspace,
-                        int64_t workspace_bytes, void *stream, const float *state_in = nullptr, float *state_out = nullptr) {
+                        int64_t workspace_bytes, void *stream, const float *state_in = nullptr, float *state_out = nullptr,
+                        b2cnn_handle *const *heads = nullptr, int32_t n_heads = 0) {
     bool tc = false;
     if (int rc = record_path(fn, h, dtype, path, &tc)) return rc;
     if (!x || !age || !out) return fail(B2CNN_EINVAL, std::string(fn) + ": null argument");
+    std::vector<RecordHead> rh((size_t)n_heads);
+    if (n_heads > 0) {
+        // every head: the model's architecture, device and front-end weights, and on the tensor-core path its packed W_ih
+        // chunks in the model's layout (what b2cnn_slide_set_heads checks)
+        const std::string pre = std::string(fn) + ": ";
+        const b2cnn_config &c = h->cfg;
+        for (int i = 0; i < n_heads; ++i) {
+            const b2cnn_handle *e = heads[i];
+            const std::string which = "head " + std::to_string(i) + ": ";
+            if (!e) return fail(B2CNN_EINVAL, pre + which + "null handle");
+            if (!e->weights_set) return fail(B2CNN_EINVAL, pre + which + "weights not set (call b2cnn_set_weights)");
+            if (e->device != h->device) return fail(B2CNN_EINVAL, pre + which + "on another device than the model");
+            const b2cnn_config &k = e->cfg;
+            if (k.in_channels != c.in_channels || k.k1 != c.k1 || k.c_mid != c.c_mid || k.k2 != c.k2 || k.pool_k != c.pool_k ||
+                k.pool_s != c.pool_s || k.hidden != c.hidden || k.layers != c.layers || k.act != c.act || k.flags != c.flags ||
+                k.window != c.window || k.lstm_input != c.lstm_input)
+                return fail(B2CNN_EARCH, pre + which + "another architecture than the model's (only age_coef may differ)");
+            if (tc && (!e->tc.fused || e->tc.n_ranges != h->tc.n_ranges || e->tc.chunks_per_cta != h->tc.chunks_per_cta))
+                return fail(B2CNN_EARCH, pre + which + "no packed W_ih chunks of the model's layout");
+            rh[i] = RecordHead{&e->hw, &e->tc, e->d.age_coef};
+        }
+        const uint64_t mine = frontend_digest(h->d, h->cw);
+        for (int i = 0; i < n_heads; ++i)
+            if (frontend_digest(heads[i]->d, heads[i]->cw) != mine)
+                return fail(B2CNN_ESTATE, pre + "head " + std::to_string(i) + ": other front-end (conv / affine) weights than the model's");
+    }
     DEVICE_GUARD(h->device);
     const char *err = "";
     const int rc = score_record(h->d, h->cw, h->hw, h->tc, tc, h->num_sms, x, dtype, B, N, pitch, stride, mode, age, n_age, apply_sigmoid,
-                                out, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream), &err, state_in, state_out);
+                                out, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream), &err, state_in, state_out,
+                                rh.data(), n_heads);
     if (rc != B2CNN_OK) return finish(fn, rc, err);
     h->last_path = tc ? B2CNN_PATH_TENSORCORE : B2CNN_PATH_GENERIC;
     return B2CNN_OK;
@@ -1026,6 +1054,28 @@ extern "C" int b2cnn_score_record_state(b2cnn_handle *h, const void *x, int dtyp
     if (mode != B2CNN_MODE_SEQUENCE) return fail(B2CNN_EINVAL, "b2cnn_score_record_state: mode must be B2CNN_MODE_SEQUENCE");
     return record_score("b2cnn_score_record_state", h, x, dtype, B, N, pitch, stride, path, mode, age, n_age, apply_sigmoid, out, workspace,
                         workspace_bytes, stream, state_in, state_out);
+}
+
+extern "C" int64_t b2cnn_record_workspace_bytes_heads(b2cnn_handle *h, int32_t n_heads, int64_t B, int64_t N, int64_t pitch, int64_t stride,
+                                                      int dtype, int path, int mode) {
+    if (n_heads < 0 || n_heads > B2CNN_SLIDE_MAX_HEADS) {
+        fail(B2CNN_EINVAL, "b2cnn_record_workspace_bytes_heads: n_heads must be in [0, " + std::to_string(B2CNN_SLIDE_MAX_HEADS) + "]");
+        return -1;
+    }
+    return record_workspace("b2cnn_record_workspace_bytes_heads", h, B, N, pitch, stride, dtype, path, mode, n_heads);
+}
+
+extern "C" int b2cnn_score_record_heads(b2cnn_handle *h, b2cnn_handle *const *heads, int32_t n_heads, const void *x, int dtype, int64_t B,
+                                        int64_t N, int64_t pitch, int64_t stride, int path, int mode, const float *age, int64_t n_age,
+                                        int apply_sigmoid, float *out, const float *state_in, float *state_out, void *workspace,
+                                        int64_t workspace_bytes, void *stream) {
+    const char *fn = "b2cnn_score_record_heads";
+    if (!h) return fail(B2CNN_EINVAL, std::string(fn) + ": null argument");
+    if (n_heads < 0 || n_heads > B2CNN_SLIDE_MAX_HEADS)
+        return fail(B2CNN_EINVAL, std::string(fn) + ": n_heads must be in [0, " + std::to_string(B2CNN_SLIDE_MAX_HEADS) + "]");
+    if (n_heads > 0 && !heads) return fail(B2CNN_EINVAL, std::string(fn) + ": null argument");
+    return record_score(fn, h, x, dtype, B, N, pitch, stride, path, mode, age, n_age, apply_sigmoid, out, workspace, workspace_bytes, stream,
+                        state_in, state_out, heads, n_heads);
 }
 
 // ---- host-pointer entry: chunked H2D overlapped with compute -----------------------------

@@ -334,4 +334,8 @@ int train_backward(const b2cnn_config *cfg, const float *params, const float *x,
 
 void launch_transpose_wih(const float *wih0, float *wih0T, int L, cudaStream_t st);
 
+// 64-bit FNV-1a over what the features depend on: the front-end geometry and the used conv weights (affine when on);
+// b2cnn_slide_state_header's frontend_digest (b2cnn_slide.cu)
+uint64_t frontend_digest(const Dims &d, const ConvWeights &cw);
+
 }  // namespace b2cnn

@@ -74,11 +74,21 @@ __device__ __forceinline__ void rp_store_partial(float *part, int range, int n_r
 // recording, or from state_in[b] when state_in is not null; state_out[b] receives recording b's state after its last
 // window, state_in[b] (or zeros) when it has none).  state_in / state_out: device [B][64] = h0 | c0 | h1 | c1, null
 // or sequence mode only (else B2CNN_EINVAL).
+// Candidate heads (b2cnn_score_record_heads): rows 1 .. n_heads of out [1 + n_heads][B][n_w] and of the states [1 +
+// n_heads][B][64] are those of heads[i - 1] -- its LSTM / Linear weights, packed W_ih chunks (tensor-core path; the
+// model's n_ranges and chunks_per_cta) and age_coef over the model's features (the caller has checked that every head
+// has the model's architecture and front-end weights).  Row 0 is the call without heads.  n_heads > 0 adds one range
+// partial buffer to the tensor-core workspace.
+struct RecordHead {
+    const HeadWeights *hw;
+    const TcState *tc;
+    float age_coef;
+};
 int64_t record_workspace_bytes(const Dims &d, const TcState &tc, bool use_tc, int64_t B, int64_t N, int64_t stride, int dtype, int mode,
-                               const char **err);
+                               const char **err, int n_heads = 0);
 int score_record(const Dims &d, const ConvWeights &cw, const HeadWeights &hw, const TcState &tc, bool use_tc, int num_sms, const void *x,
                  int dtype, int64_t B, int64_t N, int64_t pitch, int64_t stride, int mode, const float *age, int64_t n_age, int apply_sigmoid,
                  float *out, void *ws, int64_t ws_bytes, cudaStream_t st, const char **err, const float *state_in = nullptr,
-                 float *state_out = nullptr);
+                 float *state_out = nullptr, const RecordHead *heads = nullptr, int n_heads = 0);
 
 }  // namespace b2cnn

@@ -2,6 +2,7 @@
 // call, each window feature computed once.  Stateless: a call on a handle, no scorer involved.
 #include <algorithm>
 #include <cstring>
+#include <type_traits>
 
 #include "b2cnn_proj_tc.cuh"
 
@@ -27,18 +28,23 @@ namespace b2cnn {
 // Launches per call: stage, tensor-core front end, flag compaction, exact re-computation, age, projection, head
 // (tensor-core path, plus the flag memset; reduction + scan in sequence mode) or stage, front end, age, projection,
 // reduction, head (generic path) -- whatever B, N and S.
+//   * heads (b2cnn_score_record_heads): rows 0 (the model) .. K (candidate heads of the same front end) share stage,
+//     front end, flags and age.  Tensor-core path: the rows run in pairs, one HP = 2 projection per pair into the two
+//     partial buffers (each row's partials those of its model's own call), then each row's head on its buffer with its
+//     own HeadWeights and age_coef, before the next pair reuses the buffers; an odd last row runs the HP = 1 kernel
+//     alone.  Generic path: launch_record_head per row on the one partial / gates buffer.
 constexpr int64_t kRecRowFeats = 4096;
 
 struct RecordPlan {
     bool tc, seq;
     int F, R, ranges;
     int64_t n_w, L_N, K, nr, rows, Lp, row_len, Kp, step, M;
-    size_t stage, feats, flags, partial, gates, age, total;
+    size_t stage, feats, flags, partial, gates, age, partial2, total;   // partial2: the second row of a pair (heads)
 };
 
 // the plan of a call; false with *err and *code when an argument is out of range
 static bool record_plan(const Dims &d, const TcState &tc, bool use_tc, int64_t B, int64_t N, int64_t stride, int dtype, int mode,
-                        RecordPlan *o, int *code, const char **err) {
+                        int n_heads, RecordPlan *o, int *code, const char **err) {
     RecordPlan &p = *o;
     memset(&p, 0, sizeof p);
     p.tc = use_tc;
@@ -84,7 +90,8 @@ static bool record_plan(const Dims &d, const TcState &tc, bool use_tc, int64_t B
     p.partial = al256(sizeof(float) * (size_t)p.ranges * (size_t)p.M * kGates);
     p.gates = use_tc && !p.seq ? 0 : al256(sizeof(float) * (size_t)p.M * kGates);   // the fused tensor-core head sums in registers
     p.age = al256(sizeof(float) * (size_t)p.M);
-    p.total = p.stage + p.feats + p.flags + p.partial + p.gates + p.age;
+    p.partial2 = use_tc && n_heads > 0 ? p.partial : 0;
+    p.total = p.stage + p.feats + p.flags + p.partial + p.gates + p.age + p.partial2;
     *code = B2CNN_OK;
     return true;
 }
@@ -129,13 +136,38 @@ struct RecordProjParams {
     int64_t rec_pitch, step;         // recording pitch and window step in features
     int M, n_w, L, feats_per_cta, chunks_per_cta, foff;
 };
-constexpr size_t kRecProjSmem = 1024 + 2 * kRpWChunk + 3 * kRpPiece + 64;
+// Two rows of a call with heads (score_record with n_heads > 0) per CTA: p's wpack / partial are the first row's, these
+// the second's.  HP: rows per CTA, each with its own W_ih chunk slot per stage and its own accumulators.
+struct RecordProjPair {
+    RecordProjParams p;
+    const uint8_t *wpack1;
+    float *partial1;
+};
+template <int HP>
+using RecordProjArgs = std::conditional_t<HP == 1, RecordProjParams, RecordProjPair>;
+__device__ __forceinline__ const RecordProjParams &rec_base(const RecordProjParams &a) { return a; }
+__device__ __forceinline__ const RecordProjParams &rec_base(const RecordProjPair &a) { return a.p; }
+template <int HP>
+constexpr size_t kRecProjSmemHP = 1024 + 2 * HP * kRpWChunk + 3 * kRpPiece + 64;
 
-__global__ void __launch_bounds__(kRpThreads) slide_record_proj_kernel(const __grid_constant__ RecordProjParams p) {
+// Per row the instructions are those of HP = 1: the A pieces split once from the window's features serve both rows,
+// and each row gets the same 12 MMAs per chunk in the same chunk order -- so each row's partials are bit-identical to
+// those of its model's own call.
+template <int HP>
+__global__ void __launch_bounds__(kRpThreads) slide_record_proj_kernel(const __grid_constant__ RecordProjArgs<HP> args) {
+    const RecordProjParams &p = rec_base(args);
+    auto wpack_of = [&](int j) {
+        if constexpr (HP == 1) return p.wpack;
+        else return j == 0 ? p.wpack : args.wpack1;
+    };
+    auto partial_of = [&](int j) {
+        if constexpr (HP == 1) return p.partial;
+        else return j == 0 ? p.partial : args.partial1;
+    };
     extern __shared__ uint8_t smem_raw[];
     uint8_t *smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-    uint8_t *sW = smem;                                            // [2 stages][6 KB]
-    uint8_t *sPc = sW + 2 * kRpWChunk;                             // [3 pieces][4 KB]
+    uint8_t *sW = smem;                                            // [2 stages][HP][6 KB]
+    uint8_t *sPc = sW + 2 * HP * kRpWChunk;                        // [3 pieces][4 KB]
     uint64_t *bars = reinterpret_cast<uint64_t *>(sPc + 3 * kRpPiece);
     const uint32_t bar_full = smem_u32(bars + 0), bar_empty = smem_u32(bars + 2);
     const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);
@@ -153,8 +185,11 @@ __global__ void __launch_bounds__(kRpThreads) slide_record_proj_kernel(const __g
             for (int m = 0; m < nch; ++m) {
                 const int u = m & 1;
                 mbar_wait(bar_empty + 8 * u, ((m >> 1) & 1) ^ 1);
-                mbar_expect_tx(bar_full + 8 * u, kRpWChunk);
-                bulk_load_1d(smem_u32(sW + u * kRpWChunk), p.wpack + ((size_t)blockIdx.y * nch + m) * kRpWChunk, kRpWChunk, bar_full + 8 * u);
+                mbar_expect_tx(bar_full + 8 * u, HP * kRpWChunk);
+#pragma unroll
+                for (int j = 0; j < HP; ++j)
+                    bulk_load_1d(smem_u32(sW + (u * HP + j) * kRpWChunk), wpack_of(j) + ((size_t)blockIdx.y * nch + m) * kRpWChunk,
+                                 kRpWChunk, bar_full + 8 * u);
             }
         }
         return;
@@ -166,11 +201,13 @@ __global__ void __launch_bounds__(kRpThreads) slide_record_proj_kernel(const __g
         const int r = b / p.n_w;
         fr += (int64_t)r * p.rec_pitch + (int64_t)(b - r * p.n_w) * p.step;
     }
-    float gacc[2][32];
+    float gacc[HP][2][32];
 #pragma unroll
-    for (int h = 0; h < 2; ++h)
+    for (int j = 0; j < HP; ++j)
 #pragma unroll
-        for (int i = 0; i < 32; ++i) gacc[h][i] = 0.f;
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int i = 0; i < 32; ++i) gacc[j][h][i] = 0.f;
     uint8_t *arow = sPc + (row >> 3) * 256 + (row & 7) * 16;
     float v[16];
     auto load = [&](int m) {
@@ -190,7 +227,8 @@ __global__ void __launch_bounds__(kRpThreads) slide_record_proj_kernel(const __g
         wg_bar();
         mbar_wait(bar_full + 8 * u, (m >> 1) & 1);
         wgmma_fence();
-        rp_mma_chunk(gacc, smem_u32(sPc), smem_u32(sW + u * kRpWChunk));
+#pragma unroll
+        for (int j = 0; j < HP; ++j) rp_mma_chunk(gacc[j], smem_u32(sPc), smem_u32(sW + (u * HP + j) * kRpWChunk));
         wgmma_commit();
         if (m + 1 < nch) load(m + 1);                              // in flight during the MMAs
         wgmma_wait<0>();
@@ -198,30 +236,33 @@ __global__ void __launch_bounds__(kRpThreads) slide_record_proj_kernel(const __g
         if (lane == 0) mbar_arrive(bar_empty + 8 * u);
         wg_bar();                                                  // A tile free for the next chunk
     }
-    rp_store_partial(p.partial, blockIdx.y, p.M, b0, warp, lane, gacc);
+#pragma unroll
+    for (int j = 0; j < HP; ++j) rp_store_partial(partial_of(j), blockIdx.y, p.M, b0, warp, lane, gacc[j]);
 }
 
 int64_t record_workspace_bytes(const Dims &d, const TcState &tc, bool use_tc, int64_t B, int64_t N, int64_t stride, int dtype, int mode,
-                               const char **err) {
+                               const char **err, int n_heads) {
     RecordPlan p;
     int code;
-    if (!record_plan(d, tc, use_tc, B, N, stride, dtype, mode, &p, &code, err)) return -1;
+    if (!record_plan(d, tc, use_tc, B, N, stride, dtype, mode, n_heads, &p, &code, err)) return -1;
     return (int64_t)p.total;
 }
 
 int score_record(const Dims &d, const ConvWeights &cw, const HeadWeights &hw, const TcState &tc, bool use_tc, int num_sms, const void *x,
                  int dtype, int64_t B, int64_t N, int64_t pitch, int64_t stride, int mode, const float *age, int64_t n_age, int apply_sigmoid,
-                 float *out, void *ws, int64_t ws_bytes, cudaStream_t st, const char **err, const float *state_in, float *state_out) {
+                 float *out, void *ws, int64_t ws_bytes, cudaStream_t st, const char **err, const float *state_in, float *state_out,
+                 const RecordHead *heads, int n_heads) {
     RecordPlan p;
     int code;
-    if (!record_plan(d, tc, use_tc, B, N, stride, dtype, mode, &p, &code, err)) return code;
+    if (!record_plan(d, tc, use_tc, B, N, stride, dtype, mode, n_heads, &p, &code, err)) return code;
+    const int rows = 1 + n_heads;                                  // output rows: the model's, then each head's
     if (pitch < N || pitch < 1) { *err = "pitch must be >= the recording length"; return B2CNN_EINVAL; }
     if (n_age != 1 && n_age != B) { *err = "age must have 1 or B elements"; return B2CNN_EINVAL; }
     if ((state_in || state_out) && !p.seq) { *err = "an LSTM state needs sequence mode"; return B2CNN_EINVAL; }
-    if (overlap(state_in, state_out, sizeof(float) * kGates * (size_t)B)) { *err = "state_in and state_out overlap"; return B2CNN_EINVAL; }
+    if (overlap(state_in, state_out, sizeof(float) * kGates * (size_t)B * rows)) { *err = "state_in and state_out overlap"; return B2CNN_EINVAL; }
     if (p.n_w == 0) {
         // no window: the state passes through unchanged
-        const size_t bytes = sizeof(float) * (size_t)B * kGates;
+        const size_t bytes = sizeof(float) * (size_t)B * kGates * rows;
         if (state_out && (state_in ? cudaMemcpyAsync(state_out, state_in, bytes, cudaMemcpyDeviceToDevice, st)
                                    : cudaMemsetAsync(state_out, 0, bytes, st)) != cudaSuccess) {
             *err = "copy of the LSTM state"; return B2CNN_ECUDA;
@@ -244,6 +285,15 @@ int score_record(const Dims &d, const ConvWeights &cw, const HeadWeights &hw, co
     float *partial = reinterpret_cast<float *>(base + p.stage + p.feats + p.flags);
     float *gates = reinterpret_cast<float *>(base + p.stage + p.feats + p.flags + p.partial);
     float *ages = reinterpret_cast<float *>(base + p.stage + p.feats + p.flags + p.partial + p.gates);
+    float *partial2 = reinterpret_cast<float *>(base + p.stage + p.feats + p.flags + p.partial + p.gates + p.age);
+    // row r: its head weights, packed W_ih chunks, geometry with its age_coef, and its slices of out and the states
+    struct Row { const HeadWeights *hw; const TcState *tc; Dims d; float *out; const float *state_in; float *state_out; };
+    auto row_of = [&](int r) {
+        Row w{r == 0 ? &hw : heads[r - 1].hw, r == 0 ? &tc : heads[r - 1].tc, d, out + (size_t)r * p.M,
+              state_in ? state_in + (size_t)r * B * kGates : nullptr, state_out ? state_out + (size_t)r * B * kGates : nullptr};
+        if (r > 0) w.d.age_coef = heads[r - 1].age_coef;
+        return w;
+    };
     // ---- fold: staging rows
     {
         const int64_t rc = p.rows * d.C;
@@ -273,9 +323,12 @@ int score_record(const Dims &d, const ConvWeights &cw, const HeadWeights &hw, co
     if (cudaGetLastError() != cudaSuccess) { *err = "age launch"; return B2CNN_ECUDA; }
     // ---- projection + head over the B n_w windows
     if (!use_tc) {
-        if (launch_record_head(d, hw, feats, p.Lp, (int)p.n_w, p.step, p.M, ages, p.M, mode, apply_sigmoid, out, gates, partial, st, err,
-                               state_in, state_out) < 0)
-            return B2CNN_ECUDA;
+        for (int r = 0; r < rows; ++r) {
+            const Row w = row_of(r);
+            if (launch_record_head(w.d, *w.hw, feats, p.Lp, (int)p.n_w, p.step, p.M, ages, p.M, mode, apply_sigmoid, w.out, gates, partial, st,
+                                   err, w.state_in, w.state_out) < 0)
+                return B2CNN_ECUDA;
+        }
         return B2CNN_OK;
     }
     RecordProjParams rp;
@@ -283,18 +336,41 @@ int score_record(const Dims &d, const ConvWeights &cw, const HeadWeights &hw, co
     rp.rec_pitch = p.Lp; rp.step = p.step;
     rp.M = (int)p.M; rp.n_w = (int)p.n_w; rp.L = d.L;
     rp.feats_per_cta = tc.feats_per_cta; rp.chunks_per_cta = tc.chunks_per_cta; rp.foff = d.K1 == 10 ? 3 : 2;
-    if (cudaFuncSetAttribute(slide_record_proj_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kRecProjSmem) != cudaSuccess) {
-        *err = "projection smem attribute"; return B2CNN_ECUDA;
+    const dim3 grid((unsigned)((p.M + kRpM - 1) / kRpM), (unsigned)tc.n_ranges);
+    // one row's head over its range partials
+    auto head = [&](const Row &w, const float *part) {
+        if (p.seq)
+            return launch_reduce_gates(part, tc.n_ranges, p.M, *w.hw, gates, st, err) < 0 ||
+                           launch_sequence_segments(w.d, *w.hw, gates, B, p.n_w, ages, p.M, apply_sigmoid, w.out, st, err, nullptr,
+                                                    w.state_in, w.state_out) < 0
+                       ? B2CNN_ECUDA : B2CNN_OK;
+        return launch_reduce_lstm_head(w.d, *w.hw, part, tc.n_ranges, p.M, ages, p.M, apply_sigmoid, w.out, st, err) < 0 ? B2CNN_ECUDA
+                                                                                                                         : B2CNN_OK;
+    };
+    for (int r = 0; r < rows; r += 2) {
+        const Row w0 = row_of(r);
+        rp.wpack = reinterpret_cast<const uint8_t *>(w0.tc->d_wpack);
+        if (r + 1 < rows) {
+            const Row w1 = row_of(r + 1);
+            const RecordProjPair pair{rp, reinterpret_cast<const uint8_t *>(w1.tc->d_wpack), partial2};
+            if (cudaFuncSetAttribute(slide_record_proj_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kRecProjSmemHP<2>) !=
+                cudaSuccess) {
+                *err = "projection smem attribute"; return B2CNN_ECUDA;
+            }
+            slide_record_proj_kernel<2><<<grid, kRpThreads, kRecProjSmemHP<2>, st>>>(pair);
+            if (cudaGetLastError() != cudaSuccess) { *err = "projection launch"; return B2CNN_ECUDA; }
+            if (int rc = head(w0, partial)) return rc;
+            if (int rc = head(w1, partial2)) return rc;
+            continue;
+        }
+        if (cudaFuncSetAttribute(slide_record_proj_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kRecProjSmemHP<1>) !=
+            cudaSuccess) {
+            *err = "projection smem attribute"; return B2CNN_ECUDA;
+        }
+        slide_record_proj_kernel<1><<<grid, kRpThreads, kRecProjSmemHP<1>, st>>>(rp);
+        if (cudaGetLastError() != cudaSuccess) { *err = "projection launch"; return B2CNN_ECUDA; }
+        if (int rc = head(w0, partial)) return rc;
     }
-    slide_record_proj_kernel<<<dim3((unsigned)((p.M + kRpM - 1) / kRpM), (unsigned)tc.n_ranges), kRpThreads, kRecProjSmem, st>>>(rp);
-    if (cudaGetLastError() != cudaSuccess) { *err = "projection launch"; return B2CNN_ECUDA; }
-    if (p.seq) {
-        if (launch_reduce_gates(partial, tc.n_ranges, p.M, hw, gates, st, err) < 0 ||
-            launch_sequence_segments(d, hw, gates, B, p.n_w, ages, p.M, apply_sigmoid, out, st, err, nullptr, state_in, state_out) < 0)
-            return B2CNN_ECUDA;
-        return B2CNN_OK;
-    }
-    if (launch_reduce_lstm_head(d, hw, partial, tc.n_ranges, p.M, ages, p.M, apply_sigmoid, out, st, err) < 0) return B2CNN_ECUDA;
     return B2CNN_OK;
 }
 

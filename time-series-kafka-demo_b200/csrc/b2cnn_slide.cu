@@ -1051,8 +1051,7 @@ static uint64_t fnv1a(uint64_t h, const void *p, size_t n) {
     return h;
 }
 
-// FNV-1a over what the features depend on: the front-end geometry and the used conv weights (affine when on)
-static uint64_t frontend_digest(const Dims &d, const ConvWeights &cw) {
+uint64_t frontend_digest(const Dims &d, const ConvWeights &cw) {
     const int32_t geo[7] = {d.C, d.K1, d.K2, d.PK, d.PS, d.act, d.has_affine};
     uint64_t h = fnv1a(0xcbf29ce484222325ull, geo, sizeof geo);
     h = fnv1a(h, cw.w1, sizeof(float) * (size_t)d.C * d.K1 * kCMid);

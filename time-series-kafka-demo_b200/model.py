@@ -35,23 +35,56 @@ _PATH_NAMES[3] = "stream"            # B2CNN_PATH_STREAM: fp32 windows through t
 LSTM_STATE = (2, 2, 16)              # one recording's or patient's LSTM state: [layer][h | c][unit]
 
 
-def check_lstm_state(state, n: int, name: str, what: str) -> None:
-    """ValueError unless ``state`` is a float tensor ``[n, 2, 2, 16]``, indexed [``what``][layer][h | c][unit]."""
-    want = (n,) + LSTM_STATE
+def check_lstm_state(state, n, name: str, what: str) -> None:
+    """ValueError unless ``state`` is a float tensor ``[n, 2, 2, 16]`` (``[*n, 2, 2, 16]`` for a tuple ``n``), indexed
+    [``what``][layer][h | c][unit]."""
+    want = (tuple(n) if isinstance(n, tuple) else (n,)) + LSTM_STATE
     if not torch.is_tensor(state) or tuple(state.shape) != want or not state.dtype.is_floating_point:
         got = (tuple(state.shape), state.dtype) if torch.is_tensor(state) else type(state).__name__
         raise ValueError(f"{name} must be a float tensor {list(want)} ([{what}][layer][h | c][unit]), got {got}")
 
 
-def check_record_state(records: torch.Tensor, mode: str, state=None, return_state: bool = False) -> None:
+def check_record_state(records: torch.Tensor, mode: str, state=None, return_state: bool = False, n_models=None) -> None:
     """The LSTM state arguments of a whole-recording call, refused (ValueError) before anything runs: both need mode
-    "sequence", and ``state`` is None or a float tensor ``[B, 2, 2, 16]``."""
+    "sequence", and ``state`` is None or a float tensor ``[B, 2, 2, 16]`` (``[n_models, B, 2, 2, 16]`` when
+    ``n_models`` is given: a call with heads)."""
     if not isinstance(return_state, bool):
         raise ValueError(f"return_state must be True or False, got {type(return_state).__name__}")
     if (state is not None or return_state) and mode != "sequence":
         raise ValueError("state and return_state need mode 'sequence': independent windows carry no LSTM state")
     if state is not None:
-        check_lstm_state(state, records.shape[0], "state", "recording")
+        if n_models is None:
+            check_lstm_state(state, records.shape[0], "state", "recording")
+        else:
+            check_lstm_state(state, (n_models, records.shape[0]), "state", "model][recording")
+
+
+# the ArchConfig fields a head must share with the model it is scored beside (age_coef may differ)
+HEAD_ARCH_FIELDS = ("in_channels", "window", "k1", "k2", "pool_k", "pool_s", "act", "affine", "l_out", "c_mid", "hidden", "layers")
+
+
+def check_head_models(models, arch, device, caller: str, model_name: str, owner: str, fields=HEAD_ARCH_FIELDS,
+                      extra=None) -> tuple:
+    """Extra heads (``SlidingScorer.set_heads``, ``B200MyCNN.predict_record``) validated without touching the library:
+    a list of at most 8 ``B200MyCNN`` models (TypeError otherwise) whose ``fields`` equal ``arch``'s and which live on
+    ``device`` (ValueError otherwise).  ``model_name`` and ``owner`` name what they are scored beside in the messages;
+    ``extra(i, model)`` adds a check before the device's.  Returns the models as a tuple."""
+    if isinstance(models, (B200MyCNN, torch.Tensor, str, bytes)) or not hasattr(models, "__iter__"):
+        raise TypeError(f"{caller} takes a list of B200MyCNN models")
+    models = tuple(models)
+    if len(models) > capi.SLIDE_MAX_HEADS:
+        raise ValueError(f"at most {capi.SLIDE_MAX_HEADS} heads, got {len(models)}")
+    for i, m in enumerate(models):
+        if not isinstance(m, B200MyCNN):
+            raise TypeError(f"heads[{i}] is a {type(m).__name__}, not a B200MyCNN")
+        bad = [f for f in fields if getattr(m.arch, f) != getattr(arch, f)]
+        if bad:
+            raise ValueError(f"heads[{i}] differs from {model_name} in {', '.join(bad)}")
+        if extra is not None:
+            extra(i, m)
+        if m._device() != device:
+            raise ValueError(f"heads[{i}] is on {m._device()}, {owner} on {device}")
+    return models
 
 
 class B200MyCNN(nn.Module):
@@ -457,7 +490,7 @@ class B200MyCNN(nn.Module):
 
     @torch.no_grad()
     def predict_record(self, records: torch.Tensor, stride: int, age=None, return_prob: bool = False,
-                       path: str = "auto", mode: str = "independent", state=None, return_state: bool = False):
+                       path: str = "auto", mode: str = "independent", state=None, return_state: bool = False, heads=None):
         """Every window of whole recordings in one call: ``records`` ``[B, C, N]`` (float32 or bfloat16; contiguous or
         a row-padded view), windows of the model's W samples starting every ``stride`` samples.  Returns ``[B, n_w]``,
         ``n_w = (N - W) // stride + 1`` (0 when N < W): element ``[b, w]`` is ``predict(records[b, :, w*stride :
@@ -483,8 +516,20 @@ class B200MyCNN(nn.Module):
         the model's device).  ``return_state=True`` returns ``(out, state_out)``, ``state_out[b]`` the state after
         recording b's last window (``state`` itself, or zeros, when n_w = 0).  A recording cut at window k into ``x[...,
         :(k - 1) * stride + W]`` and ``x[..., k * stride:]``, the first call's ``state_out`` passed to the second, gives
-        the outputs and final state of one call over the recording, bit for bit on both paths."""
+        the outputs and final state of one call over the recording, bit for bit on both paths.
+
+        Candidate heads (backtesting retrained heads before ``SlidingScorer.set_heads``): ``heads=[m1, ..., mK]``, K <=
+        8 models with this model's architecture (``age_coef`` may differ), conv / affine weights and device, returns
+        ``out`` ``[1 + K, B, n_w]``: ``out[0]`` is this call without heads and ``out[i]`` is exactly
+        ``heads[i - 1].predict_record(records, stride, age, ...)`` with the same arguments, bit for bit and NaN for NaN
+        -- each head's own LSTM, Linear and ``age_coef`` over features computed once.  With heads, ``state`` and
+        ``state_out`` are ``[1 + K, B, 2, 2, 16]``, row i model i's.  ``heads=None`` or ``[]`` is the call without."""
         stride, age = self.check_record_args(records, stride, age, path, mode)
+        if heads is not None:
+            heads = check_head_models(heads, self.arch, self._device(), "predict_record", "the model", "the model")
+        if heads:
+            check_record_state(records, mode, state, return_state, 1 + len(heads))
+            return self._predict_record_heads(records, stride, age, return_prob, path, mode, state, return_state, heads)
         check_record_state(records, mode, state, return_state)
         B, N, W = records.shape[0], records.shape[2], self.arch.window
         lib, h = self._ensure_handle()
@@ -497,16 +542,8 @@ class B200MyCNN(nn.Module):
             if not return_state:
                 return out
             return out, (state.clone() if state is not None else torch.zeros((B,) + LSTM_STATE, dtype=torch.float32, device=dev))
-        if records.device != dev:
-            records = records.to(dev)
+        records, pitch = self._record_pitch(records)
         age = age.to(dev).contiguous()
-        C = self.arch.in_channels
-        if records.is_contiguous():
-            pitch = N
-        elif records.stride(2) == 1 and records.stride(1) >= N and (B == 1 or records.stride(0) == C * records.stride(1)):
-            pitch = records.stride(1)                            # a row-padded view, read in place
-        else:
-            records, pitch = records.contiguous(), N
         dtype = capi.DTYPE_BF16 if records.dtype == torch.bfloat16 else capi.DTYPE_F32
         out = torch.empty(B, n_w, dtype=torch.float32, device=dev)
         m = capi.MODE_SEQUENCE if mode == "sequence" else capi.MODE_INDEPENDENT
@@ -527,6 +564,52 @@ class B200MyCNN(nn.Module):
                                                     None if state is None else state.data_ptr(),
                                                     None if state_out is None else state_out.data_ptr(), ws.data_ptr(), ws.numel(), st),
                        "b2cnn_score_record_state")
+        return (out, state_out) if return_state else out
+
+    def _record_pitch(self, records: torch.Tensor):
+        """records on the handle's device as the record calls read them, and their channel-row pitch"""
+        B, C, N = records.shape
+        if records.device != self._handle_device:
+            records = records.to(self._handle_device)
+        if records.is_contiguous():
+            return records, N
+        if records.stride(2) == 1 and records.stride(1) >= N and (B == 1 or records.stride(0) == C * records.stride(1)):
+            return records, records.stride(1)                   # a row-padded view, read in place
+        return records.contiguous(), N
+
+    def _predict_record_heads(self, records, stride, age, return_prob, path, mode, state, return_state, heads):
+        """predict_record with K >= 1 checked heads: b2cnn_score_record_heads"""
+        B, N, W = records.shape[0], records.shape[2], self.arch.window
+        rows = 1 + len(heads)
+        lib, h = self._ensure_handle()
+        hs = [m._ensure_handle()[1].value for m in heads]
+        dev = self._handle_device
+        if state is not None:
+            state = state.detach().to(device=dev, dtype=torch.float32).contiguous()
+        n_w = (N - W) // stride + 1 if N >= W else 0
+        if n_w == 0:
+            out = torch.empty(rows, B, 0, dtype=torch.float32, device=dev)
+            if not return_state:
+                return out
+            return out, (state.clone() if state is not None else torch.zeros((rows, B) + LSTM_STATE, dtype=torch.float32, device=dev))
+        records, pitch = self._record_pitch(records)
+        age = age.to(dev).contiguous()
+        dtype = capi.DTYPE_BF16 if records.dtype == torch.bfloat16 else capi.DTYPE_F32
+        out = torch.empty(rows, B, n_w, dtype=torch.float32, device=dev)
+        m = capi.MODE_SEQUENCE if mode == "sequence" else capi.MODE_INDEPENDENT
+        arr = (ctypes.c_void_p * len(hs))(*hs)
+        with torch.cuda.device(dev):
+            need = int(lib.b2cnn_record_workspace_bytes_heads(h, len(hs), B, N, pitch, stride, dtype, _PATHS[path], m))
+            if need < 0:
+                raise RuntimeError(capi.last_error())
+            ws = torch.empty(max(need, 256), dtype=torch.uint8, device=dev)
+            st = torch.cuda.current_stream().cuda_stream
+            state_out = torch.empty((rows, B) + LSTM_STATE, dtype=torch.float32, device=dev) if return_state else None
+            capi.check(lib.b2cnn_score_record_heads(h, arr, len(hs), records.data_ptr(), dtype, B, N, pitch, stride, _PATHS[path], m,
+                                                    age.data_ptr(), age.numel(), int(return_prob), out.data_ptr(),
+                                                    None if state is None else state.data_ptr(),
+                                                    None if state_out is None else state_out.data_ptr(), ws.data_ptr(), ws.numel(), st),
+                       "b2cnn_score_record_heads")
         return (out, state_out) if return_state else out
 
     def call_plan(self, window_tensor: torch.Tensor, age: torch.Tensor, mode: str = "independent",

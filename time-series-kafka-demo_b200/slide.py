@@ -55,7 +55,7 @@ import operator
 import torch
 
 from . import capi
-from .model import check_lstm_state
+from .model import HEAD_ARCH_FIELDS, check_head_models, check_lstm_state
 
 
 class SlidingScorer:
@@ -89,7 +89,7 @@ class SlidingScorer:
     incomplete window; the age scales the output only.  A sequence scorer takes no extra heads.  ``scorer.mode``
     tells which one runs."""
 
-    ARCH_FIELDS = ("in_channels", "window", "k1", "k2", "pool_k", "pool_s", "act", "affine", "l_out", "c_mid", "hidden", "layers")
+    ARCH_FIELDS = HEAD_ARCH_FIELDS
 
     PATHS = {"tensorcore": capi.PATH_TENSORCORE, "generic": capi.PATH_GENERIC, "auto": capi.PATH_AUTO}
     MODES = {"independent": capi.MODE_INDEPENDENT, "sequence": capi.MODE_SEQUENCE}
@@ -230,27 +230,11 @@ class SlidingScorer:
 
     def check_heads(self, models, shorter_windows: bool = False) -> tuple:
         """Validates ``set_heads``' argument without touching the library; returns the models as a tuple."""
-        from .model import B200MyCNN
-        if isinstance(models, (B200MyCNN, torch.Tensor, str, bytes)) or not hasattr(models, "__iter__"):
-            raise TypeError("set_heads takes a list of B200MyCNN models")
         if not isinstance(shorter_windows, bool):
             raise TypeError(f"shorter_windows must be True or False, got {type(shorter_windows).__name__}")
-        models = tuple(models)
-        if len(models) > capi.SLIDE_MAX_HEADS:
-            raise ValueError(f"at most {capi.SLIDE_MAX_HEADS} heads, got {len(models)}")
-        mine = self.model.arch
         fields = [f for f in self.ARCH_FIELDS if not (shorter_windows and f in ("window", "l_out"))]
-        for i, m in enumerate(models):
-            if not isinstance(m, B200MyCNN):
-                raise TypeError(f"heads[{i}] is a {type(m).__name__}, not a B200MyCNN")
-            bad = [f for f in fields if getattr(m.arch, f) != getattr(mine, f)]
-            if bad:
-                raise ValueError(f"heads[{i}] differs from the scorer's model in {', '.join(bad)}")
-            if shorter_windows:
-                self._check_head_window(i, m.arch)
-            if m._device() != self.device:
-                raise ValueError(f"heads[{i}] is on {m._device()}, the scorer on {self.device}")
-        return models
+        return check_head_models(models, self.model.arch, self.device, "set_heads", "the scorer's model", "the scorer", fields,
+                                 (lambda i, m: self._check_head_window(i, m.arch)) if shorter_windows else None)
 
     def _check_head_window(self, i: int, arch):
         """a head window W_k ends where the scorer's does: W_k <= W, W - W_k a multiple of the feature stride F, and
