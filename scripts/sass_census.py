@@ -182,8 +182,11 @@ def main() -> int:
 
     r2ur = sum(1 for _, op, _ in body if op.startswith("R2UR"))
     waits = [(a, b) for a, op, b in body if op.startswith("WARPGROUP.DEPBAR")]
-    # the source waits once per block (conv1) and once per projection: any more are ptxas's
-    print(f"\nin the loop: R2UR {r2ur}, warpgroup waits {len(waits)} (the source's: {blocks + nproj})")
+    bars = [(a, b) for a, op, b in body if op.startswith("BAR.SYNC")]
+    # the source waits once per block (it retires the block's conv1 and the projection issued a block earlier) and
+    # passes one warpgroup barrier per block (the a1 exchange): any more waits are ptxas's
+    print(f"\nin the loop: R2UR {r2ur}, warpgroup waits {len(waits)} (the source's: {blocks}), "
+          f"named barriers {len(bars)} (the source's: {blocks})")
 
     # registers per role: setmaxnreg limits and the highest register each role's code names
     # (a role's code ends at the next setmaxnreg or the function's last EXIT: the mbarrier retry loops ptxas moves

@@ -14,7 +14,8 @@
 //     (tiles advance by 24 samples; the 8 overlapping samples are re-read from L2, not HBM).
 //     The small tile keeps the kernel at about 100 KB of shared memory: two CTAs share an SM.
 //   * B = T_c: the fp32 conv1 weights expanded to a 16 x 32 band matrix (8 output shifts s x 4
-//     output channels o) and split into 2 or 3 bf16 pieces (hi/mid/lo) so that, the inputs
+//     output channels o, column 8 (s/2) + 2 o + s%2, so that each lane of the accumulator fragment
+//     holds every shift of one channel) and split into 2 or 3 bf16 pieces (hi/mid/lo) so that, the inputs
 //     being exactly bf16, every product is exact and the fp32 accumulation carries the full
 //     fp32 weight precision.  One wgmma m64n32k16 per (row half, block, channel, piece).
 //   * The one tap that does not fit a 16-sample slice (s=7, k=9 -> sample 8n+16) is added by
@@ -116,7 +117,9 @@ int tc_prepare(TcState &s, const Dims &d, const ConvWeights &cw, const float *d_
         }
     }
     // band matrices: piece sp of T_c[k][(s,o)] = w1[o][c][k-s], stored as GMMA K-major
-    // no-swizzle core matrices: byte = (n/8)*256 + (k/8)*128 + (n%8)*16 + (k%8)*2, n = s*4+o.
+    // no-swizzle core matrices: byte = (n/8)*256 + (k/8)*128 + (n%8)*16 + (k%8)*2, with column
+    // n = 8 (s/2) + 2 o + s%2: lane l of the accumulator fragment, which holds columns 8 j + 2 (l%4) + {0, 1},
+    // then holds all 8 shifts of out channel l%4 (see b2cnn_tc_fused.cuh).
     //   d_bmats   [C][3][1 KB]  three bf16 pieces (hi/mid/lo: the full 24-bit fp32 mantissa)
     //   d_bmats2  [C][2][1 KB]  the first two pieces only (16 mantissa bits; tc_splits=2, an option:
     //                           6 instead of 9 MMAs per block, weights rounded to 2^-17 relative)
@@ -128,7 +131,7 @@ int tc_prepare(TcState &s, const Dims &d, const ConvWeights &cw, const float *d_
                     const int tap = k - sft;
                     if (tap < 0 || tap >= d.K1) continue;
                     float w = cw.w1[(c * d.K1 + tap) * kCMid + o];
-                    const int n = sft * 4 + o;
+                    const int n = 8 * (sft >> 1) + 2 * o + (sft & 1);   // column of (shift, out channel)
                     const size_t off = (size_t)(n / 8) * 128 + (k / 8) * 64 + (n % 8) * 8 + (k % 8);   // in bf16 units
                     for (int sp = 0; sp < 3; ++sp) {
                         const uint16_t piece = bf16_rn(w);

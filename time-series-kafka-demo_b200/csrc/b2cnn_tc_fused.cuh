@@ -7,19 +7,21 @@
 // conv1 of bf16 windows is the banded-Toeplitz GEMM described in b2cnn_tc.cu, on wgmma: per 8-position block,
 // two m64n32k16 row halves x C channels x SPLITS weight pieces, A in registers (one ldmatrix.x4 per row half and
 // channel of the block's 16-sample slice of the TMA tile: 32-sample boxes, SWIZZLE_64B, 3 blocks per tile, shared by
-// the SPLITS pieces), B = the band-matrix piece, D in registers.  The accumulator fragment (two windows x 16 values
-// per thread) is turned into thread == window through a 16 KB shared-memory transpose (XOR-swizzled, conflict-free
-// both ways); the next block's MMAs run while the epilogue of this one computes.  The three blocks of a tile are
+// the SPLITS pieces), B = the band-matrix piece, D in registers.  The band matrices' columns are ordered so that each
+// lane of the accumulator fragment holds all 8 shifts of one conv1 channel for its four windows: pool1 and the
+// activation run there, register-local, and only the pooled a1 (16 floats per window) cross to thread == window through
+// a double-buffered 2 x 8 KB shared-memory exchange (XOR-swizzled, conflict-free both ways, one barrier per block); the
+// next block's MMAs run while the epilogue of this one computes.  The three blocks of a tile are
 // unrolled, so their addresses are the tile's plus immediates.  About 100 KB of shared memory and 128 registers per
 // thread at launch let two CTAs share an SM, so each SM sub-partition has two consumer warps to interleave;
 // setmaxnreg then gives the consumer warpgroup 232 of them and the producer warpgroup 24.  fp32 windows (F32IN) evaluate conv1 in exact fp32
 // FMAs straight from the tile instead (the same 32-sample boxes as 128-byte SWIZZLE_128B rows; one CTA per SM).
 //
-// Epilogue, thread == window: each thread streams through its window's positions in order, so pool1 -> tanh ->
-// conv2 -> pool2 -> tanh are register-local sliding windows; tanh is 1 - 2/(1+2^(2x log2 e)) on MUFU.EX2 +
-// MUFU.RCP with the bias folded into the exponent FMA; pooling runs BEFORE the activation (monotone) with
-// max.NaN so NaNs propagate exactly like ATen's max_pool1d.  conv2 consumes r = (1 - tanh)/2 (weights
-// pre-multiplied by -2, the bias absorbs sum(w)).
+// Epilogue, thread == window (after the a1 exchange for bf16 windows): each thread streams through its window's
+// positions in order, so conv2 -> pool2 -> tanh (fp32 windows: pool1 -> tanh first) are register-local sliding
+// windows; tanh is 1 - 2/(1+2^(2x log2 e)) on MUFU.EX2 + MUFU.RCP with the bias folded into the exponent FMA; pooling
+// runs BEFORE the activation (monotone) with max.NaN so NaNs propagate exactly like ATen's max_pool1d.  conv2
+// consumes r = (1 - tanh)/2 (weights pre-multiplied by -2, the bias absorbs sum(w)).
 //
 // Projection: the two features of a step are split into three bf16 pieces and stored into a [128 x 16]
 // K-major A tile per piece; every 16 positions the warpgroup issues 2 row halves x 6 m64n64k16 MMAs (piece
@@ -38,12 +40,13 @@ namespace b2cnn {
 // 6 and 7 idle) to the consumer one; fp32 windows: 192 threads
 __host__ __device__ constexpr int hp_threads(bool f32in) { return f32in ? 192 : 256; }
 constexpr int kHpProducerRegs = 24, kHpConsumerRegs = 232;   // 128 x 24 + 128 x 232 = 256 x 128: two CTAs per SM
-// accumulator transpose: 32 floats per window row, 16-byte chunk q of row r stored at chunk q ^ hp_tswz(r).  The
-// rotation makes both sides conflict-free: the 8 rows an LDS.128 quarter-warp reads get 8 distinct masks, and the
-// 4 rows x 2 chunks an STS.64 half-warp writes (rows 0-3 or 4-7 of a group of 8: even or odd masks) 8 distinct chunks.
-constexpr int kHpTStride = 32;
-constexpr int kHpTBytes = kTcM * kHpTStride * 4;
-__device__ __forceinline__ uint32_t hp_tswz(uint32_t r) { return ((r << 1) | ((r >> 2) & 1u)) & 7u; }   // r % 8 rotated left
+// a1 exchange (bf16 windows), double-buffered by block parity: per window row the 16 pooled activations of a block,
+// 16-byte chunk o = channel o's 4 positions, stored at chunk o ^ (r / 2) % 4.  Both sides are conflict-free: an STS.128
+// quarter-warp writes two whole adjacent 64-byte rows, and an LDS.128 quarter-warp reads 8 rows whose
+// (r % 2, (r / 2) % 4) pairs are all distinct.
+constexpr int kHpXStride = 16;
+constexpr int kHpXBuf = kTcM * kHpXStride * 4;
+constexpr int kHpXBytes = 2 * kHpXBuf;
 constexpr int kHpPieceBytes = kTcM * 16 * 2;      // one bf16 piece of the projection A operand
 constexpr int kFuWChunkBytes = 3 * 64 * 16 * 2;   // 3 pieces x (64 gates x 16 positions) bf16
 // kOutRing: the features of a sliding-window scorer's new segment (b2cnn_slide.cu) into its position-major
@@ -70,7 +73,7 @@ struct TcFusedParams {
 };
 
 __host__ __device__ constexpr size_t hp_smem_bytes(int C, int SPLITS, bool f32in, int out) {
-    return 1024 + (size_t)2 * C * kTcM * (f32in ? kTcF32ARow : kTcARow) + (f32in ? 0 : (size_t)C * SPLITS * kTcBBytes + kHpTBytes) +
+    return 1024 + (size_t)2 * C * kTcM * (f32in ? kTcF32ARow : kTcARow) + (f32in ? 0 : (size_t)C * SPLITS * kTcBBytes + kHpXBytes) +
            (out == kOutGates ? (size_t)2 * kFuWChunkBytes + 2 * 3 * kHpPieceBytes : 0) + 8 * 8;
 }
 
@@ -87,14 +90,14 @@ tc_stream_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant
     constexpr int kABytes = kTcM * kARow;             // one channel of one stage
     constexpr int FOFF = ARCH == 0 ? 3 : 2;           // step j emits features 2j-FOFF, 2j-FOFF+1
     extern __shared__ uint8_t smem_raw[];
-    // [2 stages][C][8 KB bf16 | 16 KB fp32] | bands | transpose | W ring [2][6 KB] | A pieces [2][3][4 KB] | barriers
-    // aligned by an offset from smem_raw, not by rounding the generic address as an integer: the compiler then still
-    // knows every pointer below is shared memory and emits 32-bit LDS / STS instead of 64-bit generic LD / ST
+    // [2 stages][C][8 KB bf16 | 16 KB fp32] | bands | a1 exchange [2][8 KB] | W ring [2][6 KB] | A pieces [2][3][4 KB] |
+    // barriers, aligned by an offset from smem_raw, not by rounding the generic address as an integer: the compiler then
+    // still knows every pointer below is shared memory and emits 32-bit LDS / STS instead of 64-bit generic LD / ST
     uint8_t *smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     uint8_t *sA = smem;
     uint8_t *sBm = sA + 2 * C * kABytes;
-    float *sT = reinterpret_cast<float *>(sBm + (F32IN ? 0 : C * SPLITS * kTcBBytes));
-    uint8_t *sW = reinterpret_cast<uint8_t *>(sT) + (F32IN ? 0 : kHpTBytes);
+    uint8_t *sX = sBm + (F32IN ? 0 : C * SPLITS * kTcBBytes);
+    uint8_t *sW = sX + (F32IN ? 0 : kHpXBytes);
     uint8_t *sPc = sW + (OUT == kOutGates ? 2 * kFuWChunkBytes : 0);
     uint64_t *bars = reinterpret_cast<uint64_t *>(sPc + (OUT == kOutGates ? 2 * 3 * kHpPieceBytes : 0));
     const uint32_t bar_full = smem_u32(bars + 0), bar_empty = smem_u32(bars + 2);
@@ -163,12 +166,20 @@ tc_stream_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant
         const bool row_ok = b < p.B;
         // 16-byte chunk k of a row sits at chunk k ^ swz: SWIZZLE_64B (bf16) k ^ (row / 2) % 4, SWIZZLE_128B (fp32) k ^ row % 8
         const uint32_t swz = F32IN ? (uint32_t)(row & 7) : (uint32_t)((row >> 1) & 3);
-        // transpose addresses.  Rows are 128 bytes, so a chunk mask only flips bits 4-6 of an address.  Writes: this
-        // thread's rows (all == lane / 4 mod 8) at 8 (lane & 1) bytes of chunk (2 E + (lane >> 1) % 2) ^ mask, i.e.
-        // t_w ^ 32 E, plus 128 bytes per row; reads: its own row's chunk q at t_r ^ 16 q.
-        const uint32_t t_w = smem_u32(sT) + (uint32_t)(16 * warp + (lane >> 2)) * (kHpTStride * 4) + 8 * (lane & 1) +
-                             16 * (((lane >> 1) & 1) ^ hp_tswz((uint32_t)lane >> 2));
-        const uint32_t t_r = smem_u32(sT) + (uint32_t)row * (kHpTStride * 4) + 16 * hp_tswz((uint32_t)row);
+        // bf16 windows: lane l of the conv1 accumulator fragment holds every shift of out channel q = l % 4 for four
+        // windows, rows 64 h + 16 warp + l / 4 + 8 e (row halves h, fragment row groups e), acc[h][4 (s / 2) + 2 e + s % 2]
+        // for shift s (b2cnn_tc.cu packs the band matrices so).  Pool1 and the activation run there; only the pooled a1
+        // cross to thread == window.  Rows are 64 bytes and every window of a lane has the same (r / 2) % 4 == l / 8, so
+        // the lane writes chunk q ^ (l / 8) at x_w plus an immediate per window; a thread reads its own row's chunk o at
+        // x_r ^ 16 o.  Block j uses buffer j % 2.
+        const int q = lane & 3;
+        const uint32_t x_w = smem_u32(sX) + (uint32_t)(16 * warp + (lane >> 2)) * (kHpXStride * 4) + 16 * (q ^ (lane >> 3));
+        const uint32_t x_r = smem_u32(sX) + (uint32_t)row * (kHpXStride * 4) + 16 * swz;
+        // the lane's own conv1 constants, in registers for the whole loop
+        const float b1q = p.b1s[q];
+        float w9q[C];
+#pragma unroll
+        for (int c = 0; c < C; ++c) w9q[c] = p.w9[c][q];
         float acc[2][16];                             // conv1 accumulators of one block (two m64 row halves)
         float gacc[2][32];                            // gate pre-activations (two m64 row halves)
 #pragma unroll
@@ -178,6 +189,8 @@ tc_stream_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant
 #pragma unroll
             for (int i = 0; i < 32; ++i) gacc[h][i] = 0.f;
         }
+        // conv1 positions 6 and 7 of the previous block: fp32 windows per out channel o of the thread's window, bf16
+        // windows per window 2 h + e of the lane's out channel q
         float pm6[kCMid], pm7[kCMid], ah[4][kCMid], c2c = 0.f, nan_probe = 0.f;
 #pragma unroll
         for (int o = 0; o < kCMid; ++o) {
@@ -197,8 +210,9 @@ tc_stream_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant
         const uint32_t a_swz = (lane >> 1) & 3, a_k = lane >> 4;
         // chunk (n + a_k) ^ a_swz of a 64-byte row: blocks 0 and 2 at a_b02 ^ 16 n, block 1 ((1 + a_k) == 1 << a_k) at a_b1
         const uint32_t a_b02 = a_lane | ((a_k ^ a_swz) << 4), a_b1 = a_lane | (((1u << a_k) ^ a_swz) << 4);
-        // tap 9 of block n: chunk (n + 1) ^ swz of this thread's row, t9_row ^ 16 (n + 1)
-        const uint32_t t9_row = smem_u32(sA) + (uint32_t)(row * kARow) + (swz << 4);
+        // tap 9 of block n for the lane's four windows: chunk (n + 1) ^ (lane / 8) of their rows (SWIZZLE_64B), t9 ^ 16 (n + 1)
+        // plus an immediate per window.  The 8 rows a warp reads get 8 distinct banks; a quad's lanes share an address.
+        const uint32_t t9 = smem_u32(sA) + (uint32_t)(16 * warp + (lane >> 2)) * kARow + ((uint32_t)(lane >> 3) << 4);
         // B descriptor built once: a block's MMAs only add (start address offset) >> 4 to it
         const uint64_t bdesc0 = gdesc_none_kmajor(smem_u32(sBm), 128, 256);
         auto issue_conv1 = [&](int s, int n) {
@@ -238,7 +252,7 @@ tc_stream_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant
             wgmma_commit();
         };
         // A chunk that ends at step jc inside the range is projected without draining the tensor pipe: bf16 windows issue
-        // it at step jc + 1 behind that step's transpose barrier and before its conv1, and the wait of step jc + 2 retires
+        // it at step jc + 1 behind that step's barrier and the next block's conv1, and the wait of step jc + 2 retires
         // both; fp32 windows issue it at the end of step jc and retire it at step jc + 1, after the CUDA-core conv1.  The
         // step that retires it gives its W slot back.  The range's last chunk is projected after the loop.
         constexpr int kLag = F32IN ? 1 : 2;
@@ -262,17 +276,21 @@ tc_stream_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant
         // compile-time constant, so a block's tile, ldmatrix and tap-9 addresses are the tile's plus immediates.
         auto step = [&](const int j, const int i, const int n) {
             const int s = i & 1;
-            float D[32];                              // conv1 pre-activations of block j: D[shift * 4 + out channel]
+            float an[4][kCMid];                       // a1 of block j, thread == window: an[position][channel]
             if constexpr (!F32IN) {
+                // tap 9 of the previous block's position 7 (sample 8n + 8 of this tile), added while the MMAs run, in
+                // the same order over c as the fp32 path
                 if constexpr (ARCH == 0) {
-                    // tap 9 of the previous block's position 7: sample 8n + 8 of this tile
 #pragma unroll
-                    for (int c = 0; c < C; ++c) {
-                        const uint32_t raw = ld_shared_u16((t9_row ^ (uint32_t)(16 * (n + 1))) + (uint32_t)((s * C + c) * kABytes));
-                        const float xv = __uint_as_float(raw << 16);
+                    for (int h = 0; h < 2; ++h)
 #pragma unroll
-                        for (int o = 0; o < kCMid; ++o) pm7[o] = fmaf(p.w9[c][o], xv, pm7[o]);
-                    }
+                        for (int e = 0; e < 2; ++e)
+#pragma unroll
+                            for (int c = 0; c < C; ++c) {
+                                const uint32_t raw = ld_shared_u16((t9 ^ (uint32_t)(16 * (n + 1))) +
+                                                                   (uint32_t)((s * C + c) * kABytes + (64 * h + 8 * e) * kARow));
+                                pm7[2 * h + e] = fmaf(w9q[c], __uint_as_float(raw << 16), pm7[2 * h + e]);
+                            }
                 }
                 wgmma_wait<0>();                      // conv1 of this block (and the projection issued at step j - 1)
 #pragma unroll
@@ -280,31 +298,59 @@ tc_stream_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant
 #pragma unroll
                     for (int c = 0; c < C; ++c) wgmma_keep(afr[h][c]);
                 release_w(j);
+                // ---- pool1 on pre-activations in the fragment layout: window 2 h + e, channel q, position r
+                float m[2][2][4];
 #pragma unroll
                 for (int h = 0; h < 2; ++h)
 #pragma unroll
-                    for (int e = 0; e < 16; e += 2)   // row 64 h + 16 warp + lane / 4 + 8 ((e / 2) % 2), column 8 (e / 4) + 2 (lane % 4)
-                        st_shared_v2((t_w ^ (uint32_t)(32 * (e >> 2))) + (uint32_t)((64 * h + 8 * ((e >> 1) & 1)) * kHpTStride * 4),
-                                     acc[h][e], acc[h][e + 1]);
-                wg_bar();
-                if (n == kBlocks - 1 && lane == 0) mbar_arrive(bar_empty + 8 * s);   // stage fully consumed
-                // the chunk that ended at step j - 1, its pieces published by the barrier above, ahead of the next conv1
-                // (behind it, measured no faster than draining)
-                if (OUT == kOutGates && (j & 7) == 0 && j > 0) issue_proj((j >> 3) - 1);
-                if (n < kBlocks - 1) {                // the next block's MMAs overlap this block's epilogue
+                    for (int e = 0; e < 2; ++e) {
+                        const float *d = acc[h] + 2 * e;   // shift t at d[4 (t / 2) + t % 2]
+                        const int w = 2 * h + e;
+                        if constexpr (ARCH == 0) {
+                            m[h][e][0] = max3_nan(pm6[w], pm7[w], d[0]);
+                            m[h][e][1] = max3_nan(d[0], d[1], d[4]);
+                            m[h][e][2] = max3_nan(d[4], d[5], d[8]);
+                            m[h][e][3] = max3_nan(d[8], d[9], d[12]);
+                            pm6[w] = acc_copy(d[12]);
+                            pm7[w] = acc_copy(d[13]);
+                        } else {
+#pragma unroll
+                            for (int r = 0; r < 4; ++r) m[h][e][r] = max_nan(d[4 * r], d[4 * r + 1]);
+                        }
+                    }
+                // acc is free once the maxima and the carries are taken: the next block's MMAs run on the tensor core
+                // during this block's activations and the rest of its epilogue (issued after the barrier instead, behind
+                // the projection, the step measured about 3 % slower)
+                if (n < kBlocks - 1) {
                     issue_conv1(s, n + 1);
                 } else if (i + 1 < ntiles) {          // (J is a whole number of tiles)
                     mbar_wait(bar_full + 8 * (s ^ 1), ((i + 1) >> 1) & 1);
                     issue_conv1(s ^ 1, 0);
                 }
+                // ---- r = (1 - tanh(+bias)) / 2, then the exchange: 4 positions of channel q per window and STS.128
+                const uint32_t xb = (uint32_t)(((i + n) & 1) * kHpXBuf);
 #pragma unroll
-                for (int k = 0; k < 32; k += 4) {
-                    const float4 v = ld_shared_v4(t_r ^ (uint32_t)(4 * k));
-                    D[k] = v.x; D[k + 1] = v.y; D[k + 2] = v.z; D[k + 3] = v.w;
+                for (int h = 0; h < 2; ++h)
+#pragma unroll
+                    for (int e = 0; e < 2; ++e)
+                        st_shared_v4(x_w + xb + (uint32_t)((64 * h + 8 * e) * kHpXStride * 4), sig_fold(m[h][e][0], b1q),
+                                     sig_fold(m[h][e][1], b1q), sig_fold(m[h][e][2], b1q), sig_fold(m[h][e][3], b1q));
+                // One barrier per block.  It publishes block j's a1 (buffer j % 2) and every warp's projection pieces of
+                // step j - 1.  A warp writes buffer j % 2 again at block j + 2, after barrier j + 1, which every warp
+                // reaches only after reading its block-j row, so the buffer needs no second barrier.
+                wg_bar();
+                if (n == kBlocks - 1 && lane == 0) mbar_arrive(bar_empty + 8 * s);   // stage fully consumed
+                // the chunk that ended at step j - 1, its pieces published by the barrier above, behind the next conv1;
+                // the next step's wait retires both
+                if (OUT == kOutGates && (j & 7) == 0 && j > 0) issue_proj((j >> 3) - 1);
+#pragma unroll
+                for (int o = 0; o < kCMid; ++o) {
+                    const float4 v = ld_shared_v4((x_r ^ (uint32_t)(16 * o)) + xb);
+                    an[0][o] = v.x; an[1][o] = v.y; an[2][o] = v.z; an[3][o] = v.w;
                 }
-                wg_bar();                             // transpose buffer free for the next block
             } else {
                 // conv1 of block j on the CUDA cores, exact fp32, from the 16 samples at tile offset 8n
+                float D[32];                          // conv1 pre-activations of block j: D[shift * 4 + out channel]
                 if (n == 0) mbar_wait(bar_full + 8 * s, (i >> 1) & 1);
 #pragma unroll
                 for (int k = 0; k < 32; ++k) D[k] = 0.f;
@@ -337,21 +383,20 @@ tc_stream_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant
                     __syncwarp();
                     if (lane == 0) mbar_arrive(bar_empty + 8 * s);
                 }
-            }
-            // ---- pool1 on pre-activations, then r = (1 - tanh(+bias)) / 2: a1 positions of this block
-            float an[4][kCMid];
+                // ---- pool1 on pre-activations, then r = (1 - tanh(+bias)) / 2: a1 positions of this block
 #pragma unroll
-            for (int o = 0; o < kCMid; ++o) {
-                if constexpr (ARCH == 0) {
-                    an[0][o] = sig_fold(max3_nan(pm6[o], pm7[o], D[0 * 4 + o]), p.b1s[o]);
-                    an[1][o] = sig_fold(max3_nan(D[0 * 4 + o], D[1 * 4 + o], D[2 * 4 + o]), p.b1s[o]);
-                    an[2][o] = sig_fold(max3_nan(D[2 * 4 + o], D[3 * 4 + o], D[4 * 4 + o]), p.b1s[o]);
-                    an[3][o] = sig_fold(max3_nan(D[4 * 4 + o], D[5 * 4 + o], D[6 * 4 + o]), p.b1s[o]);
-                    pm6[o] = D[6 * 4 + o];
-                    pm7[o] = D[7 * 4 + o];
-                } else {
+                for (int o = 0; o < kCMid; ++o) {
+                    if constexpr (ARCH == 0) {
+                        an[0][o] = sig_fold(max3_nan(pm6[o], pm7[o], D[0 * 4 + o]), p.b1s[o]);
+                        an[1][o] = sig_fold(max3_nan(D[0 * 4 + o], D[1 * 4 + o], D[2 * 4 + o]), p.b1s[o]);
+                        an[2][o] = sig_fold(max3_nan(D[2 * 4 + o], D[3 * 4 + o], D[4 * 4 + o]), p.b1s[o]);
+                        an[3][o] = sig_fold(max3_nan(D[4 * 4 + o], D[5 * 4 + o], D[6 * 4 + o]), p.b1s[o]);
+                        pm6[o] = D[6 * 4 + o];
+                        pm7[o] = D[7 * 4 + o];
+                    } else {
 #pragma unroll
-                    for (int r = 0; r < 4; ++r) an[r][o] = sig_fold(max_nan(D[(2 * r) * 4 + o], D[(2 * r + 1) * 4 + o]), p.b1s[o]);
+                        for (int r = 0; r < 4; ++r) an[r][o] = sig_fold(max_nan(D[(2 * r) * 4 + o], D[(2 * r + 1) * 4 + o]), p.b1s[o]);
+                    }
                 }
             }
             // ---- conv2 over the previous block's and this block's a1 (no bias yet)

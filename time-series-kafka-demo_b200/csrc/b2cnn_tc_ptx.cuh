@@ -56,8 +56,8 @@ __device__ __forceinline__ void wg_bar() { asm volatile("bar.sync 1, 128;" ::: "
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // shared-memory accesses by 32-bit shared address (for addresses built with XOR swizzles)
-__device__ __forceinline__ void st_shared_v2(uint32_t addr, float x, float y) {
-    asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(x), "f"(y) : "memory");
+__device__ __forceinline__ void st_shared_v4(uint32_t addr, float x, float y, float z, float w) {
+    asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "f"(x), "f"(y), "f"(z), "f"(w) : "memory");
 }
 __device__ __forceinline__ uint32_t ld_shared_u16(uint32_t addr) {
     uint16_t v;
@@ -127,6 +127,14 @@ __device__ __forceinline__ void wgmma_m64n32_rs(float *d, const uint32_t *a, uin
 // keeps the A fragment registers of in-flight wgmmas alive (and unmodified) up to this point: place after the wait
 __device__ __forceinline__ void wgmma_keep(uint32_t *a) {
     asm volatile("" : "+r"(a[0]), "+r"(a[1]), "+r"(a[2]), "+r"(a[3]) :: "memory");
+}
+// an accumulator value copied out at this point, ahead of the next wgmma that overwrites its register.  A plain
+// assignment of a value carried to the next block may be sunk past that wgmma's issue; it then reads an in-flight
+// accumulator, and ptxas serializes every wgmma of the kernel (C7511).
+__device__ __forceinline__ float acc_copy(float x) {
+    float y;
+    asm volatile("mov.b32 %0, %1;" : "=f"(y) : "f"(x));
+    return y;
 }
 // four 8x8 b16 matrices from shared memory; lanes 8i .. 8i+7 give the row addresses of matrix i, which lands in r[i]
 __device__ __forceinline__ void ldmatrix_x4(uint32_t *r, uint32_t saddr) {
