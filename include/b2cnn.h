@@ -721,6 +721,38 @@ int b2cnn_train_backward_record_state(const b2cnn_config *cfg, const float *para
                                       float *d_records, float *dage, float *d_state_in, int flags, void *workspace, int64_t workspace_bytes,
                                       void *stream);
 
+
+/* ---- Candidate heads on one frozen front end (DESIGN.md §8, training candidate heads) ----
+ * One fused training step for n_heads in [1, B2CNN_SLIDE_MAX_HEADS] models that share conv1 / conv2: the conv forward
+ * runs once on `frontend` (a packed blob of b2cnn_weight_count() floats, read for its conv entries only), and each head
+ * trains its own LSTM and Linear entries (blob entries from W_ih_l0 on) with its own Adam state.  Nothing back-propagates
+ * into the front end.  params, adam_m, adam_v and grads are HOST arrays of n_heads DEVICE pointers, each a full packed
+ * blob; only entries from W_ih_l0 on are written, and the conv entries of grads are set to zero.  lr is a HOST array of
+ * n_heads learning rates; opt gives beta1, beta2 and eps for every head (opt->lr is not read).  loss_out is a DEVICE array
+ * of n_heads floats.  Every other argument is b2cnn_train_step_seq's / b2cnn_train_step_record's, shared by all heads:
+ * the batch, the mode, the masks and pos_weight (NULL or one host float).  b2cnn_train_heads_step takes mode and, when
+ * seq_lengths != NULL, the sequence lengths (mode must then be B2CNN_MODE_SEQUENCE).
+ * Head h's loss and gradients are the bits b2cnn_train_step_seq / _weighted / _record computes on params[h] with the same
+ * arguments, and its updated blob the bits of that call with apply_update.  The launch list does not depend on n_heads.
+ * B2CNN_EINVAL before any CUDA call: n_heads outside [1, 8], a NULL pointer (adam_m / adam_v only with apply_update), two
+ * heads sharing or overlapping a blob (params, grads and, with apply_update, adam_m / adam_v: none may overlap another),
+ * and whatever the single-model calls refuse.  A workspace smaller than b2cnn_train_heads_workspace_bytes[_record]() is
+ * B2CNN_ESTATE before any launch.  The call allocates nothing and is asynchronous on `stream`. */
+int64_t b2cnn_train_heads_workspace_bytes(const b2cnn_config *cfg, int32_t n_heads, int64_t B, const int64_t *seq_lengths, int64_t n_seq);
+int b2cnn_train_heads_step(const b2cnn_config *cfg, const float *frontend, int32_t n_heads, float *const *params, float *const *adam_m,
+                           float *const *adam_v, float *const *grads, const float *lr, int64_t step, const b2cnn_adam *opt,
+                           int apply_update, const float *x, int64_t B, const float *age, const float *target, const float *pos_weight,
+                           int mode, const int64_t *seq_lengths, int64_t n_seq, const float *mask1, const float *mask2, float *loss_out,
+                           void *workspace, int64_t workspace_bytes, void *stream);
+int64_t b2cnn_train_heads_workspace_bytes_record(const b2cnn_config *cfg, int32_t n_heads, int64_t B, int64_t N, int64_t stride,
+                                                 const int64_t *window_counts, int mode);
+int b2cnn_train_heads_step_record(const b2cnn_config *cfg, const float *frontend, int32_t n_heads, float *const *params,
+                                  float *const *adam_m, float *const *adam_v, float *const *grads, const float *lr, int64_t step,
+                                  const b2cnn_adam *opt, int apply_update, const float *records, int64_t B, int64_t N, int64_t stride,
+                                  const int64_t *window_counts, int mode, const float *age, const float *target, const float *pos_weight,
+                                  const float *mask1, const float *mask2, float *loss_out, void *workspace, int64_t workspace_bytes,
+                                  void *stream);
+
 #ifdef __cplusplus
 }
 #endif

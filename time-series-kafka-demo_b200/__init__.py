@@ -16,11 +16,11 @@ from .arch import ArchConfig, ARCH_PRESETS, arch_from_state_dict  # noqa: F401
 from .capi import LibraryNotBuilt, lib_path, load_library  # noqa: F401
 from .checkpoint import load_reference_checkpoint  # noqa: F401
 from .model import B200MyCNN  # noqa: F401
-from .trainer import B200Trainer  # noqa: F401
+from .trainer import B200HeadTrainer, B200Trainer  # noqa: F401
 from .autograd import B200TrainableMyCNN, mycnn_train_forward, mycnn_train_record_forward  # noqa: F401
 from .slide import SlidingScorer  # noqa: F401
 from .stream import PatientRing  # noqa: F401
 from . import synth  # noqa: F401
 
-__all__ = ["ArchConfig", "ARCH_PRESETS", "arch_from_state_dict", "B200MyCNN", "B200Trainer", "B200TrainableMyCNN", "mycnn_train_forward", "mycnn_train_record_forward", "SlidingScorer", "PatientRing",
+__all__ = ["ArchConfig", "ARCH_PRESETS", "arch_from_state_dict", "B200MyCNN", "B200Trainer", "B200HeadTrainer", "B200TrainableMyCNN", "mycnn_train_forward", "mycnn_train_record_forward", "SlidingScorer", "PatientRing",
            "load_reference_checkpoint", "load_library", "lib_path", "LibraryNotBuilt", "synth"]

@@ -41,6 +41,8 @@ SYMBOLS = ("b2cnn_l_out", "b2cnn_weight_count", "b2cnn_create", "b2cnn_destroy",
            "b2cnn_record_workspace_bytes", "b2cnn_score_record", "b2cnn_record_workspace_bytes_ex", "b2cnn_score_record_ex",
            "b2cnn_score_record_state", "b2cnn_slide_admit_ex", "b2cnn_train_step_record_state", "b2cnn_train_forward_record_state",
            "b2cnn_train_backward_record_state", "b2cnn_record_workspace_bytes_heads", "b2cnn_score_record_heads",
+           "b2cnn_train_heads_workspace_bytes", "b2cnn_train_heads_step", "b2cnn_train_heads_workspace_bytes_record",
+           "b2cnn_train_heads_step_record",
            "b2cnn_decode_sample_messages", "b2cnn_decode_array_messages", "b2cnn_parse_decimal", "b2cnn_frame_check")
 
 
@@ -238,6 +240,16 @@ def load_library() -> ctypes.CDLL:
     lib.b2cnn_train_backward_record_state.argtypes = [cfgp, c_vp, c_vp, c_i64, c_i64, c_i64, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
                                                       c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_i64, c_vp]
     lib.b2cnn_train_backward_record_state.restype = c_int
+    lib.b2cnn_train_heads_workspace_bytes.argtypes = [cfgp, c_i32, c_i64, c_vp, c_i64]
+    lib.b2cnn_train_heads_workspace_bytes.restype = c_i64
+    lib.b2cnn_train_heads_step.argtypes = [cfgp, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, ctypes.POINTER(Adam), c_int, c_vp, c_i64,
+                                           c_vp, c_vp, c_vp, c_int, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp]
+    lib.b2cnn_train_heads_step.restype = c_int
+    lib.b2cnn_train_heads_workspace_bytes_record.argtypes = [cfgp, c_i32, c_i64, c_i64, c_i64, c_vp, c_int]
+    lib.b2cnn_train_heads_workspace_bytes_record.restype = c_i64
+    lib.b2cnn_train_heads_step_record.argtypes = [cfgp, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, ctypes.POINTER(Adam), c_int, c_vp,
+                                                  c_i64, c_i64, c_i64, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp]
+    lib.b2cnn_train_heads_step_record.restype = c_int
     lib.b2cnn_workspace_bytes_seq.argtypes = [c_vp, c_i64, c_vp, c_i64]; lib.b2cnn_workspace_bytes_seq.restype = c_i64
     lib.b2cnn_forward_seq.argtypes = [c_vp, c_vp, c_int, c_i64, c_i64, c_vp, c_i64, c_vp, c_i64, c_int, c_vp, c_vp, c_i64, c_vp]
     lib.b2cnn_forward_seq.restype = c_int

@@ -241,6 +241,55 @@ extern "C" int b2cnn_train_backward_record_state(const b2cnn_config *cfg, const 
     return finish("b2cnn_train_backward_record_state", rc, err);
 }
 
+// ---- candidate heads on one frozen front end (b2cnn_train.cu) ----
+extern "C" int64_t b2cnn_train_heads_workspace_bytes(const b2cnn_config *cfg, int32_t n_heads, int64_t B, const int64_t *seq_lengths,
+                                                    int64_t n_seq) {
+    const SeqLengths sl = seq_lengths ? SeqLengths{true, seq_lengths, n_seq} : kNoSeq;
+    const int64_t n = n_heads < 1 ? -1 : train_workspace_bytes(cfg, B, sl, kNoRec, B2CNN_MODE_SEQUENCE, n_heads);
+    if (n < 0) fail(B2CNN_EINVAL, "b2cnn_train_heads_workspace_bytes: bad configuration / n_heads / batch / sequence lengths");
+    return n;
+}
+extern "C" int64_t b2cnn_train_heads_workspace_bytes_record(const b2cnn_config *cfg, int32_t n_heads, int64_t B, int64_t N, int64_t stride,
+                                                           const int64_t *window_counts, int mode) {
+    const int64_t n = n_heads < 1 ? -1 : train_workspace_bytes(cfg, B, kNoSeq, RecordArgs{true, N, stride, window_counts}, mode, n_heads);
+    if (n < 0) fail(B2CNN_EINVAL, "b2cnn_train_heads_workspace_bytes_record: bad configuration / n_heads / batch / stride / window counts / mode");
+    return n;
+}
+static int train_heads_api(const char *name, const b2cnn_config *cfg, const float *frontend, int32_t n_heads, float *const *params,
+                           float *const *adam_m, float *const *adam_v, float *const *grads, const float *lr, int64_t step,
+                           const b2cnn_adam *opt, int apply_update, const float *x, int64_t B, const float *age, const float *target,
+                           const float *pos_weight, int mode, const SeqLengths &sl, const RecordArgs &ra, const float *mask1,
+                           const float *mask2, float *loss_out, void *workspace, int64_t workspace_bytes, void *stream) {
+    if (!cfg || !opt) return fail(B2CNN_EINVAL, std::string(name) + ": null configuration");
+    const char *err = "";
+    const int rc = train_heads_step(cfg, frontend, n_heads, params, adam_m, adam_v, grads, lr, step, opt->beta1, opt->beta2, opt->eps,
+                                    apply_update, x, B, age, target, pos_weight ? 1 : 0, pos_weight ? *pos_weight : 1.f, mode, sl, ra,
+                                    mask1, mask2, loss_out, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream), &err);
+    return finish(name, rc, err);
+}
+extern "C" int b2cnn_train_heads_step(const b2cnn_config *cfg, const float *frontend, int32_t n_heads, float *const *params,
+                                      float *const *adam_m, float *const *adam_v, float *const *grads, const float *lr, int64_t step,
+                                      const b2cnn_adam *opt, int apply_update, const float *x, int64_t B, const float *age,
+                                      const float *target, const float *pos_weight, int mode, const int64_t *seq_lengths, int64_t n_seq,
+                                      const float *mask1, const float *mask2, float *loss_out, void *workspace, int64_t workspace_bytes,
+                                      void *stream) {
+    if (seq_lengths && mode != B2CNN_MODE_SEQUENCE)
+        return fail(B2CNN_EINVAL, "b2cnn_train_heads_step: seq_lengths needs mode B2CNN_MODE_SEQUENCE");
+    return train_heads_api("b2cnn_train_heads_step", cfg, frontend, n_heads, params, adam_m, adam_v, grads, lr, step, opt, apply_update, x,
+                           B, age, target, pos_weight, mode, seq_lengths ? SeqLengths{true, seq_lengths, n_seq} : kNoSeq, kNoRec, mask1,
+                           mask2, loss_out, workspace, workspace_bytes, stream);
+}
+extern "C" int b2cnn_train_heads_step_record(const b2cnn_config *cfg, const float *frontend, int32_t n_heads, float *const *params,
+                                             float *const *adam_m, float *const *adam_v, float *const *grads, const float *lr,
+                                             int64_t step, const b2cnn_adam *opt, int apply_update, const float *records, int64_t B,
+                                             int64_t N, int64_t stride, const int64_t *window_counts, int mode, const float *age,
+                                             const float *target, const float *pos_weight, const float *mask1, const float *mask2,
+                                             float *loss_out, void *workspace, int64_t workspace_bytes, void *stream) {
+    return train_heads_api("b2cnn_train_heads_step_record", cfg, frontend, n_heads, params, adam_m, adam_v, grads, lr, step, opt,
+                           apply_update, records, B, age, target, pos_weight, mode, kNoSeq, RecordArgs{true, N, stride, window_counts},
+                           mask1, mask2, loss_out, workspace, workspace_bytes, stream);
+}
+
 // ---- preprocessing + window assembly (b2cnn_prep.cu) ----
 extern "C" int64_t b2cnn_prep_window_count(int64_t n_samples, double fs, const b2cnn_prep_config *cfg) {
     const int64_t n = prep_window_count(n_samples, fs, cfg);

@@ -319,7 +319,8 @@ double wire_parse_decimal_host(const char *s, int64_t len, int *status);
 // b2cnn_train.cu: one training step (row f4).  mode is B2CNN_MODE_*; every entry point checks all its arguments before
 // any CUDA call, then makes cfg->device current for the call (a negative device: the current one)
 // sl: the sequence lengths of a _seq call (mode is then B2CNN_MODE_SEQUENCE), or {false} for the calls that take a mode
-int64_t train_workspace_bytes(const b2cnn_config *cfg, int64_t B, const SeqLengths &sl, const RecordArgs &ra, int mode);
+// heads: 0 for the calls that train one model, K in [1, B2CNN_SLIDE_MAX_HEADS] for b2cnn_train_heads_*
+int64_t train_workspace_bytes(const b2cnn_config *cfg, int64_t B, const SeqLengths &sl, const RecordArgs &ra, int mode, int heads = 0);
 // weighted != 0: BCEWithLogitsLoss(pos_weight=pos_weight), else plain BCEWithLogitsLoss
 int train_step(const b2cnn_config *cfg, float *params, float *adam_m, float *adam_v, float *grads, int64_t step, float lr, float beta1,
                float beta2, float eps, int apply_update, const float *x, int64_t B, const float *age, const float *target,
@@ -331,6 +332,13 @@ int train_forward(const b2cnn_config *cfg, const float *params, const float *x, 
 int train_backward(const b2cnn_config *cfg, const float *params, const float *x, int64_t B, const float *age, int mode, const SeqLengths &sl,
                    const RecordArgs &ra, const float *mask1, const float *mask2, const float *dz, float *grads, float *dx, float *dage, int flags,
                    void *workspace, int64_t ws_bytes, cudaStream_t st, const char **err);
+// b2cnn_train_heads_step / _record: n_heads blobs on the conv weights of `frontend`; params, adam_m, adam_v, grads and lr
+// are host arrays of n_heads entries, loss_out a device array of n_heads floats
+int train_heads_step(const b2cnn_config *cfg, const float *frontend, int n_heads, float *const *params, float *const *adam_m,
+                     float *const *adam_v, float *const *grads, const float *lr, int64_t step, float beta1, float beta2, float eps,
+                     int apply_update, const float *x, int64_t B, const float *age, const float *target, int weighted, float pos_weight,
+                     int mode, const SeqLengths &sl, const RecordArgs &ra, const float *mask1, const float *mask2, float *loss_out,
+                     void *workspace, int64_t ws_bytes, cudaStream_t st, const char **err);
 
 void launch_transpose_wih(const float *wih0, float *wih0T, int L, cudaStream_t st);
 

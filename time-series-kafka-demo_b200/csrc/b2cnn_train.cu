@@ -36,6 +36,9 @@
 //   train_conv_grad_reduce sums the per-CTA partials in a fixed order (no atomic on a parameter gradient: gradients
 //                          repeat bit for bit)
 //   train_adam             torch.optim.Adam (no amsgrad, weight_decay 0) on the packed parameter blob
+// Candidate heads on one frozen front end (the train_heads_* entry points, train_heads_step at the end of this file):
+// the conv forward once, the *_heads kernels (projection and dW_ih_l0 two heads per CTA, Adam per head) and the scan
+// kernels with one grid row per head; no d f and no conv backward.
 // The head of the two LSTM kernels is a template parameter (Head): the fused step's BCE, BCE with pos_weight, or logits
 // only, with d loss / d z supplied by the caller (b2cnn_train_forward / b2cnn_train_backward, driven by torch autograd).
 // Everything below f is linear in d f, so the sum over tiles of what each tile back-propagates from its own features is
@@ -119,8 +122,11 @@ struct TrainPlan {
 // n_seq: the number of sequences of a _seq call, 0 for the calls that take a mode (their layout has no offsets region).
 // rd: a _record call's recording geometry, whose n_rec recordings the conv kernels run over; B is then the number of
 // counted windows (the scans' rows), and the layout gains the per-window d f [B][L] and the row offsets [n_rec + 1].
-static TrainPlan train_plan(const Dims &d, int64_t B, int64_t n_seq = 0, const Dims *rd = nullptr, int64_t n_rec = 0) {
+// heads: 0 for the calls that train one whole model; K >= 1 for a b2cnn_train_heads_* call, whose layout is f once and
+// K copies of every per-row region ([K][B][...], head-major), with no d f and no conv-gradient partials.
+static TrainPlan train_plan(const Dims &d, int64_t B, int64_t n_seq = 0, const Dims *rd = nullptr, int64_t n_rec = 0, int heads = 0) {
     TrainPlan pl{};
+    const int64_t K = heads > 0 ? heads : 1;
     const Dims &cd = rd ? *rd : d;                      // the conv kernels' geometry and rows
     const int64_t cb = rd ? n_rec : B;
     // consecutive sequences per scan CTA: ceil(n_seq / kSeqCtas), from (B, n_seq) alone, never the device
@@ -142,23 +148,23 @@ static TrainPlan train_plan(const Dims &d, int64_t B, int64_t n_seq = 0, const D
     int64_t p = 0;
     auto take = [&](int64_t n) { int64_t at = p; p += (n + 63) / 64 * 64; return at; };
     w.f = take(cb * cd.L);
-    w.pre0 = take(B * kGates);          // f . W_ih_l0^T
-    w.acts = take(B * 2 * kGates);      // [t][layer][i f g o] post-activation
-    w.cs = take(B * 2 * kHidden);       // [t][layer] cell state
-    w.hs = take(B * 2 * kHidden);       // [t][layer] hidden state
-    w.lin = take(B);                    // out(h1) before the age scale (d age needs it)
-    w.z = take(B);
-    w.da0 = take(B * kGates);           // d loss / d (layer-0 gate pre-activations)
-    w.dfeat = take(cb * cd.L);
+    w.pre0 = take(K * B * kGates);      // f . W_ih_l0^T
+    w.acts = take(K * B * 2 * kGates);  // [t][layer][i f g o] post-activation
+    w.cs = take(K * B * 2 * kHidden);   // [t][layer] cell state
+    w.hs = take(K * B * 2 * kHidden);   // [t][layer] hidden state
+    w.lin = take(K * B);                // out(h1) before the age scale (d age needs it)
+    w.z = take(K * B);
+    w.da0 = take(K * B * kGates);       // d loss / d (layer-0 gate pre-activations)
+    w.dfeat = take(heads ? 0 : cb * cd.L);
     // one region for the partial sums of three reductions that never overlap in time
-    int64_t part = (int64_t)pl.slices * B * kGates;
-    if ((int64_t)pl.wih_chunks * kGates * d.L > part) part = (int64_t)pl.wih_chunks * kGates * d.L;
-    if (pl.part_rows * pl.n_conv > part) part = pl.part_rows * pl.n_conv;
+    int64_t part = (int64_t)pl.slices * K * B * kGates;
+    if ((int64_t)pl.wih_chunks * K * kGates * d.L > part) part = (int64_t)pl.wih_chunks * K * kGates * d.L;
+    if (!heads && pl.part_rows * pl.n_conv > part) part = pl.part_rows * pl.n_conv;
     // the scan CTAs' head rows: written by the LSTM kernels and summed before any other reduction uses the region
-    if (pl.seq_ctas > 1 && pl.seq_ctas * head_row_len(blob_offsets(d)) > part) part = pl.seq_ctas * head_row_len(blob_offsets(d));
+    if (pl.seq_ctas > 1 && K * pl.seq_ctas * head_row_len(blob_offsets(d)) > part) part = K * pl.seq_ctas * head_row_len(blob_offsets(d));
     w.part = take(part);
     w.off = n_seq > 0 ? take(2 * (n_seq + 1)) : 0;     // int64 sequence offsets [n_seq + 1], copied in by every _seq call
-    w.dfw = rd ? take(B * d.L) : 0;                    // the windows' d f, folded into dfeat
+    w.dfw = rd && !heads ? take(B * d.L) : 0;          // the windows' d f, folded into dfeat
     w.roff = rd ? take(2 * (n_rec + 1)) : 0;           // int64 row offsets of the recordings, copied in by every _record call
     w.total = p;
     return pl;
@@ -218,6 +224,21 @@ __device__ __forceinline__ bool rec_reads(const RecRows &r, int64_t n, int s) {
     return w >= 0 && s < w * r.S + r.W;
 }
 
+// The heads the scans train: blockIdx.y = h reads head h's blob prm[h] and writes its gradients to grad[h].  The calls
+// that train one model launch gridDim.y = 1 with their blob at h = 0; a b2cnn_train_heads_* call launches one grid row
+// per head, and head h's per-row regions lie at h B rows into each region of the workspace.
+constexpr int kMaxHeads = B2CNN_SLIDE_MAX_HEADS;
+struct ScanHeads {
+    const float *prm[kMaxHeads];
+    float *grad[kMaxHeads];
+};
+// a b2cnn_train_heads_* call's blobs, Adam state and learning rates (host arrays copied into the kernel parameters)
+struct AdamHeads {
+    float *prm[kMaxHeads], *m[kMaxHeads], *v[kMaxHeads];
+    const float *grad[kMaxHeads];
+    float lr[kMaxHeads];
+};
+
 // The LSTM state of each recording of a _record_state call (RecordArgs), [nrec][64] = h0 | c0 | h1 | c1; every pointer
 // null for every other call.  A scan's sequence is a recording with windows, found from its first row in roff.
 struct ScanState {
@@ -244,14 +265,14 @@ __device__ __forceinline__ int64_t scan_recording(const ScanState &ss, int64_t m
 // computed before the scan (pre0[t][r]).  sequence == 0: every step starts from the zero state (independent windows).
 // A sequence starts from the zero state, or from its recording's row of ss.in, and with ss.out its final state is
 // stored there (STATE == false: ss is ignored, and the kernel compiles to the scan without it).  HEAD == kHeadLogits:
-// target and loss_out are not used.
+// target and loss_out are not used.  blockIdx.y: the head (ScanHeads), whose mean loss goes to loss_out[blockIdx.y].
 // ------------------------------------------------------------------------------------------------------------------
 template <int HEAD, bool STATE>
-__global__ void __launch_bounds__(64)
-train_lstm_fwd(const float *__restrict__ pre0, const float *__restrict__ prm, BlobOff o, Dims d, int64_t B, int sequence, SeqSpan sq,
-               const float *__restrict__ age, const float *__restrict__ target, float pos_weight, float *__restrict__ acts,
-               float *__restrict__ cs, float *__restrict__ hs, float *__restrict__ lin, float *__restrict__ z,
-               float *__restrict__ loss_out, ScanState ss) {
+__device__ __forceinline__ void
+lstm_fwd_body(const float *__restrict__ pre0, const float *__restrict__ prm, BlobOff o, Dims d, int64_t B, int sequence, SeqSpan sq,
+              const float *__restrict__ age, const float *__restrict__ target, float pos_weight, float *__restrict__ acts,
+              float *__restrict__ cs, float *__restrict__ hs, float *__restrict__ lin, float *__restrict__ z,
+              float *__restrict__ loss_out, ScanState ss) {
     if constexpr (!STATE) ss = ScanState{};
     __shared__ float g[kGates], h0[kHidden], c0[kHidden], h1[kHidden], c1s[kHidden];
     const int r = threadIdx.x;
@@ -358,14 +379,14 @@ train_lstm_fwd(const float *__restrict__ pre0, const float *__restrict__ prm, Bl
 // With ss.in, a sequence's first step reads its recording's initial state (h_{t-1}, c_{t-1}) there instead of zeros;
 // with ss.d_out, the carried d h / d c start from the gradient arriving at the final state instead of zeros; with
 // ss.d_in, the carries after the first step -- d loss / d (initial state) -- are stored there (STATE == false: as for
-// train_lstm_fwd).
+// train_lstm_fwd).  blockIdx.y: the head, as in train_lstm_fwd (dz_in and dage belong to gridDim.y = 1 launches).
 // ------------------------------------------------------------------------------------------------------------------
 template <int HEAD, bool STATE>
-__global__ void __launch_bounds__(64, 1)   // the 48 gradient sums stay in registers: no spill
-train_lstm_bwd(const float *__restrict__ prm, BlobOff o, Dims d, int64_t B, int sequence, SeqSpan sq, const float *__restrict__ age,
-               const float *__restrict__ target, float pos_weight, const float *__restrict__ dz_in, const float *__restrict__ acts,
-               const float *__restrict__ cs, const float *__restrict__ hs, const float *__restrict__ lin, const float *__restrict__ z,
-               float *__restrict__ da0, float *__restrict__ grad, float *__restrict__ dage, ScanState ss) {
+__device__ __forceinline__ void
+lstm_bwd_body(const float *__restrict__ prm, BlobOff o, Dims d, int64_t B, int sequence, SeqSpan sq, const float *__restrict__ age,
+              const float *__restrict__ target, float pos_weight, const float *__restrict__ dz_in, const float *__restrict__ acts,
+              const float *__restrict__ cs, const float *__restrict__ hs, const float *__restrict__ lin, const float *__restrict__ z,
+              float *__restrict__ da0, float *__restrict__ grad, float *__restrict__ dage, ScanState ss) {
     if constexpr (!STATE) ss = ScanState{};
     __shared__ float da[kGates], dh0c[kHidden], dc0c[kHidden], dh1c[kHidden], dc1c[kHidden], dh0ext[kHidden], dh1ext[kHidden];
     const int r = threadIdx.x, u = r & 15, q = r >> 4;
@@ -497,16 +518,44 @@ train_lstm_bwd(const float *__restrict__ prm, BlobOff o, Dims d, int64_t B, int 
     if (r == 0) gout[o.bo - base] = gbo;
 }
 
+// The scans of head blockIdx.y: its blob and gradients from hd, its rows of every per-row region at blockIdx.y B, its
+// loss at loss_out[blockIdx.y] and its CTAs' head rows after the previous head's.  The bodies take the pointers as
+// __restrict__ arguments, so the weights' loads are hoisted out of the scan as in a kernel of one model.
+template <int HEAD, bool STATE>
+__global__ void __launch_bounds__(64)
+train_lstm_fwd(const float *__restrict__ pre0, const __grid_constant__ ScanHeads hd, BlobOff o, Dims d, int64_t B, int sequence, SeqSpan sq,
+               const float *__restrict__ age, const float *__restrict__ target, float pos_weight, float *__restrict__ acts,
+               float *__restrict__ cs, float *__restrict__ hs, float *__restrict__ lin, float *__restrict__ z,
+               float *__restrict__ loss_out, ScanState ss) {
+    const int64_t hb = (int64_t)blockIdx.y * B;
+    if (sq.rows) sq.rows += (int64_t)blockIdx.y * gridDim.x * head_row_len(o);
+    lstm_fwd_body<HEAD, STATE>(pre0 + hb * kGates, hd.prm[blockIdx.y], o, d, B, sequence, sq, age, target, pos_weight, acts + hb * 2 * kGates,
+                               cs + hb * 2 * kHidden, hs + hb * 2 * kHidden, lin + hb, z + hb, loss_out ? loss_out + blockIdx.y : nullptr, ss);
+}
+template <int HEAD, bool STATE>
+__global__ void __launch_bounds__(64, 1)   // the 48 gradient sums stay in registers: no spill
+train_lstm_bwd(const __grid_constant__ ScanHeads hd, BlobOff o, Dims d, int64_t B, int sequence, SeqSpan sq, const float *__restrict__ age,
+               const float *__restrict__ target, float pos_weight, const float *__restrict__ dz_in, const float *__restrict__ acts,
+               const float *__restrict__ cs, const float *__restrict__ hs, const float *__restrict__ lin, const float *__restrict__ z,
+               float *__restrict__ da0, float *__restrict__ dage, ScanState ss) {
+    const int64_t hb = (int64_t)blockIdx.y * B;
+    if (sq.rows) sq.rows += (int64_t)blockIdx.y * gridDim.x * head_row_len(o);
+    lstm_bwd_body<HEAD, STATE>(hd.prm[blockIdx.y], o, d, B, sequence, sq, age, target, pos_weight, dz_in, acts + hb * 2 * kGates,
+                               cs + hb * 2 * kHidden, hs + hb * 2 * kHidden, lin + hb, z + hb, da0 + hb * kGates, hd.grad[blockIdx.y], dage, ss);
+}
+
 // grad[o.whh0 + e] = the sum of rows[c][e] over the scan CTAs c in order, i.e. in sequence order (no atomic: gradients
-// repeat bit for bit); the rows' last column is the loss sum, and loss_out (when not NULL) gets that sum / B
+// repeat bit for bit); the rows' last column is the loss sum, and loss_out (when not NULL) gets that sum / B.
+// blockIdx.y: the head, whose rows follow the previous head's and whose gradients go to hd.grad[blockIdx.y]
 __global__ void __launch_bounds__(256)
-train_head_reduce(const float *__restrict__ rows, int n_rows, BlobOff o, int64_t B, float *__restrict__ grad, float *__restrict__ loss_out) {
+train_head_reduce(const float *__restrict__ rows, int n_rows, BlobOff o, int64_t B, const __grid_constant__ ScanHeads hd, float *__restrict__ loss_out) {
     const int64_t len = head_row_len(o), e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (e >= len) return;
+    rows += (int64_t)blockIdx.y * n_rows * len;
     float a = rows[e];
     for (int c = 1; c < n_rows; ++c) a += rows[c * len + e];
-    if (e < len - 1) grad[o.whh0 + e] = a;
-    else if (loss_out) *loss_out = a / (float)B;
+    if (e < len - 1) hd.grad[blockIdx.y][o.whh0 + e] = a;
+    else if (loss_out) loss_out[blockIdx.y] = a / (float)B;
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -623,12 +672,16 @@ train_conv_fwd_record(const float *__restrict__ x, const float *__restrict__ prm
 
 // pre0 partial[slice][b][g] = sum over the slice's positions of f[b][p] W_ih_l0[g][p]: 64 windows x 64 gates per CTA,
 // K chunks of 32, a 4 x 4 register tile per thread (the tiling of the inference projection, reading W_ih_l0 as stored)
-// REC: row b is a window of a recording (rr), read in place from the recording's feature row
+// REC: row b is a window of a recording (rr), read in place from the recording's feature row.
+// HP heads per CTA: the f tile is staged once for all of them, head h multiplies it by its own W_ih_l0 wih0[h] into its
+// own accumulators (in the order of HP = 1) and writes partial[slice][b][g] at part[h] + slice pstride 64 (pstride = B
+// for one head; K B for K heads' partials laid out [slice][K][B][64])
 constexpr int kGemmK = 32, kGemmStride = 68;
-template <bool REC>
-__device__ __forceinline__ void train_pre0_partial_body(const float *__restrict__ f, const float *__restrict__ wih0, int64_t B, int L, float *__restrict__ part, const RecRows &rr) {
+template <bool REC, int HP>
+__device__ __forceinline__ void train_pre0_partial_body(const float *__restrict__ f, const float *const (&wih0)[HP], int64_t B, int64_t pstride,
+                                                        int L, float *const (&part)[HP], const RecRows &rr) {
     __shared__ __align__(16) float Fs[kGemmK][kGemmStride];
-    __shared__ __align__(16) float Ws[kGemmK][kGemmStride];
+    __shared__ __align__(16) float Ws[HP][kGemmK][kGemmStride];
     const int tid = threadIdx.x, tm = tid >> 4, tn = tid & 15;
     const int64_t b0 = (int64_t)blockIdx.x * 64;
     const int kbeg = blockIdx.y * kPre0Slice, kend = min(L, kbeg + kPre0Slice);
@@ -637,45 +690,77 @@ __device__ __forceinline__ void train_pre0_partial_body(const float *__restrict_
         if (tid < 64 && b0 + tid < B) row_at[tid] = rec_row_base(rr, b0 + tid);
         __syncthreads();
     }
-    float acc[4][4];
+    float acc[HP][4][4];
 #pragma unroll
-    for (int i = 0; i < 4; ++i)
+    for (int h = 0; h < HP; ++h)
 #pragma unroll
-        for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
+        for (int i = 0; i < 4; ++i)
+#pragma unroll
+            for (int j = 0; j < 4; ++j) acc[h][i][j] = 0.f;
     for (int k0 = kbeg; k0 < kend; k0 += kGemmK) {
 #pragma unroll
         for (int it = 0; it < 8; ++it) {
             const int e = tid + it * 256, m = e >> 5, kk = e & 31, k = k0 + kk;
             if constexpr (REC) Fs[kk][m] = (b0 + m < B && k < kend) ? f[row_at[m] + k] : 0.f;
             else Fs[kk][m] = (b0 + m < B && k < kend) ? f[(b0 + m) * L + k] : 0.f;
-            Ws[kk][m] = k < kend ? wih0[(int64_t)m * L + k] : 0.f;
+#pragma unroll
+            for (int h = 0; h < HP; ++h) Ws[h][kk][m] = k < kend ? wih0[h][(int64_t)m * L + k] : 0.f;
         }
         __syncthreads();
 #pragma unroll
         for (int kk = 0; kk < kGemmK; ++kk) {
             const float4 a = *reinterpret_cast<const float4 *>(&Fs[kk][4 * tm]);
-            const float4 w = *reinterpret_cast<const float4 *>(&Ws[kk][4 * tn]);
-            const float av[4] = {a.x, a.y, a.z, a.w}, wv[4] = {w.x, w.y, w.z, w.w};
+            const float av[4] = {a.x, a.y, a.z, a.w};
 #pragma unroll
-            for (int i = 0; i < 4; ++i)
+            for (int h = 0; h < HP; ++h) {
+                const float4 w = *reinterpret_cast<const float4 *>(&Ws[h][kk][4 * tn]);
+                const float wv[4] = {w.x, w.y, w.z, w.w};
 #pragma unroll
-                for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(av[i], wv[j], acc[i][j]);
+                for (int i = 0; i < 4; ++i)
+#pragma unroll
+                    for (int j = 0; j < 4; ++j) acc[h][i][j] = fmaf(av[i], wv[j], acc[h][i][j]);
+            }
         }
         __syncthreads();
     }
 #pragma unroll
-    for (int i = 0; i < 4; ++i) {
-        const int64_t b = b0 + 4 * tm + i;
-        if (b < B) *reinterpret_cast<float4 *>(part + ((int64_t)blockIdx.y * B + b) * kGates + 4 * tn) = make_float4(acc[i][0], acc[i][1], acc[i][2], acc[i][3]);
-    }
+    for (int h = 0; h < HP; ++h)
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const int64_t b = b0 + 4 * tm + i;
+            if (b < B)
+                *reinterpret_cast<float4 *>(part[h] + ((int64_t)blockIdx.y * pstride + b) * kGates + 4 * tn) =
+                    make_float4(acc[h][i][0], acc[h][i][1], acc[h][i][2], acc[h][i][3]);
+        }
 }
 __global__ void __launch_bounds__(256)
 train_pre0_partial(const float *__restrict__ f, const float *__restrict__ wih0, int64_t B, int L, float *__restrict__ part) {
-    train_pre0_partial_body<false>(f, wih0, B, L, part, RecRows{});
+    const float *const w[1] = {wih0};
+    float *const p[1] = {part};
+    train_pre0_partial_body<false, 1>(f, w, B, B, L, p, RecRows{});
 }
 __global__ void __launch_bounds__(256)
 train_pre0_partial_record(const float *__restrict__ f, const float *__restrict__ wih0, int64_t B, int L, float *__restrict__ part, RecRows rr) {
-    train_pre0_partial_body<true>(f, wih0, B, L, part, rr);
+    const float *const w[1] = {wih0};
+    float *const p[1] = {part};
+    train_pre0_partial_body<true, 1>(f, w, B, B, L, p, rr);
+}
+// The K heads of a b2cnn_train_heads_* call, kPre0Heads per CTA on gridDim.z: CTA z projects heads 2z and 2z + 1 into
+// their slots of part [slice][K][B][64].  With an odd K the last CTA's second head is its first again: it computes the
+// same partials twice and stores the same bits to the same place.
+constexpr int kPre0Heads = 2;
+template <bool REC>
+__global__ void __launch_bounds__(256)
+train_pre0_partial_heads(const float *__restrict__ f, const __grid_constant__ ScanHeads hd, int n_heads, BlobOff o, int64_t B, int L, float *__restrict__ part, RecRows rr) {
+    const float *w[kPre0Heads];
+    float *p[kPre0Heads];
+#pragma unroll
+    for (int i = 0; i < kPre0Heads; ++i) {
+        const int h = min((int)blockIdx.z * kPre0Heads + i, n_heads - 1);
+        w[i] = hd.prm[h] + o.wih0;
+        p[i] = part + (int64_t)h * B * kGates;
+    }
+    train_pre0_partial_body<REC, kPre0Heads>(f, w, B, (int64_t)n_heads * B, L, p, rr);
 }
 
 // out[e] = part[0][e] + part[1][e] + ... in that order (split-K slices of pre0, batch chunks of dW_ih_l0)
@@ -689,20 +774,26 @@ __global__ void train_sum_chunks(const float *__restrict__ part, int n_chunks, i
 
 // dW_ih_l0 partial[chunk][g][p] = sum over the chunk's windows t (ascending) of da0[t][g] f[t][p].  Thread = position p
 // with the 64 gate rows' sums in registers, so f is read once; grid (position tiles of 128, batch chunks).  REC: window t
-// is read in place from its recording's feature row (rr).
-template <bool REC>
-__device__ __forceinline__ void train_wih0_grad_body(const float *__restrict__ da0, const float *__restrict__ f, int64_t B, int L, int chunk, float *__restrict__ part, const RecRows &rr) {
-    __shared__ __align__(16) float sda[kRowBatch * kGates];
+// is read in place from its recording's feature row (rr).  HP heads per CTA: f is read once per position for all of
+// them, head h's sums (in the order of HP = 1) come from its own da0[h] and go to part[h].
+template <bool REC, int HP>
+__device__ __forceinline__ void train_wih0_grad_body(const float *const (&da0)[HP], const float *__restrict__ f, int64_t B, int L, int chunk,
+                                                     float *const (&part)[HP], const RecRows &rr) {
+    __shared__ __align__(16) float sda[HP][kRowBatch * kGates];
     [[maybe_unused]] __shared__ int64_t row_at[REC ? kRowBatch : 1];
     const int p = blockIdx.x * 128 + threadIdx.x;
     const int64_t t0 = (int64_t)blockIdx.y * chunk, t1 = min(B, t0 + chunk);
-    float acc[kGates];
+    float acc[HP][kGates];
 #pragma unroll
-    for (int g = 0; g < kGates; ++g) acc[g] = 0.f;
+    for (int h = 0; h < HP; ++h)
+#pragma unroll
+        for (int g = 0; g < kGates; ++g) acc[h][g] = 0.f;
     for (int64_t tb = t0; tb < t1; tb += kRowBatch) {
         const int rows = (int)min((int64_t)kRowBatch, t1 - tb);
         __syncthreads();
-        for (int e = threadIdx.x; e < rows * kGates; e += 128) sda[e] = da0[tb * kGates + e];
+        for (int e = threadIdx.x; e < rows * kGates; e += 128)
+#pragma unroll
+            for (int h = 0; h < HP; ++h) sda[h][e] = da0[h][tb * kGates + e];
         if constexpr (REC) {
             if (threadIdx.x < rows) row_at[threadIdx.x] = rec_row_base(rr, tb + threadIdx.x);
         }
@@ -713,24 +804,64 @@ __device__ __forceinline__ void train_wih0_grad_body(const float *__restrict__ d
                 if constexpr (REC) fv = f[row_at[r] + p];
                 else fv = f[(tb + r) * L + p];
 #pragma unroll
-                for (int g4 = 0; g4 < kGates / 4; ++g4) {
-                    const float4 a = *reinterpret_cast<const float4 *>(sda + r * kGates + 4 * g4);
-                    acc[4 * g4 + 0] = fmaf(a.x, fv, acc[4 * g4 + 0]); acc[4 * g4 + 1] = fmaf(a.y, fv, acc[4 * g4 + 1]);
-                    acc[4 * g4 + 2] = fmaf(a.z, fv, acc[4 * g4 + 2]); acc[4 * g4 + 3] = fmaf(a.w, fv, acc[4 * g4 + 3]);
-                }
+                for (int h = 0; h < HP; ++h)
+#pragma unroll
+                    for (int g4 = 0; g4 < kGates / 4; ++g4) {
+                        const float4 a = *reinterpret_cast<const float4 *>(sda[h] + r * kGates + 4 * g4);
+                        acc[h][4 * g4 + 0] = fmaf(a.x, fv, acc[h][4 * g4 + 0]); acc[h][4 * g4 + 1] = fmaf(a.y, fv, acc[h][4 * g4 + 1]);
+                        acc[h][4 * g4 + 2] = fmaf(a.z, fv, acc[h][4 * g4 + 2]); acc[h][4 * g4 + 3] = fmaf(a.w, fv, acc[h][4 * g4 + 3]);
+                    }
             }
     }
     if (p < L)
 #pragma unroll
-        for (int g = 0; g < kGates; ++g) part[((int64_t)blockIdx.y * kGates + g) * L + p] = acc[g];
+        for (int h = 0; h < HP; ++h)
+#pragma unroll
+            for (int g = 0; g < kGates; ++g) part[h][((int64_t)blockIdx.y * kGates + g) * L + p] = acc[h][g];
 }
 __global__ void __launch_bounds__(128)
 train_wih0_grad(const float *__restrict__ da0, const float *__restrict__ f, int64_t B, int L, int chunk, float *__restrict__ part) {
-    train_wih0_grad_body<false>(da0, f, B, L, chunk, part, RecRows{});
+    const float *const a[1] = {da0};
+    float *const p[1] = {part};
+    train_wih0_grad_body<false, 1>(a, f, B, L, chunk, p, RecRows{});
 }
 __global__ void __launch_bounds__(128)
 train_wih0_grad_record(const float *__restrict__ da0, const float *__restrict__ f, int64_t B, int L, int chunk, float *__restrict__ part, RecRows rr) {
-    train_wih0_grad_body<true>(da0, f, B, L, chunk, part, rr);
+    const float *const a[1] = {da0};
+    float *const p[1] = {part};
+    train_wih0_grad_body<true, 1>(a, f, B, L, chunk, p, rr);
+}
+// The K heads of a b2cnn_train_heads_* call, kWihHeads per CTA on gridDim.z (an odd K's last CTA repeats its head, as
+// train_pre0_partial_heads does).  Head h reads its da0 at h B rows; with one batch chunk its sums go straight to its
+// gradient blob, else to its slot of part [K][chunks][64][L].  The CTAs of the first position tile and chunk also zero
+// their heads' conv entries of the gradient blob: the front end is frozen.
+constexpr int kWihHeads = 2;
+template <bool REC>
+__global__ void __launch_bounds__(128)
+train_wih0_grad_heads(const float *__restrict__ da0, const float *__restrict__ f, const __grid_constant__ ScanHeads hd, int n_heads, BlobOff o, int64_t B, int L,
+                      int chunk, int n_chunks, float *__restrict__ part, RecRows rr) {
+    const float *a[kWihHeads];
+    float *p[kWihHeads];
+#pragma unroll
+    for (int i = 0; i < kWihHeads; ++i) {
+        const int h = min((int)blockIdx.z * kWihHeads + i, n_heads - 1);
+        a[i] = da0 + (int64_t)h * B * kGates;
+        p[i] = n_chunks > 1 ? part + (int64_t)h * n_chunks * kGates * L : hd.grad[h] + o.wih0;
+        if (blockIdx.x == 0 && blockIdx.y == 0)
+            for (int e = threadIdx.x; e < o.wih0; e += 128) hd.grad[h][e] = 0.f;
+    }
+    train_wih0_grad_body<REC, kWihHeads>(a, f, B, L, chunk, p, rr);
+}
+
+// dW_ih_l0 of head blockIdx.y = the sum of its batch-chunk partials in chunk order (train_sum_chunks per head)
+__global__ void __launch_bounds__(256)
+train_wih0_sum_heads(const float *__restrict__ part, int n_chunks, int64_t n, const __grid_constant__ ScanHeads hd, BlobOff o) {
+    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= n) return;
+    part += (int64_t)blockIdx.y * n_chunks * n;
+    float a = part[e];
+    for (int c = 1; c < n_chunks; ++c) a += part[(int64_t)c * n + e];
+    hd.grad[blockIdx.y][o.wih0 + e] = a;
 }
 
 // d f[t][p] = sum_g da0[t][g] W_ih_l0[g][p], g ascending; thread = position p with its 64 weights in registers, grid
@@ -950,6 +1081,19 @@ __global__ void train_adam(float *__restrict__ prm, float *__restrict__ m, float
     const float denom = sqrtf(vv) / bc2_sqrt + eps;
     prm[e] = prm[e] - (lr / bc1) * (mm / denom);
 }
+// train_adam on the blob entries [o.wih0, o.total) of head blockIdx.y, with its own learning rate
+__global__ void train_adam_heads(const __grid_constant__ AdamHeads ah, BlobOff o, float b1, float b2, float eps, float bc1, float bc2_sqrt) {
+    const int64_t e = o.wih0 + (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= o.total) return;
+    const int h = blockIdx.y;
+    float *__restrict__ prm = ah.prm[h], *__restrict__ m = ah.m[h], *__restrict__ v = ah.v[h];
+    const float g = ah.grad[h][e], lr = ah.lr[h];
+    const float mm = m[e] + (g - m[e]) * (1.f - b1);
+    const float vv = b2 * v[e] + (1.f - b2) * g * g;
+    m[e] = mm; v[e] = vv;
+    const float denom = sqrtf(vv) / bc2_sqrt + eps;
+    prm[e] = prm[e] - (lr / bc1) * (mm / denom);
+}
 
 // the geometry of a configuration, refusing what the training kernels do not cover; no CUDA call
 static bool train_geometry(const b2cnn_config *cfg, Dims &d, const char **err) {
@@ -1010,14 +1154,15 @@ static bool plan_fits(const Dims &cd, const TrainPlan &pl, int64_t B, const char
     return true;
 }
 
-int64_t train_workspace_bytes(const b2cnn_config *cfg, int64_t B, const SeqLengths &sl, const RecordArgs &ra, int mode) {
+int64_t train_workspace_bytes(const b2cnn_config *cfg, int64_t B, const SeqLengths &sl, const RecordArgs &ra, int mode, int heads) {
     Dims d;
     const char *err = "";
     std::vector<int64_t> off;
     Rec rec;
+    if (heads < 0 || heads > kMaxHeads) return -1;
     if (B < 1 || !train_geometry(cfg, d, &err) || (sl.on && !seq_offsets(sl, B, off, &err))) return -1;
     if (ra.on && ((mode != B2CNN_MODE_INDEPENDENT && mode != B2CNN_MODE_SEQUENCE) || !record_rows(*cfg, d, B, mode, ra, rec, off, &err))) return -1;
-    const TrainPlan pl = train_plan(d, ra.on ? rec.rows : B, off.empty() ? 0 : (int64_t)off.size() - 1, ra.on ? &rec.rd : nullptr, B);
+    const TrainPlan pl = train_plan(d, ra.on ? rec.rows : B, off.empty() ? 0 : (int64_t)off.size() - 1, ra.on ? &rec.rd : nullptr, B, heads);
     if (ra.on && !plan_fits(rec.rd, pl, B, &err)) return -1;      // a shape the _record calls refuse has no workspace
     return pl.w.total * (int64_t)sizeof(float);
 }
@@ -1086,7 +1231,7 @@ static bool launch_backward_tail(const Dims &d, const Dims &cd, const BlobOff &o
 // needs (ptrs_ok) and the batch, the sequence lengths of a _seq call (into off), the windows of a _record call (into rec
 // and off), what the kernels hold, and the workspace size.
 static int train_args(const b2cnn_config *cfg, int64_t B, int mode, const SeqLengths &sl, const RecordArgs &ra, bool ptrs_ok,
-                      int64_t ws_bytes, Dims &d, TrainPlan &pl, std::vector<int64_t> &off, Rec &rec, const char **err) {
+                      int64_t ws_bytes, Dims &d, TrainPlan &pl, std::vector<int64_t> &off, Rec &rec, const char **err, int heads = 0) {
     if (!train_geometry(cfg, d, err)) return B2CNN_EINVAL;
     if (mode != B2CNN_MODE_INDEPENDENT && mode != B2CNN_MODE_SEQUENCE) { *err = "training: bad mode"; return B2CNN_EINVAL; }
     if (!ptrs_ok || B < 1) { *err = "training: null argument / bad batch"; return B2CNN_EINVAL; }
@@ -1095,10 +1240,12 @@ static int train_args(const b2cnn_config *cfg, int64_t B, int mode, const SeqLen
     if (ra.has_state() && (!ra.on || mode != B2CNN_MODE_SEQUENCE)) { *err = "training: an LSTM state needs sequence mode"; return B2CNN_EINVAL; }
     if (ra.states_overlap(B)) { *err = "training: the LSTM state arrays overlap"; return B2CNN_EINVAL; }
     if (!ra.on) rec.rows = B;
-    pl = train_plan(d, rec.rows, off.empty() ? 0 : (int64_t)off.size() - 1, ra.on ? &rec.rd : nullptr, B);
+    pl = train_plan(d, rec.rows, off.empty() ? 0 : (int64_t)off.size() - 1, ra.on ? &rec.rd : nullptr, B, heads);
     if (!plan_fits(ra.on ? rec.rd : d, pl, B, err)) return B2CNN_EINVAL;
     if (ws_bytes < pl.w.total * (int64_t)sizeof(float)) {
-        *err = ra.on ? "training: workspace smaller than b2cnn_train_workspace_bytes_record()"
+        *err = heads ? (ra.on ? "training: workspace smaller than b2cnn_train_heads_workspace_bytes_record()"
+                              : "training: workspace smaller than b2cnn_train_heads_workspace_bytes()")
+             : ra.on ? "training: workspace smaller than b2cnn_train_workspace_bytes_record()"
              : sl.on ? "training: workspace smaller than b2cnn_train_workspace_bytes_seq()" : "training: workspace smaller than b2cnn_train_workspace_bytes()";
         return B2CNN_ESTATE;
     }
@@ -1116,11 +1263,19 @@ static bool seq_span(const TrainPlan &pl, const std::vector<int64_t> &off, float
     return true;
 }
 
+// the scans' view of the one model a call trains (gridDim.y = 1)
+static ScanHeads one_head(const float *params, float *grads) {
+    ScanHeads hd{};
+    hd.prm[0] = params;
+    hd.grad[0] = grads;
+    return hd;
+}
+
 // with more than one scan CTA: the head's gradients (and, with loss_out, the mean loss) from the CTAs' rows
 static void launch_head_reduce(const TrainPlan &pl, const BlobOff &o, const SeqSpan &sq, int64_t B, float *grads, float *loss_out,
                                cudaStream_t st) {
     if (!sq.rows) return;
-    train_head_reduce<<<(unsigned)((head_row_len(o) + 255) / 256), 256, 0, st>>>(sq.rows, pl.seq_ctas, o, B, grads, loss_out);
+    train_head_reduce<<<(unsigned)((head_row_len(o) + 255) / 256), 256, 0, st>>>(sq.rows, pl.seq_ctas, o, B, one_head(nullptr, grads), loss_out);
 }
 
 // The row addressing of a _record call over its B recordings; it first copies the row offsets into the workspace (from
@@ -1136,12 +1291,12 @@ static bool record_span(const TrainPlan &pl, const Rec &rec, const Dims &d, int6
 
 // the scan kernels of one HEAD, the STATE instance for a call with states
 template <int HEAD, typename... A>
-static void lstm_fwd(unsigned grid, cudaStream_t st, bool state, A... a) {
+static void lstm_fwd(dim3 grid, cudaStream_t st, bool state, A... a) {
     if (state) train_lstm_fwd<HEAD, true><<<grid, 64, 0, st>>>(a...);
     else train_lstm_fwd<HEAD, false><<<grid, 64, 0, st>>>(a...);
 }
 template <int HEAD, typename... A>
-static void lstm_bwd(unsigned grid, cudaStream_t st, bool state, A... a) {
+static void lstm_bwd(dim3 grid, cudaStream_t st, bool state, A... a) {
     if (state) train_lstm_bwd<HEAD, true><<<grid, 64, 0, st>>>(a...);
     else train_lstm_bwd<HEAD, false><<<grid, 64, 0, st>>>(a...);
 }
@@ -1205,16 +1360,17 @@ int train_step(const b2cnn_config *cfg, float *params, float *adam_m, float *ada
     if (!pass_state(ra.state_out, ra.state_in, B, st)) { *err = "copy of the LSTM state"; return B2CNN_ECUDA; }
     const bool on = ra.has_state();
     const float *const nul = nullptr;
+    const ScanHeads hd = one_head(params, grads);
     if (weighted) {
-        lstm_fwd<kHeadBcePw>(scans, st, on, ws + w.pre0, params, o, d, R, sequence, sq, age, target, pos_weight, ws + w.acts, ws + w.cs,
+        lstm_fwd<kHeadBcePw>(scans, st, on, ws + w.pre0, hd, o, d, R, sequence, sq, age, target, pos_weight, ws + w.acts, ws + w.cs,
                              ws + w.hs, ws + w.lin, ws + w.z, loss_out, ss);
-        lstm_bwd<kHeadBcePw>(scans, st, on, params, o, d, R, sequence, sq, age, target, pos_weight, nul, ws + w.acts, ws + w.cs, ws + w.hs,
-                             ws + w.lin, ws + w.z, ws + w.da0, grads, (float *)nullptr, ss);
+        lstm_bwd<kHeadBcePw>(scans, st, on, hd, o, d, R, sequence, sq, age, target, pos_weight, nul, ws + w.acts, ws + w.cs, ws + w.hs,
+                             ws + w.lin, ws + w.z, ws + w.da0, (float *)nullptr, ss);
     } else {
-        lstm_fwd<kHeadBce>(scans, st, on, ws + w.pre0, params, o, d, R, sequence, sq, age, target, 1.f, ws + w.acts, ws + w.cs, ws + w.hs,
+        lstm_fwd<kHeadBce>(scans, st, on, ws + w.pre0, hd, o, d, R, sequence, sq, age, target, 1.f, ws + w.acts, ws + w.cs, ws + w.hs,
                            ws + w.lin, ws + w.z, loss_out, ss);
-        lstm_bwd<kHeadBce>(scans, st, on, params, o, d, R, sequence, sq, age, target, 1.f, nul, ws + w.acts, ws + w.cs, ws + w.hs,
-                           ws + w.lin, ws + w.z, ws + w.da0, grads, (float *)nullptr, ss);
+        lstm_bwd<kHeadBce>(scans, st, on, hd, o, d, R, sequence, sq, age, target, 1.f, nul, ws + w.acts, ws + w.cs, ws + w.hs,
+                           ws + w.lin, ws + w.z, ws + w.da0, (float *)nullptr, ss);
     }
     launch_head_reduce(pl, o, sq, R, grads, loss_out, st);
     if (!backward_tail(d, rec, o, pl, ws, params, x, B, mask1, mask2, grads, nullptr, false, rr, st)) { *err = "memset dx"; return B2CNN_ECUDA; }
@@ -1248,7 +1404,7 @@ int train_forward(const b2cnn_config *cfg, const float *params, const float *x, 
     if (!record_span(pl, rec, d, B, ws, st, rr)) { *err = "copy row offsets"; return B2CNN_ECUDA; }
     conv_forward(d, rec, o, pl, ws, params, x, B, mask1, mask2, rr, st);
     if (!pass_state(ra.state_out, ra.state_in, B, st)) { *err = "copy of the LSTM state"; return B2CNN_ECUDA; }
-    lstm_fwd<kHeadLogits>((unsigned)pl.seq_ctas, st, ra.has_state(), ws + w.pre0, params, o, d, rec.rows, sequence, sq, age,
+    lstm_fwd<kHeadLogits>((unsigned)pl.seq_ctas, st, ra.has_state(), ws + w.pre0, one_head(params, nullptr), o, d, rec.rows, sequence, sq, age,
                           (const float *)nullptr, 1.f, ws + w.acts, ws + w.cs, ws + w.hs, ws + w.lin, z_out, (float *)nullptr,
                           scan_state(ra, rr));
     cudaError_t e = cudaGetLastError();
@@ -1281,11 +1437,123 @@ int train_backward(const b2cnn_config *cfg, const float *params, const float *x,
     // zeroed: a frozen front end leaves the conv entries as they are
     if (cudaMemsetAsync(grads, 0, sizeof(float) * o.total, st) != cudaSuccess) { *err = "memset grads"; return B2CNN_ECUDA; }
     if (!pass_state(ra.d_state_in, ra.d_state_out, B, st)) { *err = "copy of the LSTM state gradient"; return B2CNN_ECUDA; }
-    lstm_bwd<kHeadLogits>((unsigned)pl.seq_ctas, st, ra.has_state(), params, o, d, rec.rows, sequence, sq, age, (const float *)nullptr, 1.f,
-                          dz, ws + w.acts, ws + w.cs, ws + w.hs, ws + w.lin, (const float *)nullptr, ws + w.da0, grads, dage,
+    lstm_bwd<kHeadLogits>((unsigned)pl.seq_ctas, st, ra.has_state(), one_head(params, grads), o, d, rec.rows, sequence, sq, age,
+                          (const float *)nullptr, 1.f, dz, ws + w.acts, ws + w.cs, ws + w.hs, ws + w.lin, (const float *)nullptr, ws + w.da0, dage,
                           scan_state(ra, rr));
     launch_head_reduce(pl, o, sq, rec.rows, grads, nullptr, st);
     if (!backward_tail(d, rec, o, pl, ws, params, x, B, mask1, mask2, grads, dx, frozen_conv, rr, st)) { *err = "memset dx"; return B2CNN_ECUDA; }
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) { *err = cudaGetErrorString(e); return B2CNN_ECUDA; }
+    return B2CNN_OK;
+}
+
+}  // namespace b2cnn
+
+namespace b2cnn {
+
+// K candidate heads on one frozen front end (b2cnn_train_heads_step / _record, include/b2cnn.h): the conv forward once
+// on the front end's conv weights, then every later kernel of the fused step with a head axis -- the projection and
+// dW_ih_l0 two heads per CTA on gridDim.z, the scans and their reductions one grid row per head, Adam over every head's
+// entries from W_ih_l0 on -- and no conv backward.  Head h computes the bits b2cnn_train_step computes for its blob:
+// every sum it makes is the fused step's, in the fused step's order.  The launch list does not depend on K.
+int train_heads_step(const b2cnn_config *cfg, const float *frontend, int n_heads, float *const *params, float *const *adam_m,
+                     float *const *adam_v, float *const *grads, const float *lr, int64_t step, float beta1, float beta2, float eps,
+                     int apply_update, const float *x, int64_t B, const float *age, const float *target, int weighted, float pos_weight,
+                     int mode, const SeqLengths &sl, const RecordArgs &ra, const float *mask1, const float *mask2, float *loss_out,
+                     void *workspace, int64_t ws_bytes, cudaStream_t st, const char **err) {
+    if (n_heads < 1 || n_heads > kMaxHeads) { *err = "training: n_heads must be in [1, B2CNN_SLIDE_MAX_HEADS = 8]"; return B2CNN_EINVAL; }
+    if (!params || !grads || !lr || (apply_update && (!adam_m || !adam_v))) { *err = "training: null head array"; return B2CNN_EINVAL; }
+    Dims d;
+    if (!train_geometry(cfg, d, err)) return B2CNN_EINVAL;
+    const BlobOff o = blob_offsets(d);
+    // every array a head writes: its blob, its gradients and (with an update) its Adam state, none shared with another's
+    std::vector<const float *> arrays;
+    for (int h = 0; h < n_heads; ++h) {
+        if (!params[h] || !grads[h] || (apply_update && (!adam_m[h] || !adam_v[h]))) { *err = "training: null head pointer"; return B2CNN_EINVAL; }
+        arrays.push_back(params[h]);
+        arrays.push_back(grads[h]);
+        if (apply_update) { arrays.push_back(adam_m[h]); arrays.push_back(adam_v[h]); }
+    }
+    for (size_t i = 0; i < arrays.size(); ++i)
+        for (size_t j = i + 1; j < arrays.size(); ++j)
+            if (arrays[i] < arrays[j] + o.total && arrays[j] < arrays[i] + o.total) {
+                *err = "training: two heads share a blob (or a head's blob, gradients and Adam state overlap)";
+                return B2CNN_EINVAL;
+            }
+    TrainPlan pl;
+    std::vector<int64_t> off;
+    Rec rec;
+    const int rc = train_args(cfg, B, mode, sl, ra, frontend && x && age && target && loss_out && workspace, ws_bytes, d, pl, off, rec, err, n_heads);
+    if (rc != B2CNN_OK) return rc;
+    if (ra.has_state()) { *err = "training: heads carry no LSTM state"; return B2CNN_EINVAL; }
+    if (step < 1) { *err = "training: step must be >= 1"; return B2CNN_EINVAL; }
+    if (weighted && !(pos_weight > 0.f && pos_weight <= FLT_MAX)) { *err = "training: pos_weight must be positive and finite"; return B2CNN_EINVAL; }
+    DeviceGuard dev(cfg->device);
+    if (dev.err != cudaSuccess) { *err = "cudaSetDevice"; return B2CNN_ECUDA; }
+    const TrainWs &w = pl.w;
+    const int sequence = mode == B2CNN_MODE_SEQUENCE ? 1 : 0;
+    const int64_t R = rec.rows;
+    float *ws = reinterpret_cast<float *>(workspace);
+    SeqSpan sq;
+    if (!seq_span(pl, off, ws, st, sq)) { *err = "copy sequence offsets"; return B2CNN_ECUDA; }
+    RecRows rr;
+    if (!record_span(pl, rec, d, B, ws, st, rr)) { *err = "copy row offsets"; return B2CNN_ECUDA; }
+    ScanHeads hd{};
+    AdamHeads ah{};
+    for (int h = 0; h < n_heads; ++h) {
+        hd.prm[h] = ah.prm[h] = params[h];
+        hd.grad[h] = grads[h];
+        ah.grad[h] = grads[h];
+        ah.m[h] = apply_update ? adam_m[h] : nullptr;
+        ah.v[h] = apply_update ? adam_v[h] : nullptr;
+        ah.lr[h] = lr[h];
+    }
+    // the front end once, then every head's layer-0 pre-activations
+    const Dims &cd = rec.on ? rec.rd : d;
+    const dim3 conv((unsigned)(B * pl.tiles)), proj((unsigned)((R + 63) / 64), (unsigned)pl.slices, (unsigned)((n_heads + kPre0Heads - 1) / kPre0Heads));
+    float *const pre0 = ws + (pl.slices > 1 ? w.part : w.pre0);
+    if (rec.on) {
+        if (pl.smem_fwd > 48 * 1024) cudaFuncSetAttribute(train_conv_fwd_record, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.smem_fwd);
+        train_conv_fwd_record<<<conv, kThreads, pl.smem_fwd, st>>>(x, frontend, o, cd, pl.tiles, mask1, mask2, ws + w.f, rr);
+        train_pre0_partial_heads<true><<<proj, 256, 0, st>>>(ws + w.f, hd, n_heads, o, R, d.L, pre0, rr);
+    } else {
+        if (pl.smem_fwd > 48 * 1024) cudaFuncSetAttribute(train_conv_fwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.smem_fwd);
+        train_conv_fwd<<<conv, kThreads, pl.smem_fwd, st>>>(x, frontend, o, cd, pl.tiles, mask1, mask2, ws + w.f);
+        train_pre0_partial_heads<false><<<proj, 256, 0, st>>>(ws + w.f, hd, n_heads, o, R, d.L, pre0, rr);
+    }
+    if (pl.slices > 1) {
+        const int64_t n = (int64_t)n_heads * R * kGates;
+        train_sum_chunks<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(ws + w.part, pl.slices, n, ws + w.pre0);
+    }
+    // the K heads' scans side by side
+    const dim3 scans((unsigned)pl.seq_ctas, (unsigned)n_heads);
+    const float *const nul = nullptr;
+    if (weighted) {
+        lstm_fwd<kHeadBcePw>(scans, st, false, ws + w.pre0, hd, o, d, R, sequence, sq, age, target, pos_weight, ws + w.acts, ws + w.cs,
+                             ws + w.hs, ws + w.lin, ws + w.z, loss_out, ScanState{});
+        lstm_bwd<kHeadBcePw>(scans, st, false, hd, o, d, R, sequence, sq, age, target, pos_weight, nul, ws + w.acts, ws + w.cs, ws + w.hs,
+                             ws + w.lin, ws + w.z, ws + w.da0, (float *)nullptr, ScanState{});
+    } else {
+        lstm_fwd<kHeadBce>(scans, st, false, ws + w.pre0, hd, o, d, R, sequence, sq, age, target, 1.f, ws + w.acts, ws + w.cs, ws + w.hs,
+                           ws + w.lin, ws + w.z, loss_out, ScanState{});
+        lstm_bwd<kHeadBce>(scans, st, false, hd, o, d, R, sequence, sq, age, target, 1.f, nul, ws + w.acts, ws + w.cs, ws + w.hs,
+                           ws + w.lin, ws + w.z, ws + w.da0, (float *)nullptr, ScanState{});
+    }
+    if (sq.rows)
+        train_head_reduce<<<dim3((unsigned)((head_row_len(o) + 255) / 256), (unsigned)n_heads), 256, 0, st>>>(sq.rows, pl.seq_ctas, o, R, hd, loss_out);
+    // dW_ih_l0 (and the zeroed conv entries), then Adam
+    const int64_t n1 = (int64_t)kGates * d.L;
+    const dim3 wgrid((unsigned)((d.L + 127) / 128), (unsigned)pl.wih_chunks, (unsigned)((n_heads + kWihHeads - 1) / kWihHeads));
+    if (rec.on)
+        train_wih0_grad_heads<true><<<wgrid, 128, 0, st>>>(ws + w.da0, ws + w.f, hd, n_heads, o, R, d.L, pl.wih_chunk, pl.wih_chunks, ws + w.part, rr);
+    else
+        train_wih0_grad_heads<false><<<wgrid, 128, 0, st>>>(ws + w.da0, ws + w.f, hd, n_heads, o, R, d.L, pl.wih_chunk, pl.wih_chunks, ws + w.part, rr);
+    if (pl.wih_chunks > 1)
+        train_wih0_sum_heads<<<dim3((unsigned)((n1 + 255) / 256), (unsigned)n_heads), 256, 0, st>>>(ws + w.part, pl.wih_chunks, n1, hd, o);
+    if (apply_update) {
+        const float bc1 = 1.f - powf(beta1, (float)step), bc2 = 1.f - powf(beta2, (float)step);
+        train_adam_heads<<<dim3((unsigned)((o.total - o.wih0 + 255) / 256), (unsigned)n_heads), 256, 0, st>>>(ah, o, beta1, beta2, eps, bc1, sqrtf(bc2));
+    }
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) { *err = cudaGetErrorString(e); return B2CNN_ECUDA; }
     return B2CNN_OK;

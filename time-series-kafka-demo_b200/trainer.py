@@ -27,14 +27,14 @@ from __future__ import annotations
 
 import ctypes
 import math
-from typing import Dict, Optional, Tuple
+from typing import Dict, List, Optional, Tuple
 
 import torch
 
 from . import capi
 from .arch import BLOB_KEYS
 from .autograd import check_masks, check_record_batch, check_trainable, draw_masks, window_ages
-from .model import B200MyCNN, check_record_state
+from .model import B200MyCNN, check_head_models, check_record_state
 
 
 class B200Trainer:
@@ -199,3 +199,184 @@ class B200Trainer:
                     sd[k].copy_(v)
             self.model.sync_weights()
         return self._loss[0].clone()
+
+
+class B200HeadTrainer:
+    """Train up to 8 candidate heads on one frozen front end in one fused step per batch.
+
+    ``model``'s conv1 / conv2 are the front end: the conv forward runs once per step on them and nothing
+    back-propagates into them.  Each of ``heads`` (1 to 8 distinct :class:`B200MyCNN` with the model's architecture,
+    device and conv weights; ``model`` itself may be one of them) trains its own LSTM and ``out`` parameters with its own
+    Adam state::
+
+        trainer = B200HeadTrainer(model, [cand_a, cand_b, model], lr=[1e-3, 3e-4, 1e-4])
+        for x, age, y in loader:
+            losses = trainer.step(x, age, y)        # Tensor[K]: head i's loss
+        model.predict_record(records, stride, ages, heads=trainer.heads)   # backtest them, then SlidingScorer.set_heads
+
+    Every head sees the same features and the same dropout masks (one draw per step, :meth:`draw_masks`); row i is
+    what :class:`B200Trainer` on a copy of head i gives for its LSTM / Linear entries with those masks.  ``lr`` is one
+    float or one per head; betas, eps, ``pos_weight``, ``mode`` and ``dropout`` are shared.  After an update each head's
+    state dict holds its new weights and :meth:`B200MyCNN.sync_weights` has run."""
+
+    def __init__(self, model: B200MyCNN, heads, lr=1e-3, betas: Tuple[float, float] = (0.9, 0.999), eps: float = 1e-8,
+                 mode: str = "sequence", dropout: float = 0.1, seed: int = 0, pos_weight: Optional[float] = None):
+        if not isinstance(model, B200MyCNN):
+            raise TypeError(f"model must be a B200MyCNN, got {type(model).__name__}")
+        check_trainable(model.arch)
+        if mode not in ("sequence", "independent"):
+            raise ValueError("mode must be 'sequence' or 'independent'")
+        if not 0.0 <= float(dropout) < 1.0:
+            raise ValueError("dropout must be in [0, 1)")
+        if pos_weight is not None:
+            pos_weight = float(pos_weight)
+            if not (math.isfinite(pos_weight) and pos_weight > 0.0):
+                raise ValueError("pos_weight must be a positive finite number")
+        dev = model._device()
+        sd = model.state_dict()
+        front = {k: sd[k] for k in BLOB_KEYS[:BLOB_KEYS.index("lstm.weight_ih_l0")]}
+
+        def same_front_end(i, m):
+            if m._device() != dev:
+                return                                   # check_head_models refuses it next
+            hsd = m.state_dict()
+            bad = [k for k, v in front.items() if not torch.equal(hsd[k], v)]
+            if bad:
+                raise ValueError(f"heads[{i}] differs from the model's front end in {', '.join(bad)}")
+
+        heads = check_head_models(heads, model.arch, dev, "B200HeadTrainer", "the model", "the model", extra=same_front_end)
+        if not heads:
+            raise ValueError("B200HeadTrainer needs at least one head")
+        if len({id(h) for h in heads}) != len(heads):
+            raise ValueError("heads must be distinct models")
+        K = len(heads)
+        if isinstance(lr, (int, float)) and not isinstance(lr, bool):
+            lrs = [float(lr)] * K
+        else:
+            lrs = [float(v) for v in lr]
+            if len(lrs) != K:
+                raise ValueError(f"lr must be one float or {K} floats (one per head), got {len(lrs)}")
+        if not all(math.isfinite(v) and v >= 0.0 for v in lrs):
+            raise ValueError("every lr must be a finite number >= 0")
+        if dev.type != "cuda":
+            raise RuntimeError("B200HeadTrainer needs the model on a CUDA device (there is no CPU fallback)")
+        self.model, self.heads, self.mode, self.dropout, self.pos_weight = model, heads, mode, float(dropout), pos_weight
+        self._lib = capi.load_library()
+        self._cfg = capi.make_config(model.arch, dev.index if dev.index is not None else torch.cuda.current_device())
+        self._opt = capi.Adam(0.0, betas[0], betas[1], eps)
+        self._lr = (ctypes.c_float * K)(*lrs)
+        self._front = model.packed_weights().to(dev).contiguous()         # read for its conv entries only
+        self._params = torch.stack([h.packed_weights().to(dev) for h in heads]).contiguous()   # [K, n]: one blob per head
+        self._m = torch.zeros_like(self._params)
+        self._v = torch.zeros_like(self._params)
+        self._grads = torch.zeros_like(self._params)
+        self._loss = torch.zeros(K, device=dev)
+        ptrs = lambda t: (ctypes.c_void_p * K)(*[t[i].data_ptr() for i in range(K)])
+        self._pp, self._pm, self._pv, self._pg = ptrs(self._params), ptrs(self._m), ptrs(self._v), ptrs(self._grads)
+        self._ws: Optional[torch.Tensor] = None
+        self._gen = torch.Generator(device=dev)
+        self._gen.manual_seed(seed)
+        self.steps = 0
+
+    def _views(self, flat: torch.Tensor) -> Dict[str, torch.Tensor]:
+        sd, out, at = self.model.state_dict(), {}, 0
+        for k in BLOB_KEYS:
+            n = sd[k].numel()
+            out[k] = flat[at:at + n].view(sd[k].shape)
+            at += n
+        return out
+
+    def grads(self) -> List[Dict[str, torch.Tensor]]:
+        """d loss / d parameter of the most recent step, one dict per head, keyed like the reference's state_dict from
+        ``lstm.weight_ih_l0`` on (the front end gets no gradient)."""
+        first = BLOB_KEYS.index("lstm.weight_ih_l0")
+        return [{k: v for k, v in self._views(self._grads[i]).items() if k in BLOB_KEYS[first:]} for i in range(len(self.heads))]
+
+    def draw_masks(self, B: int, n_samples: Optional[int] = None) -> Tuple[Optional[torch.Tensor], Optional[torch.Tensor]]:
+        """One draw of the two dropout masks (as :meth:`B200Trainer.draw_masks`), shared by every head."""
+        arch = self.model.arch if n_samples is None else self.model.arch.with_shape(self.model.arch.in_channels, n_samples)
+        return draw_masks(arch, B, self.dropout, self._params.device, self._gen)
+
+    def _ptr(self, t):
+        return ctypes.c_void_p(t.data_ptr()) if t is not None else None
+
+    def _workspace(self, need: int, what: str) -> torch.Tensor:
+        if need < 0:
+            capi.check(capi.EINVAL, what)
+        if self._ws is None or self._ws.numel() < need:
+            self._ws = torch.empty(need, dtype=torch.uint8, device=self._params.device)
+        return self._ws
+
+    def step(self, x: torch.Tensor, age: torch.Tensor, target: torch.Tensor,
+             masks: Optional[Tuple[Optional[torch.Tensor], Optional[torch.Tensor]]] = None, update: bool = True,
+             seq_lengths=None) -> torch.Tensor:
+        """:meth:`B200Trainer.step` for every head at once, with its rules; returns the K heads' batch losses, a device
+        tensor [K]."""
+        dev = self._params.device
+        a = self.model.arch
+        if x.dim() != 3 or x.shape[1] != a.in_channels or x.shape[2] != a.window:
+            raise RuntimeError(f"expected x of shape [B, {a.in_channels}, {a.window}], got {tuple(x.shape)}")
+        B = x.shape[0]
+        lens = None
+        if seq_lengths is not None:
+            if self.mode != "sequence":
+                raise ValueError("seq_lengths needs a trainer in mode='sequence'")
+            lens = capi.seq_lengths_array(seq_lengths, B)
+        x = x.to(dev, torch.float32).contiguous()
+        age = age.to(dev, torch.float32).reshape(-1).contiguous()
+        target = target.to(dev, torch.float32).reshape(-1).contiguous()
+        if age.numel() != B or target.numel() != B:
+            raise RuntimeError("age and target must have one entry per window")
+        m1, m2 = check_masks(a, B, dev, *(masks if masks is not None else self.draw_masks(B)))
+        K = len(self.heads)
+        need = self._lib.b2cnn_train_heads_workspace_bytes(ctypes.byref(self._cfg), K, B, lens, len(lens) if lens is not None else 0)
+        ws = self._workspace(need, "b2cnn_train_heads_workspace_bytes")
+        p = self._ptr
+        pw = None if self.pos_weight is None else ctypes.byref(ctypes.c_float(self.pos_weight))
+        mode = capi.MODE_SEQUENCE if self.mode == "sequence" else capi.MODE_INDEPENDENT
+        st = torch.cuda.current_stream(dev).cuda_stream
+        capi.check(self._lib.b2cnn_train_heads_step(ctypes.byref(self._cfg), p(self._front), K, self._pp, self._pm, self._pv, self._pg,
+                                                    self._lr, self.steps + 1, ctypes.byref(self._opt), 1 if update else 0, p(x), B,
+                                                    p(age), p(target), pw, mode, lens, len(lens) if lens is not None else 0, p(m1), p(m2),
+                                                    p(self._loss), p(ws), need, ctypes.c_void_p(st)), "b2cnn_train_heads_step")
+        return self._finish(update)
+
+    def step_record(self, records: torch.Tensor, stride: int, age, target: torch.Tensor, window_counts=None,
+                    masks: Optional[Tuple[Optional[torch.Tensor], Optional[torch.Tensor]]] = None, update: bool = True,
+                    state=None, return_state: bool = False) -> torch.Tensor:
+        """:meth:`B200Trainer.step_record` for every head at once, in both modes; returns the K heads' losses [K].
+        Carrying an LSTM state across chunks (``state`` / ``return_state``) is not supported (ValueError)."""
+        if state is not None or return_state:
+            raise ValueError("B200HeadTrainer.step_record carries no LSTM state across calls (state / return_state)")
+        dev = self._params.device
+        stride, age, counts, M, rarch = check_record_batch(self.model.arch, records, stride, age, window_counts)
+        B, N = records.shape[0], records.shape[2]
+        target = torch.as_tensor(target).detach().to(dev, torch.float32).reshape(-1).contiguous()
+        if target.numel() != M:
+            raise ValueError(f"target must have one entry per window ({M}), got {target.numel()}")
+        m1, m2 = check_masks(rarch, B, dev, *(masks if masks is not None else self.draw_masks(B, N)))
+        mode = capi.MODE_SEQUENCE if self.mode == "sequence" else capi.MODE_INDEPENDENT
+        K = len(self.heads)
+        need = self._lib.b2cnn_train_heads_workspace_bytes_record(ctypes.byref(self._cfg), K, B, N, stride, counts, mode)
+        ws = self._workspace(need, "b2cnn_train_heads_workspace_bytes_record")
+        records = records.to(dev, torch.float32).contiguous()
+        age = window_ages(age.detach(), counts, M, dev)
+        p = self._ptr
+        pw = None if self.pos_weight is None else ctypes.byref(ctypes.c_float(self.pos_weight))
+        st = torch.cuda.current_stream(dev).cuda_stream
+        capi.check(self._lib.b2cnn_train_heads_step_record(ctypes.byref(self._cfg), p(self._front), K, self._pp, self._pm, self._pv,
+                                                           self._pg, self._lr, self.steps + 1, ctypes.byref(self._opt), 1 if update else 0,
+                                                           p(records), B, N, stride, counts, mode, p(age), p(target), pw, p(m1), p(m2),
+                                                           p(self._loss), p(ws), need, ctypes.c_void_p(st)), "b2cnn_train_heads_step_record")
+        return self._finish(update)
+
+    def _finish(self, update: bool) -> torch.Tensor:
+        if update:
+            self.steps += 1
+            with torch.no_grad():                        # the inference kernels read the module's parameters
+                for i, h in enumerate(self.heads):
+                    sd = h.state_dict()
+                    for k, v in self._views(self._params[i]).items():
+                        sd[k].copy_(v)
+                    h.sync_weights()
+        return self._loss.clone()
