@@ -102,16 +102,20 @@ extern "C" int64_t b2cnn_train_workspace_bytes_seq(const b2cnn_config *cfg, int6
     if (n < 0) fail(B2CNN_EINVAL, "b2cnn_train_workspace_bytes_seq: bad configuration / batch / sequence lengths");
     return n;
 }
+// a training entry point's call on `stream`, its outcome recorded under `name`
+template <typename F, typename... A>
+static int train_api(const char *name, F fn, void *stream, A... a) {
+    const char *err = "";
+    const int rc = fn(a..., reinterpret_cast<cudaStream_t>(stream), &err);
+    return finish(name, rc, err);
+}
 static int train_step_api(const char *name, const b2cnn_config *cfg, float *params, float *adam_m, float *adam_v, float *grads,
                           int64_t step, const b2cnn_adam *opt, int apply_update, const float *x, int64_t B, const float *age,
                           const float *target, int weighted, float pos_weight, int mode, const SeqLengths &sl, const RecordArgs &ra,
                           const float *mask1, const float *mask2, float *loss_out, void *workspace, int64_t workspace_bytes, void *stream) {
     if (!cfg || !opt) return fail(B2CNN_EINVAL, std::string(name) + ": null configuration");
-    const char *err = "";
-    const int rc = train_step(cfg, params, adam_m, adam_v, grads, step, opt->lr, opt->beta1, opt->beta2, opt->eps, apply_update, x, B, age,
-                              target, weighted, pos_weight, mode, sl, ra, mask1, mask2, loss_out, workspace, workspace_bytes,
-                              reinterpret_cast<cudaStream_t>(stream), &err);
-    return finish(name, rc, err);
+    return train_api(name, train_step, stream, cfg, params, adam_m, adam_v, grads, step, opt->lr, opt->beta1, opt->beta2, opt->eps,
+                     apply_update, x, B, age, target, weighted, pos_weight, mode, sl, ra, mask1, mask2, loss_out, workspace, workspace_bytes);
 }
 extern "C" int b2cnn_train_step(const b2cnn_config *cfg, float *params, float *adam_m, float *adam_v, float *grads, int64_t step,
                                 const b2cnn_adam *opt, int apply_update, const float *x, int64_t B, const float *age,
@@ -139,26 +143,20 @@ extern "C" int b2cnn_train_step_seq(const b2cnn_config *cfg, float *params, floa
 extern "C" int b2cnn_train_forward(const b2cnn_config *cfg, const float *params, const float *x, int64_t B, const float *age, int mode,
                                    const float *mask1, const float *mask2, float *z_out, void *workspace, int64_t workspace_bytes,
                                    void *stream) {
-    const char *err = "";
-    const int rc = train_forward(cfg, params, x, B, age, mode, kNoSeq, kNoRec, mask1, mask2, z_out, workspace, workspace_bytes,
-                                 reinterpret_cast<cudaStream_t>(stream), &err);
-    return finish("b2cnn_train_forward", rc, err);
+    return train_api("b2cnn_train_forward", train_forward, stream, cfg, params, x, B, age, mode, kNoSeq, kNoRec, mask1, mask2, z_out,
+                     workspace, workspace_bytes);
 }
 extern "C" int b2cnn_train_forward_seq(const b2cnn_config *cfg, const float *params, const float *x, int64_t B, const float *age,
                                        const int64_t *seq_lengths, int64_t n_seq, const float *mask1, const float *mask2, float *z_out,
                                        void *workspace, int64_t workspace_bytes, void *stream) {
-    const char *err = "";
-    const int rc = train_forward(cfg, params, x, B, age, B2CNN_MODE_SEQUENCE, SeqLengths{true, seq_lengths, n_seq}, kNoRec, mask1, mask2, z_out,
-                                 workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream), &err);
-    return finish("b2cnn_train_forward_seq", rc, err);
+    return train_api("b2cnn_train_forward_seq", train_forward, stream, cfg, params, x, B, age, B2CNN_MODE_SEQUENCE,
+                     SeqLengths{true, seq_lengths, n_seq}, kNoRec, mask1, mask2, z_out, workspace, workspace_bytes);
 }
 extern "C" int b2cnn_train_backward_ex(const b2cnn_config *cfg, const float *params, const float *x, int64_t B, const float *age, int mode,
                                        const float *mask1, const float *mask2, const float *dz, float *grads, float *dx, float *dage,
                                        int flags, void *workspace, int64_t workspace_bytes, void *stream) {
-    const char *err = "";
-    const int rc = train_backward(cfg, params, x, B, age, mode, kNoSeq, kNoRec, mask1, mask2, dz, grads, dx, dage, flags, workspace, workspace_bytes,
-                                  reinterpret_cast<cudaStream_t>(stream), &err);
-    return finish("b2cnn_train_backward", rc, err);
+    return train_api("b2cnn_train_backward", train_backward, stream, cfg, params, x, B, age, mode, kNoSeq, kNoRec, mask1, mask2, dz, grads,
+                     dx, dage, flags, workspace, workspace_bytes);
 }
 extern "C" int b2cnn_train_backward(const b2cnn_config *cfg, const float *params, const float *x, int64_t B, const float *age, int mode,
                                     const float *mask1, const float *mask2, const float *dz, float *grads, float *dx, float *dage,
@@ -169,10 +167,8 @@ extern "C" int b2cnn_train_backward_seq(const b2cnn_config *cfg, const float *pa
                                         const int64_t *seq_lengths, int64_t n_seq, const float *mask1, const float *mask2, const float *dz,
                                         float *grads, float *dx, float *dage, int flags, void *workspace, int64_t workspace_bytes,
                                         void *stream) {
-    const char *err = "";
-    const int rc = train_backward(cfg, params, x, B, age, B2CNN_MODE_SEQUENCE, SeqLengths{true, seq_lengths, n_seq}, kNoRec, mask1, mask2, dz, grads,
-                                  dx, dage, flags, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream), &err);
-    return finish("b2cnn_train_backward_seq", rc, err);
+    return train_api("b2cnn_train_backward_seq", train_backward, stream, cfg, params, x, B, age, B2CNN_MODE_SEQUENCE,
+                     SeqLengths{true, seq_lengths, n_seq}, kNoRec, mask1, mask2, dz, grads, dx, dage, flags, workspace, workspace_bytes);
 }
 extern "C" int64_t b2cnn_train_workspace_bytes_record(const b2cnn_config *cfg, int64_t B, int64_t N, int64_t stride,
                                                      const int64_t *window_counts, int mode) {
@@ -192,19 +188,16 @@ extern "C" int b2cnn_train_step_record(const b2cnn_config *cfg, float *params, f
 extern "C" int b2cnn_train_forward_record(const b2cnn_config *cfg, const float *params, const float *records, int64_t B, int64_t N,
                                           int64_t stride, const int64_t *window_counts, int mode, const float *age, const float *mask1,
                                           const float *mask2, float *z_out, void *workspace, int64_t workspace_bytes, void *stream) {
-    const char *err = "";
-    const int rc = train_forward(cfg, params, records, B, age, mode, kNoSeq, RecordArgs{true, N, stride, window_counts}, mask1, mask2, z_out,
-                                 workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream), &err);
-    return finish("b2cnn_train_forward_record", rc, err);
+    return train_api("b2cnn_train_forward_record", train_forward, stream, cfg, params, records, B, age, mode, kNoSeq,
+                     RecordArgs{true, N, stride, window_counts}, mask1, mask2, z_out, workspace, workspace_bytes);
 }
 extern "C" int b2cnn_train_backward_record(const b2cnn_config *cfg, const float *params, const float *records, int64_t B, int64_t N,
                                            int64_t stride, const int64_t *window_counts, int mode, const float *age, const float *mask1,
                                            const float *mask2, const float *dz, float *grads, float *d_records, float *dage, int flags,
                                            void *workspace, int64_t workspace_bytes, void *stream) {
-    const char *err = "";
-    const int rc = train_backward(cfg, params, records, B, age, mode, kNoSeq, RecordArgs{true, N, stride, window_counts}, mask1, mask2, dz,
-                                  grads, d_records, dage, flags, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream), &err);
-    return finish("b2cnn_train_backward_record", rc, err);
+    return train_api("b2cnn_train_backward_record", train_backward, stream, cfg, params, records, B, age, mode, kNoSeq,
+                     RecordArgs{true, N, stride, window_counts}, mask1, mask2, dz, grads, d_records, dage, flags, workspace,
+                     workspace_bytes);
 }
 extern "C" int b2cnn_train_step_record_state(const b2cnn_config *cfg, float *params, float *adam_m, float *adam_v, float *grads,
                                              int64_t step, const b2cnn_adam *opt, int apply_update, const float *records, int64_t B,
@@ -223,10 +216,8 @@ extern "C" int b2cnn_train_forward_record_state(const b2cnn_config *cfg, const f
                                                 const float *mask2, const float *state_in, float *state_out, float *z_out, void *workspace,
                                                 int64_t workspace_bytes, void *stream) {
     if (mode != B2CNN_MODE_SEQUENCE) return fail(B2CNN_EINVAL, "b2cnn_train_forward_record_state: mode must be B2CNN_MODE_SEQUENCE");
-    const char *err = "";
-    const int rc = train_forward(cfg, params, records, B, age, mode, kNoSeq, RecordArgs{true, N, stride, window_counts, state_in, state_out},
-                                 mask1, mask2, z_out, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream), &err);
-    return finish("b2cnn_train_forward_record_state", rc, err);
+    return train_api("b2cnn_train_forward_record_state", train_forward, stream, cfg, params, records, B, age, mode, kNoSeq,
+                     RecordArgs{true, N, stride, window_counts, state_in, state_out}, mask1, mask2, z_out, workspace, workspace_bytes);
 }
 extern "C" int b2cnn_train_backward_record_state(const b2cnn_config *cfg, const float *params, const float *records, int64_t B, int64_t N,
                                                  int64_t stride, const int64_t *window_counts, int mode, const float *age,
@@ -234,11 +225,9 @@ extern "C" int b2cnn_train_backward_record_state(const b2cnn_config *cfg, const 
                                                  const float *d_state_out, float *grads, float *d_records, float *dage, float *d_state_in,
                                                  int flags, void *workspace, int64_t workspace_bytes, void *stream) {
     if (mode != B2CNN_MODE_SEQUENCE) return fail(B2CNN_EINVAL, "b2cnn_train_backward_record_state: mode must be B2CNN_MODE_SEQUENCE");
-    const char *err = "";
-    const int rc = train_backward(cfg, params, records, B, age, mode, kNoSeq,
-                                  RecordArgs{true, N, stride, window_counts, state_in, nullptr, d_state_out, d_state_in}, mask1, mask2, dz,
-                                  grads, d_records, dage, flags, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream), &err);
-    return finish("b2cnn_train_backward_record_state", rc, err);
+    return train_api("b2cnn_train_backward_record_state", train_backward, stream, cfg, params, records, B, age, mode, kNoSeq,
+                     RecordArgs{true, N, stride, window_counts, state_in, nullptr, d_state_out, d_state_in}, mask1, mask2, dz, grads,
+                     d_records, dage, flags, workspace, workspace_bytes);
 }
 
 // ---- candidate heads on one frozen front end (b2cnn_train.cu) ----
@@ -261,11 +250,9 @@ static int train_heads_api(const char *name, const b2cnn_config *cfg, const floa
                            const float *pos_weight, int mode, const SeqLengths &sl, const RecordArgs &ra, const float *mask1,
                            const float *mask2, float *loss_out, void *workspace, int64_t workspace_bytes, void *stream) {
     if (!cfg || !opt) return fail(B2CNN_EINVAL, std::string(name) + ": null configuration");
-    const char *err = "";
-    const int rc = train_heads_step(cfg, frontend, n_heads, params, adam_m, adam_v, grads, lr, step, opt->beta1, opt->beta2, opt->eps,
-                                    apply_update, x, B, age, target, pos_weight ? 1 : 0, pos_weight ? *pos_weight : 1.f, mode, sl, ra,
-                                    mask1, mask2, loss_out, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream), &err);
-    return finish(name, rc, err);
+    return train_api(name, train_heads_step, stream, cfg, frontend, n_heads, params, adam_m, adam_v, grads, lr, step, opt->beta1, opt->beta2,
+                     opt->eps, apply_update, x, B, age, target, pos_weight ? 1 : 0, pos_weight ? *pos_weight : 1.f, mode, sl, ra, mask1,
+                     mask2, loss_out, workspace, workspace_bytes);
 }
 extern "C" int b2cnn_train_heads_step(const b2cnn_config *cfg, const float *frontend, int32_t n_heads, float *const *params,
                                       float *const *adam_m, float *const *adam_v, float *const *grads, const float *lr, int64_t step,

@@ -54,6 +54,7 @@
 // window reads, so NaN / inf there cannot reach a gradient.
 #include <cfloat>
 #include <cstring>
+#include <optional>
 #include <vector>
 
 #include "b2cnn_internal.cuh"
@@ -1167,37 +1168,127 @@ int64_t train_workspace_bytes(const b2cnn_config *cfg, int64_t B, const SeqLengt
     return pl.w.total * (int64_t)sizeof(float);
 }
 
-// conv forward into ws.f and the layer-0 pre-activations of the R rows into ws.pre0 (one slice is the whole sum: no
-// reduction).  cd / B: the conv kernels' geometry and rows (the recordings' with REC, else d and the windows)
-template <bool REC>
-static void launch_conv_forward(const Dims &d, const Dims &cd, const BlobOff &o, const TrainPlan &pl, float *ws, const float *params,
-                                const float *x, int64_t B, int64_t R, const float *mask1, const float *mask2, const RecRows &rr,
+// A training call after the checks every entry point shares (check): the geometry, the plan, the sequence offsets of a
+// _seq call and the windows of a _record call (rec.rows: the scans' rows, the batch without one).  open() then makes
+// the call's device current for the life of this object and copies the offsets into the workspace, which every launch
+// below addresses through it.
+struct TrainCall {
+    Dims d;
+    TrainPlan pl;
+    BlobOff o{};
+    std::vector<int64_t> off;
+    Rec rec;
+    int64_t B = 0;
+    int device = -1, sequence = 0;
+    std::optional<DeviceGuard> dev;
+    float *ws = nullptr;
+    SeqSpan sq{nullptr, 0, 1, nullptr};
+    RecRows rr{nullptr, 0, 0, 1, 0, 0, 0};
+
+    // The checks of every training entry point, before any CUDA call: the configuration, the mode, the pointers the call
+    // needs (ptrs_ok) and the batch, the sequence lengths of a _seq call (into off), the windows of a _record call (into
+    // rec and off), what the kernels hold, and the workspace size.
+    int check(const b2cnn_config *cfg, int64_t batch, int mode, const SeqLengths &sl, const RecordArgs &ra, bool ptrs_ok, int64_t ws_bytes,
+              const char **err, int heads = 0) {
+        if (!train_geometry(cfg, d, err)) return B2CNN_EINVAL;
+        if (mode != B2CNN_MODE_INDEPENDENT && mode != B2CNN_MODE_SEQUENCE) { *err = "training: bad mode"; return B2CNN_EINVAL; }
+        if (!ptrs_ok || batch < 1) { *err = "training: null argument / bad batch"; return B2CNN_EINVAL; }
+        if (sl.on && !seq_offsets(sl, batch, off, err)) return B2CNN_EINVAL;
+        if (ra.on && !record_rows(*cfg, d, batch, mode, ra, rec, off, err)) return B2CNN_EINVAL;
+        if (ra.has_state() && (!ra.on || mode != B2CNN_MODE_SEQUENCE)) { *err = "training: an LSTM state needs sequence mode"; return B2CNN_EINVAL; }
+        if (ra.states_overlap(batch)) { *err = "training: the LSTM state arrays overlap"; return B2CNN_EINVAL; }
+        if (!ra.on) rec.rows = batch;
+        pl = train_plan(d, rec.rows, off.empty() ? 0 : (int64_t)off.size() - 1, ra.on ? &rec.rd : nullptr, batch, heads);
+        if (!plan_fits(cd(), pl, batch, err)) return B2CNN_EINVAL;
+        if (ws_bytes < pl.w.total * (int64_t)sizeof(float)) {
+            *err = heads ? (ra.on ? "training: workspace smaller than b2cnn_train_heads_workspace_bytes_record()"
+                                  : "training: workspace smaller than b2cnn_train_heads_workspace_bytes()")
+                 : ra.on ? "training: workspace smaller than b2cnn_train_workspace_bytes_record()"
+                 : sl.on ? "training: workspace smaller than b2cnn_train_workspace_bytes_seq()" : "training: workspace smaller than b2cnn_train_workspace_bytes()";
+            return B2CNN_ESTATE;
+        }
+        o = blob_offsets(d);
+        B = batch;
+        device = cfg->device;
+        sequence = mode == B2CNN_MODE_SEQUENCE ? 1 : 0;
+        return B2CNN_OK;
+    }
+
+    // After the entry point's own checks.  The offsets are copied from pageable memory: the copies have read them when
+    // they return.
+    int open(void *workspace, cudaStream_t st, const char **err) {
+        dev.emplace(device);
+        if (dev->err != cudaSuccess) { *err = "cudaSetDevice"; return B2CNN_ECUDA; }
+        ws = reinterpret_cast<float *>(workspace);
+        if (!off.empty()) {
+            int64_t *doff = reinterpret_cast<int64_t *>(ws + pl.w.off);
+            if (cudaMemcpyAsync(doff, off.data(), sizeof(int64_t) * off.size(), cudaMemcpyHostToDevice, st) != cudaSuccess) {
+                *err = "copy sequence offsets";
+                return B2CNN_ECUDA;
+            }
+            sq = SeqSpan{doff, (int64_t)off.size() - 1, pl.seq_per, pl.seq_ctas > 1 ? ws + pl.w.part : nullptr};
+        }
+        if (rec.on) {
+            int64_t *droff = reinterpret_cast<int64_t *>(ws + pl.w.roff);
+            if (cudaMemcpyAsync(droff, rec.roff.data(), sizeof(int64_t) * rec.roff.size(), cudaMemcpyHostToDevice, st) != cudaSuccess) {
+                *err = "copy row offsets";
+                return B2CNN_ECUDA;
+            }
+            rr = RecRows{droff, B, (int)rec.S, (int)(rec.S / d.feature_stride()), d.W, d.L, rec.rd.L};
+        }
+        return B2CNN_OK;
+    }
+
+    // the conv kernels' geometry: the recordings' with a _record call, else the windows'
+    const Dims &cd() const { return rec.on ? rec.rd : d; }
+    // the layer-0 pre-activation GEMM of n_heads heads: (row tiles of 64, split-K slices, head pairs), written to the
+    // slices' partials, or with one slice (the whole sum: no reduction) to ws.pre0
+    dim3 pre0_grid(int n_heads) const {
+        return dim3((unsigned)((rec.rows + 63) / 64), (unsigned)pl.slices, (unsigned)((n_heads + kPre0Heads - 1) / kPre0Heads));
+    }
+    float *pre0_out() const { return ws + (pl.slices > 1 ? pl.w.part : pl.w.pre0); }
+};
+
+// the conv forward into ws.f over the windows, or with a _record call over the recordings, on the conv entries of params
+static void launch_conv_forward(const TrainCall &c, const float *params, const float *x, const float *mask1, const float *mask2,
                                 cudaStream_t st) {
-    const TrainWs &w = pl.w;
-    const dim3 conv((unsigned)(B * pl.tiles)), proj((unsigned)((R + 63) / 64), (unsigned)pl.slices);
-    float *const pre0 = ws + (pl.slices > 1 ? w.part : w.pre0);
-    if constexpr (REC) {
+    const TrainPlan &pl = c.pl;
+    const dim3 conv((unsigned)(c.B * pl.tiles));
+    if (c.rec.on) {
         if (pl.smem_fwd > 48 * 1024) cudaFuncSetAttribute(train_conv_fwd_record, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.smem_fwd);
-        train_conv_fwd_record<<<conv, kThreads, pl.smem_fwd, st>>>(x, params, o, cd, pl.tiles, mask1, mask2, ws + w.f, rr);
-        train_pre0_partial_record<<<proj, 256, 0, st>>>(ws + w.f, params + o.wih0, R, d.L, pre0, rr);
+        train_conv_fwd_record<<<conv, kThreads, pl.smem_fwd, st>>>(x, params, c.o, c.rec.rd, pl.tiles, mask1, mask2, c.ws + pl.w.f, c.rr);
     } else {
         if (pl.smem_fwd > 48 * 1024) cudaFuncSetAttribute(train_conv_fwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.smem_fwd);
-        train_conv_fwd<<<conv, kThreads, pl.smem_fwd, st>>>(x, params, o, cd, pl.tiles, mask1, mask2, ws + w.f);
-        train_pre0_partial<<<proj, 256, 0, st>>>(ws + w.f, params + o.wih0, R, d.L, pre0);
+        train_conv_fwd<<<conv, kThreads, pl.smem_fwd, st>>>(x, params, c.o, c.d, pl.tiles, mask1, mask2, c.ws + pl.w.f);
     }
-    if (pl.slices > 1) {
-        const int64_t n = R * kGates;
-        train_sum_chunks<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(ws + w.part, pl.slices, n, ws + w.pre0);
-    }
+}
+// with several split-K slices: the layer-0 pre-activations [n_heads][R][64] summed from their partials into ws.pre0
+static void sum_pre0(const TrainCall &c, int n_heads, cudaStream_t st) {
+    if (c.pl.slices <= 1) return;
+    const int64_t n = (int64_t)n_heads * c.rec.rows * kGates;
+    train_sum_chunks<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(c.ws + c.pl.w.part, c.pl.slices, n, c.ws + c.pl.w.pre0);
+}
+// the conv forward and the layer-0 pre-activations of the one model a call trains
+static void conv_forward(const TrainCall &c, const float *params, const float *x, const float *mask1, const float *mask2, cudaStream_t st) {
+    launch_conv_forward(c, params, x, mask1, mask2, st);
+    const float *const f = c.ws + c.pl.w.f;
+    if (c.rec.on) train_pre0_partial_record<<<c.pre0_grid(1), 256, 0, st>>>(f, params + c.o.wih0, c.rec.rows, c.d.L, c.pre0_out(), c.rr);
+    else train_pre0_partial<<<c.pre0_grid(1), 256, 0, st>>>(f, params + c.o.wih0, c.rec.rows, c.d.L, c.pre0_out());
+    sum_pre0(c, 1, st);
 }
 
 // everything after d(head): d W_ih_l0 and, unless the front end is frozen, d f (with REC folded onto the recordings), the
 // convolutional backward into `grads` and, when dx != NULL, the input gradient (added into dx, zeroed here)
 template <bool REC>
-static bool launch_backward_tail(const Dims &d, const Dims &cd, const BlobOff &o, const TrainPlan &pl, float *ws, const float *params,
-                                 const float *x, int64_t B, int64_t R, const float *mask1, const float *mask2, float *grads, float *dx,
-                                 bool frozen_conv, const RecRows &rr, cudaStream_t st) {
+static bool launch_backward_tail(const TrainCall &c, const float *params, const float *x, const float *mask1, const float *mask2,
+                                 float *grads, float *dx, bool frozen_conv, cudaStream_t st) {
+    const Dims &d = c.d, &cd = c.cd();
+    const TrainPlan &pl = c.pl;
     const TrainWs &w = pl.w;
+    const BlobOff &o = c.o;
+    const RecRows &rr = c.rr;
+    float *const ws = c.ws;
+    const int64_t B = c.B, R = c.rec.rows;
     const int64_t n1 = (int64_t)kGates * d.L;
     const unsigned ptiles = (unsigned)((d.L + 127) / 128);
     const dim3 wgrid(ptiles, (unsigned)pl.wih_chunks);
@@ -1226,41 +1317,10 @@ static bool launch_backward_tail(const Dims &d, const Dims &cd, const BlobOff &o
     train_conv_grad_reduce<<<(unsigned)pl.n_conv, 256, 0, st>>>(ws + w.part, pl.part_rows, pl.n_conv, grads);
     return true;
 }
-
-// The checks every training entry point shares, before any CUDA call: the configuration, the mode, the pointers the call
-// needs (ptrs_ok) and the batch, the sequence lengths of a _seq call (into off), the windows of a _record call (into rec
-// and off), what the kernels hold, and the workspace size.
-static int train_args(const b2cnn_config *cfg, int64_t B, int mode, const SeqLengths &sl, const RecordArgs &ra, bool ptrs_ok,
-                      int64_t ws_bytes, Dims &d, TrainPlan &pl, std::vector<int64_t> &off, Rec &rec, const char **err, int heads = 0) {
-    if (!train_geometry(cfg, d, err)) return B2CNN_EINVAL;
-    if (mode != B2CNN_MODE_INDEPENDENT && mode != B2CNN_MODE_SEQUENCE) { *err = "training: bad mode"; return B2CNN_EINVAL; }
-    if (!ptrs_ok || B < 1) { *err = "training: null argument / bad batch"; return B2CNN_EINVAL; }
-    if (sl.on && !seq_offsets(sl, B, off, err)) return B2CNN_EINVAL;
-    if (ra.on && !record_rows(*cfg, d, B, mode, ra, rec, off, err)) return B2CNN_EINVAL;
-    if (ra.has_state() && (!ra.on || mode != B2CNN_MODE_SEQUENCE)) { *err = "training: an LSTM state needs sequence mode"; return B2CNN_EINVAL; }
-    if (ra.states_overlap(B)) { *err = "training: the LSTM state arrays overlap"; return B2CNN_EINVAL; }
-    if (!ra.on) rec.rows = B;
-    pl = train_plan(d, rec.rows, off.empty() ? 0 : (int64_t)off.size() - 1, ra.on ? &rec.rd : nullptr, B, heads);
-    if (!plan_fits(ra.on ? rec.rd : d, pl, B, err)) return B2CNN_EINVAL;
-    if (ws_bytes < pl.w.total * (int64_t)sizeof(float)) {
-        *err = heads ? (ra.on ? "training: workspace smaller than b2cnn_train_heads_workspace_bytes_record()"
-                              : "training: workspace smaller than b2cnn_train_heads_workspace_bytes()")
-             : ra.on ? "training: workspace smaller than b2cnn_train_workspace_bytes_record()"
-             : sl.on ? "training: workspace smaller than b2cnn_train_workspace_bytes_seq()" : "training: workspace smaller than b2cnn_train_workspace_bytes()";
-        return B2CNN_ESTATE;
-    }
-    return B2CNN_OK;
-}
-
-// The scan's SeqSpan; a _seq call first copies its offsets into the workspace (from pageable memory: the copy has read
-// `off` when it returns)
-static bool seq_span(const TrainPlan &pl, const std::vector<int64_t> &off, float *ws, cudaStream_t st, SeqSpan &sq) {
-    sq = SeqSpan{nullptr, 0, 1, nullptr};
-    if (off.empty()) return true;
-    int64_t *doff = reinterpret_cast<int64_t *>(ws + pl.w.off);
-    if (cudaMemcpyAsync(doff, off.data(), sizeof(int64_t) * off.size(), cudaMemcpyHostToDevice, st) != cudaSuccess) return false;
-    sq = SeqSpan{doff, (int64_t)off.size() - 1, pl.seq_per, pl.seq_ctas > 1 ? ws + pl.w.part : nullptr};
-    return true;
+static bool backward_tail(const TrainCall &c, const float *params, const float *x, const float *mask1, const float *mask2, float *grads,
+                          float *dx, bool frozen_conv, cudaStream_t st) {
+    if (c.rec.on) return launch_backward_tail<true>(c, params, x, mask1, mask2, grads, dx, frozen_conv, st);
+    return launch_backward_tail<false>(c, params, x, mask1, mask2, grads, dx, frozen_conv, st);
 }
 
 // the scans' view of the one model a call trains (gridDim.y = 1)
@@ -1271,22 +1331,11 @@ static ScanHeads one_head(const float *params, float *grads) {
     return hd;
 }
 
-// with more than one scan CTA: the head's gradients (and, with loss_out, the mean loss) from the CTAs' rows
-static void launch_head_reduce(const TrainPlan &pl, const BlobOff &o, const SeqSpan &sq, int64_t B, float *grads, float *loss_out,
-                               cudaStream_t st) {
-    if (!sq.rows) return;
-    train_head_reduce<<<(unsigned)((head_row_len(o) + 255) / 256), 256, 0, st>>>(sq.rows, pl.seq_ctas, o, B, one_head(nullptr, grads), loss_out);
-}
-
-// The row addressing of a _record call over its B recordings; it first copies the row offsets into the workspace (from
-// pageable memory, as seq_span does)
-static bool record_span(const TrainPlan &pl, const Rec &rec, const Dims &d, int64_t B, float *ws, cudaStream_t st, RecRows &rr) {
-    rr = RecRows{nullptr, 0, 0, 1, 0, 0, 0};
-    if (!rec.on) return true;
-    int64_t *droff = reinterpret_cast<int64_t *>(ws + pl.w.roff);
-    if (cudaMemcpyAsync(droff, rec.roff.data(), sizeof(int64_t) * rec.roff.size(), cudaMemcpyHostToDevice, st) != cudaSuccess) return false;
-    rr = RecRows{droff, B, (int)rec.S, (int)(rec.S / d.feature_stride()), d.W, d.L, rec.rd.L};
-    return true;
+// with more than one scan CTA: each head's gradients (and, with loss_out, its mean loss) from its CTAs' rows
+static void launch_head_reduce(const TrainCall &c, const ScanHeads &hd, int n_heads, float *loss_out, cudaStream_t st) {
+    if (!c.sq.rows) return;
+    const dim3 grid((unsigned)((head_row_len(c.o) + 255) / 256), (unsigned)n_heads);
+    train_head_reduce<<<grid, 256, 0, st>>>(c.sq.rows, c.pl.seq_ctas, c.o, c.rec.rows, hd, loss_out);
 }
 
 // the scan kernels of one HEAD, the STATE instance for a call with states
@@ -1313,17 +1362,22 @@ static bool pass_state(float *dst, const float *src, int64_t B, cudaStream_t st)
     return (src ? cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, st) : cudaMemsetAsync(dst, 0, bytes, st)) == cudaSuccess;
 }
 
-// the conv kernels over the windows, or with a _record call over the recordings
-static void conv_forward(const Dims &d, const Rec &rec, const BlobOff &o, const TrainPlan &pl, float *ws, const float *params,
-                         const float *x, int64_t B, const float *mask1, const float *mask2, const RecRows &rr, cudaStream_t st) {
-    if (rec.on) launch_conv_forward<true>(d, rec.rd, o, pl, ws, params, x, B, rec.rows, mask1, mask2, rr, st);
-    else launch_conv_forward<false>(d, d, o, pl, ws, params, x, B, B, mask1, mask2, rr, st);
+// The fused step's forward and backward scans of the n_heads heads hd, one grid row per head, on the BCE loss of HEAD
+// (the unweighted loss takes pos_weight 1); `state`: they start from and end in the states of ss
+template <int HEAD>
+static void fused_scans(const TrainCall &c, const ScanHeads &hd, int n_heads, const float *age, const float *target, float pos_weight,
+                        float *loss_out, bool state, const ScanState &ss, cudaStream_t st) {
+    const TrainWs &w = c.pl.w;
+    float *const ws = c.ws;
+    const dim3 grid((unsigned)c.pl.seq_ctas, (unsigned)n_heads);
+    lstm_fwd<HEAD>(grid, st, state, ws + w.pre0, hd, c.o, c.d, c.rec.rows, c.sequence, c.sq, age, target, pos_weight, ws + w.acts, ws + w.cs,
+                   ws + w.hs, ws + w.lin, ws + w.z, loss_out, ss);
+    lstm_bwd<HEAD>(grid, st, state, hd, c.o, c.d, c.rec.rows, c.sequence, c.sq, age, target, pos_weight, (const float *)nullptr, ws + w.acts,
+                   ws + w.cs, ws + w.hs, ws + w.lin, ws + w.z, ws + w.da0, (float *)nullptr, ss);
 }
-static bool backward_tail(const Dims &d, const Rec &rec, const BlobOff &o, const TrainPlan &pl, float *ws, const float *params,
-                          const float *x, int64_t B, const float *mask1, const float *mask2, float *grads, float *dx, bool frozen_conv,
-                          const RecRows &rr, cudaStream_t st) {
-    if (rec.on) return launch_backward_tail<true>(d, rec.rd, o, pl, ws, params, x, B, rec.rows, mask1, mask2, grads, dx, frozen_conv, rr, st);
-    return launch_backward_tail<false>(d, d, o, pl, ws, params, x, B, B, mask1, mask2, grads, dx, frozen_conv, rr, st);
+static void launch_scans(const TrainCall &c, const ScanHeads &hd, int n_heads, const float *age, const float *target, bool weighted,
+                         float pos_weight, float *loss_out, bool state, const ScanState &ss, cudaStream_t st) {
+    (weighted ? fused_scans<kHeadBcePw> : fused_scans<kHeadBce>)(c, hd, n_heads, age, target, weighted ? pos_weight : 1.f, loss_out, state, ss, st);
 }
 
 // B: the windows, or with a _record call (ra.on) the recordings x [B][C][N], whose R counted windows are the rows that age,
@@ -1332,48 +1386,23 @@ int train_step(const b2cnn_config *cfg, float *params, float *adam_m, float *ada
                float beta2, float eps, int apply_update, const float *x, int64_t B, const float *age, const float *target,
                int weighted, float pos_weight, int mode, const SeqLengths &sl, const RecordArgs &ra, const float *mask1, const float *mask2,
                float *loss_out, void *workspace, int64_t ws_bytes, cudaStream_t st, const char **err) {
-    Dims d;
-    TrainPlan pl;
-    std::vector<int64_t> off;
-    Rec rec;
-    const int rc = train_args(cfg, B, mode, sl, ra, params && grads && x && age && target && loss_out && workspace, ws_bytes, d, pl, off, rec, err);
+    TrainCall c;
+    int rc = c.check(cfg, B, mode, sl, ra, params && grads && x && age && target && loss_out && workspace, ws_bytes, err);
     if (rc != B2CNN_OK) return rc;
     if (step < 1) { *err = "training: step must be >= 1"; return B2CNN_EINVAL; }
     if (apply_update && (!adam_m || !adam_v)) { *err = "training: Adam state missing"; return B2CNN_EINVAL; }
     if (weighted && !(pos_weight > 0.f && pos_weight <= FLT_MAX)) { *err = "training: pos_weight must be positive and finite"; return B2CNN_EINVAL; }
-    DeviceGuard dev(cfg->device);
-    if (dev.err != cudaSuccess) { *err = "cudaSetDevice"; return B2CNN_ECUDA; }
-    const TrainWs &w = pl.w;
-    const BlobOff o = blob_offsets(d);
-    const int sequence = mode == B2CNN_MODE_SEQUENCE ? 1 : 0;
-    const int64_t R = rec.rows;
-    float *ws = reinterpret_cast<float *>(workspace);
-    SeqSpan sq;
-    if (!seq_span(pl, off, ws, st, sq)) { *err = "copy sequence offsets"; return B2CNN_ECUDA; }
-    RecRows rr;
-    if (!record_span(pl, rec, d, B, ws, st, rr)) { *err = "copy row offsets"; return B2CNN_ECUDA; }
+    if ((rc = c.open(workspace, st, err)) != B2CNN_OK) return rc;
+    const BlobOff &o = c.o;
     if (cudaMemsetAsync(grads, 0, sizeof(float) * o.total, st) != cudaSuccess) { *err = "memset grads"; return B2CNN_ECUDA; }
-    conv_forward(d, rec, o, pl, ws, params, x, B, mask1, mask2, rr, st);
-    const unsigned scans = (unsigned)pl.seq_ctas;
+    conv_forward(c, params, x, mask1, mask2, st);
     // the fused step is truncated back-propagation through time: no gradient enters through the final state
-    const ScanState ss = scan_state(RecordArgs{ra.on, ra.N, ra.S, ra.counts, ra.state_in, ra.state_out}, rr);
+    const ScanState ss = scan_state(RecordArgs{ra.on, ra.N, ra.S, ra.counts, ra.state_in, ra.state_out}, c.rr);
     if (!pass_state(ra.state_out, ra.state_in, B, st)) { *err = "copy of the LSTM state"; return B2CNN_ECUDA; }
-    const bool on = ra.has_state();
-    const float *const nul = nullptr;
     const ScanHeads hd = one_head(params, grads);
-    if (weighted) {
-        lstm_fwd<kHeadBcePw>(scans, st, on, ws + w.pre0, hd, o, d, R, sequence, sq, age, target, pos_weight, ws + w.acts, ws + w.cs,
-                             ws + w.hs, ws + w.lin, ws + w.z, loss_out, ss);
-        lstm_bwd<kHeadBcePw>(scans, st, on, hd, o, d, R, sequence, sq, age, target, pos_weight, nul, ws + w.acts, ws + w.cs, ws + w.hs,
-                             ws + w.lin, ws + w.z, ws + w.da0, (float *)nullptr, ss);
-    } else {
-        lstm_fwd<kHeadBce>(scans, st, on, ws + w.pre0, hd, o, d, R, sequence, sq, age, target, 1.f, ws + w.acts, ws + w.cs, ws + w.hs,
-                           ws + w.lin, ws + w.z, loss_out, ss);
-        lstm_bwd<kHeadBce>(scans, st, on, hd, o, d, R, sequence, sq, age, target, 1.f, nul, ws + w.acts, ws + w.cs, ws + w.hs,
-                           ws + w.lin, ws + w.z, ws + w.da0, (float *)nullptr, ss);
-    }
-    launch_head_reduce(pl, o, sq, R, grads, loss_out, st);
-    if (!backward_tail(d, rec, o, pl, ws, params, x, B, mask1, mask2, grads, nullptr, false, rr, st)) { *err = "memset dx"; return B2CNN_ECUDA; }
+    launch_scans(c, hd, 1, age, target, weighted, pos_weight, loss_out, ra.has_state(), ss, st);
+    launch_head_reduce(c, hd, 1, loss_out, st);
+    if (!backward_tail(c, params, x, mask1, mask2, grads, nullptr, false, st)) { *err = "memset dx"; return B2CNN_ECUDA; }
     if (apply_update) {
         const float bc1 = 1.f - powf(beta1, (float)step), bc2 = 1.f - powf(beta2, (float)step);
         train_adam<<<(unsigned)((o.total + 255) / 256), 256, 0, st>>>(params, adam_m, adam_v, grads, o.total, lr, beta1, beta2, eps, bc1, sqrtf(bc2));
@@ -1386,27 +1415,16 @@ int train_step(const b2cnn_config *cfg, float *params, float *adam_m, float *ada
 int train_forward(const b2cnn_config *cfg, const float *params, const float *x, int64_t B, const float *age, int mode, const SeqLengths &sl,
                   const RecordArgs &ra, const float *mask1, const float *mask2, float *z_out, void *workspace, int64_t ws_bytes,
                   cudaStream_t st, const char **err) {
-    Dims d;
-    TrainPlan pl;
-    std::vector<int64_t> off;
-    Rec rec;
-    const int rc = train_args(cfg, B, mode, sl, ra, params && x && age && z_out && workspace, ws_bytes, d, pl, off, rec, err);
-    if (rc != B2CNN_OK) return rc;
-    DeviceGuard dev(cfg->device);
-    if (dev.err != cudaSuccess) { *err = "cudaSetDevice"; return B2CNN_ECUDA; }
-    const TrainWs &w = pl.w;
-    const BlobOff o = blob_offsets(d);
-    const int sequence = mode == B2CNN_MODE_SEQUENCE ? 1 : 0;
-    float *ws = reinterpret_cast<float *>(workspace);
-    SeqSpan sq;
-    if (!seq_span(pl, off, ws, st, sq)) { *err = "copy sequence offsets"; return B2CNN_ECUDA; }
-    RecRows rr;
-    if (!record_span(pl, rec, d, B, ws, st, rr)) { *err = "copy row offsets"; return B2CNN_ECUDA; }
-    conv_forward(d, rec, o, pl, ws, params, x, B, mask1, mask2, rr, st);
+    TrainCall c;
+    int rc = c.check(cfg, B, mode, sl, ra, params && x && age && z_out && workspace, ws_bytes, err);
+    if (rc != B2CNN_OK || (rc = c.open(workspace, st, err)) != B2CNN_OK) return rc;
+    const TrainWs &w = c.pl.w;
+    float *const ws = c.ws;
+    conv_forward(c, params, x, mask1, mask2, st);
     if (!pass_state(ra.state_out, ra.state_in, B, st)) { *err = "copy of the LSTM state"; return B2CNN_ECUDA; }
-    lstm_fwd<kHeadLogits>((unsigned)pl.seq_ctas, st, ra.has_state(), ws + w.pre0, one_head(params, nullptr), o, d, rec.rows, sequence, sq, age,
-                          (const float *)nullptr, 1.f, ws + w.acts, ws + w.cs, ws + w.hs, ws + w.lin, z_out, (float *)nullptr,
-                          scan_state(ra, rr));
+    lstm_fwd<kHeadLogits>((unsigned)c.pl.seq_ctas, st, ra.has_state(), ws + w.pre0, one_head(params, nullptr), c.o, c.d, c.rec.rows, c.sequence,
+                          c.sq, age, (const float *)nullptr, 1.f, ws + w.acts, ws + w.cs, ws + w.hs, ws + w.lin, z_out, (float *)nullptr,
+                          scan_state(ra, c.rr));
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) { *err = cudaGetErrorString(e); return B2CNN_ECUDA; }
     return B2CNN_OK;
@@ -1415,33 +1433,24 @@ int train_forward(const b2cnn_config *cfg, const float *params, const float *x, 
 int train_backward(const b2cnn_config *cfg, const float *params, const float *x, int64_t B, const float *age, int mode, const SeqLengths &sl,
                    const RecordArgs &ra, const float *mask1, const float *mask2, const float *dz, float *grads, float *dx, float *dage,
                    int flags, void *workspace, int64_t ws_bytes, cudaStream_t st, const char **err) {
-    Dims d;
-    TrainPlan pl;
-    std::vector<int64_t> off;
-    Rec rec;
-    const int rc = train_args(cfg, B, mode, sl, ra, params && x && age && dz && grads && workspace, ws_bytes, d, pl, off, rec, err);
+    TrainCall c;
+    int rc = c.check(cfg, B, mode, sl, ra, params && x && age && dz && grads && workspace, ws_bytes, err);
     if (rc != B2CNN_OK) return rc;
     if (flags & ~B2CNN_TRAIN_FROZEN_CONV) { *err = "training: unknown flag"; return B2CNN_EINVAL; }
     const bool frozen_conv = (flags & B2CNN_TRAIN_FROZEN_CONV) != 0;
     if (frozen_conv && dx) { *err = "training: B2CNN_TRAIN_FROZEN_CONV computes no input gradient (dx must be NULL)"; return B2CNN_EINVAL; }
-    DeviceGuard dev(cfg->device);
-    if (dev.err != cudaSuccess) { *err = "cudaSetDevice"; return B2CNN_ECUDA; }
-    const TrainWs &w = pl.w;
-    const BlobOff o = blob_offsets(d);
-    const int sequence = mode == B2CNN_MODE_SEQUENCE ? 1 : 0;
-    float *ws = reinterpret_cast<float *>(workspace);
-    SeqSpan sq;
-    if (!seq_span(pl, off, ws, st, sq)) { *err = "copy sequence offsets"; return B2CNN_ECUDA; }
-    RecRows rr;
-    if (!record_span(pl, rec, d, B, ws, st, rr)) { *err = "copy row offsets"; return B2CNN_ECUDA; }
+    if ((rc = c.open(workspace, st, err)) != B2CNN_OK) return rc;
+    const TrainWs &w = c.pl.w;
+    float *const ws = c.ws;
     // zeroed: a frozen front end leaves the conv entries as they are
-    if (cudaMemsetAsync(grads, 0, sizeof(float) * o.total, st) != cudaSuccess) { *err = "memset grads"; return B2CNN_ECUDA; }
+    if (cudaMemsetAsync(grads, 0, sizeof(float) * c.o.total, st) != cudaSuccess) { *err = "memset grads"; return B2CNN_ECUDA; }
     if (!pass_state(ra.d_state_in, ra.d_state_out, B, st)) { *err = "copy of the LSTM state gradient"; return B2CNN_ECUDA; }
-    lstm_bwd<kHeadLogits>((unsigned)pl.seq_ctas, st, ra.has_state(), one_head(params, grads), o, d, rec.rows, sequence, sq, age,
+    const ScanHeads hd = one_head(params, grads);
+    lstm_bwd<kHeadLogits>((unsigned)c.pl.seq_ctas, st, ra.has_state(), hd, c.o, c.d, c.rec.rows, c.sequence, c.sq, age,
                           (const float *)nullptr, 1.f, dz, ws + w.acts, ws + w.cs, ws + w.hs, ws + w.lin, (const float *)nullptr, ws + w.da0, dage,
-                          scan_state(ra, rr));
-    launch_head_reduce(pl, o, sq, rec.rows, grads, nullptr, st);
-    if (!backward_tail(d, rec, o, pl, ws, params, x, B, mask1, mask2, grads, dx, frozen_conv, rr, st)) { *err = "memset dx"; return B2CNN_ECUDA; }
+                          scan_state(ra, c.rr));
+    launch_head_reduce(c, hd, 1, nullptr, st);
+    if (!backward_tail(c, params, x, mask1, mask2, grads, dx, frozen_conv, st)) { *err = "memset dx"; return B2CNN_ECUDA; }
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) { *err = cudaGetErrorString(e); return B2CNN_ECUDA; }
     return B2CNN_OK;
@@ -1465,7 +1474,7 @@ int train_heads_step(const b2cnn_config *cfg, const float *frontend, int n_heads
     if (!params || !grads || !lr || (apply_update && (!adam_m || !adam_v))) { *err = "training: null head array"; return B2CNN_EINVAL; }
     Dims d;
     if (!train_geometry(cfg, d, err)) return B2CNN_EINVAL;
-    const BlobOff o = blob_offsets(d);
+    const size_t blob_bytes = sizeof(float) * blob_offsets(d).total;
     // every array a head writes: its blob, its gradients and (with an update) its Adam state, none shared with another's
     std::vector<const float *> arrays;
     for (int h = 0; h < n_heads; ++h) {
@@ -1476,28 +1485,21 @@ int train_heads_step(const b2cnn_config *cfg, const float *frontend, int n_heads
     }
     for (size_t i = 0; i < arrays.size(); ++i)
         for (size_t j = i + 1; j < arrays.size(); ++j)
-            if (arrays[i] < arrays[j] + o.total && arrays[j] < arrays[i] + o.total) {
+            if (overlap(arrays[i], arrays[j], blob_bytes)) {
                 *err = "training: two heads share a blob (or a head's blob, gradients and Adam state overlap)";
                 return B2CNN_EINVAL;
             }
-    TrainPlan pl;
-    std::vector<int64_t> off;
-    Rec rec;
-    const int rc = train_args(cfg, B, mode, sl, ra, frontend && x && age && target && loss_out && workspace, ws_bytes, d, pl, off, rec, err, n_heads);
+    TrainCall c;
+    int rc = c.check(cfg, B, mode, sl, ra, frontend && x && age && target && loss_out && workspace, ws_bytes, err, n_heads);
     if (rc != B2CNN_OK) return rc;
     if (ra.has_state()) { *err = "training: heads carry no LSTM state"; return B2CNN_EINVAL; }
     if (step < 1) { *err = "training: step must be >= 1"; return B2CNN_EINVAL; }
     if (weighted && !(pos_weight > 0.f && pos_weight <= FLT_MAX)) { *err = "training: pos_weight must be positive and finite"; return B2CNN_EINVAL; }
-    DeviceGuard dev(cfg->device);
-    if (dev.err != cudaSuccess) { *err = "cudaSetDevice"; return B2CNN_ECUDA; }
-    const TrainWs &w = pl.w;
-    const int sequence = mode == B2CNN_MODE_SEQUENCE ? 1 : 0;
-    const int64_t R = rec.rows;
-    float *ws = reinterpret_cast<float *>(workspace);
-    SeqSpan sq;
-    if (!seq_span(pl, off, ws, st, sq)) { *err = "copy sequence offsets"; return B2CNN_ECUDA; }
-    RecRows rr;
-    if (!record_span(pl, rec, d, B, ws, st, rr)) { *err = "copy row offsets"; return B2CNN_ECUDA; }
+    if ((rc = c.open(workspace, st, err)) != B2CNN_OK) return rc;
+    const TrainWs &w = c.pl.w;
+    const BlobOff &o = c.o;
+    float *const ws = c.ws;
+    const int64_t R = c.rec.rows;
     ScanHeads hd{};
     AdamHeads ah{};
     for (int h = 0; h < n_heads; ++h) {
@@ -1508,48 +1510,22 @@ int train_heads_step(const b2cnn_config *cfg, const float *frontend, int n_heads
         ah.v[h] = apply_update ? adam_v[h] : nullptr;
         ah.lr[h] = lr[h];
     }
-    // the front end once, then every head's layer-0 pre-activations
-    const Dims &cd = rec.on ? rec.rd : d;
-    const dim3 conv((unsigned)(B * pl.tiles)), proj((unsigned)((R + 63) / 64), (unsigned)pl.slices, (unsigned)((n_heads + kPre0Heads - 1) / kPre0Heads));
-    float *const pre0 = ws + (pl.slices > 1 ? w.part : w.pre0);
-    if (rec.on) {
-        if (pl.smem_fwd > 48 * 1024) cudaFuncSetAttribute(train_conv_fwd_record, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.smem_fwd);
-        train_conv_fwd_record<<<conv, kThreads, pl.smem_fwd, st>>>(x, frontend, o, cd, pl.tiles, mask1, mask2, ws + w.f, rr);
-        train_pre0_partial_heads<true><<<proj, 256, 0, st>>>(ws + w.f, hd, n_heads, o, R, d.L, pre0, rr);
-    } else {
-        if (pl.smem_fwd > 48 * 1024) cudaFuncSetAttribute(train_conv_fwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.smem_fwd);
-        train_conv_fwd<<<conv, kThreads, pl.smem_fwd, st>>>(x, frontend, o, cd, pl.tiles, mask1, mask2, ws + w.f);
-        train_pre0_partial_heads<false><<<proj, 256, 0, st>>>(ws + w.f, hd, n_heads, o, R, d.L, pre0, rr);
-    }
-    if (pl.slices > 1) {
-        const int64_t n = (int64_t)n_heads * R * kGates;
-        train_sum_chunks<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(ws + w.part, pl.slices, n, ws + w.pre0);
-    }
-    // the K heads' scans side by side
-    const dim3 scans((unsigned)pl.seq_ctas, (unsigned)n_heads);
-    const float *const nul = nullptr;
-    if (weighted) {
-        lstm_fwd<kHeadBcePw>(scans, st, false, ws + w.pre0, hd, o, d, R, sequence, sq, age, target, pos_weight, ws + w.acts, ws + w.cs,
-                             ws + w.hs, ws + w.lin, ws + w.z, loss_out, ScanState{});
-        lstm_bwd<kHeadBcePw>(scans, st, false, hd, o, d, R, sequence, sq, age, target, pos_weight, nul, ws + w.acts, ws + w.cs, ws + w.hs,
-                             ws + w.lin, ws + w.z, ws + w.da0, (float *)nullptr, ScanState{});
-    } else {
-        lstm_fwd<kHeadBce>(scans, st, false, ws + w.pre0, hd, o, d, R, sequence, sq, age, target, 1.f, ws + w.acts, ws + w.cs, ws + w.hs,
-                           ws + w.lin, ws + w.z, loss_out, ScanState{});
-        lstm_bwd<kHeadBce>(scans, st, false, hd, o, d, R, sequence, sq, age, target, 1.f, nul, ws + w.acts, ws + w.cs, ws + w.hs,
-                           ws + w.lin, ws + w.z, ws + w.da0, (float *)nullptr, ScanState{});
-    }
-    if (sq.rows)
-        train_head_reduce<<<dim3((unsigned)((head_row_len(o) + 255) / 256), (unsigned)n_heads), 256, 0, st>>>(sq.rows, pl.seq_ctas, o, R, hd, loss_out);
+    // the front end once, then every head's layer-0 pre-activations and the K heads' scans side by side
+    launch_conv_forward(c, frontend, x, mask1, mask2, st);
+    if (c.rec.on) train_pre0_partial_heads<true><<<c.pre0_grid(n_heads), 256, 0, st>>>(ws + w.f, hd, n_heads, o, R, c.d.L, c.pre0_out(), c.rr);
+    else train_pre0_partial_heads<false><<<c.pre0_grid(n_heads), 256, 0, st>>>(ws + w.f, hd, n_heads, o, R, c.d.L, c.pre0_out(), c.rr);
+    sum_pre0(c, n_heads, st);
+    launch_scans(c, hd, n_heads, age, target, weighted, pos_weight, loss_out, false, ScanState{}, st);
+    launch_head_reduce(c, hd, n_heads, loss_out, st);
     // dW_ih_l0 (and the zeroed conv entries), then Adam
-    const int64_t n1 = (int64_t)kGates * d.L;
-    const dim3 wgrid((unsigned)((d.L + 127) / 128), (unsigned)pl.wih_chunks, (unsigned)((n_heads + kWihHeads - 1) / kWihHeads));
-    if (rec.on)
-        train_wih0_grad_heads<true><<<wgrid, 128, 0, st>>>(ws + w.da0, ws + w.f, hd, n_heads, o, R, d.L, pl.wih_chunk, pl.wih_chunks, ws + w.part, rr);
+    const int64_t n1 = (int64_t)kGates * c.d.L;
+    const dim3 wgrid((unsigned)((c.d.L + 127) / 128), (unsigned)c.pl.wih_chunks, (unsigned)((n_heads + kWihHeads - 1) / kWihHeads));
+    if (c.rec.on)
+        train_wih0_grad_heads<true><<<wgrid, 128, 0, st>>>(ws + w.da0, ws + w.f, hd, n_heads, o, R, c.d.L, c.pl.wih_chunk, c.pl.wih_chunks, ws + w.part, c.rr);
     else
-        train_wih0_grad_heads<false><<<wgrid, 128, 0, st>>>(ws + w.da0, ws + w.f, hd, n_heads, o, R, d.L, pl.wih_chunk, pl.wih_chunks, ws + w.part, rr);
-    if (pl.wih_chunks > 1)
-        train_wih0_sum_heads<<<dim3((unsigned)((n1 + 255) / 256), (unsigned)n_heads), 256, 0, st>>>(ws + w.part, pl.wih_chunks, n1, hd, o);
+        train_wih0_grad_heads<false><<<wgrid, 128, 0, st>>>(ws + w.da0, ws + w.f, hd, n_heads, o, R, c.d.L, c.pl.wih_chunk, c.pl.wih_chunks, ws + w.part, c.rr);
+    if (c.pl.wih_chunks > 1)
+        train_wih0_sum_heads<<<dim3((unsigned)((n1 + 255) / 256), (unsigned)n_heads), 256, 0, st>>>(ws + w.part, c.pl.wih_chunks, n1, hd, o);
     if (apply_update) {
         const float bc1 = 1.f - powf(beta1, (float)step), bc2 = 1.f - powf(beta2, (float)step);
         train_adam_heads<<<dim3((unsigned)((o.total - o.wih0 + 255) / 256), (unsigned)n_heads), 256, 0, st>>>(ah, o, beta1, beta2, eps, bc1, sqrtf(bc2));

@@ -37,38 +37,48 @@ from .autograd import check_masks, check_record_batch, check_trainable, draw_mas
 from .model import B200MyCNN, check_head_models, check_record_state
 
 
-class B200Trainer:
-    def __init__(self, model: B200MyCNN, lr: float = 1e-3, betas: Tuple[float, float] = (0.9, 0.999), eps: float = 1e-8,
-                 mode: str = "sequence", dropout: float = 0.1, seed: int = 0, pos_weight: Optional[float] = None):
-        """``pos_weight``: the class weight of ``nn.BCEWithLogitsLoss(pos_weight=...)`` (a positive number; None = the
-        unweighted loss)."""
-        check_trainable(model.arch)
-        if mode not in ("sequence", "independent"):
-            raise ValueError("mode must be 'sequence' or 'independent'")
-        if not 0.0 <= float(dropout) < 1.0:
-            raise ValueError("dropout must be in [0, 1)")
-        if pos_weight is not None:
-            pos_weight = float(pos_weight)
-            if not (math.isfinite(pos_weight) and pos_weight > 0.0):
-                raise ValueError("pos_weight must be a positive finite number")
-        dev = model._device()
+def _check_options(arch, mode: str, dropout: float, pos_weight: Optional[float]) -> Optional[float]:
+    """The options both trainers take, refused before anything runs; returns pos_weight as a float (None: unweighted)."""
+    check_trainable(arch)
+    if mode not in ("sequence", "independent"):
+        raise ValueError("mode must be 'sequence' or 'independent'")
+    if not 0.0 <= float(dropout) < 1.0:
+        raise ValueError("dropout must be in [0, 1)")
+    if pos_weight is not None:
+        pos_weight = float(pos_weight)
+        if not (math.isfinite(pos_weight) and pos_weight > 0.0):
+            raise ValueError("pos_weight must be a positive finite number")
+    return pos_weight
+
+
+class _FusedTrainer:
+    """What :class:`B200Trainer` and :class:`B200HeadTrainer` share: the checks of their options and batches, the
+    library's configuration and Adam arguments, the dropout generator and the workspace."""
+
+    def _setup(self, who: str, model: B200MyCNN, dev: torch.device, lr: float, betas: Tuple[float, float], eps: float, mode: str,
+               dropout: float, seed: int, pos_weight: Optional[float], heads=None) -> None:
+        """After the checks of :func:`_check_options`: refuses a model off the GPU, then binds the library to its device
+        and takes the blob of ``model`` (or with ``heads`` one row per head), its Adam state and gradients."""
         if dev.type != "cuda":
-            raise RuntimeError("B200Trainer needs the model on a CUDA device (there is no CPU fallback)")
+            raise RuntimeError(f"{who} needs the model on a CUDA device (there is no CPU fallback)")
         self.model, self.mode, self.dropout, self.pos_weight = model, mode, float(dropout), pos_weight
+        self._mode = capi.MODE_SEQUENCE if mode == "sequence" else capi.MODE_INDEPENDENT
         self._lib = capi.load_library()
         self._cfg = capi.make_config(model.arch, dev.index if dev.index is not None else torch.cuda.current_device())
         self._opt = capi.Adam(lr, betas[0], betas[1], eps)
-        self._params = model.packed_weights().to(dev).contiguous()          # master copy, updated in place by the library
+        if heads is None:
+            self._params = model.packed_weights().to(dev).contiguous()     # master copy, updated in place by the library
+        else:
+            self._params = torch.stack([h.packed_weights().to(dev) for h in heads]).contiguous()   # [K, n]: one blob per head
         self._m = torch.zeros_like(self._params)
         self._v = torch.zeros_like(self._params)
         self._grads = torch.zeros_like(self._params)
-        self._loss = torch.zeros(1, device=dev)
+        self._loss = torch.zeros(1 if heads is None else len(heads), device=dev)
         self._ws: Optional[torch.Tensor] = None
         self._gen = torch.Generator(device=dev)
         self._gen.manual_seed(seed)
         self.steps = 0
 
-    # ------------------------------------------------------------------
     def _views(self, flat: torch.Tensor) -> Dict[str, torch.Tensor]:
         sd, out, at = self.model.state_dict(), {}, 0
         for k in BLOB_KEYS:
@@ -77,26 +87,34 @@ class B200Trainer:
             at += n
         return out
 
-    def grads(self) -> Dict[str, torch.Tensor]:
-        """d loss / d parameter of the most recent step, keyed like the reference's state_dict."""
-        return self._views(self._grads)
-
     def draw_masks(self, B: int, n_samples: Optional[int] = None) -> Tuple[Optional[torch.Tensor], Optional[torch.Tensor]]:
         """The two nn.Dropout masks of bin/models.py:25,28, scaled by 1/(1-p) like torch's dropout, from the trainer's
-        seeded generator: of B windows, or with ``n_samples`` of B recordings of that many samples (:meth:`step_record`)."""
+        seeded generator: of B windows, or with ``n_samples`` of B recordings of that many samples (:meth:`step_record`).
+        A :class:`B200HeadTrainer` shares one draw between all its heads."""
         arch = self.model.arch if n_samples is None else self.model.arch.with_shape(self.model.arch.in_channels, n_samples)
         return draw_masks(arch, B, self.dropout, self._params.device, self._gen)
 
-    def step(self, x: torch.Tensor, age: torch.Tensor, target: torch.Tensor,
-             masks: Optional[Tuple[Optional[torch.Tensor], Optional[torch.Tensor]]] = None, update: bool = True,
-             seq_lengths=None) -> torch.Tensor:
-        """zero_grad + forward + BCEWithLogitsLoss(pos_weight) + backward + Adam step; returns the batch loss (a 0-d device
-        tensor).
+    @staticmethod
+    def _ptr(t):
+        return ctypes.c_void_p(t.data_ptr()) if t is not None else None
 
-        ``seq_lengths`` [n_0, ..., n_{N-1}] (sequence mode only; a list, tuple or integer tensor, each >= 1, adding up to
-        B): the batch is N consecutive sequences -- one patient's windows each -- and the LSTM starts every one from the
-        zero state, as ``torch.cat([model(x[o:o+n], age[o:o+n]) for ...])`` would; the loss is still the mean over all B
-        windows and one Adam step updates the parameters."""
+    def _pos_weight(self):
+        """pos_weight as the ``const float *`` of the C calls (NULL: the unweighted loss)."""
+        return None if self.pos_weight is None else ctypes.byref(ctypes.c_float(self.pos_weight))
+
+    def _stream(self):
+        return ctypes.c_void_p(torch.cuda.current_stream(self._params.device).cuda_stream)
+
+    def _workspace(self, need: int, what: str) -> torch.Tensor:
+        if need < 0:
+            capi.check(capi.EINVAL, what)
+        if self._ws is None or self._ws.numel() < need:
+            self._ws = torch.empty(need, dtype=torch.uint8, device=self._params.device)
+        return self._ws
+
+    def _window_batch(self, x: torch.Tensor, age: torch.Tensor, target: torch.Tensor, masks, seq_lengths):
+        """A batch of :meth:`step` on the device: ``(x, age, target, B, lens, mask1, mask2)``, ``lens`` the host array of
+        ``seq_lengths`` (None without)."""
         dev = self._params.device
         a = self.model.arch
         if x.dim() != 3 or x.shape[1] != a.in_channels or x.shape[2] != a.window:
@@ -113,27 +131,62 @@ class B200Trainer:
         if age.numel() != B or target.numel() != B:
             raise RuntimeError("age and target must have one entry per window")
         m1, m2 = check_masks(a, B, dev, *(masks if masks is not None else self.draw_masks(B)))
+        return x, age, target, B, lens, m1, m2
+
+    def _record_batch(self, records: torch.Tensor, stride, age, target, window_counts, masks, state, return_state):
+        """A batch of :meth:`step_record` on the device: ``(records, B, N, stride, counts, age, target, mask1, mask2)``,
+        one age per window."""
+        dev = self._params.device
+        stride, age, counts, M, rarch = check_record_batch(self.model.arch, records, stride, age, window_counts)
+        check_record_state(records, self.mode, state, return_state)
+        B, N = records.shape[0], records.shape[2]
+        target = torch.as_tensor(target).detach().to(dev, torch.float32).reshape(-1).contiguous()
+        if target.numel() != M:
+            raise ValueError(f"target must have one entry per window ({M}), got {target.numel()}")
+        m1, m2 = check_masks(rarch, B, dev, *(masks if masks is not None else self.draw_masks(B, N)))
+        records = records.to(dev, torch.float32).contiguous()
+        return records, B, N, stride, counts, window_ages(age.detach(), counts, M, dev), target, m1, m2
+
+
+class B200Trainer(_FusedTrainer):
+    def __init__(self, model: B200MyCNN, lr: float = 1e-3, betas: Tuple[float, float] = (0.9, 0.999), eps: float = 1e-8,
+                 mode: str = "sequence", dropout: float = 0.1, seed: int = 0, pos_weight: Optional[float] = None):
+        """``pos_weight``: the class weight of ``nn.BCEWithLogitsLoss(pos_weight=...)`` (a positive number; None = the
+        unweighted loss)."""
+        pos_weight = _check_options(model.arch, mode, dropout, pos_weight)
+        self._setup("B200Trainer", model, model._device(), lr, betas, eps, mode, dropout, seed, pos_weight)
+
+    # ------------------------------------------------------------------
+    def grads(self) -> Dict[str, torch.Tensor]:
+        """d loss / d parameter of the most recent step, keyed like the reference's state_dict."""
+        return self._views(self._grads)
+
+    def step(self, x: torch.Tensor, age: torch.Tensor, target: torch.Tensor,
+             masks: Optional[Tuple[Optional[torch.Tensor], Optional[torch.Tensor]]] = None, update: bool = True,
+             seq_lengths=None) -> torch.Tensor:
+        """zero_grad + forward + BCEWithLogitsLoss(pos_weight) + backward + Adam step; returns the batch loss (a 0-d device
+        tensor).
+
+        ``seq_lengths`` [n_0, ..., n_{N-1}] (sequence mode only; a list, tuple or integer tensor, each >= 1, adding up to
+        B): the batch is N consecutive sequences -- one patient's windows each -- and the LSTM starts every one from the
+        zero state, as ``torch.cat([model(x[o:o+n], age[o:o+n]) for ...])`` would; the loss is still the mean over all B
+        windows and one Adam step updates the parameters."""
+        x, age, target, B, lens, m1, m2 = self._window_batch(x, age, target, masks, seq_lengths)
         if lens is None:
             need = self._lib.b2cnn_train_workspace_bytes(ctypes.byref(self._cfg), B)
         else:
             need = self._lib.b2cnn_train_workspace_bytes_seq(ctypes.byref(self._cfg), B, lens, len(lens))
-        if need < 0:
-            capi.check(capi.EINVAL, "b2cnn_train_workspace_bytes")
-        if self._ws is None or self._ws.numel() < need:
-            self._ws = torch.empty(need, dtype=torch.uint8, device=dev)
-        ptr = lambda t: ctypes.c_void_p(t.data_ptr()) if t is not None else None
-        st = torch.cuda.current_stream(dev).cuda_stream
-        head = (ctypes.byref(self._cfg), ptr(self._params), ptr(self._m), ptr(self._v), ptr(self._grads), self.steps + 1,
-                ctypes.byref(self._opt), 1 if update else 0, ptr(x), B, ptr(age), ptr(target))
-        tail = (capi.MODE_SEQUENCE if self.mode == "sequence" else capi.MODE_INDEPENDENT, ptr(m1), ptr(m2), ptr(self._loss),
-                ptr(self._ws), need, ctypes.c_void_p(st))
+        ws = self._workspace(need, "b2cnn_train_workspace_bytes")
+        p = self._ptr
+        head = (ctypes.byref(self._cfg), p(self._params), p(self._m), p(self._v), p(self._grads), self.steps + 1,
+                ctypes.byref(self._opt), 1 if update else 0, p(x), B, p(age), p(target))
+        tail = (p(m1), p(m2), p(self._loss), p(ws), need, self._stream())
         if lens is not None:
-            pw = None if self.pos_weight is None else ctypes.byref(ctypes.c_float(self.pos_weight))
-            capi.check(self._lib.b2cnn_train_step_seq(*head, pw, lens, len(lens), *tail[1:]), "b2cnn_train_step_seq")
+            capi.check(self._lib.b2cnn_train_step_seq(*head, self._pos_weight(), lens, len(lens), *tail), "b2cnn_train_step_seq")
         elif self.pos_weight is None:
-            capi.check(self._lib.b2cnn_train_step(*head, *tail), "b2cnn_train_step")
+            capi.check(self._lib.b2cnn_train_step(*head, self._mode, *tail), "b2cnn_train_step")
         else:
-            capi.check(self._lib.b2cnn_train_step_weighted(*head, self.pos_weight, *tail), "b2cnn_train_step_weighted")
+            capi.check(self._lib.b2cnn_train_step_weighted(*head, self.pos_weight, self._mode, *tail), "b2cnn_train_step_weighted")
         return self._finish(update)
 
     def step_record(self, records: torch.Tensor, stride: int, age, target: torch.Tensor, window_counts=None,
@@ -154,39 +207,21 @@ class B200Trainer:
         ([recording][layer][h | c][unit]; None: zeros) is the LSTM state each recording starts from, and with
         ``return_state=True`` the call returns ``(loss, state_out)``, ``state_out`` detached: the state after each
         recording's last counted window (``state[b]`` for a count of 0), to pass to the step on the next chunk."""
-        dev = self._params.device
-        stride, age, counts, M, rarch = check_record_batch(self.model.arch, records, stride, age, window_counts)
-        check_record_state(records, self.mode, state, return_state)
-        B, N = records.shape[0], records.shape[2]
-        target = torch.as_tensor(target).detach().to(dev, torch.float32).reshape(-1).contiguous()
-        if target.numel() != M:
-            raise ValueError(f"target must have one entry per window ({M}), got {target.numel()}")
-        m1, m2 = check_masks(rarch, B, dev, *(masks if masks is not None else self.draw_masks(B, N)))
-        mode = capi.MODE_SEQUENCE if self.mode == "sequence" else capi.MODE_INDEPENDENT
-        need = self._lib.b2cnn_train_workspace_bytes_record(ctypes.byref(self._cfg), B, N, stride, counts, mode)
-        if need < 0:
-            capi.check(capi.EINVAL, "b2cnn_train_workspace_bytes_record")
-        records = records.to(dev, torch.float32).contiguous()
-        age = window_ages(age.detach(), counts, M, dev)
-        if self._ws is None or self._ws.numel() < need:
-            self._ws = torch.empty(need, dtype=torch.uint8, device=dev)
-        ptr = lambda t: ctypes.c_void_p(t.data_ptr()) if t is not None else None
-        pw = None if self.pos_weight is None else ctypes.byref(ctypes.c_float(self.pos_weight))
-        st = torch.cuda.current_stream(dev).cuda_stream
+        records, B, N, stride, counts, age, target, m1, m2 = self._record_batch(records, stride, age, target, window_counts, masks,
+                                                                                state, return_state)
+        need = self._lib.b2cnn_train_workspace_bytes_record(ctypes.byref(self._cfg), B, N, stride, counts, self._mode)
+        ws = self._workspace(need, "b2cnn_train_workspace_bytes_record")
+        p = self._ptr
+        head = (ctypes.byref(self._cfg), p(self._params), p(self._m), p(self._v), p(self._grads), self.steps + 1, ctypes.byref(self._opt),
+                1 if update else 0, p(records), B, N, stride, counts, self._mode, p(age), p(target), self._pos_weight(), p(m1), p(m2))
+        tail = (p(self._loss), p(ws), need, self._stream())
         if state is None and not return_state:
-            capi.check(self._lib.b2cnn_train_step_record(ctypes.byref(self._cfg), ptr(self._params), ptr(self._m), ptr(self._v),
-                                                         ptr(self._grads), self.steps + 1, ctypes.byref(self._opt), 1 if update else 0,
-                                                         ptr(records), B, N, stride, counts, mode, ptr(age), ptr(target), pw, ptr(m1), ptr(m2),
-                                                         ptr(self._loss), ptr(self._ws), need, ctypes.c_void_p(st)), "b2cnn_train_step_record")
+            capi.check(self._lib.b2cnn_train_step_record(*head, *tail), "b2cnn_train_step_record")
             return self._finish(update)
         if state is not None:
-            state = state.detach().to(dev, torch.float32).contiguous()
-        state_out = torch.empty(B, 2, 2, 16, dtype=torch.float32, device=dev)
-        capi.check(self._lib.b2cnn_train_step_record_state(ctypes.byref(self._cfg), ptr(self._params), ptr(self._m), ptr(self._v),
-                                                           ptr(self._grads), self.steps + 1, ctypes.byref(self._opt), 1 if update else 0,
-                                                           ptr(records), B, N, stride, counts, mode, ptr(age), ptr(target), pw, ptr(m1),
-                                                           ptr(m2), ptr(state), ptr(state_out), ptr(self._loss), ptr(self._ws), need,
-                                                           ctypes.c_void_p(st)), "b2cnn_train_step_record_state")
+            state = state.detach().to(self._params.device, torch.float32).contiguous()
+        state_out = torch.empty(B, 2, 2, 16, dtype=torch.float32, device=self._params.device)
+        capi.check(self._lib.b2cnn_train_step_record_state(*head, p(state), p(state_out), *tail), "b2cnn_train_step_record_state")
         loss = self._finish(update)
         return (loss, state_out) if return_state else loss
 
@@ -201,7 +236,7 @@ class B200Trainer:
         return self._loss[0].clone()
 
 
-class B200HeadTrainer:
+class B200HeadTrainer(_FusedTrainer):
     """Train up to 8 candidate heads on one frozen front end in one fused step per batch.
 
     ``model``'s conv1 / conv2 are the front end: the conv forward runs once per step on them and nothing
@@ -223,15 +258,7 @@ class B200HeadTrainer:
                  mode: str = "sequence", dropout: float = 0.1, seed: int = 0, pos_weight: Optional[float] = None):
         if not isinstance(model, B200MyCNN):
             raise TypeError(f"model must be a B200MyCNN, got {type(model).__name__}")
-        check_trainable(model.arch)
-        if mode not in ("sequence", "independent"):
-            raise ValueError("mode must be 'sequence' or 'independent'")
-        if not 0.0 <= float(dropout) < 1.0:
-            raise ValueError("dropout must be in [0, 1)")
-        if pos_weight is not None:
-            pos_weight = float(pos_weight)
-            if not (math.isfinite(pos_weight) and pos_weight > 0.0):
-                raise ValueError("pos_weight must be a positive finite number")
+        pos_weight = _check_options(model.arch, mode, dropout, pos_weight)
         dev = model._device()
         sd = model.state_dict()
         front = {k: sd[k] for k in BLOB_KEYS[:BLOB_KEYS.index("lstm.weight_ih_l0")]}
@@ -258,33 +285,12 @@ class B200HeadTrainer:
                 raise ValueError(f"lr must be one float or {K} floats (one per head), got {len(lrs)}")
         if not all(math.isfinite(v) and v >= 0.0 for v in lrs):
             raise ValueError("every lr must be a finite number >= 0")
-        if dev.type != "cuda":
-            raise RuntimeError("B200HeadTrainer needs the model on a CUDA device (there is no CPU fallback)")
-        self.model, self.heads, self.mode, self.dropout, self.pos_weight = model, heads, mode, float(dropout), pos_weight
-        self._lib = capi.load_library()
-        self._cfg = capi.make_config(model.arch, dev.index if dev.index is not None else torch.cuda.current_device())
-        self._opt = capi.Adam(0.0, betas[0], betas[1], eps)
+        self._setup("B200HeadTrainer", model, dev, 0.0, betas, eps, mode, dropout, seed, pos_weight, heads=heads)
+        self.heads = heads
         self._lr = (ctypes.c_float * K)(*lrs)
         self._front = model.packed_weights().to(dev).contiguous()         # read for its conv entries only
-        self._params = torch.stack([h.packed_weights().to(dev) for h in heads]).contiguous()   # [K, n]: one blob per head
-        self._m = torch.zeros_like(self._params)
-        self._v = torch.zeros_like(self._params)
-        self._grads = torch.zeros_like(self._params)
-        self._loss = torch.zeros(K, device=dev)
         ptrs = lambda t: (ctypes.c_void_p * K)(*[t[i].data_ptr() for i in range(K)])
         self._pp, self._pm, self._pv, self._pg = ptrs(self._params), ptrs(self._m), ptrs(self._v), ptrs(self._grads)
-        self._ws: Optional[torch.Tensor] = None
-        self._gen = torch.Generator(device=dev)
-        self._gen.manual_seed(seed)
-        self.steps = 0
-
-    def _views(self, flat: torch.Tensor) -> Dict[str, torch.Tensor]:
-        sd, out, at = self.model.state_dict(), {}, 0
-        for k in BLOB_KEYS:
-            n = sd[k].numel()
-            out[k] = flat[at:at + n].view(sd[k].shape)
-            at += n
-        return out
 
     def grads(self) -> List[Dict[str, torch.Tensor]]:
         """d loss / d parameter of the most recent step, one dict per head, keyed like the reference's state_dict from
@@ -292,53 +298,20 @@ class B200HeadTrainer:
         first = BLOB_KEYS.index("lstm.weight_ih_l0")
         return [{k: v for k, v in self._views(self._grads[i]).items() if k in BLOB_KEYS[first:]} for i in range(len(self.heads))]
 
-    def draw_masks(self, B: int, n_samples: Optional[int] = None) -> Tuple[Optional[torch.Tensor], Optional[torch.Tensor]]:
-        """One draw of the two dropout masks (as :meth:`B200Trainer.draw_masks`), shared by every head."""
-        arch = self.model.arch if n_samples is None else self.model.arch.with_shape(self.model.arch.in_channels, n_samples)
-        return draw_masks(arch, B, self.dropout, self._params.device, self._gen)
-
-    def _ptr(self, t):
-        return ctypes.c_void_p(t.data_ptr()) if t is not None else None
-
-    def _workspace(self, need: int, what: str) -> torch.Tensor:
-        if need < 0:
-            capi.check(capi.EINVAL, what)
-        if self._ws is None or self._ws.numel() < need:
-            self._ws = torch.empty(need, dtype=torch.uint8, device=self._params.device)
-        return self._ws
-
     def step(self, x: torch.Tensor, age: torch.Tensor, target: torch.Tensor,
              masks: Optional[Tuple[Optional[torch.Tensor], Optional[torch.Tensor]]] = None, update: bool = True,
              seq_lengths=None) -> torch.Tensor:
         """:meth:`B200Trainer.step` for every head at once, with its rules; returns the K heads' batch losses, a device
         tensor [K]."""
-        dev = self._params.device
-        a = self.model.arch
-        if x.dim() != 3 or x.shape[1] != a.in_channels or x.shape[2] != a.window:
-            raise RuntimeError(f"expected x of shape [B, {a.in_channels}, {a.window}], got {tuple(x.shape)}")
-        B = x.shape[0]
-        lens = None
-        if seq_lengths is not None:
-            if self.mode != "sequence":
-                raise ValueError("seq_lengths needs a trainer in mode='sequence'")
-            lens = capi.seq_lengths_array(seq_lengths, B)
-        x = x.to(dev, torch.float32).contiguous()
-        age = age.to(dev, torch.float32).reshape(-1).contiguous()
-        target = target.to(dev, torch.float32).reshape(-1).contiguous()
-        if age.numel() != B or target.numel() != B:
-            raise RuntimeError("age and target must have one entry per window")
-        m1, m2 = check_masks(a, B, dev, *(masks if masks is not None else self.draw_masks(B)))
-        K = len(self.heads)
-        need = self._lib.b2cnn_train_heads_workspace_bytes(ctypes.byref(self._cfg), K, B, lens, len(lens) if lens is not None else 0)
+        x, age, target, B, lens, m1, m2 = self._window_batch(x, age, target, masks, seq_lengths)
+        K, n_seq = len(self.heads), len(lens) if lens is not None else 0
+        need = self._lib.b2cnn_train_heads_workspace_bytes(ctypes.byref(self._cfg), K, B, lens, n_seq)
         ws = self._workspace(need, "b2cnn_train_heads_workspace_bytes")
         p = self._ptr
-        pw = None if self.pos_weight is None else ctypes.byref(ctypes.c_float(self.pos_weight))
-        mode = capi.MODE_SEQUENCE if self.mode == "sequence" else capi.MODE_INDEPENDENT
-        st = torch.cuda.current_stream(dev).cuda_stream
         capi.check(self._lib.b2cnn_train_heads_step(ctypes.byref(self._cfg), p(self._front), K, self._pp, self._pm, self._pv, self._pg,
                                                     self._lr, self.steps + 1, ctypes.byref(self._opt), 1 if update else 0, p(x), B,
-                                                    p(age), p(target), pw, mode, lens, len(lens) if lens is not None else 0, p(m1), p(m2),
-                                                    p(self._loss), p(ws), need, ctypes.c_void_p(st)), "b2cnn_train_heads_step")
+                                                    p(age), p(target), self._pos_weight(), self._mode, lens, n_seq, p(m1), p(m2),
+                                                    p(self._loss), p(ws), need, self._stream()), "b2cnn_train_heads_step")
         return self._finish(update)
 
     def step_record(self, records: torch.Tensor, stride: int, age, target: torch.Tensor, window_counts=None,
@@ -348,26 +321,16 @@ class B200HeadTrainer:
         Carrying an LSTM state across chunks (``state`` / ``return_state``) is not supported (ValueError)."""
         if state is not None or return_state:
             raise ValueError("B200HeadTrainer.step_record carries no LSTM state across calls (state / return_state)")
-        dev = self._params.device
-        stride, age, counts, M, rarch = check_record_batch(self.model.arch, records, stride, age, window_counts)
-        B, N = records.shape[0], records.shape[2]
-        target = torch.as_tensor(target).detach().to(dev, torch.float32).reshape(-1).contiguous()
-        if target.numel() != M:
-            raise ValueError(f"target must have one entry per window ({M}), got {target.numel()}")
-        m1, m2 = check_masks(rarch, B, dev, *(masks if masks is not None else self.draw_masks(B, N)))
-        mode = capi.MODE_SEQUENCE if self.mode == "sequence" else capi.MODE_INDEPENDENT
+        records, B, N, stride, counts, age, target, m1, m2 = self._record_batch(records, stride, age, target, window_counts, masks,
+                                                                                None, False)
         K = len(self.heads)
-        need = self._lib.b2cnn_train_heads_workspace_bytes_record(ctypes.byref(self._cfg), K, B, N, stride, counts, mode)
+        need = self._lib.b2cnn_train_heads_workspace_bytes_record(ctypes.byref(self._cfg), K, B, N, stride, counts, self._mode)
         ws = self._workspace(need, "b2cnn_train_heads_workspace_bytes_record")
-        records = records.to(dev, torch.float32).contiguous()
-        age = window_ages(age.detach(), counts, M, dev)
         p = self._ptr
-        pw = None if self.pos_weight is None else ctypes.byref(ctypes.c_float(self.pos_weight))
-        st = torch.cuda.current_stream(dev).cuda_stream
         capi.check(self._lib.b2cnn_train_heads_step_record(ctypes.byref(self._cfg), p(self._front), K, self._pp, self._pm, self._pv,
                                                            self._pg, self._lr, self.steps + 1, ctypes.byref(self._opt), 1 if update else 0,
-                                                           p(records), B, N, stride, counts, mode, p(age), p(target), pw, p(m1), p(m2),
-                                                           p(self._loss), p(ws), need, ctypes.c_void_p(st)), "b2cnn_train_heads_step_record")
+                                                           p(records), B, N, stride, counts, self._mode, p(age), p(target), self._pos_weight(),
+                                                           p(m1), p(m2), p(self._loss), p(ws), need, self._stream()), "b2cnn_train_heads_step_record")
         return self._finish(update)
 
     def _finish(self, update: bool) -> torch.Tensor:
